@@ -1,6 +1,6 @@
-// Library-level entry points: error reporting and version.
+// Library-level entry points and host-side state: error reporting, version, per-device facts.
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
+#include <mutex>
 #include <stdarg.h>
 
 static thread_local char g_err[512] = "";
@@ -16,6 +16,7 @@ extern "C" const char* n3d_last_error(void) { return g_err; }
 extern "C" int n3d_version(void) { return 100; }
 
 static N3DDeviceState g_dev_state[128];
+static std::mutex g_smem_mutex;              // guards the smem tables: entry points may be called from several host threads
 
 N3DDeviceState* n3d_device_state(void) {
     int dev = 0;
@@ -26,8 +27,30 @@ N3DDeviceState* n3d_device_state(void) {
     N3DDeviceState* d = &g_dev_state[dev];
     if (!d->num_sms) {
         int n = 0;
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        d->num_sms = n > 0 ? n : 132;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+            n3d_set_error("cannot query the SM count of CUDA device %d", dev);
+            return nullptr;
+        }
+        d->num_sms = n;
     }
     return d;
+}
+
+int n3d_smem_optin(const void* kernel, int bytes, const char* who) {
+    N3DDeviceState* d = n3d_device_state();
+    if (!d) return N3D_ERR_CUDA;
+    std::lock_guard<std::mutex> lock(g_smem_mutex);
+    int i = 0;
+    while (i < d->n_smem && d->smem[i].kernel != kernel) ++i;
+    if (i < d->n_smem && d->smem[i].bytes >= bytes) return N3D_OK;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) {
+        n3d_set_error("%s: cannot raise dynamic shared memory to %d bytes: %s", who, bytes, cudaGetErrorString(e));
+        return N3D_ERR_CUDA;
+    }
+    if (i < N3DDeviceState::kSmemSlots) {            // a full table only costs repeated calls
+        d->smem[i] = {kernel, bytes};
+        if (i == d->n_smem) ++d->n_smem;
+    }
+    return N3D_OK;
 }

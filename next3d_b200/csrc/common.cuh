@@ -5,12 +5,7 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
-
-// Error codes returned by every extern "C" entry point (include/next3d_b200.h).
-#define N3D_OK 0
-#define N3D_ERR_INVALID_ARG (-1)
-#define N3D_ERR_UNSUPPORTED (-2)
-#define N3D_ERR_CUDA (-3)
+#include "../../include/next3d_b200.h"       // status codes N3D_OK / N3D_ERR_* of every extern "C" entry point
 
 void n3d_set_error(const char* fmt, ...);
 
@@ -34,13 +29,27 @@ void n3d_set_error(const char* fmt, ...);
 static inline int n3d_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // Host-side facts cached PER DEVICE (the library holds no device memory and no device-global state): SM count and which kernels
-// already had their dynamic shared-memory limit raised on that device.  Indexed by the current device at call time.
+// already had their dynamic shared-memory limit raised on that device (n3d_smem_optin).  Indexed by the current device at call time.
 struct N3DDeviceState {
+    static constexpr int kSmemSlots = 32;
     int num_sms;
-    unsigned configured;     // bit per kernel, see N3D_CFG_*
+    int n_smem;
+    struct { const void* kernel; int bytes; } smem[kSmemSlots];
 };
-enum { N3D_CFG_CONV = 1u, N3D_CFG_FILL_MOUTH = 2u, N3D_CFG_RENDER16 = 4u, N3D_CFG_RENDER32 = 8u, N3D_CFG_POINTS = 16u, N3D_CFG_FIR_STREAM = 32u, N3D_CFG_FIR_DOWN_STREAM = 64u };
 N3DDeviceState* n3d_device_state(void);      // api.cu; nullptr (+ error message) when the current device cannot be queried
+
+// Raises `kernel`'s dynamic shared-memory limit to at least `bytes` on the current device, once per (device, kernel).
+// N3D_OK, or N3D_ERR_CUDA with a message that starts with `who`.
+int n3d_smem_optin(const void* kernel, int bytes, const char* who);     // api.cu
+
+// Grid of a grid-stride launch: one block per `threads` work items, at least 1 and at most `per_sm` blocks per SM of the current
+// device.  0 when the device cannot be queried, so that the launch fails and N3D_CHECK_LAUNCH reports it.
+inline int n3d_grid(int64_t work_items, int threads, int per_sm = 8) {
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return 0;
+    const int64_t g = (work_items + threads - 1) / threads, cap = (int64_t)D->num_sms * per_sm;
+    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
 
 // fp32 -> (hi, lo) bf16 pair with hi + lo ~= x to ~16 mantissa bits (used by the 3-product tensor-core scheme).
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {

@@ -14,9 +14,8 @@
 //   modulation -> bf16 split / fp32 stores) through a small shared-memory transpose (thread = tile row).  Warpgroup 2 = TMA
 //   producer (one lane), which keeps filling the stage ring during the epilogue.  setmaxnreg lowers the producer to 40 registers
 //   and raises the consumers to 232: ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
-#include <cstdlib>
+#include <cstring>
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 #include <cuda.h>
 #include "tc_ptx.cuh"
 
@@ -498,11 +497,7 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
             bn = cands[i];
             break;
         }
-        int min_tiles = kMinTiles;
-        if (splits > 1) {                                   // split launches: short K loops, so spread over (nearly) all SMs
-            min_tiles = kMinTilesSplit;
-            if (const char* e = getenv("N3D_SPLITK_MINTILES")) min_tiles = atoi(e);      // A/B diagnostics (tools/bench_splitk.py)
-        }
+        const int min_tiles = splits > 1 ? kMinTilesSplit : kMinTiles;     // split launches: short K loops, so spread over (nearly) all SMs
         while (bn > 32 && tiles_m * splits * n3d_div_up(p->Cout, bn) < min_tiles) bn = (bn == 96) ? 32 : bn / 2;
         if (p->rgb.out) {                                   // fused ToRGB needs every output channel of a pixel in one tile
             N3D_CHECK_ARG(cout16 <= 256 && cout16 % 16 == 0, "n3d_conv_gemm: fused ToRGB needs Cout <= 256");
@@ -553,19 +548,11 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
     N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
-    if (!(D->configured & N3D_CFG_CONV)) {
-        const void* kernels[6] = {(const void*)conv_gemm_kernel<16>, (const void*)conv_gemm_kernel<32>, (const void*)conv_gemm_kernel<64>,
-                                  (const void*)conv_gemm_kernel<96>, (const void*)conv_gemm_kernel<128>, (const void*)conv_gemm_kernel<256>};
-        for (int i = 0; i < 6; ++i)
-            if (cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
-                n3d_set_error("n3d_conv_gemm: cannot raise dynamic shared memory to 227 KiB");
-                return N3D_ERR_CUDA;
-            }
-        D->configured |= N3D_CFG_CONV;
-    }
-    const int total_tiles = tiles_m * K.tiles_n * splits;
-    const int num_sms = D->num_sms;
-    const int grid = min(total_tiles, num_sms);
+    const void* kernels[6] = {(const void*)conv_gemm_kernel<16>, (const void*)conv_gemm_kernel<32>, (const void*)conv_gemm_kernel<64>,
+                              (const void*)conv_gemm_kernel<96>, (const void*)conv_gemm_kernel<128>, (const void*)conv_gemm_kernel<256>};
+    for (const void* k : kernels)
+        if ((rc = n3d_smem_optin(k, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
+    const int grid = min(tiles_m * K.tiles_n * splits, D->num_sms);
     switch (bn) {
         case 16: conv_gemm_kernel<16><<<grid, kThreads, smem, st>>>(K); break;
         case 32: conv_gemm_kernel<32><<<grid, kThreads, smem, st>>>(K); break;

@@ -3,18 +3,10 @@
 // multiples of the SM count.
 #include <cstdlib>
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 #include <cuda.h>
 #include "tc_ptx.cuh"
 
 namespace {
-constexpr int kSMs = 132;
-inline int grid_for(int64_t work_items, int threads, int per_sm = 8) {
-    int64_t g = (work_items + threads - 1) / threads;
-    int64_t cap = (int64_t)kSMs * per_sm;
-    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -640,7 +632,7 @@ extern "C" int n3d_styles(const float* ws, int N, int num_ws, int wdim, const fl
                           float* styles, int rows, void* stream) {
     N3D_CHECK_ARG(ws && affine_w && affine_b && row_widx && row_scale && row_ooff && row_cin && styles, "n3d_styles: null pointer");
     N3D_CHECK_ARG(wdim % 4 == 0 && rows > 0 && N > 0, "n3d_styles: bad sizes");
-    styles_kernel<<<grid_for((int64_t)rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(ws, N, num_ws, wdim, affine_w, affine_b, row_widx,
+    styles_kernel<<<n3d_grid((int64_t)rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(ws, N, num_ws, wdim, affine_w, affine_b, row_widx,
                                                                                       row_scale, row_ooff, row_cin, styles, rows);
     N3D_CHECK_LAUNCH("n3d_styles");
     return N3D_OK;
@@ -650,7 +642,7 @@ extern "C" int n3d_demod(const float* styles, const float* wsq, const int64_t* r
                          const int64_t* row_soff, const int64_t* row_ooff, const int32_t* row_cout, float* dcoef, int rows, int N,
                          void* stream) {
     N3D_CHECK_ARG(styles && wsq && row_woff && row_cin && row_soff && row_ooff && row_cout && dcoef, "n3d_demod: null pointer");
-    demod_kernel<<<grid_for((int64_t)rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(styles, wsq, row_woff, row_cin, row_soff, row_ooff,
+    demod_kernel<<<n3d_grid((int64_t)rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(styles, wsq, row_woff, row_cin, row_soff, row_ooff,
                                                                                      row_cout, dcoef, rows, N);
     N3D_CHECK_LAUNCH("n3d_demod");
     return N3D_OK;
@@ -658,10 +650,28 @@ extern "C" int n3d_demod(const float* styles, const float* wsq, const int64_t* r
 
 // Rows per thread strip of the FIR kernels: 16 (3 re-read halo rows per strip) for launches with >= 1024 threads per SM, halved
 // down to 4 for smaller ones: longer strips re-read fewer halo rows, shorter ones keep small launches filling the SMs.
-static int fir_strip_rows(int64_t threads_per_row, int rows) {
+static int fir_strip_rows(int num_sms, int64_t threads_per_row, int rows) {
     int S = 16;
-    while (S > 4 && threads_per_row * n3d_div_up(rows, S) < (int64_t)kSMs * 1024) S >>= 1;
+    while (S > 4 && threads_per_row * n3d_div_up(rows, S) < (int64_t)num_sms * 1024) S >>= 1;
     return min(S, rows);
+}
+
+// N3D_FIR_STREAM=0: the register-tiled FIR kernels everywhere (the reference of the streamed ones in the bit-identity tests).  Read
+// at call time so that one process can run both forms.
+static bool fir_stream_enabled() {
+    const char* e = getenv("N3D_FIR_STREAM");
+    return !e || atoi(e) != 0;
+}
+
+// Epilogue descriptor of n3d_fir_up_epilogue and n3d_splitk_epilogue, with the checks both need of it.
+static int make_epi(EpiParams* E, const char* who, const float* dcoef, const float* bias, const float* noise, int64_t noise_nstride,
+                    float gain, float slope, float clamp, const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff) {
+    N3D_CHECK_ARG(gain > 0.f && slope >= 0.f && slope <= 1.f, "%s: needs gain > 0 and 0 <= slope <= 1 (lrelu / linear)", who);
+    for (int k = 0; k < 2; ++k)
+        N3D_CHECK_ARG(!out[k].hi || (out[k].cstride % 4 == 0 && out[k].coff % 4 == 0), "%s: unaligned split output", who);
+    N3D_CHECK_ARG(!out_f32 || (f32_cstride % 4 == 0 && f32_coff % 4 == 0), "%s: unaligned fp32 output", who);
+    *E = EpiParams{dcoef, bias, noise, noise_nstride, gain, slope, clamp, {out[0], out[1]}, out_f32, f32_cstride, f32_coff};
+    return N3D_OK;
 }
 
 extern "C" int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* hi, void* lo,
@@ -669,7 +679,7 @@ extern "C" int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, i
     N3D_CHECK_ARG(x && hi && lo, "n3d_modulate_split: null pointer");
     N3D_CHECK_ARG(C % 4 == 0 && out_cstride % 4 == 0 && out_coff % 4 == 0, "n3d_modulate_split: channels must be multiples of 4");
     const int64_t total = (int64_t)N * npix_per_img * (C / 4);
-    modulate_split_kernel<<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)hi,
+    modulate_split_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)hi,
                                                                                      (__nv_bfloat16*)lo, out_cstride, out_coff);
     N3D_CHECK_LAUNCH("n3d_modulate_split");
     return N3D_OK;
@@ -680,55 +690,41 @@ extern "C" int n3d_fir_up_epilogue(const float* raw, int N, int H2, int W2, int 
                                    const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff, void* stream) {
     N3D_CHECK_ARG(raw && out, "n3d_fir_up_epilogue: null pointer");
     N3D_CHECK_ARG(C % 4 == 0, "n3d_fir_up_epilogue: C must be a multiple of 4");
-    N3D_CHECK_ARG(gain > 0.f && slope >= 0.f && slope <= 1.f, "n3d_fir_up_epilogue: needs gain > 0 and 0 <= slope <= 1 (lrelu / linear)");
-    EpiParams E;
-    E.dcoef = dcoef; E.bias = bias; E.noise = noise; E.noise_nstride = noise_nstride; E.gain = gain; E.slope = slope; E.clamp = clamp;
-    E.out[0] = out[0]; E.out[1] = out[1]; E.out_f32 = out_f32; E.f32_cstride = f32_cstride; E.f32_coff = f32_coff;
-    for (int k = 0; k < 2; ++k)
-        N3D_CHECK_ARG(!E.out[k].hi || ((E.out[k].cstride % 4 == 0) && (E.out[k].coff % 4 == 0)), "n3d_fir_up_epilogue: unaligned split output");
-    N3D_CHECK_ARG(!out_f32 || (f32_cstride % 4 == 0 && f32_coff % 4 == 0), "n3d_fir_up_epilogue: unaligned fp32 output");
     N3D_CHECK_ARG(H2 % 2 == 0 && W2 % 2 == 0, "n3d_fir_up_epilogue: output size must be even");
-    {   // streamed variant (fir_up_stream_kernel) for the large layers: (TC / 2) * (C / 4) == 256 consumer threads, >= one CTA per SM
-        const char* e = getenv("N3D_FIR_STREAM");               // N3D_FIR_STREAM=0: the register-tiled kernel (A/B diagnostics, tests)
-        const int stream_mode = e ? atoi(e) : 1;
-        const int TC = (C >= 64 && C <= 512 && (2048 % C) == 0) ? 2048 / C : 0;
-        // rows per tile: the candidate with the best (fill of the last wave of 2 CTAs per SM) x (1 - vertical halo).  The tiling does not change the arithmetic (results are bit-identical for every TR).
-        int TR = 0;
-        if (TC >= 4 && W2 % TC == 0) {
-            double best = 0.0;
-            for (int tr = 32; tr <= 128; tr *= 2) {
-                if (H2 % tr) continue;
-                const int64_t ctas = (int64_t)N * (W2 / TC) * (H2 / tr);
-                if (ctas < kSMs) continue;
-                const double eff = (double)ctas / (double)(n3d_div_up(ctas, 2 * kSMs) * 2 * kSMs) * tr / (tr + 3);
-                if (eff > best) { best = eff; TR = tr; }
-            }
-        }
-        if (const char* t = getenv("N3D_FIR_TR")) { TR = atoi(t); if (TR > H2) TR = H2; }      // tuning sweep only
-        if (stream_mode && TR > 0 && TC >= 4 && W2 % TC == 0 && H2 % TR == 0 && ((uintptr_t)raw & 15) == 0 &&
-            (int64_t)N * (W2 / TC) * (H2 / TR) >= kSMs) {
-            const int row_bytes = (TC + 3) * C * 4;
-            int NR = min(4, (100 * 1024) / row_bytes);         // ring depth: 4 stages (N3D_FIR_NR overrides for tuning)
-            if (const char* t = getenv("N3D_FIR_NR")) NR = max(3, min(atoi(t), (110 * 1024) / row_bytes));
-            const int smem = NR * row_bytes + 16 * NR;
-            N3DDeviceState* D = n3d_device_state();
-            if (!D) return N3D_ERR_CUDA;
-            if (!(D->configured & N3D_CFG_FIR_STREAM)) {
-                if (cudaFuncSetAttribute(fir_up_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024) != cudaSuccess) {
-                    n3d_set_error("n3d_fir_up_epilogue: cannot raise dynamic shared memory to 112 KiB");
-                    return N3D_ERR_CUDA;
-                }
-                D->configured |= N3D_CFG_FIR_STREAM;
-            }
-            fir_up_stream_kernel<<<N * (W2 / TC) * (H2 / TR), kFsThreads, smem, (cudaStream_t)stream>>>(raw, N, H2, W2, C, TC, TR, NR, E);
-            N3D_CHECK_LAUNCH("n3d_fir_up_epilogue");
-            return N3D_OK;
+    EpiParams E;
+    if (int rc = make_epi(&E, "n3d_fir_up_epilogue", dcoef, bias, noise, noise_nstride, gain, slope, clamp, out, out_f32, f32_cstride, f32_coff))
+        return rc;
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
+    const int sms = D->num_sms;
+    // streamed variant (fir_up_stream_kernel) for the large layers: (TC / 2) * (C / 4) == 256 consumer threads, >= one CTA per SM.
+    // Rows per tile: the candidate with the best (fill of the last wave of 2 CTAs per SM) x (1 - vertical halo).  The tiling does not
+    // change the arithmetic (results are bit-identical for every TR).
+    const int TC = (C >= 64 && C <= 512 && (2048 % C) == 0) ? 2048 / C : 0;
+    int TR = 0;
+    if (TC >= 4 && W2 % TC == 0) {
+        double best = 0.0;
+        for (int tr = 32; tr <= 128; tr *= 2) {
+            if (H2 % tr) continue;
+            const int64_t ctas = (int64_t)N * (W2 / TC) * (H2 / tr);
+            if (ctas < sms) continue;
+            const double eff = (double)ctas / (double)(n3d_div_up(ctas, 2 * sms) * 2 * sms) * tr / (tr + 3);
+            if (eff > best) { best = eff; TR = tr; }
         }
     }
-    const int S = fir_strip_rows((int64_t)N * (W2 / 2) * (C / 4), H2 / 2);
+    if (TR > 0 && ((uintptr_t)raw & 15) == 0 && fir_stream_enabled()) {
+        const int row_bytes = (TC + 3) * C * 4;
+        const int NR = min(4, (100 * 1024) / row_bytes);        // ring depth: 4 stages
+        const int smem = NR * row_bytes + 16 * NR;
+        if (int rc = n3d_smem_optin((const void*)fir_up_stream_kernel, 112 * 1024, "n3d_fir_up_epilogue")) return rc;
+        fir_up_stream_kernel<<<N * (W2 / TC) * (H2 / TR), kFsThreads, smem, (cudaStream_t)stream>>>(raw, N, H2, W2, C, TC, TR, NR, E);
+        N3D_CHECK_LAUNCH("n3d_fir_up_epilogue");
+        return N3D_OK;
+    }
+    const int S = fir_strip_rows(sms, (int64_t)N * (W2 / 2) * (C / 4), H2 / 2);
     const int64_t total = (int64_t)N * n3d_div_up(H2 / 2, S) * (W2 / 2) * (C / 4);
     // 2 output columns per thread: the two columns share each input row's loads
-    fir_up_epilogue_kernel<2><<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(raw, N, H2, W2, C, S, E);
+    fir_up_epilogue_kernel<2><<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(raw, N, H2, W2, C, S, E);
     N3D_CHECK_LAUNCH("n3d_fir_up_epilogue");
     return N3D_OK;
 }
@@ -738,15 +734,11 @@ extern "C" int n3d_splitk_epilogue(const float* partial, int S, int64_t split_st
                                    const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff, void* stream) {
     N3D_CHECK_ARG(partial && out && S >= 1 && N > 0 && H > 0 && W > 0, "n3d_splitk_epilogue: bad args");
     N3D_CHECK_ARG(C % 4 == 0 && split_stride % 4 == 0 && ((uintptr_t)partial & 15) == 0, "n3d_splitk_epilogue: C and the split stride must be multiples of 4");
-    N3D_CHECK_ARG(gain > 0.f && slope >= 0.f && slope <= 1.f, "n3d_splitk_epilogue: needs gain > 0 and 0 <= slope <= 1 (lrelu / linear)");
     EpiParams E;
-    E.dcoef = dcoef; E.bias = bias; E.noise = noise; E.noise_nstride = noise_nstride; E.gain = gain; E.slope = slope; E.clamp = clamp;
-    E.out[0] = out[0]; E.out[1] = out[1]; E.out_f32 = out_f32; E.f32_cstride = f32_cstride; E.f32_coff = f32_coff;
-    for (int k = 0; k < 2; ++k)
-        N3D_CHECK_ARG(!E.out[k].hi || ((E.out[k].cstride % 4 == 0) && (E.out[k].coff % 4 == 0)), "n3d_splitk_epilogue: unaligned split output");
-    N3D_CHECK_ARG(!out_f32 || (f32_cstride % 4 == 0 && f32_coff % 4 == 0), "n3d_splitk_epilogue: unaligned fp32 output");
+    if (int rc = make_epi(&E, "n3d_splitk_epilogue", dcoef, bias, noise, noise_nstride, gain, slope, clamp, out, out_f32, f32_cstride, f32_coff))
+        return rc;
     const int64_t total = (int64_t)N * H * W * (C / 4);
-    splitk_epilogue_kernel<<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(partial, S, split_stride, N, H, W, C, E);
+    splitk_epilogue_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(partial, S, split_stride, N, H, W, C, E);
     N3D_CHECK_LAUNCH("n3d_splitk_epilogue");
     return N3D_OK;
 }
@@ -754,34 +746,27 @@ extern "C" int n3d_splitk_epilogue(const float* partial, int S, int64_t split_st
 extern "C" int n3d_fir_down_split(const float* x, int N, int H, int W, int C, void* hi, void* lo, void* stream) {
     N3D_CHECK_ARG(x && hi && lo, "n3d_fir_down_split: null pointer");
     N3D_CHECK_ARG(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "n3d_fir_down_split: C %% 4 and even H, W required");
-    {   // streamed variant for the large layers (see fir_down_stream_kernel); N3D_FIR_STREAM=0: the register-tiled kernel
-        const char* e = getenv("N3D_FIR_STREAM");
-        const int c4n = C / 4, SH = (H + 2) / 2, SW = (W + 2) / 2;
-        const int TSC = (c4n >= 8 && c4n <= 128 && 256 % c4n == 0) ? 256 / c4n : 0;
-        int TS = 0;
-        for (int ts = 32; ts >= 16 && TSC; ts >>= 1)
-            if ((int64_t)N * n3d_div_up(SW, TSC) * n3d_div_up(SH, ts) >= kSMs) { TS = ts; break; }
-        if ((!e || atoi(e) != 0) && TS > 0 && ((uintptr_t)x & 15) == 0) {
-            const int row_bytes = (2 * TSC + 3) * C * 4, NR = 4;
-            const int smem = NR * row_bytes + 16 * NR;
-            N3DDeviceState* D = n3d_device_state();
-            if (!D) return N3D_ERR_CUDA;
-            if (!(D->configured & N3D_CFG_FIR_DOWN_STREAM)) {
-                if (cudaFuncSetAttribute(fir_down_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024) != cudaSuccess) {
-                    n3d_set_error("n3d_fir_down_split: cannot raise dynamic shared memory to 112 KiB");
-                    return N3D_ERR_CUDA;
-                }
-                D->configured |= N3D_CFG_FIR_DOWN_STREAM;
-            }
-            fir_down_stream_kernel<<<N * n3d_div_up(SW, TSC) * n3d_div_up(SH, TS), kFsThreads, smem, (cudaStream_t)stream>>>(
-                x, N, H, W, C, TSC, TS, NR, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
-            N3D_CHECK_LAUNCH("n3d_fir_down_split");
-            return N3D_OK;
-        }
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
+    const int sms = D->num_sms;
+    // streamed variant for the large layers (see fir_down_stream_kernel)
+    const int c4n = C / 4, SH = (H + 2) / 2, SW = (W + 2) / 2;
+    const int TSC = (c4n >= 8 && c4n <= 128 && 256 % c4n == 0) ? 256 / c4n : 0;
+    int TS = 0;
+    for (int ts = 32; ts >= 16 && TSC; ts >>= 1)
+        if ((int64_t)N * n3d_div_up(SW, TSC) * n3d_div_up(SH, ts) >= sms) { TS = ts; break; }
+    if (TS > 0 && ((uintptr_t)x & 15) == 0 && fir_stream_enabled()) {
+        const int row_bytes = (2 * TSC + 3) * C * 4, NR = 4;
+        const int smem = NR * row_bytes + 16 * NR;
+        if (int rc = n3d_smem_optin((const void*)fir_down_stream_kernel, 112 * 1024, "n3d_fir_down_split")) return rc;
+        fir_down_stream_kernel<<<N * n3d_div_up(SW, TSC) * n3d_div_up(SH, TS), kFsThreads, smem, (cudaStream_t)stream>>>(
+            x, N, H, W, C, TSC, TS, NR, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
+        N3D_CHECK_LAUNCH("n3d_fir_down_split");
+        return N3D_OK;
     }
-    const int S = fir_strip_rows((int64_t)N * ((W + 2) / 2) * (C / 4), (H + 2) / 2);
-    const int64_t total = (int64_t)N * n3d_div_up((H + 2) / 2, S) * ((W + 2) / 2) * (C / 4);
-    fir_down_split_kernel<<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, S, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
+    const int S = fir_strip_rows(sms, (int64_t)N * SW * c4n, SH);
+    const int64_t total = (int64_t)N * n3d_div_up(SH, S) * SW * c4n;
+    fir_down_split_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, S, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
     N3D_CHECK_LAUNCH("n3d_fir_down_split");
     return N3D_OK;
 }
@@ -789,16 +774,16 @@ extern "C" int n3d_fir_down_split(const float* x, int N, int H, int W, int C, vo
 extern "C" int n3d_upsample2d_nhwc(const float* x, int N, int H, int W, int C, float* y, int y_nchw, void* stream) {
     N3D_CHECK_ARG(x && y, "n3d_upsample2d_nhwc: null pointer");
     if (C % 4 == 0)
-        upsample2d_kernel<4><<<grid_for((int64_t)N * H * W * (C / 4), 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);
+        upsample2d_kernel<4><<<n3d_grid((int64_t)N * H * W * (C / 4), 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);
     else
-        upsample2d_kernel<1><<<grid_for((int64_t)N * H * W * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);
+        upsample2d_kernel<1><<<n3d_grid((int64_t)N * H * W * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);
     N3D_CHECK_LAUNCH("n3d_upsample2d_nhwc");
     return N3D_OK;
 }
 
 extern "C" int n3d_downsample2d_nhwc(const float* x, int N, int H, int W, int C, float* y, void* stream) {
     N3D_CHECK_ARG(x && y && H % 2 == 0 && W % 2 == 0, "n3d_downsample2d_nhwc: bad args");
-    downsample2d_kernel<<<grid_for((int64_t)N * (H / 2) * (W / 2) * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y);
+    downsample2d_kernel<<<n3d_grid((int64_t)N * (H / 2) * (W / 2) * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y);
     N3D_CHECK_LAUNCH("n3d_downsample2d_nhwc");
     return N3D_OK;
 }

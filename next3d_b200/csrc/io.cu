@@ -3,7 +3,6 @@
 // gen_videos_next3d.py:118-131).  Plain C++ (no device code): one pass over the text, strtod per number, so that the
 // float64 -> float32 values are bit-identical to `float(token)` / `np.loadtxt` followed by `.float()`.
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 #include <stdlib.h>
 #include <string.h>
 #include <charconv>

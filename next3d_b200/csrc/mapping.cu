@@ -4,7 +4,6 @@
 // the weight matrices, warp-shuffle dot products); the ~3.1 MB of fp32 weights stay L2-resident across the batch.
 // Also here: row interpolation out[f] = sum_k B[f,k] * Y[k] used by the frame drivers (latent interpolation, camera smoothing).
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 
 namespace {
 constexpr int kZ = 512, kW = 512, kC = 25, kThreads = 512;
@@ -121,9 +120,7 @@ extern "C" int n3d_mapping(const float* z, const float* c, int N, float c_scale,
 
 extern "C" int n3d_interp_rows(const float* B, const float* Y, int F, int K, int64_t D, float* out, void* stream) {
     N3D_CHECK_ARG(B && Y && out && F >= 1 && K >= 1 && D >= 1, "n3d_interp_rows: bad args");
-    const int64_t total = (int64_t)F * D;
-    const int grid = (int)((total + 255) / 256 > 132 * 8 ? 132 * 8 : (total + 255) / 256);
-    interp_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(B, Y, F, K, D, out);
+    interp_rows_kernel<<<n3d_grid((int64_t)F * D, 256), 256, 0, (cudaStream_t)stream>>>(B, Y, F, K, D, out);
     N3D_CHECK_LAUNCH("n3d_interp_rows");
     return N3D_OK;
 }

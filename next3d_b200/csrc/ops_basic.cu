@@ -1,7 +1,6 @@
 // Op-level kernels behind torch_utils.ops.{bias_act, upfirdn2d, filtered_lrelu} (forward only).
 // Memory-bound: one pass, 128-bit accesses where the layout allows, grid sized to the SM count.
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 
 template <typename T> struct Vec4;
 template <> struct Vec4<float> { typedef float4 type; };
@@ -68,7 +67,7 @@ extern "C" int n3d_bias_act(const void* x, const void* b, void* y, int dtype, in
     N3D_CHECK_ARG(dtype == N3D_DTYPE_F32 || dtype == N3D_DTYPE_F16, "n3d_bias_act: unsupported dtype %d", dtype);
     N3D_CHECK_ARG(!b || (size_b > 0 && step_b > 0), "n3d_bias_act: bad bias geometry");
     if (numel == 0) return N3D_OK;
-    const int grid = (int)min((int64_t)132 * 8, (int64_t)n3d_div_up(numel, 1024));
+    const int grid = n3d_grid((numel + 3) / 4, 256);        // 4 elements per thread
     if (dtype == N3D_DTYPE_F32)
         bias_act_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)x, (const float*)b, (float*)y, numel,
                                                                         size_b, step_b, act, alpha, gain, clamp);
@@ -146,7 +145,7 @@ extern "C" int n3d_upfirdn2d(const void* x, const float* f, void* y, int dtype, 
     p.w_fastest = (y_strides[3] == 1) ? 1 : 0;
     const int64_t total = (int64_t)N * C * outH * outW;
     if (total == 0) return N3D_OK;
-    const int grid = (int)min((int64_t)132 * 16, (int64_t)n3d_div_up(total, 256));
+    const int grid = n3d_grid(total, 256, 16);
     const size_t smem = (size_t)fh * fw * sizeof(float);
     if (dtype == N3D_DTYPE_F32)
         upfirdn2d_kernel<float><<<grid, 256, smem, (cudaStream_t)stream>>>((const float*)x, f, (float*)y, p);
@@ -228,7 +227,7 @@ extern "C" int n3d_filtered_lrelu(const void* x, const float* fu, const float* f
     N3D_CHECK_ARG(outH == (upH - fdh + down) / down && outW == (upW - fdw + down) / down, "n3d_filtered_lrelu: bad output size");
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t t1 = (int64_t)N * C * upH * upW, t2 = (int64_t)N * C * outH * outW;
-    const int g1 = (int)min((int64_t)132 * 16, (int64_t)n3d_div_up(t1, 256)), g2 = (int)min((int64_t)132 * 16, (int64_t)n3d_div_up(t2, 256));
+    const int g1 = n3d_grid(t1, 256, 16), g2 = n3d_grid(t2, 256, 16);
     if (dtype == N3D_DTYPE_F32) {
         flrelu_up_kernel<float><<<g1, 256, fuh * fuw * 4, st>>>((const float*)x, (const float*)b, fu, tmp, N, C, H, W, fuh, fuw, up,
                                                                 padx0, pady0, flip, upH, upW, gain, slope, clamp);

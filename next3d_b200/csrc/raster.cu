@@ -3,16 +3,8 @@
 // These replace pytorch3d.rasterize_meshes, F.grid_sample, cv2.floodFill (host round trip), numpy (host round trip)
 // and F.interpolate(antialias=True) on the reference's path (triplane_next3d.py:146-174, 190-230, 330-344).
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 
 namespace {
-constexpr int kSMs = 132;
-inline int grid_for(int64_t work_items, int threads, int per_sm = 8) {
-    int64_t g = (work_items + threads - 1) / threads;
-    int64_t cap = (int64_t)kSMs * per_sm;
-    return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // ---------------------------------------------------------------------------------------------- transform
 // p' = ((p*[1,-1,1]) @ R + [0,-.01,-.01]) * 5 ; y,z negated ; z += zoff ; optional NDC x,y negation.  The 3-term dot products
 // are evaluated as the fused chain fma(z, R2j, fma(y, R1j, x * R0j)) -- what torch.bmm's CPU kernel computes for K = 3 -- so the
@@ -504,7 +496,7 @@ __global__ void __launch_bounds__(256) blend_kernel(const float* __restrict__ fr
 extern "C" int n3d_transform_points(const float* pts, int N, int P, const float* rot, int nviews, float zoff, int ndc_flip,
                                     float* out, void* stream) {
     N3D_CHECK_ARG(pts && rot && out && N > 0 && P > 0 && nviews > 0, "n3d_transform_points: bad args");
-    transform_kernel<<<grid_for((int64_t)N * nviews * P, 256), 256, 0, (cudaStream_t)stream>>>(pts, N, P, rot, nviews, zoff, ndc_flip, out);
+    transform_kernel<<<n3d_grid((int64_t)N * nviews * P, 256), 256, 0, (cudaStream_t)stream>>>(pts, N, P, rot, nviews, zoff, ndc_flip, out);
     N3D_CHECK_LAUNCH("n3d_transform_points");
     return N3D_OK;
 }
@@ -514,7 +506,7 @@ extern "C" int n3d_rasterize(const float* verts, const int32_t* faces, int NM, i
     N3D_CHECK_ARG(verts && faces && pix_to_face && bary && workspace && NM > 0 && F > 0 && H > 0 && W > 0, "n3d_rasterize: bad args");
     N3D_CHECK_ARG(NM <= 65535, "n3d_rasterize: too many images (%d)", NM);
     N3D_CHECK_ARG(((uintptr_t)workspace & 15) == 0, "n3d_rasterize: workspace must be 16-byte aligned");
-    raster_setup_kernel<<<grid_for((int64_t)NM * F, 256), 256, 0, (cudaStream_t)stream>>>(verts, faces, NM, V, F, workspace);
+    raster_setup_kernel<<<n3d_grid((int64_t)NM * F, 256), 256, 0, (cudaStream_t)stream>>>(verts, faces, NM, V, F, workspace);
     dim3 grid(((W + kBin - 1) / kBin) * ((H + kBin - 1) / kBin), NM);
     rasterize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(workspace, F, H, W, pix_to_face, bary);
     N3D_CHECK_LAUNCH("n3d_rasterize");
@@ -526,7 +518,7 @@ extern "C" int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, cons
                              float* tex_planes, float* alpha, void* stream) {
     N3D_CHECK_ARG(pix_to_face && bary && face_uv && texture && eye_mask && tex_planes && alpha, "n3d_uv_sample: null pointer");
     N3D_CHECK_ARG(C <= 32, "n3d_uv_sample: C %d > 32 not supported", C);
-    uv_sample_kernel<<<grid_for((int64_t)N * H * W * 32, 256, 16), 256, 0, (cudaStream_t)stream>>>(pix_to_face, bary, face_uv, texture, eye_mask, N, H,
+    uv_sample_kernel<<<n3d_grid((int64_t)N * H * W * 32, 256, 16), 256, 0, (cudaStream_t)stream>>>(pix_to_face, bary, face_uv, texture, eye_mask, N, H,
                                                                                                 W, TH, TW, C, MH, MW, tex_planes, alpha);
     N3D_CHECK_LAUNCH("n3d_uv_sample");
     return N3D_OK;
@@ -535,15 +527,7 @@ extern "C" int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, cons
 extern "C" int n3d_fill_mouth(float* alpha, int NI, int H, int W, void* stream) {
     N3D_CHECK_ARG(alpha && NI > 0 && H > 0 && W > 0, "n3d_fill_mouth: bad args");
     N3D_CHECK_ARG((int64_t)H * (W + 4) <= 200 * 1024, "n3d_fill_mouth: image %dx%d too large for the shared-memory state map", H, W);
-    N3DDeviceState* D = n3d_device_state();
-    if (!D) return N3D_ERR_CUDA;
-    if (!(D->configured & N3D_CFG_FILL_MOUTH)) {
-        if (cudaFuncSetAttribute(fill_mouth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) {
-            n3d_set_error("n3d_fill_mouth: cannot raise dynamic shared memory");
-            return N3D_ERR_CUDA;
-        }
-        D->configured |= N3D_CFG_FILL_MOUTH;
-    }
+    if (int rc = n3d_smem_optin((const void*)fill_mouth_kernel, 200 * 1024, "n3d_fill_mouth")) return rc;
     fill_mouth_kernel<<<NI, 1024, (size_t)H * (W + 4), (cudaStream_t)stream>>>(alpha, H, W);
     N3D_CHECK_LAUNCH("n3d_fill_mouth");
     return N3D_OK;
@@ -563,10 +547,10 @@ extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, con
     const bool wide = (C % 4 == 0) && C <= 128 && (32 % (C / 4) == 0) && ((uintptr_t)src % 16 == 0);
     const int ppw = 4;
     if (wide)
-        resize_aa_kernel<<<grid_for((int64_t)N * DH * DW * 32 / ppw, 256, 16), 256, 0, (cudaStream_t)stream>>>(
+        resize_aa_kernel<<<n3d_grid((int64_t)N * DH * DW * 32 / ppw, 256, 16), 256, 0, (cudaStream_t)stream>>>(
             src, N, SH, SW, C, src_box, dst, DH, DW, dst_box, style, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, ppw);
     else
-        resize_aa_scalar_kernel<<<grid_for((int64_t)N * DH * DW * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(
+        resize_aa_scalar_kernel<<<n3d_grid((int64_t)N * DH * DW * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(
             src, N, SH, SW, C, src_box, dst, DH, DW, dst_box, style, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
     N3D_CHECK_LAUNCH("n3d_resize_aa");
     return N3D_OK;
@@ -575,7 +559,7 @@ extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, con
 extern "C" int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
                                 int N, int H, int W, float* planes, void* stream) {
     N3D_CHECK_ARG(blended_front && tex_planes && alpha && static_planes && planes, "n3d_blend_planes: null pointer");
-    blend_kernel<<<grid_for((int64_t)N * 3 * H * W * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(blended_front, tex_planes, alpha, static_planes, N, H * W, planes);
+    blend_kernel<<<n3d_grid((int64_t)N * 3 * H * W * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(blended_front, tex_planes, alpha, static_planes, N, H * W, planes);
     N3D_CHECK_LAUNCH("n3d_blend_planes");
     return N3D_OK;
 }

@@ -1,4 +1,4 @@
-// Device helpers shared by the fused renderer (render_fused.cu) and the point-sampling kernel (renderer.cu): counter RNG,
+// Device helpers shared by the fused renderer and the point-sampling kernel (both in render_fused.cu): counter RNG,
 // torch.linspace arithmetic, the manual shared-memory swizzles matching the TMA / wgmma SWIZZLE_64B / SWIZZLE_128B layouts, MUFU-based
 // activations and the decoder-weight staging (fp32 -> bf16 hi/lo B-operand tiles).
 #pragma once

@@ -23,7 +23,6 @@
 // are known, stored as 16-bit unsigned normalised values (absolute error <= 2^-17, below the fp32 decoder's own error after
 // compositing); then each thread accumulates coefficient x colour for its own rows.
 #include "common.cuh"
-#include "../../include/next3d_b200.h"
 #include "tc_ptx.cuh"
 #include "render_common.cuh"
 
@@ -67,7 +66,6 @@ struct FusedK {
     int gw, log2gw;              // pixel block of a group: gw x 2
     int blocks_x, gpi;           // group map: blocks of 4 x 8 groups, groups per image (padded)
     long long total_groups;
-    int mode;                    // diagnostics: bit 0 = all taps read texel 0 (no cache misses)
 };
 
 // ---------------------------------------------------------------------------------------------------------------- group -> rays
@@ -508,7 +506,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             } else if (valid) {
                 depth = coarse_depth(K, seed, ray.gr, k);
             }
-            setup_taps(taps, lane, ray.ox + depth * ray.dx, ray.oy + depth * ray.dy, ray.oz + depth * ray.dz, valid && !(K.mode & 1), ray.img4, P.PH, P.PW,
+            setup_taps(taps, lane, ray.ox + depth * ray.dx, ray.oy + depth * ray.dy, ray.oz + depth * ray.dz, valid, ray.img4, P.PH, P.PW,
                        K.scale);
             __syncwarp();
             const int b = ti % kNF;
@@ -1123,7 +1121,7 @@ __global__ void __launch_bounds__(kThreads, 1) gather_floor_kernel(const __grid_
         const bool valid = ray.ok && k < P.depth_coarse;
         // second pass: the fine samples sit near the coarse ones (shifted by half a step) -- same count, same locality
         const float depth = valid ? coarse_depth(K, P.seed + pass, ray.gr, k) + (pass ? 0.5f * K.delta_coarse : 0.f) : 0.f;
-        setup_taps(taps, lane, ray.ox + depth * ray.dx, ray.oy + depth * ray.dy, ray.oz + depth * ray.dz, valid && !(K.mode & 1), ray.img4, P.PH, P.PW,
+        setup_taps(taps, lane, ray.ox + depth * ray.dx, ray.oy + depth * ray.dy, ray.oz + depth * ray.dz, valid, ray.img4, P.PH, P.PW,
                    K.scale);
         __syncwarp();
         gather_rows(P.planes, taps, f_hi, f_lo, q * 32, lane);
@@ -1161,13 +1159,24 @@ __global__ void __launch_bounds__(kThreads, 1) mufu_floor_kernel(long long sampl
     }
     if (sink && acc == 123.456f) sink[0] = acc;
 }
-}  // namespace
 
-int n3d_render_floor_launch(const N3DRender* p, int kind, float* sink, void* stream) {
-    N3DDeviceState* D = n3d_device_state();
-    if (!D) return N3D_ERR_CUDA;
-    const int dmaxv = p->depth_coarse > p->depth_fine ? p->depth_coarse : p->depth_fine;
-    const int L = dmaxv <= 48 ? 16 : 32;
+// Depth clamp of the composited depth to the batch-global depth range (ray_marcher.py:53-54).
+__global__ void __launch_bounds__(256) depth_clamp_kernel(float* __restrict__ depth, int64_t n, const float* __restrict__ mm) {
+    const float lo = mm[0], hi = mm[1];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float d = depth[i];
+        if (isnan(d)) d = INFINITY;
+        depth[i] = fminf(fmaxf(d, lo), hi);
+    }
+}
+
+constexpr int kMaxD = kMaxT * 32;               // depth samples per pass the fused kernel lays out (3 tiles x 32 lanes per ray)
+
+// Work decomposition of the renderer and of the floor micro-kernels for the workload p; L = lanes per ray (16 up to 48 samples
+// per pass, else 32).
+FusedK make_fused(const N3DRender* p, int& L) {
+    const int dmax = p->depth_coarse > p->depth_fine ? p->depth_coarse : p->depth_fine;
+    L = dmax <= 48 ? 16 : 32;
     FusedK K;
     K.p = *p;
     K.M = p->res * p->res;
@@ -1181,66 +1190,14 @@ int n3d_render_floor_launch(const N3DRender* p, int kind, float* sink, void* str
     K.blocks_x = (tiles_x + 3) / 4;
     K.gpi = K.blocks_x * ((tiles_y + 7) / 8) * 32;
     K.total_groups = (long long)p->N * K.gpi;
-    K.mode = 0;
-    const int grid = (int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms);
-    if (kind == 0) {
-        const size_t smem = 32768 + kWarps * kTapBytesPerWarp + 1024;
-        if (cudaFuncSetAttribute(gather_floor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-            n3d_set_error("n3d_render_floor: cannot raise dynamic shared memory");
-            return N3D_ERR_CUDA;
-        }
-        gather_floor_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(K, sink);
-    } else {
-        const long long samples = (long long)p->N * K.M * (p->depth_coarse + p->depth_fine);
-        mufu_floor_kernel<<<D->num_sms, kThreads, 0, (cudaStream_t)stream>>>(samples, sink);
-    }
-    N3D_CHECK_LAUNCH("n3d_render_floor");
-    return N3D_OK;
-}
-
-int n3d_render_fused_launch(const N3DRender* p, void* stream, int mode) {
-    const int dmaxv = p->depth_coarse > p->depth_fine ? p->depth_coarse : p->depth_fine;
-    const int L = dmaxv <= 48 ? 16 : 32;
-    FusedK K;
-    K.p = *p;
-    K.M = p->res * p->res;
-    K.delta_coarse = (float)(((double)p->ray_end - (double)p->ray_start) / (double)(p->depth_coarse - 1));
-    K.scale = 2.f / p->box_warp;
-    K.Tc = (p->depth_coarse + L - 1) / L;
-    K.Tf = (p->depth_fine + L - 1) / L;
-    K.gw = L == 16 ? 4 : 2;
-    K.log2gw = L == 16 ? 2 : 1;
-    const int tiles_x = (p->res + K.gw - 1) / K.gw, tiles_y = (p->res + 1) / 2;
-    K.blocks_x = (tiles_x + 3) / 4;
-    const int blocks_y = (tiles_y + 7) / 8;
-    K.gpi = K.blocks_x * blocks_y * 32;
-    K.total_groups = (long long)p->N * K.gpi;
-    K.mode = mode;
-    N3DDeviceState* D = n3d_device_state();
-    if (!D) return N3D_ERR_CUDA;
-    const size_t smem = (size_t)kSmemBytes + 1024;
-    const unsigned bit = L == 16 ? N3D_CFG_RENDER16 : N3D_CFG_RENDER32;
-    if (!(D->configured & bit)) {
-        const cudaError_t e = L == 16 ? cudaFuncSetAttribute(render_fused_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                      : cudaFuncSetAttribute(render_fused_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) {
-            n3d_set_error("n3d_render_rays: cannot raise dynamic shared memory: %s", cudaGetErrorString(e));
-            return N3D_ERR_CUDA;
-        }
-        D->configured |= bit;
-    }
-    const int grid = (int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms);
-    if (L == 16) render_fused_kernel<16><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
-    else render_fused_kernel<32><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
-    N3D_CHECK_LAUNCH("n3d_render_rays");
-    return N3D_OK;
+    return K;
 }
 
 // coords != nullptr: arbitrary points [N, Pn, 3].  coords == nullptr: voxel grid of `grid_n`^3 points (image 0), flat indices
 // head .. head + Pn - 1, sigma written flipped + trimmed into the [grid_n]^3 output.
-int n3d_points_fused_launch(const float* planes, int N, int PH, int PW, const float* coords, long long Pn, float box_warp, const float* w0,
-                            const float* b0, const float* w1, const float* b1, float* sigma, float* rgb, int grid_n, float cube_length, long long head,
-                            int pad, float pad_value, void* stream) {
+int launch_points(const float* planes, int N, int PH, int PW, const float* coords, long long Pn, float box_warp, const float* w0,
+                  const float* b0, const float* w1, const float* b1, float* sigma, float* rgb, int grid_n, float cube_length, long long head,
+                  int pad, float pad_value, void* stream) {
     PointsK K;
     K.planes = planes; K.N = N; K.PH = PH; K.PW = PW; K.coords = coords; K.Pn = Pn; K.total = (long long)N * Pn;
     K.scale = 2.f / box_warp;
@@ -1252,21 +1209,87 @@ int n3d_points_fused_launch(const float* planes, int N, int PH, int PW, const fl
         K.voxel_size = (float)((double)cube_length / (double)(grid_n - 1));
         K.org0 = K.org1 = K.org2 = (float)(0.0 - (double)cube_length / 2.0);
     }
-    N3DDeviceState* D = n3d_device_state();
+    const int smem = kSmemBytes + 1024;
+    if (int rc = n3d_smem_optin(rgb ? (const void*)points_fused_kernel<true> : (const void*)points_fused_kernel<false>, smem, "n3d_sample_points"))
+        return rc;
+    const N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
-    const size_t smem = (size_t)kSmemBytes + 1024;
-    if (!(D->configured & N3D_CFG_POINTS)) {
-        if (cudaFuncSetAttribute(points_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-            cudaFuncSetAttribute(points_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-            n3d_set_error("n3d_sample_points: cannot raise dynamic shared memory");
-            return N3D_ERR_CUDA;
-        }
-        D->configured |= N3D_CFG_POINTS;
-    }
     const long long tiles = (K.total + 127) / 128;
     const int grid = (int)(tiles < D->num_sms ? tiles : D->num_sms);
     if (rgb) points_fused_kernel<true><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
     else points_fused_kernel<false><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
     N3D_CHECK_LAUNCH("n3d_sample_points");
     return N3D_OK;
+}
+}  // namespace
+
+extern "C" int n3d_render_rays(const N3DRender* p, void* stream) {
+    N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && p->w0 && p->b0 && p->w1 && p->b1 && p->rgb && p->depth && p->wsum,
+                  "n3d_render_rays: null pointer");
+    if (p->depth_coarse > kMaxD || p->depth_fine > kMaxD) {
+        n3d_set_error("n3d_render_rays: depth resolutions (%d, %d) above %d samples per pass are not supported", p->depth_coarse, p->depth_fine, kMaxD);
+        return N3D_ERR_UNSUPPORTED;
+    }
+    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_fine >= 0, "n3d_render_rays: depth resolutions (%d, %d): need coarse >= 4, fine >= 0",
+                  p->depth_coarse, p->depth_fine);
+    N3D_CHECK_ARG(p->res >= 1 && p->N >= 1 && p->ray_start > 0.f && p->ray_end > p->ray_start && p->box_warp > 0.f, "n3d_render_rays: bad ray setup");
+    N3D_CHECK_ARG((long long)p->N * 3 * p->PH * p->PW * 128 < (1ll << 32), "n3d_render_rays: plane tensor too large for 32-bit texel offsets");
+    int L;
+    const FusedK K = make_fused(p, L);
+    const int smem = kSmemBytes + 1024;
+    if (int rc = n3d_smem_optin(L == 16 ? (const void*)render_fused_kernel<16> : (const void*)render_fused_kernel<32>, smem, "n3d_render_rays"))
+        return rc;
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
+    const int grid = (int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms);
+    if (L == 16) render_fused_kernel<16><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    else render_fused_kernel<32><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    N3D_CHECK_LAUNCH("n3d_render_rays");
+    return N3D_OK;
+}
+
+extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream) {
+    N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && (kind == 0 || kind == 1), "n3d_render_floor: bad args");
+    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_coarse <= kMaxD && p->depth_fine >= 0 && p->depth_fine <= kMaxD, "n3d_render_floor: depth resolutions");
+    int L;
+    const FusedK K = make_fused(p, L);
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
+    if (kind == 0) {
+        const int smem = 32768 + kWarps * kTapBytesPerWarp + 1024;
+        if (int rc = n3d_smem_optin((const void*)gather_floor_kernel, smem, "n3d_render_floor")) return rc;
+        gather_floor_kernel<<<(int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms), kThreads, smem, (cudaStream_t)stream>>>(K, sink);
+    } else {
+        const long long samples = (long long)p->N * K.M * (p->depth_coarse + p->depth_fine);
+        mufu_floor_kernel<<<D->num_sms, kThreads, 0, (cudaStream_t)stream>>>(samples, sink);
+    }
+    N3D_CHECK_LAUNCH("n3d_render_floor");
+    return N3D_OK;
+}
+
+extern "C" int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* stream) {
+    N3D_CHECK_ARG(depth && depth_minmax && n >= 0, "n3d_depth_clamp: bad args");
+    if (n == 0) return N3D_OK;
+    depth_clamp_kernel<<<n3d_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(depth, n, depth_minmax);
+    N3D_CHECK_LAUNCH("n3d_depth_clamp");
+    return N3D_OK;
+}
+
+extern "C" int n3d_sample_points(const float* planes, int N, int PH, int PW, const float* coords, int64_t P, float box_warp,
+                                 const float* w0, const float* b0, const float* w1, const float* b1, float* sigma, float* rgb,
+                                 void* stream) {
+    N3D_CHECK_ARG(planes && coords && w0 && b0 && w1 && b1 && sigma && N >= 1 && P >= 1 && box_warp > 0.f, "n3d_sample_points: bad args");
+    N3D_CHECK_ARG((long long)N * 3 * PH * PW * 128 < (1ll << 32), "n3d_sample_points: plane tensor too large for 32-bit texel offsets");
+    return launch_points(planes, N, PH, PW, coords, P, box_warp, w0, b0, w1, b1, sigma, rgb, 0, 0.f, 0, 0, 0.f, stream);
+}
+
+extern "C" int n3d_sample_grid(const float* planes, int PH, int PW, int grid_n, float cube_length, float box_warp, int64_t head, int64_t count,
+                               int pad, float pad_value, const float* w0, const float* b0, const float* w1, const float* b1, float* sigma_grid,
+                               void* stream) {
+    N3D_CHECK_ARG(planes && w0 && b0 && w1 && b1 && sigma_grid && grid_n >= 2 && cube_length > 0.f && box_warp > 0.f, "n3d_sample_grid: bad args");
+    N3D_CHECK_ARG(head >= 0 && count >= 1 && head + count <= (int64_t)grid_n * grid_n * grid_n, "n3d_sample_grid: index range outside the grid");
+    N3D_CHECK_ARG(pad >= 0 && 2 * pad <= grid_n, "n3d_sample_grid: bad trim width");
+    N3D_CHECK_ARG((long long)3 * PH * PW * 128 < (1ll << 32), "n3d_sample_grid: plane tensor too large for 32-bit texel offsets");
+    return launch_points(planes, 1, PH, PW, nullptr, count, box_warp, w0, b0, w1, b1, sigma_grid, nullptr, grid_n, cube_length, head, pad,
+                         pad_value, stream);
 }

@@ -8,7 +8,7 @@ Execution model (see DESIGN.md):
     demodulation is applied in the epilogue), with noise / bias / lrelu / clamp / next-layer modulation / bf16 split fused;
   * up-convs: 4 parity-class GEMMs (stride-2 transposed conv, conv2d_resample.py:114-127) + one FIR-epilogue kernel;
   * down-convs: FIR + parity split kernel, then one GEMM over 9 unit-stride taps;
-  * mesh path, volume renderer, resizes, blending: one kernel each (raster.cu, renderer.cu).
+  * mesh path, volume renderer, resizes, blending: one kernel each (raster.cu, render_fused.cu).
 Reference call order: triplane_next3d.py:117-188.
 """
 import math
@@ -72,7 +72,7 @@ class Engine:
         self.cfg, self.device, self.nprod = cfg, torch.device(device), nprod
         self.rk = cfg.rendering_kwargs
         self.mod, self.plain = {}, {}
-        self.launches = 0
+        self.launches = 0                       # kernels launched by the last synthesis() / compute_planes() call (counted in kernels.py)
         self.conv_flops = 0.0
         self.prof = None
         self._cur_layer = ''
@@ -285,7 +285,6 @@ class Engine:
         ev = self._prof_begin()                  # the reduction pass is part of this convolution: counted as conv time (0 extra FLOPs)
         K.splitk_epilogue(part, **epi)
         self._prof_end(ev, 'conv_gemm', 0.0, (name, a.hi.shape[-1], L.cout, res, res, 0))
-        self.launches += 2
 
     def _modconv(self, name, a, res_in, outs, noise_mode, f32=None, rgb=None):
         """SynthesisLayer (networks_stylegan2.py:311-330); `a` already carries this layer's modulation."""
@@ -301,7 +300,6 @@ class Engine:
             self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_conv3x3(), N, res_in, res_in, nprod=self.nprod, dcoef=self._dcoef(L), bias=L.bias,
                         noise=noise, noise_nstride=nstride, gain=SQRT2, slope=0.2, clamp=clamp, outs=outs, out_f32=f32,
                         f32_cstride=L.cout if f32 is not None else 0, rgb=rgb)
-            self.launches += 1
             return
         assert rgb is None
         raw = self._f32(N, 2 * res_in + 1, 2 * res_in + 1, L.cout)
@@ -312,7 +310,6 @@ class Engine:
         self._prof_end(ev, 'conv_gemm', flops, (name, L.cin, L.cout, res_in + 1, res_in + 1, 9))
         K.fir_up_epilogue(raw, L.cout, self._dcoef(L), L.bias, noise, SQRT2, 0.2, clamp, outs=outs, out_f32=f32,
                           f32_cstride=L.cout if f32 is not None else 0, noise_nstride=nstride)
-        self.launches += 2
 
     def _torgb(self, name, a, res, img, accumulate, nchw=False):
         """ToRGBLayer (networks_stylegan2.py:353-357): 1x1 modulated conv without demodulation, linear bias (+ clamp)."""
@@ -320,7 +317,6 @@ class Engine:
         self._cur_layer = name
         self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_conv1x1(), self._N, res, res, nprod=self.nprod, bias=L.bias,
                     clamp=L.clamp if L.clamp is not None else -1.0, out_f32=img, f32_cstride=L.cout, f32_nchw=nchw, f32_accumulate=accumulate)
-        self.launches += 1
 
     def _plainconv(self, name, a, res, act, outs=(), f32=None, accumulate=False, stride2=False):
         """styleunet Conv2dLayer (networks_stylegan2_styleunet.py:198-207): weight_gain folded into the packed weights."""
@@ -338,7 +334,6 @@ class Engine:
             taps = K.taps_conv3x3() if L.k == 3 else K.taps_conv1x1()
             self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, taps, N, res, res, nprod=self.nprod, bias=L.bias, gain=gain, slope=slope, outs=outs,
                         out_f32=f32, f32_cstride=L.cout if f32 is not None else 0, f32_accumulate=accumulate)
-        self.launches += 1
 
     # ------------------------------------------------------------------------------------------ networks
     def _synthesis_blocks(self, prefix, x, res_list, cimg, noise_mode, concat_next=None, final_nchw=None, img=None):
@@ -376,7 +371,6 @@ class Engine:
                     K.upsample2d_nhwc(img, up)
                     self._torgb(f'{p}.torgb', rgb_in, res, up, accumulate=True)
                     img = up
-                self.launches += 1
             if concat_next and res in concat_next:
                 x = concat_next[res][1]()                      # run the fusion conv, returns the next conv0's input
         return img
@@ -393,7 +387,6 @@ class Engine:
         self._modconv(f'{prefix}.b4.conv1', x0, 4, [self._out(rgb_in, f'{prefix}.b4.torgb'), self._out(x, f'{prefix}.b8.conv0')], noise_mode)
         img = self._f32(N, 4, 4, cimg)
         self._torgb(f'{prefix}.b4.torgb', rgb_in, 4, img, accumulate=False)
-        self.launches += 1
         return self._synthesis_blocks(prefix, x, _config.block_resolutions(cfg.plane_res)[1:], cimg, noise_mode, img=img)
 
     def _styleunet(self, prefix, x_in, in_size, final_size, num_cond_res, noise_mode):
@@ -421,24 +414,20 @@ class Engine:
             if i > 0:
                 xd = self._f32(N, r, r, cfg.plane_ch)
                 K.downsample2d_nhwc(x, xd)
-                self.launches += 1
                 x = xd
             xs = Split((N, r, r, cfg.plane_ch), dev)
             K.modulate_split(x, None, xs.hi, xs.lo)
-            self.launches += 1
             h = Split((N, r, r, cin), dev)
             if skip is None:
                 self._plainconv(f'{p}.fromrgb', xs, r, 'linear', outs=[K.make_split_out(h.hi, h.lo, None, cin, 0)])
             else:
                 self._plainconv(f'{p}.fromrgb', xs, r, 'linear', f32=skip, accumulate=True)       # out = fromrgb(x) + skip
                 K.modulate_split(skip, None, h.hi, h.lo)
-                self.launches += 1
             c1 = self._f32(N, r, r, cin)
             self._plainconv(f'{p}.conv1', h, r, 'lrelu', f32=c1)
             sh = (r + 2) // 2
             par = Split((4 * N, sh, sh, cin), dev)
             K.fir_down_split(c1, par.hi, par.lo)
-            self.launches += 1
             # cond of this block lives at resolution r/2; cond_list (reversed) index:
             j = n_enc - 1 - i
             cout = cfg.channels(r // 2)
@@ -481,11 +470,9 @@ class Engine:
             K.resize_aa(feat, None, r0, r0, style=self._style(self.mod[f'{p0}.conv0']), hi=x.hi, lo=x.lo)
             rgb = self._f32(N, r0, r0, 3)
             K.resize_aa(rgb_lo, rgb)
-            self.launches += 2
         else:
             K.modulate_split(feat, self._style(self.mod[f'{p0}.conv0']), x.hi, x.lo)
             rgb = rgb_lo
-            self.launches += 1
         # block0
         res0 = r0 * (2 if cfg.sr_module == '8XDC' else 1)
         x1 = Split((N, res0, res0, c0), dev)
@@ -494,7 +481,6 @@ class Engine:
         if cfg.sr_module == '8XDC':
             img = self._f32(N, res0, res0, 3)
             K.upsample2d_nhwc(rgb, img)
-            self.launches += 1
         else:
             img = rgb.clone()                                                   # SynthesisBlockNoUp: no image upsample
         # the two ToRGB layers (3 channels) run inside the conv1 epilogues: img += torgb(conv1 output)
@@ -505,7 +491,6 @@ class Engine:
         self._modconv(f'{p1}.conv0', x2, res0, [self._out(x3, f'{p1}.conv1')], noise_mode_sr)
         K.upsample2d_nhwc(img, image_out, y_nchw=True)
         self._modconv(f'{p1}.conv1', x3, res1, [], noise_mode_sr, rgb=self._fused_rgb(f'{p1}.torgb', image_out, True, nchw=True))
-        self.launches += 1
 
     # ------------------------------------------------------------------------------------------ planes + synthesis
     def _on_device(self, **tensors):
@@ -520,7 +505,10 @@ class Engine:
         """Everything up to the blended tri-planes (triplane_next3d.py:137-174) -> [N,3,256,256,32] channels-last fp32."""
         self._on_device(ws=ws, v=v)
         with torch.cuda.device(self.device):
-            return self._compute_planes(ws, v, noise_mode, return_intermediates)
+            n0 = K.launches
+            out = self._compute_planes(ws, v, noise_mode, return_intermediates)
+            self.launches = K.launches - n0
+            return out
 
     def _compute_planes(self, ws, v, noise_mode='const', return_intermediates=False):
         cfg, dev = self.cfg, self.device
@@ -535,7 +523,6 @@ class Engine:
         self._dcoefs = self._f32(self.dcoef_elems * N)
         K.styles(ws, self.aff_w, self.aff_b, self.row_widx, self.row_scale, s_ooff, self.row_cin, self._styles)
         K.demod(self._styles, self.wsq, self.d_woff, self.d_cin, d_soff, d_ooff, self.d_cout, self._dcoefs, N)
-        self.launches += 2
         # Three independent branches (triplane_next3d.py:137-170): (1) neural texture -> UV lookup -> mouth / blending UNets,
         # (2) mesh rasterization + mouth box (needs only the vertices), (3) the static tri-plane backbone (needed only by the final
         # blend).  (2) and (3) run on side streams: their latency-bound kernels (4^2..32^2 layers on a few dozen SMs, the flood
@@ -572,7 +559,6 @@ class Engine:
         alpha = self._f32(3, N, P, P)
         K.uv_sample(p2f, bary, self.face_uv, textures, self.eye_mask, tex_planes, alpha)
         K.fill_mouth(alpha)
-        self.launches += 7                                                          # rasterize = setup pass + bin pass
         # mouth crop -> StyleUNet -> paste back -> neural blending
         front = tex_planes[0]
         crop = self._f32(N, 64, 64, cfg.plane_ch)
@@ -586,7 +572,6 @@ class Engine:
             static.record_stream(main)
         planes = self._f32(N, 3, P, P, cfg.plane_ch)
         K.blend_planes(blended, tex_planes, alpha, static, planes)
-        self.launches += 3
         if return_intermediates:
             return planes, dict(textures=textures, pix_to_face=p2f.view(N, 4, P, P), tex_planes=tex_planes, alpha=alpha, boxes=boxes,
                                 mouth_crop=crop, mouth_plane=mouth, stitched=stitched, blended_front=blended, static=static, lm2d=lm2d)
@@ -603,7 +588,7 @@ class Engine:
         cfg, dev = self.cfg, self.device
         N = ws.shape[0]
         R = neural_rendering_resolution or cfg.neural_rendering_resolution
-        self.launches = 0
+        n0 = K.launches
         self.conv_flops = 0.0
         out = self._compute_planes(ws, v, noise_mode, return_intermediates)
         planes, inter = out if return_intermediates else (out, None)
@@ -624,7 +609,7 @@ class Engine:
         K.depth_clamp(depth, mm)
         image = self._f32(N, 3, cfg.img_resolution, cfg.img_resolution)
         self._superresolution(feat, self.rk['superresolution_noise_mode'], image)
-        self.launches += 2
+        self.launches = K.launches - n0
         result = {'image': image, 'image_raw': feat.permute(0, 3, 1, 2)[:, :3], 'image_depth': depth}
         if return_intermediates:
             inter.update(planes=planes, feature_image=feat, weights_sum=wsum)

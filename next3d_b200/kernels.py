@@ -12,6 +12,17 @@ from ._lib import lib, check, ptr, stream_ptr
 
 BF16 = torch.bfloat16
 
+# Kernels launched through this module so far (Engine.launches is its difference across one forward).  One counter per process is
+# enough: the supported multi-GPU model is one process per GPU (DESIGN.md section 7).
+launches = 0
+
+
+def _run(fn, *args, kernels=1):
+    """Call entry point `fn`, raise on an error status, and count the `kernels` it launches."""
+    global launches
+    check(getattr(lib, fn)(*args), fn)
+    launches += kernels
+
 
 # ------------------------------------------------------------------------------------------------ packing helpers
 def split_bf16(x):
@@ -52,10 +63,8 @@ def make_split_out(hi=None, lo=None, style=None, cstride=0, coff=0):
 
 
 # ------------------------------------------------------------------------------------------------ kernels
-def conv_gemm(a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, *, a_img_mul=0, nprod=3, mode=0, dcoef=None, bias=None, noise=None,
-              noise_nstride=0, gain=1.0, slope=1.0, clamp=-1.0, outs=(), out_f32=None, f32_cstride=0, f32_coff=0, f32_nchw=False,
-              f32_accumulate=False, oy_mul=1, oy_off=0, ox_mul=1, ox_off=0, OH=None, OW=None, rgb=None, splits=1, split_stride=0):
-    """a_*: bf16 [NI, AH, AW, Cin]; w_*: bf16 [T, Cout, Cin]; taps: list of (dy, dx, img_off, wtap)."""
+def _conv_desc(a_hi, a_lo, w_hi, w_lo, N, MH, MW, nprod):
+    """ConvGemm descriptor with the operands (a_*: bf16 [NI, AH, AW, Cin]; w_*: bf16 [T, Cout, Cin]) and the M-space filled in."""
     NI, AH, AW, Cin = a_hi.shape
     T, Cout, Cin_w = w_hi.shape
     assert Cin_w == Cin, (Cin_w, Cin)
@@ -64,11 +73,21 @@ def conv_gemm(a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, *, a_img_mul=0, nprod=3, 
     p.NI, p.AH, p.AW, p.Cin = NI, AH, AW, Cin
     p.w_hi, p.w_lo = ptr(w_hi), ptr(w_lo)
     p.T, p.Cout = T, Cout
-    p.N, p.MH, p.MW, p.a_img_mul = N, MH, MW, a_img_mul
+    p.N, p.MH, p.MW = N, MH, MW
+    p.nprod = nprod
+    return p
+
+
+def conv_gemm(a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, *, a_img_mul=0, nprod=3, mode=0, dcoef=None, bias=None, noise=None,
+              noise_nstride=0, gain=1.0, slope=1.0, clamp=-1.0, outs=(), out_f32=None, f32_cstride=0, f32_coff=0, f32_nchw=False,
+              f32_accumulate=False, oy_mul=1, oy_off=0, ox_mul=1, ox_off=0, OH=None, OW=None, rgb=None, splits=1, split_stride=0):
+    """a_*: bf16 [NI, AH, AW, Cin]; w_*: bf16 [T, Cout, Cin]; taps: list of (dy, dx, img_off, wtap)."""
+    p = _conv_desc(a_hi, a_lo, w_hi, w_lo, N, MH, MW, nprod)
+    p.a_img_mul = a_img_mul
     p.ntaps = len(taps)
     for i, (dy, dx, io, wt) in enumerate(taps):
         p.taps[i] = _lib.ConvTap(dy, dx, io, wt)
-    p.nprod, p.mode = nprod, mode
+    p.mode = mode
     p.dcoef, p.bias, p.noise, p.noise_nstride = ptr(dcoef), ptr(bias), ptr(noise), noise_nstride
     p.gain, p.slope, p.clamp = gain, slope, clamp
     for i, o in enumerate(outs):
@@ -82,30 +101,21 @@ def conv_gemm(a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, *, a_img_mul=0, nprod=3, 
         p.rgb = _lib.FusedRgb(ptr(rgb['out']), ptr(rgb['weight']), ptr(rgb['style']), ptr(rgb['bias']), float(rgb.get('clamp', -1.0)),
                               rgb['weight'].shape[0], int(rgb.get('nchw', False)), int(rgb.get('accumulate', False)))
     p.splits, p.split_stride = splits, split_stride
-    check(lib.n3d_conv_gemm(C.byref(p), stream_ptr()), 'n3d_conv_gemm')
+    _run('n3d_conv_gemm', C.byref(p), stream_ptr())
 
 
 def conv_transposed_gemm(a_hi, a_lo, w_hi, w_lo, N, H, W, raw, nprod=3):
     """Stride-2 transposed 3x3 conv of a [N,H,W,Cin] split activation -> raw fp32 [N,2H+1,2W+1,Cout] (one launch, 4 parity classes)."""
-    NI, AH, AW, Cin = a_hi.shape
-    T, Cout, _ = w_hi.shape
-    p = _lib.ConvGemm()
-    p.a_hi, p.a_lo = ptr(a_hi), ptr(a_lo)
-    p.NI, p.AH, p.AW, p.Cin = NI, AH, AW, Cin
-    p.w_hi, p.w_lo = ptr(w_hi), ptr(w_lo)
-    p.T, p.Cout = T, Cout
-    p.N, p.MH, p.MW = N, H, W
-    p.nprod = nprod
+    p = _conv_desc(a_hi, a_lo, w_hi, w_lo, N, H, W, nprod)
     p.gain, p.slope, p.clamp = 1.0, 1.0, -1.0
     p.out_f32, p.f32_cstride = ptr(raw), raw.shape[-1]
-    check(lib.n3d_conv_transposed_gemm(C.byref(p), stream_ptr()), 'n3d_conv_transposed_gemm')
+    _run('n3d_conv_transposed_gemm', C.byref(p), stream_ptr())
 
 
 def modulate_split(x, style, hi, lo, cstride=None, coff=0):
     """x fp32 NHWC [N,H,W,C]; style [N,C] or None -> hi/lo bf16 (written at channel offset `coff`, stride `cstride`)."""
     N, H, W, Cc = x.shape
-    check(lib.n3d_modulate_split(ptr(x), H * W, N, Cc, ptr(style), ptr(hi), ptr(lo), cstride or Cc, coff, stream_ptr()),
-          'n3d_modulate_split')
+    _run('n3d_modulate_split', ptr(x), H * W, N, Cc, ptr(style), ptr(hi), ptr(lo), cstride or Cc, coff, stream_ptr())
 
 
 def fir_up_epilogue(raw, C_, dcoef, bias, noise, gain, slope, clamp, outs=(), out_f32=None, f32_cstride=0, f32_coff=0, noise_nstride=0):
@@ -113,8 +123,8 @@ def fir_up_epilogue(raw, C_, dcoef, bias, noise, gain, slope, clamp, outs=(), ou
     arr = (_lib.SplitOut * 2)()
     for i, o in enumerate(outs):
         arr[i] = o
-    check(lib.n3d_fir_up_epilogue(ptr(raw), N, RH - 1, RW - 1, C_, ptr(dcoef), ptr(bias), ptr(noise), noise_nstride, gain, slope, clamp, arr,
-                                  ptr(out_f32), f32_cstride, f32_coff, stream_ptr()), 'n3d_fir_up_epilogue')
+    _run('n3d_fir_up_epilogue', ptr(raw), N, RH - 1, RW - 1, C_, ptr(dcoef), ptr(bias), ptr(noise), noise_nstride, gain, slope, clamp, arr,
+                                ptr(out_f32), f32_cstride, f32_coff, stream_ptr())
 
 
 def splitk_epilogue(part, dcoef, bias, noise, gain, slope, clamp, outs=(), out_f32=None, f32_cstride=0, f32_coff=0, noise_nstride=0):
@@ -123,82 +133,91 @@ def splitk_epilogue(part, dcoef, bias, noise, gain, slope, clamp, outs=(), out_f
     arr = (_lib.SplitOut * 2)()
     for i, o in enumerate(outs):
         arr[i] = o
-    check(lib.n3d_splitk_epilogue(ptr(part), S, N * H * W * Cc, N, H, W, Cc, ptr(dcoef), ptr(bias), ptr(noise), noise_nstride, gain, slope, clamp, arr,
-                                  ptr(out_f32), f32_cstride, f32_coff, stream_ptr()), 'n3d_splitk_epilogue')
+    _run('n3d_splitk_epilogue', ptr(part), S, N * H * W * Cc, N, H, W, Cc, ptr(dcoef), ptr(bias), ptr(noise), noise_nstride, gain, slope, clamp, arr,
+                                ptr(out_f32), f32_cstride, f32_coff, stream_ptr())
 
 
 def fir_down_split(x, hi, lo):
     N, H, W, Cc = x.shape
-    check(lib.n3d_fir_down_split(ptr(x), N, H, W, Cc, ptr(hi), ptr(lo), stream_ptr()), 'n3d_fir_down_split')
+    _run('n3d_fir_down_split', ptr(x), N, H, W, Cc, ptr(hi), ptr(lo), stream_ptr())
 
 
 def upsample2d_nhwc(x, y, y_nchw=False):
     N, H, W, Cc = x.shape
-    check(lib.n3d_upsample2d_nhwc(ptr(x), N, H, W, Cc, ptr(y), int(y_nchw), stream_ptr()), 'n3d_upsample2d_nhwc')
+    _run('n3d_upsample2d_nhwc', ptr(x), N, H, W, Cc, ptr(y), int(y_nchw), stream_ptr())
 
 
 def downsample2d_nhwc(x, y):
     N, H, W, Cc = x.shape
-    check(lib.n3d_downsample2d_nhwc(ptr(x), N, H, W, Cc, ptr(y), stream_ptr()), 'n3d_downsample2d_nhwc')
+    _run('n3d_downsample2d_nhwc', ptr(x), N, H, W, Cc, ptr(y), stream_ptr())
 
 
 def styles(ws, affine_w, affine_b, row_widx, row_scale, row_ooff, row_cin, out):
     """out: flat fp32; layer blocks are dense [N, Cin] at row_ooff (see include/next3d_b200.h)."""
     N, num_ws, wdim = ws.shape
     rows = affine_w.shape[0]
-    check(lib.n3d_styles(ptr(ws), N, num_ws, wdim, ptr(affine_w), ptr(affine_b), ptr(row_widx), ptr(row_scale), ptr(row_ooff),
-                         ptr(row_cin), ptr(out), rows, stream_ptr()), 'n3d_styles')
+    _run('n3d_styles', ptr(ws), N, num_ws, wdim, ptr(affine_w), ptr(affine_b), ptr(row_widx), ptr(row_scale), ptr(row_ooff),
+                       ptr(row_cin), ptr(out), rows, stream_ptr())
 
 
 def demod(styles_flat, wsq, row_woff, row_cin, row_soff, row_ooff, row_cout, out, N):
     rows = row_cin.shape[0]
-    check(lib.n3d_demod(ptr(styles_flat), ptr(wsq), ptr(row_woff), ptr(row_cin), ptr(row_soff), ptr(row_ooff), ptr(row_cout),
-                        ptr(out), rows, N, stream_ptr()), 'n3d_demod')
+    _run('n3d_demod', ptr(styles_flat), ptr(wsq), ptr(row_woff), ptr(row_cin), ptr(row_soff), ptr(row_ooff), ptr(row_cout),
+                      ptr(out), rows, N, stream_ptr())
 
 
 def transform_points(pts, rot, zoff, ndc_flip, out):
     N, Pn, _ = pts.shape
-    check(lib.n3d_transform_points(ptr(pts), N, Pn, ptr(rot), rot.shape[0], zoff, int(ndc_flip), ptr(out), stream_ptr()),
-          'n3d_transform_points')
+    _run('n3d_transform_points', ptr(pts), N, Pn, ptr(rot), rot.shape[0], zoff, int(ndc_flip), ptr(out), stream_ptr())
 
 
 def rasterize(verts, faces, H, W, p2f, bary, workspace=None):
     NM, V, _ = verts.shape
     if workspace is None:
         workspace = torch.empty(NM * faces.shape[0] * 16, dtype=torch.float32, device=verts.device)
-    check(lib.n3d_rasterize(ptr(verts), ptr(faces), NM, V, faces.shape[0], H, W, ptr(p2f), ptr(bary), ptr(workspace), stream_ptr()),
-          'n3d_rasterize')
+    _run('n3d_rasterize', ptr(verts), ptr(faces), NM, V, faces.shape[0], H, W, ptr(p2f), ptr(bary), ptr(workspace), stream_ptr(), kernels=2)
 
 
 def uv_sample(p2f, bary, face_uv, texture, eye_mask, tex_planes, alpha):
     N, TH, TW, Cc = texture.shape
     _, H, W = p2f.shape
     MH, MW = eye_mask.shape[-2:]
-    check(lib.n3d_uv_sample(ptr(p2f), ptr(bary), ptr(face_uv), ptr(texture), ptr(eye_mask), N, H, W, TH, TW, Cc, MH, MW,
-                            ptr(tex_planes), ptr(alpha), stream_ptr()), 'n3d_uv_sample')
+    _run('n3d_uv_sample', ptr(p2f), ptr(bary), ptr(face_uv), ptr(texture), ptr(eye_mask), N, H, W, TH, TW, Cc, MH, MW,
+                          ptr(tex_planes), ptr(alpha), stream_ptr())
 
 
 def fill_mouth(alpha):
     NI = alpha.numel() // (alpha.shape[-1] * alpha.shape[-2])
-    check(lib.n3d_fill_mouth(ptr(alpha), NI, alpha.shape[-2], alpha.shape[-1], stream_ptr()), 'n3d_fill_mouth')
+    _run('n3d_fill_mouth', ptr(alpha), NI, alpha.shape[-2], alpha.shape[-1], stream_ptr())
 
 
 def mouth_box(lm2d, boxes):
-    check(lib.n3d_mouth_box(ptr(lm2d), lm2d.shape[0], ptr(boxes), stream_ptr()), 'n3d_mouth_box')
+    _run('n3d_mouth_box', ptr(lm2d), lm2d.shape[0], ptr(boxes), stream_ptr())
 
 
 def resize_aa(src, dst=None, DH=None, DW=None, src_box=None, dst_box=None, style=None, hi=None, lo=None):
     N, SH, SW, Cc = src.shape
     if dst is not None:
         DH, DW = dst.shape[1:3]
-    check(lib.n3d_resize_aa(ptr(src), N, SH, SW, Cc, ptr(src_box), ptr(dst), DH, DW, ptr(dst_box), ptr(style), ptr(hi), ptr(lo),
-                            stream_ptr()), 'n3d_resize_aa')
+    _run('n3d_resize_aa', ptr(src), N, SH, SW, Cc, ptr(src_box), ptr(dst), DH, DW, ptr(dst_box), ptr(style), ptr(hi), ptr(lo),
+                          stream_ptr())
 
 
 def blend_planes(front, tex_planes, alpha, static, planes):
     N, H, W, _ = front.shape
-    check(lib.n3d_blend_planes(ptr(front), ptr(tex_planes), ptr(alpha), ptr(static), N, H, W, ptr(planes), stream_ptr()),
-          'n3d_blend_planes')
+    _run('n3d_blend_planes', ptr(front), ptr(tex_planes), ptr(alpha), ptr(static), N, H, W, ptr(planes), stream_ptr())
+
+
+def _render_desc(planes, cam2world, intrinsics, res, opts, seed):
+    """Render descriptor with the workload (planes, cameras, resolution, sampling options, seed) filled in."""
+    p = _lib.Render()
+    N, _, PH, PW, _ = planes.shape
+    p.planes, p.N, p.PH, p.PW = ptr(planes), N, PH, PW
+    p.cam2world, p.intrinsics, p.res = ptr(cam2world), ptr(intrinsics), res
+    p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
+    p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
+    p.seed = seed
+    return p
 
 
 def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
@@ -211,45 +230,40 @@ def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum,
     if unsupported:     # renderer.py:98-107 (auto near/far), :153 (density noise), :186-196 (disparity sampling), ray_marcher.py:41-44
         raise RuntimeError(f'libnext3d_b200 n3d_render_rays failed (code -2, unsupported): rendering option(s) {unsupported} are not '
                            f'implemented by the fused renderer (supported: linear stratified sampling, fixed ray_start / ray_end, softplus)')
-    p = _lib.Render()
-    N, _, PH, PW, _ = planes.shape
-    p.planes, p.N, p.PH, p.PW = ptr(planes), N, PH, PW
-    p.cam2world, p.intrinsics, p.res = ptr(cam2world), ptr(intrinsics), res
-    p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
-    p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
-    p.u_coarse, p.u_fine, p.seed, p.seed_ptr = ptr(u_coarse), ptr(u_fine), seed, ptr(seed_ptr)
+    p = _render_desc(planes, cam2world, intrinsics, res, opts, seed)
+    p.u_coarse, p.u_fine, p.seed_ptr = ptr(u_coarse), ptr(u_fine), ptr(seed_ptr)
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
     p.rgb, p.depth, p.wsum, p.depth_minmax = ptr(rgb), ptr(depth), ptr(wsum), ptr(depth_minmax)
     p.white_back = int(bool(opts.get('white_back', False)))
-    check(lib.n3d_render_rays(C.byref(p), stream_ptr()), 'n3d_render_rays')
+    _run('n3d_render_rays', C.byref(p), stream_ptr())
 
 
 def depth_clamp(depth, depth_minmax):
-    check(lib.n3d_depth_clamp(ptr(depth), depth.numel(), ptr(depth_minmax), stream_ptr()), 'n3d_depth_clamp')
+    _run('n3d_depth_clamp', ptr(depth), depth.numel(), ptr(depth_minmax), stream_ptr())
 
 
 def sample_points(planes, coords, box_warp, dec, sigma, rgb=None):
     N, _, PH, PW, _ = planes.shape
     Pn = coords.shape[1]
-    check(lib.n3d_sample_points(ptr(planes), N, PH, PW, ptr(coords), Pn, float(box_warp), *(ptr(t) for t in dec), ptr(sigma), ptr(rgb),
-                                stream_ptr()), 'n3d_sample_points')
+    _run('n3d_sample_points', ptr(planes), N, PH, PW, ptr(coords), Pn, float(box_warp), *(ptr(t) for t in dec), ptr(sigma), ptr(rgb),
+                              stream_ptr())
 
 
 def sample_grid(planes, grid_n, cube_length, box_warp, dec, sigma_grid, head=0, count=None, pad=0, pad_value=-1000.0):
     """sigma of the create_samples voxel grid (in-kernel coordinates), written flipped + trimmed into sigma_grid [grid_n]^3."""
     _, PH, PW, _ = planes.shape[-4:]
     count = grid_n ** 3 - head if count is None else count
-    check(lib.n3d_sample_grid(ptr(planes), PH, PW, grid_n, float(cube_length), float(box_warp), head, count, pad, float(pad_value),
-                              *(ptr(t) for t in dec), ptr(sigma_grid), stream_ptr()), 'n3d_sample_grid')
+    _run('n3d_sample_grid', ptr(planes), PH, PW, grid_n, float(cube_length), float(box_warp), head, count, pad, float(pad_value),
+                            *(ptr(t) for t in dec), ptr(sigma_grid), stream_ptr())
 
 
 def mapping(z, c, c_scale, m, truncation_psi=1.0, truncation_cutoff=None, num_ws=28):
     """MappingNetwork + truncation in one launch.  m: dict with embed_w/embed_b/fc0_w/fc0_b/fc1_w/fc1_b/w_avg fp32 device tensors."""
     N = z.shape[0]
     ws = torch.empty(N, num_ws, 512, device=z.device, dtype=torch.float32)
-    check(lib.n3d_mapping(ptr(z), ptr(c), N, float(c_scale), ptr(m['embed_w']), ptr(m['embed_b']), ptr(m['fc0_w']), ptr(m['fc0_b']),
-                          ptr(m['fc1_w']), ptr(m['fc1_b']), ptr(m['w_avg']), float(truncation_psi),
-                          -1 if truncation_cutoff is None else int(truncation_cutoff), num_ws, ptr(ws), stream_ptr()), 'n3d_mapping')
+    _run('n3d_mapping', ptr(z), ptr(c), N, float(c_scale), ptr(m['embed_w']), ptr(m['embed_b']), ptr(m['fc0_w']), ptr(m['fc0_b']),
+                        ptr(m['fc1_w']), ptr(m['fc1_b']), ptr(m['w_avg']), float(truncation_psi),
+                        -1 if truncation_cutoff is None else int(truncation_cutoff), num_ws, ptr(ws), stream_ptr())
     return ws
 
 
@@ -258,17 +272,11 @@ def interp_rows(B, Y):
     F_, K_ = B.shape
     D = Y[0].numel()
     out = torch.empty((F_,) + tuple(Y.shape[1:]), device=Y.device, dtype=torch.float32)
-    check(lib.n3d_interp_rows(ptr(B), ptr(Y), F_, K_, D, ptr(out), stream_ptr()), 'n3d_interp_rows')
+    _run('n3d_interp_rows', ptr(B), ptr(Y), F_, K_, D, ptr(out), stream_ptr())
     return out
 
 
 def render_floor(planes, cam2world, intrinsics, res, opts, kind, seed=0):
     """Diagnostics (n3d_render_floor): launch the gather-only (kind 0) or activations-only (kind 1) micro-kernel on the renderer's workload."""
-    p = _lib.Render()
-    N, _, PH, PW, _ = planes.shape
-    p.planes, p.N, p.PH, p.PW = ptr(planes), N, PH, PW
-    p.cam2world, p.intrinsics, p.res = ptr(cam2world), ptr(intrinsics), res
-    p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
-    p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
-    p.seed = seed
-    check(lib.n3d_render_floor(C.byref(p), int(kind), None, stream_ptr()), 'n3d_render_floor')
+    p = _render_desc(planes, cam2world, intrinsics, res, opts, seed)
+    _run('n3d_render_floor', C.byref(p), int(kind), None, stream_ptr())

@@ -1,5 +1,4 @@
-"""Time the fused renderer alone on a benchmark workload (random planes).  python tools/bench_render.py [c2|c3] [modes...]
-modes: N3D_RENDER_MODE values to time in separate processes is not needed -- the mode is read once per process, so run one mode per call."""
+"""Time the fused renderer alone on a benchmark workload (random planes).  python tools/bench_render.py [c2|c3]"""
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -28,7 +27,7 @@ for i in range(10):
     e1.record(); torch.cuda.synchronize()
     ts.append(e0.elapsed_time(e1))
 ts.sort()
-print(which, 'N3D_RENDER_MODE', os.environ.get('N3D_RENDER_MODE', '0'), 'render_fused_kernel median', ts[len(ts) // 2], 'ms  min', ts[0], 'ms', flush=True)
+print(which, 'render_fused_kernel median', ts[len(ts) // 2], 'ms  min', ts[0], 'ms', flush=True)
 if which == 'c2' and os.environ.get('N3D_BENCH_GRID', '1') == '1':
     Rg = 256
     out = torch.empty(Rg, Rg, Rg, device='cuda')

@@ -45,17 +45,14 @@ def main():
         line = f'{cin:4d}->{cout:3d} @{res:2d}^2 N={N}: fused {base:6.1f} us |'
         for S in (3, 9):
             part = torch.empty(S, N, res, res, cout, device=DEV)
-            for mt in (64, 128, 256):
-                os.environ['N3D_SPLITK_MINTILES'] = str(mt)
 
-                def run():
-                    K.conv_gemm(hi, lo, w_hi, w_lo, K.taps_conv3x3(), N, res, res, mode=1, out_f32=part, f32_cstride=cout, splits=S, split_stride=N * res * res * cout)
-                    K.splitk_epilogue(part, d, b, None, math.sqrt(2), 0.2, 256.0, outs=outs)
-                t = timeit(run)
-                diff = (o_hi.float() - ref_hi.float()).abs().max().item() / ref_hi.float().abs().max().item()
-                line += f' S{S}/mt{mt} {t:6.1f} ({diff:.0e})'
+            def run():
+                K.conv_gemm(hi, lo, w_hi, w_lo, K.taps_conv3x3(), N, res, res, mode=1, out_f32=part, f32_cstride=cout, splits=S, split_stride=N * res * res * cout)
+                K.splitk_epilogue(part, d, b, None, math.sqrt(2), 0.2, 256.0, outs=outs)
+            t = timeit(run)
+            diff = (o_hi.float() - ref_hi.float()).abs().max().item() / ref_hi.float().abs().max().item()
+            line += f' S{S} {t:6.1f} ({diff:.0e})'
         print(line, flush=True)
-    os.environ.pop('N3D_SPLITK_MINTILES', None)
 
 
 if __name__ == '__main__':
