@@ -2,18 +2,19 @@
 // generator (modulated 3x3 / 1x1, transposed-conv parity classes, stride-2 convs, ToRGB).
 //
 //   M = 128 output pixels per tile (TN x TH x TW patch), N = block_n output channels, K = taps x Cin.
-//   A (activations, NHWC bf16, split hi/lo) is fetched per (tap, 64-channel chunk) as one 4-D TMA box whose
+//   A (activations, NHWC bf16, split hi/lo) is fetched per (tap, 64- or 32-channel chunk) as one 4-D TMA box whose
 //   coordinates are shifted by the tap offset; out-of-range rows/columns are zero-filled by TMA, which *is* the
 //   convolution padding.  B (weights [T, Cout, Cin] bf16 hi/lo) is a 3-D TMA box.  Both land in shared memory in the
-//   K-major SWIZZLE_128B layout that wgmma consumes directly.
+//   K-major SWIZZLE_128B / SWIZZLE_64B layout that wgmma consumes directly.
 //   Precision: fp32 = hi + lo with bf16 hi, lo; acc += Ahi*Bhi + Ahi*Blo + Alo*Bhi (3 MMAs, fp32 accumulate in registers)
 //   reproduces an fp32 convolution to ~2^-16 relative -- inside the 1e-3 end-to-end budget where single-pass
 //   bf16/fp16/tf32 is not (SURVEY.md section 7 "Precision vs tensor cores").
-//   Warp roles (384 threads, persistent over tiles): warps 0-7 = two consumer warpgroups, warpgroup g owns tile rows
-//   64g..64g+63: wgmma into a register accumulator, then the fused epilogue (demod/noise/bias/lrelu/clamp -> next layer's
-//   modulation -> bf16 split / fp32 stores) through a small shared-memory transpose (thread = tile row).  Warpgroup 2 = TMA
-//   producer (one lane), which keeps filling the stage ring during the epilogue.  setmaxnreg lowers the producer to 40 registers
-//   and raises the consumers to 232: ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
+//   Warp roles (384 threads, persistent over work items): warps 0-7 = two ping-pong consumer warpgroups; the CTA's work items
+//   alternate between them, and each owns all 128 rows of its tiles: wgmma into a register accumulator (two m64 halves), then the
+//   fused epilogue (demod/noise/bias/lrelu/clamp -> next layer's modulation -> bf16 split / fp32 stores) through a small
+//   shared-memory transpose (thread = tile row, one 64-row half at a time), overlapping the other warpgroup's MMAs.  Warpgroup 2 = TMA
+//   producer (one lane), which keeps filling the stage ring during the epilogue.  setmaxnreg lowers the producer to 24 registers
+//   and raises the consumers to 240 (2 x 128 x 240 + 128 x 24 = 384 x 168): ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
 #include <cstring>
 #include "common.cuh"
 #include <cuda.h>
@@ -23,17 +24,22 @@ namespace {
 using namespace n3d_tc;
 
 constexpr int kBlockM = 128;
-// K per pipeline stage: 64 bf16 (128-byte rows, SWIZZLE_128B) or, for Cin % 64 == 32 (the 32-channel feature images),
-// 32 bf16 (64-byte rows, SWIZZLE_64B) so that no TMA box hangs over the channel extent.
-constexpr int kConsumerThreads = 256;         // two warpgroups of 64 tile rows each
+// K per pipeline stage (block_k, a template parameter): 64 bf16 (128-byte rows, SWIZZLE_128B) or 32 bf16 (64-byte rows,
+// SWIZZLE_64B).  32 is used for Cin % 64 == 32 (the 32-channel feature images: no TMA box hangs over the channel extent) and
+// wherever 64-channel stages would leave fewer than kMinStages in the ring (block_n 96 and 128).
+constexpr int kConsumerThreads = 256;         // two ping-pong warpgroups of 128 tile rows each
 constexpr int kThreads = kConsumerThreads + 128;   // + the producer warpgroup (one TMA lane)
-constexpr int kMaxBlockN = 256;
+constexpr int kMaxBlockN = 128;
+constexpr int kMinStages = 4;
+constexpr int kMaxStages = 8;
 constexpr int kMinTiles = 64;                 // see the block_n choice in launch_conv
 constexpr int kMinTilesSplit = 128;           // same for split-K launches
 constexpr int kStageArrays = 8;               // dcoef | bias | style0 | style1 | up to 4 modulated ToRGB weight rows
 constexpr int kXStride = 36;                  // floats per row of the accumulator transpose buffer (32 columns + pad)
 // per-warpgroup epilogue area: staged vectors | accumulator transpose [64][kXStride] | ToRGB partial sums [64][4]
 constexpr int kEpiBytes = kStageArrays * kMaxBlockN * 4 + 64 * kXStride * 4 + 64 * 4 * 4;
+// shared memory left for the stage ring: opt-in maximum - both epilogue areas - barriers - 1024-byte alignment slack
+constexpr int kRingBytes = 227 * 1024 - 2 * kEpiBytes - 1024 - 256;
 
 struct KParams {
     CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
@@ -44,7 +50,8 @@ struct KParams {
     int nsub;
     struct Sub { int tap_begin, ntaps, MH, MW, tiles_x, tiles_y, oy_off, ox_off, tile_end; } sub[4];
     int splits; long long split_stride;   // split-K: work item = (tile, K slice); slice s writes its raw partial sums to out_f32 + s * split_stride
-    int block_n, stages, stage_bytes, b_bytes, a_bytes, block_k;
+    int block_n, stages, stage_bytes, b_bytes, a_bytes;
+    int item_tiles;                  // n-tiles per work item: tiles_n for the fused ToRGB (all channels of a pixel), else 1
     int cin_chunks, ntaps, nprod, a_img_stride;
     N3DConvTap taps[9];
     int mode;
@@ -57,7 +64,7 @@ struct KParams {
     int* err_flag;
 };
 
-__device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.TN == 1 && P.mode == 0 && P.tiles_n == 1) ? P.rgb.channels : 0; }
+__device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.TN == 1 && P.mode == 0 && P.item_tiles == P.tiles_n) ? P.rgb.channels : 0; }
 
 struct TileInfo { int sub, tn, x0, y0, n0, split; };
 // Tiles are numbered sub-problem-major (all tiles of parity class 0, then class 1, ...), n-tile minor, so that the heaviest
@@ -86,8 +93,59 @@ __device__ __forceinline__ void k_range(const KParams& P, const TileInfo& t, int
     ke = min(nsteps, kb + per);
 }
 
+// One stage's MMAs as a fixed instruction sequence: one fence, BK/16 x NPROD x 2 wgmmas back to back, one commit.  The warpgroup
+// owns all 128 tile rows: acc0 = rows 0-63, acc1 = rows 64-127 (two m64 wgmmas sharing the B descriptor).  FIRST (the first
+// stage of a tile) overwrites the accumulator with its first product instead of adding to it.
+template <int BN, int BK, int NPROD, bool FIRST>
+__device__ __forceinline__ void stage_mma(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+    constexpr uint32_t h1 = 64u * BK * 2u;         // rows 64-127 of the A tile
+    constexpr uint64_t dhi = wgmma_desc_hi(BK);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+        const uint32_t koff = (uint32_t)k * 32u;     // 16 bf16 = 32 bytes inside the swizzle row
+        wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
+        wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
+        if (NPROD == 3) {
+            wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc0, wgmma_desc(a_lo + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc1, wgmma_desc(a_lo + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
+        }
+    }
+    wgmma_commit();
+}
+
+// Main loop of one tile: one stage = one (tap, channel chunk); a stage is released once its wgmmas retired (wait_group 1 after
+// the next stage's wgmmas are issued, so that the tensor cores always have one group queued).  Each of the warpgroup's 4 warps
+// arrives on the stage's empty barrier.
+template <int BN, int BK, int NPROD>
+__device__ __forceinline__ void tile_mainloop(const KParams& P, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int ksteps, uint32_t smem_base,
+                                              uint32_t bar_base, int lane, int& s, uint32_t& ph) {
+    const uint32_t a_bytes = (uint32_t)P.a_bytes, b_bytes = (uint32_t)P.b_bytes, stage_bytes = (uint32_t)P.stage_bytes;
+    const uint32_t empty_base = bar_base + 8u * (uint32_t)P.stages;
+    uint32_t sa = smem_base + (uint32_t)s * stage_bytes;
+    mbar_wait(bar_base + 8u * (uint32_t)s, ph, P.err_flag, 3);           // first stage (ksteps >= 1): overwrite the accumulator
+    stage_mma<BN, BK, NPROD, true>(acc0, acc1, sa, sa + a_bytes, sa + 2u * a_bytes, sa + 2u * a_bytes + b_bytes);
+    int prev_s = s;
+    if (++s == P.stages) { s = 0; ph ^= 1u; }
+    for (int ks = 1; ks < ksteps; ++ks) {
+        sa = smem_base + (uint32_t)s * stage_bytes;
+        mbar_wait(bar_base + 8u * (uint32_t)s, ph, P.err_flag, 3);
+        stage_mma<BN, BK, NPROD, false>(acc0, acc1, sa, sa + a_bytes, sa + 2u * a_bytes, sa + 2u * a_bytes + b_bytes);
+        wgmma_wait<1>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_base + 8u * (uint32_t)prev_s);
+        prev_s = s;
+        if (++s == P.stages) { s = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_base + 8u * (uint32_t)prev_s);
+}
+
 // ---------------------------------------------------------------------------------------------- the kernel
-template <int BN>
+template <int BN, int BK>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-B aligned: round up to 1024 (SWIZZLE_128B atoms)
@@ -103,20 +161,22 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     if (warp == kConsumerThreads / 32 && lane == 0) {
         tma_prefetch_desc(&P.tmA_hi); tma_prefetch_desc(&P.tmB_hi);
         if (P.nprod == 3) { tma_prefetch_desc(&P.tmA_lo); tma_prefetch_desc(&P.tmB_lo); }
-        for (int s = 0; s < P.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerThreads / 32); }
+        for (int s = 0; s < P.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4); }   // one stage feeds one warpgroup
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    const int total_tiles = P.sub[P.nsub - 1].tile_end * P.splits;
+    // work item = item_tiles consecutive tiles (n-tile minor: all n-tiles of one M tile for the fused ToRGB), one CTA each
+    const int total_items = P.sub[P.nsub - 1].tile_end * P.splits / P.item_tiles;
 
     if (warp >= kConsumerThreads / 32) {
         // ===================================================== TMA producer
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
         if (warp == kConsumerThreads / 32 && lane == 0) {
             int s = 0; uint32_t ph = 0;
             const uint32_t tx_bytes = (uint32_t)(P.nprod == 3 ? 2 : 1) * (uint32_t)(P.a_bytes + P.b_bytes);
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            for (int item = blockIdx.x; item < total_items; item += gridDim.x)
+            for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
                 const TileInfo ti = decode_tile(P, tile);
                 const int tn = ti.tn, x0 = ti.x0, y0 = ti.y0, n0 = ti.n0;
                 const int tap_begin = P.sub[ti.sub].tap_begin;
@@ -130,38 +190,49 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     const uint32_t fb = full_bar(s);
                     mbar_expect_tx(fb, tx_bytes);
                     const int img = n0 + (int)tap.img_off * P.a_img_stride;
-                    tma_load_4d(sa, &P.tmA_hi, fb, kc * P.block_k, x0 + tap.dx, y0 + tap.dy, img);
-                    tma_load_3d(sa + 2 * P.a_bytes, &P.tmB_hi, fb, kc * P.block_k, tn * P.block_n, tap.wtap);
+                    tma_load_4d(sa, &P.tmA_hi, fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
+                    tma_load_3d(sa + 2 * P.a_bytes, &P.tmB_hi, fb, kc * BK, tn * P.block_n, tap.wtap);
                     if (P.nprod == 3) {
-                        tma_load_4d(sa + P.a_bytes, &P.tmA_lo, fb, kc * P.block_k, x0 + tap.dx, y0 + tap.dy, img);
-                        tma_load_3d(sa + 2 * P.a_bytes + P.b_bytes, &P.tmB_lo, fb, kc * P.block_k, tn * P.block_n, tap.wtap);
+                        tma_load_4d(sa + P.a_bytes, &P.tmA_lo, fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
+                        tma_load_3d(sa + 2 * P.a_bytes + P.b_bytes, &P.tmB_lo, fb, kc * BK, tn * P.block_n, tap.wtap);
                     }
                     if (++s == P.stages) { s = 0; ph ^= 1u; }
                 }
             }
         }
     } else {
-        // ===================================================== consumers: warpgroup g = tile rows 64g .. 64g+63
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ===================================================== consumers: ping-pong, warpgroup g = work items 2i + g of this CTA
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
         const int g = warp >> 2;
         const int gtid = threadIdx.x & 127;                    // thread index inside the warpgroup
-        const int xrow = gtid & 63, half = gtid >> 6;          // epilogue: tile row 64g + xrow, columns 16 * half of each 32-column chunk
-        const int row = 64 * g + xrow;
-        const int tw = row % P.TW, th = (row / P.TW) % P.TH, tnn = row / (P.TW * P.TH);
+        const int xrow = gtid & 63, half = gtid >> 6;          // epilogue: tile row 64h + xrow, columns 16 * half of each 32-column chunk
         uint8_t* const epi = smem_raw + epi_off + (uint32_t)g * (uint32_t)kEpiBytes;
         float* const stg = reinterpret_cast<float*>(epi);                                   // [kStageArrays][kMaxBlockN]
         float* const xbuf = stg + kStageArrays * kMaxBlockN;                                // [64][kXStride]
         float* const rbuf = xbuf + 64 * kXStride;                                           // [64][4]
         const int nrgb = staged_rgb_channels(P);
         const bool staged = (P.TN == 1) && (P.mode == 0);
-        const uint64_t dhi = wgmma_desc_hi(P.block_k);
-        const int k16 = P.block_k / 16;
-        const uint32_t a_wg = (uint32_t)(g * 64 * P.block_k * 2);   // this warpgroup's 64 rows inside the A tile
         int s = 0; uint32_t ph = 0;
-        float acc[BN / 2];
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        // fused ToRGB: the partial sums of a pixel run over all n-tiles of its work item, in column order
+        float raccs[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+        // The producer fills the ring in work-item order; the CTA's items alternate between the warpgroups, so one warpgroup's
+        // epilogue runs while the other's MMAs run.  A warpgroup steps its ring position past the other one's K steps.
+        auto skip_item = [&](int item) {
+            for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
+                int kb, ke;
+                k_range(P, decode_tile(P, tile), kb, ke);
+                const int pos = s + (ke - kb);
+                ph ^= (uint32_t)((pos / P.stages) & 1);
+                s = pos % P.stages;
+            }
+        };
+        // Order barrier (named barriers 3 + g): a warpgroup starts an item's main loop only after the other warpgroup has issued
+        // the main loop of the item before it.  Every stage of that item has then been waited on, so the first stage this warpgroup
+        // waits for is at most one phase ahead of its full barrier (a parity wait cannot tell phases two apart).
+        if (g == 1 && (int)blockIdx.x < total_items) skip_item(blockIdx.x);
+        for (int item = blockIdx.x + g * gridDim.x; item < total_items; item += 2 * gridDim.x) {
+        if (item != (int)blockIdx.x) asm volatile("bar.sync %0, 256;" ::"r"(3 + g) : "memory");
+        for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
             const TileInfo ti = decode_tile(P, tile);
             const int tn = ti.tn, n0 = ti.n0;
             if (staged) {
@@ -177,48 +248,30 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     stg[arr * kMaxBlockN + c] = val;
                 }
                 for (int i = gtid; i < nrgb * P.block_n; i += 128) {          // fused ToRGB: W_rgb[c, co] * style_rgb[n, co]
-                    const int c = i / P.block_n, co = i - c * P.block_n;
+                    const int c = i / P.block_n, cl = i - c * P.block_n, co = tn * P.block_n + cl;
                     float val = 0.f;
                     if (co < P.Cout && n0 < P.N) val = __ldg(P.rgb.weight + (int64_t)c * P.Cout + co) * __ldg(P.rgb.style + (int64_t)n0 * P.Cout + co);
-                    stg[(4 + c) * kMaxBlockN + co] = val;
+                    stg[(4 + c) * kMaxBlockN + cl] = val;
                 }
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
             }
 
-            // ---- main loop: one stage = one (tap, channel chunk); the previous stage is released once its wgmmas retired
+            // ---- main loop (nprod and the accumulator overwrite of the first stage are fixed outside the instruction stream)
             int kb, ke;
             k_range(P, ti, kb, ke);
-            const int ksteps = ke - kb;
-            int prev_s = -1;
-            for (int ks = 0; ks < ksteps; ++ks) {
-                mbar_wait(full_bar(s), ph, P.err_flag, 3);
-                const uint32_t sa = smem_base + (uint32_t)s * (uint32_t)P.stage_bytes;
-                const uint32_t a_hi = sa + a_wg, a_lo = sa + (uint32_t)P.a_bytes + a_wg, b_hi = sa + 2u * (uint32_t)P.a_bytes, b_lo = b_hi + (uint32_t)P.b_bytes;
-                wgmma_fence();
-                for (int k = 0; k < k16; ++k) {
-                    const uint32_t koff = (uint32_t)k * 32u;     // 16 bf16 = 32 bytes inside the swizzle row
-                    wgmma_bf16<BN>(acc, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_hi + koff, dhi), (ks | k) != 0);
-                    if (P.nprod == 3) {
-                        wgmma_bf16<BN>(acc, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
-                        wgmma_bf16<BN>(acc, wgmma_desc(a_lo + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-                    }
-                }
-                wgmma_commit();
-                if (P.stages == 1) {                           // a single stage: retire it before the producer may refill it
-                    wgmma_wait<0>();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(empty_bar(s));
-                } else {
-                    wgmma_wait<1>();
-                    if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev_s)); }
-                    prev_s = s;
-                }
-                if (++s == P.stages) { s = 0; ph ^= 1u; }
-            }
-            wgmma_wait<0>();
-            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev_s)); }
+            float accs[2][BN / 2];                                 // rows 0-63 | 64-127; the first stage overwrites them
+            if (P.nprod == 3) tile_mainloop<BN, BK, 3>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
+            else tile_mainloop<BN, BK, 1>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
+            if (tile == (item + 1) * P.item_tiles - 1 && item + (int)gridDim.x < total_items)
+                asm volatile("bar.arrive %0, 256;" ::"r"(4 - g) : "memory");     // the other warpgroup's next item may start
 
-            // ---- epilogue (thread = tile row, 16 columns of each 32-column chunk)
+            // ---- epilogue (thread = tile row, 16 columns of each 32-column chunk), two 64-row halves
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+            float (&acc)[BN / 2] = accs[h];
+            float (&racc)[4] = raccs[h];
+            const int row = 64 * h + xrow;
+            const int tw = row % P.TW, th = (row / P.TW) % P.TH, tnn = row / (P.TW * P.TH);
             const int x = ti.x0 + tw;
             const int n = n0 + tnn;
             const int ox = x * P.ox_mul + P.sub[ti.sub].ox_off;
@@ -228,7 +281,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             const int64_t opix = ((int64_t)n * P.OH + oy) * P.OW + ox;
             float nz = 0.f;
             if (valid && P.noise) nz = __ldg(P.noise + (int64_t)n * P.noise_nstride + (int64_t)oy * P.OW + ox);
-            float racc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 1
             for (int c32 = 0; c32 < BN; c32 += 32) {
                 // accumulator columns c32 .. c32+31 -> xbuf[row][column]
@@ -384,7 +436,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     }
                 }
             }
-            if (nrgb > 0) {                                // the two column halves of a row meet in rbuf
+            if (nrgb > 0 && tile == (item + 1) * P.item_tiles - 1) {     // last n-tile: the two column halves of a row meet in rbuf
                 if (half == 1 && valid) *reinterpret_cast<float4*>(rbuf + 4 * xrow) = make_float4(racc[0], racc[1], racc[2], racc[3]);
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
                 if (half == 0 && valid) {                  // ToRGBLayer: linear bias (+ clamp), added to the up-sampled skip image
@@ -400,7 +452,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         }
                     }
                 }
+#pragma unroll
+                for (int c = 0; c < 4; ++c) racc[c] = 0.f;
             }
+            }
+        }
+        if (item + (int)gridDim.x < total_items) skip_item(item + gridDim.x);
         }
     }
 }
@@ -488,8 +545,8 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     // tiles re-fetch the activation tile once per n-tile, so a few wide tiles beat many narrow ones that merely fill more SMs.
     const int cout16 = ((p->Cout + 15) / 16) * 16;
     int bn = 16;
+    int item_tiles = 1;
     {
-        // 256 only for the fused ToRGB below: a 256-wide bf16x3 stage (96 KiB) leaves room for one stage, no TMA / MMA overlap
         const int cands[5] = {128, 96, 64, 32, 16};
         for (int i = 0; i < 5; ++i) {
             if (cands[i] > cout16) continue;
@@ -499,22 +556,26 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
         }
         const int min_tiles = splits > 1 ? kMinTilesSplit : kMinTiles;     // split launches: short K loops, so spread over (nearly) all SMs
         while (bn > 32 && tiles_m * splits * n3d_div_up(p->Cout, bn) < min_tiles) bn = (bn == 96) ? 32 : bn / 2;
-        if (p->rgb.out) {                                   // fused ToRGB needs every output channel of a pixel in one tile
+        if (p->rgb.out) {                                   // fused ToRGB: one work item covers every output channel of its pixels
             N3D_CHECK_ARG(cout16 <= 256 && cout16 % 16 == 0, "n3d_conv_gemm: fused ToRGB needs Cout <= 256");
             N3D_CHECK_ARG(p->rgb.channels >= 1 && p->rgb.channels <= 4 && p->rgb.weight && p->rgb.style && p->rgb.bias, "n3d_conv_gemm: bad fused ToRGB descriptor");
             N3D_CHECK_ARG(p->mode == 0 && nsub == 1 && K.TN == 1, "n3d_conv_gemm: fused ToRGB needs mode 0 and >= 128 output positions per image");
-            bn = 256;                                       // the narrowest instantiated width holding every channel
+            bn = kMaxBlockN;                                // the narrowest width holding every channel, else 128-wide n-tiles in turn
             for (const int w : {16, 32, 64, 96, 128}) if (w >= cout16) { bn = w; break; }
+            item_tiles = n3d_div_up(p->Cout, bn);
         }
     }
     K.block_n = bn;
     K.tiles_n = n3d_div_up(p->Cout, bn);
-    K.block_k = (p->Cin % 64 == 0 || p->Cin % 32 != 0) ? 64 : 32;
-    K.a_bytes = kBlockM * K.block_k * 2;
-    K.b_bytes = bn * K.block_k * 2;
+    K.item_tiles = item_tiles;
+    // block_k: 64-channel stages where the ring still holds kMinStages of them, else 32 (same (tap, 16-channel) MMA sequence, so
+    // the same accumulation order either way)
+    const int block_k = (p->Cin % 64 == 32 || kRingBytes / (2 * (kBlockM + bn) * 64 * 2) < kMinStages) ? 32 : 64;
+    K.a_bytes = kBlockM * block_k * 2;
+    K.b_bytes = bn * block_k * 2;
     K.stage_bytes = 2 * K.a_bytes + 2 * K.b_bytes;
-    K.stages = min(6, (227 * 1024 - 2 * kEpiBytes - 1024 - 256) / K.stage_bytes);   // + epilogue areas + barriers + alignment slack
-    K.cin_chunks = n3d_div_up(p->Cin, K.block_k);
+    K.stages = min(kMaxStages, kRingBytes / K.stage_bytes);
+    K.cin_chunks = n3d_div_up(p->Cin, block_k);
     if (splits > 1) {                                        // every K slice must own at least one step
         const int nsteps = tap_total * K.cin_chunks, per = n3d_div_up(nsteps, splits);
         N3D_CHECK_ARG(per * (splits - 1) < nsteps, "n3d_conv_gemm: %d K slices for %d K steps", splits, nsteps);
@@ -534,34 +595,29 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     K.err_flag = nullptr;       // a protocol timeout traps (the launch fails with an error); no device-side flag is kept
 
     const uint64_t adims[4] = {(uint64_t)p->Cin, (uint64_t)p->AW, (uint64_t)p->AH, (uint64_t)p->NI};
-    const uint32_t abox[4] = {(uint32_t)K.block_k, (uint32_t)K.TW, (uint32_t)K.TH, (uint32_t)K.TN};
+    const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)K.TW, (uint32_t)K.TH, (uint32_t)K.TN};
     const uint64_t wdims[3] = {(uint64_t)p->Cin, (uint64_t)p->Cout, (uint64_t)p->T};
-    const uint32_t wbox[3] = {(uint32_t)K.block_k, (uint32_t)bn, 1u};
+    const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)bn, 1u};
     int rc;
-    if ((rc = make_tmap(&K.tmA_hi, p->a_hi, 4, adims, abox, K.block_k)) != N3D_OK) return rc;
-    if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, K.block_k)) != N3D_OK) return rc;
+    if ((rc = make_tmap(&K.tmA_hi, p->a_hi, 4, adims, abox, block_k)) != N3D_OK) return rc;
+    if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
     if (p->nprod == 3) {
-        if ((rc = make_tmap(&K.tmA_lo, p->a_lo, 4, adims, abox, K.block_k)) != N3D_OK) return rc;
-        if ((rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, K.block_k)) != N3D_OK) return rc;
+        if ((rc = make_tmap(&K.tmA_lo, p->a_lo, 4, adims, abox, block_k)) != N3D_OK) return rc;
+        if ((rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
     }
 
     const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
     N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
-    const void* kernels[6] = {(const void*)conv_gemm_kernel<16>, (const void*)conv_gemm_kernel<32>, (const void*)conv_gemm_kernel<64>,
-                              (const void*)conv_gemm_kernel<96>, (const void*)conv_gemm_kernel<128>, (const void*)conv_gemm_kernel<256>};
-    for (const void* k : kernels)
-        if ((rc = n3d_smem_optin(k, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
-    const int grid = min(tiles_m * K.tiles_n * splits, D->num_sms);
-    switch (bn) {
-        case 16: conv_gemm_kernel<16><<<grid, kThreads, smem, st>>>(K); break;
-        case 32: conv_gemm_kernel<32><<<grid, kThreads, smem, st>>>(K); break;
-        case 64: conv_gemm_kernel<64><<<grid, kThreads, smem, st>>>(K); break;
-        case 96: conv_gemm_kernel<96><<<grid, kThreads, smem, st>>>(K); break;
-        case 128: conv_gemm_kernel<128><<<grid, kThreads, smem, st>>>(K); break;
-        case 256: conv_gemm_kernel<256><<<grid, kThreads, smem, st>>>(K); break;
-        default: n3d_set_error("n3d_conv_gemm: no kernel for block_n %d", bn); return N3D_ERR_UNSUPPORTED;
-    }
+    typedef void (*ConvKernel)(const KParams);
+    const ConvKernel kernels[2][5] = {
+        {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
+        {conv_gemm_kernel<16, 64>, conv_gemm_kernel<32, 64>, conv_gemm_kernel<64, 64>, conv_gemm_kernel<96, 64>, conv_gemm_kernel<128, 64>}};
+    const int bi = bn == 16 ? 0 : bn == 32 ? 1 : bn == 64 ? 2 : bn == 96 ? 3 : 4;
+    const ConvKernel kern = kernels[block_k == 64][bi];
+    if ((rc = n3d_smem_optin((const void*)kern, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
+    const int grid = min(tiles_m * K.tiles_n * splits / item_tiles, D->num_sms);
+    kern<<<grid, kThreads, smem, st>>>(K);
     N3D_CHECK_LAUNCH("n3d_conv_gemm");
     return N3D_OK;
 }
