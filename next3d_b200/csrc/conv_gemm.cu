@@ -40,19 +40,22 @@ constexpr int kXStride = 36;                  // floats per row of the accumulat
 constexpr int kEpiBytes = kStageArrays * kMaxBlockN * 4 + 64 * kXStride * 4 + 64 * 4 * 4;
 // shared memory left for the stage ring: opt-in maximum - both epilogue areas - barriers - 1024-byte alignment slack
 constexpr int kRingBytes = 227 * 1024 - 2 * kEpiBytes - 1024 - 256;
+constexpr int kMaxSubs = 9;                   // a stride-2 transposed conv: 4 parity-class interiors + 5 edge strips / corner
+constexpr int kMaxBoxes = 4;                  // distinct A box shapes (tile geometries) of one launch
 
 struct KParams {
-    CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
-    int N, MH, MW, Cout;
-    int TW, TH, TN;                  // TW*TH*TN == 128, all powers of two
-    int tiles_i, tiles_n;
-    // up to 4 sub-problems sharing operands / tile shape / epilogue (the 4 output-parity classes of a stride-2 transposed conv)
-    int nsub;
-    struct Sub { int tap_begin, ntaps, MH, MW, tiles_x, tiles_y, oy_off, ox_off, tile_end; } sub[4];
+    CUtensorMap tmA[kMaxBoxes][2];   // A (hi, lo) per tile geometry: box (block_k, TW, TH, TN) of the sub-problems using it
+    CUtensorMap tmB_hi, tmB_lo;
+    int N, Cout;
+    int tiles_n;
+    // sub-problems sharing operands and epilogue (the output-parity classes of a stride-2 transposed conv and their edges), each
+    // with its own tile geometry (TW*TH*TN == 128, all powers of two) over the M-space rectangle [y0, y_end) x [x0, x_end)
+    int nsub, nint, groups, nbox;    // the first nint sub-problems are interleaved (see decode_tile), groups: see unit_item
+    struct Sub { int tap_begin, ntaps, TW, TH, TN, box, tiles_x, tiles_y, y0, x0, y_end, x_end, oy_off, ox_off, tile_end; } sub[kMaxSubs];
     int splits; long long split_stride;   // split-K: work item = (tile, K slice); slice s writes its raw partial sums to out_f32 + s * split_stride
     int block_n, stages, stage_bytes, b_bytes, a_bytes;
     int item_tiles;                  // n-tiles per work item: tiles_n for the fused ToRGB (all channels of a pixel), else 1
-    int cin_chunks, ntaps, nprod, a_img_stride;
+    int cin_chunks, nprod, a_img_stride;
     N3DConvTap taps[9];
     int mode;
     const float* dcoef; const float* bias; const float* noise; int64_t noise_nstride;
@@ -64,26 +67,41 @@ struct KParams {
     int* err_flag;
 };
 
-__device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.TN == 1 && P.mode == 0 && P.item_tiles == P.tiles_n) ? P.rgb.channels : 0; }
+// mode-0 launches always have a single sub-problem
+__device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.sub[0].TN == 1 && P.mode == 0 && P.item_tiles == P.tiles_n) ? P.rgb.channels : 0; }
 
 struct TileInfo { int sub, tn, x0, y0, n0, split; };
-// Tiles are numbered sub-problem-major (all tiles of parity class 0, then class 1, ...), n-tile minor, so that the heaviest
-// parity classes (4 taps) are dealt out first.
+// Tiles are numbered sub-problem-major, n-tile minor, except that the first nint sub-problems (the four parity classes of a
+// transposed conv over the same input rectangle, one tile geometry) are interleaved class-minor: the classes of one M tile and
+// n-tile are consecutive tiles.  They share one tile_end, so the search below steps over all of them at once.
 __device__ __forceinline__ TileInfo decode_tile(const KParams& P, int tile) {
     const int split = tile % P.splits;                         // K slices of one tile are neighbouring work items (run concurrently)
     tile /= P.splits;
     int sidx = 0, begin = 0;
     while (sidx + 1 < P.nsub && tile >= P.sub[sidx].tile_end) { begin = P.sub[sidx].tile_end; ++sidx; }
-    const int local = tile - begin;
+    int local = tile - begin;
+    if (sidx < P.nint) { sidx = local % P.nint; local /= P.nint; }
+    const KParams::Sub& S = P.sub[sidx];
     TileInfo t;
     t.sub = sidx;
     t.tn = local % P.tiles_n;
-    const int tm = local / P.tiles_n, tx = P.sub[sidx].tiles_x, ty = P.sub[sidx].tiles_y;
-    t.x0 = (tm % tx) * P.TW;
-    t.y0 = ((tm / tx) % ty) * P.TH;
-    t.n0 = (tm / (tx * ty)) * P.TN;
+    const int tm = local / P.tiles_n;
+    t.x0 = S.x0 + (tm % S.tiles_x) * S.TW;
+    t.y0 = S.y0 + ((tm / S.tiles_x) % S.tiles_y) * S.TH;
+    t.n0 = (tm / (S.tiles_x * S.tiles_y)) * S.TN;
     t.split = split;
     return t;
+}
+
+// Work distribution: CTAs take units round-robin (unit blockIdx.x, then + gridDim.x, ...).  The first P.groups units are P.nint
+// consecutive items each (the parity classes of one M tile and n-tile: they read the same input rows, so all but the first read
+// them from L2, and every such unit costs the same); every later unit is one item.  With P.groups == 0 a CTA's items are
+// blockIdx.x + k * gridDim.x.
+__device__ __forceinline__ int unit_item(const KParams& P, int unit) { return unit < P.groups ? unit * P.nint : unit + P.groups * (P.nint - 1); }
+__device__ __forceinline__ int next_item(const KParams& P, int item) {      // this CTA's work item after `item`
+    const int grouped = P.groups * P.nint;
+    if (item < grouped && (item + 1) % P.nint != 0) return item + 1;
+    return unit_item(P, (item < grouped ? item / P.nint : item - grouped + P.groups) + (int)gridDim.x);
 }
 
 // K-step range [kb, ke) of a work item: all taps x channel chunks, or the item's slice of them under split-K.
@@ -159,8 +177,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (warp == kConsumerThreads / 32 && lane == 0) {
-        tma_prefetch_desc(&P.tmA_hi); tma_prefetch_desc(&P.tmB_hi);
-        if (P.nprod == 3) { tma_prefetch_desc(&P.tmA_lo); tma_prefetch_desc(&P.tmB_lo); }
+        tma_prefetch_desc(&P.tmB_hi);
+        if (P.nprod == 3) tma_prefetch_desc(&P.tmB_lo);
+        for (int b = 0; b < P.nbox; ++b) {
+            tma_prefetch_desc(&P.tmA[b][0]);
+            if (P.nprod == 3) tma_prefetch_desc(&P.tmA[b][1]);
+        }
         for (int s = 0; s < P.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4); }   // one stage feeds one warpgroup
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -175,11 +197,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (warp == kConsumerThreads / 32 && lane == 0) {
             int s = 0; uint32_t ph = 0;
             const uint32_t tx_bytes = (uint32_t)(P.nprod == 3 ? 2 : 1) * (uint32_t)(P.a_bytes + P.b_bytes);
-            for (int item = blockIdx.x; item < total_items; item += gridDim.x)
+            for (int item = unit_item(P, blockIdx.x); item < total_items; item = next_item(P, item))
             for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
                 const TileInfo ti = decode_tile(P, tile);
                 const int tn = ti.tn, x0 = ti.x0, y0 = ti.y0, n0 = ti.n0;
                 const int tap_begin = P.sub[ti.sub].tap_begin;
+                const CUtensorMap* const tmA = P.tmA[P.sub[ti.sub].box];
                 int kb, ke;
                 k_range(P, ti, kb, ke);
                 for (int idx = kb; idx < ke; ++idx) {
@@ -190,10 +213,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     const uint32_t fb = full_bar(s);
                     mbar_expect_tx(fb, tx_bytes);
                     const int img = n0 + (int)tap.img_off * P.a_img_stride;
-                    tma_load_4d(sa, &P.tmA_hi, fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
+                    tma_load_4d(sa, &tmA[0], fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
                     tma_load_3d(sa + 2 * P.a_bytes, &P.tmB_hi, fb, kc * BK, tn * P.block_n, tap.wtap);
                     if (P.nprod == 3) {
-                        tma_load_4d(sa + P.a_bytes, &P.tmA_lo, fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
+                        tma_load_4d(sa + P.a_bytes, &tmA[1], fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
                         tma_load_3d(sa + 2 * P.a_bytes + P.b_bytes, &P.tmB_lo, fb, kc * BK, tn * P.block_n, tap.wtap);
                     }
                     if (++s == P.stages) { s = 0; ph ^= 1u; }
@@ -211,11 +234,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         float* const xbuf = stg + kStageArrays * kMaxBlockN;                                // [64][kXStride]
         float* const rbuf = xbuf + 64 * kXStride;                                           // [64][4]
         const int nrgb = staged_rgb_channels(P);
-        const bool staged = (P.TN == 1) && (P.mode == 0);
+        const bool staged = (P.sub[0].TN == 1) && (P.mode == 0);
         int s = 0; uint32_t ph = 0;
         // fused ToRGB: the partial sums of a pixel run over all n-tiles of its work item, in column order
         float raccs[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-        // The producer fills the ring in work-item order; the CTA's items alternate between the warpgroups, so one warpgroup's
+        // The producer fills the ring in the CTA's item order; the items alternate between the warpgroups, so one warpgroup's
         // epilogue runs while the other's MMAs run.  A warpgroup steps its ring position past the other one's K steps.
         auto skip_item = [&](int item) {
             for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
@@ -229,9 +252,15 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         // Order barrier (named barriers 3 + g): a warpgroup starts an item's main loop only after the other warpgroup has issued
         // the main loop of the item before it.  Every stage of that item has then been waited on, so the first stage this warpgroup
         // waits for is at most one phase ahead of its full barrier (a parity wait cannot tell phases two apart).
-        if (g == 1 && (int)blockIdx.x < total_items) skip_item(blockIdx.x);
-        for (int item = blockIdx.x + g * gridDim.x; item < total_items; item += 2 * gridDim.x) {
-        if (item != (int)blockIdx.x) asm volatile("bar.sync %0, 256;" ::"r"(3 + g) : "memory");
+        const int first_item = unit_item(P, blockIdx.x);
+        int item = first_item;
+        if (g == 1) {
+            if (item < total_items) skip_item(item);
+            item = next_item(P, item);
+        }
+        for (; item < total_items; item = next_item(P, item)) {
+        const int other_item = next_item(P, item);             // the other warpgroup's next item
+        if (item != first_item) asm volatile("bar.sync %0, 256;" ::"r"(3 + g) : "memory");
         for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
             const TileInfo ti = decode_tile(P, tile);
             const int tn = ti.tn, n0 = ti.n0;
@@ -262,7 +291,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             float accs[2][BN / 2];                                 // rows 0-63 | 64-127; the first stage overwrites them
             if (P.nprod == 3) tile_mainloop<BN, BK, 3>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
             else tile_mainloop<BN, BK, 1>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
-            if (tile == (item + 1) * P.item_tiles - 1 && item + (int)gridDim.x < total_items)
+            if (tile == (item + 1) * P.item_tiles - 1 && other_item < total_items)
                 asm volatile("bar.arrive %0, 256;" ::"r"(4 - g) : "memory");     // the other warpgroup's next item may start
 
             // ---- epilogue (thread = tile row, 16 columns of each 32-column chunk), two 64-row halves
@@ -271,13 +300,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             float (&acc)[BN / 2] = accs[h];
             float (&racc)[4] = raccs[h];
             const int row = 64 * h + xrow;
-            const int tw = row % P.TW, th = (row / P.TW) % P.TH, tnn = row / (P.TW * P.TH);
+            const KParams::Sub& S = P.sub[ti.sub];
+            const int tw = row % S.TW, th = (row / S.TW) % S.TH, tnn = row / (S.TW * S.TH);
             const int x = ti.x0 + tw;
             const int n = n0 + tnn;
-            const int ox = x * P.ox_mul + P.sub[ti.sub].ox_off;
+            const int ox = x * P.ox_mul + S.ox_off;
             const int y = ti.y0 + th;
-            const int oy = y * P.oy_mul + P.sub[ti.sub].oy_off;
-            const bool valid = (n < P.N) && (y < P.sub[ti.sub].MH) && (x < P.sub[ti.sub].MW) && (oy < P.OH) && (ox < P.OW);
+            const int oy = y * P.oy_mul + S.oy_off;
+            const bool valid = (n < P.N) && (y < S.y_end) && (x < S.x_end) && (oy < P.OH) && (ox < P.OW);
             const int64_t opix = ((int64_t)n * P.OH + oy) * P.OW + ox;
             float nz = 0.f;
             if (valid && P.noise) nz = __ldg(P.noise + (int64_t)n * P.noise_nstride + (int64_t)oy * P.OW + ox);
@@ -457,7 +487,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             }
             }
         }
-        if (item + (int)gridDim.x < total_items) skip_item(item + gridDim.x);
+        if (other_item < total_items) skip_item(other_item);
+        item = other_item;
         }
     }
 }
@@ -502,9 +533,13 @@ int pow2_ceil(int v) { int p = 1; while (p < v) p <<= 1; return p; }
 }  // namespace
 
 namespace {
-struct SubSpec { int ntaps; N3DConvTap taps[9]; int MH, MW, oy_off, ox_off; };
+// Sub-problem: taps [tap_begin, tap_begin + ntaps) of the launch's tap list over the M-space rectangle [y0, y0 + MH) x [x0, x0 + MW),
+// written to output pixel (y * oy_mul + oy_off, x * ox_mul + ox_off).
+struct SubSpec { int tap_begin, ntaps, y0, x0, MH, MW, oy_off, ox_off; };
 
-int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stream) {
+// nint: the first nint sub-problems cover the same rectangle and are interleaved (decode_tile); they are the four parity classes
+// of a transposed conv, or the one sub-problem of an ordinary conv.
+int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nint, int nsub, const SubSpec* specs, void* stream) {
     N3D_CHECK_ARG(p && p->a_hi && p->w_hi, "n3d_conv_gemm: null operand");
     N3D_CHECK_ARG(p->nprod == 1 || p->nprod == 3, "n3d_conv_gemm: nprod must be 1 or 3");
     N3D_CHECK_ARG(p->nprod == 1 || (p->a_lo && p->w_lo), "n3d_conv_gemm: nprod 3 needs lo operands");
@@ -521,25 +556,34 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     memset(&K, 0, sizeof(K));
     K.N = p->N; K.Cout = p->Cout;
     K.splits = splits; K.split_stride = p->split_stride;
-    int maxH = 1, maxW = 1;
-    for (int i = 0; i < nsub; ++i) { maxH = max(maxH, specs[i].MH); maxW = max(maxW, specs[i].MW); }
-    K.TW = min(16, pow2_ceil(maxW));
-    K.TH = min(kBlockM / K.TW, pow2_ceil(maxH));
-    K.TN = kBlockM / (K.TW * K.TH);
-    K.tiles_i = n3d_div_up(p->N, K.TN);
-    K.nsub = nsub;
-    int tiles_m = 0, tap_total = 0;
+    N3D_CHECK_ARG(ntaps >= 1 && ntaps <= 9, "n3d_conv_gemm: %d taps", ntaps);
+    for (int t = 0; t < ntaps; ++t) {
+        N3D_CHECK_ARG(taps[t].wtap >= 0 && taps[t].wtap < p->T, "n3d_conv_gemm: tap weight slab out of range");
+        K.taps[t] = taps[t];
+    }
+    // Each sub-problem gets the tile geometry of its own M-space: TW up to 16 wide, then TH, then TN images; one A box per
+    // distinct geometry.
+    K.nsub = nsub; K.nint = nint;
+    int tiles_m = 0, sub_m[kMaxSubs], box_sub[kMaxBoxes];     // M tiles per sub-problem; first sub-problem of each box
     for (int i = 0; i < nsub; ++i) {
-        N3D_CHECK_ARG(specs[i].ntaps >= 1 && specs[i].MH >= 1 && specs[i].MW >= 1, "n3d_conv_gemm: bad sub-problem %d", i);
-        K.sub[i].tap_begin = tap_total; K.sub[i].ntaps = specs[i].ntaps;
-        for (int t = 0; t < specs[i].ntaps; ++t) {
-            N3D_CHECK_ARG(tap_total < 9, "n3d_conv_gemm: more than 9 taps in total");
-            N3D_CHECK_ARG(specs[i].taps[t].wtap >= 0 && specs[i].taps[t].wtap < p->T, "n3d_conv_gemm: tap weight slab out of range");
-            K.taps[tap_total++] = specs[i].taps[t];
-        }
-        K.sub[i].MH = specs[i].MH; K.sub[i].MW = specs[i].MW; K.sub[i].oy_off = specs[i].oy_off; K.sub[i].ox_off = specs[i].ox_off;
-        K.sub[i].tiles_x = n3d_div_up(specs[i].MW, K.TW); K.sub[i].tiles_y = n3d_div_up(specs[i].MH, K.TH);
-        tiles_m += K.sub[i].tiles_x * K.sub[i].tiles_y * K.tiles_i;
+        const SubSpec& sp = specs[i];
+        KParams::Sub& S = K.sub[i];
+        N3D_CHECK_ARG(sp.ntaps >= 1 && sp.tap_begin >= 0 && sp.tap_begin + sp.ntaps <= ntaps && sp.MH >= 1 && sp.MW >= 1,
+                      "n3d_conv_gemm: bad sub-problem %d", i);
+        S.tap_begin = sp.tap_begin; S.ntaps = sp.ntaps;
+        S.TW = min(16, pow2_ceil(sp.MW));
+        S.TH = min(kBlockM / S.TW, pow2_ceil(sp.MH));
+        S.TN = kBlockM / (S.TW * S.TH);
+        S.box = 0;
+        while (S.box < K.nbox && (K.sub[box_sub[S.box]].TW != S.TW || K.sub[box_sub[S.box]].TH != S.TH)) ++S.box;
+        if (S.box == K.nbox) { N3D_CHECK_ARG(K.nbox < kMaxBoxes, "n3d_conv_gemm: too many tile shapes"); box_sub[K.nbox++] = i; }
+        S.tiles_x = n3d_div_up(sp.MW, S.TW); S.tiles_y = n3d_div_up(sp.MH, S.TH);
+        S.y0 = sp.y0; S.x0 = sp.x0; S.y_end = sp.y0 + sp.MH; S.x_end = sp.x0 + sp.MW;
+        S.oy_off = sp.oy_off; S.ox_off = sp.ox_off;
+        sub_m[i] = S.tiles_x * S.tiles_y * n3d_div_up(p->N, S.TN);
+        tiles_m += sub_m[i];
+        N3D_CHECK_ARG(i >= nint || (sp.MH == specs[0].MH && sp.MW == specs[0].MW && sp.y0 == specs[0].y0 && sp.x0 == specs[0].x0),
+                      "n3d_conv_gemm: interleaved sub-problems must cover the same M-space");
     }
     // block_n: the largest wgmma N used here not exceeding Cout, halved while the launch has fewer than kMinTiles tiles.  Narrow
     // tiles re-fetch the activation tile once per n-tile, so a few wide tiles beat many narrow ones that merely fill more SMs.
@@ -559,7 +603,7 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
         if (p->rgb.out) {                                   // fused ToRGB: one work item covers every output channel of its pixels
             N3D_CHECK_ARG(cout16 <= 256 && cout16 % 16 == 0, "n3d_conv_gemm: fused ToRGB needs Cout <= 256");
             N3D_CHECK_ARG(p->rgb.channels >= 1 && p->rgb.channels <= 4 && p->rgb.weight && p->rgb.style && p->rgb.bias, "n3d_conv_gemm: bad fused ToRGB descriptor");
-            N3D_CHECK_ARG(p->mode == 0 && nsub == 1 && K.TN == 1, "n3d_conv_gemm: fused ToRGB needs mode 0 and >= 128 output positions per image");
+            N3D_CHECK_ARG(p->mode == 0 && nsub == 1 && K.sub[0].TN == 1, "n3d_conv_gemm: fused ToRGB needs mode 0 and >= 128 output positions per image");
             bn = kMaxBlockN;                                // the narrowest width holding every channel, else 128-wide n-tiles in turn
             for (const int w : {16, 32, 64, 96, 128}) if (w >= cout16) { bn = w; break; }
             item_tiles = n3d_div_up(p->Cout, bn);
@@ -577,14 +621,24 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     K.stages = min(kMaxStages, kRingBytes / K.stage_bytes);
     K.cin_chunks = n3d_div_up(p->Cin, block_k);
     if (splits > 1) {                                        // every K slice must own at least one step
-        const int nsteps = tap_total * K.cin_chunks, per = n3d_div_up(nsteps, splits);
+        const int nsteps = specs[0].ntaps * K.cin_chunks, per = n3d_div_up(nsteps, splits);
         N3D_CHECK_ARG(per * (splits - 1) < nsteps, "n3d_conv_gemm: %d K slices for %d K steps", splits, nsteps);
     }
-    K.ntaps = tap_total; K.nprod = p->nprod; K.a_img_stride = p->a_img_mul;
+    K.nprod = p->nprod; K.a_img_stride = p->a_img_mul;
+    N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
     {
-        int end = 0;
-        for (int i = 0; i < nsub; ++i) { end += K.sub[i].tiles_x * K.sub[i].tiles_y * K.tiles_i * K.tiles_n; K.sub[i].tile_end = end; }
+        int end = nint * sub_m[0] * K.tiles_n;                // the interleaved sub-problems share one tile_end
+        for (int i = 0; i < nsub; ++i) {
+            if (i >= nint) end += sub_m[i] * K.tiles_n;
+            K.sub[i].tile_end = end;
+        }
     }
+    // Interleaved parity classes go to one CTA as a unit (same input rows, equal cost per unit) once there are more of their
+    // items than SMs; with fewer, each item gets its own CTA (a shorter critical path than a 4 + 2 + 2 + 1-tap unit).
+    const int units_grouped = sub_m[0] * K.tiles_n;
+    K.groups = (nint > 1 && nint * units_grouped > D->num_sms) ? units_grouped : 0;
+    const int units = K.sub[nsub - 1].tile_end * splits / item_tiles - K.groups * (nint - 1);
     K.mode = p->mode; K.dcoef = p->dcoef; K.bias = p->bias; K.noise = p->noise; K.noise_nstride = p->noise_nstride;
     K.gain = p->gain; K.slope = p->slope; K.clamp = p->clamp;
     K.out[0] = p->out[0]; K.out[1] = p->out[1];
@@ -595,20 +649,19 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     K.err_flag = nullptr;       // a protocol timeout traps (the launch fails with an error); no device-side flag is kept
 
     const uint64_t adims[4] = {(uint64_t)p->Cin, (uint64_t)p->AW, (uint64_t)p->AH, (uint64_t)p->NI};
-    const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)K.TW, (uint32_t)K.TH, (uint32_t)K.TN};
     const uint64_t wdims[3] = {(uint64_t)p->Cin, (uint64_t)p->Cout, (uint64_t)p->T};
     const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)bn, 1u};
     int rc;
-    if ((rc = make_tmap(&K.tmA_hi, p->a_hi, 4, adims, abox, block_k)) != N3D_OK) return rc;
-    if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
-    if (p->nprod == 3) {
-        if ((rc = make_tmap(&K.tmA_lo, p->a_lo, 4, adims, abox, block_k)) != N3D_OK) return rc;
-        if ((rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
+    for (int b = 0; b < K.nbox; ++b) {
+        const KParams::Sub& S = K.sub[box_sub[b]];
+        const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)S.TW, (uint32_t)S.TH, (uint32_t)S.TN};
+        if ((rc = make_tmap(&K.tmA[b][0], p->a_hi, 4, adims, abox, block_k)) != N3D_OK) return rc;
+        if (p->nprod == 3 && (rc = make_tmap(&K.tmA[b][1], p->a_lo, 4, adims, abox, block_k)) != N3D_OK) return rc;
     }
+    if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
+    if (p->nprod == 3 && (rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
 
     const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
-    N3DDeviceState* D = n3d_device_state();
-    if (!D) return N3D_ERR_CUDA;
     typedef void (*ConvKernel)(const KParams);
     const ConvKernel kernels[2][5] = {
         {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
@@ -616,7 +669,7 @@ int launch_conv(const N3DConvGemm* p, int nsub, const SubSpec* specs, void* stre
     const int bi = bn == 16 ? 0 : bn == 32 ? 1 : bn == 64 ? 2 : bn == 96 ? 3 : 4;
     const ConvKernel kern = kernels[block_k == 64][bi];
     if ((rc = n3d_smem_optin((const void*)kern, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
-    const int grid = min(tiles_m * K.tiles_n * splits / item_tiles, D->num_sms);
+    const int grid = min(units, D->num_sms);
     kern<<<grid, kThreads, smem, st>>>(K);
     N3D_CHECK_LAUNCH("n3d_conv_gemm");
     return N3D_OK;
@@ -627,35 +680,44 @@ extern "C" int n3d_conv_gemm(const N3DConvGemm* p, void* stream) {
     N3D_CHECK_ARG(p, "n3d_conv_gemm: null descriptor");
     N3D_CHECK_ARG(p->ntaps >= 1 && p->ntaps <= 9, "n3d_conv_gemm: ntaps %d", p->ntaps);
     N3D_CHECK_ARG(p->MH >= 1 && p->MW >= 1, "n3d_conv_gemm: bad M-space");
-    SubSpec sp;
-    sp.ntaps = p->ntaps;
-    for (int i = 0; i < p->ntaps; ++i) sp.taps[i] = p->taps[i];
-    sp.MH = p->MH; sp.MW = p->MW; sp.oy_off = p->oy_off; sp.ox_off = p->ox_off;
-    return launch_conv(p, 1, &sp, stream);
+    const SubSpec sp = {0, p->ntaps, 0, 0, p->MH, p->MW, p->oy_off, p->ox_off};
+    return launch_conv(p, p->taps, p->ntaps, 1, 1, &sp, stream);
 }
 
 // Stride-2 transposed 3x3 convolution (conv_transpose2d(stride 2), conv2d_resample.py:114-127) as ONE launch: the four
-// output-parity classes (a, b) -- out[2p+a, 2q+b] = sum_{ky = a mod 2, kx = b mod 2} W[ky,kx] x[p-(ky-a)/2, q-(kx-b)/2] -- become four
-// sub-problems (4 / 2 / 2 / 1 taps) of the same persistent kernel, heaviest first.  p->MH, p->MW = INPUT height/width; the raw fp32
-// result [(2H+1), (2W+1)] goes to p->out_f32 (mode 1); taps / offsets / OH / OW of the descriptor are ignored and derived here.
+// output-parity classes (a, b) -- out[2p+a, 2q+b] = sum_{ky = a mod 2, kx = b mod 2} W[ky,kx] x[p-(ky-a)/2, q-(kx-b)/2] -- over
+// p <= H - a, q <= W - b.  Each class's interior p < H, q < W is one of four interleaved sub-problems (4 / 2 / 2 / 1 taps) with the
+// tile geometry of an H x W conv; the extra row p = H (a = 0) and column q = W (b = 0) are five thin sub-problems of their own
+// (two row strips, two column strips, one corner pixel), so no tile row or column is spent on a single edge row.  Every output
+// pixel sees its class's taps in the same order as in a separate launch of that class.  p->MH, p->MW = INPUT height/width; the
+// raw fp32 result [(2H+1), (2W+1)] goes to p->out_f32 (mode 1); taps / offsets / OH / OW of the descriptor are ignored and derived here.
 extern "C" int n3d_conv_transposed_gemm(const N3DConvGemm* p, void* stream) {
     N3D_CHECK_ARG(p && p->out_f32, "n3d_conv_transposed_gemm: null descriptor / output");
     N3D_CHECK_ARG(p->T == 9, "n3d_conv_transposed_gemm: needs 3x3 weights (T == 9)");
+    N3D_CHECK_ARG(p->MH >= 1 && p->MW >= 1, "n3d_conv_transposed_gemm: bad input size");
     N3DConvGemm q = *p;
     q.mode = 1; q.oy_mul = 2; q.ox_mul = 2; q.OH = 2 * p->MH + 1; q.OW = 2 * p->MW + 1; q.a_img_mul = 0;
-    SubSpec sp[4];
-    const int order[4][2] = {{0, 0}, {0, 1}, {1, 0}, {1, 1}};
-    for (int c = 0; c < 4; ++c) {
-        const int a = order[c][0], b = order[c][1];
-        sp[c].ntaps = 0;
+    const int H = p->MH, W = p->MW;
+    N3DConvTap taps[9];
+    SubSpec sp[kMaxSubs];
+    int nt = 0;
+    for (int c = 0; c < 4; ++c) {                       // classes (0,0), (0,1), (1,0), (1,1): interiors
+        const int a = c >> 1, b = c & 1;
+        sp[c] = {nt, 0, 0, 0, H, W, a, b};
         for (int ky = 0; ky < 3; ++ky)
             for (int kx = 0; kx < 3; ++kx)
                 if ((ky - a) % 2 == 0 && (kx - b) % 2 == 0) {
                     N3DConvTap t;
                     t.dy = (int8_t)(-(ky - a) / 2); t.dx = (int8_t)(-(kx - b) / 2); t.img_off = 0; t.wtap = ky * 3 + kx;
-                    sp[c].taps[sp[c].ntaps++] = t;
+                    taps[nt++] = t;
+                    ++sp[c].ntaps;
                 }
-        sp[c].MH = p->MH + 1 - a; sp[c].MW = p->MW + 1 - b; sp[c].oy_off = a; sp[c].ox_off = b;
     }
-    return launch_conv(&q, 4, sp, stream);
+    auto edge = [&](int c, int y0, int x0, int MH, int MW) { return SubSpec{sp[c].tap_begin, sp[c].ntaps, y0, x0, MH, MW, c >> 1, c & 1}; };
+    sp[4] = edge(0, H, 0, 1, W);                        // row p = H of classes (0,0) and (0,1)
+    sp[5] = edge(1, H, 0, 1, W);
+    sp[6] = edge(0, 0, W, H, 1);                        // column q = W of classes (0,0) and (1,0)
+    sp[7] = edge(2, 0, W, H, 1);
+    sp[8] = edge(0, H, W, 1, 1);                        // corner (H, W) of class (0,0)
+    return launch_conv(&q, taps, nt, 4, 9, sp, stream);
 }
