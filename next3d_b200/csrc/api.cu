@@ -54,3 +54,31 @@ int n3d_smem_optin(const void* kernel, int bytes, const char* who) {
     }
     return N3D_OK;
 }
+
+int n3d_max_clusters(const void* kernel, int threads, int smem_bytes, int cluster, const char* who) {
+    N3DDeviceState* d = n3d_device_state();
+    if (!d) return 0;
+    std::lock_guard<std::mutex> lock(g_smem_mutex);
+    int i = 0;
+    while (i < d->n_clusters && d->clusters[i].kernel != kernel) ++i;
+    if (i < d->n_clusters) return d->clusters[i].clusters;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cluster; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.gridDim = dim3(cluster);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    int n = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg);
+    if (e != cudaSuccess || n <= 0) {
+        n3d_set_error("%s: cannot place clusters of %d CTAs: %s", who, cluster, e != cudaSuccess ? cudaGetErrorString(e) : "none fit");
+        return 0;
+    }
+    if (i < N3DDeviceState::kSmemSlots) {
+        d->clusters[i] = {kernel, n};
+        ++d->n_clusters;
+    }
+    return n;
+}

@@ -28,19 +28,26 @@ void n3d_set_error(const char* fmt, ...);
 
 static inline int n3d_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// Host-side facts cached PER DEVICE (the library holds no device memory and no device-global state): SM count and which kernels
-// already had their dynamic shared-memory limit raised on that device (n3d_smem_optin).  Indexed by the current device at call time.
+// Host-side facts cached PER DEVICE (the library holds no device memory and no device-global state): SM count, which kernels
+// already had their dynamic shared-memory limit raised on that device (n3d_smem_optin), and how many clusters of a kernel fit
+// at once (n3d_max_clusters).  Indexed by the current device at call time.
 struct N3DDeviceState {
     static constexpr int kSmemSlots = 32;
     int num_sms;
-    int n_smem;
+    int n_smem, n_clusters;
     struct { const void* kernel; int bytes; } smem[kSmemSlots];
+    struct { const void* kernel; int clusters; } clusters[kSmemSlots];
 };
 N3DDeviceState* n3d_device_state(void);      // api.cu; nullptr (+ error message) when the current device cannot be queried
 
 // Raises `kernel`'s dynamic shared-memory limit to at least `bytes` on the current device, once per (device, kernel).
 // N3D_OK, or N3D_ERR_CUDA with a message that starts with `who`.
 int n3d_smem_optin(const void* kernel, int bytes, const char* who);     // api.cu
+
+// Clusters of `cluster` CTAs (`threads` threads, `smem_bytes` dynamic shared memory each) of `kernel` that the current device
+// runs at once (cudaOccupancyMaxActiveClusters), queried once per (device, kernel): the kernel's occupancy must not depend on
+// the shared memory below `smem_bytes`.  0 with a message that starts with `who` when the query fails.
+int n3d_max_clusters(const void* kernel, int threads, int smem_bytes, int cluster, const char* who);     // api.cu
 
 // Grid of a grid-stride launch: one block per `threads` work items, at least 1 and at most `per_sm` blocks per SM of the current
 // device.  0 when the device cannot be queried, so that the launch fails and N3D_CHECK_LAUNCH reports it.

@@ -15,6 +15,8 @@
 //   shared-memory transpose (thread = tile row, one 64-row half at a time), overlapping the other warpgroup's MMAs.  Warpgroup 2 = TMA
 //   producer (one lane), which keeps filling the stage ring during the epilogue.  setmaxnreg lowers the producer to 24 registers
 //   and raises the consumers to 240 (2 x 128 x 240 + 128 x 24 = 384 x 168): ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
+//   Launches with wide tiles run as 2-CTA clusters: the two CTAs take neighbouring M tiles of the same n-tile and K steps, and
+//   each loads half of the shared weight tile, multicast into both (decode_tile, the producer, release_stage, launch_conv).
 #include <cstring>
 #include "common.cuh"
 #include <cuda.h>
@@ -51,10 +53,12 @@ struct KParams {
     // sub-problems sharing operands and epilogue (the output-parity classes of a stride-2 transposed conv and their edges), each
     // with its own tile geometry (TW*TH*TN == 128, all powers of two) over the M-space rectangle [y0, y_end) x [x0, x_end)
     int nsub, nint, groups, nbox;    // the first nint sub-problems are interleaved (see decode_tile), groups: see unit_item
-    struct Sub { int tap_begin, ntaps, TW, TH, TN, box, tiles_x, tiles_y, y0, x0, y_end, x_end, oy_off, ox_off, tile_end; } sub[kMaxSubs];
+    struct Sub { int tap_begin, ntaps, TW, TH, TN, box, tiles_x, tiles_y, tiles_m, y0, x0, y_end, x_end, oy_off, ox_off, tile_end; } sub[kMaxSubs];
+    int cluster, b_rows;             // CTAs per cluster (1 or 2): a pair shares the weight tile, each loads b_rows = block_n / cluster of its rows
     int splits; long long split_stride;   // split-K: work item = (tile, K slice); slice s writes its raw partial sums to out_f32 + s * split_stride
     int block_n, stages, stage_bytes, b_bytes, a_bytes;
     int item_tiles;                  // n-tiles per work item: tiles_n for the fused ToRGB (all channels of a pixel), else 1
+    int total_items;                 // sub[nsub - 1].tile_end * splits / item_tiles (a kernel parameter: the producer has no register for it)
     int cin_chunks, nprod, a_img_stride;
     N3DConvTap taps[9];
     int mode;
@@ -70,10 +74,14 @@ struct KParams {
 // mode-0 launches always have a single sub-problem
 __device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.sub[0].TN == 1 && P.mode == 0 && P.item_tiles == P.tiles_n) ? P.rgb.channels : 0; }
 
-struct TileInfo { int sub, tn, x0, y0, n0, split; };
+struct TileInfo { int sub, tn, x0, y0, n0, split; bool pad; };
 // Tiles are numbered sub-problem-major, n-tile minor, except that the first nint sub-problems (the four parity classes of a
 // transposed conv over the same input rectangle, one tile geometry) are interleaved class-minor: the classes of one M tile and
 // n-tile are consecutive tiles.  They share one tile_end, so the search below steps over all of them at once.
+// In a 2-CTA cluster a tile number stands for a pair of M tiles: CTA rank r takes M tile 2m + r with the same sub-problem,
+// n-tile and K slice, so both CTAs run the same K-step sequence on the same weight tiles.  A sub-problem with an odd number of
+// M tiles ends in a pad tile: it repeats its partner's A tile (so that both CTAs still load and consume the same stages) and
+// its epilogue writes nothing.
 __device__ __forceinline__ TileInfo decode_tile(const KParams& P, int tile) {
     const int split = tile % P.splits;                         // K slices of one tile are neighbouring work items (run concurrently)
     tile /= P.splits;
@@ -85,7 +93,13 @@ __device__ __forceinline__ TileInfo decode_tile(const KParams& P, int tile) {
     TileInfo t;
     t.sub = sidx;
     t.tn = local % P.tiles_n;
-    const int tm = local / P.tiles_n;
+    int tm = local / P.tiles_n;
+    t.pad = false;
+    if (P.cluster > 1) {
+        tm = tm * P.cluster + (int)cluster_ctarank();
+        t.pad = tm >= S.tiles_m;
+        if (t.pad) tm -= 1;
+    }
     t.x0 = S.x0 + (tm % S.tiles_x) * S.TW;
     t.y0 = S.y0 + ((tm / S.tiles_x) % S.tiles_y) * S.TH;
     t.n0 = (tm / (S.tiles_x * S.tiles_y)) * S.TN;
@@ -93,15 +107,23 @@ __device__ __forceinline__ TileInfo decode_tile(const KParams& P, int tile) {
     return t;
 }
 
-// Work distribution: CTAs take units round-robin (unit blockIdx.x, then + gridDim.x, ...).  The first P.groups units are P.nint
-// consecutive items each (the parity classes of one M tile and n-tile: they read the same input rows, so all but the first read
-// them from L2, and every such unit costs the same); every later unit is one item.  With P.groups == 0 a CTA's items are
+// Work distribution: clusters take units round-robin (unit c, then + the number of clusters, ...; a launch without clusters has
+// one per CTA), and both CTAs of a cluster take the same units.  The first P.groups units are P.nint consecutive items each (the
+// parity classes of one M tile and n-tile: they read the same input rows, so all but the first read them from L2, and every such
+// unit costs the same); every later unit is one item.  With P.groups == 0 and no clusters a CTA's items are
 // blockIdx.x + k * gridDim.x.
 __device__ __forceinline__ int unit_item(const KParams& P, int unit) { return unit < P.groups ? unit * P.nint : unit + P.groups * (P.nint - 1); }
 __device__ __forceinline__ int next_item(const KParams& P, int item) {      // this CTA's work item after `item`
     const int grouped = P.groups * P.nint;
     if (item < grouped && (item + 1) % P.nint != 0) return item + 1;
-    return unit_item(P, (item < grouped ? item / P.nint : item - grouped + P.groups) + (int)gridDim.x);
+    return unit_item(P, (item < grouped ? item / P.nint : item - grouped + P.groups) + num_clusters_x());
+}
+
+// A consumer warp releases a stage: it arrives on the stage's empty barrier in every CTA of the cluster, since the producer of
+// each CTA multicasts its half of the weight tile into both.
+__device__ __forceinline__ void release_stage(const KParams& P, uint32_t empty_bar) {
+    if (P.cluster == 1) mbar_arrive(empty_bar);
+    else { mbar_arrive_cluster(empty_bar, 0); mbar_arrive_cluster(empty_bar, 1); }
 }
 
 // K-step range [kb, ke) of a work item: all taps x channel chunks, or the item's slice of them under split-K.
@@ -136,7 +158,7 @@ __device__ __forceinline__ void stage_mma(float (&acc0)[BN / 2], float (&acc1)[B
 
 // Main loop of one tile: one stage = one (tap, channel chunk); a stage is released once its wgmmas retired (wait_group 1 after
 // the next stage's wgmmas are issued, so that the tensor cores always have one group queued).  Each of the warpgroup's 4 warps
-// arrives on the stage's empty barrier.
+// arrives on the stage's empty barrier (of both CTAs in a cluster).
 template <int BN, int BK, int NPROD>
 __device__ __forceinline__ void tile_mainloop(const KParams& P, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int ksteps, uint32_t smem_base,
                                               uint32_t bar_base, int lane, int& s, uint32_t& ph) {
@@ -153,13 +175,13 @@ __device__ __forceinline__ void tile_mainloop(const KParams& P, float (&acc0)[BN
         stage_mma<BN, BK, NPROD, false>(acc0, acc1, sa, sa + a_bytes, sa + 2u * a_bytes, sa + 2u * a_bytes + b_bytes);
         wgmma_wait<1>();
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty_base + 8u * (uint32_t)prev_s);
+        if (lane == 0) release_stage(P, empty_base + 8u * (uint32_t)prev_s);
         prev_s = s;
         if (++s == P.stages) { s = 0; ph ^= 1u; }
     }
     wgmma_wait<0>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(empty_base + 8u * (uint32_t)prev_s);
+    if (lane == 0) release_stage(P, empty_base + 8u * (uint32_t)prev_s);
 }
 
 // ---------------------------------------------------------------------------------------------- the kernel
@@ -183,21 +205,25 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             tma_prefetch_desc(&P.tmA[b][0]);
             if (P.nprod == 3) tma_prefetch_desc(&P.tmA[b][1]);
         }
-        for (int s = 0; s < P.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4); }   // one stage feeds one warpgroup
+        // one stage feeds one warpgroup in each CTA of the cluster, and all of them must be done before either producer refills it
+        for (int s = 0; s < P.stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4 * P.cluster); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncthreads();
+    // the partner's first multicast and remote arrivals need this CTA's barriers initialised
+    if (P.cluster > 1) cluster_sync();
+    else __syncthreads();
 
     // work item = item_tiles consecutive tiles (n-tile minor: all n-tiles of one M tile for the fused ToRGB), one CTA each
-    const int total_items = P.sub[P.nsub - 1].tile_end * P.splits / P.item_tiles;
+    const int total_items = P.total_items;
 
     if (warp >= kConsumerThreads / 32) {
         // ===================================================== TMA producer
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
         if (warp == kConsumerThreads / 32 && lane == 0) {
             int s = 0; uint32_t ph = 0;
+            // the full barrier counts the whole stage: this CTA's A tile and both halves of the B tile (one multicast by each CTA)
             const uint32_t tx_bytes = (uint32_t)(P.nprod == 3 ? 2 : 1) * (uint32_t)(P.a_bytes + P.b_bytes);
-            for (int item = unit_item(P, blockIdx.x); item < total_items; item = next_item(P, item))
+            for (int item = unit_item(P, cluster_idx_x()); item < total_items; item = next_item(P, item))
             for (int tile = item * P.item_tiles; tile < (item + 1) * P.item_tiles; ++tile) {
                 const TileInfo ti = decode_tile(P, tile);
                 const int tn = ti.tn, x0 = ti.x0, y0 = ti.y0, n0 = ti.n0;
@@ -214,10 +240,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     mbar_expect_tx(fb, tx_bytes);
                     const int img = n0 + (int)tap.img_off * P.a_img_stride;
                     tma_load_4d(sa, &tmA[0], fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
-                    tma_load_3d(sa + 2 * P.a_bytes, &P.tmB_hi, fb, kc * BK, tn * P.block_n, tap.wtap);
-                    if (P.nprod == 3) {
-                        tma_load_4d(sa + P.a_bytes, &tmA[1], fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
-                        tma_load_3d(sa + 2 * P.a_bytes + P.b_bytes, &P.tmB_lo, fb, kc * BK, tn * P.block_n, tap.wtap);
+                    if (P.nprod == 3) tma_load_4d(sa + P.a_bytes, &tmA[1], fb, kc * BK, x0 + tap.dx, y0 + tap.dy, img);
+                    // B: rows [r * b_rows, (r + 1) * b_rows) of the n-tile (all of them without a cluster, r = 0), multicast to the
+                    // same offset in both CTAs of a cluster.  The rank is read here, not kept: the producer's 24 registers hold no
+                    // further live value without spilling.
+                    const int r = (int)cluster_ctarank();
+                    const uint32_t sb = sa + 2 * P.a_bytes + (uint32_t)(r * P.b_rows * BK * 2);
+                    const int brow = tn * P.block_n + r * P.b_rows;
+                    if (P.cluster == 1) {
+                        tma_load_3d(sb, &P.tmB_hi, fb, kc * BK, brow, tap.wtap);
+                        if (P.nprod == 3) tma_load_3d(sb + P.b_bytes, &P.tmB_lo, fb, kc * BK, brow, tap.wtap);
+                    } else {
+                        tma_load_3d_multicast(sb, &P.tmB_hi, fb, kc * BK, brow, tap.wtap, 0x3);
+                        if (P.nprod == 3) tma_load_3d_multicast(sb + P.b_bytes, &P.tmB_lo, fb, kc * BK, brow, tap.wtap, 0x3);
                     }
                     if (++s == P.stages) { s = 0; ph ^= 1u; }
                 }
@@ -252,7 +287,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         // Order barrier (named barriers 3 + g): a warpgroup starts an item's main loop only after the other warpgroup has issued
         // the main loop of the item before it.  Every stage of that item has then been waited on, so the first stage this warpgroup
         // waits for is at most one phase ahead of its full barrier (a parity wait cannot tell phases two apart).
-        const int first_item = unit_item(P, blockIdx.x);
+        const int first_item = unit_item(P, cluster_idx_x());
         int item = first_item;
         if (g == 1) {
             if (item < total_items) skip_item(item);
@@ -307,7 +342,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             const int ox = x * P.ox_mul + S.ox_off;
             const int y = ti.y0 + th;
             const int oy = y * P.oy_mul + S.oy_off;
-            const bool valid = (n < P.N) && (y < S.y_end) && (x < S.x_end) && (oy < P.OH) && (ox < P.OW);
+            const bool valid = !ti.pad && (n < P.N) && (y < S.y_end) && (x < S.x_end) && (oy < P.OH) && (ox < P.OW);
             const int64_t opix = ((int64_t)n * P.OH + oy) * P.OW + ox;
             float nz = 0.f;
             if (valid && P.noise) nz = __ldg(P.noise + (int64_t)n * P.noise_nstride + (int64_t)oy * P.OW + ox);
@@ -490,6 +525,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (other_item < total_items) skip_item(other_item);
         item = other_item;
         }
+        // Exit barrier of the cluster: the partner may arrive on this CTA's empty barriers until its consumers are done with
+        // their last item, so neither CTA exits before the consumers of both get here.  The producer warpgroup takes no part:
+        // its threads exit when they are done, and a cluster barrier waits for the threads that have not exited.  (Its CTA
+        // lives while the consumers do, and every multicast it issued lands before the partner's consumers get here.)
+        if (P.cluster > 1) cluster_sync();
     }
 }
 
@@ -627,18 +667,39 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     K.nprod = p->nprod; K.a_img_stride = p->a_img_mul;
     N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
+    const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
+    typedef void (*ConvKernel)(const KParams);
+    const ConvKernel kernels[2][5] = {
+        {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
+        {conv_gemm_kernel<16, 64>, conv_gemm_kernel<32, 64>, conv_gemm_kernel<64, 64>, conv_gemm_kernel<96, 64>, conv_gemm_kernel<128, 64>}};
+    const int bi = bn == 16 ? 0 : bn == 32 ? 1 : bn == 64 ? 2 : bn == 96 ? 3 : 4;
+    const ConvKernel kern = kernels[block_k == 64][bi];
+    int rc;
+    if ((rc = n3d_smem_optin((const void*)kern, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
+    // Cluster of 2 for the wide tiles (block_n 96 and 128) without split-K, where some sub-problem has two M tiles to pair.  The
+    // pair shares each weight tile (one half-box multicast per CTA), so a stage costs each CTA 2 * (128 + block_n / 2) rows of
+    // L2 -> shared traffic instead of 2 * (128 + block_n).  The split-K launches and block_n <= 64 gain nothing from pairing on
+    // the H100 (DESIGN.md section 6) and stay unclustered.
+    int max_m = 0;
+    for (int i = 0; i < nsub; ++i) max_m = max(max_m, sub_m[i]);
+    const int cl = (splits == 1 && bn >= 96 && max_m >= 2) ? 2 : 1;
+    const int slots = cl == 1 ? D->num_sms : n3d_max_clusters((const void*)kern, kThreads, 227 * 1024, cl, "n3d_conv_gemm");
+    if (slots <= 0) return N3D_ERR_CUDA;
+    K.cluster = cl; K.b_rows = bn / cl;
     {
-        int end = nint * sub_m[0] * K.tiles_n;                // the interleaved sub-problems share one tile_end
+        for (int i = 0; i < nsub; ++i) K.sub[i].tiles_m = sub_m[i];
+        int end = nint * n3d_div_up(sub_m[0], cl) * K.tiles_n;  // the interleaved sub-problems share one tile_end
         for (int i = 0; i < nsub; ++i) {
-            if (i >= nint) end += sub_m[i] * K.tiles_n;
+            if (i >= nint) end += n3d_div_up(sub_m[i], cl) * K.tiles_n;
             K.sub[i].tile_end = end;
         }
     }
-    // Interleaved parity classes go to one CTA as a unit (same input rows, equal cost per unit) once there are more of their
-    // items than SMs; with fewer, each item gets its own CTA (a shorter critical path than a 4 + 2 + 2 + 1-tap unit).
-    const int units_grouped = sub_m[0] * K.tiles_n;
-    K.groups = (nint > 1 && nint * units_grouped > D->num_sms) ? units_grouped : 0;
-    const int units = K.sub[nsub - 1].tile_end * splits / item_tiles - K.groups * (nint - 1);
+    // Interleaved parity classes go to one CTA (cluster) as a unit (same input rows, equal cost per unit) once there are more of
+    // their items than CTAs (clusters); with fewer, each item gets its own (a shorter critical path than a 4 + 2 + 2 + 1-tap unit).
+    const int units_grouped = n3d_div_up(sub_m[0], cl) * K.tiles_n;
+    K.groups = (nint > 1 && nint * units_grouped > slots) ? units_grouped : 0;
+    K.total_items = K.sub[nsub - 1].tile_end * splits / item_tiles;
+    const int units = K.total_items - K.groups * (nint - 1);
     K.mode = p->mode; K.dcoef = p->dcoef; K.bias = p->bias; K.noise = p->noise; K.noise_nstride = p->noise_nstride;
     K.gain = p->gain; K.slope = p->slope; K.clamp = p->clamp;
     K.out[0] = p->out[0]; K.out[1] = p->out[1];
@@ -650,8 +711,7 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
 
     const uint64_t adims[4] = {(uint64_t)p->Cin, (uint64_t)p->AW, (uint64_t)p->AH, (uint64_t)p->NI};
     const uint64_t wdims[3] = {(uint64_t)p->Cin, (uint64_t)p->Cout, (uint64_t)p->T};
-    const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)bn, 1u};
-    int rc;
+    const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)K.b_rows, 1u};   // bn / 2 is a multiple of 8: whole swizzle atoms
     for (int b = 0; b < K.nbox; ++b) {
         const KParams::Sub& S = K.sub[box_sub[b]];
         const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)S.TW, (uint32_t)S.TH, (uint32_t)S.TN};
@@ -661,16 +721,18 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
     if (p->nprod == 3 && (rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
 
-    const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
-    typedef void (*ConvKernel)(const KParams);
-    const ConvKernel kernels[2][5] = {
-        {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
-        {conv_gemm_kernel<16, 64>, conv_gemm_kernel<32, 64>, conv_gemm_kernel<64, 64>, conv_gemm_kernel<96, 64>, conv_gemm_kernel<128, 64>}};
-    const int bi = bn == 16 ? 0 : bn == 32 ? 1 : bn == 64 ? 2 : bn == 96 ? 3 : 4;
-    const ConvKernel kern = kernels[block_k == 64][bi];
-    if ((rc = n3d_smem_optin((const void*)kern, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
-    const int grid = min(units, D->num_sms);
-    kern<<<grid, kThreads, smem, st>>>(K);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    cfg.gridDim = dim3(cl * min(units, slots));
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    if (cl > 1) {
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr; cfg.numAttrs = 1;
+    }
+    cudaLaunchKernelEx(&cfg, kern, K);
     N3D_CHECK_LAUNCH("n3d_conv_gemm");
     return N3D_OK;
 }

@@ -20,6 +20,37 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// Arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster (which may be this CTA).  Default (CTA
+// scope) release, as for a local arrive: it only signals that this thread's reads of a stage are done (their wgmmas retired).
+// A .cluster-scope release would compile to a GPU-wide memory barrier per arrive, which waits for the epilogue's global stores.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+    asm volatile(
+        "{\n\t.reg .b32 remote;\n\t"
+        "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}"
+        ::"r"(bar), "r"(rank) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// cluster index and number of clusters along x (blockIdx.x and gridDim.x for a launch without clusters)
+__device__ __forceinline__ int cluster_idx_x() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return (int)r;
+}
+__device__ __forceinline__ int num_clusters_x() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+    return (int)r;
+}
+// Cluster barrier: arrive (release), then wait (acquire) for every thread of the cluster that has not exited.  Not .aligned:
+// warps may be diverged here.
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -64,6 +95,13 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm,
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// 3-D tensor load multicast to the CTAs of `cta_mask`: the box lands at shared offset `dst` of each of them and signals the
+// mbarrier at offset `bar` of each.
+__device__ __forceinline__ void tma_load_3d_multicast(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
+        ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask) : "memory");
 }
 // 1-D bulk copy global -> shared (TMA engine, no tensor map): `bytes` contiguous bytes, 16-byte aligned on both sides, completion
 // counted on the mbarrier like the tensor loads.

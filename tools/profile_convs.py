@@ -7,7 +7,11 @@ bench.py measures `roofline.achieved` of conv_gemm_kernel.
 --classes adds, for every distinct stride-2 transposed (up-sampling conv0) shape of the synthesis, the one-launch
 n3d_conv_transposed_gemm against its four output-parity classes (a, b) run as separate n3d_conv_gemm launches, on random operands
 of the same shape: median ms over --reps launches each, and TFLOP/s of the useful work (taps x output positions of the class).
-Usage (GPU box): python tools/profile_convs.py [--config c2|c3] [--batch B] [--top K] [--classes] [--reps R]"""
+
+--nprod 1 runs every launch with one MMA product (hi x hi) instead of three: the same stage ring, half the bytes loaded and a
+third of the MMAs.  A layer's time ratio t(nprod 1) / t(nprod 3) near 1/2 says that feeding the operands bounds it, near 1/3
+that the tensor pipe does.  (The TFLOP/s column stays algorithmic, i.e. it counts the 3-product work.)
+Usage (GPU box): python tools/profile_convs.py [--config c2|c3] [--batch B] [--top K] [--classes] [--reps R] [--nprod 1|3]"""
 import argparse
 import os
 import statistics
@@ -57,6 +61,9 @@ def main():
     ap.add_argument('--top', type=int, default=0, help='print only the K slowest launches (0 = all)')
     ap.add_argument('--classes', action='store_true', help='also time the four parity classes of every transposed layer shape')
     ap.add_argument('--reps', type=int, default=20, help='launches per timing of --classes (median)')
+    ap.add_argument('--nprod', type=int, default=3, choices=[1, 3],
+                    help='MMA products per k-step of the synthesis launches: 3 = bf16x3 (what the engine runs), 1 = hi*hi only '
+                         '(the same stage ring with half the bytes loaded and a third of the MMAs)')
     args = ap.parse_args()
 
     import torch
@@ -77,6 +84,7 @@ def main():
         c_d, v_d = c_cam.to(dev), v.to(dev)
         eng = G._get_engine()
         eng.concurrent = False
+        eng.nprod = args.nprod
         for _ in range(2):                                   # warm-up: module load, allocator, every launch shape once
             G.synthesis(ws, c_d, v_d, noise_mode='const', seed=5)
         eng.prof = []
@@ -89,7 +97,7 @@ def main():
         L = eng.mod.get(info[0])
         return L is not None and L.up == 2
 
-    print(f'# {torch.cuda.get_device_name(dev)}  config {args.config}  batch {B}  conv_gemm launches {len(rows)}')
+    print(f'# {torch.cuda.get_device_name(dev)}  config {args.config}  batch {B}  nprod {args.nprod}  conv_gemm launches {len(rows)}')
     print(f'{"layer":40s} {"Cin":>5s} {"Cout":>5s} {"MH":>4s} {"MW":>4s} {"taps":>4s} {"ms":>8s} {"TFLOP/s":>8s}')
     tot_ms = sum(r[0] for r in rows)
     tot_fl = sum(r[1] for r in rows)
