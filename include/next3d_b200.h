@@ -90,6 +90,7 @@ typedef struct {
     int32_t wtap;         /* index of the [Cout, Cin] weight slab for this tap */
 } N3DConvTap;
 
+/* Split output of a conv / epilogue.  hi and lo (and style, where the epilogue entry points read it) must be 16-byte aligned. */
 typedef struct {
     void* hi;             /* bf16 [.., cstride] or NULL */
     void* lo;
@@ -118,7 +119,9 @@ typedef struct {
  * Epilogue (mode 1): out_f32 <- acc (raw), used by the transposed-conv parity classes and by split-K.
  * Split-K (splits > 1): for launches with a handful of tiles and a long K loop (the 4^2 / 8^2 layers: one 128-row tile, K = 9 * 512)
  * the taps x channel-chunks are cut into `splits` slices that run as independent work items; deterministic (no atomics).
- * Output pixel of tile pixel (y, x) is (y*oy_mul + oy_off, x*ox_mul + ox_off) in an OH x OW image. */
+ * Output pixel of tile pixel (y, x) is (y*oy_mul + oy_off, x*ox_mul + ox_off) in an OH x OW image.
+ * Alignment: a_hi, w_hi, out_f32 and every out[k].hi / lo must be 16-byte aligned (else N3D_ERR_INVALID_ARG); split_stride is a
+ * multiple of 4.  f32_accumulate cannot be combined with split outputs (N3D_ERR_INVALID_ARG). */
 typedef struct {
     const void* a_hi; const void* a_lo;      /* bf16 NHWC [NI, AH, AW, Cin] */
     int32_t NI, AH, AW, Cin;
@@ -158,7 +161,9 @@ int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, int C, const
 
 /* Second half of an up-sampling modulated conv (conv2d_resample.py:114-131 + networks_stylegan2.py:320-329):
  * raw [(2H+1),(2W+1)] transposed-conv output (fp32 NHWC) -> 4x4 FIR [1,3,3,1]^2/64 * 4, pad 1 -> [2H,2W], then the
- * same epilogue as n3d_conv_gemm mode 0 (requires gain > 0 and 0 <= slope <= 1: lrelu / linear). */
+ * same epilogue as n3d_conv_gemm mode 0 (requires gain > 0 and 0 <= slope <= 1: lrelu / linear).
+ * Alignment (this and n3d_splitk_epilogue): raw / partial, dcoef, bias, out_f32 and each used out[k].hi / lo / style must be 16-byte
+ * aligned; f32_cstride, f32_coff, out[k].cstride and out[k].coff are multiples of 4. */
 int n3d_fir_up_epilogue(const float* raw, int N, int H2, int W2, int C, const float* dcoef, const float* bias,
                         const float* noise, int64_t noise_nstride, float gain, float slope, float clamp,
                         const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff, void* stream);

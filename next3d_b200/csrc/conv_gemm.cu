@@ -587,9 +587,15 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     N3D_CHECK_ARG(p->Cout >= 1 && p->N >= 1, "n3d_conv_gemm: bad sizes");
     N3D_CHECK_ARG(((uintptr_t)p->a_hi & 15) == 0 && ((uintptr_t)p->w_hi & 15) == 0, "n3d_conv_gemm: operands must be 16-byte aligned");
     N3D_CHECK_ARG(p->mode == 0 || (p->mode == 1 && p->out_f32), "n3d_conv_gemm: bad mode");
+    // the epilogue's vector stores (float4 / uint4 / 256-bit) test strides and offsets, not the base pointers
+    N3D_CHECK_ARG(((uintptr_t)p->out_f32 & 15) == 0, "n3d_conv_gemm: out_f32 must be 16-byte aligned");
+    for (int k = 0; k < 2; ++k)
+        N3D_CHECK_ARG((((uintptr_t)p->out[k].hi | (uintptr_t)p->out[k].lo) & 15) == 0, "n3d_conv_gemm: split output %d (hi / lo) must be 16-byte aligned", k);
+    // the accumulating fp32 store adds the old values into the epilogue's registers before the split outputs are formed from them
+    N3D_CHECK_ARG(!p->f32_accumulate || (!p->out[0].hi && !p->out[1].hi), "n3d_conv_gemm: f32_accumulate cannot be combined with split outputs");
     const int splits = p->splits > 1 ? p->splits : 1;
-    N3D_CHECK_ARG(splits == 1 || (p->mode == 1 && nsub == 1 && !p->f32_nchw && !p->f32_accumulate && p->split_stride > 0),
-                  "n3d_conv_gemm: split-K needs mode 1 (raw NHWC fp32 partial sums) and a split stride");
+    N3D_CHECK_ARG(splits == 1 || (p->mode == 1 && nsub == 1 && !p->f32_nchw && !p->f32_accumulate && p->split_stride > 0 && p->split_stride % 4 == 0),
+                  "n3d_conv_gemm: split-K needs mode 1 (raw NHWC fp32 partial sums) and a split stride that is a multiple of 4");
     cudaStream_t st = (cudaStream_t)stream;
 
     KParams K;

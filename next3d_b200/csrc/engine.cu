@@ -663,13 +663,19 @@ static bool fir_stream_enabled() {
     return !e || atoi(e) != 0;
 }
 
-// Epilogue descriptor of n3d_fir_up_epilogue and n3d_splitk_epilogue, with the checks both need of it.
+// Epilogue descriptor of n3d_fir_up_epilogue and n3d_splitk_epilogue, with the checks both need of it.  epi_load reads dcoef,
+// bias and the styles as float4, epi_store writes float4 / uint2: strides, offsets and base pointers must all keep that alignment.
 static int make_epi(EpiParams* E, const char* who, const float* dcoef, const float* bias, const float* noise, int64_t noise_nstride,
                     float gain, float slope, float clamp, const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff) {
     N3D_CHECK_ARG(gain > 0.f && slope >= 0.f && slope <= 1.f, "%s: needs gain > 0 and 0 <= slope <= 1 (lrelu / linear)", who);
-    for (int k = 0; k < 2; ++k)
+    for (int k = 0; k < 2; ++k) {
         N3D_CHECK_ARG(!out[k].hi || (out[k].cstride % 4 == 0 && out[k].coff % 4 == 0), "%s: unaligned split output", who);
+        N3D_CHECK_ARG(!out[k].hi || (((uintptr_t)out[k].hi | (uintptr_t)out[k].lo | (uintptr_t)out[k].style) & 15) == 0,
+                      "%s: split output %d (hi / lo / style) must be 16-byte aligned", who, k);
+    }
     N3D_CHECK_ARG(!out_f32 || (f32_cstride % 4 == 0 && f32_coff % 4 == 0), "%s: unaligned fp32 output", who);
+    N3D_CHECK_ARG(((uintptr_t)out_f32 & 15) == 0, "%s: out_f32 must be 16-byte aligned", who);
+    N3D_CHECK_ARG((((uintptr_t)dcoef | (uintptr_t)bias) & 15) == 0, "%s: dcoef and bias must be 16-byte aligned", who);
     *E = EpiParams{dcoef, bias, noise, noise_nstride, gain, slope, clamp, {out[0], out[1]}, out_f32, f32_cstride, f32_coff};
     return N3D_OK;
 }
@@ -689,6 +695,7 @@ extern "C" int n3d_fir_up_epilogue(const float* raw, int N, int H2, int W2, int 
                                    const float* noise, int64_t noise_nstride, float gain, float slope, float clamp,
                                    const N3DSplitOut out[2], float* out_f32, int f32_cstride, int f32_coff, void* stream) {
     N3D_CHECK_ARG(raw && out, "n3d_fir_up_epilogue: null pointer");
+    N3D_CHECK_ARG(((uintptr_t)raw & 15) == 0, "n3d_fir_up_epilogue: raw must be 16-byte aligned");     // float4 loads (both kernels)
     N3D_CHECK_ARG(C % 4 == 0, "n3d_fir_up_epilogue: C must be a multiple of 4");
     N3D_CHECK_ARG(H2 % 2 == 0 && W2 % 2 == 0, "n3d_fir_up_epilogue: output size must be even");
     EpiParams E;
@@ -712,7 +719,7 @@ extern "C" int n3d_fir_up_epilogue(const float* raw, int N, int H2, int W2, int 
             if (eff > best) { best = eff; TR = tr; }
         }
     }
-    if (TR > 0 && ((uintptr_t)raw & 15) == 0 && fir_stream_enabled()) {
+    if (TR > 0 && fir_stream_enabled()) {
         const int row_bytes = (TC + 3) * C * 4;
         const int NR = min(4, (100 * 1024) / row_bytes);        // ring depth: 4 stages
         const int smem = NR * row_bytes + 16 * NR;

@@ -50,12 +50,16 @@ def mapping(sd, cfg, z, c, truncation_psi=1.0, truncation_cutoff=None, prefix='b
 # ------------------------------------------------------------------------------------------ StyleGAN2 blocks
 
 def synthesis_layer(sd, p, x, w, up=1, noise_mode='const', clamp=None):
+    """noise_mode: 'const', 'none', or a dict {layer name: [N,1,H,W] noise already multiplied by noise_strength} that stands for
+    'random' with known draws (networks_stylegan2.py:318-319)."""
     styles = ops.fully_connected(w, sd[f'{p}.affine.weight'], sd[f'{p}.affine.bias'])
     noise = None
-    if noise_mode == 'const':
+    if isinstance(noise_mode, dict):
+        noise = noise_mode[p]
+    elif noise_mode == 'const':
         noise = sd[f'{p}.noise_const'] * sd[f'{p}.noise_strength']
     elif noise_mode != 'none':
-        raise ValueError('oracle supports noise_mode const/none (random is not reproducible)')
+        raise ValueError('oracle supports noise_mode const/none or injected per-layer noise (random is not reproducible)')
     x = ops.modulated_conv2d(x, sd[f'{p}.weight'], styles, noise=noise, up=up, padding=1,
                              resample_filter=sd[f'{p}.resample_filter'], flip_weight=(up == 1))
     return ops.bias_act(x, sd[f'{p}.bias'], act='lrelu', clamp=clamp)

@@ -115,18 +115,21 @@ def test_conv1x1_torgb_nchw_accumulate(K):
     assert range_rel_err(out.cpu(), ref) < 3e-5
 
 
+@pytest.mark.parametrize('per_sample_noise', [False, True], ids=['shared-noise', 'per-sample-noise'])
 @pytest.mark.parametrize('N,Cin,Cout,res,S', [(8, 512, 512, 4, 9), (8, 512, 512, 8, 9), (2, 32, 32, 16, 9), (3, 1024, 512, 8, 4), (1, 64, 96, 8, 3)])
-def test_conv_splitk(K, N, Cin, Cout, res, S):
+def test_conv_splitk(K, N, Cin, Cout, res, S, per_sample_noise):
     """Split-K (deterministic two-pass): S K-slices write raw partial sums, n3d_splitk_epilogue sums them in fixed order and applies
-    the SynthesisLayer epilogue.  Same result as the one-pass kernel (up to fp32 summation order) and bit-reproducible."""
+    the SynthesisLayer epilogue.  Same result as the one-pass kernel (up to fp32 summation order) and bit-reproducible.  Noise is one
+    map for the batch ('const') or one per image (noise_nstride = H * W, 'random')."""
     g = _g(23 + Cin + res)
     x = torch.randn(N, Cin, res, res, generator=g)
     w = torch.randn(Cout, Cin, 3, 3, generator=g) / math.sqrt(Cin * 9)
     d = torch.rand(N, Cout, generator=g) + 0.5
     b = torch.randn(Cout, generator=g)
-    nz = torch.randn(res, res, generator=g) * 0.1
+    nz = torch.randn(*((N,) if per_sample_noise else ()), res, res, generator=g) * 0.1
+    nstride = res * res if per_sample_noise else 0
     s1 = torch.randn(N, Cout, generator=g)
-    y = F.conv2d(x.double(), w.double(), padding=1).float() * d[:, :, None, None] + nz[None, None]
+    y = F.conv2d(x.double(), w.double(), padding=1).float() * d[:, :, None, None] + nz.reshape(-1, 1, res, res)
     y = (F.leaky_relu(y + b[None, :, None, None], 0.2) * math.sqrt(2)).clamp(-2.0, 2.0)
     a_hi, a_lo = _nhwc_split(K, x)
     w_hi, w_lo = K.pack_conv_weight(w.to(DEV))
@@ -140,7 +143,8 @@ def test_conv_splitk(K, N, Cin, Cout, res, S):
         o_hi = torch.zeros(N, res, res, Cout, device=DEV, dtype=torch.bfloat16)
         o_lo = torch.zeros_like(o_hi)
         f32 = torch.zeros(N, res, res, Cout, device=DEV)
-        K.splitk_epilogue(part, dd, bd, nzd, math.sqrt(2), 0.2, 2.0, outs=[K.make_split_out(o_hi, o_lo, s1d, Cout, 0)], out_f32=f32, f32_cstride=Cout)
+        K.splitk_epilogue(part, dd, bd, nzd, math.sqrt(2), 0.2, 2.0, outs=[K.make_split_out(o_hi, o_lo, s1d, Cout, 0)], out_f32=f32, f32_cstride=Cout,
+                          noise_nstride=nstride)
         return f32, o_hi, o_lo
 
     f32, o_hi, o_lo = run()
@@ -212,15 +216,18 @@ def test_upconv_modulated(K, N, Cin, Cout, res):
     assert range_rel_err(out.permute(0, 3, 1, 2).cpu(), ref) < 3e-5
 
 
+@pytest.mark.parametrize('per_sample_noise', [False, True], ids=['shared-noise', 'per-sample-noise'])
 @pytest.mark.parametrize('N,C,H2', [(3, 128, 256), (3, 256, 128), (5, 512, 64), (5, 64, 256), (1, 128, 512)])
-def test_fir_up_streamed_kernel_is_bit_identical(K, N, C, H2, monkeypatch):
+def test_fir_up_streamed_kernel_is_bit_identical(K, N, C, H2, per_sample_noise, monkeypatch):
     """The large layers take the streamed variant (bulk copies of raw rows through a shared-memory ring); it must reproduce the
     register-tiled kernel bit for bit -- fp32 copy, both modulated split-bf16 outputs (one into a concat buffer at a channel offset),
-    noise, clamp -- and both must match an fp64 evaluation of upfirdn2d (upfirdn2d.py:120-164, pad 1/1, gain 4) + bias_act."""
+    noise (one map for the batch, or one per image), clamp -- and both must match an fp64 evaluation of upfirdn2d (upfirdn2d.py:120-164,
+    pad 1/1, gain 4) + bias_act."""
     g = _g(31 + C + H2)
     raw = torch.randn(N, H2 + 1, H2 + 1, C, generator=g).to(DEV)
     d, b = (torch.rand(N, C, generator=g) + 0.5).to(DEV), torch.randn(C, generator=g).to(DEV)
-    nz = (torch.randn(H2, H2, generator=g) * 0.1).to(DEV)
+    nz = (torch.randn(*((N,) if per_sample_noise else ()), H2, H2, generator=g) * 0.1).to(DEV)
+    nstride = H2 * H2 if per_sample_noise else 0
     s0, s1 = torch.randn(N, C, generator=g).to(DEV), torch.randn(N, C, generator=g).to(DEV)
 
     def run(mode):
@@ -229,7 +236,7 @@ def test_fir_up_streamed_kernel_is_bit_identical(K, N, C, H2, monkeypatch):
         o0 = [torch.zeros(N, H2, H2, C, device=DEV, dtype=torch.bfloat16) for _ in range(2)]
         o1 = [torch.zeros(N, H2, H2, 2 * C, device=DEV, dtype=torch.bfloat16) for _ in range(2)]      # concat buffer, second half
         outs = [K.make_split_out(o0[0], o0[1], s0, C, 0), K.make_split_out(o1[0], o1[1], s1, 2 * C, C)]
-        K.fir_up_epilogue(raw, C, d, b, nz, math.sqrt(2), 0.2, 1.5, outs=outs, out_f32=f32, f32_cstride=C)
+        K.fir_up_epilogue(raw, C, d, b, nz, math.sqrt(2), 0.2, 1.5, outs=outs, out_f32=f32, f32_cstride=C, noise_nstride=nstride)
         torch.cuda.synchronize()
         return [f32] + o0 + o1
 
@@ -240,7 +247,7 @@ def test_fir_up_streamed_kernel_is_bit_identical(K, N, C, H2, monkeypatch):
     x = raw.double().permute(0, 3, 1, 2)
     x = F.pad(x, (1, 1, 1, 1))
     y = F.conv2d(x.reshape(N * C, 1, H2 + 3, H2 + 3), torch.outer(f1, f1)[None, None]).reshape(N, C, H2, H2)
-    y = y * d.double()[:, :, None, None] + nz.double()[None, None] + b.double()[None, :, None, None]
+    y = y * d.double()[:, :, None, None] + nz.double().reshape(-1, 1, H2, H2) + b.double()[None, :, None, None]
     y = (F.leaky_relu(y, 0.2) * math.sqrt(2)).clamp(-1.5, 1.5)
     assert range_rel_err(a[0].permute(0, 3, 1, 2).cpu(), y.cpu()) < 1e-6
     assert range_rel_err(_join(a[1], a[2]).permute(0, 3, 1, 2).cpu(), (y * s0.double()[:, :, None, None]).cpu()) < 2e-5
