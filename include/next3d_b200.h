@@ -262,6 +262,17 @@ typedef struct {
 } N3DRender;
 
 int n3d_render_rays(const N3DRender* p, void* stream);
+/* n3d_render_rays plus surface normals (ImportanceRenderer.normal_forward + MipRayMarcher2 with return_normal,
+ * renderer.py:271-355, ray_marcher.py:32-33,61-64): writes rgb / depth / wsum / depth_minmax exactly as n3d_render_rays does and
+ * normal [N, M, 3] = the unit-length composite of n = -d sigma_raw / d x (world space) over the same samples and final weights.
+ * workspace: device float32 buffer of N * M * (2D - 1) floats, D = depth_coarse + depth_fine (depth_coarse when depth_fine = 0);
+ * it holds each ray's sorted sample depths and final weights between the renderer and the normal kernel.  Same argument checks
+ * and sample-count limits as n3d_render_rays.  Two kernel launches. */
+int n3d_render_rays_normals(const N3DRender* p, float* normal, float* workspace, void* stream);
+/* Diagnostics: the normal pass of n3d_render_rays_normals alone, over the samples an earlier n3d_render_rays_normals call with the
+ * same p left in `workspace`; forward = 0 runs the shipped reverse-mode formulation, 1 the forward-mode one (derivative rows through
+ * layer 1).  tools/bench_render.py --normals times the two against each other (DESIGN.md section 3.2a). */
+int n3d_render_normals_pass(const N3DRender* p, int forward, const float* workspace, float* normal, void* stream);
 /* Diagnostics: micro-kernels that measure the hard per-SM limits of the renderer's formulation on the workload described by p
  * (only planes / cameras / res / depth_* / ray_* / box_warp are read; nothing is written but sink[0], which may be NULL):
  * kind 0 = the tri-plane gather alone (rays, depths, 12 taps per sample, 256-bit loads, weighted sum, bf16 split, shared-memory

@@ -58,4 +58,26 @@ __device__ __forceinline__ float softplus_from_log2(float y) {
 __device__ __forceinline__ float softplus_fast(float x) { return softplus_from_log2(x * kLog2e); }
 __device__ __forceinline__ float sigmoid_fast(float x) { return rcp_approx(1.f + ex2_approx(-kLog2e * x)); }
 
+// Camera ray of pixel (row, col) of image n (ray_sampler.py:43-63): origin o and unit direction d.  The renderer and the normal
+// pass both call this, so a sample's position o + t * d is the same float expression in both kernels.
+__device__ __forceinline__ void camera_ray(const N3DRender& P, int n, int row, int col, float (&o)[3], float (&d)[3]) {
+    const float inv = 1.f / (float)P.res, half = 0.5f / (float)P.res;
+    const float xc = (float)col * inv + half, yc = (float)row * inv + half;
+    const float* I = P.intrinsics + n * 9;
+    const float fx = __ldg(I), sk = __ldg(I + 1), cx = __ldg(I + 2), fy = __ldg(I + 4), cy = __ldg(I + 5);
+    const float xl = (xc - cx + cy * sk / fy - sk * yc / fy) / fx;
+    const float yl = (yc - cy) / fy;
+    const float* C = P.cam2world + n * 16;
+    float wv[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        wv[a] = __ldg(C + a * 4) * xl + __ldg(C + a * 4 + 1) * yl + __ldg(C + a * 4 + 2) + __ldg(C + a * 4 + 3);
+        o[a] = __ldg(C + a * 4 + 3);
+        wv[a] -= o[a];
+    }
+    const float nrm = fmaxf(sqrtf(wv[0] * wv[0] + wv[1] * wv[1] + wv[2] * wv[2]), 1e-12f);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) d[a] = wv[a] / nrm;
+}
+
 }  // namespace n3d_rc

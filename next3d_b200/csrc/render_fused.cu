@@ -66,6 +66,7 @@ struct FusedK {
     int gw, log2gw;              // pixel block of a group: gw x 2
     int blocks_x, gpi;           // group map: blocks of 4 x 8 groups, groups per image (padded)
     long long total_groups;
+    float* samples;              // render_fused_kernel<L, true>: per ray the D sorted depths, then the D - 1 final weights
 };
 
 // ---------------------------------------------------------------------------------------------------------------- group -> rays
@@ -95,7 +96,7 @@ struct Ray {
     long long gr;
     bool ok;
 };
-// ray_sampler.py:43-63 for pixel (row i, column j)
+// ray_sampler.py:43-63 for the ray in slot rs of group gg
 __device__ __forceinline__ Ray make_ray(const FusedK& K, int gg, int rs) {
     const N3DRender& P = K.p;
     const RayId id = ray_of(K, gg, rs);
@@ -105,23 +106,10 @@ __device__ __forceinline__ Ray make_ray(const FusedK& K, int gg, int rs) {
     r.img4 = (uint32_t)id.n * (uint32_t)(3 * P.PH * P.PW * 128);       // byte offset of the image's planes
     r.ox = r.oy = r.oz = r.dx = r.dy = r.dz = 0.f;
     if (id.ok) {
-        const float inv = 1.f / (float)P.res, half = 0.5f / (float)P.res;
-        const float xc = (float)id.col * inv + half, yc = (float)id.row * inv + half;
-        const float* I = P.intrinsics + id.n * 9;
-        const float fx = __ldg(I), sk = __ldg(I + 1), cx = __ldg(I + 2), fy = __ldg(I + 4), cy = __ldg(I + 5);
-        const float xl = (xc - cx + cy * sk / fy - sk * yc / fy) / fx;
-        const float yl = (yc - cy) / fy;
-        const float* C = P.cam2world + id.n * 16;
-        float wv[3], o[3];
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            wv[a] = __ldg(C + a * 4) * xl + __ldg(C + a * 4 + 1) * yl + __ldg(C + a * 4 + 2) + __ldg(C + a * 4 + 3);
-            o[a] = __ldg(C + a * 4 + 3);
-            wv[a] -= o[a];
-        }
-        const float nrm = fmaxf(sqrtf(wv[0] * wv[0] + wv[1] * wv[1] + wv[2] * wv[2]), 1e-12f);
+        float o[3], d[3];
+        camera_ray(P, id.n, id.row, id.col, o, d);
         r.ox = o[0]; r.oy = o[1]; r.oz = o[2];
-        r.dx = wv[0] / nrm; r.dy = wv[1] / nrm; r.dz = wv[2] / nrm;
+        r.dx = d[0]; r.dy = d[1]; r.dz = d[2];
     }
     return r;
 }
@@ -457,7 +445,9 @@ __device__ __forceinline__ void init_pipeline_barriers(const Smem& S) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------- the kernel
-template <int L>
+// kExport: also write every ray's merged sorted depths and final interval weights to K.samples (the input of the normal pass,
+// normals_fused_kernel); nothing else changes.
+template <int L, bool kExport>
 __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_constant__ FusedK K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     constexpr int RPW = 32 / L;                 // rays per warp
@@ -763,6 +753,17 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     s6[t] = p < cnt ? s_sg[p] : 0.f;
                 }
                 march_weights<L, 2 * kMaxT>(d6, s6, cnt, lane, w6, tm6);
+                if constexpr (kExport) {
+                    if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
+                        float* const out = K.samples + gr * (2 * cnt - 1);
+#pragma unroll
+                        for (int t = 0; t < 2 * kMaxT; ++t) {
+                            const int p = t * L + j;
+                            if (p < cnt) out[p] = d6[t];
+                            if (p < cnt - 1) out[cnt + p] = w6[t];
+                        }
+                    }
+                }
                 float ws = 0.f, da = 0.f;
                 if (j == 0) s_wb[0] = 0.f;
 #pragma unroll
@@ -786,6 +787,17 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             } else {
                 float w3[kMaxT], tm3[kMaxT];
                 march_weights<L, kMaxT>(tc, sc, cnt, lane, w3, tm3);
+                if constexpr (kExport) {
+                    if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
+                        float* const out = K.samples + gr * (2 * cnt - 1);
+#pragma unroll
+                        for (int t = 0; t < kMaxT; ++t) {
+                            const int k = t * L + j;
+                            if (k < cnt) out[k] = tc[t];
+                            if (k < cnt - 1) out[cnt + k] = w3[t];
+                        }
+                    }
+                }
                 float ws = 0.f, da = 0.f;
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { ws += w3[t]; da += w3[t] * tm3[t]; }
@@ -1088,6 +1100,297 @@ __global__ void __launch_bounds__(kThreads, 1) points_fused_kernel(const __grid_
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------- normals
+// n = -grad_x sigma_raw at every sample the renderer composited, composited with the renderer's final weights
+// (renderer.py:271-355 normal_forward, ray_marcher.py:32-33, 61-64).  Input: the sorted depths and final interval weights that
+// render_fused_kernel<L, true> exported per ray.  Per sample, from ONE fetch of its 12 bilinear taps:
+//   f = plane-mean feature and J_a = d f / d x_a (a = x, y, z; the bilinear-derivative weights of the same tap fractions),
+//   sigma' = sigmoid(W0 f + b0) (softplus' = sigmoid),  d sigma / d x_a = sum_k sigma'_k W1[0, k] (W0 J_a)_k.
+// Two formulations of the last line (template kForward; DESIGN.md section 3.2a has their timings):
+//   reverse (shipped): g = W0^T (sigma' * W1[0, :]) = d sigma / d f on the tensor cores, then three 32-long dot products g . J_a;
+//   forward          : the three derivative rows J_a through layer 1 on the tensor cores, reduced against sigma' * W1[0, :].
+// One warp = one ray at a time, 16 samples per chunk (tile row = sample); every product runs on mma.sync m16n8k16, bf16x3 with fp32
+// accumulation, like the renderer's decoder.  Reverse mode feeds the layer-1 accumulator fragments straight into the second
+// product as its A operand.
+struct NormalsK {
+    N3DRender p;
+    int D;                       // samples per ray in `samples`: Dc + Df, or Dc when coarse-only
+    float scale;                 // 2 / box_warp
+    long long rays;              // N * res * res
+    const float* samples;        // [rays][2D - 1]: D sorted depths, then D - 1 final weights
+    float* normal;               // [rays][3]
+};
+
+constexpr int kNWarps = 8, kNThreads = kNWarps * 32;
+constexpr int kNRows = 16;                                      // samples per chunk
+constexpr int kNFrags = 64;                                     // B fragments per lane: 32 of W0^T (layer 1), then 32 of W0 (layer 1 transposed)
+constexpr int kNOffB0 = kNFrags * 32 * 8;                       // [kNFrags][32 lanes] (hi, lo) words, then b0 [64] | W1[0, :] [64]
+constexpr int kNJStride = 100;                                  // reverse: floats per row of the fp32 J tile ([3][32] + pad)
+constexpr int kNOffWarp = kNOffB0 + 2 * kHidden * 4;
+// per warp: f tile hi | lo ([16] x 64-byte SWIZZLE_64B rows), then the J tile: reverse [16][100] fp32, forward 3 x (hi | lo) bf16 tiles
+constexpr int kNJBytes = kNRows * kNJStride * 4 > 6 * kNRows * 64 ? kNRows * kNJStride * 4 : 6 * kNRows * 64;
+constexpr int kNWarpBytes = 2 * kNRows * 64 + kNJBytes;
+constexpr int kNSmemBytes = kNOffWarp + kNWarps * kNWarpBytes;  // 84480: two CTAs per SM
+
+// The four bilinear taps of plane pl at scaled point (x, y, z), as setup_taps: texel byte offsets, weights and the derivatives of
+// the weights along the plane's two world axes (a, b) = (x, y), (x, z), (z, y) (grid_sample align_corners=False:
+// d ix / d x_a = scale * PW / 2); the 1/3 of the plane mean is folded into all three.  Taps outside the plane (zeros padding) and
+// invalid samples get weight 0 and point at texel 0.
+struct PlaneTaps {
+    uint32_t off[4];
+    float w[4], wa[4], wb[4];
+};
+__device__ __forceinline__ PlaneTaps plane_taps(int pl, float x, float y, float z, bool valid, uint32_t img4, int PH, int PW, float scale) {
+    PlaneTaps t;
+    const float gx = pl == 2 ? z : x, gy = pl == 1 ? z : y;
+    const float ix = ((gx + 1.f) * (float)PW - 1.f) * 0.5f, iy = ((gy + 1.f) * (float)PH - 1.f) * 0.5f;
+    const float flx = floorf(ix), fly = floorf(iy);
+    const float fx = ix - flx, fy = iy - fly;
+    const int x0 = (int)fminf(fmaxf(flx, -2.f), (float)PW), y0 = (int)fminf(fmaxf(fly, -2.f), (float)PH);
+    const uint32_t pbase = img4 + (uint32_t)(pl * PH * PW) * 128u;
+    const float ka = scale * (float)PW * (0.5f / 3.f), kb = scale * (float)PH * (0.5f / 3.f);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const int xi = x0 + (c & 1), yi = y0 + (c >> 1);
+        const float wx = (c & 1) ? fx : 1.f - fx, wy = (c >> 1) ? fy : 1.f - fy;
+        const bool inside = valid && xi >= 0 && xi < PW && yi >= 0 && yi < PH;
+        t.off[c] = inside ? pbase + (uint32_t)(yi * PW + xi) * 128u : 0u;
+        t.w[c] = inside ? wx * wy * (1.f / 3.f) : 0.f;
+        t.wa[c] = inside ? ((c & 1) ? wy : -wy) * ka : 0.f;
+        t.wb[c] = inside ? ((c >> 1) ? wx : -wx) * kb : 0.f;
+    }
+    return t;
+}
+
+// Layer 1 of the 16 rows of a bf16 (hi, lo) SWIZZLE_64B tile: acc[nt] = rows x hidden units 8 nt .. 8 nt + 7 (m16n8 fragments).
+__device__ __forceinline__ void normals_layer1(const uint8_t* th, const uint8_t* tl, const uint2* frag, int lane, float (&acc)[8][4]) {
+    const int g = lane >> 2, c = lane & 3;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < kFeat / 16; ++ks) {
+        uint32_t ah[4], al[4];
+        ah[0] = lds32(th + sw64_off(g, ks * 32 + 4 * c)); ah[1] = lds32(th + sw64_off(g + 8, ks * 32 + 4 * c));
+        ah[2] = lds32(th + sw64_off(g, ks * 32 + 16 + 4 * c)); ah[3] = lds32(th + sw64_off(g + 8, ks * 32 + 16 + 4 * c));
+        al[0] = lds32(tl + sw64_off(g, ks * 32 + 4 * c)); al[1] = lds32(tl + sw64_off(g + 8, ks * 32 + 4 * c));
+        al[2] = lds32(tl + sw64_off(g, ks * 32 + 16 + 4 * c)); al[3] = lds32(tl + sw64_off(g + 8, ks * 32 + 16 + 4 * c));
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+            const uint2 b0 = frag[((ks * 8 + nt) * 2) * 32 + lane], b1 = frag[((ks * 8 + nt) * 2 + 1) * 32 + lane];
+            mma_bf16_16816(acc[nt], ah, b0.x, b1.x);
+            mma_bf16_16816(acc[nt], ah, b0.y, b1.y);
+            mma_bf16_16816(acc[nt], al, b0.x, b1.x);
+        }
+    }
+}
+
+__device__ __forceinline__ void store_split_row(uint8_t* th, uint8_t* tl, int row, int c, const float (&v)[8]) {
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) split_bf16x2(v[2 * q], v[2 * q + 1], h[q], l[q]);
+    const uint32_t off = sw64_off(row, c * 16);
+    *reinterpret_cast<uint4*>(th + off) = make_uint4(h[0], h[1], h[2], h[3]);
+    *reinterpret_cast<uint4*>(tl + off) = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
+template <bool kForward>
+__global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __grid_constant__ NormalsK K) {
+    extern __shared__ __align__(16) uint8_t nsm[];
+    const N3DRender& P = K.p;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint2* const frag = reinterpret_cast<const uint2*>(nsm);
+    const float* const sB0 = reinterpret_cast<const float*>(nsm + kNOffB0);
+    const float* const sW1 = sB0 + kHidden;
+
+    // ---- B fragments (mma.m16n8k16: b0 = B[2c, 2c+1][g], b1 = B[2c+8, 2c+9][g]) split into bf16 (hi, lo), one (hi, lo) pair per lane
+    for (int i = tid; i < kNFrags * 32; i += kNThreads) {
+        const int f = i >> 5, g = (i >> 2) & 7, c = i & 3;
+        float v0, v1;
+        if (f < 32) {            // B[k = feature][n = hidden] = W0[n][k];  f = (ks * 8 + nt) * 2 + reg
+            const int ks = f >> 4, nt = (f >> 1) & 7, k0 = 16 * ks + 8 * (f & 1) + 2 * c;
+            v0 = __ldg(P.w0 + (8 * nt + g) * kFeat + k0);
+            v1 = __ldg(P.w0 + (8 * nt + g) * kFeat + k0 + 1);
+        } else {                 // B[k = hidden][n = feature] = W0[k][n];  f - 32 = (ks * 4 + nt) * 2 + reg
+            const int e = f - 32, ks = e >> 3, nt = (e >> 1) & 3, k0 = 16 * ks + 8 * (e & 1) + 2 * c;
+            v0 = __ldg(P.w0 + k0 * kFeat + 8 * nt + g);
+            v1 = __ldg(P.w0 + (k0 + 1) * kFeat + 8 * nt + g);
+        }
+        uint32_t h, l;
+        split_bf16x2(v0, v1, h, l);
+        reinterpret_cast<uint2*>(nsm)[i] = make_uint2(h, l);
+    }
+    for (int i = tid; i < kHidden; i += kNThreads) {
+        reinterpret_cast<float*>(nsm + kNOffB0)[i] = __ldg(P.b0 + i);
+        reinterpret_cast<float*>(nsm + kNOffB0)[kHidden + i] = __ldg(P.w1 + i);       // sigma row of W1
+    }
+    __syncthreads();
+
+    uint8_t* const fh = nsm + kNOffWarp + warp * kNWarpBytes;
+    uint8_t* const fl = fh + kNRows * 64;
+    uint8_t* const jb = fh + 2 * kNRows * 64;                      // J tile
+    float* const jt = reinterpret_cast<float*>(jb);
+    const char* const planes = reinterpret_cast<const char*>(P.planes);
+    const int g = lane >> 2, c = lane & 3;               // fetch: sample g of a step, channel octet c; mma: fragment row g, column pair c
+    const int D = K.D, M = P.res * P.res;
+    const long long warps = (long long)gridDim.x * kNWarps;
+    for (long long gr = (long long)blockIdx.x * kNWarps + warp; gr < K.rays; gr += warps) {
+        const int n = (int)(gr / M), m = (int)(gr - (long long)n * M);
+        float o[3], d[3];
+        camera_ray(P, n, m / P.res, m % P.res, o, d);
+        const uint32_t img4 = (uint32_t)n * (uint32_t)(3 * P.PH * P.PW * 128);
+        const float* const ts = K.samples + gr * (2 * D - 1);
+        const float* const wts = ts + D;
+        float nacc[3] = {0.f, 0.f, 0.f}, wsum = 0.f;
+        for (int i0 = 0; i0 < D; i0 += kNRows) {
+            // ---- fetch: f and J_x, J_y, J_z of samples i0 .. i0 + 15 from one read of the 12 taps; 8 samples x 4 channel octets per
+            // step, so lane (g, c) fetches rows g and g + 8 -- the two rows its mma fragments hold
+#pragma unroll 1
+            for (int step = 0; step < 2; ++step) {
+                const int row = step * 8 + g, i = i0 + row;
+                const bool valid = i < D;
+                const float t = valid ? __ldg(ts + i) : 0.f;
+                const float x = K.scale * (o[0] + t * d[0]), y = K.scale * (o[1] + t * d[1]), z = K.scale * (o[2] + t * d[2]);
+                float fv[8], jv[3][8];
+#pragma unroll
+                for (int ch = 0; ch < 8; ++ch) { fv[ch] = 0.f; jv[0][ch] = 0.f; jv[1][ch] = 0.f; jv[2][ch] = 0.f; }
+#pragma unroll 1
+                for (int pl = 0; pl < 3; ++pl) {                  // one plane's four taps in flight: keeps the 32 accumulators in registers
+                    const PlaneTaps tp = plane_taps(pl, x, y, z, valid, img4, P.PH, P.PW, K.scale);
+                    float v[4][8], da[8], db[8];
+#pragma unroll
+                    for (int cc = 0; cc < 4; ++cc) ldg_nc_256(reinterpret_cast<const float*>(planes + tp.off[cc] + c * 32), v[cc]);
+#pragma unroll
+                    for (int ch = 0; ch < 8; ++ch) {
+                        da[ch] = 0.f; db[ch] = 0.f;
+#pragma unroll
+                        for (int cc = 0; cc < 4; ++cc) {
+                            fv[ch] = fmaf(tp.w[cc], v[cc][ch], fv[ch]);
+                            da[ch] = fmaf(tp.wa[cc], v[cc][ch], da[ch]);
+                            db[ch] = fmaf(tp.wb[cc], v[cc][ch], db[ch]);
+                        }
+                        // plane 0 <- (x, y), 1 <- (x, z), 2 <- (z, y)
+                        jv[0][ch] += pl != 2 ? da[ch] : 0.f;
+                        jv[1][ch] += pl != 1 ? db[ch] : 0.f;
+                        jv[2][ch] += pl == 1 ? db[ch] : (pl == 2 ? da[ch] : 0.f);
+                    }
+                }
+                store_split_row(fh, fl, row, c, fv);
+#pragma unroll
+                for (int a = 0; a < 3; ++a) {
+                    if constexpr (kForward) {
+                        store_split_row(jb + a * 2 * kNRows * 64, jb + a * 2 * kNRows * 64 + kNRows * 64, row, c, jv[a]);
+                    } else {
+                        float* const dst = jt + row * kNJStride + a * 32 + c * 8;
+                        *reinterpret_cast<float4*>(dst) = make_float4(jv[a][0], jv[a][1], jv[a][2], jv[a][3]);
+                        *reinterpret_cast<float4*>(dst + 4) = make_float4(jv[a][4], jv[a][5], jv[a][6], jv[a][7]);
+                    }
+                }
+            }
+            __syncwarp();
+            // ---- u = sigmoid(W0 f + b0) * W1[0, :] for the 16 rows
+            float u[8][4];
+            normals_layer1(fh, fl, frag, lane, u);
+#pragma unroll
+            for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int k = 8 * nt + 2 * c + (e & 1);
+                    u[nt][e] = sigmoid_fast(u[nt][e] + sB0[k]) * sW1[k];
+                }
+            float gs[2][3];                                  // d sigma / d x_a of rows g (hr 0) and g + 8 (hr 1), partial over this lane's columns
+            if constexpr (kForward) {
+#pragma unroll 1
+                for (int a = 0; a < 3; ++a) {                  // one derivative row set at a time (register budget)
+                    float pa[8][4];
+                    normals_layer1(jb + a * 2 * kNRows * 64, jb + a * 2 * kNRows * 64 + kNRows * 64, frag, lane, pa);
+                    float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+                    for (int nt = 0; nt < 8; ++nt) {
+                        s0 = fmaf(u[nt][0], pa[nt][0], fmaf(u[nt][1], pa[nt][1], s0));
+                        s1 = fmaf(u[nt][2], pa[nt][2], fmaf(u[nt][3], pa[nt][3], s1));
+                    }
+                    if (a == 0) { gs[0][0] = s0; gs[1][0] = s1; }
+                    else if (a == 1) { gs[0][1] = s0; gs[1][1] = s1; }
+                    else { gs[0][2] = s0; gs[1][2] = s1; }
+                }
+            } else {
+                // g [16 x 32] = u W0: the accumulator fragments of hidden units 16 ks .. 16 ks + 15 are the A fragment of k-step ks
+                float gacc[4][4];
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) gacc[nt][e] = 0.f;
+#pragma unroll
+                for (int ks = 0; ks < kHidden / 16; ++ks) {
+                    uint32_t ah[4], al[4];
+                    split_bf16x2(u[2 * ks][0], u[2 * ks][1], ah[0], al[0]);
+                    split_bf16x2(u[2 * ks][2], u[2 * ks][3], ah[1], al[1]);
+                    split_bf16x2(u[2 * ks + 1][0], u[2 * ks + 1][1], ah[2], al[2]);
+                    split_bf16x2(u[2 * ks + 1][2], u[2 * ks + 1][3], ah[3], al[3]);
+#pragma unroll
+                    for (int nt = 0; nt < 4; ++nt) {
+                        const uint2 b0 = frag[(32 + (ks * 4 + nt) * 2) * 32 + lane], b1 = frag[(32 + (ks * 4 + nt) * 2 + 1) * 32 + lane];
+                        mma_bf16_16816(gacc[nt], ah, b0.x, b1.x);
+                        mma_bf16_16816(gacc[nt], ah, b0.y, b1.y);
+                        mma_bf16_16816(gacc[nt], al, b0.x, b1.x);
+                    }
+                }
+                // g . J_a over this lane's 8 features of rows g and g + 8
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                    for (int a = 0; a < 3; ++a) {
+                        const float* const jr = jt + (g + 8 * hr) * kNJStride + a * 32 + 2 * c;
+                        float s = 0.f;
+#pragma unroll
+                        for (int nt = 0; nt < 4; ++nt) {
+                            const float2 j2 = *reinterpret_cast<const float2*>(jr + 8 * nt);
+                            s = fmaf(gacc[nt][2 * hr], j2.x, fmaf(gacc[nt][2 * hr + 1], j2.y, s));
+                        }
+                        gs[hr][a] = s;
+                    }
+            }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                for (int a = 0; a < 3; ++a) {
+                    gs[hr][a] += __shfl_xor_sync(FULL, gs[hr][a], 1);
+                    gs[hr][a] += __shfl_xor_sync(FULL, gs[hr][a], 2);
+                }
+            if (c == 0) {
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int i = i0 + g + 8 * hr;
+                    if (i < D) {
+                        // n_mid composite: sum_i w_i (n_i + n_i+1) / 2 = sum_i n_i (w_i-1 + w_i) / 2 (w_-1 = w_D-1 = 0)
+                        const float wi = i < D - 1 ? __ldg(wts + i) : 0.f;
+                        const float coef = 0.5f * ((i > 0 ? __ldg(wts + i - 1) : 0.f) + wi);
+                        nacc[0] -= coef * gs[hr][0]; nacc[1] -= coef * gs[hr][1]; nacc[2] -= coef * gs[hr][2];
+                        wsum += wi;
+                    }
+                }
+            }
+            __syncwarp();                                    // tiles free for the next chunk
+        }
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) {
+            nacc[0] += __shfl_xor_sync(FULL, nacc[0], s);
+            nacc[1] += __shfl_xor_sync(FULL, nacc[1], s);
+            nacc[2] += __shfl_xor_sync(FULL, nacc[2], s);
+            wsum += __shfl_xor_sync(FULL, wsum, s);
+        }
+        if (lane == 0) {
+            const float rx = nacc[0] / wsum, ry = nacc[1] / wsum, rz = nacc[2] / wsum;
+            const float len = sqrtf(rx * rx + ry * ry + rz * rz) + 1e-7f;
+            K.normal[gr * 3 + 0] = rx / len;
+            K.normal[gr * 3 + 1] = ry / len;
+            K.normal[gr * 3 + 2] = rz / len;
+        }
+    }
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------- ceilings
@@ -1223,29 +1526,81 @@ int launch_points(const float* planes, int N, int PH, int PW, const float* coord
 }
 }  // namespace
 
-extern "C" int n3d_render_rays(const N3DRender* p, void* stream) {
+namespace {
+// Argument checks of n3d_render_rays / n3d_render_rays_normals (messages start with `who`).
+int check_render(const N3DRender* p, const char* who) {
     N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && p->w0 && p->b0 && p->w1 && p->b1 && p->rgb && p->depth && p->wsum,
-                  "n3d_render_rays: null pointer");
+                  "%s: null pointer", who);
     if (p->depth_coarse > kMaxD || p->depth_fine > kMaxD) {
-        n3d_set_error("n3d_render_rays: depth resolutions (%d, %d) above %d samples per pass are not supported", p->depth_coarse, p->depth_fine, kMaxD);
+        n3d_set_error("%s: depth resolutions (%d, %d) above %d samples per pass are not supported", who, p->depth_coarse, p->depth_fine, kMaxD);
         return N3D_ERR_UNSUPPORTED;
     }
-    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_fine >= 0, "n3d_render_rays: depth resolutions (%d, %d): need coarse >= 4, fine >= 0",
+    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_fine >= 0, "%s: depth resolutions (%d, %d): need coarse >= 4, fine >= 0", who,
                   p->depth_coarse, p->depth_fine);
-    N3D_CHECK_ARG(p->res >= 1 && p->N >= 1 && p->ray_start > 0.f && p->ray_end > p->ray_start && p->box_warp > 0.f, "n3d_render_rays: bad ray setup");
-    N3D_CHECK_ARG((long long)p->N * 3 * p->PH * p->PW * 128 < (1ll << 32), "n3d_render_rays: plane tensor too large for 32-bit texel offsets");
+    N3D_CHECK_ARG(p->res >= 1 && p->N >= 1 && p->ray_start > 0.f && p->ray_end > p->ray_start && p->box_warp > 0.f, "%s: bad ray setup", who);
+    N3D_CHECK_ARG((long long)p->N * 3 * p->PH * p->PW * 128 < (1ll << 32), "%s: plane tensor too large for 32-bit texel offsets", who);
+    return N3D_OK;
+}
+
+// render_fused_kernel<L, kExport> on the checked workload p; kExport writes the per-ray samples to `samples`.
+template <bool kExport>
+int launch_render(const N3DRender* p, float* samples, const char* who, void* stream) {
     int L;
-    const FusedK K = make_fused(p, L);
+    FusedK K = make_fused(p, L);
+    K.samples = samples;
     const int smem = kSmemBytes + 1024;
-    if (int rc = n3d_smem_optin(L == 16 ? (const void*)render_fused_kernel<16> : (const void*)render_fused_kernel<32>, smem, "n3d_render_rays"))
+    if (int rc = n3d_smem_optin(L == 16 ? (const void*)render_fused_kernel<16, kExport> : (const void*)render_fused_kernel<32, kExport>, smem, who))
         return rc;
     const N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
     const int grid = (int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms);
-    if (L == 16) render_fused_kernel<16><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
-    else render_fused_kernel<32><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
-    N3D_CHECK_LAUNCH("n3d_render_rays");
+    if (L == 16) render_fused_kernel<16, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    else render_fused_kernel<32, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    N3D_CHECK_LAUNCH(who);
     return N3D_OK;
+}
+}  // namespace
+
+extern "C" int n3d_render_rays(const N3DRender* p, void* stream) {
+    if (int rc = check_render(p, "n3d_render_rays")) return rc;
+    return launch_render<false>(p, nullptr, "n3d_render_rays", stream);
+}
+
+namespace {
+// normals_fused_kernel<kForward> over the samples render_fused_kernel<L, true> left in `workspace`.
+template <bool kForward>
+int launch_normals(const N3DRender* p, const float* workspace, float* normal, const char* who, void* stream) {
+    NormalsK K;
+    K.p = *p;
+    K.D = p->depth_fine > 0 ? p->depth_coarse + p->depth_fine : p->depth_coarse;
+    K.scale = 2.f / p->box_warp;
+    K.rays = (long long)p->N * p->res * p->res;
+    K.samples = workspace;
+    K.normal = normal;
+    if (int rc = n3d_smem_optin((const void*)normals_fused_kernel<kForward>, kNSmemBytes, who)) return rc;
+    const N3DDeviceState* D = n3d_device_state();
+    if (!D) return N3D_ERR_CUDA;
+    const long long blocks = (K.rays + kNWarps - 1) / kNWarps;
+    const int grid = (int)(blocks < 2ll * D->num_sms ? blocks : 2ll * D->num_sms);
+    normals_fused_kernel<kForward><<<grid, kNThreads, kNSmemBytes, (cudaStream_t)stream>>>(K);
+    N3D_CHECK_LAUNCH(who);
+    return N3D_OK;
+}
+}  // namespace
+
+extern "C" int n3d_render_rays_normals(const N3DRender* p, float* normal, float* workspace, void* stream) {
+    const char* who = "n3d_render_rays_normals";
+    if (int rc = check_render(p, who)) return rc;
+    N3D_CHECK_ARG(normal && workspace, "%s: null pointer", who);
+    if (int rc = launch_render<true>(p, workspace, who, stream)) return rc;
+    return launch_normals<false>(p, workspace, normal, who, stream);
+}
+
+extern "C" int n3d_render_normals_pass(const N3DRender* p, int forward, const float* workspace, float* normal, void* stream) {
+    const char* who = "n3d_render_normals_pass";
+    if (int rc = check_render(p, who)) return rc;
+    N3D_CHECK_ARG(normal && workspace && (forward == 0 || forward == 1), "%s: bad args", who);
+    return forward ? launch_normals<true>(p, workspace, normal, who, stream) : launch_normals<false>(p, workspace, normal, who, stream);
 }
 
 extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream) {

@@ -603,16 +603,26 @@ class Engine:
         u_c, u_f = sampler_noise if sampler_noise is not None else (None, None)
         if u_c is not None:
             u_c, u_f = u_c.to(dev, torch.float32).contiguous(), u_f.to(dev, torch.float32).contiguous()
+        normal = self._f32(N, M, 3) if self.rk.get('return_normal', False) else None
         ev = self._prof_begin()
-        K.render_rays(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, u_coarse=u_c, u_fine=u_f, seed=seed, seed_ptr=seed_ptr)
+        if normal is None:
+            K.render_rays(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, u_coarse=u_c, u_fine=u_f, seed=seed, seed_ptr=seed_ptr)
+        else:                                                               # return_normal (renderer.py:271-355, ray_marcher.py:61-64)
+            ws_normals = self._f32(K.normals_workspace_floats(N, R, self.rk))
+            K.render_rays_normals(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, normal, ws_normals, u_coarse=u_c, u_fine=u_f,
+                                  seed=seed, seed_ptr=seed_ptr)
         self._prof_end(ev, 'render_rays')
         K.depth_clamp(depth, mm)
         image = self._f32(N, 3, cfg.img_resolution, cfg.img_resolution)
         self._superresolution(feat, self.rk['superresolution_noise_mode'], image)
         self.launches = K.launches - n0
         result = {'image': image, 'image_raw': feat.permute(0, 3, 1, 2)[:, :3], 'image_depth': depth}
+        if normal is not None:
+            result['image_normal'] = normal.view(N, R, R, 3).permute(0, 3, 1, 2)          # ray m = i * R + j -> pixel (i, j)
         if return_intermediates:
             inter.update(planes=planes, feature_image=feat, weights_sum=wsum)
+            if normal is not None:                                          # per ray: D sorted sample depths, then D - 1 final weights
+                inter['normal_samples'] = ws_normals.view(N, M, -1)
             result['intermediates'] = inter
         return result
 
@@ -631,7 +641,7 @@ class Engine:
         rk = self.rk
         key = (ws.shape[0], R, noise_mode, tuple(v.shape), rk['depth_resolution'], rk['depth_resolution_importance'], float(rk['ray_start']),
                float(rk['ray_end']), float(rk['box_warp']), bool(rk.get('white_back', False)), rk['superresolution_noise_mode'],
-               bool(rk.get('sr_antialias', True)))
+               bool(rk.get('sr_antialias', True)), bool(rk.get('return_normal', False)))
         g = self._graphs.get(key)
         if g is None:
             st = dict(ws=torch.empty(ws.shape, dtype=torch.float32, device=self.device), c=torch.empty(c.shape, dtype=torch.float32, device=self.device),

@@ -220,9 +220,8 @@ def _render_desc(planes, cam2world, intrinsics, res, opts, seed):
     return p
 
 
-def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
-                seed_ptr=None):
-    """planes [N,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in."""
+def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr):
+    """Render descriptor of n3d_render_rays / n3d_render_rays_normals, after rejecting the rendering options the renderer lacks."""
     unsupported = [k for k, bad in (('disparity_space_sampling', bool(opts.get('disparity_space_sampling', False))),
                                     ('density_noise', float(opts.get('density_noise', 0) or 0) > 0),
                                     ('clamp_mode', opts.get('clamp_mode', 'softplus') != 'softplus'),
@@ -235,7 +234,45 @@ def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum,
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
     p.rgb, p.depth, p.wsum, p.depth_minmax = ptr(rgb), ptr(depth), ptr(wsum), ptr(depth_minmax)
     p.white_back = int(bool(opts.get('white_back', False)))
+    return p
+
+
+def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
+                seed_ptr=None):
+    """planes [N,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in."""
+    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
     _run('n3d_render_rays', C.byref(p), stream_ptr())
+
+
+def normals_workspace_floats(N, res, opts):
+    """Floats of the n3d_render_rays_normals workspace: N * M * (2D - 1), D = samples per ray after the merge."""
+    Dc, Df = opts['depth_resolution'], opts['depth_resolution_importance']
+    return N * res * res * (2 * (Dc + Df if Df > 0 else Dc) - 1)
+
+
+def render_rays_normals(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, normal, workspace=None, u_coarse=None,
+                        u_fine=None, seed=0, seed_ptr=None):
+    """render_rays (same outputs, bit for bit) plus normal [N, M, 3]: unit world-space normals -grad sigma composited with the final
+    weights (rendering option return_normal).  workspace: fp32 device buffer of normals_workspace_floats() floats, or None to
+    allocate one here."""
+    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
+    n_ws = normals_workspace_floats(planes.shape[0], res, opts)
+    if workspace is None:
+        workspace = torch.empty(n_ws, dtype=torch.float32, device=planes.device)
+    elif workspace.numel() < n_ws or workspace.dtype != torch.float32:
+        raise RuntimeError(f'render_rays_normals: workspace needs {n_ws} float32 elements, got {workspace.numel()} {workspace.dtype}')
+    if normal.numel() != planes.shape[0] * res * res * 3 or normal.dtype != torch.float32:
+        raise RuntimeError(f'render_rays_normals: normal must be float32 [N, M, 3], got {tuple(normal.shape)} {normal.dtype}')
+    _run('n3d_render_rays_normals', C.byref(p), ptr(normal), ptr(workspace), stream_ptr(), kernels=2)
+
+
+def render_normals_pass(planes, cam2world, intrinsics, res, opts, dec, normal, workspace, forward=False):
+    """Diagnostics (n3d_render_normals_pass): the normal pass alone over the samples an earlier render_rays_normals call with the same
+    workload left in `workspace`; forward=True runs the forward-mode formulation instead of the shipped reverse mode."""
+    p = _render_desc(planes, cam2world, intrinsics, res, opts, 0)
+    p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
+    p.rgb = p.depth = p.wsum = ptr(normal)         # not written; the argument checks are n3d_render_rays'
+    _run('n3d_render_normals_pass', C.byref(p), int(bool(forward)), ptr(workspace), ptr(normal), stream_ptr())
 
 
 def depth_clamp(depth, depth_minmax):

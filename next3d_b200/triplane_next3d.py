@@ -188,7 +188,9 @@ class TriPlaneGenerator(torch.nn.Module):
                   sampler_noise=None, seed=None, **synthesis_kwargs):
         """-> {'image': [N,3,R,R], 'image_raw': [N,3,r,r], 'image_depth': [N,1,r,r]} (triplane_next3d.py:117-188).
         Extra keyword `sampler_noise=(u_coarse [N,M,Dc,1], u_fine [N*M,Df])` injects the stratified / importance sampling
-        uniforms (parity tests); by default the renderer draws them from an in-kernel counter RNG seeded per call."""
+        uniforms (parity tests); by default the renderer draws them from an in-kernel counter RNG seeded per call.
+        With `rendering_kwargs['return_normal']` set the output also holds 'image_normal' [N,3,r,r]: unit world-space normals
+        -grad sigma composited like the colours (renderer.py:271-355, ray_marcher.py:61-64)."""
         if neural_rendering_resolution is None:
             neural_rendering_resolution = self.neural_rendering_resolution
         else:

@@ -1,10 +1,70 @@
-"""Time the fused renderer alone on a benchmark workload (random planes).  python tools/bench_render.py [c2|c3]"""
-import sys, os, math
+"""Time the fused renderer alone on a benchmark workload (random planes).  python tools/bench_render.py [c2|c3] [--normals]
+--normals: n3d_render_rays_normals (renderer + normal pass) against n3d_render_rays on both the C2 and the C3 workload, and the
+normal pass alone in its shipped reverse-mode and its forward-mode formulation (n3d_render_normals_pass), alternated."""
+import sys, os, math, subprocess
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from next3d_b200 import config, weights, kernels as K
 cfg = config.full_config(512)
-which = sys.argv[1] if len(sys.argv) > 1 else 'c2'
+args = [a for a in sys.argv[1:] if not a.startswith('--')]
+which = args[0] if args else 'c2'
+
+
+def _events(fn, reps, flush):
+    ts = []
+    for i in range(reps):
+        flush.zero_()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        fn(i)
+        e1.record(); torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1))
+    ts.sort()
+    return ts[len(ts) // 2], ts[0]
+
+
+if '--normals' in sys.argv:
+    power = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader', '-i', str(torch.cuda.current_device())],
+                           capture_output=True, text=True).stdout.strip()
+    print(f'card {torch.cuda.get_device_name()}  power limit {power or "unknown"}', flush=True)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')
+    for name, (N, R, D) in (('c2', (8, 64, 48)), ('c3', (16, 128, 96))):
+        opts = dict(cfg.rendering_kwargs, depth_resolution=D, depth_resolution_importance=D)
+        g = torch.Generator().manual_seed(0)
+        planes = torch.randn(N, 3, 256, 256, 32, generator=g).cuda()
+        dec = (torch.randn(64, 32, generator=g).cuda() / math.sqrt(32), torch.randn(64, generator=g).cuda() * 0.1,
+               torch.randn(33, 64, generator=g).cuda() / math.sqrt(64), torch.randn(33, generator=g).cuda() * 0.1)
+        _, _, c, _ = weights.demo_inputs(cfg, N)
+        cam, intr = c[:, :16].contiguous().cuda(), c[:, 16:25].contiguous().cuda()
+        rgb = torch.zeros(N, R * R, 32, device='cuda'); depth = torch.zeros(N, R * R, device='cuda'); wsum = torch.zeros_like(depth)
+        mm = torch.tensor([float('inf'), 0.0], device='cuda')
+        normal = torch.zeros(N, R * R, 3, device='cuda')
+        work = torch.empty(K.normals_workspace_floats(N, R, opts), device='cuda')
+        plain = lambda i: K.render_rays(planes, cam, intr, R, opts, dec, rgb, depth, wsum, mm, seed=i)
+        normals = lambda i: K.render_rays_normals(planes, cam, intr, R, opts, dec, rgb, depth, wsum, mm, normal, work, seed=i)
+        for i in range(3):
+            plain(i); normals(i)
+        tp = _events(plain, 15, flush)          # alternated blocks: plain, normals, plain, normals
+        tn = _events(normals, 15, flush)
+        tp2 = _events(plain, 15, flush)
+        tn2 = _events(normals, 15, flush)
+        p_med, n_med = min(tp[0], tp2[0]), min(tn[0], tn2[0])
+        print(f'{name} N={N} r={R} D={D}+{D}: n3d_render_rays median {tp[0]:.3f} / {tp2[0]:.3f} ms, n3d_render_rays_normals median '
+              f'{tn[0]:.3f} / {tn2[0]:.3f} ms, normal pass ~{n_med - p_med:.3f} ms ({n_med / p_med:.2f}x)', flush=True)
+        # the normal pass alone on the samples the last call exported: shipped reverse mode against forward mode, alternated
+        normals(0)
+        ref = normal.clone()
+        alt = torch.zeros_like(normal)
+        rev = lambda i: K.render_normals_pass(planes, cam, intr, R, opts, dec, normal, work, forward=False)
+        fwd = lambda i: K.render_normals_pass(planes, cam, intr, R, opts, dec, alt, work, forward=True)
+        rev(0); fwd(0); torch.cuda.synchronize()
+        live = wsum > 1e-3
+        diff = (alt - ref)[live].norm(dim=-1).max().item()
+        tr, tf, tr2, tf2 = _events(rev, 15, flush), _events(fwd, 15, flush), _events(rev, 15, flush), _events(fwd, 15, flush)
+        print(f'{name} normal pass alone: reverse mode median {tr[0]:.3f} / {tr2[0]:.3f} ms, forward mode median {tf[0]:.3f} / {tf2[0]:.3f} ms '
+              f'(max |n_forward - n_reverse| {diff:.2e}); gather-only floor (n3d_render_floor kind 0, both passes) '
+              f'{_events(lambda i: K.render_floor(planes, cam, intr, R, opts, 0, seed=i), 15, flush)[0]:.3f} ms', flush=True)
+    sys.exit(0)
 N, R, D = (8, 64, 48) if which == 'c2' else (16, 128, 96)
 opts = dict(cfg.rendering_kwargs, depth_resolution=D, depth_resolution_importance=D)
 g = torch.Generator().manual_seed(0)
