@@ -246,7 +246,7 @@ typedef struct {
     const float* cam2world;    /* [N,16] */
     const float* intrinsics;   /* [N,9]  */
     int32_t res;               /* rays = res*res per sample */
-    int32_t depth_coarse, depth_fine;
+    int32_t depth_coarse, depth_fine;  /* samples per pass: 4 .. 192 coarse, 0 (coarse only) .. 192 fine; above 192 -> N3D_ERR_UNSUPPORTED */
     float ray_start, ray_end, box_warp;
     const float* u_coarse;     /* [N, M, Dc] injected uniforms or NULL (= in-kernel counter RNG with `seed`) */
     const float* u_fine;       /* [N*M, Df] or NULL */
@@ -277,7 +277,8 @@ int n3d_render_normals_pass(const N3DRender* p, int forward, const float* worksp
  * (only planes / cameras / res / depth_* / ray_* / box_warp are read; nothing is written but sink[0], which may be NULL):
  * kind 0 = the tri-plane gather alone (rays, depths, 12 taps per sample, 256-bit loads, weighted sum, bf16 split, shared-memory
  * tile) on all warps; kind 1 = the decoder's activations alone (192 MUFU operations per sample).  bench.py times them next to
- * n3d_render_rays to report how far the fused kernel is from what a per-sample gather + MLP can reach (DESIGN.md section 3.2). */
+ * n3d_render_rays to report how far the fused kernel is from what a per-sample gather + MLP can reach (DESIGN.md section 3.2).
+ * Up to 96 samples per pass (the 16- and 32-lane layouts). */
 int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream);
 /* composite depth clamp to the batch-global depth range (ray_marcher.py:53-54). */
 int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* stream);

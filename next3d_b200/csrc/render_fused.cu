@@ -12,10 +12,12 @@
 //   warps  8-15  G ("gather")   : build the layer-1 A operand in shared memory; work item = 32 rows (a quarter) of a tile, items
 //                dealt round-robin to the eight warps; 12 bilinear taps per sample fetched as 128-bit loads, 8 lanes x 4
 //                channels per sample.
-// Work unit: a GROUP = 128/L rays (a 4x2 or 2x2 pixel block) x L lanes each, L = 16 (<= 48 samples per pass) or 32 (<= 96).
-// A pass of a group is T = ceil(D / L) <= 3 tiles of 128 rows; row = ray_slot * L + j holds sample k = tile * L + j of that ray,
-// so a ray's samples always sit in the same L lanes of the same warp and every per-ray phase (transmittance scan, PDF/CDF,
-// inverse-CDF sampling, rank merge, weighted colour sum) runs on registers + warp shuffles, no CTA-wide barrier anywhere.
+// Work unit: a GROUP = 128/L rays (a 4x2, 2x2 or 1x2 pixel block) x L lanes each, L = 16 (<= 48 samples per pass), 32 (<= 96)
+// or 64 (<= 192).  A pass of a group is T = ceil(D / L) <= 3 tiles of 128 rows; row = ray_slot * L + j holds sample k = tile * L + j
+// of that ray, so a ray's samples always sit in the same L lanes and every per-ray phase (transmittance scan, PDF/CDF,
+// inverse-CDF sampling, rank merge, weighted colour sum) runs on registers + warp shuffles, no CTA-wide barrier anywhere.  At
+// L = 64 a ray spans the two warps 2r, 2r + 1 of one E set; the steps that cross the warp boundary (scan carries, sums, the
+// neighbour sample, the merge's bucket prefix) exchange a few words through shared memory under a 64-thread named barrier.
 // Tile stream of a CTA: C(0) | C(1) F(0) | C(2) F(1) | ...  (coarse tiles of group r+1 are issued before the fine tiles of
 // group r, so the importance sampling of a group never stalls the gather warps).
 //
@@ -258,6 +260,116 @@ __device__ __forceinline__ void march_weights(const float (&d)[NT], const float 
     }
 }
 
+// ---- L = 64: the same steps for a ray held by a warp pair, half h = warp & 1 holding j = 32 h + lane.  Every exchange writes one of
+// two ping-pong buffers and passes the pair's barrier once; a buffer is rewritten only after the partner has passed the next
+// barrier, i.e. after it read the buffer's previous contents.
+struct Pair {
+    float* x;                    // 2 x 32 exchange words in the pair's scratch
+    int bar, h, ph;              // named barrier id (5 .. 8), warp half, current buffer
+};
+__device__ __forceinline__ void pair_sync(const Pair& X) { asm volatile("bar.sync %0, 64;" ::"r"(X.bar) : "memory"); }
+__device__ __forceinline__ float* pair_buf(Pair& X) {
+    float* const b = X.x + 32 * X.ph;
+    X.ph ^= 1;
+    return b;
+}
+__device__ __forceinline__ bool pair_any(const Pair& X, bool p) {
+    int r;
+    asm volatile("{\n\t.reg .pred a, b;\n\tsetp.ne.s32 a, %1, 0;\n\tbar.red.or.pred b, %2, 64, a;\n\tselp.s32 %0, 1, 0, b;\n\t}"
+                 : "=r"(r) : "r"((int)p), "r"(X.bar) : "memory");
+    return r != 0;
+}
+__device__ __forceinline__ float pair_sum(Pair& X, float v, int lane) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+    float* const b = pair_buf(X);
+    if (lane == 0) b[X.h] = v;
+    pair_sync(X);
+    return b[0] + b[1];                                              // same order in both halves: both get the same bits
+}
+// out[t] = value of sample k + 1 (`last` after the final slot)
+template <int NT>
+__device__ __forceinline__ void pair_next(Pair& X, const float (&v)[NT], float last, float (&out)[NT], int lane) {
+    float* const b = pair_buf(X);
+    if (lane == 0) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = X.h ? v[t] : (t + 1 < NT ? v[t + 1] : last);
+    }
+    pair_sync(X);
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+        const float a = __shfl_down_sync(FULL, v[t], 1);
+        out[t] = lane == 31 ? b[8 * (X.h ^ 1) + t] : a;
+    }
+}
+// out[t] = value of sample k - 1 (`first` before sample 0)
+template <int NT>
+__device__ __forceinline__ void pair_prev(Pair& X, const float (&v)[NT], float first, float (&out)[NT], int lane) {
+    float* const b = pair_buf(X);
+    if (lane == 31) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = X.h ? (t > 0 ? v[t - 1] : first) : v[t];
+    }
+    pair_sync(X);
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+        const float a = __shfl_up_sync(FULL, v[t], 1);
+        out[t] = lane == 0 ? b[8 * (X.h ^ 1) + t] : a;
+    }
+}
+template <int NT, bool MUL>
+__device__ __forceinline__ void pair_scan(Pair& X, float (&x)[NT], int lane) {                 // inclusive scan in sample order
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+        float v = x[t];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const float up = __shfl_up_sync(FULL, v, o);
+            if (lane >= o) v = MUL ? v * up : v + up;
+        }
+        x[t] = v;
+    }
+    float* const b = pair_buf(X);
+    if (lane == 31) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = x[t];
+    }
+    pair_sync(X);
+    float carry = MUL ? 1.f : 0.f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+        const float c1 = MUL ? carry * b[t] : carry + b[t];          // carry into half 1 of slot t
+        x[t] = MUL ? x[t] * (X.h ? c1 : carry) : x[t] + (X.h ? c1 : carry);
+        carry = MUL ? c1 * b[8 + t] : c1 + b[8 + t];
+    }
+}
+template <int NT>
+__device__ __forceinline__ void march_weights_pair(Pair& X, const float (&d)[NT], const float (&sg)[NT], int cnt, int lane, float (&w)[NT],
+                                                   float (&tmid)[NT]) {
+    const int j = 32 * X.h + lane;
+    float dn[NT], sn[NT], fac[NT], al[NT];
+    pair_next<NT>(X, d, 0.f, dn, lane);
+    pair_next<NT>(X, sg, 0.f, sn, lane);
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+        const int k = t * 64 + j;
+        float alpha = 0.f;
+        if (k < cnt - 1) {
+            const float xx = softplus_fast((sg[t] + sn[t]) * 0.5f - 1.f) * (dn[t] - d[t]);
+            const float ser = xx * (1.f - xx * (0.5f - xx * (0.16666667f - xx * (0.041666668f - xx * 0.0083333338f))));
+            alpha = xx < 0.0625f ? ser : 1.f - ex2_approx(-kLog2e * xx);             // as march_weights
+        }
+        al[t] = alpha;
+        fac[t] = k < cnt - 1 ? (1.f - alpha + 1e-10f) : 1.f;
+        tmid[t] = (d[t] + dn[t]) * 0.5f;
+    }
+    pair_scan<NT, true>(X, fac, lane);
+    float ex[NT];
+    pair_prev<NT>(X, fac, 1.f, ex, lane);
+#pragma unroll
+    for (int t = 0; t < NT; ++t) w[t] = al[t] * ((t == 0 && j == 0) ? 1.f : ex[t]);
+}
+
 // Tile stream of a CTA with n groups: C(0) | C(1) F(0) | ... | C(n-1) F(n-2) | F(n-1); every role walks it with the same iterator.
 struct TileIter {
     int n, Tc, Tf;
@@ -450,7 +562,7 @@ __device__ __forceinline__ void init_pipeline_barriers(const Smem& S) {
 template <int L, bool kExport>
 __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_constant__ FusedK K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    constexpr int RPW = 32 / L;                 // rays per warp
+    constexpr int RPW = L == 64 ? 1 : 32 / L;   // rays per scratch area (L = 64: one ray per warp pair, the pair's two areas)
     const N3DRender& P = K.p;
     Smem S;
     S.base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);       // pointer arithmetic keeps the shared address space
@@ -518,18 +630,23 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
     else {
         const int eset = warp >> 2, q = warp & 3;
         const int row = q * 32 + lane, rs = row / L, j = row & (L - 1), rw = lane / L;
-        float* const es = reinterpret_cast<float*>(sb + kOffEscr) + warp * kEscrFloats;
+        float* const es = reinterpret_cast<float*>(sb + kOffEscr) + (L == 64 ? (warp & ~1) : warp) * kEscrFloats;
         // per-warp scratch (floats): region A [0, 640) = sd | sg | wb (RPW x (Dt + 2) each), aliased by the cdf during importance sampling
-        // and by the u-bucket tables during ranking; tcs at 640 (RPW x Dc), tfs at 736 (RPW x Df), hist at 832 (RPW x (Dc + 1))
+        // and by the u-bucket tables during ranking; tcs at 640 (RPW x Dc), tfs at 736 (RPW x Df), hist at 832 (RPW x (Dc + 1)).
+        // L = 64, the pair's 1920 floats: region A [0, 1160) (3 x 386; 2 x 512 bucket words), tcs at 1160, tfs at 1352, hist at
+        // 1544 (193), the pair's exchange words at 1752 (2 x 32).
+        constexpr int kTcOff = L == 64 ? 1160 : 640, kTfOff = L == 64 ? 1352 : 736, kHistOff = L == 64 ? 1544 : 832;
         constexpr int NB = 8 * L;                                   // u-buckets per ray (8 per lane)
         const int strD = Dt + 2;
         float* const s_sd = es + rw * strD;                         // sorted depths
         float* const s_sg = es + RPW * strD + rw * strD;
         float* const s_wb = es + 2 * RPW * strD + rw * strD;
         int* const s_ub = reinterpret_cast<int*>(es) + rw * 2 * NB; // [NB] count | prefix << 8, then [NB] member indices (4 bytes)
-        float* const s_tc = es + 640 + rw * Dc;
-        float* const s_tf = es + 736 + rw * Df;
-        int* const s_hist = reinterpret_cast<int*>(es + 832) + rw * (Dc + 1);
+        float* const s_tc = es + kTcOff + rw * Dc;
+        float* const s_tf = es + kTfOff + rw * Df;
+        int* const s_hist = reinterpret_cast<int*>(es + kHistOff) + rw * (Dc + 1);
+        Pair X;                                                     // L = 64 only
+        X.x = es + 1752; X.bar = 5 + (warp >> 1); X.h = warp & 1; X.ph = 0;
 
         // state of the group in its fine phase (cur) and of the group in its coarse phase (nxt)
         float cur_tc[kMaxT], cur_sc[kMaxT], cur_tf[kMaxT], cur_sf[kMaxT];
@@ -572,23 +689,36 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
         // ---- coarse weights -> smoothed pdf -> cdf -> inverse-CDF fine depths (renderer.py:209-268) for the group in `nxt`
         auto importance = [&](int r) {
             float w[kMaxT], tm[kMaxT];
-            march_weights<L, kMaxT>(nxt_tc, nxt_sc, Dc, lane, w, tm);
+            if constexpr (L == 64) {
+                pair_sync(X);                                       // the partner is done with the scratch of its previous phase
+                march_weights_pair<kMaxT>(X, nxt_tc, nxt_sc, Dc, lane, w, tm);
+            } else {
+                march_weights<L, kMaxT>(nxt_tc, nxt_sc, Dc, lane, w, tm);
+            }
             // max_pool1d(k2,s1,pad1) -> avg_pool1d(k2,s1) -> + 0.01; entries [1:-1] => pdf weights at k = 1 .. Dc-3, + 1e-5
             const int nw = Dc - 3;
             float c[kMaxT];
             float part = 0.f;
+            float wpv[kMaxT], wnv[kMaxT];
+            if constexpr (L == 64) {
+                pair_prev<kMaxT>(X, w, 0.f, wpv, lane);
+                pair_next<kMaxT>(X, w, 0.f, wnv, lane);
+            }
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) {
-                const float wp = seg_prev<L>(w[t], t > 0 ? w[t - 1] : 0.f, lane);
-                const float wn = seg_next<L>(w[t], t + 1 < kMaxT ? w[t + 1] : 0.f, lane);
+                const float wp = L == 64 ? wpv[t] : seg_prev<L>(w[t], t > 0 ? w[t - 1] : 0.f, lane);
+                const float wn = L == 64 ? wnv[t] : seg_next<L>(w[t], t + 1 < kMaxT ? w[t + 1] : 0.f, lane);
                 const int k = t * L + j;
                 c[t] = (k >= 1 && k <= nw) ? (fmaxf(wp, w[t]) + fmaxf(w[t], wn)) * 0.5f + 0.01f + 1e-5f : 0.f;
                 part += c[t];
             }
-            const float total = seg_sum<L>(part);
+            float total;
+            if constexpr (L == 64) total = pair_sum(X, part, lane);
+            else total = seg_sum<L>(part);
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) c[t] = c[t] / total;
-            seg_scan<L, kMaxT, false>(c, lane);                     // c[t] = cdf[k], k = 0 .. nw
+            if constexpr (L == 64) pair_scan<kMaxT, false>(X, c, lane);
+            else seg_scan<L, kMaxT, false>(c, lane);                // c[t] = cdf[k], k = 0 .. nw
             float* const cdf = s_sd;
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) {
@@ -596,7 +726,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 if (k <= nw) cdf[k] = c[t];
                 if (k < Dc) s_tc[k] = nxt_tc[t];
             }
-            __syncwarp();
+            if constexpr (L == 64) pair_sync(X);
+            else __syncwarp();
             float uu[kMaxT];
             int lo[kMaxT], hi[kMaxT];
 #pragma unroll
@@ -645,6 +776,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             float coef_c[kMaxT], coef_f[kMaxT];
             float wsum, dacc;
             float d_first, d_last;
+            // L = 64: the ray's two warps meet at every point where the L <= 32 code needs only its own warp
+            auto ray_sync = [&]() {
+                if constexpr (L == 64) pair_sync(X);
+                else __syncwarp();
+            };
+            if constexpr (L == 64) pair_sync(X);                    // the partner is done with the scratch of its previous phase
             if (use_fine) {
                 // stable sort-merge of coarse (sorted) + fine depths by rank (torch.sort of the concatenation, renderer.py:164-182)
 #pragma unroll
@@ -655,10 +792,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     if (k <= Dc) s_hist[k] = 0;
                 }
                 if (j == 0 && L * kMaxT <= Dc) s_hist[Dc] = 0;
-                __syncwarp();
+                ray_sync();
                 // zero the u-bucket tables (they alias the sorted arrays, which are written after the ranks are known)
                 for (int i = j; i < 2 * NB; i += L) s_ub[i] = 0;
-                __syncwarp();
+                ray_sync();
                 // Rank of a fine sample among the fine ones.  Fine depths are the inverse CDF of iid uniforms u, a monotone map, so the
                 // order of the depths is the order of the u's: bucket the samples by u (NB uniform buckets, ~0.4 samples each), take
                 // the bucket prefix count and order the few members of a bucket by (depth, index).  The number of coarse samples <= v
@@ -685,19 +822,25 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         atomicAdd(&s_hist[c], 1);
                     }
                 }
-                __syncwarp();
+                ray_sync();
                 {   // exclusive prefix over the buckets: lane j owns buckets 8j .. 8j+7; count and prefix share a word
                     int cn[8], run = 0;
 #pragma unroll
                     for (int i = 0; i < 8; ++i) { cn[i] = s_ub[8 * j + i]; run += cn[i]; }
                     int inc = run;
+                    if constexpr (L == 64) {                        // counts <= 192: exact in fp32
+                        float f[1] = {(float)run};
+                        pair_scan<1, false>(X, f, lane);
+                        inc = (int)f[0];
+                    } else {
 #pragma unroll
-                    for (int o = 1; o < L; o <<= 1) { const int up = __shfl_up_sync(FULL, inc, o); if (j >= o) inc += up; }
+                        for (int o = 1; o < L; o <<= 1) { const int up = __shfl_up_sync(FULL, inc, o); if (j >= o) inc += up; }
+                    }
                     int pre = inc - run;
 #pragma unroll
                     for (int i = 0; i < 8; ++i) { s_ub[8 * j + i] = cn[i] | (pre << 8); pre += cn[i]; }
                 }
-                __syncwarp();
+                ray_sync();
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
                     const int jf = t * L + j;
@@ -719,7 +862,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         pos_f[t] = cntc[t] + (word >> 8) + within;
                     }
                 }
-                if (__any_sync(FULL, overflow)) {                    // a crowded bucket (degenerate u's): full O(Df^2) rank count
+                bool crowded;
+                if constexpr (L == 64) crowded = pair_any(X, overflow);
+                else crowded = __any_sync(FULL, overflow);
+                if (crowded) {                                       // a crowded bucket (degenerate u's): full O(Df^2) rank count
 #pragma unroll
                     for (int t = 0; t < kMaxT; ++t) {
                         const int jf = t * L + j;
@@ -731,12 +877,13 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         }
                     }
                 }
-                __syncwarp();
+                ray_sync();
                 // coarse sample a lands after every fine sample with fewer than a+1 coarse samples <= it: a + #{fine: cnt_c <= a}
                 float hc[kMaxT];
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { const int k = t * L + j; hc[t] = k < Dc ? (float)s_hist[k] : 0.f; }
-                seg_scan<L, kMaxT, false>(hc, lane);
+                if constexpr (L == 64) pair_scan<kMaxT, false>(X, hc, lane);
+                else seg_scan<L, kMaxT, false>(hc, lane);
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
                     const int k = t * L + j;
@@ -744,7 +891,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     if (k < Dc) { s_sd[pos_c[t]] = tc[t]; s_sg[pos_c[t]] = sc[t]; }
                     if (k < Df) { s_sd[pos_f[t]] = cur_tf[t]; s_sg[pos_f[t]] = cur_sf[t]; }
                 }
-                __syncwarp();
+                ray_sync();
                 float d6[2 * kMaxT], s6[2 * kMaxT], w6[2 * kMaxT], tm6[2 * kMaxT];
 #pragma unroll
                 for (int t = 0; t < 2 * kMaxT; ++t) {
@@ -752,7 +899,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     d6[t] = p < cnt ? s_sd[p] : 0.f;
                     s6[t] = p < cnt ? s_sg[p] : 0.f;
                 }
-                march_weights<L, 2 * kMaxT>(d6, s6, cnt, lane, w6, tm6);
+                if constexpr (L == 64) march_weights_pair<2 * kMaxT>(X, d6, s6, cnt, lane, w6, tm6);
+                else march_weights<L, 2 * kMaxT>(d6, s6, cnt, lane, w6, tm6);
                 if constexpr (kExport) {
                     if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
                         float* const out = K.samples + gr * (2 * cnt - 1);
@@ -773,10 +921,16 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     ws += w6[t];
                     da += w6[t] * tm6[t];
                 }
-                wsum = seg_sum<L>(ws);
-                dacc = seg_sum<L>(da);
-                d_first = __shfl_sync(FULL, d6[0], lane & ~(L - 1));
-                __syncwarp();
+                if constexpr (L == 64) {
+                    wsum = pair_sum(X, ws, lane);
+                    dacc = pair_sum(X, da, lane);
+                    d_first = d6[0];                                 // read on j == 0 only
+                } else {
+                    wsum = seg_sum<L>(ws);
+                    dacc = seg_sum<L>(da);
+                    d_first = __shfl_sync(FULL, d6[0], lane & ~(L - 1));
+                }
+                ray_sync();
                 d_last = s_sd[cnt - 1];
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
@@ -786,7 +940,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 }
             } else {
                 float w3[kMaxT], tm3[kMaxT];
-                march_weights<L, kMaxT>(tc, sc, cnt, lane, w3, tm3);
+                if constexpr (L == 64) march_weights_pair<kMaxT>(X, tc, sc, cnt, lane, w3, tm3);
+                else march_weights<L, kMaxT>(tc, sc, cnt, lane, w3, tm3);
                 if constexpr (kExport) {
                     if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
                         float* const out = K.samples + gr * (2 * cnt - 1);
@@ -801,20 +956,27 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 float ws = 0.f, da = 0.f;
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { ws += w3[t]; da += w3[t] * tm3[t]; }
-                wsum = seg_sum<L>(ws);
-                dacc = seg_sum<L>(da);
+                float wpv[kMaxT];
+                if constexpr (L == 64) {
+                    wsum = pair_sum(X, ws, lane);
+                    dacc = pair_sum(X, da, lane);
+                    pair_prev<kMaxT>(X, w3, 0.f, wpv, lane);
+                } else {
+                    wsum = seg_sum<L>(ws);
+                    dacc = seg_sum<L>(da);
+                }
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
-                    const float wp = seg_prev<L>(w3[t], t > 0 ? w3[t - 1] : 0.f, lane);
+                    const float wp = L == 64 ? wpv[t] : seg_prev<L>(w3[t], t > 0 ? w3[t - 1] : 0.f, lane);
                     const int k = t * L + j;
                     coef_c[t] = k < Dc ? 0.5f * ((k > 0 ? wp : 0.f) + w3[t]) : 0.f;
                     coef_f[t] = 0.f;
                 }
-                d_first = __shfl_sync(FULL, tc[0], lane & ~(L - 1));
+                d_first = L == 64 ? tc[0] : __shfl_sync(FULL, tc[0], lane & ~(L - 1));     // read on j == 0 only
                 if (j == 0) s_wb[0] = 0.f;                          // keep the scratch race-free across phases
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { const int k = t * L + j; if (k < Dc) s_sd[k] = tc[t]; }
-                __syncwarp();
+                ray_sync();
                 d_last = s_sd[Dc - 1];
             }
             // colours: acc[c] += coef * sigmoid(logit + b1) over this thread's rows, channels 16*eset .. +15 (sigmoid * 1.002 - 0.001,
@@ -841,7 +1003,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     if (t < Tf) add_tile(6 + t, coef_f[t]);
             }
             // segment reduce-scatter: lane j ends with channel (j & 15) summed over the L lanes
-            if (L == 32) {
+            if (L >= 32) {
 #pragma unroll
                 for (int c = 0; c < 16; ++c) acc[c] += __shfl_xor_sync(FULL, acc[c], 16);
             }
@@ -854,6 +1016,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     const float keep = up ? acc[c + h] : acc[c];
                     acc[c] = keep + __shfl_xor_sync(FULL, send, h);
                 }
+            }
+            if constexpr (L == 64) {                                // half 1's channel sums join half 0's (j = lane < 16)
+                float* const b = pair_buf(X);
+                if (X.h == 1 && lane < 16) b[lane] = acc[0];
+                pair_sync(X);
+                if (X.h == 0 && lane < 16) acc[0] += b[lane];
             }
             if (ok && j < 16) {
                 float v = fmaf(acc[0], 1.002f, -0.001f * wsum);     // sum_k coef_k (1.002 sigmoid_k - 0.001), sum_k coef_k = wsum
@@ -1473,13 +1641,14 @@ __global__ void __launch_bounds__(256) depth_clamp_kernel(float* __restrict__ de
     }
 }
 
-constexpr int kMaxD = kMaxT * 32;               // depth samples per pass the fused kernel lays out (3 tiles x 32 lanes per ray)
+constexpr int kMaxD = kMaxT * 64;               // depth samples per pass the fused kernel lays out (3 tiles x 64 lanes per ray)
+constexpr int kMaxDFloor = kMaxT * 32;          // the floor micro-kernels know the 16- and 32-lane layouts only
 
 // Work decomposition of the renderer and of the floor micro-kernels for the workload p; L = lanes per ray (16 up to 48 samples
-// per pass, else 32).
+// per pass, 32 up to 96, else 64).
 FusedK make_fused(const N3DRender* p, int& L) {
     const int dmax = p->depth_coarse > p->depth_fine ? p->depth_coarse : p->depth_fine;
-    L = dmax <= 48 ? 16 : 32;
+    L = dmax <= 48 ? 16 : dmax <= 96 ? 32 : 64;
     FusedK K;
     K.p = *p;
     K.M = p->res * p->res;
@@ -1487,8 +1656,8 @@ FusedK make_fused(const N3DRender* p, int& L) {
     K.scale = 2.f / p->box_warp;
     K.Tc = (p->depth_coarse + L - 1) / L;
     K.Tf = (p->depth_fine + L - 1) / L;
-    K.gw = L == 16 ? 4 : 2;
-    K.log2gw = L == 16 ? 2 : 1;
+    K.gw = 64 / L;                                  // pixel block of a group: 4 x 2, 2 x 2 or 1 x 2
+    K.log2gw = L == 16 ? 2 : L == 32 ? 1 : 0;
     const int tiles_x = (p->res + K.gw - 1) / K.gw, tiles_y = (p->res + 1) / 2;
     K.blocks_x = (tiles_x + 3) / 4;
     K.gpi = K.blocks_x * ((tiles_y + 7) / 8) * 32;
@@ -1549,13 +1718,15 @@ int launch_render(const N3DRender* p, float* samples, const char* who, void* str
     FusedK K = make_fused(p, L);
     K.samples = samples;
     const int smem = kSmemBytes + 1024;
-    if (int rc = n3d_smem_optin(L == 16 ? (const void*)render_fused_kernel<16, kExport> : (const void*)render_fused_kernel<32, kExport>, smem, who))
-        return rc;
+    const void* const fn = L == 16 ? (const void*)render_fused_kernel<16, kExport>
+                         : L == 32 ? (const void*)render_fused_kernel<32, kExport> : (const void*)render_fused_kernel<64, kExport>;
+    if (int rc = n3d_smem_optin(fn, smem, who)) return rc;
     const N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
     const int grid = (int)(K.total_groups < D->num_sms ? K.total_groups : D->num_sms);
     if (L == 16) render_fused_kernel<16, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
-    else render_fused_kernel<32, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    else if (L == 32) render_fused_kernel<32, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
+    else render_fused_kernel<64, kExport><<<grid, kThreads, smem, (cudaStream_t)stream>>>(K);
     N3D_CHECK_LAUNCH(who);
     return N3D_OK;
 }
@@ -1605,7 +1776,8 @@ extern "C" int n3d_render_normals_pass(const N3DRender* p, int forward, const fl
 
 extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream) {
     N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && (kind == 0 || kind == 1), "n3d_render_floor: bad args");
-    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_coarse <= kMaxD && p->depth_fine >= 0 && p->depth_fine <= kMaxD, "n3d_render_floor: depth resolutions");
+    N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_coarse <= kMaxDFloor && p->depth_fine >= 0 && p->depth_fine <= kMaxDFloor,
+                  "n3d_render_floor: depth resolutions");
     int L;
     const FusedK K = make_fused(p, L);
     const N3DDeviceState* D = n3d_device_state();

@@ -239,7 +239,9 @@ def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth,
 
 def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
                 seed_ptr=None):
-    """planes [N,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in."""
+    """planes [N,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in.
+    opts['depth_resolution'] (4 .. 192) and opts['depth_resolution_importance'] (0 = coarse only .. 192) are samples per pass; a
+    count above 192 raises (code -2, unsupported)."""
     p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
     _run('n3d_render_rays', C.byref(p), stream_ptr())
 
@@ -254,7 +256,7 @@ def render_rays_normals(planes, cam2world, intrinsics, res, opts, dec, rgb, dept
                         u_fine=None, seed=0, seed_ptr=None):
     """render_rays (same outputs, bit for bit) plus normal [N, M, 3]: unit world-space normals -grad sigma composited with the final
     weights (rendering option return_normal).  workspace: fp32 device buffer of normals_workspace_floats() floats, or None to
-    allocate one here."""
+    allocate one here.  Same sample-count limits as render_rays (up to 192 + 192)."""
     p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
     n_ws = normals_workspace_floats(planes.shape[0], res, opts)
     if workspace is None:
