@@ -259,6 +259,9 @@ typedef struct {
     float* wsum;               /* [N, M] */
     float* depth_minmax;       /* [2] device: running min / max of all sample depths (init +inf / -inf by caller) */
     int32_t white_back;
+    int32_t views;             /* camera views per plane set: 0 or 1 = image n reads plane set n; V >= 2 = image n reads plane set
+                                  n / V, so `planes` holds N / V sets (N a multiple of V).  Cameras, uniforms, outputs and depth_minmax
+                                  stay per image. */
 } N3DRender;
 
 int n3d_render_rays(const N3DRender* p, void* stream);
@@ -278,7 +281,7 @@ int n3d_render_normals_pass(const N3DRender* p, int forward, const float* worksp
  * kind 0 = the tri-plane gather alone (rays, depths, 12 taps per sample, 256-bit loads, weighted sum, bf16 split, shared-memory
  * tile) on all warps; kind 1 = the decoder's activations alone (192 MUFU operations per sample).  bench.py times them next to
  * n3d_render_rays to report how far the fused kernel is from what a per-sample gather + MLP can reach (DESIGN.md section 3.2).
- * Up to 96 samples per pass (the 16- and 32-lane layouts). */
+ * Up to 96 samples per pass (the 16- and 32-lane layouts); `views` is honoured and checked as in n3d_render_rays. */
 int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream);
 /* composite depth clamp to the batch-global depth range (ray_marcher.py:53-54). */
 int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* stream);

@@ -58,7 +58,7 @@ class Render(C.Structure):
         ('ray_start', F32), ('ray_end', F32), ('box_warp', F32),
         ('u_coarse', P), ('u_fine', P), ('seed', C.c_uint64), ('seed_ptr', P),
         ('w0', P), ('b0', P), ('w1', P), ('b1', P),
-        ('rgb', P), ('depth', P), ('wsum', P), ('depth_minmax', P), ('white_back', I32),
+        ('rgb', P), ('depth', P), ('wsum', P), ('depth_minmax', P), ('white_back', I32), ('views', I32),
     ]
 
 

@@ -105,7 +105,7 @@ __device__ __forceinline__ Ray make_ray(const FusedK& K, int gg, int rs) {
     Ray r;
     r.ok = id.ok;
     r.gr = id.gr;
-    r.img4 = (uint32_t)id.n * (uint32_t)(3 * P.PH * P.PW * 128);       // byte offset of the image's planes
+    r.img4 = (uint32_t)(id.n / P.views) * (uint32_t)(3 * P.PH * P.PW * 128);       // byte offset of the image's plane set
     r.ox = r.oy = r.oz = r.dx = r.dy = r.dz = 0.f;
     if (id.ok) {
         float o[3], d[3];
@@ -1407,7 +1407,7 @@ __global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __gri
         const int n = (int)(gr / M), m = (int)(gr - (long long)n * M);
         float o[3], d[3];
         camera_ray(P, n, m / P.res, m % P.res, o, d);
-        const uint32_t img4 = (uint32_t)n * (uint32_t)(3 * P.PH * P.PW * 128);
+        const uint32_t img4 = (uint32_t)(n / P.views) * (uint32_t)(3 * P.PH * P.PW * 128);
         const float* const ts = K.samples + gr * (2 * D - 1);
         const float* const wts = ts + D;
         float nacc[3] = {0.f, 0.f, 0.f}, wsum = 0.f;
@@ -1644,6 +1644,15 @@ __global__ void __launch_bounds__(256) depth_clamp_kernel(float* __restrict__ de
 constexpr int kMaxD = kMaxT * 64;               // depth samples per pass the fused kernel lays out (3 tiles x 64 lanes per ray)
 constexpr int kMaxDFloor = kMaxT * 32;          // the floor micro-kernels know the 16- and 32-lane layouts only
 
+// Images per plane set (N3DRender::views, 0 read as 1): the kernels divide the image index by it.
+int plane_views(const N3DRender* p) { return p->views > 1 ? p->views : 1; }
+
+// views >= 0 and N a multiple of it; messages start with `who`.
+int check_views(const N3DRender* p, const char* who) {
+    N3D_CHECK_ARG(p->views >= 0 && p->N % plane_views(p) == 0, "%s: views = %d must be >= 0 and divide N = %d", who, p->views, p->N);
+    return N3D_OK;
+}
+
 // Work decomposition of the renderer and of the floor micro-kernels for the workload p; L = lanes per ray (16 up to 48 samples
 // per pass, 32 up to 96, else 64).
 FusedK make_fused(const N3DRender* p, int& L) {
@@ -1651,6 +1660,7 @@ FusedK make_fused(const N3DRender* p, int& L) {
     L = dmax <= 48 ? 16 : dmax <= 96 ? 32 : 64;
     FusedK K;
     K.p = *p;
+    K.p.views = plane_views(p);
     K.M = p->res * p->res;
     K.delta_coarse = (float)(((double)p->ray_end - (double)p->ray_start) / (double)(p->depth_coarse - 1));
     K.scale = 2.f / p->box_warp;
@@ -1706,8 +1716,10 @@ int check_render(const N3DRender* p, const char* who) {
     }
     N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_fine >= 0, "%s: depth resolutions (%d, %d): need coarse >= 4, fine >= 0", who,
                   p->depth_coarse, p->depth_fine);
+    if (int rc = check_views(p, who)) return rc;
+    N3D_CHECK_ARG((long long)(p->N / plane_views(p)) * 3 * p->PH * p->PW * 128 < (1ll << 32), "%s: plane tensor too large for 32-bit texel offsets",
+                  who);
     N3D_CHECK_ARG(p->res >= 1 && p->N >= 1 && p->ray_start > 0.f && p->ray_end > p->ray_start && p->box_warp > 0.f, "%s: bad ray setup", who);
-    N3D_CHECK_ARG((long long)p->N * 3 * p->PH * p->PW * 128 < (1ll << 32), "%s: plane tensor too large for 32-bit texel offsets", who);
     return N3D_OK;
 }
 
@@ -1743,6 +1755,7 @@ template <bool kForward>
 int launch_normals(const N3DRender* p, const float* workspace, float* normal, const char* who, void* stream) {
     NormalsK K;
     K.p = *p;
+    K.p.views = plane_views(p);
     K.D = p->depth_fine > 0 ? p->depth_coarse + p->depth_fine : p->depth_coarse;
     K.scale = 2.f / p->box_warp;
     K.rays = (long long)p->N * p->res * p->res;
@@ -1778,6 +1791,7 @@ extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void*
     N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && (kind == 0 || kind == 1), "n3d_render_floor: bad args");
     N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_coarse <= kMaxDFloor && p->depth_fine >= 0 && p->depth_fine <= kMaxDFloor,
                   "n3d_render_floor: depth resolutions");
+    if (int rc = check_views(p, "n3d_render_floor")) return rc;
     int L;
     const FusedK K = make_fused(p, L);
     const N3DDeviceState* D = n3d_device_state();

@@ -53,12 +53,67 @@ def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_
     sampler's RNG (batch k uses seed + k); None = a fresh random seed per call, like the reference's torch.rand.
     `sampler_noise=(u_coarse [F, M, Dc, 1], u_fine [F, M, Df])`: per-frame sampler uniforms instead of the in-kernel RNG (parity tests:
     frame f gets the same noise whichever batch slot it lands in)."""
+    yield from _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, False)
+
+
+def render_orbit(G, ws, cams, verts, batch=8, image_mode='image', seed=None, sampler_noise=None):
+    """Yield one uint8 HWC numpy frame per camera of cams [F, 25] for ONE head: ws [1, L, D] and mesh verts [1, V, 3] stay fixed
+    (gen_videos_next3d.py with one seed, sample sheets), so the tri-planes are computed once (noise_mode 'const') and every batch of
+    `batch` cameras is rendered from them by G.render_views -- volume rendering and super-resolution only.  Padding, `seed` and
+    `sampler_noise` as in render_frames."""
+    device = next(G.parameters()).device
+    G.synthesis(ws.to(device, torch.float32), cams[:1].to(device, torch.float32), verts.to(device, torch.float32), noise_mode='const',
+                cache_backbone=True, seed=0)
+
+    def outputs():
+        for idx, n, kw in _batches(cams.shape[0], batch, seed, sampler_noise):
+            yield G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **kw), n
+    yield from _frames(outputs(), image_mode, device)
+
+
+def _batches(F, batch, seed, sampler_noise):
+    """(frame indices, valid count, sampler keywords) of each batch of `batch` frames; the last batch is padded by repeating its final
+    frame (one graph shape).  Batch k gets sampler seed `seed` + k, or its frames' rows of `sampler_noise`."""
+    for b0 in range(0, F, batch):
+        n = min(batch, F - b0)
+        idx = list(range(b0, b0 + n)) + [b0 + n - 1] * (batch - n)
+        kw = {} if seed is None else {'seed': int(seed) + b0 // batch}
+        if sampler_noise is not None:
+            u_c, u_f = sampler_noise
+            kw['sampler_noise'] = (u_c[idx], u_f[idx].reshape(-1, u_f.shape[-1]))
+        yield idx, n, kw
+
+
+def _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, reuse_backbone):
+    """render_frames.  reuse_backbone: every frame has the same ws (one identity), so the first batch caches the ws-only backbones
+    and the later ones reuse them (use_cached_backbone); with noise_mode 'const' or 'none' those are a function of ws alone, so the
+    frames are the same."""
     device = device or next(G.parameters()).device
-    F = ws_frames.shape[0]
-    cuda = torch.device(device).type == 'cuda'
     vit = None
     if not torch.is_tensor(verts):
         vit = iter(verts)
+
+    def outputs():
+        for k, (idx, n, kw) in enumerate(_batches(ws_frames.shape[0], batch, seed, sampler_noise)):
+            w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
+            c = cams[idx].to(device, torch.float32, non_blocking=True)
+            if vit is not None:
+                vs = [next(vit) for _ in range(n)]
+                v = torch.cat(vs + [vs[-1]] * (batch - n), 0).to(device, torch.float32, non_blocking=True)
+            elif verts.shape[0] == 1:
+                v = verts.to(device, torch.float32).expand(batch, -1, -1)
+            else:
+                v = verts[idx].to(device, torch.float32, non_blocking=True)
+            if reuse_backbone:
+                kw['use_cached_backbone' if k else 'cache_backbone'] = True
+            yield G.synthesis(w, c, v, noise_mode=noise_mode, **kw), n
+    yield from _frames(outputs(), image_mode, device)
+
+
+def _frames(outputs, image_mode, device):
+    """uint8 HWC numpy frames of successive batches, in order; `outputs` yields (generator output dict, valid count) per batch.  The
+    conversion runs on the device, and the device->host copy of batch i overlaps the rendering of batch i+1."""
+    cuda = torch.device(device).type == 'cuda'
     copy_s = torch.cuda.Stream(device) if cuda else None
     pending = None                                               # (host tensor, event, valid count) of the previous batch
 
@@ -69,23 +124,8 @@ def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_
         for k in range(n):
             yield host[k].numpy()
 
-    for b0 in range(0, F, batch):
-        n = min(batch, F - b0)
-        idx = list(range(b0, b0 + n)) + [b0 + n - 1] * (batch - n)
-        w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
-        c = cams[idx].to(device, torch.float32, non_blocking=True)
-        if vit is not None:
-            vs = [next(vit) for _ in range(n)]
-            v = torch.cat(vs + [vs[-1]] * (batch - n), 0).to(device, torch.float32, non_blocking=True)
-        elif verts.shape[0] == 1:
-            v = verts.to(device, torch.float32).expand(batch, -1, -1)
-        else:
-            v = verts[idx].to(device, torch.float32, non_blocking=True)
-        kw = {} if seed is None else {'seed': int(seed) + b0 // batch}
-        if sampler_noise is not None:
-            u_c, u_f = sampler_noise
-            kw['sampler_noise'] = (u_c[idx], u_f[idx].reshape(-1, u_f.shape[-1]))
-        img = G.synthesis(w, c, v, noise_mode=noise_mode, **kw)[image_mode]
+    for out, n in outputs:
+        img = out[image_mode]
         if image_mode == 'image_depth':                          # gen_videos_next3d.py:160-162, per frame
             img = -img
             lo, hi = img.amin(dim=(1, 2, 3), keepdim=True), img.amax(dim=(1, 2, 3), keepdim=True)
@@ -149,7 +189,7 @@ def reenact_frames(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_
     if n == 0:
         return
     wsf = ws.detach().cpu().float().reshape(1, *ws.shape[-2:]).expand(n, -1, -1)
-    yield from render_frames(G, wsf, cams, verts, batch=batch, noise_mode=noise_mode, seed=seed, sampler_noise=sampler_noise)
+    yield from _render_frames(G, wsf, cams, verts, batch, 'image', noise_mode, None, seed, sampler_noise, noise_mode in ('const', 'none'))
 
 
 def interpolate_ws_device(ws_keyframes, w_frames, wraps=2, kind='cubic'):

@@ -82,8 +82,9 @@ class Engine:
         mask = torch.ones(1, 1, 256, 256) if uv_face_mask is None else uv_face_mask
         self.eye_mask = mask.reshape(mask.shape[-2], mask.shape[-1]).to(self.device, torch.float32).contiguous()
         self._mm_init = torch.tensor([float('inf'), 0.0], device=self.device)
-        self._graphs = {}
-        self._side = None                       # side streams of the concurrent branches (compute_planes)
+        self._graphs = {}                       # key[0]: the graph reads or writes the backbone cache
+        self._cache = None                      # backbone cache (synthesis with cache_backbone=True), see _cache_buffers
+        self._side = None                      # side streams of the concurrent branches (compute_planes)
         self.concurrent = os.environ.get('N3D_CONCURRENT', '1') != '0'
         self.splitk = os.environ.get('N3D_SPLITK', '1') != '0'
         self.splitk_maxres = int(os.environ.get('N3D_SPLITK_MAXRES', '16'))
@@ -510,19 +511,59 @@ class Engine:
             self.launches = K.launches - n0
             return out
 
-    def _compute_planes(self, ws, v, noise_mode='const', return_intermediates=False):
-        cfg, dev = self.cfg, self.device
+    # ------------------------------------------------------------------------------------------ backbone cache
+    # synthesis(cache_backbone=True) keeps (a) the two ws-only backbone outputs, (b) the blended planes and (c) the call's ws and
+    # noise_mode in engine-owned buffers at fixed addresses, so that captured graphs can read and write them and no graph replay
+    # overwrites them.  use_cached_backbone=True re-runs everything but (a) (triplane.py:120-128 of EG3D); render_views renders new
+    # cameras from (b).  The cache lives until the next cache_backbone call with another batch size or the engine is rebuilt.
+    def _cache_buffers(self, B, ws_shape):
+        """The cache buffers for batch B; a new B (or ws shape) reallocates them, which empties the cache and drops every graph that
+        reads or writes them."""
+        c = self._cache
+        if c is None or c['B'] != B or tuple(c['ws'].shape[1:]) != tuple(ws_shape[1:]):
+            P, C = self.cfg.plane_res, self.cfg.plane_ch
+            self._graphs = {k: g for k, g in self._graphs.items() if not k[0]}
+            c = self._cache = dict(B=B, textures=self._f32(B, P, P, C), static=self._f32(B, P, P, 3 * C), planes=self._f32(B, 3, P, P, C),
+                                   ws=self._f32(B, *ws_shape[1:]), noise_mode=None)          # noise_mode None: nothing cached yet
+        return c
+
+    def _cached(self, N, who):
+        """The filled cache for a call with batch N (None when nothing is cached); a cache of another batch size raises."""
+        c = self._cache
+        if c is None or c['noise_mode'] is None:
+            return None
+        if c['B'] != N:
+            raise RuntimeError(f'next3d_b200: {who} with batch {N}, but the cached backbone holds batch {c["B"]}')
+        return c
+
+    def _views_cache(self, N):
+        """(cache, views per plane set) for render_views of N cameras."""
+        c = self._cache
+        if c is None or c['noise_mode'] is None:
+            raise RuntimeError('next3d_b200: render_views needs cached planes: run synthesis(..., cache_backbone=True) first')
+        if N % c['B']:
+            raise RuntimeError(f'next3d_b200: render_views got {N} cameras, not a multiple of the cached batch {c["B"]}')
+        return c, N // c['B']
+
+    def _set_styles(self, ws):
+        """Style vectors and demodulation coefficients of every modulated layer for the batch ws [N, L, D]."""
         N = ws.shape[0]
         self._N = N
-        P = cfg.plane_res
         ws = ws.to(torch.float32).contiguous()
-        v = v.to(torch.float32)
-        verts, lms = v[:, :5023].contiguous(), v[:, 5023:].contiguous()
         s_ooff, d_soff, d_ooff = self._batch_tables(N)
         self._styles = self._f32(self.style_elems * N)
         self._dcoefs = self._f32(self.dcoef_elems * N)
         K.styles(ws, self.aff_w, self.aff_b, self.row_widx, self.row_scale, s_ooff, self.row_cin, self._styles)
         K.demod(self._styles, self.wsq, self.d_woff, self.d_cin, d_soff, d_ooff, self.d_cout, self._dcoefs, N)
+
+    def _compute_planes(self, ws, v, noise_mode='const', return_intermediates=False, cache_backbone=False, use_cached_backbone=False):
+        cfg, dev = self.cfg, self.device
+        N = ws.shape[0]
+        P = cfg.plane_res
+        cached = self._cached(N, 'use_cached_backbone') if use_cached_backbone else None
+        v = v.to(torch.float32)
+        verts, lms = v[:, :5023].contiguous(), v[:, 5023:].contiguous()
+        self._set_styles(ws)
         # Three independent branches (triplane_next3d.py:137-170): (1) neural texture -> UV lookup -> mouth / blending UNets,
         # (2) mesh rasterization + mouth box (needs only the vertices), (3) the static tri-plane backbone (needed only by the final
         # blend).  (2) and (3) run on side streams: their latency-bound kernels (4^2..32^2 layers on a few dozen SMs, the flood
@@ -547,9 +588,12 @@ class Engine:
             boxes = torch.empty(N, 4, dtype=torch.int32, device=dev)
             lm2d = tl[:, 0, :, :2].contiguous()
             K.mouth_box(lm2d, boxes)
-        with torch.cuda.stream(s_static):
-            static = self._backbone('backbone.synthesis', cfg.plane_ch * 3, noise_mode)             # [N,256,256,96]
-        textures = self._backbone('texture_backbone.synthesis', cfg.plane_ch, noise_mode)          # [N,256,256,32]
+        if cached is None:
+            with torch.cuda.stream(s_static):
+                static = self._backbone('backbone.synthesis', cfg.plane_ch * 3, noise_mode)         # [N,256,256,96]
+            textures = self._backbone('texture_backbone.synthesis', cfg.plane_ch, noise_mode)      # [N,256,256,32]
+        else:
+            static, textures = cached['static'], cached['textures']
         if self.concurrent:
             main.wait_stream(s_rast)
             for t in (p2f, bary, boxes, lm2d):
@@ -567,31 +611,54 @@ class Engine:
         stitched = front.clone()
         K.resize_aa(mouth, stitched, dst_box=boxes)
         blended = self._styleunet('neural_blending.synthesis', stitched, 256, 32, 256, noise_mode)
-        if self.concurrent:
+        if self.concurrent and cached is None:
             main.wait_stream(s_static)
             static.record_stream(main)
         planes = self._f32(N, 3, P, P, cfg.plane_ch)
         K.blend_planes(blended, tex_planes, alpha, static, planes)
+        if cache_backbone:
+            c = self._cache_buffers(N, ws.shape)
+            if cached is None:
+                c['textures'].copy_(textures)
+                c['static'].copy_(static)
+                c['noise_mode'] = noise_mode
+            c['planes'].copy_(planes)
+            c['ws'].copy_(ws)
         if return_intermediates:
             return planes, dict(textures=textures, pix_to_face=p2f.view(N, 4, P, P), tex_planes=tex_planes, alpha=alpha, boxes=boxes,
                                 mouth_crop=crop, mouth_plane=mouth, stitched=stitched, blended_front=blended, static=static, lm2d=lm2d)
         return planes
 
     def synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
-                  return_intermediates=False, seed_ptr=None):
+                  return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False):
+        """cache_backbone: also keep the backbone outputs, planes and ws (see _cache_buffers); use_cached_backbone: take the two
+        ws-only backbones from that cache (a cache of another batch size raises; no cache = computed as usual)."""
         self._on_device(ws=ws, c=c, v=v)
         with torch.cuda.device(self.device):
-            return self._synthesis(ws, c, v, noise_mode, neural_rendering_resolution, sampler_noise, seed, return_intermediates, seed_ptr)
+            return self._synthesis(ws, c, v, noise_mode, neural_rendering_resolution, sampler_noise, seed, return_intermediates, seed_ptr,
+                                   cache_backbone, use_cached_backbone)
 
     def _synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
-                   return_intermediates=False, seed_ptr=None):
-        cfg, dev = self.cfg, self.device
-        N = ws.shape[0]
-        R = neural_rendering_resolution or cfg.neural_rendering_resolution
+                   return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False):
+        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
         n0 = K.launches
         self.conv_flops = 0.0
-        out = self._compute_planes(ws, v, noise_mode, return_intermediates)
+        out = self._compute_planes(ws, v, noise_mode, return_intermediates, cache_backbone, use_cached_backbone)
         planes, inter = out if return_intermediates else (out, None)
+        result, feat, wsum, ws_normals = self._render(planes, c, R, sampler_noise, seed, seed_ptr)
+        self.launches = K.launches - n0
+        if return_intermediates:
+            inter.update(planes=planes, feature_image=feat, weights_sum=wsum)
+            if ws_normals is not None:                                      # per ray: D sorted sample depths, then D - 1 final weights
+                inter['normal_samples'] = ws_normals.view(feat.shape[0], R * R, -1)
+            result['intermediates'] = inter
+        return result
+
+    def _render(self, planes, c, R, sampler_noise, seed, seed_ptr, views=1):
+        """Volume rendering, depth clamp and super-resolution of N = planes.shape[0] * views images (image n reads plane set
+        n // views) with the current batch's styles -> (synthesis output dict, feature image, weight sums, normal workspace)."""
+        cfg, dev = self.cfg, self.device
+        N = planes.shape[0] * views
         c = c.to(torch.float32)
         cam = c[:, :16].contiguous()
         intr = c[:, 16:25].contiguous()
@@ -604,61 +671,107 @@ class Engine:
         if u_c is not None:
             u_c, u_f = u_c.to(dev, torch.float32).contiguous(), u_f.to(dev, torch.float32).contiguous()
         normal = self._f32(N, M, 3) if self.rk.get('return_normal', False) else None
+        ws_normals = None
         ev = self._prof_begin()
         if normal is None:
-            K.render_rays(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, u_coarse=u_c, u_fine=u_f, seed=seed, seed_ptr=seed_ptr)
+            K.render_rays(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, u_coarse=u_c, u_fine=u_f, seed=seed, seed_ptr=seed_ptr,
+                          views=views)
         else:                                                               # return_normal (renderer.py:271-355, ray_marcher.py:61-64)
             ws_normals = self._f32(K.normals_workspace_floats(N, R, self.rk))
             K.render_rays_normals(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, normal, ws_normals, u_coarse=u_c, u_fine=u_f,
-                                  seed=seed, seed_ptr=seed_ptr)
+                                  seed=seed, seed_ptr=seed_ptr, views=views)
         self._prof_end(ev, 'render_rays')
         K.depth_clamp(depth, mm)
         image = self._f32(N, 3, cfg.img_resolution, cfg.img_resolution)
         self._superresolution(feat, self.rk['superresolution_noise_mode'], image)
-        self.launches = K.launches - n0
         result = {'image': image, 'image_raw': feat.permute(0, 3, 1, 2)[:, :3], 'image_depth': depth}
         if normal is not None:
             result['image_normal'] = normal.view(N, R, R, 3).permute(0, 3, 1, 2)          # ray m = i * R + j -> pixel (i, j)
-        if return_intermediates:
-            inter.update(planes=planes, feature_image=feat, weights_sum=wsum)
-            if normal is not None:                                          # per ray: D sorted sample depths, then D - 1 final weights
-                inter['normal_samples'] = ws_normals.view(N, M, -1)
-            result['intermediates'] = inter
+        return result, feat, wsum, ws_normals
+
+    def render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None):
+        """New camera views of the cached heads: c [N, 25] with N = B * V for a cache of batch B; view n belongs to head n // V.
+        Renders from the cached planes and runs super-resolution with the cached ws; returns what synthesis returns."""
+        self._on_device(c=c)
+        with torch.cuda.device(self.device):
+            return self._render_views(c, neural_rendering_resolution, sampler_noise, seed, seed_ptr)
+
+    def _render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None):
+        cache, V = self._views_cache(c.shape[0])
+        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+        n0 = K.launches
+        self.conv_flops = 0.0
+        ws = cache['ws']
+        self._set_styles(ws[:, None].expand(ws.shape[0], V, *ws.shape[1:]).reshape(-1, *ws.shape[1:]))     # ws of head n // V
+        result = self._render(cache['planes'], c, R, sampler_noise, seed, seed_ptr, views=V)[0]
+        self.launches = K.launches - n0
         return result
 
     # ------------------------------------------------------------------------------------------ CUDA graph replay
-    def synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0):
-        with torch.cuda.device(self.device):
-            return self._synthesis_graphed(ws, c, v, noise_mode, neural_rendering_resolution, seed)
-
-    def _synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0):
-        """Same as synthesis() (in-kernel sampler RNG) but the ~200 launches of one forward are captured once per
-        (batch, resolution, noise_mode) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
-        leaves the GPU idle between kernels.  Inputs are copied into static buffers; the returned tensors are the graph's
-        static outputs and are overwritten by the next call with the same key."""
-        self._on_device(ws=ws, c=c, v=v)
-        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+    def _render_key(self, R):
         rk = self.rk
-        key = (ws.shape[0], R, noise_mode, tuple(v.shape), rk['depth_resolution'], rk['depth_resolution_importance'], float(rk['ray_start']),
-               float(rk['ray_end']), float(rk['box_warp']), bool(rk.get('white_back', False)), rk['superresolution_noise_mode'],
-               bool(rk.get('sr_antialias', True)), bool(rk.get('return_normal', False)))
+        return (R, rk['depth_resolution'], rk['depth_resolution_importance'], float(rk['ray_start']), float(rk['ray_end']), float(rk['box_warp']),
+                bool(rk.get('white_back', False)), rk['superresolution_noise_mode'], bool(rk.get('sr_antialias', True)),
+                bool(rk.get('return_normal', False)))
+
+    def _replay(self, key, inputs, run, seed):
+        """Capture run(static inputs) once per key into a CUDA graph and replay it: inputs are copied into static buffers (plus a
+        device seed counter for the in-kernel sampler RNG); the returned tensors are the graph's static outputs and are overwritten
+        by the next call with the same key."""
         g = self._graphs.get(key)
         if g is None:
-            st = dict(ws=torch.empty(ws.shape, dtype=torch.float32, device=self.device), c=torch.empty(c.shape, dtype=torch.float32, device=self.device),
-                      v=torch.empty(v.shape, dtype=torch.float32, device=self.device), seed=torch.zeros(1, dtype=torch.int64, device=self.device))
-            st['ws'].copy_(ws); st['c'].copy_(c); st['v'].copy_(v)
+            st = {k: torch.empty(t.shape, dtype=torch.float32, device=self.device) for k, t in inputs.items()}
+            st['seed'] = torch.zeros(1, dtype=torch.int64, device=self.device)
+            for k, t in inputs.items():
+                st[k].copy_(t)
             side = torch.cuda.Stream(self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):                                   # warm-up outside capture (lazy attribute setup, allocator)
-                self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'])
+                run(st)
             torch.cuda.current_stream(self.device).wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out = self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'])
+                out = run(st)
             g = self._graphs[key] = (graph, st, out, self.launches, self.conv_flops)
         graph, st, out, launches, flops = g
-        st['ws'].copy_(ws, non_blocking=True); st['c'].copy_(c, non_blocking=True); st['v'].copy_(v, non_blocking=True)
+        for k, t in inputs.items():
+            st[k].copy_(t, non_blocking=True)
         st['seed'].fill_(int(seed))
         graph.replay()
         self.launches, self.conv_flops = launches, flops
         return out
+
+    def synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
+                          use_cached_backbone=False):
+        with torch.cuda.device(self.device):
+            return self._synthesis_graphed(ws, c, v, noise_mode, neural_rendering_resolution, seed, cache_backbone, use_cached_backbone)
+
+    def _synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
+                           use_cached_backbone=False):
+        """Same as synthesis() (in-kernel sampler RNG) but the ~200 launches of one forward are captured once per
+        (batch, resolution, noise_mode, cache use) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
+        leaves the GPU idle between kernels.  The cache-using graphs read and write the engine's cache buffers in place."""
+        self._on_device(ws=ws, c=c, v=v)
+        N = ws.shape[0]
+        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+        reuse = use_cached_backbone and self._cached(N, 'use_cached_backbone') is not None
+        if cache_backbone:
+            self._cache_buffers(N, ws.shape)              # allocated before capture: the graph writes the cache at fixed addresses
+        key = (cache_backbone or reuse, cache_backbone, reuse, N, noise_mode, tuple(v.shape)) + self._render_key(R)
+
+        def run(st):
+            return self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,
+                                   use_cached_backbone=reuse)
+        out = self._replay(key, dict(ws=ws, c=c, v=v), run, seed)
+        if cache_backbone and not reuse:
+            self._cache['noise_mode'] = noise_mode
+        return out
+
+    def render_views_graphed(self, c, neural_rendering_resolution=None, seed=0):
+        """render_views() replayed from a CUDA graph per (N, V, resolution, rendering options); in-kernel sampler RNG."""
+        self._on_device(c=c)
+        with torch.cuda.device(self.device):
+            _, V = self._views_cache(c.shape[0])
+            R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+            key = (True, 'views', c.shape[0], V) + self._render_key(R)
+            return self._replay(key, dict(c=c), lambda st: self._render_views(st['c'], R, seed=0, seed_ptr=st['seed']), seed)

@@ -208,11 +208,12 @@ def blend_planes(front, tex_planes, alpha, static, planes):
     _run('n3d_blend_planes', ptr(front), ptr(tex_planes), ptr(alpha), ptr(static), N, H, W, ptr(planes), stream_ptr())
 
 
-def _render_desc(planes, cam2world, intrinsics, res, opts, seed):
-    """Render descriptor with the workload (planes, cameras, resolution, sampling options, seed) filled in."""
+def _render_desc(planes, cam2world, intrinsics, res, opts, seed, views=1):
+    """Render descriptor with the workload (planes, cameras, resolution, sampling options, seed) filled in: views images per plane set,
+    so planes.shape[0] * views images."""
     p = _lib.Render()
-    N, _, PH, PW, _ = planes.shape
-    p.planes, p.N, p.PH, p.PW = ptr(planes), N, PH, PW
+    B, _, PH, PW, _ = planes.shape
+    p.planes, p.N, p.PH, p.PW, p.views = ptr(planes), B * max(views, 1), PH, PW, views
     p.cam2world, p.intrinsics, p.res = ptr(cam2world), ptr(intrinsics), res
     p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
     p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
@@ -220,7 +221,7 @@ def _render_desc(planes, cam2world, intrinsics, res, opts, seed):
     return p
 
 
-def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr):
+def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr, views=1):
     """Render descriptor of n3d_render_rays / n3d_render_rays_normals, after rejecting the rendering options the renderer lacks."""
     unsupported = [k for k, bad in (('disparity_space_sampling', bool(opts.get('disparity_space_sampling', False))),
                                     ('density_noise', float(opts.get('density_noise', 0) or 0) > 0),
@@ -229,7 +230,7 @@ def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth,
     if unsupported:     # renderer.py:98-107 (auto near/far), :153 (density noise), :186-196 (disparity sampling), ray_marcher.py:41-44
         raise RuntimeError(f'libnext3d_b200 n3d_render_rays failed (code -2, unsupported): rendering option(s) {unsupported} are not '
                            f'implemented by the fused renderer (supported: linear stratified sampling, fixed ray_start / ray_end, softplus)')
-    p = _render_desc(planes, cam2world, intrinsics, res, opts, seed)
+    p = _render_desc(planes, cam2world, intrinsics, res, opts, seed, views)
     p.u_coarse, p.u_fine, p.seed_ptr = ptr(u_coarse), ptr(u_fine), ptr(seed_ptr)
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
     p.rgb, p.depth, p.wsum, p.depth_minmax = ptr(rgb), ptr(depth), ptr(wsum), ptr(depth_minmax)
@@ -238,11 +239,13 @@ def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth,
 
 
 def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
-                seed_ptr=None):
-    """planes [N,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in.
+                seed_ptr=None, views=1):
+    """planes [B,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in.
     opts['depth_resolution'] (4 .. 192) and opts['depth_resolution_importance'] (0 = coarse only .. 192) are samples per pass; a
-    count above 192 raises (code -2, unsupported)."""
-    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
+    count above 192 raises (code -2, unsupported).  views: camera views per plane set -- N = B * views images, image n reads plane
+    set n // views; cameras, uniforms and outputs are per image."""
+    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr,
+                          views)
     _run('n3d_render_rays', C.byref(p), stream_ptr())
 
 
@@ -253,17 +256,18 @@ def normals_workspace_floats(N, res, opts):
 
 
 def render_rays_normals(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, normal, workspace=None, u_coarse=None,
-                        u_fine=None, seed=0, seed_ptr=None):
+                        u_fine=None, seed=0, seed_ptr=None, views=1):
     """render_rays (same outputs, bit for bit) plus normal [N, M, 3]: unit world-space normals -grad sigma composited with the final
     weights (rendering option return_normal).  workspace: fp32 device buffer of normals_workspace_floats() floats, or None to
-    allocate one here.  Same sample-count limits as render_rays (up to 192 + 192)."""
-    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr)
-    n_ws = normals_workspace_floats(planes.shape[0], res, opts)
+    allocate one here.  Same sample-count limits and `views` as render_rays (N = planes.shape[0] * views images)."""
+    p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr,
+                          views)
+    n_ws = normals_workspace_floats(p.N, res, opts)
     if workspace is None:
         workspace = torch.empty(n_ws, dtype=torch.float32, device=planes.device)
     elif workspace.numel() < n_ws or workspace.dtype != torch.float32:
         raise RuntimeError(f'render_rays_normals: workspace needs {n_ws} float32 elements, got {workspace.numel()} {workspace.dtype}')
-    if normal.numel() != planes.shape[0] * res * res * 3 or normal.dtype != torch.float32:
+    if normal.numel() != p.N * res * res * 3 or normal.dtype != torch.float32:
         raise RuntimeError(f'render_rays_normals: normal must be float32 [N, M, 3], got {tuple(normal.shape)} {normal.dtype}')
     _run('n3d_render_rays_normals', C.byref(p), ptr(normal), ptr(workspace), stream_ptr(), kernels=2)
 

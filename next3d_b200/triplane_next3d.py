@@ -190,19 +190,46 @@ class TriPlaneGenerator(torch.nn.Module):
         Extra keyword `sampler_noise=(u_coarse [N,M,Dc,1], u_fine [N*M,Df])` injects the stratified / importance sampling
         uniforms (parity tests); by default the renderer draws them from an in-kernel counter RNG seeded per call.
         With `rendering_kwargs['return_normal']` set the output also holds 'image_normal' [N,3,r,r]: unit world-space normals
-        -grad sigma composited like the colours (renderer.py:271-355, ray_marcher.py:61-64)."""
-        if neural_rendering_resolution is None:
-            neural_rendering_resolution = self.neural_rendering_resolution
-        else:
-            self.neural_rendering_resolution = neural_rendering_resolution
+        -grad sigma composited like the colours (renderer.py:271-355, ray_marcher.py:61-64).
+        `cache_backbone=True` also keeps this call's ws-only backbone outputs, blended planes, ws and noise_mode until the next caching
+        call or a weight change; `use_cached_backbone=True` takes the two ws-only backbones from that cache and re-runs everything
+        that depends on the mesh (triplane.py:120-128 of EG3D; a cache of another batch size raises, no cache computes them), and
+        `render_views` renders new cameras from the cached planes."""
+        neural_rendering_resolution = self._rendering_resolution(neural_rendering_resolution)
         noise_mode = synthesis_kwargs.get('noise_mode', 'random')
-        if seed is None:
-            seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if sampler_noise is None else 0
+        seed = self._sampler_seed(seed, sampler_noise)
         eng = self._get_engine()
+        flags = dict(cache_backbone=bool(cache_backbone), use_cached_backbone=bool(use_cached_backbone))
         if self.use_cuda_graph and sampler_noise is None and not synthesis_kwargs.get('return_intermediates', False):
-            return eng.synthesis_graphed(ws, c, v, noise_mode=noise_mode, neural_rendering_resolution=neural_rendering_resolution, seed=seed)
+            return eng.synthesis_graphed(ws, c, v, noise_mode=noise_mode, neural_rendering_resolution=neural_rendering_resolution, seed=seed,
+                                         **flags)
         return eng.synthesis(ws, c, v, noise_mode=noise_mode, neural_rendering_resolution=neural_rendering_resolution,
-                             sampler_noise=sampler_noise, seed=seed, return_intermediates=synthesis_kwargs.get('return_intermediates', False))
+                             sampler_noise=sampler_noise, seed=seed, return_intermediates=synthesis_kwargs.get('return_intermediates', False),
+                             **flags)
+
+    def render_views(self, c, neural_rendering_resolution=None, seed=None, sampler_noise=None):
+        """New camera views of the heads cached by `synthesis(..., cache_backbone=True)` with batch B, without regenerating them:
+        c [N, 25] with N = B * V, view n belongs to head n // V -> the dict `synthesis` returns, for N images.  Renders the cached
+        planes and runs super-resolution with the cached ws (the backbones' noise_mode is the caching call's; SR noise follows
+        rendering_kwargs['superresolution_noise_mode']).  Raises RuntimeError when nothing is cached or B does not divide N."""
+        neural_rendering_resolution = self._rendering_resolution(neural_rendering_resolution)
+        seed = self._sampler_seed(seed, sampler_noise)
+        eng = self._get_engine()
+        if self.use_cuda_graph and sampler_noise is None:
+            return eng.render_views_graphed(c, neural_rendering_resolution=neural_rendering_resolution, seed=seed)
+        return eng.render_views(c, neural_rendering_resolution=neural_rendering_resolution, sampler_noise=sampler_noise, seed=seed)
+
+    def _rendering_resolution(self, r):
+        if r is None:
+            return self.neural_rendering_resolution
+        self.neural_rendering_resolution = r
+        return r
+
+    @staticmethod
+    def _sampler_seed(seed, sampler_noise):
+        if seed is None:
+            return int(torch.randint(0, 2 ** 31 - 1, (1,)).item()) if sampler_noise is None else 0
+        return seed
 
     def sample_mixed(self, coordinates, directions, ws, v, truncation_psi=1, truncation_cutoff=None, update_emas=False, **synthesis_kwargs):
         """run_model on arbitrary points (triplane_next3d.py:278-323): -> {'rgb': [N,P,32], 'sigma': [N,P,1]}."""
