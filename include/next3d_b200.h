@@ -257,11 +257,16 @@ typedef struct {
     float* rgb;                /* [N, M, 32] */
     float* depth;              /* [N, M] (unclamped) */
     float* wsum;               /* [N, M] */
-    float* depth_minmax;       /* [2] device: running min / max of all sample depths (init +inf / -inf by caller) */
+    float* depth_minmax;       /* [2] device: running min / max of all sample depths (init +inf / -inf by caller); [N, 2] when
+                                  depth_range_per_image = 1 */
     int32_t white_back;
     int32_t views;             /* camera views per plane set: 0 or 1 = image n reads plane set n; V >= 2 = image n reads plane set
                                   n / V, so `planes` holds N / V sets (N a multiple of V).  Cameras, uniforms, outputs and depth_minmax
                                   stay per image. */
+    int32_t depth_range_per_image;  /* 0: depth_minmax [2] covers the whole launch (ray_marcher.py:54 on a batch).  1: depth_minmax
+                                  [N, 2], pair n reduced over image n's samples only (each pair initialised to +inf / -inf by the
+                                  caller; with views = V the pair is the image's, not the plane set's), as when every image is rendered
+                                  by a launch of its own.  Any other value -> N3D_ERR_INVALID_ARG. */
 } N3DRender;
 
 int n3d_render_rays(const N3DRender* p, void* stream);
@@ -285,6 +290,9 @@ int n3d_render_normals_pass(const N3DRender* p, int forward, const float* worksp
 int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream);
 /* composite depth clamp to the batch-global depth range (ray_marcher.py:53-54). */
 int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* stream);
+/* the same clamp per image (depth_range_per_image = 1): depth [N, per_image] elements of image n clamped to depth_minmax[n] of
+ * depth_minmax [N, 2].  N >= 0, per_image >= 0, non-null pointers; otherwise N3D_ERR_INVALID_ARG. */
+int n3d_depth_clamp_images(float* depth, int N, int64_t per_image, const float* depth_minmax, void* stream);
 /* run_model only (TriPlaneGenerator.sample, triplane_next3d.py:276): coords [N,P,3] -> sigma [N,P], rgb [N,P,32] (or NULL). */
 int n3d_sample_points(const float* planes, int N, int PH, int PW, const float* coords, int64_t P, float box_warp,
                       const float* w0, const float* b0, const float* w1, const float* b1, float* sigma, float* rgb,

@@ -58,7 +58,7 @@ class Render(C.Structure):
         ('ray_start', F32), ('ray_end', F32), ('box_warp', F32),
         ('u_coarse', P), ('u_fine', P), ('seed', C.c_uint64), ('seed_ptr', P),
         ('w0', P), ('b0', P), ('w1', P), ('b1', P),
-        ('rgb', P), ('depth', P), ('wsum', P), ('depth_minmax', P), ('white_back', I32), ('views', I32),
+        ('rgb', P), ('depth', P), ('wsum', P), ('depth_minmax', P), ('white_back', I32), ('views', I32), ('depth_range_per_image', I32),
     ]
 
 
@@ -91,6 +91,7 @@ _SIGNATURES = {
     'n3d_render_rays_normals': ([C.POINTER(Render), P, P, P], C.c_int),
     'n3d_render_normals_pass': ([C.POINTER(Render), C.c_int, P, P, P], C.c_int),
     'n3d_depth_clamp': ([P, I64, P, P], C.c_int),
+    'n3d_depth_clamp_images': ([P, C.c_int, I64, P, P], C.c_int),
     'n3d_sample_points': ([P, C.c_int, C.c_int, C.c_int, P, I64, F32, P, P, P, P, P, P, P], C.c_int),
     'n3d_render_floor': ([P, C.c_int, P, P], C.c_int),
     'n3d_mapping': ([P, P, C.c_int, F32, P, P, P, P, P, P, P, F32, C.c_int, C.c_int, P, P], C.c_int),

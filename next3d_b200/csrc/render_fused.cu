@@ -657,6 +657,21 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
 #pragma unroll
         for (int t = 0; t < kMaxT; ++t) { cur_tc[t] = cur_sc[t] = cur_tf[t] = cur_sf[t] = nxt_tc[t] = nxt_sc[t] = nxt_tf[t] = 0.f; }
         float dmin = INFINITY, dmax = -INFINITY;
+        int dimg = 0;                                               // depth_minmax pair dmin / dmax fold into (per-image mode)
+        // fold this warp's running depth range into pair dimg and restart it: one atomic pair per warp of set 0 (warp-uniform)
+        auto flush_range = [&]() {
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                dmin = fminf(dmin, __shfl_xor_sync(FULL, dmin, o));
+                dmax = fmaxf(dmax, __shfl_xor_sync(FULL, dmax, o));
+            }
+            if (lane == 0) {       // depths are positive (ray_start > 0): IEEE ordering == signed-int ordering
+                int* const mm = reinterpret_cast<int*>(P.depth_minmax) + 2 * dimg;
+                if (dmin < INFINITY) atomicMin(mm, __float_as_int(dmin));
+                if (dmax > -INFINITY) atomicMax(mm + 1, __float_as_int(dmax));
+            }
+            dmin = INFINITY; dmax = -INFINITY;
+        };
 
         // ---- decoder of tile ti, layer 1 (frees the A buffer; hidden layer -> shared memory)
         auto epi1 = [&](int ti) { layer1_tile(S, q, eset, lane, ti); };
@@ -1028,6 +1043,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 if (P.white_back) v = v + 1.f - wsum;
                 P.rgb[gr * kFeat + 16 * eset + j] = v * 2.f - 1.f;
             }
+            if (P.depth_range_per_image && eset == 0) {              // a group's rays all belong to image (g_begin + r) / gpi
+                const int n = (g_begin + r) / K.gpi;
+                if (n != dimg) { flush_range(); dimg = n; }
+            }
             if (ok && eset == 0 && j == 0) {
                 float depth = dacc / wsum;
                 if (isnan(depth)) depth = INFINITY;                  // nan_to_num(nan=inf); the clamp kernel finishes the job
@@ -1096,18 +1115,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             pend_kind = it.kind; pend_r = it.group(); pend_t = it.t; pend_i = i;
         }
 
-        // batch-global depth range (ray_marcher.py:54): one atomic pair per warp of set 0
-        if (eset == 0 && P.depth_minmax) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                dmin = fminf(dmin, __shfl_xor_sync(FULL, dmin, o));
-                dmax = fmaxf(dmax, __shfl_xor_sync(FULL, dmax, o));
-            }
-            if (lane == 0) {       // depths are positive (ray_start > 0): IEEE ordering == signed-int ordering
-                if (dmin < INFINITY) atomicMin(reinterpret_cast<int*>(P.depth_minmax), __float_as_int(dmin));
-                if (dmax > -INFINITY) atomicMax(reinterpret_cast<int*>(P.depth_minmax) + 1, __float_as_int(dmax));
-            }
-        }
+        // depth range (ray_marcher.py:54): batch-global into pair 0, or per image into pair dimg (the last image this warp composited)
+        if (eset == 0 && P.depth_minmax) flush_range();
     }
 
 }
@@ -1641,6 +1650,17 @@ __global__ void __launch_bounds__(256) depth_clamp_kernel(float* __restrict__ de
     }
 }
 
+// The same clamp with one depth range per image: image i / per_image is clamped to its own pair of mm [N, 2].
+__global__ void __launch_bounds__(256) depth_clamp_images_kernel(float* __restrict__ depth, int64_t n, int64_t per_image,
+                                                                 const float* __restrict__ mm) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t img = i / per_image;
+        float d = depth[i];
+        if (isnan(d)) d = INFINITY;
+        depth[i] = fminf(fmaxf(d, __ldg(mm + 2 * img)), __ldg(mm + 2 * img + 1));
+    }
+}
+
 constexpr int kMaxD = kMaxT * 64;               // depth samples per pass the fused kernel lays out (3 tiles x 64 lanes per ray)
 constexpr int kMaxDFloor = kMaxT * 32;          // the floor micro-kernels know the 16- and 32-lane layouts only
 
@@ -1717,6 +1737,9 @@ int check_render(const N3DRender* p, const char* who) {
     N3D_CHECK_ARG(p->depth_coarse >= 4 && p->depth_fine >= 0, "%s: depth resolutions (%d, %d): need coarse >= 4, fine >= 0", who,
                   p->depth_coarse, p->depth_fine);
     if (int rc = check_views(p, who)) return rc;
+    N3D_CHECK_ARG(p->depth_range_per_image == 0 || p->depth_range_per_image == 1, "%s: depth_range_per_image = %d must be 0 or 1", who,
+                  p->depth_range_per_image);
+    N3D_CHECK_ARG(!p->depth_range_per_image || p->depth_minmax, "%s: depth_range_per_image = 1 needs depth_minmax [N, 2]", who);
     N3D_CHECK_ARG((long long)(p->N / plane_views(p)) * 3 * p->PH * p->PW * 128 < (1ll << 32), "%s: plane tensor too large for 32-bit texel offsets",
                   who);
     N3D_CHECK_ARG(p->res >= 1 && p->N >= 1 && p->ray_start > 0.f && p->ray_end > p->ray_start && p->box_warp > 0.f, "%s: bad ray setup", who);
@@ -1813,6 +1836,16 @@ extern "C" int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minma
     if (n == 0) return N3D_OK;
     depth_clamp_kernel<<<n3d_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(depth, n, depth_minmax);
     N3D_CHECK_LAUNCH("n3d_depth_clamp");
+    return N3D_OK;
+}
+
+extern "C" int n3d_depth_clamp_images(float* depth, int N, int64_t per_image, const float* depth_minmax, void* stream) {
+    N3D_CHECK_ARG(depth && depth_minmax && N >= 0 && per_image >= 0, "n3d_depth_clamp_images: bad args (N = %d, per_image = %lld)", N,
+                  (long long)per_image);
+    const int64_t n = (int64_t)N * per_image;
+    if (n == 0) return N3D_OK;
+    depth_clamp_images_kernel<<<n3d_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(depth, n, per_image, depth_minmax);
+    N3D_CHECK_LAUNCH("n3d_depth_clamp_images");
     return N3D_OK;
 }
 

@@ -7,6 +7,7 @@ Everything here is host logic around the hot path; the per-frame values (camera 
 reference's, checked in tests/test_drivers_cpu.py against the reference's own code.
 """
 import math
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -52,7 +53,8 @@ def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_
     the padding is dropped.  The device->host copy of batch i overlaps the synthesis of batch i+1.  `seed`: base seed of the ray
     sampler's RNG (batch k uses seed + k); None = a fresh random seed per call, like the reference's torch.rand.
     `sampler_noise=(u_coarse [F, M, Dc, 1], u_fine [F, M, Df])`: per-frame sampler uniforms instead of the in-kernel RNG (parity tests:
-    frame f gets the same noise whichever batch slot it lands in)."""
+    frame f gets the same noise whichever batch slot it lands in).  image_mode 'image_depth' renders with depth_range='image', so
+    each depth frame is clamped to its own range as in the script (one frame per synthesis call), whatever the batching."""
     yield from _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, False)
 
 
@@ -67,7 +69,7 @@ def render_orbit(G, ws, cams, verts, batch=8, image_mode='image', seed=None, sam
 
     def outputs():
         for idx, n, kw in _batches(cams.shape[0], batch, seed, sampler_noise):
-            yield G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **kw), n
+            yield G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device), **kw), n
     yield from _frames(outputs(), image_mode, device)
 
 
@@ -79,9 +81,21 @@ def _batches(F, batch, seed, sampler_noise):
         idx = list(range(b0, b0 + n)) + [b0 + n - 1] * (batch - n)
         kw = {} if seed is None else {'seed': int(seed) + b0 // batch}
         if sampler_noise is not None:
-            u_c, u_f = sampler_noise
-            kw['sampler_noise'] = (u_c[idx], u_f[idx].reshape(-1, u_f.shape[-1]))
+            kw['sampler_noise'] = _noise_rows(sampler_noise, idx)
         yield idx, n, kw
+
+
+def _noise_rows(sampler_noise, idx):
+    """The synthesis `sampler_noise` of the frames idx from per-frame rows (u_coarse [F, M, Dc, 1], u_fine [F, M, Df])."""
+    u_c, u_f = sampler_noise
+    return u_c[idx], u_f[idx].reshape(-1, u_f.shape[-1])
+
+
+def _depth_kw(image_mode, device):
+    """Depth frames are clamped to their own depth range, as the scripts' one frame per call does (gen_videos_next3d.py:155,
+    reenact_avatar_next3d.py:164), whatever the batching; the other image modes do not read the range.  The range is the CUDA
+    renderer's (depth_range='image'); a generator on another device is called without the keyword."""
+    return {'depth_range': 'image'} if image_mode == 'image_depth' and torch.device(device).type == 'cuda' else {}
 
 
 def _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, reuse_backbone):
@@ -106,8 +120,19 @@ def _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, dev
                 v = verts[idx].to(device, torch.float32, non_blocking=True)
             if reuse_backbone:
                 kw['use_cached_backbone' if k else 'cache_backbone'] = True
-            yield G.synthesis(w, c, v, noise_mode=noise_mode, **kw), n
+            yield G.synthesis(w, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw), n
     yield from _frames(outputs(), image_mode, device)
+
+
+def _frames_u8(out, image_mode):
+    """[N, H, W, 3] uint8 frames of a generator output dict: out[image_mode], depth normalised per frame to [-1, 1] first."""
+    img = out[image_mode]
+    if image_mode == 'image_depth':                              # gen_videos_next3d.py:160-162, per frame
+        img = -img
+        lo, hi = img.amin(dim=(1, 2, 3), keepdim=True), img.amax(dim=(1, 2, 3), keepdim=True)
+        img = (img - lo) / (hi - lo) * 2 - 1
+        img = img.expand(-1, 3, -1, -1) if img.shape[1] == 1 else img
+    return to_uint8_hwc(img)
 
 
 def _frames(outputs, image_mode, device):
@@ -125,13 +150,7 @@ def _frames(outputs, image_mode, device):
             yield host[k].numpy()
 
     for out, n in outputs:
-        img = out[image_mode]
-        if image_mode == 'image_depth':                          # gen_videos_next3d.py:160-162, per frame
-            img = -img
-            lo, hi = img.amin(dim=(1, 2, 3), keepdim=True), img.amax(dim=(1, 2, 3), keepdim=True)
-            img = (img - lo) / (hi - lo) * 2 - 1
-            img = img.expand(-1, 3, -1, -1) if img.shape[1] == 1 else img
-        u8 = to_uint8_hwc(img)                                   # fresh tensor: the generator's static output buffer is free again
+        u8 = _frames_u8(out, image_mode)                         # fresh tensor: the generator's static output buffer is free again
         if cuda:
             host = torch.empty(u8.shape, dtype=torch.uint8).pin_memory()
             copy_s.wait_stream(torch.cuda.current_stream(device))
@@ -168,28 +187,42 @@ def reenact_schedule(drive_root, num_frames, lms_cond=True):
 
 
 def reenact_frames(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=None,
-                   sampler_noise=None, prefetch_depth=8, workers=4):
+                   sampler_noise=None, prefetch_depth=8, workers=4, image_mode='image'):
     """reenact_avatar_next3d.py:125-167 for ONE identity `ws` [1, L, D]: yields the rendered uint8 HWC frame of every driving frame,
     in order.  Meshes are parsed by the native parsers on worker threads (inputs.FramePrefetcher, pinned memory) while the GPU renders
     batches of `batch` frames; `fixed_camera` [1, 25] replaces the per-frame cameras (the script's --fixed_camera).
-    A `.n3dpack` file written by inputs.write_frame_pack can be given instead of a directory (no parsing at all)."""
+    A `.n3dpack` file written by inputs.write_frame_pack can be given instead of a directory (no parsing at all).  image_mode as in
+    render_frames."""
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers)
+    if n == 0:
+        return
+    wsf = ws.detach().cpu().float().reshape(1, *ws.shape[-2:]).expand(n, -1, -1)
+    yield from _render_frames(G, wsf, cams, frames(0, n), batch, image_mode, noise_mode, None, seed, sampler_noise,
+                              noise_mode in ('const', 'none'))
+
+
+def _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers):
+    """(frame count n, cameras [n, 25], frames(a, b) -> in-order iterable of the [1, V, 3] meshes of frames a .. b-1) of a driving
+    directory (reenact_schedule; only the requested frames are parsed, on worker threads) or of a `.n3dpack` (memory-mapped)."""
     from . import inputs
     if str(drive_root).endswith('.n3dpack'):
         pack = inputs.FramePack(drive_root)
         n = min(len(pack), num_frames)
-        cams, verts = torch.from_numpy(np.array(pack.cams[:n])), (t for i, t in enumerate(pack) if i < n)
+        cams = torch.from_numpy(np.array(pack.cams[:n]))
+
+        def frames(a, b):
+            return pack[a:b]
     else:
         sch = reenact_schedule(drive_root, num_frames, lms_cond)
         n = len(sch['ks'])
         cams = sch['cams']
         pairs = list(zip(sch['obj_paths'], sch['lms_paths'] if lms_cond else [None] * n))
-        verts = inputs.FramePrefetcher(pairs, depth=prefetch_depth, workers=workers)
+
+        def frames(a, b):
+            return inputs.FramePrefetcher(pairs[a:b], depth=prefetch_depth, workers=workers)
     if fixed_camera is not None:
         cams = fixed_camera.reshape(1, 25).cpu().float().expand(n, -1)
-    if n == 0:
-        return
-    wsf = ws.detach().cpu().float().reshape(1, *ws.shape[-2:]).expand(n, -1, -1)
-    yield from _render_frames(G, wsf, cams, verts, batch, 'image', noise_mode, None, seed, sampler_noise, noise_mode in ('const', 'none'))
+    return n, cams, frames
 
 
 def interpolate_ws_device(ws_keyframes, w_frames, wraps=2, kind='cubic'):
@@ -206,47 +239,151 @@ def interpolate_ws_device(ws_keyframes, w_frames, wraps=2, kind='cubic'):
     return K.interp_rows(B, ws_keyframes.to(torch.float32).contiguous())
 
 
-def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const', seed=0, device=None, out=None):
+def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const', seed=0, device=None, out=None, sampler_noise=None):
     """Strong-scaling video driver (BASELINE.json configs[3]: one clip split over the GPUs of a box): rank r renders the contiguous
     frame range shard_range(F, r, world) in batches through `G.synthesis`, converts to uint8 HWC on the device (4x fewer bytes than
     the fp32 images) and the batches are gathered to rank 0 over NCCL on a side stream from a ping-pong staging buffer, so batch
     i+1 renders while batch i is in flight; rank 0 copies every gathered batch to pinned host memory on a third stream.
-    Returns the [F, H, W, 3] uint8 host tensor (frame order) on rank 0, None elsewhere.  World size 1: no collective.
+    Returns the [F, H, W, 3] uint8 host tensor (frame order) on rank 0, None elsewhere, filled in stream order (synchronise the
+    current stream before reading it).  World size 1: no collective.
     `batch` is an upper bound: the per-call batch is the size in [batch/2, batch] that pads the rank's frame count least (30 frames per
     rank -> 5 batches of 6, not 4 of 8).  `out`: optional pinned [F, H, W, 3] uint8 host tensor to fill on rank 0 (pinning 190 MB per
-    clip costs tens of milliseconds)."""
+    clip costs tens of milliseconds).  `sampler_noise`: per-frame uniforms as in render_frames, rows indexed by the global frame id,
+    so the frames do not depend on the number of ranks (batch k of rank r otherwise draws sampler seed seed + r * steps + k)."""
+    device = device or next(G.parameters()).device
+    plan = shard_plan(ws_frames.shape[0], batch)
+    static_mesh = verts.shape[0] == 1
+
+    def step(k, idx):
+        w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
+        c = cams[idx].to(device, torch.float32, non_blocking=True)
+        v = verts.to(device, torch.float32).expand(plan.batch, -1, -1) if static_mesh else verts[idx].to(device, torch.float32, non_blocking=True)
+        return G.synthesis(w, c, v, noise_mode=noise_mode, **_shard_sampler(plan, k, idx, seed, sampler_noise))
+    return _gather_frames(plan, step, 'image', G.img_resolution, device, out)
+
+
+def reenact_frames_sharded(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=0,
+                           sampler_noise=None, image_mode='image', out=None, device=None, prefetch_depth=8, workers=4):
+    """reenact_frames over the GPUs of a box (one process per GPU, as render_frames_sharded): every rank computes the frame schedule
+    (reenact_schedule, or the pack's cameras), parses -- or reads from the memory-mapped `.n3dpack` -- only the meshes of its own
+    contiguous frame range, and renders them in batches; for noise_mode 'const' / 'none' its first batch caches the ws-only backbones
+    and the later ones reuse them.  The uint8 frames are gathered to rank 0 as in render_frames_sharded.
+    -> [F, H, W, 3] uint8 host tensor on rank 0 (F = the schedule's frame count; H = W = G.img_resolution for 'image', the neural
+    rendering resolution for 'image_raw' / 'image_depth'), None elsewhere.  `sampler_noise` rows are indexed by the global frame id;
+    image_mode and `batch` as in reenact_frames / render_frames_sharded."""
+    device = device or next(G.parameters()).device
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers)
+    plan = shard_plan(n, batch)
+    wsd = ws.detach().to(device, torch.float32).reshape(1, *ws.shape[-2:]).expand(plan.batch, -1, -1)
+    reuse = noise_mode in ('const', 'none')
+    mesh = None
+    if n > 0:
+        first = plan.frames(0)[0]                                          # a rank without frames repeats the previous rank's last
+        mesh = _InOrder(frames(first, max(plan.spans[plan.rank][1], first + 1)), first)
+
+    def step(k, idx):
+        c = cams[idx].to(device, torch.float32, non_blocking=True)
+        v = mesh.take(idx).to(device, torch.float32, non_blocking=True)
+        kw = _shard_sampler(plan, k, idx, seed, sampler_noise)
+        if reuse:
+            kw['use_cached_backbone' if k else 'cache_backbone'] = True
+        return G.synthesis(wsd, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw)
+    return _gather_frames(plan, step, image_mode, _frame_resolution(G, image_mode), device, out)
+
+
+def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None, device=None):
+    """render_orbit over the GPUs of a box: every rank computes the head's planes once (ws [1, L, D], mesh verts [1, V, 3]) and
+    renders its contiguous range of the cameras cams [F, 25] with G.render_views; the frames are gathered to rank 0 as in
+    render_frames_sharded.  -> [F, H, W, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the
+    global frame id."""
+    device = device or next(G.parameters()).device
+    plan = shard_plan(cams.shape[0], batch)
+    G.synthesis(ws.to(device, torch.float32), cams[:1].to(device, torch.float32), verts.to(device, torch.float32), noise_mode='const',
+                cache_backbone=True, seed=0)
+
+    def step(k, idx):
+        return G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device),
+                              **_shard_sampler(plan, k, idx, seed, sampler_noise))
+    return _gather_frames(plan, step, image_mode, _frame_resolution(G, image_mode), device, out)
+
+
+class ShardPlan(NamedTuple):
+    """How F frames are split over the ranks of the sharded drivers: rank r owns spans[r] = shard_range(F, r, world) and renders it
+    in `steps` batches of `batch` frames; every rank runs the same number of steps (one collective each)."""
+    rank: int
+    world: int
+    spans: list
+    batch: int
+    steps: int
+
+    def frames(self, k):
+        """Global frame ids of this rank's batch k; a short tail repeats the last frame (one graph shape)."""
+        a, b = self.spans[self.rank]
+        lo = min(a + k * self.batch, max(b - 1, a))
+        return [min(lo + j, b - 1) for j in range(self.batch)]
+
+
+def shard_plan(F, batch):
+    """The ShardPlan of F frames for this process's rank in the current torch.distributed world (world 1 when uninitialised).
+    `batch` is an upper bound: the batch is the size in [batch/2, batch] that pads the largest rank's frame count least."""
     import torch.distributed as dist
     from . import distributed as D
-    device = device or next(G.parameters()).device
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
-    F = ws_frames.shape[0]
     spans = [D.shard_range(F, r, world) for r in range(world)]
-    a, b = spans[rank]
     nmax = max(e - s for s, e in spans)
     batch = min(range(max(1, batch // 2), batch + 1), key=lambda bb: (-(-nmax // bb) * bb, -bb))     # least padding, then the largest
-    steps = -(-nmax // batch)                                             # every rank runs the same number of collective steps
-    res = G.img_resolution
+    return ShardPlan(rank, world, spans, batch, -(-nmax // batch))
+
+
+def _shard_sampler(plan, k, idx, seed, sampler_noise):
+    """Sampler keywords of batch k of a sharded driver: the frames' global rows of sampler_noise, else seed + rank * steps + k."""
+    if sampler_noise is not None:
+        return {'sampler_noise': _noise_rows(sampler_noise, idx)}
+    return {'seed': int(seed) + plan.rank * plan.steps + k}
+
+
+def _frame_resolution(G, image_mode):
+    return G.img_resolution if image_mode == 'image' else G.neural_rendering_resolution
+
+
+class _InOrder:
+    """Meshes of consecutive frames first, first + 1, ... from an in-order iterable of [1, V, 3] tensors, looked up by frame id as the
+    sharded batches advance (each id is read once; ids behind the current batch are dropped)."""
+
+    def __init__(self, frames, first):
+        self.it, self.next, self.have = iter(frames), first, {}
+
+    def take(self, idx):
+        while self.next <= max(idx):
+            self.have[self.next] = next(self.it)
+            self.next += 1
+        self.have = {i: t for i, t in self.have.items() if i >= min(idx)}
+        return torch.cat([self.have[i] for i in idx], 0)
+
+
+def _gather_frames(plan, step, image_mode, res, device, out):
+    """The loop of the sharded drivers: for k in range(plan.steps), step(k, plan.frames(k)) renders this rank's batch k and returns the
+    generator's output dict; its uint8 frames go to a ping-pong staging buffer, are gathered to rank 0 over NCCL on a side stream
+    (world > 1) and copied to pinned host memory on a third stream, so the next batch renders while this one is in flight.
+    -> [F, res, res, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere.  It is filled in stream order: the caller's
+    current stream waits for the last copy, so synchronise that stream before reading the frames (back-to-back clips do not stall)."""
+    import torch.distributed as dist
+    rank, world, spans, batch = plan.rank, plan.world, plan.spans, plan.batch
     host = None
     if rank == 0:
-        host = out if out is not None else torch.empty(F, res, res, 3, dtype=torch.uint8).pin_memory()
+        host = out if out is not None else torch.empty(spans[-1][1], res, res, 3, dtype=torch.uint8).pin_memory()
     main = torch.cuda.current_stream(device)
     side, copy_s = torch.cuda.Stream(device), torch.cuda.Stream(device)
     stage = [torch.empty(batch, res, res, 3, dtype=torch.uint8, device=device) for _ in range(2)]
     gath = [torch.empty(world, batch, res, res, 3, dtype=torch.uint8, device=device) if rank == 0 and world > 1 else None for _ in range(2)]
     drained = [None, None]
-    static_mesh = verts.shape[0] == 1
-    for k in range(steps):
-        lo = min(a + k * batch, max(b - 1, a))
-        idx = [min(lo + j, b - 1) for j in range(batch)]                   # the tail repeats the last frame (one graph shape)
-        w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
-        c = cams[idx].to(device, torch.float32, non_blocking=True)
-        v = verts.to(device, torch.float32).expand(batch, -1, -1) if static_mesh else verts[idx].to(device, torch.float32, non_blocking=True)
-        img = G.synthesis(w, c, v, noise_mode=noise_mode, seed=int(seed) + rank * steps + k)['image']
+    for k in range(plan.steps):
+        result = step(k, plan.frames(k))
         s = k & 1
         if drained[s] is not None:
             main.wait_event(drained[s])                                    # batch k-2 has left this staging buffer
-        stage[s].copy_(to_uint8_hwc(img))
+        stage[s].copy_(_frames_u8(result, image_mode))
         side.wait_stream(main)
         with torch.cuda.stream(side):
             if world > 1:

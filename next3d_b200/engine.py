@@ -82,6 +82,7 @@ class Engine:
         mask = torch.ones(1, 1, 256, 256) if uv_face_mask is None else uv_face_mask
         self.eye_mask = mask.reshape(mask.shape[-2], mask.shape[-1]).to(self.device, torch.float32).contiguous()
         self._mm_init = torch.tensor([float('inf'), 0.0], device=self.device)
+        self._mm_init_image = torch.tensor([[float('inf'), float('-inf')]], device=self.device)     # one pair per image: repeat(N, 1)
         self._graphs = {}                       # key[0]: the graph reads or writes the backbone cache
         self._cache = None                      # backbone cache (synthesis with cache_backbone=True), see _cache_buffers
         self._side = None                      # side streams of the concurrent branches (compute_planes)
@@ -630,22 +631,24 @@ class Engine:
         return planes
 
     def synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
-                  return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False):
+                  return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False, depth_range='batch'):
         """cache_backbone: also keep the backbone outputs, planes and ws (see _cache_buffers); use_cached_backbone: take the two
-        ws-only backbones from that cache (a cache of another batch size raises; no cache = computed as usual)."""
+        ws-only backbones from that cache (a cache of another batch size raises; no cache = computed as usual).  depth_range: 'batch'
+        clamps every image's depth to the range of the whole call (ray_marcher.py:54 on a batch), 'image' to the image's own range
+        (what a call per image gives)."""
         self._on_device(ws=ws, c=c, v=v)
         with torch.cuda.device(self.device):
             return self._synthesis(ws, c, v, noise_mode, neural_rendering_resolution, sampler_noise, seed, return_intermediates, seed_ptr,
-                                   cache_backbone, use_cached_backbone)
+                                   cache_backbone, use_cached_backbone, _depth_range(depth_range))
 
     def _synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
-                   return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False):
+                   return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False, depth_range='batch'):
         R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
         n0 = K.launches
         self.conv_flops = 0.0
         out = self._compute_planes(ws, v, noise_mode, return_intermediates, cache_backbone, use_cached_backbone)
         planes, inter = out if return_intermediates else (out, None)
-        result, feat, wsum, ws_normals = self._render(planes, c, R, sampler_noise, seed, seed_ptr)
+        result, feat, wsum, ws_normals = self._render(planes, c, R, sampler_noise, seed, seed_ptr, depth_range=depth_range)
         self.launches = K.launches - n0
         if return_intermediates:
             inter.update(planes=planes, feature_image=feat, weights_sum=wsum)
@@ -654,9 +657,10 @@ class Engine:
             result['intermediates'] = inter
         return result
 
-    def _render(self, planes, c, R, sampler_noise, seed, seed_ptr, views=1):
+    def _render(self, planes, c, R, sampler_noise, seed, seed_ptr, views=1, depth_range='batch'):
         """Volume rendering, depth clamp and super-resolution of N = planes.shape[0] * views images (image n reads plane set
-        n // views) with the current batch's styles -> (synthesis output dict, feature image, weight sums, normal workspace)."""
+        n // views) with the current batch's styles -> (synthesis output dict, feature image, weight sums, normal workspace).
+        depth_range 'image': one (min, max) pair per image, each image clamped to its own."""
         cfg, dev = self.cfg, self.device
         N = planes.shape[0] * views
         c = c.to(torch.float32)
@@ -666,7 +670,11 @@ class Engine:
         feat = self._f32(N, R, R, cfg.plane_ch)                                 # [N, M, 32] == NHWC feature image
         depth = self._f32(N, 1, R, R)
         wsum = self._f32(N, M)
-        mm = self._mm_init.clone()                                          # running (min, max) of all sample depths
+        per_image = int(depth_range == 'image')
+        if per_image:                                                       # running (min, max) of each image's sample depths
+            mm = self._mm_init_image.repeat(N, 1)
+        else:
+            mm = self._mm_init.clone()                                      # running (min, max) of all sample depths
         u_c, u_f = sampler_noise if sampler_noise is not None else (None, None)
         if u_c is not None:
             u_c, u_f = u_c.to(dev, torch.float32).contiguous(), u_f.to(dev, torch.float32).contiguous()
@@ -675,13 +683,16 @@ class Engine:
         ev = self._prof_begin()
         if normal is None:
             K.render_rays(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, u_coarse=u_c, u_fine=u_f, seed=seed, seed_ptr=seed_ptr,
-                          views=views)
+                          views=views, depth_range_per_image=per_image)
         else:                                                               # return_normal (renderer.py:271-355, ray_marcher.py:61-64)
             ws_normals = self._f32(K.normals_workspace_floats(N, R, self.rk))
             K.render_rays_normals(planes, cam, intr, R, self.rk, self.dec, feat, depth, wsum, mm, normal, ws_normals, u_coarse=u_c, u_fine=u_f,
-                                  seed=seed, seed_ptr=seed_ptr, views=views)
+                                  seed=seed, seed_ptr=seed_ptr, views=views, depth_range_per_image=per_image)
         self._prof_end(ev, 'render_rays')
-        K.depth_clamp(depth, mm)
+        if per_image:
+            K.depth_clamp_images(depth, mm)
+        else:
+            K.depth_clamp(depth, mm)
         image = self._f32(N, 3, cfg.img_resolution, cfg.img_resolution)
         self._superresolution(feat, self.rk['superresolution_noise_mode'], image)
         result = {'image': image, 'image_raw': feat.permute(0, 3, 1, 2)[:, :3], 'image_depth': depth}
@@ -689,21 +700,22 @@ class Engine:
             result['image_normal'] = normal.view(N, R, R, 3).permute(0, 3, 1, 2)          # ray m = i * R + j -> pixel (i, j)
         return result, feat, wsum, ws_normals
 
-    def render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None):
+    def render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None, depth_range='batch'):
         """New camera views of the cached heads: c [N, 25] with N = B * V for a cache of batch B; view n belongs to head n // V.
-        Renders from the cached planes and runs super-resolution with the cached ws; returns what synthesis returns."""
+        Renders from the cached planes and runs super-resolution with the cached ws; returns what synthesis returns (depth_range as
+        there: 'image' gives every view its own depth range)."""
         self._on_device(c=c)
         with torch.cuda.device(self.device):
-            return self._render_views(c, neural_rendering_resolution, sampler_noise, seed, seed_ptr)
+            return self._render_views(c, neural_rendering_resolution, sampler_noise, seed, seed_ptr, _depth_range(depth_range))
 
-    def _render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None):
+    def _render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None, depth_range='batch'):
         cache, V = self._views_cache(c.shape[0])
         R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
         n0 = K.launches
         self.conv_flops = 0.0
         ws = cache['ws']
         self._set_styles(ws[:, None].expand(ws.shape[0], V, *ws.shape[1:]).reshape(-1, *ws.shape[1:]))     # ws of head n // V
-        result = self._render(cache['planes'], c, R, sampler_noise, seed, seed_ptr, views=V)[0]
+        result = self._render(cache['planes'], c, R, sampler_noise, seed, seed_ptr, views=V, depth_range=depth_range)[0]
         self.launches = K.launches - n0
         return result
 
@@ -742,12 +754,13 @@ class Engine:
         return out
 
     def synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
-                          use_cached_backbone=False):
+                          use_cached_backbone=False, depth_range='batch'):
         with torch.cuda.device(self.device):
-            return self._synthesis_graphed(ws, c, v, noise_mode, neural_rendering_resolution, seed, cache_backbone, use_cached_backbone)
+            return self._synthesis_graphed(ws, c, v, noise_mode, neural_rendering_resolution, seed, cache_backbone, use_cached_backbone,
+                                           _depth_range(depth_range))
 
     def _synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
-                           use_cached_backbone=False):
+                           use_cached_backbone=False, depth_range='batch'):
         """Same as synthesis() (in-kernel sampler RNG) but the ~200 launches of one forward are captured once per
         (batch, resolution, noise_mode, cache use) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
         leaves the GPU idle between kernels.  The cache-using graphs read and write the engine's cache buffers in place."""
@@ -757,21 +770,30 @@ class Engine:
         reuse = use_cached_backbone and self._cached(N, 'use_cached_backbone') is not None
         if cache_backbone:
             self._cache_buffers(N, ws.shape)              # allocated before capture: the graph writes the cache at fixed addresses
-        key = (cache_backbone or reuse, cache_backbone, reuse, N, noise_mode, tuple(v.shape)) + self._render_key(R)
+        key = (cache_backbone or reuse, cache_backbone, reuse, N, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
 
         def run(st):
             return self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,
-                                   use_cached_backbone=reuse)
+                                   use_cached_backbone=reuse, depth_range=depth_range)
         out = self._replay(key, dict(ws=ws, c=c, v=v), run, seed)
         if cache_backbone and not reuse:
             self._cache['noise_mode'] = noise_mode
         return out
 
-    def render_views_graphed(self, c, neural_rendering_resolution=None, seed=0):
-        """render_views() replayed from a CUDA graph per (N, V, resolution, rendering options); in-kernel sampler RNG."""
+    def render_views_graphed(self, c, neural_rendering_resolution=None, seed=0, depth_range='batch'):
+        """render_views() replayed from a CUDA graph per (N, V, resolution, depth range, rendering options); in-kernel sampler RNG."""
         self._on_device(c=c)
+        depth_range = _depth_range(depth_range)
         with torch.cuda.device(self.device):
             _, V = self._views_cache(c.shape[0])
             R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-            key = (True, 'views', c.shape[0], V) + self._render_key(R)
-            return self._replay(key, dict(c=c), lambda st: self._render_views(st['c'], R, seed=0, seed_ptr=st['seed']), seed)
+            key = (True, 'views', c.shape[0], V, depth_range) + self._render_key(R)
+            return self._replay(key, dict(c=c), lambda st: self._render_views(st['c'], R, seed=0, seed_ptr=st['seed'], depth_range=depth_range),
+                                seed)
+
+
+def _depth_range(depth_range):
+    """The `depth_range` keyword: 'batch' (one depth range per call) or 'image' (one per image)."""
+    if depth_range not in ('batch', 'image'):
+        raise ValueError(f"depth_range must be 'batch' or 'image', got {depth_range!r}")
+    return depth_range

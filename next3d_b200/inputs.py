@@ -8,6 +8,7 @@ Also here: the `dataset.json` camera labels of the reenactment script (reenact_a
 pack (all meshes + cameras of a driving sequence in one memory-mappable file) so that a clip is parsed once, not per run.
 """
 import concurrent.futures
+import copy
 import ctypes as C
 import json
 import os
@@ -133,7 +134,8 @@ def write_frame_pack(path, verts, cams, ids=None):
 
 class FramePack:
     """Memory-mapped reader of write_frame_pack files: `.verts` [F, V, 3], `.cams` [F, 25] (numpy memmaps), `.ids`;
-    iterating yields pinned `[1, V, 3]` tensors in order (drop-in for FramePrefetcher in drivers.render_frames)."""
+    iterating yields pinned `[1, V, 3]` tensors in order (drop-in for FramePrefetcher in drivers.render_frames); `pack[a:b]` is
+    the same reader over frames a .. b-1 (one rank's share of a clip)."""
 
     def __init__(self, path, pin=None):
         with open(path, 'rb') as f:
@@ -150,6 +152,15 @@ class FramePack:
 
     def __len__(self):
         return self.verts.shape[0]
+
+    def __getitem__(self, frames):
+        """pack[a:b]: the frames a .. b-1 as a FramePack over the same mapping (nothing is read until iterated)."""
+        if not isinstance(frames, slice) or frames.step not in (None, 1):
+            raise TypeError('FramePack supports contiguous slices only (pack[a:b])')
+        view = copy.copy(self)
+        view.verts, view.cams = self.verts[frames], self.cams[frames]
+        view.ids = self.ids[frames] if self.ids is not None else None
+        return view
 
     def __iter__(self):
         for i in range(len(self)):

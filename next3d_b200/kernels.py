@@ -221,7 +221,8 @@ def _render_desc(planes, cam2world, intrinsics, res, opts, seed, views=1):
     return p
 
 
-def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr, views=1):
+def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr, views=1,
+                      depth_range_per_image=0):
     """Render descriptor of n3d_render_rays / n3d_render_rays_normals, after rejecting the rendering options the renderer lacks."""
     unsupported = [k for k, bad in (('disparity_space_sampling', bool(opts.get('disparity_space_sampling', False))),
                                     ('density_noise', float(opts.get('density_noise', 0) or 0) > 0),
@@ -235,17 +236,19 @@ def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth,
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
     p.rgb, p.depth, p.wsum, p.depth_minmax = ptr(rgb), ptr(depth), ptr(wsum), ptr(depth_minmax)
     p.white_back = int(bool(opts.get('white_back', False)))
+    p.depth_range_per_image = depth_range_per_image
     return p
 
 
 def render_rays(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse=None, u_fine=None, seed=0,
-                seed_ptr=None, views=1):
+                seed_ptr=None, views=1, depth_range_per_image=0):
     """planes [B,3,PH,PW,32] channels-last; dec = (w0 [64,32], b0 [64], w1 [33,64], b1 [33]) with gains folded in.
     opts['depth_resolution'] (4 .. 192) and opts['depth_resolution_importance'] (0 = coarse only .. 192) are samples per pass; a
     count above 192 raises (code -2, unsupported).  views: camera views per plane set -- N = B * views images, image n reads plane
-    set n // views; cameras, uniforms and outputs are per image."""
+    set n // views; cameras, uniforms and outputs are per image.  depth_range_per_image=1: depth_minmax is [N, 2] (each pair
+    initialised to (+inf, -inf)) and pair n covers image n's samples only; 0: depth_minmax [2] covers the launch."""
     p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr,
-                          views)
+                          views, depth_range_per_image)
     _run('n3d_render_rays', C.byref(p), stream_ptr())
 
 
@@ -256,12 +259,13 @@ def normals_workspace_floats(N, res, opts):
 
 
 def render_rays_normals(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, normal, workspace=None, u_coarse=None,
-                        u_fine=None, seed=0, seed_ptr=None, views=1):
+                        u_fine=None, seed=0, seed_ptr=None, views=1, depth_range_per_image=0):
     """render_rays (same outputs, bit for bit) plus normal [N, M, 3]: unit world-space normals -grad sigma composited with the final
     weights (rendering option return_normal).  workspace: fp32 device buffer of normals_workspace_floats() floats, or None to
-    allocate one here.  Same sample-count limits and `views` as render_rays (N = planes.shape[0] * views images)."""
+    allocate one here.  Same sample-count limits, `views` and `depth_range_per_image` as render_rays (N = planes.shape[0] * views
+    images)."""
     p = _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr,
-                          views)
+                          views, depth_range_per_image)
     n_ws = normals_workspace_floats(p.N, res, opts)
     if workspace is None:
         workspace = torch.empty(n_ws, dtype=torch.float32, device=planes.device)
@@ -283,6 +287,15 @@ def render_normals_pass(planes, cam2world, intrinsics, res, opts, dec, normal, w
 
 def depth_clamp(depth, depth_minmax):
     _run('n3d_depth_clamp', ptr(depth), depth.numel(), ptr(depth_minmax), stream_ptr())
+
+
+def depth_clamp_images(depth, depth_minmax):
+    """Clamp image n of depth [N, ...] to its own range depth_minmax[n] of depth_minmax [N, 2] (render_rays with
+    depth_range_per_image=1)."""
+    N = depth.shape[0]
+    if depth_minmax.numel() != 2 * N:
+        raise RuntimeError(f'depth_clamp_images: depth_minmax must be [{N}, 2], got {tuple(depth_minmax.shape)}')
+    _run('n3d_depth_clamp_images', ptr(depth), N, depth.numel() // max(N, 1), ptr(depth_minmax), stream_ptr())
 
 
 def sample_points(planes, coords, box_warp, dec, sigma, rgb=None):

@@ -185,7 +185,7 @@ class TriPlaneGenerator(torch.nn.Module):
         return x
 
     def synthesis(self, ws, c, v, neural_rendering_resolution=None, update_emas=False, cache_backbone=False, use_cached_backbone=False,
-                  sampler_noise=None, seed=None, **synthesis_kwargs):
+                  sampler_noise=None, seed=None, depth_range='batch', **synthesis_kwargs):
         """-> {'image': [N,3,R,R], 'image_raw': [N,3,r,r], 'image_depth': [N,1,r,r]} (triplane_next3d.py:117-188).
         Extra keyword `sampler_noise=(u_coarse [N,M,Dc,1], u_fine [N*M,Df])` injects the stratified / importance sampling
         uniforms (parity tests); by default the renderer draws them from an in-kernel counter RNG seeded per call.
@@ -194,12 +194,15 @@ class TriPlaneGenerator(torch.nn.Module):
         `cache_backbone=True` also keeps this call's ws-only backbone outputs, blended planes, ws and noise_mode until the next caching
         call or a weight change; `use_cached_backbone=True` takes the two ws-only backbones from that cache and re-runs everything
         that depends on the mesh (triplane.py:120-128 of EG3D; a cache of another batch size raises, no cache computes them), and
-        `render_views` renders new cameras from the cached planes."""
+        `render_views` renders new cameras from the cached planes.
+        Extra keyword `depth_range`: 'batch' (default, the reference's semantics for a batched call) clamps every image's depth to the
+        range of all the call's samples (ray_marcher.py:54); 'image' clamps each image to its own range, so 'image_depth' of a batch
+        equals that of one call per image (the reference's scripts render one frame per call)."""
         neural_rendering_resolution = self._rendering_resolution(neural_rendering_resolution)
         noise_mode = synthesis_kwargs.get('noise_mode', 'random')
         seed = self._sampler_seed(seed, sampler_noise)
         eng = self._get_engine()
-        flags = dict(cache_backbone=bool(cache_backbone), use_cached_backbone=bool(use_cached_backbone))
+        flags = dict(cache_backbone=bool(cache_backbone), use_cached_backbone=bool(use_cached_backbone), depth_range=depth_range)
         if self.use_cuda_graph and sampler_noise is None and not synthesis_kwargs.get('return_intermediates', False):
             return eng.synthesis_graphed(ws, c, v, noise_mode=noise_mode, neural_rendering_resolution=neural_rendering_resolution, seed=seed,
                                          **flags)
@@ -207,17 +210,19 @@ class TriPlaneGenerator(torch.nn.Module):
                              sampler_noise=sampler_noise, seed=seed, return_intermediates=synthesis_kwargs.get('return_intermediates', False),
                              **flags)
 
-    def render_views(self, c, neural_rendering_resolution=None, seed=None, sampler_noise=None):
+    def render_views(self, c, neural_rendering_resolution=None, seed=None, sampler_noise=None, depth_range='batch'):
         """New camera views of the heads cached by `synthesis(..., cache_backbone=True)` with batch B, without regenerating them:
         c [N, 25] with N = B * V, view n belongs to head n // V -> the dict `synthesis` returns, for N images.  Renders the cached
         planes and runs super-resolution with the cached ws (the backbones' noise_mode is the caching call's; SR noise follows
-        rendering_kwargs['superresolution_noise_mode']).  Raises RuntimeError when nothing is cached or B does not divide N."""
+        rendering_kwargs['superresolution_noise_mode']).  `depth_range` as in `synthesis`.  Raises RuntimeError when nothing is cached
+        or B does not divide N."""
         neural_rendering_resolution = self._rendering_resolution(neural_rendering_resolution)
         seed = self._sampler_seed(seed, sampler_noise)
         eng = self._get_engine()
         if self.use_cuda_graph and sampler_noise is None:
-            return eng.render_views_graphed(c, neural_rendering_resolution=neural_rendering_resolution, seed=seed)
-        return eng.render_views(c, neural_rendering_resolution=neural_rendering_resolution, sampler_noise=sampler_noise, seed=seed)
+            return eng.render_views_graphed(c, neural_rendering_resolution=neural_rendering_resolution, seed=seed, depth_range=depth_range)
+        return eng.render_views(c, neural_rendering_resolution=neural_rendering_resolution, sampler_noise=sampler_noise, seed=seed,
+                                depth_range=depth_range)
 
     def _rendering_resolution(self, r):
         if r is None:
