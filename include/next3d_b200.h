@@ -240,8 +240,9 @@ int n3d_blend_planes(const float* blended_front, const float* tex_planes, const 
  * sort-merge + alpha compositing in one kernel per ray batch (ray_sampler.py:24-63, renderer.py:95-268,
  * triplane_next3d.py:348-371, ray_marcher.py:27-66).
  * ---------------------------------------------------------------------------------------------------------- */
+/* Alignment: planes must be 32-byte aligned (each texel's 32 channels are read as 256-bit loads), else N3D_ERR_INVALID_ARG. */
 typedef struct {
-    const float* planes;       /* [N,3,PH,PW,32] channels-last fp32 */
+    const float* planes;       /* [N,3,PH,PW,32] channels-last fp32, 32-byte aligned */
     int32_t N, PH, PW;
     const float* cam2world;    /* [N,16] */
     const float* intrinsics;   /* [N,9]  */
@@ -267,6 +268,9 @@ typedef struct {
                                   [N, 2], pair n reduced over image n's samples only (each pair initialised to +inf / -inf by the
                                   caller; with views = V the pair is the image's, not the plane set's), as when every image is rendered
                                   by a launch of its own.  Any other value -> N3D_ERR_INVALID_ARG. */
+    double ray_span;           /* ray_end - ray_start as the caller holds them (double), or 0 = the difference of the float fields.  The
+                                  coarse jitter spacing is ray_span / (depth_coarse - 1) rounded to float, as renderer.py:204 forms it
+                                  from Python floats; the float endpoints are each off by up to half an ulp, 1.7e-4 of a 1e-3 interval. */
 } N3DRender;
 
 int n3d_render_rays(const N3DRender* p, void* stream);
@@ -293,7 +297,8 @@ int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* st
 /* the same clamp per image (depth_range_per_image = 1): depth [N, per_image] elements of image n clamped to depth_minmax[n] of
  * depth_minmax [N, 2].  N >= 0, per_image >= 0, non-null pointers; otherwise N3D_ERR_INVALID_ARG. */
 int n3d_depth_clamp_images(float* depth, int N, int64_t per_image, const float* depth_minmax, void* stream);
-/* run_model only (TriPlaneGenerator.sample, triplane_next3d.py:276): coords [N,P,3] -> sigma [N,P], rgb [N,P,32] (or NULL). */
+/* run_model only (TriPlaneGenerator.sample, triplane_next3d.py:276): coords [N,P,3] -> sigma [N,P], rgb [N,P,32] (or NULL).
+ * planes must be 32-byte aligned (256-bit texel loads) and rgb 8-byte aligned (float2 stores), else N3D_ERR_INVALID_ARG. */
 int n3d_sample_points(const float* planes, int N, int PH, int PW, const float* coords, int64_t P, float box_warp,
                       const float* w0, const float* b0, const float* w1, const float* b1, float* sigma, float* rgb,
                       void* stream);
@@ -302,7 +307,8 @@ int n3d_sample_points(const float* planes, int N, int PH, int PW, const float* c
  * cube_length) for the flat indices head .. head+count-1, coordinates generated in the kernel with the script's own float32
  * operations (no [N^3,3] coordinate tensor), written into sigma_grid [grid_n]^3 at the position the script's
  * flip(dims=[0]) + border trim leaves them; voxels inside the trimmed border (width `pad`, the script's int(30 * N / 256))
- * receive pad_value and are not decoded.  pad = 0: plain flip.  Planes of ONE sample [3,PH,PW,32]. */
+ * receive pad_value and are not decoded.  pad = 0: plain flip.  Planes of ONE sample [3,PH,PW,32], 32-byte aligned (else
+ * N3D_ERR_INVALID_ARG). */
 int n3d_sample_grid(const float* planes, int PH, int PW, int grid_n, float cube_length, float box_warp, int64_t head, int64_t count,
                     int pad, float pad_value, const float* w0, const float* b0, const float* w1, const float* b1, float* sigma_grid,
                     void* stream);

@@ -59,6 +59,7 @@ class Render(C.Structure):
         ('u_coarse', P), ('u_fine', P), ('seed', C.c_uint64), ('seed_ptr', P),
         ('w0', P), ('b0', P), ('w1', P), ('b1', P),
         ('rgb', P), ('depth', P), ('wsum', P), ('depth_minmax', P), ('white_back', I32), ('views', I32), ('depth_range_per_image', I32),
+        ('ray_span', C.c_double),
     ]
 
 

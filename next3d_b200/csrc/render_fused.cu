@@ -1682,7 +1682,8 @@ FusedK make_fused(const N3DRender* p, int& L) {
     K.p = *p;
     K.p.views = plane_views(p);
     K.M = p->res * p->res;
-    K.delta_coarse = (float)(((double)p->ray_end - (double)p->ray_start) / (double)(p->depth_coarse - 1));
+    const double span = p->ray_span > 0.0 ? p->ray_span : (double)p->ray_end - (double)p->ray_start;
+    K.delta_coarse = (float)(span / (double)(p->depth_coarse - 1));
     K.scale = 2.f / p->box_warp;
     K.Tc = (p->depth_coarse + L - 1) / L;
     K.Tf = (p->depth_fine + L - 1) / L;
@@ -1730,6 +1731,7 @@ namespace {
 int check_render(const N3DRender* p, const char* who) {
     N3D_CHECK_ARG(p && p->planes && p->cam2world && p->intrinsics && p->w0 && p->b0 && p->w1 && p->b1 && p->rgb && p->depth && p->wsum,
                   "%s: null pointer", who);
+    N3D_CHECK_ARG(((uintptr_t)p->planes & 31) == 0, "%s: planes must be 32-byte aligned", who);      // 256-bit texel loads
     if (p->depth_coarse > kMaxD || p->depth_fine > kMaxD) {
         n3d_set_error("%s: depth resolutions (%d, %d) above %d samples per pass are not supported", who, p->depth_coarse, p->depth_fine, kMaxD);
         return N3D_ERR_UNSUPPORTED;
@@ -1854,6 +1856,8 @@ extern "C" int n3d_sample_points(const float* planes, int N, int PH, int PW, con
                                  void* stream) {
     N3D_CHECK_ARG(planes && coords && w0 && b0 && w1 && b1 && sigma && N >= 1 && P >= 1 && box_warp > 0.f, "n3d_sample_points: bad args");
     N3D_CHECK_ARG((long long)N * 3 * PH * PW * 128 < (1ll << 32), "n3d_sample_points: plane tensor too large for 32-bit texel offsets");
+    N3D_CHECK_ARG(((uintptr_t)planes & 31) == 0, "n3d_sample_points: planes must be 32-byte aligned");       // 256-bit texel loads
+    N3D_CHECK_ARG(((uintptr_t)rgb & 7) == 0, "n3d_sample_points: rgb must be 8-byte aligned");              // float2 stores
     return launch_points(planes, N, PH, PW, coords, P, box_warp, w0, b0, w1, b1, sigma, rgb, 0, 0.f, 0, 0, 0.f, stream);
 }
 
@@ -1864,6 +1868,7 @@ extern "C" int n3d_sample_grid(const float* planes, int PH, int PW, int grid_n, 
     N3D_CHECK_ARG(head >= 0 && count >= 1 && head + count <= (int64_t)grid_n * grid_n * grid_n, "n3d_sample_grid: index range outside the grid");
     N3D_CHECK_ARG(pad >= 0 && 2 * pad <= grid_n, "n3d_sample_grid: bad trim width");
     N3D_CHECK_ARG((long long)3 * PH * PW * 128 < (1ll << 32), "n3d_sample_grid: plane tensor too large for 32-bit texel offsets");
+    N3D_CHECK_ARG(((uintptr_t)planes & 31) == 0, "n3d_sample_grid: planes must be 32-byte aligned");         // 256-bit texel loads
     return launch_points(planes, 1, PH, PW, nullptr, count, box_warp, w0, b0, w1, b1, sigma_grid, nullptr, grid_n, cube_length, head, pad,
                          pad_value, stream);
 }

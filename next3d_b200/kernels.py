@@ -217,6 +217,7 @@ def _render_desc(planes, cam2world, intrinsics, res, opts, seed, views=1):
     p.cam2world, p.intrinsics, p.res = ptr(cam2world), ptr(intrinsics), res
     p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
     p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
+    p.ray_span = float(opts['ray_end']) - float(opts['ray_start'])        # the jitter spacing's numerator, in double as the reference has it
     p.seed = seed
     return p
 

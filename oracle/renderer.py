@@ -22,12 +22,12 @@ def ray_sampler(cam2world, intrinsics, res):
     fx, fy = intrinsics[:, 0, 0:1], intrinsics[:, 1, 1:2]
     cx, cy = intrinsics[:, 0, 2:3], intrinsics[:, 1, 2:3]
     sk = intrinsics[:, 0, 1:2]
-    idx = torch.arange(res, dtype=torch.float32)
+    idx = torch.arange(res, dtype=cam2world.dtype)            # float32 in the reference; float64 for a high-precision evaluation
     centers = idx * (1.0 / res) + (0.5 / res)
     # ray m = i*res + j: x from column j, y from row i (ray_sampler.py:43-45: meshgrid 'ij', flip(0))
     y_cam = centers[:, None].expand(res, res).reshape(1, -1).expand(N, -1)
     x_cam = centers[None, :].expand(res, res).reshape(1, -1).expand(N, -1)
-    z_cam = torch.ones(N, res * res)
+    z_cam = torch.ones(N, res * res, dtype=cam2world.dtype)
     x_lift = (x_cam - cx + cy * sk / fy - sk * y_cam / fy) / fx * z_cam
     y_lift = (y_cam - cy) / fy * z_cam
     pts = torch.stack([x_lift, y_lift, z_cam, torch.ones_like(z_cam)], -1)
@@ -113,20 +113,21 @@ def sample_importance(z_vals, weights, u_fine):
     N, M, D, _ = z_vals.shape
     z = z_vals.reshape(N * M, D)
     w = weights.reshape(N * M, -1)
-    w = F.max_pool1d(w[:, None].float(), 2, 1, padding=1)
+    w = F.max_pool1d(w[:, None].to(z.dtype), 2, 1, padding=1)
     w = F.avg_pool1d(w, 2, 1).squeeze(1)
     w = w + 0.01
     z_mid = 0.5 * (z[:, :-1] + z[:, 1:])
     return sample_pdf(z_mid, w[:, 1:-1], u_fine).reshape(N, M, u_fine.shape[1], 1)
 
 
-def render(sd, planes, origins, dirs, opts, u_coarse, u_fine):
-    """-> rgb [N,M,32], depth [N,M,1], weight_sum [N,M,1]."""
+def render(sd, planes, origins, dirs, opts, u_coarse, u_fine, return_depths=False):
+    """-> rgb [N,M,32], depth [N,M,1], weight_sum [N,M,1] (+ the sorted sample depths [N,M,D] the composite used, with
+    return_depths).  Runs in the dtype of its inputs: float32 is the reference's arithmetic, float64 a high-precision evaluation."""
     N, M, _ = origins.shape
     Dc = opts['depth_resolution']
     t0, t1 = float(opts['ray_start']), float(opts['ray_end'])
     assert not opts.get('disparity_space_sampling', False)
-    depths_c = torch.linspace(t0, t1, Dc).reshape(1, 1, Dc, 1).repeat(N, M, 1, 1)
+    depths_c = torch.linspace(t0, t1, Dc, dtype=origins.dtype).reshape(1, 1, Dc, 1).repeat(N, M, 1, 1)
     depths_c = depths_c + u_coarse * ((t1 - t0) / (Dc - 1))
     pts = (origins[:, :, None] + depths_c * dirs[:, :, None]).reshape(N, -1, 3)
     rgb_c, sig_c = run_model(sd, planes, pts, opts)
@@ -149,5 +150,8 @@ def render(sd, planes, origins, dirs, opts, u_coarse, u_fine):
         all_s = torch.gather(all_s, -2, idx)
         rgb, depth, w = ray_march(all_c, all_s, all_d, opts)
     else:
+        all_d = depths_c
         rgb, depth, w = ray_march(rgb_c, sig_c, depths_c, opts)
+    if return_depths:
+        return rgb, depth, w.sum(2), all_d[..., 0]
     return rgb, depth, w.sum(2)

@@ -52,3 +52,22 @@ def test_plane_size_limit_counts_plane_sets(entry):
         assert rc == -1 and 'bad ray setup' in msg, (N, views, rc, msg)
     rc, msg = _call(entry, 342, 2, 256, 256)
     assert rc == -1 and '32-bit texel offsets' in msg, (rc, msg)
+
+
+def test_sample_points_plane_size_limit():
+    """n3d_sample_points reads N plane sets with the same 32-bit texel offsets: 171 sets at 256^2 are refused, 170 pass the size
+    check (and are then refused for an rgb buffer that is not 8-byte aligned, which the library checks next, so nothing launches)."""
+    from next3d_b200 import _lib
+    planes = torch.zeros(3 * 4 * 4 * 32)
+    dec = [torch.zeros(n) for n in (64 * 32, 64, 33 * 64, 33)]
+    coords, sigma, rgb = torch.zeros(8 * 3), torch.zeros(8), torch.zeros(8 * 32 + 1)
+
+    def call(N):
+        rc = _lib.lib.n3d_sample_points(planes.data_ptr(), N, 256, 256, coords.data_ptr(), 8, 1.0, *(t.data_ptr() for t in dec),
+                                        sigma.data_ptr(), rgb[1:].data_ptr(), None)
+        return rc, _lib.lib.n3d_last_error().decode()
+
+    rc, msg = call(171)
+    assert rc == -1 and '32-bit texel offsets' in msg, (rc, msg)
+    rc, msg = call(170)
+    assert rc == -1 and 'rgb must be 8-byte aligned' in msg, (rc, msg)
