@@ -282,9 +282,8 @@ int n3d_render_rays(const N3DRender* p, void* stream);
  * and sample-count limits as n3d_render_rays.  Two kernel launches. */
 int n3d_render_rays_normals(const N3DRender* p, float* normal, float* workspace, void* stream);
 /* Diagnostics: the normal pass of n3d_render_rays_normals alone, over the samples an earlier n3d_render_rays_normals call with the
- * same p left in `workspace`; forward = 0 runs the shipped reverse-mode formulation, 1 the forward-mode one (derivative rows through
- * layer 1).  tools/bench_render.py --normals times the two against each other (DESIGN.md section 3.2a). */
-int n3d_render_normals_pass(const N3DRender* p, int forward, const float* workspace, float* normal, void* stream);
+ * same p left in `workspace`.  tools/bench_render.py --normals times it (DESIGN.md section 3.2a). */
+int n3d_render_normals_pass(const N3DRender* p, const float* workspace, float* normal, void* stream);
 /* Diagnostics: micro-kernels that measure the hard per-SM limits of the renderer's formulation on the workload described by p
  * (only planes / cameras / res / depth_* / ray_* / box_warp are read; nothing is written but sink[0], which may be NULL):
  * kind 0 = the tri-plane gather alone (rays, depths, 12 taps per sample, 256-bit loads, weighted sum, bf16 split, shared-memory

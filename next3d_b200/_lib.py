@@ -90,7 +90,7 @@ _SIGNATURES = {
     'n3d_blend_planes': ([P, P, P, P, C.c_int, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_render_rays': ([C.POINTER(Render), P], C.c_int),
     'n3d_render_rays_normals': ([C.POINTER(Render), P, P, P], C.c_int),
-    'n3d_render_normals_pass': ([C.POINTER(Render), C.c_int, P, P, P], C.c_int),
+    'n3d_render_normals_pass': ([C.POINTER(Render), P, P, P], C.c_int),
     'n3d_depth_clamp': ([P, I64, P, P], C.c_int),
     'n3d_depth_clamp_images': ([P, C.c_int, I64, P, P], C.c_int),
     'n3d_sample_points': ([P, C.c_int, C.c_int, C.c_int, P, I64, F32, P, P, P, P, P, P, P], C.c_int),

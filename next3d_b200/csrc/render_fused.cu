@@ -123,28 +123,46 @@ __device__ __forceinline__ float coarse_depth(const FusedK& K, uint64_t seed, lo
 }
 
 // ---------------------------------------------------------------------------------------------------------------- gather warps
-// 12 bilinear taps of one sample (3 planes x 4 corners; plane 0 <- (x,y), 1 <- (x,z), 2 <- (z,y); grid_sample zeros padding,
-// align_corners=False): byte offset of the texel + weight / 3.  Zero-weight taps all point at texel 0.
-__device__ __forceinline__ void setup_taps(uint2* __restrict__ taps, int lane, float px, float py, float pz, bool valid, uint32_t img4, int PH,
-                                           int PW, float scale) {
+// The four bilinear taps of plane pl (0 <- (x, y), 1 <- (x, z), 2 <- (z, y); grid_sample zeros padding, align_corners=False) at
+// the scaled point (x, y, z): texel byte offsets, weights and the derivatives of the weights along the plane's two world axes (a, b)
+// (d ix / d x_a = scale * PW / 2); the 1/3 of the plane mean is folded into all three.  Taps outside the plane and invalid samples
+// get weight 0 and point at texel 0.  The renderer's gather (setup_taps) and the normal pass both take their taps from here, so a
+// sample's feature is the same float expression in both kernels (the gather uses the offsets and weights only).
+struct PlaneTaps {
+    uint32_t off[4];
+    float w[4], wa[4], wb[4];
+};
+__device__ __forceinline__ PlaneTaps plane_taps(int pl, float x, float y, float z, bool valid, uint32_t img4, int PH, int PW, float scale) {
+    PlaneTaps t;
+    const float gx = pl == 2 ? z : x, gy = pl == 1 ? z : y;
+    const float ix = ((gx + 1.f) * (float)PW - 1.f) * 0.5f, iy = ((gy + 1.f) * (float)PH - 1.f) * 0.5f;
+    const float flx = floorf(ix), fly = floorf(iy);
+    const float fx = ix - flx, fy = iy - fly;
+    const int x0 = (int)fminf(fmaxf(flx, -2.f), (float)PW), y0 = (int)fminf(fmaxf(fly, -2.f), (float)PH);
+    const uint32_t pbase = img4 + (uint32_t)(pl * PH * PW) * 128u;
+    const float ka = scale * (float)PW * (0.5f / 3.f), kb = scale * (float)PH * (0.5f / 3.f);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const int xi = x0 + (c & 1), yi = y0 + (c >> 1);
+        const float wx = (c & 1) ? fx : 1.f - fx, wy = (c >> 1) ? fy : 1.f - fy;
+        const bool inside = valid && xi >= 0 && xi < PW && yi >= 0 && yi < PH;
+        t.off[c] = inside ? pbase + (uint32_t)(yi * PW + xi) * 128u : 0u;
+        t.w[c] = inside ? wx * wy * (1.f / 3.f) : 0.f;
+        t.wa[c] = inside ? ((c & 1) ? wy : -wy) * ka : 0.f;
+        t.wb[c] = inside ? ((c >> 1) ? wx : -wx) * kb : 0.f;
+    }
+    return t;
+}
+
+// 12 bilinear taps of one sample (3 planes x 4 corners) into `taps`: byte offset of the texel + weight / 3.
+__device__ __forceinline__ void setup_taps(uint2* __restrict__ taps, int lane, float px, float py, float pz, bool valid, uint32_t img4, int PH, int PW,
+                                           float scale) {
     const float x = scale * px, y = scale * py, z = scale * pz;
 #pragma unroll
     for (int pl = 0; pl < 3; ++pl) {
-        const float gx = pl == 2 ? z : x, gy = pl == 1 ? z : y;
-        const float ix = ((gx + 1.f) * (float)PW - 1.f) * 0.5f, iy = ((gy + 1.f) * (float)PH - 1.f) * 0.5f;
-        const float flx = floorf(ix), fly = floorf(iy);
-        const float fx = ix - flx, fy = iy - fly;
-        const int x0 = (int)fminf(fmaxf(flx, -2.f), (float)PW), y0 = (int)fminf(fmaxf(fly, -2.f), (float)PH);
-        const uint32_t pbase = img4 + (uint32_t)(pl * PH * PW) * 128u;
+        const PlaneTaps t = plane_taps(pl, x, y, z, valid, img4, PH, PW, scale);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const int xi = x0 + (c & 1), yi = y0 + (c >> 1);
-            const float wx = (c & 1) ? fx : 1.f - fx, wy = (c >> 1) ? fy : 1.f - fy;
-            const bool inside = valid && xi >= 0 && xi < PW && yi >= 0 && yi < PH;
-            const float w = inside ? wx * wy * (1.f / 3.f) : 0.f;            // 1/3: mean over the three planes
-            const uint32_t off = inside ? pbase + (uint32_t)(yi * PW + xi) * 128u : 0u;
-            taps[(pl * 4 + c) * 32 + lane] = make_uint2(off, __float_as_uint(w));
-        }
+        for (int c = 0; c < 4; ++c) taps[(pl * 4 + c) * 32 + lane] = make_uint2(t.off[c], __float_as_uint(t.w[c]));
     }
 }
 
@@ -189,59 +207,223 @@ __device__ __forceinline__ void gather_rows(const float* __restrict__ planes, co
 }
 
 // ---------------------------------------------------------------------------------------------------------------- per-ray math
-// A ray's samples live in the L lanes [lane & ~(L-1), +L) of one warp, sample k = t * L + j in register slot t of lane j.
-template <int L>
-__device__ __forceinline__ float seg_next(float v, float v_next_slot, int lane) {      // value of sample k + 1
-    const float a = __shfl_down_sync(FULL, v, 1);
-    const float b = __shfl_sync(FULL, v_next_slot, lane & ~(L - 1));
-    return ((lane & (L - 1)) == L - 1) ? b : a;
-}
-template <int L>
-__device__ __forceinline__ float seg_prev(float v, float v_prev_slot, int lane) {      // value of sample k - 1
-    const float a = __shfl_up_sync(FULL, v, 1);
-    const float b = __shfl_sync(FULL, v_prev_slot, lane | (L - 1));
-    return ((lane & (L - 1)) == 0) ? b : a;
-}
-template <int L>
-__device__ __forceinline__ float seg_sum(float v) {
+// Reduce-scatter of 16 values over the 16 (k32 = false) or 32 lanes of a warp segment: lane ends with the sum of value (lane & 15)
+// in acc[0].
+template <bool k32>
+__device__ __forceinline__ void reduce_scatter16(float (&acc)[16], int lane) {
+    if (k32) {
 #pragma unroll
-    for (int o = L / 2; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    return v;
-}
-template <int L, int NT, bool MUL>
-__device__ __forceinline__ void seg_scan(float (&x)[NT], int lane) {                  // inclusive scan in sample order
-    float carry = MUL ? 1.f : 0.f;
-    const int j = lane & (L - 1);
+        for (int c = 0; c < 16; ++c) acc[c] += __shfl_xor_sync(FULL, acc[c], 16);
+    }
 #pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        float v = x[t];
+    for (int h = 8; h >= 1; h >>= 1) {
+        const bool up = (lane & h) != 0;
 #pragma unroll
-        for (int o = 1; o < L; o <<= 1) {
-            const float up = __shfl_up_sync(FULL, v, o);
-            if (j >= o) v = MUL ? v * up : v + up;
+        for (int c = 0; c < h; ++c) {
+            const float send = up ? acc[c] : acc[c + h];
+            const float keep = up ? acc[c + h] : acc[c];
+            acc[c] = keep + __shfl_xor_sync(FULL, send, h);
         }
-        v = MUL ? v * carry : v + carry;
-        x[t] = v;
-        carry = __shfl_sync(FULL, v, lane | (L - 1));
     }
 }
 
+// RaySeg<L>: the lanes that hold one ray.  Sample k = t * L + j of the ray sits in register slot t of the ray's lane j, and every
+// per-ray step that combines lanes is one of these methods, so the per-ray phases are written once for all three layouts.  Here
+// L = 16 or 32: the L lanes [lane & ~(L-1), +L) of one warp, j = lane & (L - 1); the steps are warp shuffles.
+template <int L>
+struct RaySeg {
+    // Scratch of the warp's kRays rays, in floats of the warp's own area: region A [0, 640) = sd | sg | wb (kRays x (Dt + 2) each),
+    // aliased by the cdf during importance sampling and by the u-bucket tables during ranking; tcs at 640 (kRays x Dc), tfs at 736
+    // (kRays x Df), hist at 832 (kRays x (Dc + 1)).
+    static constexpr int kRays = 32 / L, kTcOff = 640, kTfOff = 736, kHistOff = 832;
+    __device__ __forceinline__ static int area(int warp) { return warp; }
+
+    int lane;
+    __device__ __forceinline__ RaySeg(float*, int, int lane_) : lane(lane_) {}
+
+    // out[t] = value of sample k + 1 (`last` after the final slot)
+    template <int NT>
+    __device__ __forceinline__ void next(const float (&v)[NT], float last, float (&out)[NT]) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            const float a = __shfl_down_sync(FULL, v[t], 1);
+            const float b = __shfl_sync(FULL, t + 1 < NT ? v[t + 1] : last, lane & ~(L - 1));
+            out[t] = ((lane & (L - 1)) == L - 1) ? b : a;
+        }
+    }
+    // out[t] = value of sample k - 1 (`first` before sample 0)
+    template <int NT>
+    __device__ __forceinline__ void prev(const float (&v)[NT], float first, float (&out)[NT]) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            const float a = __shfl_up_sync(FULL, v[t], 1);
+            const float b = __shfl_sync(FULL, t > 0 ? v[t - 1] : first, lane | (L - 1));
+            out[t] = ((lane & (L - 1)) == 0) ? b : a;
+        }
+    }
+    // sum over the ray: the same bits in every lane of it
+    __device__ __forceinline__ float sum(float v) {
+#pragma unroll
+        for (int o = L / 2; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+        return v;
+    }
+    // inclusive scan (product when MUL) in sample order
+    template <bool MUL, int NT>
+    __device__ __forceinline__ void scan(float (&x)[NT]) {
+        float carry = MUL ? 1.f : 0.f;
+        const int j = lane & (L - 1);
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            float v = x[t];
+#pragma unroll
+            for (int o = 1; o < L; o <<= 1) {
+                const float up = __shfl_up_sync(FULL, v, o);
+                if (j >= o) v = MUL ? v * up : v + up;
+            }
+            v = MUL ? v * carry : v + carry;
+            x[t] = v;
+            carry = __shfl_sync(FULL, v, lane | (L - 1));
+        }
+    }
+    // inclusive prefix sum of one integer per lane, in lane order
+    __device__ __forceinline__ int prefix(int v) {
+        const int j = lane & (L - 1);
+#pragma unroll
+        for (int o = 1; o < L; o <<= 1) { const int up = __shfl_up_sync(FULL, v, o); if (j >= o) v += up; }
+        return v;
+    }
+    __device__ __forceinline__ bool any(bool p) { return __any_sync(FULL, p); }
+    __device__ __forceinline__ void sync() { __syncwarp(); }
+    // start of a per-ray phase: nothing to wait for, the ray's lanes finished the previous phase together
+    __device__ __forceinline__ void enter() {}
+    // the value of lane j = 0 (read on j = 0 only)
+    __device__ __forceinline__ float lead(float v) { return __shfl_sync(FULL, v, lane & ~(L - 1)); }
+    // colour reduce-scatter: lane j ends with channel (j & 15) summed over the ray's lanes, in acc[0]
+    __device__ __forceinline__ void reduce16(float (&acc)[16]) { reduce_scatter16<L == 32>(acc, lane); }
+};
+
+// L = 64: the two warps 2r, 2r + 1 of one E set, half h = warp & 1 holding j = 32 h + lane.  The steps that cross the warp boundary
+// exchange a few words through the pair's scratch under the pair's 64-thread named barrier.  Every exchange writes one of two
+// ping-pong buffers and passes the barrier once; a buffer is rewritten only after the partner has passed the next barrier, i.e.
+// after it read the buffer's previous contents.  Each per-ray phase starts at the barrier, so neither warp overwrites scratch its
+// partner still reads.
+template <>
+struct RaySeg<64> {
+    // Scratch of the ray: the pair's two areas, 1920 floats: region A [0, 1160) (3 x 386; 2 x 512 bucket words), tcs at 1160, tfs at
+    // 1352, hist at 1544 (193), the exchange words at 1752 (2 x 32).
+    static constexpr int kRays = 1, kTcOff = 1160, kTfOff = 1352, kHistOff = 1544, kXOff = 1752;
+    __device__ __forceinline__ static int area(int warp) { return warp & ~1; }
+
+    float* words;                // 2 x 32 exchange words
+    int lane, bar, h, ph;        // named barrier id (5 .. 8), warp half, current buffer
+    __device__ __forceinline__ RaySeg(float* es, int warp, int lane_) : words(es + kXOff), lane(lane_), bar(5 + (warp >> 1)), h(warp & 1), ph(0) {}
+
+    __device__ __forceinline__ float* buf() {
+        float* const b = words + 32 * ph;
+        ph ^= 1;
+        return b;
+    }
+    template <int NT>
+    __device__ __forceinline__ void next(const float (&v)[NT], float last, float (&out)[NT]) {
+        float* const b = buf();
+        if (lane == 0) {
+#pragma unroll
+            for (int t = 0; t < NT; ++t) b[8 * h + t] = h ? v[t] : (t + 1 < NT ? v[t + 1] : last);
+        }
+        sync();
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            const float a = __shfl_down_sync(FULL, v[t], 1);
+            out[t] = lane == 31 ? b[8 * (h ^ 1) + t] : a;
+        }
+    }
+    template <int NT>
+    __device__ __forceinline__ void prev(const float (&v)[NT], float first, float (&out)[NT]) {
+        float* const b = buf();
+        if (lane == 31) {
+#pragma unroll
+            for (int t = 0; t < NT; ++t) b[8 * h + t] = h ? (t > 0 ? v[t - 1] : first) : v[t];
+        }
+        sync();
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            const float a = __shfl_up_sync(FULL, v[t], 1);
+            out[t] = lane == 0 ? b[8 * (h ^ 1) + t] : a;
+        }
+    }
+    __device__ __forceinline__ float sum(float v) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+        float* const b = buf();
+        if (lane == 0) b[h] = v;
+        sync();
+        return b[0] + b[1];                                          // same order in both halves: both get the same bits
+    }
+    template <bool MUL, int NT>
+    __device__ __forceinline__ void scan(float (&x)[NT]) {
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            float v = x[t];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float up = __shfl_up_sync(FULL, v, o);
+                if (lane >= o) v = MUL ? v * up : v + up;
+            }
+            x[t] = v;
+        }
+        float* const b = buf();
+        if (lane == 31) {
+#pragma unroll
+            for (int t = 0; t < NT; ++t) b[8 * h + t] = x[t];
+        }
+        sync();
+        float carry = MUL ? 1.f : 0.f;
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+            const float c1 = MUL ? carry * b[t] : carry + b[t];      // carry into half 1 of slot t
+            x[t] = MUL ? x[t] * (h ? c1 : carry) : x[t] + (h ? c1 : carry);
+            carry = MUL ? c1 * b[8 + t] : c1 + b[8 + t];
+        }
+    }
+    __device__ __forceinline__ int prefix(int v) {                  // counts <= 192: exact in fp32
+        float f[1] = {(float)v};
+        scan<false>(f);
+        return (int)f[0];
+    }
+    __device__ __forceinline__ bool any(bool p) {
+        int r;
+        asm volatile("{\n\t.reg .pred a, b;\n\tsetp.ne.s32 a, %1, 0;\n\tbar.red.or.pred b, %2, 64, a;\n\tselp.s32 %0, 1, 0, b;\n\t}"
+                     : "=r"(r) : "r"((int)p), "r"(bar) : "memory");
+        return r != 0;
+    }
+    __device__ __forceinline__ void sync() { asm volatile("bar.sync %0, 64;" ::"r"(bar) : "memory"); }
+    __device__ __forceinline__ void enter() { sync(); }
+    __device__ __forceinline__ float lead(float v) { return v; }     // j = 0 is lane 0 of half 0 itself
+    __device__ __forceinline__ void reduce16(float (&acc)[16]) {
+        reduce_scatter16<true>(acc, lane);
+        float* const b = buf();                                      // half 1's channel sums join half 0's (j = lane < 16)
+        if (h == 1 && lane < 16) b[lane] = acc[0];
+        sync();
+        if (h == 0 && lane < 16) acc[0] += b[lane];
+    }
+};
+
 // MipRayMarcher2 weights (ray_marcher.py:27-46) of a depth-sorted list of `cnt` samples (d, sg):
 //   alpha_k = 1 - exp(-softplus((s_k + s_k+1)/2 - 1) * (t_k+1 - t_k)),  T_k = prod_{i<k} (1 - alpha_i + 1e-10),  w_k = alpha_k T_k
-// w_k = 0 for k >= cnt - 1.  tmid_k = (t_k + t_k+1) / 2.
+// w_k = 0 for k >= cnt - 1.  tmid_k = (t_k + t_k+1) / 2.  j: the lane's index in the ray.
 template <int L, int NT>
-__device__ __forceinline__ void march_weights(const float (&d)[NT], const float (&sg)[NT], int cnt, int lane, float (&w)[NT], float (&tmid)[NT]) {
-    const int j = lane & (L - 1);
-    float fac[NT], al[NT];
+__device__ __forceinline__ void march_weights(RaySeg<L>& seg, const float (&d)[NT], const float (&sg)[NT], int cnt, int j, float (&w)[NT],
+                                              float (&tmid)[NT]) {
+    float dn[NT], sn[NT], fac[NT], al[NT], ex[NT];
+    seg.next(d, 0.f, dn);
+    seg.next(sg, 0.f, sn);
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
-        const float dn = seg_next<L>(d[t], t + 1 < NT ? d[t + 1] : 0.f, lane);
-        const float sn = seg_next<L>(sg[t], t + 1 < NT ? sg[t + 1] : 0.f, lane);
         const int k = t * L + j;
         float alpha = 0.f;
         if (k < cnt - 1) {
-            const float delta = dn - d[t];
-            const float dens = softplus_fast((sg[t] + sn) * 0.5f - 1.f);
+            const float delta = dn[t] - d[t];
+            const float dens = softplus_fast((sg[t] + sn[t]) * 0.5f - 1.f);
             // 1 - exp(-x): the MUFU exponential is ~2e-7 off near 1, a BIAS that adds up over ~190 thin intervals; below 1/16 the
             // alternating series is exact to 1e-8 relative
             const float xx = dens * delta;
@@ -250,122 +432,10 @@ __device__ __forceinline__ void march_weights(const float (&d)[NT], const float 
         }
         al[t] = alpha;
         fac[t] = k < cnt - 1 ? (1.f - alpha + 1e-10f) : 1.f;
-        tmid[t] = (d[t] + dn) * 0.5f;
-    }
-    seg_scan<L, NT, true>(fac, lane);
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        const float ex = seg_prev<L>(fac[t], t > 0 ? fac[t - 1] : 1.f, lane);
-        w[t] = al[t] * ((t == 0 && j == 0) ? 1.f : ex);
-    }
-}
-
-// ---- L = 64: the same steps for a ray held by a warp pair, half h = warp & 1 holding j = 32 h + lane.  Every exchange writes one of
-// two ping-pong buffers and passes the pair's barrier once; a buffer is rewritten only after the partner has passed the next
-// barrier, i.e. after it read the buffer's previous contents.
-struct Pair {
-    float* x;                    // 2 x 32 exchange words in the pair's scratch
-    int bar, h, ph;              // named barrier id (5 .. 8), warp half, current buffer
-};
-__device__ __forceinline__ void pair_sync(const Pair& X) { asm volatile("bar.sync %0, 64;" ::"r"(X.bar) : "memory"); }
-__device__ __forceinline__ float* pair_buf(Pair& X) {
-    float* const b = X.x + 32 * X.ph;
-    X.ph ^= 1;
-    return b;
-}
-__device__ __forceinline__ bool pair_any(const Pair& X, bool p) {
-    int r;
-    asm volatile("{\n\t.reg .pred a, b;\n\tsetp.ne.s32 a, %1, 0;\n\tbar.red.or.pred b, %2, 64, a;\n\tselp.s32 %0, 1, 0, b;\n\t}"
-                 : "=r"(r) : "r"((int)p), "r"(X.bar) : "memory");
-    return r != 0;
-}
-__device__ __forceinline__ float pair_sum(Pair& X, float v, int lane) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    float* const b = pair_buf(X);
-    if (lane == 0) b[X.h] = v;
-    pair_sync(X);
-    return b[0] + b[1];                                              // same order in both halves: both get the same bits
-}
-// out[t] = value of sample k + 1 (`last` after the final slot)
-template <int NT>
-__device__ __forceinline__ void pair_next(Pair& X, const float (&v)[NT], float last, float (&out)[NT], int lane) {
-    float* const b = pair_buf(X);
-    if (lane == 0) {
-#pragma unroll
-        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = X.h ? v[t] : (t + 1 < NT ? v[t + 1] : last);
-    }
-    pair_sync(X);
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        const float a = __shfl_down_sync(FULL, v[t], 1);
-        out[t] = lane == 31 ? b[8 * (X.h ^ 1) + t] : a;
-    }
-}
-// out[t] = value of sample k - 1 (`first` before sample 0)
-template <int NT>
-__device__ __forceinline__ void pair_prev(Pair& X, const float (&v)[NT], float first, float (&out)[NT], int lane) {
-    float* const b = pair_buf(X);
-    if (lane == 31) {
-#pragma unroll
-        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = X.h ? (t > 0 ? v[t - 1] : first) : v[t];
-    }
-    pair_sync(X);
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        const float a = __shfl_up_sync(FULL, v[t], 1);
-        out[t] = lane == 0 ? b[8 * (X.h ^ 1) + t] : a;
-    }
-}
-template <int NT, bool MUL>
-__device__ __forceinline__ void pair_scan(Pair& X, float (&x)[NT], int lane) {                 // inclusive scan in sample order
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        float v = x[t];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const float up = __shfl_up_sync(FULL, v, o);
-            if (lane >= o) v = MUL ? v * up : v + up;
-        }
-        x[t] = v;
-    }
-    float* const b = pair_buf(X);
-    if (lane == 31) {
-#pragma unroll
-        for (int t = 0; t < NT; ++t) b[8 * X.h + t] = x[t];
-    }
-    pair_sync(X);
-    float carry = MUL ? 1.f : 0.f;
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        const float c1 = MUL ? carry * b[t] : carry + b[t];          // carry into half 1 of slot t
-        x[t] = MUL ? x[t] * (X.h ? c1 : carry) : x[t] + (X.h ? c1 : carry);
-        carry = MUL ? c1 * b[8 + t] : c1 + b[8 + t];
-    }
-}
-template <int NT>
-__device__ __forceinline__ void march_weights_pair(Pair& X, const float (&d)[NT], const float (&sg)[NT], int cnt, int lane, float (&w)[NT],
-                                                   float (&tmid)[NT]) {
-    const int j = 32 * X.h + lane;
-    float dn[NT], sn[NT], fac[NT], al[NT];
-    pair_next<NT>(X, d, 0.f, dn, lane);
-    pair_next<NT>(X, sg, 0.f, sn, lane);
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-        const int k = t * 64 + j;
-        float alpha = 0.f;
-        if (k < cnt - 1) {
-            const float xx = softplus_fast((sg[t] + sn[t]) * 0.5f - 1.f) * (dn[t] - d[t]);
-            const float ser = xx * (1.f - xx * (0.5f - xx * (0.16666667f - xx * (0.041666668f - xx * 0.0083333338f))));
-            alpha = xx < 0.0625f ? ser : 1.f - ex2_approx(-kLog2e * xx);             // as march_weights
-        }
-        al[t] = alpha;
-        fac[t] = k < cnt - 1 ? (1.f - alpha + 1e-10f) : 1.f;
         tmid[t] = (d[t] + dn[t]) * 0.5f;
     }
-    pair_scan<NT, true>(X, fac, lane);
-    float ex[NT];
-    pair_prev<NT>(X, fac, 1.f, ex, lane);
+    seg.template scan<true>(fac);
+    seg.prev(fac, 1.f, ex);
 #pragma unroll
     for (int t = 0; t < NT; ++t) w[t] = al[t] * ((t == 0 && j == 0) ? 1.f : ex[t]);
 }
@@ -394,6 +464,18 @@ struct Smem {
     uint8_t* base;
     __device__ __forceinline__ uint32_t bar(int i) const { return smem_u32(base + kOffBar + i * 8); }
 };
+
+// Gather warp: fill rows row0 .. row0 + 31 of A buffer i % kNF (the i-th tile) from the taps the warp just wrote, once the
+// epilogue has freed the buffer, and publish them.
+__device__ __forceinline__ void fill_buffer(const Smem& S, const float* __restrict__ planes, const uint2* __restrict__ taps, int i, int row0,
+                                            int lane) {
+    __syncwarp();
+    const int b = i % kNF;
+    if (i >= kNF) mbar_wait_sleep(S.bar(BAR_FEMPTY + b), (uint32_t)((i / kNF - 1) & 1), 40u);
+    gather_rows(planes, taps, S.base + kOffF + b * 16384, S.base + kOffF + b * 16384 + 8192, row0, lane);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(S.bar(BAR_FFULL + b));
+}
 
 // Decoder weights -> bf16 (hi, lo) B-operand tiles in shared memory, with the activation scalings folded in: layer 1 produces
 // x * log2(e); hidden units are kept as softplus / ln2; colour logits as -(x) * log2(e) (the argument of ex2 in the sigmoid).
@@ -562,7 +644,6 @@ __device__ __forceinline__ void init_pipeline_barriers(const Smem& S) {
 template <int L, bool kExport>
 __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_constant__ FusedK K) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    constexpr int RPW = L == 64 ? 1 : 32 / L;   // rays per scratch area (L = 64: one ray per warp pair, the pair's two areas)
     const N3DRender& P = K.p;
     Smem S;
     S.base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);       // pointer arithmetic keeps the shared address space
@@ -610,12 +691,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             }
             setup_taps(taps, lane, ray.ox + depth * ray.dx, ray.oy + depth * ray.dy, ray.oz + depth * ray.dz, valid, ray.img4, P.PH, P.PW,
                        K.scale);
-            __syncwarp();
-            const int b = ti % kNF;
-            if (ti >= kNF) mbar_wait_sleep(S.bar(BAR_FEMPTY + b), (uint32_t)((ti / kNF - 1) & 1), 40u);
-            gather_rows(P.planes, taps, sb + kOffF + b * 16384, sb + kOffF + b * 16384 + 8192, q * 32, lane);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(S.bar(BAR_FFULL + b));
+            fill_buffer(S, P.planes, taps, ti, q * 32, lane);
         };
         auto tile = [&](int ti, bool fine, int r, int t) {
             while (next_item < ti * 4 + 4) {
@@ -630,23 +706,18 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
     else {
         const int eset = warp >> 2, q = warp & 3;
         const int row = q * 32 + lane, rs = row / L, j = row & (L - 1), rw = lane / L;
-        float* const es = reinterpret_cast<float*>(sb + kOffEscr) + (L == 64 ? (warp & ~1) : warp) * kEscrFloats;
-        // per-warp scratch (floats): region A [0, 640) = sd | sg | wb (RPW x (Dt + 2) each), aliased by the cdf during importance sampling
-        // and by the u-bucket tables during ranking; tcs at 640 (RPW x Dc), tfs at 736 (RPW x Df), hist at 832 (RPW x (Dc + 1)).
-        // L = 64, the pair's 1920 floats: region A [0, 1160) (3 x 386; 2 x 512 bucket words), tcs at 1160, tfs at 1352, hist at
-        // 1544 (193), the pair's exchange words at 1752 (2 x 32).
-        constexpr int kTcOff = L == 64 ? 1160 : 640, kTfOff = L == 64 ? 1352 : 736, kHistOff = L == 64 ? 1544 : 832;
+        using Seg = RaySeg<L>;
+        float* const es = reinterpret_cast<float*>(sb + kOffEscr) + Seg::area(warp) * kEscrFloats;
+        Seg seg(es, warp, lane);
         constexpr int NB = 8 * L;                                   // u-buckets per ray (8 per lane)
         const int strD = Dt + 2;
         float* const s_sd = es + rw * strD;                         // sorted depths
-        float* const s_sg = es + RPW * strD + rw * strD;
-        float* const s_wb = es + 2 * RPW * strD + rw * strD;
+        float* const s_sg = es + Seg::kRays * strD + rw * strD;
+        float* const s_wb = es + 2 * Seg::kRays * strD + rw * strD;
         int* const s_ub = reinterpret_cast<int*>(es) + rw * 2 * NB; // [NB] count | prefix << 8, then [NB] member indices (4 bytes)
-        float* const s_tc = es + kTcOff + rw * Dc;
-        float* const s_tf = es + kTfOff + rw * Df;
-        int* const s_hist = reinterpret_cast<int*>(es + kHistOff) + rw * (Dc + 1);
-        Pair X;                                                     // L = 64 only
-        X.x = es + 1752; X.bar = 5 + (warp >> 1); X.h = warp & 1; X.ph = 0;
+        float* const s_tc = es + Seg::kTcOff + rw * Dc;
+        float* const s_tf = es + Seg::kTfOff + rw * Df;
+        int* const s_hist = reinterpret_cast<int*>(es + Seg::kHistOff) + rw * (Dc + 1);
 
         // state of the group in its fine phase (cur) and of the group in its coarse phase (nxt)
         float cur_tc[kMaxT], cur_sc[kMaxT], cur_tf[kMaxT], cur_sf[kMaxT];
@@ -704,36 +775,24 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
         // ---- coarse weights -> smoothed pdf -> cdf -> inverse-CDF fine depths (renderer.py:209-268) for the group in `nxt`
         auto importance = [&](int r) {
             float w[kMaxT], tm[kMaxT];
-            if constexpr (L == 64) {
-                pair_sync(X);                                       // the partner is done with the scratch of its previous phase
-                march_weights_pair<kMaxT>(X, nxt_tc, nxt_sc, Dc, lane, w, tm);
-            } else {
-                march_weights<L, kMaxT>(nxt_tc, nxt_sc, Dc, lane, w, tm);
-            }
+            seg.enter();
+            march_weights(seg, nxt_tc, nxt_sc, Dc, j, w, tm);
             // max_pool1d(k2,s1,pad1) -> avg_pool1d(k2,s1) -> + 0.01; entries [1:-1] => pdf weights at k = 1 .. Dc-3, + 1e-5
             const int nw = Dc - 3;
-            float c[kMaxT];
+            float c[kMaxT], wp[kMaxT], wn[kMaxT];
             float part = 0.f;
-            float wpv[kMaxT], wnv[kMaxT];
-            if constexpr (L == 64) {
-                pair_prev<kMaxT>(X, w, 0.f, wpv, lane);
-                pair_next<kMaxT>(X, w, 0.f, wnv, lane);
-            }
+            seg.prev(w, 0.f, wp);
+            seg.next(w, 0.f, wn);
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) {
-                const float wp = L == 64 ? wpv[t] : seg_prev<L>(w[t], t > 0 ? w[t - 1] : 0.f, lane);
-                const float wn = L == 64 ? wnv[t] : seg_next<L>(w[t], t + 1 < kMaxT ? w[t + 1] : 0.f, lane);
                 const int k = t * L + j;
-                c[t] = (k >= 1 && k <= nw) ? (fmaxf(wp, w[t]) + fmaxf(w[t], wn)) * 0.5f + 0.01f + 1e-5f : 0.f;
+                c[t] = (k >= 1 && k <= nw) ? (fmaxf(wp[t], w[t]) + fmaxf(w[t], wn[t])) * 0.5f + 0.01f + 1e-5f : 0.f;
                 part += c[t];
             }
-            float total;
-            if constexpr (L == 64) total = pair_sum(X, part, lane);
-            else total = seg_sum<L>(part);
+            const float total = seg.sum(part);
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) c[t] = c[t] / total;
-            if constexpr (L == 64) pair_scan<kMaxT, false>(X, c, lane);
-            else seg_scan<L, kMaxT, false>(c, lane);                // c[t] = cdf[k], k = 0 .. nw
+            seg.template scan<false>(c);                            // c[t] = cdf[k], k = 0 .. nw
             float* const cdf = s_sd;
 #pragma unroll
             for (int t = 0; t < kMaxT; ++t) {
@@ -741,8 +800,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 if (k <= nw) cdf[k] = c[t];
                 if (k < Dc) s_tc[k] = nxt_tc[t];
             }
-            if constexpr (L == 64) pair_sync(X);
-            else __syncwarp();
+            seg.sync();
             float uu[kMaxT];
             int lo[kMaxT], hi[kMaxT];
 #pragma unroll
@@ -791,12 +849,29 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
             float coef_c[kMaxT], coef_f[kMaxT];
             float wsum, dacc;
             float d_first, d_last;
-            // L = 64: the ray's two warps meet at every point where the L <= 32 code needs only its own warp
-            auto ray_sync = [&]() {
-                if constexpr (L == 64) pair_sync(X);
-                else __syncwarp();
+            // the ray's `cnt` depth-sorted samples (depths d, final weights w, interval midpoints tm): export them, sum the weights
+            // and weight x midpoint over the ray, take the first depth
+            auto ray_sums = [&](const auto& d, const auto& w, const auto& tm) {
+                constexpr int NT = sizeof(d) / sizeof(d[0]);
+                if constexpr (kExport) {
+                    if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
+                        float* const out = K.samples + gr * (2 * cnt - 1);
+#pragma unroll
+                        for (int t = 0; t < NT; ++t) {
+                            const int p = t * L + j;
+                            if (p < cnt) out[p] = d[t];
+                            if (p < cnt - 1) out[cnt + p] = w[t];
+                        }
+                    }
+                }
+                float ws = 0.f, da = 0.f;
+#pragma unroll
+                for (int t = 0; t < NT; ++t) { ws += w[t]; da += w[t] * tm[t]; }
+                wsum = seg.sum(ws);
+                dacc = seg.sum(da);
+                d_first = seg.lead(d[0]);                            // read on j == 0 only
             };
-            if constexpr (L == 64) pair_sync(X);                    // the partner is done with the scratch of its previous phase
+            seg.enter();
             if (use_fine) {
                 // stable sort-merge of coarse (sorted) + fine depths by rank (torch.sort of the concatenation, renderer.py:164-182)
 #pragma unroll
@@ -807,10 +882,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     if (k <= Dc) s_hist[k] = 0;
                 }
                 if (j == 0 && L * kMaxT <= Dc) s_hist[Dc] = 0;
-                ray_sync();
+                seg.sync();
                 // zero the u-bucket tables (they alias the sorted arrays, which are written after the ranks are known)
                 for (int i = j; i < 2 * NB; i += L) s_ub[i] = 0;
-                ray_sync();
+                seg.sync();
                 // Rank of a fine sample among the fine ones.  Fine depths are the inverse CDF of iid uniforms u, a monotone map, so the
                 // order of the depths is the order of the u's: bucket the samples by u (NB uniform buckets, ~0.4 samples each), take
                 // the bucket prefix count and order the few members of a bucket by (depth, index).  The number of coarse samples <= v
@@ -837,25 +912,16 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         atomicAdd(&s_hist[c], 1);
                     }
                 }
-                ray_sync();
+                seg.sync();
                 {   // exclusive prefix over the buckets: lane j owns buckets 8j .. 8j+7; count and prefix share a word
                     int cn[8], run = 0;
 #pragma unroll
                     for (int i = 0; i < 8; ++i) { cn[i] = s_ub[8 * j + i]; run += cn[i]; }
-                    int inc = run;
-                    if constexpr (L == 64) {                        // counts <= 192: exact in fp32
-                        float f[1] = {(float)run};
-                        pair_scan<1, false>(X, f, lane);
-                        inc = (int)f[0];
-                    } else {
-#pragma unroll
-                        for (int o = 1; o < L; o <<= 1) { const int up = __shfl_up_sync(FULL, inc, o); if (j >= o) inc += up; }
-                    }
-                    int pre = inc - run;
+                    int pre = seg.prefix(run) - run;
 #pragma unroll
                     for (int i = 0; i < 8; ++i) { s_ub[8 * j + i] = cn[i] | (pre << 8); pre += cn[i]; }
                 }
-                ray_sync();
+                seg.sync();
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
                     const int jf = t * L + j;
@@ -877,10 +943,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         pos_f[t] = cntc[t] + (word >> 8) + within;
                     }
                 }
-                bool crowded;
-                if constexpr (L == 64) crowded = pair_any(X, overflow);
-                else crowded = __any_sync(FULL, overflow);
-                if (crowded) {                                       // a crowded bucket (degenerate u's): full O(Df^2) rank count
+                if (seg.any(overflow)) {                             // a crowded bucket (degenerate u's): full O(Df^2) rank count
 #pragma unroll
                     for (int t = 0; t < kMaxT; ++t) {
                         const int jf = t * L + j;
@@ -892,13 +955,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                         }
                     }
                 }
-                ray_sync();
+                seg.sync();
                 // coarse sample a lands after every fine sample with fewer than a+1 coarse samples <= it: a + #{fine: cnt_c <= a}
                 float hc[kMaxT];
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { const int k = t * L + j; hc[t] = k < Dc ? (float)s_hist[k] : 0.f; }
-                if constexpr (L == 64) pair_scan<kMaxT, false>(X, hc, lane);
-                else seg_scan<L, kMaxT, false>(hc, lane);
+                seg.template scan<false>(hc);
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
                     const int k = t * L + j;
@@ -906,7 +968,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     if (k < Dc) { s_sd[pos_c[t]] = tc[t]; s_sg[pos_c[t]] = sc[t]; }
                     if (k < Df) { s_sd[pos_f[t]] = cur_tf[t]; s_sg[pos_f[t]] = cur_sf[t]; }
                 }
-                ray_sync();
+                seg.sync();
                 float d6[2 * kMaxT], s6[2 * kMaxT], w6[2 * kMaxT], tm6[2 * kMaxT];
 #pragma unroll
                 for (int t = 0; t < 2 * kMaxT; ++t) {
@@ -914,38 +976,15 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     d6[t] = p < cnt ? s_sd[p] : 0.f;
                     s6[t] = p < cnt ? s_sg[p] : 0.f;
                 }
-                if constexpr (L == 64) march_weights_pair<2 * kMaxT>(X, d6, s6, cnt, lane, w6, tm6);
-                else march_weights<L, 2 * kMaxT>(d6, s6, cnt, lane, w6, tm6);
-                if constexpr (kExport) {
-                    if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
-                        float* const out = K.samples + gr * (2 * cnt - 1);
-#pragma unroll
-                        for (int t = 0; t < 2 * kMaxT; ++t) {
-                            const int p = t * L + j;
-                            if (p < cnt) out[p] = d6[t];
-                            if (p < cnt - 1) out[cnt + p] = w6[t];
-                        }
-                    }
-                }
-                float ws = 0.f, da = 0.f;
+                march_weights(seg, d6, s6, cnt, j, w6, tm6);
+                ray_sums(d6, w6, tm6);
                 if (j == 0) s_wb[0] = 0.f;
 #pragma unroll
                 for (int t = 0; t < 2 * kMaxT; ++t) {
                     const int p = t * L + j;
                     if (p < cnt) s_wb[p + 1] = w6[t];
-                    ws += w6[t];
-                    da += w6[t] * tm6[t];
                 }
-                if constexpr (L == 64) {
-                    wsum = pair_sum(X, ws, lane);
-                    dacc = pair_sum(X, da, lane);
-                    d_first = d6[0];                                 // read on j == 0 only
-                } else {
-                    wsum = seg_sum<L>(ws);
-                    dacc = seg_sum<L>(da);
-                    d_first = __shfl_sync(FULL, d6[0], lane & ~(L - 1));
-                }
-                ray_sync();
+                seg.sync();
                 d_last = s_sd[cnt - 1];
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
@@ -954,44 +993,20 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                     coef_f[t] = k < Df ? 0.5f * (s_wb[pos_f[t]] + s_wb[pos_f[t] + 1]) : 0.f;
                 }
             } else {
-                float w3[kMaxT], tm3[kMaxT];
-                if constexpr (L == 64) march_weights_pair<kMaxT>(X, tc, sc, cnt, lane, w3, tm3);
-                else march_weights<L, kMaxT>(tc, sc, cnt, lane, w3, tm3);
-                if constexpr (kExport) {
-                    if (ok && eset == 0) {                           // both warp sets hold the ray; one writes
-                        float* const out = K.samples + gr * (2 * cnt - 1);
-#pragma unroll
-                        for (int t = 0; t < kMaxT; ++t) {
-                            const int k = t * L + j;
-                            if (k < cnt) out[k] = tc[t];
-                            if (k < cnt - 1) out[cnt + k] = w3[t];
-                        }
-                    }
-                }
-                float ws = 0.f, da = 0.f;
-#pragma unroll
-                for (int t = 0; t < kMaxT; ++t) { ws += w3[t]; da += w3[t] * tm3[t]; }
-                float wpv[kMaxT];
-                if constexpr (L == 64) {
-                    wsum = pair_sum(X, ws, lane);
-                    dacc = pair_sum(X, da, lane);
-                    pair_prev<kMaxT>(X, w3, 0.f, wpv, lane);
-                } else {
-                    wsum = seg_sum<L>(ws);
-                    dacc = seg_sum<L>(da);
-                }
+                float w3[kMaxT], tm3[kMaxT], wp[kMaxT];
+                march_weights(seg, tc, sc, cnt, j, w3, tm3);
+                ray_sums(tc, w3, tm3);
+                seg.prev(w3, 0.f, wp);
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) {
-                    const float wp = L == 64 ? wpv[t] : seg_prev<L>(w3[t], t > 0 ? w3[t - 1] : 0.f, lane);
                     const int k = t * L + j;
-                    coef_c[t] = k < Dc ? 0.5f * ((k > 0 ? wp : 0.f) + w3[t]) : 0.f;
+                    coef_c[t] = k < Dc ? 0.5f * ((k > 0 ? wp[t] : 0.f) + w3[t]) : 0.f;
                     coef_f[t] = 0.f;
                 }
-                d_first = L == 64 ? tc[0] : __shfl_sync(FULL, tc[0], lane & ~(L - 1));     // read on j == 0 only
                 if (j == 0) s_wb[0] = 0.f;                          // keep the scratch race-free across phases
 #pragma unroll
                 for (int t = 0; t < kMaxT; ++t) { const int k = t * L + j; if (k < Dc) s_sd[k] = tc[t]; }
-                ray_sync();
+                seg.sync();
                 d_last = s_sd[Dc - 1];
             }
             // colours: acc[c] += coef * sigmoid(logit + b1) over this thread's rows, channels 16*eset .. +15 (sigmoid * 1.002 - 0.001,
@@ -1017,27 +1032,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_fused_kernel(const __grid_
                 for (int t = 0; t < kMaxT; ++t)
                     if (t < Tf) add_tile(6 + t, coef_f[t]);
             }
-            // segment reduce-scatter: lane j ends with channel (j & 15) summed over the L lanes
-            if (L >= 32) {
-#pragma unroll
-                for (int c = 0; c < 16; ++c) acc[c] += __shfl_xor_sync(FULL, acc[c], 16);
-            }
-#pragma unroll
-            for (int h = 8; h >= 1; h >>= 1) {
-                const bool up = (j & h) != 0;
-#pragma unroll
-                for (int c = 0; c < h; ++c) {
-                    const float send = up ? acc[c] : acc[c + h];
-                    const float keep = up ? acc[c + h] : acc[c];
-                    acc[c] = keep + __shfl_xor_sync(FULL, send, h);
-                }
-            }
-            if constexpr (L == 64) {                                // half 1's channel sums join half 0's (j = lane < 16)
-                float* const b = pair_buf(X);
-                if (X.h == 1 && lane < 16) b[lane] = acc[0];
-                pair_sync(X);
-                if (X.h == 0 && lane < 16) acc[0] += b[lane];
-            }
+            seg.reduce16(acc);                                      // lane j < 16 now holds channel j of the ray
             if (ok && j < 16) {
                 float v = fmaf(acc[0], 1.002f, -0.001f * wsum);     // sum_k coef_k (1.002 sigmoid_k - 0.001), sum_k coef_k = wsum
                 if (P.white_back) v = v + 1.f - wsum;
@@ -1219,12 +1214,7 @@ __global__ void __launch_bounds__(kThreads, 1) points_fused_kernel(const __grid_
                     }
                 }
                 setup_taps(taps, lane, px, py, pz, valid, img, K.PH, K.PW, K.scale);
-                __syncwarp();
-                const int b = i % kNF;
-                if (i >= kNF) mbar_wait_sleep(S.bar(BAR_FEMPTY + b), (uint32_t)((i / kNF - 1) & 1), 40u);
-                gather_rows(K.planes, taps, sb + kOffF + b * 16384, sb + kOffF + b * 16384 + 8192, q * 32, lane);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(S.bar(BAR_FFULL + b));
+                fill_buffer(S, K.planes, taps, i, q * 32, lane);
                 next_item += kGWarps;
             }
             ++i;
@@ -1282,13 +1272,11 @@ __global__ void __launch_bounds__(kThreads, 1) points_fused_kernel(const __grid_
 // (renderer.py:271-355 normal_forward, ray_marcher.py:32-33, 61-64).  Input: the sorted depths and final interval weights that
 // render_fused_kernel<L, true> exported per ray.  Per sample, from ONE fetch of its 12 bilinear taps:
 //   f = plane-mean feature and J_a = d f / d x_a (a = x, y, z; the bilinear-derivative weights of the same tap fractions),
-//   sigma' = sigmoid(W0 f + b0) (softplus' = sigmoid),  d sigma / d x_a = sum_k sigma'_k W1[0, k] (W0 J_a)_k.
-// Two formulations of the last line (template kForward; DESIGN.md section 3.2a has their timings):
-//   reverse (shipped): g = W0^T (sigma' * W1[0, :]) = d sigma / d f on the tensor cores, then three 32-long dot products g . J_a;
-//   forward          : the three derivative rows J_a through layer 1 on the tensor cores, reduced against sigma' * W1[0, :].
+//   sigma' = sigmoid(W0 f + b0) (softplus' = sigmoid),  d sigma / d x_a = sum_k sigma'_k W1[0, k] (W0 J_a)_k,
+// evaluated in reverse mode: g = W0^T (sigma' * W1[0, :]) = d sigma / d f on the tensor cores, then three 32-long dot products
+// g . J_a (DESIGN.md section 3.2a).
 // One warp = one ray at a time, 16 samples per chunk (tile row = sample); every product runs on mma.sync m16n8k16, bf16x3 with fp32
-// accumulation, like the renderer's decoder.  Reverse mode feeds the layer-1 accumulator fragments straight into the second
-// product as its A operand.
+// accumulation, like the renderer's decoder.  The layer-1 accumulator fragments feed the second product directly as its A operand.
 struct NormalsK {
     N3DRender p;
     int D;                       // samples per ray in `samples`: Dc + Df, or Dc when coarse-only
@@ -1302,42 +1290,12 @@ constexpr int kNWarps = 8, kNThreads = kNWarps * 32;
 constexpr int kNRows = 16;                                      // samples per chunk
 constexpr int kNFrags = 64;                                     // B fragments per lane: 32 of W0^T (layer 1), then 32 of W0 (layer 1 transposed)
 constexpr int kNOffB0 = kNFrags * 32 * 8;                       // [kNFrags][32 lanes] (hi, lo) words, then b0 [64] | W1[0, :] [64]
-constexpr int kNJStride = 100;                                  // reverse: floats per row of the fp32 J tile ([3][32] + pad)
+constexpr int kNJStride = 100;                                  // floats per row of the fp32 J tile ([3][32] + pad)
 constexpr int kNOffWarp = kNOffB0 + 2 * kHidden * 4;
-// per warp: f tile hi | lo ([16] x 64-byte SWIZZLE_64B rows), then the J tile: reverse [16][100] fp32, forward 3 x (hi | lo) bf16 tiles
-constexpr int kNJBytes = kNRows * kNJStride * 4 > 6 * kNRows * 64 ? kNRows * kNJStride * 4 : 6 * kNRows * 64;
+// per warp: f tile hi | lo ([16] x 64-byte SWIZZLE_64B rows), then the J tile [16][kNJStride] fp32
+constexpr int kNJBytes = kNRows * kNJStride * 4;
 constexpr int kNWarpBytes = 2 * kNRows * 64 + kNJBytes;
 constexpr int kNSmemBytes = kNOffWarp + kNWarps * kNWarpBytes;  // 84480: two CTAs per SM
-
-// The four bilinear taps of plane pl at scaled point (x, y, z), as setup_taps: texel byte offsets, weights and the derivatives of
-// the weights along the plane's two world axes (a, b) = (x, y), (x, z), (z, y) (grid_sample align_corners=False:
-// d ix / d x_a = scale * PW / 2); the 1/3 of the plane mean is folded into all three.  Taps outside the plane (zeros padding) and
-// invalid samples get weight 0 and point at texel 0.
-struct PlaneTaps {
-    uint32_t off[4];
-    float w[4], wa[4], wb[4];
-};
-__device__ __forceinline__ PlaneTaps plane_taps(int pl, float x, float y, float z, bool valid, uint32_t img4, int PH, int PW, float scale) {
-    PlaneTaps t;
-    const float gx = pl == 2 ? z : x, gy = pl == 1 ? z : y;
-    const float ix = ((gx + 1.f) * (float)PW - 1.f) * 0.5f, iy = ((gy + 1.f) * (float)PH - 1.f) * 0.5f;
-    const float flx = floorf(ix), fly = floorf(iy);
-    const float fx = ix - flx, fy = iy - fly;
-    const int x0 = (int)fminf(fmaxf(flx, -2.f), (float)PW), y0 = (int)fminf(fmaxf(fly, -2.f), (float)PH);
-    const uint32_t pbase = img4 + (uint32_t)(pl * PH * PW) * 128u;
-    const float ka = scale * (float)PW * (0.5f / 3.f), kb = scale * (float)PH * (0.5f / 3.f);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-        const int xi = x0 + (c & 1), yi = y0 + (c >> 1);
-        const float wx = (c & 1) ? fx : 1.f - fx, wy = (c >> 1) ? fy : 1.f - fy;
-        const bool inside = valid && xi >= 0 && xi < PW && yi >= 0 && yi < PH;
-        t.off[c] = inside ? pbase + (uint32_t)(yi * PW + xi) * 128u : 0u;
-        t.w[c] = inside ? wx * wy * (1.f / 3.f) : 0.f;
-        t.wa[c] = inside ? ((c & 1) ? wy : -wy) * ka : 0.f;
-        t.wb[c] = inside ? ((c >> 1) ? wx : -wx) * kb : 0.f;
-    }
-    return t;
-}
 
 // Layer 1 of the 16 rows of a bf16 (hi, lo) SWIZZLE_64B tile: acc[nt] = rows x hidden units 8 nt .. 8 nt + 7 (m16n8 fragments).
 __device__ __forceinline__ void normals_layer1(const uint8_t* th, const uint8_t* tl, const uint2* frag, int lane, float (&acc)[8][4]) {
@@ -1372,7 +1330,6 @@ __device__ __forceinline__ void store_split_row(uint8_t* th, uint8_t* tl, int ro
     *reinterpret_cast<uint4*>(tl + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
-template <bool kForward>
 __global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __grid_constant__ NormalsK K) {
     extern __shared__ __align__(16) uint8_t nsm[];
     const N3DRender& P = K.p;
@@ -1406,8 +1363,7 @@ __global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __gri
 
     uint8_t* const fh = nsm + kNOffWarp + warp * kNWarpBytes;
     uint8_t* const fl = fh + kNRows * 64;
-    uint8_t* const jb = fh + 2 * kNRows * 64;                      // J tile
-    float* const jt = reinterpret_cast<float*>(jb);
+    float* const jt = reinterpret_cast<float*>(fh + 2 * kNRows * 64);      // J tile
     const char* const planes = reinterpret_cast<const char*>(P.planes);
     const int g = lane >> 2, c = lane & 3;               // fetch: sample g of a step, channel octet c; mma: fragment row g, column pair c
     const int D = K.D, M = P.res * P.res;
@@ -1456,13 +1412,9 @@ __global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __gri
                 store_split_row(fh, fl, row, c, fv);
 #pragma unroll
                 for (int a = 0; a < 3; ++a) {
-                    if constexpr (kForward) {
-                        store_split_row(jb + a * 2 * kNRows * 64, jb + a * 2 * kNRows * 64 + kNRows * 64, row, c, jv[a]);
-                    } else {
-                        float* const dst = jt + row * kNJStride + a * 32 + c * 8;
-                        *reinterpret_cast<float4*>(dst) = make_float4(jv[a][0], jv[a][1], jv[a][2], jv[a][3]);
-                        *reinterpret_cast<float4*>(dst + 4) = make_float4(jv[a][4], jv[a][5], jv[a][6], jv[a][7]);
-                    }
+                    float* const dst = jt + row * kNJStride + a * 32 + c * 8;
+                    *reinterpret_cast<float4*>(dst) = make_float4(jv[a][0], jv[a][1], jv[a][2], jv[a][3]);
+                    *reinterpret_cast<float4*>(dst + 4) = make_float4(jv[a][4], jv[a][5], jv[a][6], jv[a][7]);
                 }
             }
             __syncwarp();
@@ -1477,58 +1429,41 @@ __global__ void __launch_bounds__(kNThreads, 2) normals_fused_kernel(const __gri
                     u[nt][e] = sigmoid_fast(u[nt][e] + sB0[k]) * sW1[k];
                 }
             float gs[2][3];                                  // d sigma / d x_a of rows g (hr 0) and g + 8 (hr 1), partial over this lane's columns
-            if constexpr (kForward) {
-#pragma unroll 1
-                for (int a = 0; a < 3; ++a) {                  // one derivative row set at a time (register budget)
-                    float pa[8][4];
-                    normals_layer1(jb + a * 2 * kNRows * 64, jb + a * 2 * kNRows * 64 + kNRows * 64, frag, lane, pa);
-                    float s0 = 0.f, s1 = 0.f;
+            // g [16 x 32] = u W0: the accumulator fragments of hidden units 16 ks .. 16 ks + 15 are the A fragment of k-step ks
+            float gacc[4][4];
 #pragma unroll
-                    for (int nt = 0; nt < 8; ++nt) {
-                        s0 = fmaf(u[nt][0], pa[nt][0], fmaf(u[nt][1], pa[nt][1], s0));
-                        s1 = fmaf(u[nt][2], pa[nt][2], fmaf(u[nt][3], pa[nt][3], s1));
-                    }
-                    if (a == 0) { gs[0][0] = s0; gs[1][0] = s1; }
-                    else if (a == 1) { gs[0][1] = s0; gs[1][1] = s1; }
-                    else { gs[0][2] = s0; gs[1][2] = s1; }
+            for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) gacc[nt][e] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < kHidden / 16; ++ks) {
+                uint32_t ah[4], al[4];
+                split_bf16x2(u[2 * ks][0], u[2 * ks][1], ah[0], al[0]);
+                split_bf16x2(u[2 * ks][2], u[2 * ks][3], ah[1], al[1]);
+                split_bf16x2(u[2 * ks + 1][0], u[2 * ks + 1][1], ah[2], al[2]);
+                split_bf16x2(u[2 * ks + 1][2], u[2 * ks + 1][3], ah[3], al[3]);
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt) {
+                    const uint2 b0 = frag[(32 + (ks * 4 + nt) * 2) * 32 + lane], b1 = frag[(32 + (ks * 4 + nt) * 2 + 1) * 32 + lane];
+                    mma_bf16_16816(gacc[nt], ah, b0.x, b1.x);
+                    mma_bf16_16816(gacc[nt], ah, b0.y, b1.y);
+                    mma_bf16_16816(gacc[nt], al, b0.x, b1.x);
                 }
-            } else {
-                // g [16 x 32] = u W0: the accumulator fragments of hidden units 16 ks .. 16 ks + 15 are the A fragment of k-step ks
-                float gacc[4][4];
+            }
+            // g . J_a over this lane's 8 features of rows g and g + 8
 #pragma unroll
-                for (int nt = 0; nt < 4; ++nt)
+            for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) gacc[nt][e] = 0.f;
-#pragma unroll
-                for (int ks = 0; ks < kHidden / 16; ++ks) {
-                    uint32_t ah[4], al[4];
-                    split_bf16x2(u[2 * ks][0], u[2 * ks][1], ah[0], al[0]);
-                    split_bf16x2(u[2 * ks][2], u[2 * ks][3], ah[1], al[1]);
-                    split_bf16x2(u[2 * ks + 1][0], u[2 * ks + 1][1], ah[2], al[2]);
-                    split_bf16x2(u[2 * ks + 1][2], u[2 * ks + 1][3], ah[3], al[3]);
+                for (int a = 0; a < 3; ++a) {
+                    const float* const jr = jt + (g + 8 * hr) * kNJStride + a * 32 + 2 * c;
+                    float s = 0.f;
 #pragma unroll
                     for (int nt = 0; nt < 4; ++nt) {
-                        const uint2 b0 = frag[(32 + (ks * 4 + nt) * 2) * 32 + lane], b1 = frag[(32 + (ks * 4 + nt) * 2 + 1) * 32 + lane];
-                        mma_bf16_16816(gacc[nt], ah, b0.x, b1.x);
-                        mma_bf16_16816(gacc[nt], ah, b0.y, b1.y);
-                        mma_bf16_16816(gacc[nt], al, b0.x, b1.x);
+                        const float2 j2 = *reinterpret_cast<const float2*>(jr + 8 * nt);
+                        s = fmaf(gacc[nt][2 * hr], j2.x, fmaf(gacc[nt][2 * hr + 1], j2.y, s));
                     }
+                    gs[hr][a] = s;
                 }
-                // g . J_a over this lane's 8 features of rows g and g + 8
-#pragma unroll
-                for (int hr = 0; hr < 2; ++hr)
-#pragma unroll
-                    for (int a = 0; a < 3; ++a) {
-                        const float* const jr = jt + (g + 8 * hr) * kNJStride + a * 32 + 2 * c;
-                        float s = 0.f;
-#pragma unroll
-                        for (int nt = 0; nt < 4; ++nt) {
-                            const float2 j2 = *reinterpret_cast<const float2*>(jr + 8 * nt);
-                            s = fmaf(gacc[nt][2 * hr], j2.x, fmaf(gacc[nt][2 * hr + 1], j2.y, s));
-                        }
-                        gs[hr][a] = s;
-                    }
-            }
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
@@ -1584,7 +1519,7 @@ __global__ void __launch_bounds__(kThreads, 1) gather_floor_kernel(const __grid_
     uint8_t* const sb = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const N3DRender& P = K.p;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int L = P.depth_coarse <= 48 ? 16 : 32;
+    const int L = 64 / K.gw;                                     // make_fused's lanes per ray
     uint2* const taps = reinterpret_cast<uint2*>(sb + 32768 + warp * kTapBytesPerWarp);
     uint8_t* const f_hi = sb, * const f_lo = sb + 8192;          // one shared tile: the stores are part of the cost, the data is not used
     const int g_begin = (int)((K.total_groups * blockIdx.x) / gridDim.x);
@@ -1640,17 +1575,8 @@ __global__ void __launch_bounds__(kThreads, 1) mufu_floor_kernel(long long sampl
     if (sink && acc == 123.456f) sink[0] = acc;
 }
 
-// Depth clamp of the composited depth to the batch-global depth range (ray_marcher.py:53-54).
-__global__ void __launch_bounds__(256) depth_clamp_kernel(float* __restrict__ depth, int64_t n, const float* __restrict__ mm) {
-    const float lo = mm[0], hi = mm[1];
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float d = depth[i];
-        if (isnan(d)) d = INFINITY;
-        depth[i] = fminf(fmaxf(d, lo), hi);
-    }
-}
-
-// The same clamp with one depth range per image: image i / per_image is clamped to its own pair of mm [N, 2].
+// Depth clamp of the composited depth to the depth range (ray_marcher.py:53-54), one range per image: element i belongs to image
+// i / per_image and is clamped to its pair of mm [N, 2].  The batch-global clamp is the case of one image.
 __global__ void __launch_bounds__(256) depth_clamp_images_kernel(float* __restrict__ depth, int64_t n, int64_t per_image,
                                                                  const float* __restrict__ mm) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -1775,8 +1701,7 @@ extern "C" int n3d_render_rays(const N3DRender* p, void* stream) {
 }
 
 namespace {
-// normals_fused_kernel<kForward> over the samples render_fused_kernel<L, true> left in `workspace`.
-template <bool kForward>
+// normals_fused_kernel over the samples render_fused_kernel<L, true> left in `workspace`.
 int launch_normals(const N3DRender* p, const float* workspace, float* normal, const char* who, void* stream) {
     NormalsK K;
     K.p = *p;
@@ -1786,12 +1711,12 @@ int launch_normals(const N3DRender* p, const float* workspace, float* normal, co
     K.rays = (long long)p->N * p->res * p->res;
     K.samples = workspace;
     K.normal = normal;
-    if (int rc = n3d_smem_optin((const void*)normals_fused_kernel<kForward>, kNSmemBytes, who)) return rc;
+    if (int rc = n3d_smem_optin((const void*)normals_fused_kernel, kNSmemBytes, who)) return rc;
     const N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
     const long long blocks = (K.rays + kNWarps - 1) / kNWarps;
     const int grid = (int)(blocks < 2ll * D->num_sms ? blocks : 2ll * D->num_sms);
-    normals_fused_kernel<kForward><<<grid, kNThreads, kNSmemBytes, (cudaStream_t)stream>>>(K);
+    normals_fused_kernel<<<grid, kNThreads, kNSmemBytes, (cudaStream_t)stream>>>(K);
     N3D_CHECK_LAUNCH(who);
     return N3D_OK;
 }
@@ -1802,14 +1727,14 @@ extern "C" int n3d_render_rays_normals(const N3DRender* p, float* normal, float*
     if (int rc = check_render(p, who)) return rc;
     N3D_CHECK_ARG(normal && workspace, "%s: null pointer", who);
     if (int rc = launch_render<true>(p, workspace, who, stream)) return rc;
-    return launch_normals<false>(p, workspace, normal, who, stream);
+    return launch_normals(p, workspace, normal, who, stream);
 }
 
-extern "C" int n3d_render_normals_pass(const N3DRender* p, int forward, const float* workspace, float* normal, void* stream) {
+extern "C" int n3d_render_normals_pass(const N3DRender* p, const float* workspace, float* normal, void* stream) {
     const char* who = "n3d_render_normals_pass";
     if (int rc = check_render(p, who)) return rc;
-    N3D_CHECK_ARG(normal && workspace && (forward == 0 || forward == 1), "%s: bad args", who);
-    return forward ? launch_normals<true>(p, workspace, normal, who, stream) : launch_normals<false>(p, workspace, normal, who, stream);
+    N3D_CHECK_ARG(normal && workspace, "%s: bad args", who);
+    return launch_normals(p, workspace, normal, who, stream);
 }
 
 extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void* stream) {
@@ -1836,7 +1761,7 @@ extern "C" int n3d_render_floor(const N3DRender* p, int kind, float* sink, void*
 extern "C" int n3d_depth_clamp(float* depth, int64_t n, const float* depth_minmax, void* stream) {
     N3D_CHECK_ARG(depth && depth_minmax && n >= 0, "n3d_depth_clamp: bad args");
     if (n == 0) return N3D_OK;
-    depth_clamp_kernel<<<n3d_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(depth, n, depth_minmax);
+    depth_clamp_images_kernel<<<n3d_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(depth, n, n, depth_minmax);
     N3D_CHECK_LAUNCH("n3d_depth_clamp");
     return N3D_OK;
 }

@@ -277,13 +277,13 @@ def render_rays_normals(planes, cam2world, intrinsics, res, opts, dec, rgb, dept
     _run('n3d_render_rays_normals', C.byref(p), ptr(normal), ptr(workspace), stream_ptr(), kernels=2)
 
 
-def render_normals_pass(planes, cam2world, intrinsics, res, opts, dec, normal, workspace, forward=False):
+def render_normals_pass(planes, cam2world, intrinsics, res, opts, dec, normal, workspace):
     """Diagnostics (n3d_render_normals_pass): the normal pass alone over the samples an earlier render_rays_normals call with the same
-    workload left in `workspace`; forward=True runs the forward-mode formulation instead of the shipped reverse mode."""
+    workload left in `workspace`."""
     p = _render_desc(planes, cam2world, intrinsics, res, opts, 0)
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)
     p.rgb = p.depth = p.wsum = ptr(normal)         # not written; the argument checks are n3d_render_rays'
-    _run('n3d_render_normals_pass', C.byref(p), int(bool(forward)), ptr(workspace), ptr(normal), stream_ptr())
+    _run('n3d_render_normals_pass', C.byref(p), ptr(workspace), ptr(normal), stream_ptr())
 
 
 def depth_clamp(depth, depth_minmax):

@@ -70,7 +70,9 @@ def _workload(N, res, D, Df, ties):
 # the shapes of test_gpu_kernels.py::test_render_rays: both lane layouts, ragged tiles, coarse-only, unequal resolutions, ties
 @pytest.mark.parametrize('N,res,D,Df,ties', [(2, 32, 48, 48, 0), (1, 16, 96, 96, 0), (1, 24, 36, 36, 0), (1, 20, 48, 0, 0), (1, 16, 40, 24, 0),
                                              (2, 12, 12, 70, 0), (3, 64, 48, 48, 0), (1, 16, 48, 48, 1), (1, 12, 96, 96, 1), (1, 12, 96, 96, 0)])
-def test_render_rays_normals(K, N, res, D, Df, ties):
+def test_render_rays_normals_and_normal_pass(K, N, res, D, Df, ties):
+    """render_rays_normals against render_rays (bit for bit) and the oracle; the normal pass alone (n3d_render_normals_pass) over the
+    same workspace reproduces the normals exactly."""
     from oracle import normals as onr, renderer as orr
     opts, planes, sd, c, u_c, u_f = _workload(N, res, D, Df, ties)
     o, d = orr.ray_sampler(c[:, :16].reshape(-1, 4, 4), c[:, 16:25].reshape(-1, 3, 3), res)
@@ -95,11 +97,10 @@ def test_render_rays_normals(K, N, res, D, Df, ties):
             assert torch.equal(x, y), name
         if 'u_coarse' in noise:
             n_raw_ref = _check_against_oracle(sd, planes, o, d, opts, work.view(N, M, -1), normal, ref)
-            # the forward-mode formulation of the normal pass (timing diagnostics) computes the same normals, at the same positions
+            # the normal pass alone (timing diagnostics) over the same workspace reproduces the normals
             alt = torch.full_like(normal, float('nan'))
-            K.render_normals_pass(pl, cam, intr, res, opts, dec, alt, work, forward=True)
-            weighted, strong = _normal_errors(alt.cpu(), normal.cpu(), n_raw_ref)
-            assert weighted <= 1e-4 and strong <= 1e-3, (weighted, strong)
+            K.render_normals_pass(pl, cam, intr, res, opts, dec, alt, work)
+            assert torch.equal(alt, normal)
         else:                                        # in-kernel RNG: unit length wherever the ray carries weight
             live = b[2] > 1e-3
             assert torch.isfinite(normal[live]).all()

@@ -604,9 +604,9 @@ def test_plane_sets_at_the_end_of_32_bit_texel_offsets():
 
 # ------------------------------------------------------------------------------------------------ launched instances
 @pytest.mark.gpu
-def test_launched_instance_matches_plan(tmp_path):
+def test_launched_kernels_match_plan(tmp_path):
     """Every case under torch.profiler: the render_fused_kernel<L, export> it launched (the template arguments are in the demangled
-    name) and its grid are the ones `plan` predicts; normals_fused_kernel and points_fused_kernel<rgb> likewise."""
+    name) and its grid are the ones `plan` predicts; normals_fused_kernel (not a template) and points_fused_kernel<rgb> likewise."""
     from torch.profiler import ProfilerActivity, profile
     from next3d_b200 import kernels as K
     props = torch.cuda.get_device_properties(0)
@@ -631,7 +631,7 @@ def test_launched_instance_matches_plan(tmp_path):
             launch_case(setups[i], out, devs[i], normal=normal, work=work)
             p = _plan(c, sms)
             expected.append((c['name'], f'render_fused_kernel<{p["L"]}, true>', p['grid']))
-            expected.append((c['name'], 'normals_fused_kernel<false>', normals_grid(c['N'], c['res'], sms)))
+            expected.append((c['name'], 'normals_fused_kernel', normals_grid(c['N'], c['res'], sms)))
         for pc, planes, sd, coords in pts:
             launch_points(pc, planes, sd, coords)
             expected.append((pc['name'], f'points_fused_kernel<{"true" if pc["rgb"] else "false"}>', points_grid(*coords.shape[:2], sms)))
@@ -648,7 +648,7 @@ def test_launched_instance_matches_plan(tmp_path):
         pytest.skip(f'CUDA activity tracing unavailable: {e}')
     trace = tmp_path / 'trace.json'
     prof.export_chrome_trace(str(trace))
-    pat = re.compile(r'(render_fused_kernel<\d+, (?:true|false)>|normals_fused_kernel<(?:true|false)>|points_fused_kernel<(?:true|false)>)')
+    pat = re.compile(r'(render_fused_kernel<\d+, (?:true|false)>|normals_fused_kernel|points_fused_kernel<(?:true|false)>)')
     events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and pat.search(e.get('name', ''))]
     if not events:
         pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')

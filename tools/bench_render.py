@@ -1,6 +1,6 @@
 """Time the fused renderer alone on a benchmark workload (random planes).  python tools/bench_render.py [c2|c3] [--normals | --long]
 --normals: n3d_render_rays_normals (renderer + normal pass) against n3d_render_rays on both the C2 and the C3 workload, and the
-normal pass alone in its shipped reverse-mode and its forward-mode formulation (n3d_render_normals_pass), alternated.
+normal pass alone (n3d_render_normals_pass) and the gather-only floor.
 --long: both entry points at 96 + 96, 144 + 144 and 192 + 192 samples per ray on the C2 and the C3 workload, alternated, in ms
 and ms per million decoded samples."""
 import sys, os, math, subprocess
@@ -98,18 +98,12 @@ if '--normals' in sys.argv:
         p_med, n_med = min(tp[0], tp2[0]), min(tn[0], tn2[0])
         print(f'{name} N={N} r={R} D={D}+{D}: n3d_render_rays median {tp[0]:.3f} / {tp2[0]:.3f} ms, n3d_render_rays_normals median '
               f'{tn[0]:.3f} / {tn2[0]:.3f} ms, normal pass ~{n_med - p_med:.3f} ms ({n_med / p_med:.2f}x)', flush=True)
-        # the normal pass alone on the samples the last call exported: shipped reverse mode against forward mode, alternated
+        # the normal pass alone on the samples the last call exported
         normals(0)
-        ref = normal.clone()
-        alt = torch.zeros_like(normal)
-        rev = lambda i: K.render_normals_pass(planes, cam, intr, R, opts, dec, normal, work, forward=False)
-        fwd = lambda i: K.render_normals_pass(planes, cam, intr, R, opts, dec, alt, work, forward=True)
-        rev(0); fwd(0); torch.cuda.synchronize()
-        live = wsum > 1e-3
-        diff = (alt - ref)[live].norm(dim=-1).max().item()
-        tr, tf, tr2, tf2 = _events(rev, 15, flush), _events(fwd, 15, flush), _events(rev, 15, flush), _events(fwd, 15, flush)
-        print(f'{name} normal pass alone: reverse mode median {tr[0]:.3f} / {tr2[0]:.3f} ms, forward mode median {tf[0]:.3f} / {tf2[0]:.3f} ms '
-              f'(max |n_forward - n_reverse| {diff:.2e}); gather-only floor (n3d_render_floor kind 0, both passes) '
+        alone = lambda i: K.render_normals_pass(planes, cam, intr, R, opts, dec, normal, work)
+        alone(0)
+        tr, tr2 = _events(alone, 15, flush), _events(alone, 15, flush)
+        print(f'{name} normal pass alone: median {tr[0]:.3f} / {tr2[0]:.3f} ms; gather-only floor (n3d_render_floor kind 0, both passes) '
               f'{_events(lambda i: K.render_floor(planes, cam, intr, R, opts, 0, seed=i), 15, flush)[0]:.3f} ms', flush=True)
     sys.exit(0)
 N, R, D = (8, 64, 48) if which == 'c2' else (16, 128, 96)
