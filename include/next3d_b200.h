@@ -41,11 +41,20 @@ int n3d_version(void);
  * ---------------------------------------------------------------------------------------------------------- */
 
 /* y = clamp(act(x + b[(i / step_b) % size_b]) * gain, +-clamp)   -- replaces bias_act_plugin.bias_act
- * (bias_act.cpp:36-94, kernel bias_act.cu:28-151; forward only, grad == 0).  act: 1 linear, 2 relu, 3 lrelu,
+ * (bias_act.cpp:36-94, kernel bias_act.cu:28-151; forward, grad == 0; the grad modes are n3d_bias_act_grad).  act: 1 linear, 2 relu, 3 lrelu,
  * 4 tanh, 5 sigmoid, 6 elu, 7 selu, 8 softplus, 9 swish (the reference's cuda_idx, bias_act.py:23-33).
  * x dense (any memory format), b contiguous or NULL, clamp < 0 disables clamping. */
 int n3d_bias_act(const void* x, const void* b, void* y, int dtype, int64_t numel, int size_b, int step_b,
                  int act, float alpha, float gain, float clamp, void* stream);
+
+/* Gradients of n3d_bias_act: the plugin's grad modes 1 and 2 (bias_act.cu:58-146, called from BiasActCudaGrad, bias_act.py:177-205).
+ *   grad 1: dx = dy * act'(xref + b) * gain, with act' taken from yref / gain (act 2-8) or from xref + b (act 9, swish);
+ *   grad 2: dx = dy * act''(xref + b) * gain * dyref (act 4-9 only: the activations with a second derivative).
+ * Elements whose saved output lies on or outside +-clamp (clamp >= 0) get 0; swish recomputes that output from xref + b.
+ * dy, xref, yref, dyref and dx share x's dense layout; b is applied to xref only.  xref is required for act 9, yref for act 2-8
+ * (a NULL yref counts as 0, as in the plugin, so `linear` with a clamp passes every element), dyref for grad 2. */
+int n3d_bias_act_grad(const void* dy, const void* b, const void* xref, const void* yref, const void* dyref, void* dx, int dtype,
+                      int64_t numel, int size_b, int step_b, int grad, int act, float alpha, float gain, float clamp, void* stream);
 
 /* Zero-insert upsample -> pad/crop -> 2-D FIR -> decimate, per (n,c) plane  -- replaces upfirdn2d_plugin.upfirdn2d
  * (upfirdn2d.cpp:20-102, kernels upfirdn2d.cu:33-204).  f: fp32 [fh,fw] (separable filters are expanded by the
@@ -154,6 +163,38 @@ int n3d_conv_gemm(const N3DConvGemm* p, void* stream);
  * NHWC result [N, 2H+1, 2W+1, Cout] is written to p->out_f32 (f32_cstride / f32_coff honoured); taps, offsets, OH/OW, mode and
  * the epilogue fields of the descriptor are ignored (follow with n3d_fir_up_epilogue). */
 int n3d_conv_transposed_gemm(const N3DConvGemm* p, void* stream);
+
+/* Weight gradient of a convolution as one launch over all groups and taps (plus a reduction launch when splits > 1):
+ *   dw[g, t, m, n] = sum_{k < K} A[a_row[t] + g*M + m, k + a_off[t]] * B[b_row[t] + g*N + n, k + b_off[t]]
+ * A (output gradient) and B (layer input) are channel-major split bf16 (hi, lo), one row per channel, laid out by
+ * n3d_wgrad_operand; a tap is a column offset (a multiple of 8: TMA boxes start on 16-byte boundaries) plus a row offset (which
+ * selects a copy of the operand shifted by a few columns), and reads outside [0, a_cols) / [0, b_cols) are zero.  bf16x3 products, fp32
+ * accumulate.  K (a multiple of 64) is cut into `splits` slices (1 <= splits <= K / 64): slice s writes partial + s * G*T*M*N and a
+ * second kernel sums the slices in order into dw (no atomics: bit-identical from run to run).  N a multiple of 8.  Operands, partial
+ * and dw 16-byte aligned; lda, ldb multiples of 8. */
+typedef struct {
+    const void* a_hi; const void* a_lo;      /* bf16 [a_rows, lda] */
+    int32_t a_rows; int64_t a_cols, lda;
+    const void* b_hi; const void* b_lo;      /* bf16 [b_rows, ldb] */
+    int32_t b_rows; int64_t b_cols, ldb;
+    int32_t G, M, N, T;                      /* groups, rows of dw (output channels), columns (input channels), taps <= 9 */
+    int64_t K;
+    int64_t a_off[9], b_off[9];              /* per-tap column offsets: multiples of 8, may be negative */
+    int32_t a_row[9], b_row[9];              /* per-tap row offsets (>= 0, row + G*M <= a_rows, row + G*N <= b_rows) */
+    int32_t splits;
+    float* partial;                          /* fp32 [splits, G, T, M, N] (splits > 1) */
+    float* dw;                               /* fp32 [G, T, M, N] */
+} N3DConvWgrad;
+
+int n3d_conv_wgrad(const N3DConvWgrad* p, void* stream);
+
+/* Operand of n3d_conv_wgrad from an fp32 tensor x [N, C, H, W] with element strides x_strides (n, c, y, x):
+ *   hi/lo[c * ld + j - shift] = split_bf16(x[n, c, s*(py - pt) + par / s, s*(px - pl) + par % s]),  j = ((par * N + n) * PH + py) * PW + px
+ * for par < s*s (s = 1, or 2 = parity sub-images of a stride-2 tap); every other column of [0, ld) is 0 (source pixel outside x,
+ * j outside [0, s*s*N*PH*PW)).  shift moves the grid `shift` columns left (a horizontal tap shift).  ld a multiple of 8; hi / lo
+ * 16-byte aligned. */
+int n3d_wgrad_operand(const float* x, const int64_t x_strides[4], int N, int C, int H, int W, int s, int pt, int pl, int PH, int PW,
+                      int shift, int64_t ld, void* hi, void* lo, void* stream);
 
 /* fp32 NHWC -> split bf16 NHWC with optional per-(n,c) modulation: out = split(x[n,y,x,c] * style[n,c]). */
 int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* hi, void* lo,

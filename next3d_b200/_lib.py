@@ -51,6 +51,16 @@ class ConvGemm(C.Structure):
     ]
 
 
+class ConvWgrad(C.Structure):
+    _fields_ = [
+        ('a_hi', P), ('a_lo', P), ('a_rows', I32), ('a_cols', I64), ('lda', I64),
+        ('b_hi', P), ('b_lo', P), ('b_rows', I32), ('b_cols', I64), ('ldb', I64),
+        ('G', I32), ('M', I32), ('N', I32), ('T', I32), ('K', I64),
+        ('a_off', I64 * 9), ('b_off', I64 * 9), ('a_row', I32 * 9), ('b_row', I32 * 9),
+        ('splits', I32), ('partial', P), ('dw', P),
+    ]
+
+
 class Render(C.Structure):
     _fields_ = [
         ('planes', P), ('N', I32), ('PH', I32), ('PW', I32),
@@ -67,12 +77,15 @@ _SIGNATURES = {
     'n3d_version': ([], C.c_int),
     'n3d_last_error': ([], C.c_char_p),
     'n3d_bias_act': ([P, P, P, C.c_int, I64, C.c_int, C.c_int, C.c_int, F32, F32, F32, P], C.c_int),
+    'n3d_bias_act_grad': ([P, P, P, P, P, P, C.c_int, I64, C.c_int, C.c_int, C.c_int, C.c_int, F32, F32, F32, P], C.c_int),
     'n3d_upfirdn2d': ([P, P, P, C.c_int] + [C.c_int] * 4 + [C.POINTER(I64), C.POINTER(I64)] + [C.c_int] * 10 + [C.c_int, F32, C.c_int, C.c_int, P], C.c_int),
     'n3d_filtered_lrelu': ([P, P, P, P, P, P, C.c_int] + [C.c_int] * 14 + [F32, F32, F32, C.c_int, C.c_int, C.c_int, P], C.c_int),
     'n3d_styles': ([P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, C.c_int, P], C.c_int),
     'n3d_demod': ([P, P, P, P, P, P, P, P, C.c_int, C.c_int, P], C.c_int),
     'n3d_conv_gemm': ([C.POINTER(ConvGemm), P], C.c_int),
     'n3d_conv_transposed_gemm': ([C.POINTER(ConvGemm), P], C.c_int),
+    'n3d_conv_wgrad': ([C.POINTER(ConvWgrad), P], C.c_int),
+    'n3d_wgrad_operand': ([P, C.POINTER(I64)] + [C.c_int] * 10 + [I64, P, P, P], C.c_int),
     'n3d_modulate_split': ([P, I64, C.c_int, C.c_int, P, P, P, C.c_int, C.c_int, P], C.c_int),
     'n3d_fir_up_epilogue': ([P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, P, I64, F32, F32, F32, C.POINTER(SplitOut), P, C.c_int, C.c_int, P], C.c_int),
     'n3d_parse_obj_vertices': ([C.c_char_p, I64, P, I64, C.POINTER(I64)], C.c_int),

@@ -1,4 +1,5 @@
-// Op-level kernels behind torch_utils.ops.{bias_act, upfirdn2d, filtered_lrelu} (forward only).
+// Op-level kernels behind torch_utils.ops.{bias_act, upfirdn2d, filtered_lrelu}: the forward passes and bias_act's gradients
+// (upfirdn2d's gradient is upfirdn2d itself).
 // Memory-bound: one pass, 128-bit accesses where the layout allows, grid sized to the SM count.
 #include "common.cuh"
 
@@ -75,6 +76,85 @@ extern "C" int n3d_bias_act(const void* x, const void* b, void* y, int dtype, in
         bias_act_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)x, (const __half*)b, (__half*)y,
                                                                          numel, size_b, step_b, act, alpha, gain, clamp);
     N3D_CHECK_LAUNCH("n3d_bias_act");
+    return N3D_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- bias_act gradients
+// The reference plugin's grad modes (bias_act.cu:58-146) in fp32 for both storage types.  grad 1: dx = dy * act'(x + b) * gain,
+// act' taken from the saved output (yy = yref / gain) or, for swish, from the saved input xref + b.  grad 2: the derivative of
+// grad 1 with respect to its saved input, times dyref.  Elements whose saved output lies on or outside +-clamp get 0 (for swish
+// the output is recomputed from xref); a missing yref counts as 0, as in the plugin.
+__device__ __forceinline__ float n3d_act_grad(float v, float xr, float yr, float dyr, int grad, int act, float alpha, float gain,
+                                              float clamp) {
+    const float yy = gain != 0.f ? yr / gain : 0.f;
+    float y = 0.f;
+    switch (act) {
+        case 1: y = grad == 1 ? v : 0.f; break;
+        case 2: y = grad == 1 ? (yy > 0.f ? v : 0.f) : 0.f; break;
+        case 3: y = grad == 1 ? (yy > 0.f ? v : v * alpha) : 0.f; break;
+        case 4: y = grad == 1 ? v * (1.f - yy * yy) : v * (1.f - yy * yy) * (-2.f * yy); break;
+        case 5: y = grad == 1 ? v * yy * (1.f - yy) : v * yy * (1.f - yy) * (1.f - 2.f * yy); break;
+        case 6: y = grad == 1 ? (yy >= 0.f ? v : v * (yy + 1.f)) : (yy >= 0.f ? 0.f : v * (yy + 1.f)); break;
+        case 7: {
+            const float s = 1.0507009873554805f, sa = 1.0507009873554805f * 1.6732632423543772f;
+            y = grad == 1 ? (yy >= 0.f ? v * s : v * (yy + sa)) : (yy >= 0.f ? 0.f : v * (yy + sa));
+            break;
+        }
+        case 8: {
+            const float c = expf(-yy);
+            y = grad == 1 ? v * (1.f - c) : v * c * (1.f - c);
+            break;
+        }
+        case 9: {
+            const float c = expf(xr), d = c + 1.f;
+            if (grad == 1) y = xr > 40.f ? v : v * c * (xr + d) / (d * d);
+            else y = xr > 40.f ? 0.f : v * c * (xr * (2.f - d) + 2.f * d) / (d * d * d);
+            yr = xr < -80.f ? 0.f : xr / (expf(-xr) + 1.f) * gain;
+            break;
+        }
+    }
+    y *= gain * dyr;
+    if (clamp >= 0.f && !(yr > -clamp && yr < clamp)) y = 0.f;
+    return y;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) bias_act_grad_kernel(const T* __restrict__ dy, const T* __restrict__ b, const T* __restrict__ xref,
+                                                            const T* __restrict__ yref, const T* __restrict__ dyref, T* __restrict__ dx,
+                                                            int64_t numel, int size_b, int step_b, int grad, int act, float alpha,
+                                                            float gain, float clamp) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < numel; i += stride) {
+        float xr = xref ? to_f<T>(xref[i]) : 0.f;
+        if (b) xr += to_f<T>(b[(i / step_b) % size_b]);
+        const float yr = yref ? to_f<T>(yref[i]) : 0.f;
+        const float dyr = dyref ? to_f<T>(dyref[i]) : 1.f;
+        dx[i] = from_f<T>(n3d_act_grad(to_f<T>(dy[i]), xr, yr, dyr, grad, act, alpha, gain, clamp));
+    }
+}
+
+extern "C" int n3d_bias_act_grad(const void* dy, const void* b, const void* xref, const void* yref, const void* dyref, void* dx, int dtype,
+                                 int64_t numel, int size_b, int step_b, int grad, int act, float alpha, float gain, float clamp,
+                                 void* stream) {
+    N3D_CHECK_ARG(dy && dx && numel >= 0, "n3d_bias_act_grad: null pointer");
+    N3D_CHECK_ARG(act >= 1 && act <= 9, "n3d_bias_act_grad: act %d out of range", act);
+    N3D_CHECK_ARG(grad == 1 || (grad == 2 && act >= 4), "n3d_bias_act_grad: grad mode %d is not defined for act %d", grad, act);
+    N3D_CHECK_ARG(dtype == N3D_DTYPE_F32 || dtype == N3D_DTYPE_F16, "n3d_bias_act_grad: unsupported dtype %d", dtype);
+    N3D_CHECK_ARG(!b || (size_b > 0 && step_b > 0), "n3d_bias_act_grad: bad bias geometry");
+    N3D_CHECK_ARG(act != 9 || xref, "n3d_bias_act_grad: null xref (swish differentiates from its input)");
+    N3D_CHECK_ARG(act == 1 || act == 9 || yref, "n3d_bias_act_grad: null yref (act %d differentiates from its output)", act);
+    N3D_CHECK_ARG(grad == 1 || dyref, "n3d_bias_act_grad: null dyref (grad mode 2)");
+    if (numel == 0) return N3D_OK;
+    const int grid = n3d_grid(numel, 256);
+    if (dtype == N3D_DTYPE_F32)
+        bias_act_grad_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)dy, (const float*)b, (const float*)xref,
+                                                                             (const float*)yref, (const float*)dyref, (float*)dx, numel,
+                                                                             size_b, step_b, grad, act, alpha, gain, clamp);
+    else
+        bias_act_grad_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)dy, (const __half*)b, (const __half*)xref,
+                                                                              (const __half*)yref, (const __half*)dyref, (__half*)dx, numel,
+                                                                              size_b, step_b, grad, act, alpha, gain, clamp);
+    N3D_CHECK_LAUNCH("n3d_bias_act_grad");
     return N3D_OK;
 }
 

@@ -112,6 +112,41 @@ def conv_transposed_gemm(a_hi, a_lo, w_hi, w_lo, N, H, W, raw, nprod=3):
     _run('n3d_conv_transposed_gemm', C.byref(p), stream_ptr())
 
 
+def wgrad_operand(x, s, pt, pl, PH, PW, ld, hi, lo, shift=0):
+    """x fp32 [N, C, H, W] (any strides) -> channel-major split operand hi / lo bf16 [C, ld] of conv_wgrad: column
+    ((par * N + n) * PH + py) * PW + px - shift holds x[n, c, s*(py - pt) + par // s, s*(px - pl) + par % s] (0 elsewhere)."""
+    N, Cc, H, W = x.shape
+    _run('n3d_wgrad_operand', ptr(x), (_lib.I64 * 4)(*x.stride()), N, Cc, H, W, s, pt, pl, PH, PW, shift, ld, ptr(hi), ptr(lo), stream_ptr())
+
+
+def wgrad_splits(G, T, M, N, K):
+    """K slices of a conv_wgrad launch: about two waves of CTAs over the device's SMs, at least 8 K steps (of 64 positions) per slice.
+    A function of the shapes and the SM count only, so the same call always sums in the same order."""
+    bn = 32 if N <= 32 else 64 if N <= 64 else 128
+    tiles = -(-M // 128) * -(-N // bn) * T * G
+    ksteps = K // 64
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    return max(1, min(max(ksteps // 8, 1), -(-2 * sms // tiles)))
+
+
+def conv_wgrad(a_hi, a_lo, b_hi, b_lo, G, M, N, K, a_off, b_off, dw, splits=1, partial=None, a_cols=None, b_cols=None, a_row=None, b_row=None):
+    """dw fp32 [G, T, M, N] = sum_{k < K} A[a_row[t] + g*M + m, k + a_off[t]] * B[b_row[t] + g*N + n, k + b_off[t]] (a_*: bf16
+    [rows, lda], b_*: bf16 [rows, ldb], columns outside [0, a_cols) / [0, b_cols) (default: the row length) read as 0; column offsets
+    are multiples of 8, row offsets default to 0).  splits > 1 needs partial fp32 [splits, G, T, M, N]."""
+    p = _lib.ConvWgrad()
+    p.a_hi, p.a_lo, p.a_rows, p.lda = ptr(a_hi), ptr(a_lo), a_hi.shape[0], a_hi.shape[1]
+    p.a_cols = a_hi.shape[1] if a_cols is None else a_cols
+    p.b_hi, p.b_lo, p.b_rows, p.ldb = ptr(b_hi), ptr(b_lo), b_hi.shape[0], b_hi.shape[1]
+    p.b_cols = b_hi.shape[1] if b_cols is None else b_cols
+    p.G, p.M, p.N, p.T, p.K = G, M, N, len(a_off), K
+    for t, (ao, bo) in enumerate(zip(a_off, b_off)):
+        p.a_off[t], p.b_off[t] = ao, bo
+        p.a_row[t] = a_row[t] if a_row is not None else 0
+        p.b_row[t] = b_row[t] if b_row is not None else 0
+    p.splits, p.partial, p.dw = splits, ptr(partial), ptr(dw)
+    _run('n3d_conv_wgrad', C.byref(p), stream_ptr(), kernels=1 if splits == 1 else 2)
+
+
 def modulate_split(x, style, hi, lo, cstride=None, coff=0):
     """x fp32 NHWC [N,H,W,C]; style [N,C] or None -> hi/lo bf16 (written at channel offset `coff`, stride `cstride`)."""
     N, H, W, Cc = x.shape

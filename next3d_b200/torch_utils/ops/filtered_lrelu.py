@@ -1,6 +1,8 @@
 """`torch_utils.ops.filtered_lrelu` on libnext3d_b200 (reference: torch_utils/ops/filtered_lrelu.py:58-118, plugin
 filtered_lrelu.cpp:20-213).  Never executed by TriPlaneGenerator.synthesis (only reachable through networks_stylegan3,
-SURVEY.md N3); kept for API completeness: same signature, forward only, impl='ref' = torch-op reference (:123-155)."""
+SURVEY.md N3); kept for API completeness: same signature, forward only, impl='ref' = torch-op reference (:123-155).  Under grad mode
+with x or b requiring grad the CUDA path raises instead of returning a result cut from the graph: the reference's backward
+(filtered_lrelu.py:161-270, which replays the forward's sign tensor) is not implemented."""
 import numpy as np
 import torch
 
@@ -51,6 +53,9 @@ def filtered_lrelu(x, fu=None, fd=None, b=None, up=1, down=1, padding=0, gain=np
     _lib.require_cuda(x, 'filtered_lrelu(x)')
     if x.dtype not in _DTYPES:
         raise RuntimeError(f'filtered_lrelu: dtype {x.dtype} is only available with impl="ref"')
+    if torch.is_grad_enabled() and (x.requires_grad or (b is not None and b.requires_grad)):
+        raise RuntimeError('filtered_lrelu: the backward pass (the reference\'s sign-tensor gradient, filtered_lrelu.py:161-270) is not implemented; '
+                           'call it under torch.no_grad() or with impl="ref"')
     px0, px1, py0, py1 = _parse_padding(padding)
     x = x.contiguous()
     N, C, H, W = x.shape

@@ -2,7 +2,11 @@
 
 Same functions, signatures and defaults: setup_filter :72, upfirdn2d :120, filter2d :279, upsample2d :315,
 downsample2d :354 and the private helpers conv2d_resample imports (:36-66).  impl='cuda' requires CUDA tensors (no silent
-fallback); impl='ref' is the torch-op reference implementation (:169-213).  Forward only.
+fallback); impl='ref' is the torch-op reference implementation (:169-213).
+
+Differentiable with respect to x to any order, as the reference's `Upfirdn2dCuda` (:233-270): the gradient is upfirdn2d itself with
+up and down swapped, the filter flipped and the padding of :258-263, called through this same function.  A gradient with respect to
+the filter is refused.
 """
 import numpy as np
 import torch
@@ -117,12 +121,55 @@ def upfirdn2d(x, f, up=1, down=1, padding=0, flip_filter=False, gain=1, impl='cu
         f = torch.ones([1, 1], dtype=torch.float32, device=x.device)
     assert f.dtype == torch.float32 and f.ndim in [1, 2]
     f = f.to(x.device)
+    if torch.is_grad_enabled() and (x.requires_grad or f.requires_grad):
+        if f.requires_grad:
+            raise RuntimeError('upfirdn2d: gradients with respect to the filter f are not implemented (as in the reference)')
+        return _Upfirdn2dCuda.apply(x, f, (upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_filter, gain))
+    return _forward(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_filter, gain)
+
+
+def _forward(x, f, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_filter, gain):
     if f.ndim == 2:
         return _launch(x, f.contiguous(), upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_filter, gain)
     # separable: horizontal pass then vertical pass, gain split evenly (upfirdn2d.py:262-264)
     g = float(np.sqrt(gain))
     y = _launch(x, f[np.newaxis, :].contiguous(), upx, 1, downx, 1, padx0, padx1, 0, 0, flip_filter, g)
     return _launch(y, f[:, np.newaxis].contiguous(), 1, upy, 1, downy, 0, 0, pady0, pady1, flip_filter, g)
+
+
+def _adjoint_padding(x_shape, dy_shape, f, upx, upy, downx, downy, padx0, pady0):
+    """Padding of the upfirdn2d that maps dy back onto x (upfirdn2d.py:257-263)."""
+    _, _, ih, iw = x_shape
+    _, _, oh, ow = dy_shape
+    fw, fh = _get_filter_size(f)
+    return [fw - padx0 - 1, iw * upx - ow * downx + padx0 - upx + 1, fh - pady0 - 1, ih * upy - oh * downy + pady0 - upy + 1]
+
+
+def adjoint(dy, f, x_shape, up=1, down=1, padding=0, flip_filter=False, gain=1):
+    """The gradient of upfirdn2d(x, f, up, down, padding, flip_filter, gain) with respect to x (x of shape x_shape), given the output
+    gradient dy: upfirdn2d with up and down swapped and the filter flipped."""
+    upx, upy = _parse_scaling(up)
+    downx, downy = _parse_scaling(down)
+    padx0, _, pady0, _ = _parse_padding(padding)
+    p = _adjoint_padding(x_shape, dy.shape, f, upx, upy, downx, downy, padx0, pady0)
+    return upfirdn2d(dy, f, up=[downx, downy], down=[upx, upy], padding=p, flip_filter=not flip_filter, gain=gain)
+
+
+class _Upfirdn2dCuda(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, f, cfg):
+        ctx.save_for_backward(f)
+        ctx.cfg, ctx.x_shape = cfg, x.shape
+        return _forward(x, f, *cfg)
+
+    @staticmethod
+    def backward(ctx, dy):
+        f, = ctx.saved_tensors
+        upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_filter, gain = ctx.cfg
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = adjoint(dy, f, ctx.x_shape, [upx, upy], [downx, downy], [padx0, padx1, pady0, pady1], flip_filter, gain)
+        return dx, None, None
 
 
 def filter2d(x, f, padding=0, flip_filter=False, gain=1, impl='cuda'):
