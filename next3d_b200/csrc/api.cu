@@ -55,6 +55,39 @@ int n3d_smem_optin(const void* kernel, int bytes, const char* who) {
     return N3D_OK;
 }
 
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static EncodeTiledFn lookup_encode_tiled() {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess) return nullptr;
+    return (EncodeTiledFn)p;
+}
+
+int n3d_encode_tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box,
+                         CUtensorMapSwizzle swizzle, const char* who) {
+    static const EncodeTiledFn enc = lookup_encode_tiled();     // looked up once; initialisation of a static is thread-safe
+    if (!enc) {
+        n3d_set_error("%s: cuTensorMapEncodeTiled unavailable (no CUDA driver?)", who);
+        return N3D_ERR_CUDA;
+    }
+    cuuint64_t gdim[5], gstr[4];
+    cuuint32_t bdim[5], estr[5];
+    for (int i = 0; i < rank; ++i) {
+        gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1;
+        if (i < rank - 1) gstr[i] = strides[i];
+    }
+    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        n3d_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d", who, (int)r);
+        return N3D_ERR_CUDA;
+    }
+    return N3D_OK;
+}
+
 int n3d_max_clusters(const void* kernel, int threads, int smem_bytes, int cluster, const char* who) {
     N3DDeviceState* d = n3d_device_state();
     if (!d) return 0;

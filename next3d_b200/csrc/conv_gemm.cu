@@ -133,29 +133,6 @@ __device__ __forceinline__ void k_range(const KParams& P, const TileInfo& t, int
     ke = min(nsteps, kb + per);
 }
 
-// One stage's MMAs as a fixed instruction sequence: one fence, BK/16 x NPROD x 2 wgmmas back to back, one commit.  The warpgroup
-// owns all 128 tile rows: acc0 = rows 0-63, acc1 = rows 64-127 (two m64 wgmmas sharing the B descriptor).  FIRST (the first
-// stage of a tile) overwrites the accumulator with its first product instead of adding to it.
-template <int BN, int BK, int NPROD, bool FIRST>
-__device__ __forceinline__ void stage_mma(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
-    constexpr uint32_t h1 = 64u * BK * 2u;         // rows 64-127 of the A tile
-    constexpr uint64_t dhi = wgmma_desc_hi(BK);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
-        const uint32_t koff = (uint32_t)k * 32u;     // 16 bf16 = 32 bytes inside the swizzle row
-        wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
-        wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
-        if (NPROD == 3) {
-            wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
-            wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
-            wgmma_bf16<BN>(acc0, wgmma_desc(a_lo + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-            wgmma_bf16<BN>(acc1, wgmma_desc(a_lo + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-        }
-    }
-    wgmma_commit();
-}
-
 // Main loop of one tile: one stage = one (tap, channel chunk); a stage is released once its wgmmas retired (wait_group 1 after
 // the next stage's wgmmas are issued, so that the tensor cores always have one group queued).  Each of the warpgroup's 4 warps
 // arrives on the stage's empty barrier (of both CTAs in a cluster).
@@ -534,39 +511,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return nullptr;
-        fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
-int make_tmap(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint32_t* box, int block_k) {
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) { n3d_set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return N3D_ERR_CUDA; }
-    cuuint64_t gdim[5], gstr[5];
-    cuuint32_t bdim[5], estr[5];
-    uint64_t stride = 2;
-    for (int i = 0; i < rank; ++i) {
-        gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1;
-        stride *= dims[i];
-        if (i < rank - 1) gstr[i] = stride;      // byte stride of dim i+1
-    }
-    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, block_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { n3d_set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return N3D_ERR_CUDA; }
-    return N3D_OK;
-}
-
 int pow2_ceil(int v) { int p = 1; while (p < v) p <<= 1; return p; }
 
 
@@ -715,17 +659,21 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     K.oy_mul = p->oy_mul; K.ox_mul = p->ox_mul; K.OH = p->OH; K.OW = p->OW;
     K.err_flag = nullptr;       // a protocol timeout traps (the launch fails with an error); no device-side flag is kept
 
+    // A [NI][AH][AW][Cin] and B [T][Cout][Cin], both packed
     const uint64_t adims[4] = {(uint64_t)p->Cin, (uint64_t)p->AW, (uint64_t)p->AH, (uint64_t)p->NI};
+    const uint64_t astr[3] = {adims[0] * 2, adims[0] * adims[1] * 2, adims[0] * adims[1] * adims[2] * 2};
     const uint64_t wdims[3] = {(uint64_t)p->Cin, (uint64_t)p->Cout, (uint64_t)p->T};
+    const uint64_t wstr[2] = {wdims[0] * 2, wdims[0] * wdims[1] * 2};
     const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)K.b_rows, 1u};   // bn / 2 is a multiple of 8: whole swizzle atoms
+    const CUtensorMapSwizzle swz = block_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     for (int b = 0; b < K.nbox; ++b) {
         const KParams::Sub& S = K.sub[box_sub[b]];
         const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)S.TW, (uint32_t)S.TH, (uint32_t)S.TN};
-        if ((rc = make_tmap(&K.tmA[b][0], p->a_hi, 4, adims, abox, block_k)) != N3D_OK) return rc;
-        if (p->nprod == 3 && (rc = make_tmap(&K.tmA[b][1], p->a_lo, 4, adims, abox, block_k)) != N3D_OK) return rc;
+        if ((rc = n3d_encode_tmap_bf16(&K.tmA[b][0], p->a_hi, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+        if (p->nprod == 3 && (rc = n3d_encode_tmap_bf16(&K.tmA[b][1], p->a_lo, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
     }
-    if ((rc = make_tmap(&K.tmB_hi, p->w_hi, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
-    if (p->nprod == 3 && (rc = make_tmap(&K.tmB_lo, p->w_lo, 3, wdims, wbox, block_k)) != N3D_OK) return rc;
+    if ((rc = n3d_encode_tmap_bf16(&K.tmB_hi, p->w_hi, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+    if (p->nprod == 3 && (rc = n3d_encode_tmap_bf16(&K.tmB_lo, p->w_lo, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
 
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];

@@ -36,25 +36,6 @@ struct WParams {
     float* out; int64_t slice_stride;                  // K slice s writes out + s * slice_stride
 };
 
-// One stage: 4 k16 steps x (hi*hi, hi*lo, lo*hi) x two m64 halves, one commit (the accumulation order of conv_gemm_kernel's stage).
-template <int BN>
-__device__ __forceinline__ void wgrad_stage(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
-    constexpr uint32_t h1 = 64u * kBK * 2u;            // rows 64-127 of the A tile
-    constexpr uint64_t dhi = wgmma_desc_hi(kBK);
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kBK / 16; ++k) {
-        const uint32_t koff = (uint32_t)k * 32u;
-        wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-        wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-        wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
-        wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
-        wgmma_bf16<BN>(acc0, wgmma_desc(a_lo + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-        wgmma_bf16<BN>(acc1, wgmma_desc(a_lo + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
-    }
-    wgmma_commit();
-}
-
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const __grid_constant__ WParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -99,7 +80,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const __grid_co
         return;
     }
 
-    // ===================================================== consumer warpgroup
+    // ===================================================== consumer warpgroup: conv_gemm_kernel's stage, so the same summation order.
+    // Every stage adds to zeroed accumulators (not the FIRST form, which could leave -0 for an all-zero sum).
     float acc0[BN / 2], acc1[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
@@ -107,7 +89,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_wgrad_kernel(const __grid_co
     for (int ks = kb; ks < ke; ++ks) {
         mbar_wait(full_bar(s), ph, nullptr, 3);
         const uint32_t sa = smem_base + (uint32_t)s * (uint32_t)P.stage_bytes;
-        wgrad_stage<BN>(acc0, acc1, sa, sa + kABytes, sa + 2 * kABytes, sa + 2 * kABytes + kBBytes);
+        stage_mma<BN, kBK, 3, false>(acc0, acc1, sa, sa + kABytes, sa + 2 * kABytes, sa + 2 * kABytes + kBBytes);
         wgmma_wait<1>();                                 // the previous stage's wgmmas have retired: release it
         __syncwarp();
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
@@ -165,28 +147,11 @@ __global__ void __launch_bounds__(256) wgrad_operand_kernel(const float* __restr
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // 2-D bf16 tensor [rows][cols] with row stride ld elements, box = 64 columns x box_rows rows, SWIZZLE_128B, zero fill outside.
 int make_tmap_2d(CUtensorMap* tm, const void* base, int64_t cols, int64_t rows, int64_t ld, int box_rows) {
-    static EncodeTiledFn enc = nullptr;
-    if (!enc) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) {
-            n3d_set_error("n3d_conv_wgrad: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
-            return N3D_ERR_CUDA;
-        }
-        enc = (EncodeTiledFn)p;
-    }
-    const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows}, gstr[1] = {(cuuint64_t)ld * 2};
-    const cuuint32_t bdim[2] = {(cuuint32_t)kBK, (cuuint32_t)box_rows}, estr[2] = {1, 1};
-    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { n3d_set_error("n3d_conv_wgrad: cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return N3D_ERR_CUDA; }
-    return N3D_OK;
+    const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, stride = (uint64_t)ld * 2;
+    const uint32_t box[2] = {(uint32_t)kBK, (uint32_t)box_rows};
+    return n3d_encode_tmap_bf16(tm, base, 2, dims, &stride, box, CU_TENSOR_MAP_SWIZZLE_128B, "n3d_conv_wgrad");
 }
 
 bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }

@@ -87,8 +87,10 @@ __global__ void __launch_bounds__(256) modulate_split_kernel(const float* __rest
 }
 
 // ---------------------------------------------------------------------------------------------- FIR helpers
-// [1,3,3,1]/8 per axis; upfirdn2d's 2-D filter is the outer product / 64 (setup_filter, upfirdn2d.py:101-111)
-__device__ __constant__ float kFir1[4] = {0.125f, 0.375f, 0.375f, 0.125f};   // immutable constants (not runtime state)
+// [1,3,3,1]/8 per axis; upfirdn2d's 2-D filter is the outer product / 64 (setup_filter, upfirdn2d.py:101-111).  The up path's gain 4
+// is 2 per axis.  constexpr, so that unrolled loops take the taps as immediates.
+__device__ constexpr float kFirUp[4] = {0.25f, 0.75f, 0.75f, 0.25f};
+__device__ constexpr float kFirDown[4] = {0.125f, 0.375f, 0.375f, 0.125f};
 
 struct EpiParams {
     const float* dcoef; const float* bias; const float* noise; int64_t noise_nstride;
@@ -141,6 +143,14 @@ __device__ __forceinline__ EpiCursor epi_cursor(const EpiParams& E, int64_t pix,
     return P;
 }
 
+// Advances the cursor by two output rows of W2 pixels: the next 2x2 block of a strip.
+__device__ __forceinline__ void epi_advance2(EpiCursor& P, const EpiParams& E, int W2) {
+    const int64_t rows2 = 2 * (int64_t)W2;
+    P.f32 += rows2 * E.f32_cstride;
+    P.sp[0] += rows2 * E.out[0].cstride;
+    P.sp[1] += rows2 * E.out[1].cstride;
+}
+
 // bias_act (lrelu with 0 <= slope <= 1: max(t, slope * t)) + clamp + the fp32 / modulated split-bf16 stores of one pixel.
 // nzg = noise * gain; dpix = pixel offset from the cursor (0, 1, W2, W2 + 1).
 __device__ __forceinline__ void epi_store(const EpiParams& E, const EpiVec& V, const EpiCursor& P, const float4& acc, float nzg, int dpix) {
@@ -165,130 +175,214 @@ __device__ __forceinline__ void epi_store(const EpiParams& E, const EpiVec& V, c
     }
 }
 
-// Horizontal pass of the separable 4-tap FIR for one raw row: the NC outputs that start at columns xs .. xs+NC-1 (NC + 3 float4
-// loads at p, p + cs, ...; only the first / last column can fall outside the image: flags vl / vr).  `p` is null for a row outside
-// the image (zero padding).
-template <int NC>
-__device__ __forceinline__ void fir_hrow(const float4* __restrict__ p, int cs, bool vl, bool vr, const float (&g)[4], float4 (&h)[NC]) {
+// The four FIR kernels share their arithmetic through the helpers below (that is what keeps the register-tiled and the streamed
+// forms bit-identical); each kernel keeps only its own work decomposition and data movement.  A thread filters a 2x2 output block
+// per strip step from a window of five horizontally filtered input rows h[0..4], two float4 outputs per row.
+
+// One float4 load of a horizontal pass: __ldg from global memory (register-tiled kernels) or a plain shared-memory load (streamed
+// kernels, from the row ring).
+template <bool GLOBAL>
+__device__ __forceinline__ float4 fir_ld(const float4* p) {
+    if constexpr (GLOBAL) return __ldg(p);
+    else return *p;
+}
+
+// Horizontal pass of the up path over one raw row: the outputs that start at raw columns x0-1 and x0, from the five columns
+// x0-1 .. x0+3 at p, p + cs, ..., p + 4 cs.  Only the first / last column can fall outside the image (flags vl / vr); a row outside
+// the image (in == false) is zero padding and `p` is not read.
+template <bool GLOBAL>
+__device__ __forceinline__ void fir_up_hrow(const float4* __restrict__ p, bool in, int cs, bool vl, bool vr, float4 (&h)[2]) {
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    h[0] = z; h[1] = z;
+    if (!in) return;
+    float4 v[5];
+    v[0] = vl ? fir_ld<GLOBAL>(p) : z;
 #pragma unroll
-    for (int b = 0; b < NC; ++b) h[b] = z;
-    if (!p) return;
-    float4 v[NC + 3];
-    v[0] = vl ? __ldg(p) : z;
+    for (int c = 1; c < 4; ++c) v[c] = fir_ld<GLOBAL>(p + c * cs);
+    v[4] = vr ? fir_ld<GLOBAL>(p + 4 * cs) : z;
 #pragma unroll
-    for (int c = 1; c < NC + 2; ++c) v[c] = __ldg(p + c * cs);
-    v[NC + 2] = vr ? __ldg(p + (NC + 2) * cs) : z;
+    for (int b = 0; b < 2; ++b) {
+        h[b] = f4_scale(kFirUp[0], v[b]);
 #pragma unroll
-    for (int b = 0; b < NC; ++b) {
-        h[b] = f4_scale(g[0], v[b]);
-#pragma unroll
-        for (int fx = 1; fx < 4; ++fx) h[b] = f4_fma(g[fx], v[b + fx], h[b]);
+        for (int fx = 1; fx < 4; ++fx) h[b] = f4_fma(kFirUp[fx], v[b + fx], h[b]);
     }
 }
 
-// thread = (image, strip of S vertically adjacent output row pairs, NC output columns, 4-channel group).  The 4x4 FIR is separable
-// ([1,3,3,1]/8 * 2 per axis).  A 2 x NC output block needs 5 raw rows x (NC + 3) raw columns; consecutive blocks of the strip share
-// 3 of the 5 rows, so the horizontally filtered rows are kept in registers and slid down the strip: 2 (NC + 3) float4 loads per
-// 2 NC outputs instead of 5 (NC + 3) (the unshared form is bound by L2->L1 traffic, 2.5x the raw tensor).
-template <int NC>
+// Vertical pass of the up path over the window h (raw rows y0-1 .. y0+3) and the epilogue of the 2x2 output block at the cursor
+// (nzg = noise * gain per output pixel); then the window slides down two rows.
+__device__ __forceinline__ void fir_up_vstore(const EpiParams& E, const EpiVec& V, const EpiCursor& P, int W2, const float (&nzg)[2][2],
+                                              float4 (&h)[5][2]) {
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+            float4 acc = f4_scale(kFirUp[0], h[a][b]);
+#pragma unroll
+            for (int r = 1; r < 4; ++r) acc = f4_fma(kFirUp[r], h[a + r][b], acc);
+            epi_store(E, V, P, acc, nzg[a][b], a * W2 + b);
+        }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) { h[r][0] = h[r + 2][0]; h[r][1] = h[r + 2][1]; }
+}
+
+// Horizontal pass of the down path, whose window starts two columns left of x0 (input columns x0-2 .. x0+2, x0 even in [0, W]): the
+// first two are outside together (x0 == 0: vl), the next two together (x0 == W: vm), the last one when x0 + 2 >= W (vr).  Rows
+// outside the image as in fir_up_hrow.
+template <bool GLOBAL>
+__device__ __forceinline__ void fir_down_hrow(const float4* __restrict__ p, bool in, int cs, bool vl, bool vm, bool vr, float4 (&h)[2]) {
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    h[0] = z; h[1] = z;
+    if (!in) return;
+    float4 v[5];
+    v[0] = vl ? fir_ld<GLOBAL>(p) : z; v[1] = vl ? fir_ld<GLOBAL>(p + cs) : z;
+    v[2] = vm ? fir_ld<GLOBAL>(p + 2 * cs) : z; v[3] = vm ? fir_ld<GLOBAL>(p + 3 * cs) : z;
+    v[4] = vr ? fir_ld<GLOBAL>(p + 4 * cs) : z;
+    h[0] = f4_scale(kFirDown[0], v[0]); h[1] = f4_scale(kFirDown[0], v[1]);
+#pragma unroll
+    for (int fx = 1; fx < 4; ++fx) { h[0] = f4_fma(kFirDown[fx], v[fx], h[0]); h[1] = f4_fma(kFirDown[fx], v[fx + 1], h[1]); }
+}
+
+// Vertical pass of the down path over the window h (input rows y0-2 .. y0+2): the FIR outputs (y0 + a, x0 + b), zero beyond the
+// (H+1)x(W+1) output, stored as split bf16 to parity image 2a + b at element offset o (parity images par_stride apart); then the
+// window slides down two rows.
+__device__ __forceinline__ void fir_down_vstore(float4 (&h)[5][2], int y0, int x0, int H, int W, int64_t o, int64_t par_stride,
+                                                __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+            float4 v = f4_scale(kFirDown[0], h[a][b]);
+#pragma unroll
+            for (int r = 1; r < 4; ++r) v = f4_fma(kFirDown[r], h[a + r][b], v);
+            if (y0 + a > H || x0 + b > W) v = make_float4(0.f, 0.f, 0.f, 0.f);     // beyond the (H+1)x(W+1) FIR output: zero pad
+            uint2 hh, l;
+            split_bf16x2(v.x, v.y, hh.x, l.x); split_bf16x2(v.z, v.w, hh.y, l.y);
+            const int64_t off = (int64_t)(a * 2 + b) * par_stride + o;
+            *reinterpret_cast<uint2*>(hi + off) = hh;
+            *reinterpret_cast<uint2*>(lo + off) = l;
+        }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) { h[r][0] = h[r + 2][0]; h[r][1] = h[r + 2][1]; }
+}
+
+// Streamed FIR kernels: kFsConsumers consumer threads and one producer warp per CTA.
+constexpr int kFsConsumers = 256, kFsThreads = kFsConsumers + 32;
+
+// Row ring of the streamed FIR kernels in dynamic shared memory: NR stages of row_bytes (one input row segment each), then NR full
+// and NR empty mbarriers.  One producer thread fills the stages with 1-D bulk copies; each consumer warp releases a stage once its
+// lanes have read it.  Producer and consumers walk the same rows in the same order and skip the same rows outside the image.
+struct FirRing {
+    uint8_t* smem;
+    uint32_t row_bytes, bars;
+    int NR, s;              // stage count, current stage
+    uint32_t ph;            // parity of the current stage's phase
+
+    __device__ FirRing(uint8_t* smem_, int NR_, uint32_t row_bytes_)
+        : smem(smem_), row_bytes(row_bytes_), bars(n3d_tc::smem_u32(smem_) + (uint32_t)NR_ * row_bytes_), NR(NR_), s(0), ph(0) {}
+    __device__ uint32_t full_bar(int k) const { return bars + 8u * (uint32_t)k; }
+    __device__ uint32_t empty_bar(int k) const { return bars + 8u * (uint32_t)(NR + k); }
+    __device__ void advance() { if (++s == NR) { s = 0; ph ^= 1u; } }
+
+    // Called by every thread of the CTA: thread 0 initialises the barriers, then the CTA synchronises.
+    __device__ void init() const {
+        if (threadIdx.x == 0) {
+            for (int k = 0; k < NR; ++k) { n3d_tc::mbar_init(full_bar(k), 1); n3d_tc::mbar_init(empty_bar(k), kFsConsumers / 32); }
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        }
+        __syncthreads();
+    }
+
+    // Producer (one thread): rows r0 .. r1 of the NHWC image `img` [rows][cols][C], rows outside [0, rows) skipped (zero padding).  Each
+    // stage receives columns c0 .. c1 of one row clipped to the image, a contiguous segment placed so that column c0 + i is always at
+    // byte i * C * 4 of the stage.
+    __device__ void produce(const float* img, int rows, int cols, int C, int r0, int r1, int c0, int c1) {
+        using namespace n3d_tc;
+        const int col_lo = max(c0, 0), col_hi = min(c1, cols - 1);
+        const uint32_t bytes = (uint32_t)(col_hi - col_lo + 1) * (uint32_t)C * 4u;
+        const uint32_t dst = smem_u32(smem) + (uint32_t)(col_lo - c0) * (uint32_t)C * 4u;
+        const float* src = img + (int64_t)col_lo * C;
+        for (int r = r0; r <= r1; ++r) {
+            if (r < 0 || r >= rows) continue;
+            mbar_wait_short(empty_bar(s), ph ^ 1u);
+            mbar_expect_tx(full_bar(s), bytes);
+            bulk_load_1d(dst + (uint32_t)s * row_bytes, src + (int64_t)r * cols * C, bytes, full_bar(s));
+            advance();
+        }
+    }
+
+    // Consumer: waits until the current stage has landed and returns `p` (a location in stage 0) moved to it.
+    __device__ const float4* acquire(const float4* p) const {
+        n3d_tc::mbar_wait_short(full_bar(s), ph);
+        return reinterpret_cast<const float4*>(reinterpret_cast<const uint8_t*>(p) + s * row_bytes);
+    }
+    // Consumer: every lane of the warp has read the current stage; lane 0 hands it back to the producer.
+    __device__ void release(int lane) {
+        __syncwarp();
+        if (lane == 0) n3d_tc::mbar_arrive(empty_bar(s));
+        advance();
+    }
+};
+
+// thread = (image, strip of S vertically adjacent output row pairs, 2 output columns, 4-channel group).  The 4x4 FIR is separable
+// ([1,3,3,1]/8 * 2 per axis).  A 2x2 output block needs 5 raw rows x 4 raw columns; consecutive blocks of the strip share 3 of the
+// 5 rows, so the horizontally filtered rows are kept in registers and slid down the strip: 10 float4 loads per 4 outputs instead
+// of 25 (the unshared form is bound by L2->L1 traffic, 2.5x the raw tensor).
 __global__ void __launch_bounds__(256) fir_up_epilogue_kernel(const float* __restrict__ raw, int N, int H2, int W2, int C, int S, EpiParams E) {
-    const int RH = H2 + 1, RW = W2 + 1, c4n = C >> 2, BH = H2 >> 1, BW = W2 / NC, nstrip = (BH + S - 1) / S;
+    const int RH = H2 + 1, RW = W2 + 1, c4n = C >> 2, BH = H2 >> 1, BW = W2 / 2, nstrip = (BH + S - 1) / S;
     const int64_t total = (int64_t)N * nstrip * BW * c4n;
     const int64_t rstride = (int64_t)RW * c4n;                  // raw row stride in float4
-    const float g[4] = {0.25f, 0.75f, 0.75f, 0.25f};
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c4 = (int)(i % c4n);
         int64_t t = i / c4n;
         const int bx = (int)(t % BW); t /= BW;
         const int st = (int)(t % nstrip);
         const int n = (int)(t / nstrip);
-        const int x0 = bx * NC, c0 = c4 * 4;
+        const int x0 = bx * 2, c0 = c4 * 4;
         const int by_begin = st * S, by_end = min(by_begin + S, BH);
-        const bool vl = x0 > 0, vr = x0 + NC + 1 < RW;         // raw columns x0-1 .. x0+NC+1
+        const bool vl = x0 > 0, vr = x0 + 3 < RW;               // raw columns x0-1 .. x0+3
         // float4 pointer to raw(n, row 0, column x0-1, c0); rows are addressed relative to it
         const float4* col = reinterpret_cast<const float4*>(raw) + ((int64_t)n * RH * RW + (x0 - 1)) * c4n + c4;
-        auto rowp = [&](int ry) -> const float4* { return (ry >= 0 && ry < RH) ? col + ry * rstride : nullptr; };
+        auto hrow = [&](int ry, float4 (&h)[2]) { fir_up_hrow<true>(col + ry * rstride, ry >= 0 && ry < RH, c4n, vl, vr, h); };
         const EpiVec V = epi_load(E, n, C, c0);
         const float* nzp = E.noise ? E.noise + (int64_t)n * E.noise_nstride + x0 : nullptr;
-        float4 h[5][NC];
+        float4 h[5][2];
 #pragma unroll
-        for (int r = 0; r < 3; ++r) fir_hrow<NC>(rowp(2 * by_begin - 1 + r), c4n, vl, vr, g, h[r]);
+        for (int r = 0; r < 3; ++r) hrow(2 * by_begin - 1 + r, h[r]);
         EpiCursor P = epi_cursor(E, ((int64_t)n * H2 + 2 * by_begin) * W2 + x0, c0);
-        const int64_t adv_f32 = 2 * (int64_t)W2 * E.f32_cstride, adv0 = 2 * (int64_t)W2 * E.out[0].cstride, adv1 = 2 * (int64_t)W2 * E.out[1].cstride;
-        for (int by = by_begin; by < by_end; ++by, P.f32 += adv_f32, P.sp[0] += adv0, P.sp[1] += adv1) {
+        for (int by = by_begin; by < by_end; ++by, epi_advance2(P, E, W2)) {
             const int y0 = by * 2;
-            fir_hrow<NC>(rowp(y0 + 2), c4n, vl, vr, g, h[3]);
-            fir_hrow<NC>(rowp(y0 + 3), c4n, vl, vr, g, h[4]);
-            float nz[2][NC];
+            hrow(y0 + 2, h[3]);
+            hrow(y0 + 3, h[4]);
+            float nzg[2][2];
 #pragma unroll
             for (int a = 0; a < 2; ++a)
 #pragma unroll
-                for (int b = 0; b < NC; ++b) nz[a][b] = nzp ? __fmul_rn(E.gain, __ldg(nzp + (int64_t)(y0 + a) * W2 + b)) : 0.f;   // explicit: no FMA contraction into the bias add
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int b = 0; b < NC; ++b) {
-                    float4 acc = f4_scale(g[0], h[a][b]);
-#pragma unroll
-                    for (int r = 1; r < 4; ++r) acc = f4_fma(g[r], h[a + r][b], acc);
-                    epi_store(E, V, P, acc, nz[a][b], a * W2 + b);
-                }
-#pragma unroll
-            for (int r = 0; r < 3; ++r)
-#pragma unroll
-                for (int b = 0; b < NC; ++b) h[r][b] = h[r + 2][b];
+                for (int b = 0; b < 2; ++b) nzg[a][b] = nzp ? __fmul_rn(E.gain, __ldg(nzp + (int64_t)(y0 + a) * W2 + b)) : 0.f;   // explicit: no FMA contraction into the bias add
+            fir_up_vstore(E, V, P, W2, nzg, h);
         }
     }
 }
 
 // ---------------------------------------------------------------------------------------------- streamed FIR-up epilogue
-// Same arithmetic as fir_up_epilogue_kernel<2> (bit-identical results), different data movement.  The register-tiled kernel above is
-// bound by load latency at 16 warps/SM: every strip step waits for its own ten
-// 16-byte loads.  Here a CTA owns a (TR output rows) x (TC output columns) x (all C channels) tile of one image and a producer
-// thread streams the raw rows it needs -- each a CONTIGUOUS (TC + 3) * C * 4-byte segment of the NHWC tensor -- through a ring of
-// shared-memory stages with 1-D bulk copies (TMA engine, mbarrier full / empty pairs); the eight consumer warps read the five
+// Same arithmetic as fir_up_epilogue_kernel (bit-identical results), different data movement.  The register-tiled kernel above is
+// bound by load latency at 16 warps/SM: every strip step waits for its own ten 16-byte loads.  Here a CTA owns a (TR output rows)
+// x (TC output columns) x (all C channels) tile of one image and a producer thread streams the raw rows it needs -- each a
+// CONTIGUOUS (TC + 3) * C * 4-byte segment of the NHWC tensor -- through the row ring; the eight consumer warps read the five
 // columns of their 2-column output block from shared memory.  Loads are in flight NR rows ahead of the arithmetic and cost no
 // registers.  thread = (column pair, 4-channel group): (TC / 2) * (C / 4) == 256.
-constexpr int kFsConsumers = 256, kFsThreads = kFsConsumers + 32;
-
 __global__ void __launch_bounds__(kFsThreads, 2) fir_up_stream_kernel(const float* __restrict__ raw, int N, int H2, int W2, int C, int TC, int TR, int NR,
                                                                        EpiParams E) {
-    using namespace n3d_tc;
     extern __shared__ __align__(128) uint8_t fs_smem[];
     const int RH = H2 + 1, RW = W2 + 1, c4n = C >> 2;
-    const int row_f4 = (TC + 3) * c4n;                          // float4 per stage (one raw row segment)
-    const uint32_t row_bytes = (uint32_t)row_f4 * 16u;
-    const uint32_t ring = smem_u32(fs_smem), bars = ring + (uint32_t)NR * row_bytes;
-    auto full_bar = [&](int s) { return bars + 8u * (uint32_t)s; };
-    auto empty_bar = [&](int s) { return bars + 8u * (uint32_t)(NR + s); };
+    FirRing ring(fs_smem, NR, (uint32_t)(TC + 3) * (uint32_t)C * 4u);
     const int tiles_x = W2 / TC, tiles_y = H2 / TR;
     const int bx = blockIdx.x % tiles_x, by = (blockIdx.x / tiles_x) % tiles_y, n = blockIdx.x / (tiles_x * tiles_y);
     const int X0 = bx * TC, Y0 = by * TR;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    ring.init();
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NR; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kFsConsumers / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    if (warp == kFsConsumers / 32) {
-        // ===================================================== producer: raw rows Y0-1 .. Y0+TR+1, columns X0-1 .. X0+TC+1 (clipped)
-        if (lane == 0) {
-            const int col_lo = max(X0 - 1, 0), col_hi = min(X0 + TC + 1, RW - 1);
-            const uint32_t bytes = (uint32_t)(col_hi - col_lo + 1) * (uint32_t)C * 4u;
-            const uint32_t dst_off = (uint32_t)(col_lo - (X0 - 1)) * (uint32_t)C * 4u;
-            const float* src = raw + ((int64_t)n * RH * RW + col_lo) * C;
-            int s = 0; uint32_t ph = 0;
-            for (int ry = Y0 - 1; ry <= Y0 + TR + 1; ++ry) {
-                if (ry < 0 || ry >= RH) continue;               // zero padding: the consumers skip the same rows
-                mbar_wait_short(empty_bar(s), ph ^ 1u);
-                mbar_expect_tx(full_bar(s), bytes);
-                bulk_load_1d(ring + (uint32_t)s * row_bytes + dst_off, src + (int64_t)ry * RW * C, bytes, full_bar(s));
-                if (++s == NR) { s = 0; ph ^= 1u; }
-            }
-        }
+    if (warp == kFsConsumers / 32) {                            // producer: raw rows Y0-1 .. Y0+TR+1, columns X0-1 .. X0+TC+1
+        if (lane == 0) ring.produce(raw + (int64_t)n * RH * RW * C, RH, RW, C, Y0 - 1, Y0 + TR + 1, X0 - 1, X0 + TC + 1);
         return;
     }
 
@@ -296,29 +390,11 @@ __global__ void __launch_bounds__(kFsThreads, 2) fir_up_stream_kernel(const floa
     const int c4 = threadIdx.x % c4n, j = threadIdx.x / c4n;
     const int x0 = X0 + 2 * j, c0 = c4 * 4;
     const bool vl = x0 > 0, vr = x0 + 3 < RW;                   // raw columns x0-1 .. x0+3
-    const float4* base = reinterpret_cast<const float4*>(fs_smem) + (2 * j) * c4n + c4;
-    const float g[4] = {0.25f, 0.75f, 0.75f, 0.25f};
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    int s = 0; uint32_t ph = 0;
-    auto hrow = [&](int ry, float4 (&h)[2]) {
-        h[0] = z; h[1] = z;
-        if (ry < 0 || ry >= RH) return;
-        mbar_wait_short(full_bar(s), ph);
-        const float4* p = base + s * row_f4;
-        float4 v[5];
-        v[0] = vl ? p[0] : z;
-#pragma unroll
-        for (int q = 1; q < 4; ++q) v[q] = p[q * c4n];
-        v[4] = vr ? p[4 * c4n] : z;
-#pragma unroll
-        for (int b = 0; b < 2; ++b) {
-            h[b] = f4_scale(g[0], v[b]);
-#pragma unroll
-            for (int fx = 1; fx < 4; ++fx) h[b] = f4_fma(g[fx], v[b + fx], h[b]);
-        }
-        __syncwarp();                                           // every lane has consumed its values: the stage may be refilled
-        if (lane == 0) mbar_arrive(empty_bar(s));
-        if (++s == NR) { s = 0; ph ^= 1u; }
+    const float4* base = reinterpret_cast<const float4*>(fs_smem) + (2 * j) * c4n + c4;      // raw column x0-1 in stage 0
+    auto hrow = [&](int ry, float4 (&h)[2]) {                  // one call: written as in fir_down_stream_kernel, this kernel spills
+        const bool in = ry >= 0 && ry < RH;
+        fir_up_hrow<false>(in ? ring.acquire(base) : nullptr, in, c4n, vl, vr, h);
+        if (in) ring.release(lane);
     };
     const EpiVec V = epi_load(E, n, C, c0);
     const float* nzp = E.noise ? E.noise + (int64_t)n * E.noise_nstride + x0 : nullptr;
@@ -326,7 +402,6 @@ __global__ void __launch_bounds__(kFsThreads, 2) fir_up_stream_kernel(const floa
 #pragma unroll
     for (int r = 0; r < 3; ++r) hrow(Y0 - 1 + r, h[r]);
     EpiCursor P = epi_cursor(E, ((int64_t)n * H2 + Y0) * W2 + x0, c0);
-    const int64_t adv_f32 = 2 * (int64_t)W2 * E.f32_cstride, adv0 = 2 * (int64_t)W2 * E.out[0].cstride, adv1 = 2 * (int64_t)W2 * E.out[1].cstride;
     // the noise of a 2x2 block is fetched one strip step ahead, so that its global-load latency does not sit between the FIR and the
     // stores
     float nzn[2][2];
@@ -337,28 +412,16 @@ __global__ void __launch_bounds__(kFsThreads, 2) fir_up_stream_kernel(const floa
             for (int b = 0; b < 2; ++b) nzn[a][b] = nzp ? __ldg(nzp + (int64_t)(y0 + a) * W2 + b) : 0.f;
     };
     load_noise(Y0);
-    for (int y0 = Y0; y0 < Y0 + TR; y0 += 2, P.f32 += adv_f32, P.sp[0] += adv0, P.sp[1] += adv1) {
-        float nz[2][2];
+    for (int y0 = Y0; y0 < Y0 + TR; y0 += 2, epi_advance2(P, E, W2)) {
+        float nzg[2][2];
 #pragma unroll
         for (int a = 0; a < 2; ++a)
 #pragma unroll
-            for (int b = 0; b < 2; ++b) nz[a][b] = __fmul_rn(E.gain, nzn[a][b]);     // same rounding as the register-tiled kernel
+            for (int b = 0; b < 2; ++b) nzg[a][b] = __fmul_rn(E.gain, nzn[a][b]);     // same rounding as the register-tiled kernel
         if (y0 + 2 < Y0 + TR) load_noise(y0 + 2);
         hrow(y0 + 2, h[3]);
         hrow(y0 + 3, h[4]);
-#pragma unroll
-        for (int a = 0; a < 2; ++a)
-#pragma unroll
-            for (int b = 0; b < 2; ++b) {
-                float4 acc = f4_scale(g[0], h[a][b]);
-#pragma unroll
-                for (int r = 1; r < 4; ++r) acc = f4_fma(g[r], h[a + r][b], acc);
-                epi_store(E, V, P, acc, nz[a][b], a * W2 + b);
-            }
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int b = 0; b < 2; ++b) h[r][b] = h[r + 2][b];
+        fir_up_vstore(E, V, P, W2, nzg, h);
     }
 }
 
@@ -384,21 +447,6 @@ __global__ void __launch_bounds__(256) splitk_epilogue_kernel(const float* __res
     }
 }
 
-// Same for the down path, where the window starts two columns left of x0 (input columns x0-2 .. x0+2, x0 even in [0, W]): the
-// first two are outside together (x0 == 0: vl), the next two together (x0 == W: vm), the last one when x0 + 2 >= W (vr).
-__device__ __forceinline__ void fir_hrow_down(const float4* __restrict__ p, int cs, bool vl, bool vm, bool vr, const float (&g)[4], float4& h0, float4& h1) {
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    h0 = z; h1 = z;
-    if (!p) return;
-    float4 v[5];
-    v[0] = vl ? __ldg(p) : z; v[1] = vl ? __ldg(p + cs) : z;
-    v[2] = vm ? __ldg(p + 2 * cs) : z; v[3] = vm ? __ldg(p + 3 * cs) : z;
-    v[4] = vr ? __ldg(p + 4 * cs) : z;
-    h0 = f4_scale(g[0], v[0]); h1 = f4_scale(g[0], v[1]);
-#pragma unroll
-    for (int fx = 1; fx < 4; ++fx) { h0 = f4_fma(g[fx], v[fx], h0); h1 = f4_fma(g[fx], v[fx + 1], h1); }
-}
-
 // FIR (pad 2,2,2,2) -> [(H+1),(W+1)] -> parity-split bf16 hi/lo, layout [4 parities][N][SH][SW][C].
 // thread = (image, strip of S sub-pixel rows, sub-pixel column sx, 4-channel group) -> per sub-pixel the 2x2 block of FIR outputs
 // (2sy+a, 2sx+b), one per parity image; same register-resident sliding window over the horizontally filtered rows as above.
@@ -407,7 +455,6 @@ __global__ void __launch_bounds__(256) fir_down_split_kernel(const float* __rest
     const int SH = (H + 2) / 2, SW = (W + 2) / 2, c4n = C >> 2, nstrip = (SH + S - 1) / S;
     const int64_t total = (int64_t)N * nstrip * SW * c4n;
     const int64_t par_stride = (int64_t)N * SH * SW * C;
-    const float g[4] = {0.125f, 0.375f, 0.375f, 0.125f};
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c4 = (int)(i % c4n);
         int64_t t = i / c4n;
@@ -419,31 +466,15 @@ __global__ void __launch_bounds__(256) fir_down_split_kernel(const float* __rest
         const bool vl = x0 >= 2, vm = x0 < W, vr = x0 + 2 < W;
         const float4* col = reinterpret_cast<const float4*>(x) + ((int64_t)n * H * W + (x0 - 2)) * c4n + c4;
         const int64_t rstride = (int64_t)W * c4n;
-        auto rowp = [&](int iy) -> const float4* { return (iy >= 0 && iy < H) ? col + iy * rstride : nullptr; };
+        auto hrow = [&](int iy, float4 (&h)[2]) { fir_down_hrow<true>(col + iy * rstride, iy >= 0 && iy < H, c4n, vl, vm, vr, h); };
         float4 h[5][2];
 #pragma unroll
-        for (int r = 0; r < 3; ++r) fir_hrow_down(rowp(2 * sy_begin - 2 + r), c4n, vl, vm, vr, g, h[r][0], h[r][1]);
+        for (int r = 0; r < 3; ++r) hrow(2 * sy_begin - 2 + r, h[r]);
         for (int sy = sy_begin; sy < sy_end; ++sy) {
             const int y0 = sy * 2;
-            fir_hrow_down(rowp(y0 + 1), c4n, vl, vm, vr, g, h[3][0], h[3][1]);
-            fir_hrow_down(rowp(y0 + 2), c4n, vl, vm, vr, g, h[4][0], h[4][1]);
-            const int64_t o = (((int64_t)n * SH + sy) * SW + sx) * C + c4 * 4;
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int b = 0; b < 2; ++b) {
-                    float4 v = f4_scale(g[0], h[a][b]);
-#pragma unroll
-                    for (int r = 1; r < 4; ++r) v = f4_fma(g[r], h[a + r][b], v);
-                    if (y0 + a > H || x0 + b > W) v = make_float4(0.f, 0.f, 0.f, 0.f);     // beyond the (H+1)x(W+1) FIR output: zero pad
-                    uint2 hh, l;
-                    split_bf16x2(v.x, v.y, hh.x, l.x); split_bf16x2(v.z, v.w, hh.y, l.y);
-                    const int64_t off = (int64_t)(a * 2 + b) * par_stride + o;
-                    *reinterpret_cast<uint2*>(hi + off) = hh;
-                    *reinterpret_cast<uint2*>(lo + off) = l;
-                }
-#pragma unroll
-            for (int r = 0; r < 3; ++r) { h[r][0] = h[r + 2][0]; h[r][1] = h[r + 2][1]; }
+            hrow(y0 + 1, h[3]);
+            hrow(y0 + 2, h[4]);
+            fir_down_vstore(h, y0, x0, H, W, (((int64_t)n * SH + sy) * SW + sx) * C + c4 * 4, par_stride, hi, lo);
         }
     }
 }
@@ -453,41 +484,18 @@ __global__ void __launch_bounds__(256) fir_down_split_kernel(const float* __rest
 // 2 TS + 3 input rows -- contiguous (2 TSC + 3) * C * 4-byte segments -- through the shared-memory ring with 1-D bulk copies.
 __global__ void __launch_bounds__(kFsThreads, 2) fir_down_stream_kernel(const float* __restrict__ x, int N, int H, int W, int C, int TSC, int TS, int NR,
                                                                          __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
-    using namespace n3d_tc;
     extern __shared__ __align__(128) uint8_t fs_smem[];
     const int SH = (H + 2) / 2, SW = (W + 2) / 2, c4n = C >> 2;
-    const int row_f4 = (2 * TSC + 3) * c4n;
-    const uint32_t row_bytes = (uint32_t)row_f4 * 16u;
-    const uint32_t ring = smem_u32(fs_smem), bars = ring + (uint32_t)NR * row_bytes;
-    auto full_bar = [&](int s) { return bars + 8u * (uint32_t)s; };
-    auto empty_bar = [&](int s) { return bars + 8u * (uint32_t)(NR + s); };
+    FirRing ring(fs_smem, NR, (uint32_t)(2 * TSC + 3) * (uint32_t)C * 4u);
     const int tiles_x = (SW + TSC - 1) / TSC, tiles_y = (SH + TS - 1) / TS;
     const int bx = blockIdx.x % tiles_x, by = (blockIdx.x / tiles_x) % tiles_y, n = blockIdx.x / (tiles_x * tiles_y);
     const int SX0 = bx * TSC, SY0 = by * TS, rows_here = min(TS, SH - SY0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < NR; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kFsConsumers / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
+    ring.init();
     const int iy_first = 2 * SY0 - 2, iy_last = 2 * (SY0 + rows_here - 1) + 2;
 
-    if (warp == kFsConsumers / 32) {
-        if (lane == 0) {                                        // producer: input columns 2 SX0 - 2 .. 2 SX0 + 2 TSC, clipped to the image
-            const int col_lo = max(2 * SX0 - 2, 0), col_hi = min(2 * SX0 + 2 * TSC, W - 1);
-            const uint32_t bytes = (uint32_t)(col_hi - col_lo + 1) * (uint32_t)C * 4u;
-            const uint32_t dst_off = (uint32_t)(col_lo - (2 * SX0 - 2)) * (uint32_t)C * 4u;
-            const float* src = x + ((int64_t)n * H * W + col_lo) * C;
-            int s = 0; uint32_t ph = 0;
-            for (int iy = iy_first; iy <= iy_last; ++iy) {
-                if (iy < 0 || iy >= H) continue;
-                mbar_wait_short(empty_bar(s), ph ^ 1u);
-                mbar_expect_tx(full_bar(s), bytes);
-                bulk_load_1d(ring + (uint32_t)s * row_bytes + dst_off, src + (int64_t)iy * W * C, bytes, full_bar(s));
-                if (++s == NR) { s = 0; ph ^= 1u; }
-            }
-        }
+    if (warp == kFsConsumers / 32) {                            // producer: input columns 2 SX0 - 2 .. 2 SX0 + 2 TSC
+        if (lane == 0) ring.produce(x + (int64_t)n * H * W * C, H, W, C, iy_first, iy_last, 2 * SX0 - 2, 2 * SX0 + 2 * TSC);
         return;
     }
 
@@ -495,53 +503,21 @@ __global__ void __launch_bounds__(kFsThreads, 2) fir_down_stream_kernel(const fl
     const int sx = SX0 + j, x0 = 2 * sx;
     const bool active = sx < SW;                                // the last column tile is ragged (SW = W / 2 + 1)
     const bool vl = active && x0 >= 2, vm = active && x0 < W, vr = active && x0 + 2 < W;
-    const float4* base = reinterpret_cast<const float4*>(fs_smem) + (2 * j) * c4n + c4;      // input column x0 - 2
-    const float g[4] = {0.125f, 0.375f, 0.375f, 0.125f};
-    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-    int s = 0; uint32_t ph = 0;
-    auto hrow = [&](int iy, float4& h0, float4& h1) {
-        h0 = z; h1 = z;
-        if (iy < 0 || iy >= H) return;
-        mbar_wait_short(full_bar(s), ph);
-        const float4* p = base + s * row_f4;
-        float4 v[5];
-        v[0] = vl ? p[0] : z; v[1] = vl ? p[c4n] : z;
-        v[2] = vm ? p[2 * c4n] : z; v[3] = vm ? p[3 * c4n] : z;
-        v[4] = vr ? p[4 * c4n] : z;
-        h0 = f4_scale(g[0], v[0]); h1 = f4_scale(g[0], v[1]);
-#pragma unroll
-        for (int fx = 1; fx < 4; ++fx) { h0 = f4_fma(g[fx], v[fx], h0); h1 = f4_fma(g[fx], v[fx + 1], h1); }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(s));
-        if (++s == NR) { s = 0; ph ^= 1u; }
+    const float4* base = reinterpret_cast<const float4*>(fs_smem) + (2 * j) * c4n + c4;      // input column x0 - 2 in stage 0
+    auto hrow = [&](int iy, float4 (&h)[2]) {                  // two calls: fewer instructions per row than fir_up_stream_kernel's form
+        if (iy < 0 || iy >= H) return fir_down_hrow<false>(nullptr, false, c4n, vl, vm, vr, h);
+        fir_down_hrow<false>(ring.acquire(base), true, c4n, vl, vm, vr, h);
+        ring.release(lane);
     };
     const int64_t par_stride = (int64_t)N * SH * SW * C;
-    float4 h[5][2];
+    float4 h[5][2];                                             // all zero in an inactive thread: it needs no slide
 #pragma unroll
-    for (int r = 0; r < 3; ++r) hrow(iy_first + r, h[r][0], h[r][1]);
+    for (int r = 0; r < 3; ++r) hrow(iy_first + r, h[r]);
     for (int sy = SY0; sy < SY0 + rows_here; ++sy) {
         const int y0 = sy * 2;
-        hrow(y0 + 1, h[3][0], h[3][1]);
-        hrow(y0 + 2, h[4][0], h[4][1]);
-        if (active) {
-            const int64_t o = (((int64_t)n * SH + sy) * SW + sx) * C + c4 * 4;
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int b = 0; b < 2; ++b) {
-                    float4 v = f4_scale(g[0], h[a][b]);
-#pragma unroll
-                    for (int r = 1; r < 4; ++r) v = f4_fma(g[r], h[a + r][b], v);
-                    if (y0 + a > H || x0 + b > W) v = z;        // beyond the (H+1)x(W+1) FIR output: zero pad
-                    uint2 hh, l;
-                    split_bf16x2(v.x, v.y, hh.x, l.x); split_bf16x2(v.z, v.w, hh.y, l.y);
-                    const int64_t off = (int64_t)(a * 2 + b) * par_stride + o;
-                    *reinterpret_cast<uint2*>(hi + off) = hh;
-                    *reinterpret_cast<uint2*>(lo + off) = l;
-                }
-        }
-#pragma unroll
-        for (int r = 0; r < 3; ++r) { h[r][0] = h[r + 2][0]; h[r][1] = h[r + 2][1]; }
+        hrow(y0 + 1, h[3]);
+        hrow(y0 + 2, h[4]);
+        if (active) fir_down_vstore(h, y0, x0, H, W, (((int64_t)n * SH + sy) * SW + sx) * C + c4 * 4, par_stride, hi, lo);
     }
 }
 
@@ -619,7 +595,7 @@ __global__ void __launch_bounds__(256) downsample2d_kernel(const float* __restri
             for (int fx = 0; fx < 4; ++fx) {
                 const int ix = ox * 2 + fx - 1;
                 if (ix < 0 || ix >= W) continue;
-                acc += (kFir1[fy] * kFir1[fx]) * __ldg(x + (((int64_t)n * H + iy) * W + ix) * C + c);
+                acc += (kFirDown[fy] * kFirDown[fx]) * __ldg(x + (((int64_t)n * H + iy) * W + ix) * C + c);
             }
         }
         y[i] = acc;
@@ -731,7 +707,7 @@ extern "C" int n3d_fir_up_epilogue(const float* raw, int N, int H2, int W2, int 
     const int S = fir_strip_rows(sms, (int64_t)N * (W2 / 2) * (C / 4), H2 / 2);
     const int64_t total = (int64_t)N * n3d_div_up(H2 / 2, S) * (W2 / 2) * (C / 4);
     // 2 output columns per thread: the two columns share each input row's loads
-    fir_up_epilogue_kernel<2><<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(raw, N, H2, W2, C, S, E);
+    fir_up_epilogue_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(raw, N, H2, W2, C, S, E);
     N3D_CHECK_LAUNCH("n3d_fir_up_epilogue");
     return N3D_OK;
 }

@@ -223,6 +223,31 @@ __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uin
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(da), "l"(db), "r"(scale_d));
 }
+// One pipeline stage of a 128-row tile's MMAs (conv_gemm_kernel and conv_wgrad_kernel) as a fixed instruction sequence: one fence,
+// BK/16 x NPROD x 2 wgmmas back to back, one commit.  The warpgroup owns all 128 rows of the A tile: acc0 = rows 0-63, acc1 = rows
+// 64-127 (two m64 wgmmas sharing the B descriptor).  Per k16 step the products are hi*hi, then (NPROD == 3) hi*lo and lo*hi, so
+// every kernel that runs this stage sums in the same order.  FIRST (the first stage of a tile) overwrites the accumulator with its
+// first product instead of adding to it.
+template <int BN, int BK, int NPROD, bool FIRST>
+__device__ __forceinline__ void stage_mma(float (&acc0)[BN / 2], float (&acc1)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+    constexpr uint32_t h1 = 64u * BK * 2u;         // rows 64-127 of the A tile
+    constexpr uint64_t dhi = wgmma_desc_hi(BK);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+        const uint32_t koff = (uint32_t)k * 32u;     // 16 bf16 = 32 bytes inside the swizzle row
+        wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
+        wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), (FIRST && k == 0) ? 0u : 1u);
+        if (NPROD == 3) {
+            wgmma_bf16<BN>(acc0, wgmma_desc(a_hi + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc1, wgmma_desc(a_hi + h1 + koff, dhi), wgmma_desc(b_lo + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc0, wgmma_desc(a_lo + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
+            wgmma_bf16<BN>(acc1, wgmma_desc(a_lo + h1 + koff, dhi), wgmma_desc(b_hi + koff, dhi), 1u);
+        }
+    }
+    wgmma_commit();
+}
+
 // warp-level D[16 x 8] += A[16 x 16] * B[16 x 8], bf16 operands in registers (PTX fragment layouts of mma.m16n8k16), fp32 accumulate
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"

@@ -1,5 +1,6 @@
 """Micro-benchmark of the up-conv building blocks at the generator's layer shapes (batch 8): transposed-conv GEMM launch,
-FIR-up epilogue, FIR-down split.  CUDA-event timing, L2 flushed (256 MB write) before every timed launch.
+FIR-up epilogue, FIR-down split (each FIR in both forms: N3D_FIR_STREAM=0 / 1).  CUDA-event timing, L2 flushed (256 MB write) before
+every timed launch.
 Usage (GPU box): python tools/bench_layers.py [tag]"""
 import os
 import sys
@@ -76,9 +77,12 @@ def main(tag):
         sh = (res + 2) // 2
         hi = torch.empty(4, N, sh, sh, c, device=DEV, dtype=torch.bfloat16)
         lo = torch.empty_like(hi)
-        us = timeit(lambda: K.fir_down_split(x, hi, lo))
         gb = x.numel() * 4 + hi.numel() * 4
-        print(f'fir_dn  C={c:4d} in  {res:3d}^2      {us:8.1f} us  {gb / us * 1e-3:6.0f} GB/s')
+        for mode in ('0', '1'):                      # 0: register-tiled kernel, 1: streamed kernel where eligible
+            os.environ['N3D_FIR_STREAM'] = mode
+            us = timeit(lambda: K.fir_down_split(x, hi, lo))
+            print(f'fir_dn  C={c:4d} in  {res:3d}^2 stream={mode} {us:8.1f} us  {gb / us * 1e-3:6.0f} GB/s')
+        os.environ.pop('N3D_FIR_STREAM')
 
 
 if __name__ == '__main__':
