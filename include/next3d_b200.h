@@ -43,7 +43,8 @@ int n3d_version(void);
 /* y = clamp(act(x + b[(i / step_b) % size_b]) * gain, +-clamp)   -- replaces bias_act_plugin.bias_act
  * (bias_act.cpp:36-94, kernel bias_act.cu:28-151; forward, grad == 0; the grad modes are n3d_bias_act_grad).  act: 1 linear, 2 relu, 3 lrelu,
  * 4 tanh, 5 sigmoid, 6 elu, 7 selu, 8 softplus, 9 swish (the reference's cuda_idx, bias_act.py:23-33).
- * x dense (any memory format), b contiguous or NULL, clamp < 0 disables clamping. */
+ * x dense (any memory format), b contiguous or NULL, clamp < 0 disables clamping.  x and y may start anywhere (a view into a larger
+ * storage): 4-element vector accesses are used only when both are aligned for them (16 bytes fp32, 8 bytes fp16). */
 int n3d_bias_act(const void* x, const void* b, void* y, int dtype, int64_t numel, int size_b, int step_b,
                  int act, float alpha, float gain, float clamp, void* stream);
 
@@ -196,7 +197,9 @@ int n3d_conv_wgrad(const N3DConvWgrad* p, void* stream);
 int n3d_wgrad_operand(const float* x, const int64_t x_strides[4], int N, int C, int H, int W, int s, int pt, int pl, int PH, int PW,
                       int shift, int64_t ld, void* hi, void* lo, void* stream);
 
-/* fp32 NHWC -> split bf16 NHWC with optional per-(n,c) modulation: out = split(x[n,y,x,c] * style[n,c]). */
+/* fp32 NHWC -> split bf16 NHWC with optional per-(n,c) modulation: out = split(x[n,y,x,c] * style[n,c]).
+ * Alignment: x and style 16-byte aligned (float4 loads), hi and lo 8-byte aligned (4-channel stores); C, out_cstride and out_coff
+ * multiples of 4; else N3D_ERR_INVALID_ARG. */
 int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* hi, void* lo,
                        int out_cstride, int out_coff, void* stream);
 
@@ -217,11 +220,14 @@ int n3d_splitk_epilogue(const float* partial, int S, int64_t split_stride, int N
 
 /* First half of a down-sampling conv (conv2d_resample.py:108-111): fp32 NHWC [H,W] -> FIR pad (2,2,2,2) -> [(H+1),(W+1)]
  * -> split bf16, de-interleaved by pixel parity into 4 sub-images [4, N, SH, SW, C] (parity (y&1)*2 + (x&1), pixel
- * (y>>1, x>>1)), SH = (H+2)/2, so that the stride-2 conv becomes 9 unit-stride taps. */
+ * (y>>1, x>>1)), SH = (H+2)/2, so that the stride-2 conv becomes 9 unit-stride taps.
+ * Alignment: x 16-byte aligned (float4 loads), hi and lo 8-byte aligned (4-channel stores); C a multiple of 4, H and W even; else
+ * N3D_ERR_INVALID_ARG. */
 int n3d_fir_down_split(const float* x, int N, int H, int W, int C, void* hi, void* lo, void* stream);
 
 /* upfirdn2d.upsample2d on an fp32 NHWC image (up 2, pad (2,1), gain 4; networks_stylegan2.py:577); y is NHWC, or NCHW
- * when y_nchw != 0 (used for the final image). */
+ * when y_nchw != 0 (used for the final image).  Any alignment: 4 channels per thread (float4) when C % 4 == 0 and x and an NHWC y
+ * are 16-byte aligned, else one channel per thread. */
 int n3d_upsample2d_nhwc(const float* x, int N, int H, int W, int C, float* y, int y_nchw, void* stream);
 /* upfirdn2d.downsample2d on an fp32 NHWC image (pad (1,1), down 2; networks_stylegan2_styleunet.py:109). */
 int n3d_downsample2d_nhwc(const float* x, int N, int H, int W, int C, float* y, void* stream);
@@ -272,7 +278,8 @@ int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t*
 
 /* planes[n,p,y,x,c] = tex[n,p,y,x,c] * alpha[n,p,y,x] + static[n,y,x,p*32+c] * (1 - alpha)  (triplane_next3d.py:171-174);
  * tex for plane 0 = blended_front NHWC [N,H,W,32] (neural-blending output), planes 1,2 = tex_planes[1:] (plane-major
- * [3,N,H,W,32]), alpha [3,N,H,W], static_planes NHWC [N,H,W,96]; planes out channels-last [N,3,H,W,32]. */
+ * [3,N,H,W,32]), alpha [3,N,H,W], static_planes NHWC [N,H,W,96]; planes out channels-last [N,3,H,W,32].
+ * Alignment: blended_front, tex_planes, static_planes and planes 16-byte aligned (float4 loads / stores), else N3D_ERR_INVALID_ARG. */
 int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
                      int N, int H, int W, float* planes, void* stream);
 

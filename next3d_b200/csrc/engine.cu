@@ -660,6 +660,8 @@ extern "C" int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, i
                                   int out_cstride, int out_coff, void* stream) {
     N3D_CHECK_ARG(x && hi && lo, "n3d_modulate_split: null pointer");
     N3D_CHECK_ARG(C % 4 == 0 && out_cstride % 4 == 0 && out_coff % 4 == 0, "n3d_modulate_split: channels must be multiples of 4");
+    N3D_CHECK_ARG((((uintptr_t)x | (uintptr_t)style) & 15) == 0, "n3d_modulate_split: x and style must be 16-byte aligned");   // float4 loads
+    N3D_CHECK_ARG((((uintptr_t)hi | (uintptr_t)lo) & 7) == 0, "n3d_modulate_split: hi and lo must be 8-byte aligned");          // uint2 stores
     const int64_t total = (int64_t)N * npix_per_img * (C / 4);
     modulate_split_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)hi,
                                                                                      (__nv_bfloat16*)lo, out_cstride, out_coff);
@@ -729,6 +731,8 @@ extern "C" int n3d_splitk_epilogue(const float* partial, int S, int64_t split_st
 extern "C" int n3d_fir_down_split(const float* x, int N, int H, int W, int C, void* hi, void* lo, void* stream) {
     N3D_CHECK_ARG(x && hi && lo, "n3d_fir_down_split: null pointer");
     N3D_CHECK_ARG(C % 4 == 0 && H % 2 == 0 && W % 2 == 0, "n3d_fir_down_split: C %% 4 and even H, W required");
+    N3D_CHECK_ARG(((uintptr_t)x & 15) == 0, "n3d_fir_down_split: x must be 16-byte aligned");       // float4 loads / bulk copies (both kernels)
+    N3D_CHECK_ARG((((uintptr_t)hi | (uintptr_t)lo) & 7) == 0, "n3d_fir_down_split: hi and lo must be 8-byte aligned");     // uint2 stores
     const N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
     const int sms = D->num_sms;
@@ -738,7 +742,7 @@ extern "C" int n3d_fir_down_split(const float* x, int N, int H, int W, int C, vo
     int TS = 0;
     for (int ts = 32; ts >= 16 && TSC; ts >>= 1)
         if ((int64_t)N * n3d_div_up(SW, TSC) * n3d_div_up(SH, ts) >= sms) { TS = ts; break; }
-    if (TS > 0 && ((uintptr_t)x & 15) == 0 && fir_stream_enabled()) {
+    if (TS > 0 && fir_stream_enabled()) {
         const int row_bytes = (2 * TSC + 3) * C * 4, NR = 4;
         const int smem = NR * row_bytes + 16 * NR;
         if (int rc = n3d_smem_optin((const void*)fir_down_stream_kernel, 112 * 1024, "n3d_fir_down_split")) return rc;
@@ -756,7 +760,8 @@ extern "C" int n3d_fir_down_split(const float* x, int N, int H, int W, int C, vo
 
 extern "C" int n3d_upsample2d_nhwc(const float* x, int N, int H, int W, int C, float* y, int y_nchw, void* stream) {
     N3D_CHECK_ARG(x && y, "n3d_upsample2d_nhwc: null pointer");
-    if (C % 4 == 0)
+    // float4 loads of x and (NHWC) float4 stores of y where the channels and both pointers allow them, else one channel per thread
+    if (C % 4 == 0 && ((uintptr_t)x & 15) == 0 && (y_nchw || ((uintptr_t)y & 15) == 0))
         upsample2d_kernel<4><<<n3d_grid((int64_t)N * H * W * (C / 4), 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);
     else
         upsample2d_kernel<1><<<n3d_grid((int64_t)N * H * W * C, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, N, H, W, C, y, y_nchw);

@@ -29,13 +29,14 @@ template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 
-// 4 elements per thread per iteration; bias index computed per element (step_b may be 1 for channels_last).
+// 4 elements per thread per iteration; bias index computed per element (step_b may be 1 for channels_last).  vec == 0 (x or y not
+// aligned to a 4-element vector, e.g. a view that starts inside its storage): every element goes through the scalar loop.
 template <typename T>
 __global__ void __launch_bounds__(256) bias_act_kernel(const T* __restrict__ x, const T* __restrict__ b, T* __restrict__ y,
                                                        int64_t numel, int size_b, int step_b, int act, float alpha,
-                                                       float gain, float clamp) {
+                                                       float gain, float clamp, int vec) {
     typedef typename Vec4<T>::type V;
-    const int64_t nvec = numel >> 2;
+    const int64_t nvec = vec ? numel >> 2 : 0;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += stride) {
         V v = reinterpret_cast<const V*>(x)[i];
@@ -69,12 +70,14 @@ extern "C" int n3d_bias_act(const void* x, const void* b, void* y, int dtype, in
     N3D_CHECK_ARG(!b || (size_b > 0 && step_b > 0), "n3d_bias_act: bad bias geometry");
     if (numel == 0) return N3D_OK;
     const int grid = n3d_grid((numel + 3) / 4, 256);        // 4 elements per thread
+    const uintptr_t vec_align = dtype == N3D_DTYPE_F32 ? 15 : 7;     // float4 / 4 x half
+    const int vec = (((uintptr_t)x | (uintptr_t)y) & vec_align) == 0;
     if (dtype == N3D_DTYPE_F32)
         bias_act_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)x, (const float*)b, (float*)y, numel,
-                                                                        size_b, step_b, act, alpha, gain, clamp);
+                                                                        size_b, step_b, act, alpha, gain, clamp, vec);
     else
         bias_act_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)x, (const __half*)b, (__half*)y,
-                                                                         numel, size_b, step_b, act, alpha, gain, clamp);
+                                                                         numel, size_b, step_b, act, alpha, gain, clamp, vec);
     N3D_CHECK_LAUNCH("n3d_bias_act");
     return N3D_OK;
 }

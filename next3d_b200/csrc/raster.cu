@@ -559,6 +559,8 @@ extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, con
 extern "C" int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
                                 int N, int H, int W, float* planes, void* stream) {
     N3D_CHECK_ARG(blended_front && tex_planes && alpha && static_planes && planes, "n3d_blend_planes: null pointer");
+    N3D_CHECK_ARG((((uintptr_t)blended_front | (uintptr_t)tex_planes | (uintptr_t)static_planes | (uintptr_t)planes) & 15) == 0,
+                  "n3d_blend_planes: blended_front, tex_planes, static_planes and planes must be 16-byte aligned");     // float4 loads / stores
     blend_kernel<<<n3d_grid((int64_t)N * 3 * H * W * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(blended_front, tex_planes, alpha, static_planes, N, H * W, planes);
     N3D_CHECK_LAUNCH("n3d_blend_planes");
     return N3D_OK;

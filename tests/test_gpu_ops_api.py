@@ -42,6 +42,25 @@ def test_bias_act(ops, dtype, fmt):
     assert torch.equal(ops.bias_act.bias_act(x2, b2, act='lrelu', impl='ref'), oo.bias_act(x2, b2, act='lrelu'))
 
 
+@pytest.mark.parametrize('dtype', [torch.float32, torch.float16])
+@pytest.mark.parametrize('fmt', [torch.contiguous_format, torch.channels_last])
+@pytest.mark.parametrize('offset', [1, 2, 3])
+def test_bias_act_on_views_at_any_storage_offset(ops, dtype, fmt, offset):
+    """Dense views that start 1-3 elements into their storage (not aligned for 4-element vector accesses), numel % 4 in {0..3}."""
+    from oracle import ops as oo
+    b = torch.randn(5, generator=_g(15)).to(dtype)
+    for shape in [(2, 5, 2, 7), (1, 5, 3, 7), (2, 5, 3, 7), (1, 5, 1, 7)]:          # numel % 4 = 0, 1, 2, 3
+        N, Cc, H, W = shape
+        strides = (Cc * H * W, H * W, W, 1) if fmt == torch.contiguous_format else (H * W * Cc, 1, W * Cc, Cc)
+        buf = (torch.randn(N * Cc * H * W + 8, generator=_g(16)) * 2).to(dtype).cuda()
+        x = buf.as_strided(shape, strides, offset)
+        assert x.is_contiguous(memory_format=fmt) and x.data_ptr() % (4 * x.element_size()) != 0
+        y = ops.bias_act.bias_act(x, b.cuda(), act='lrelu', clamp=1.5)
+        ref = oo.bias_act(x.cpu().float(), b.float(), act='lrelu', clamp=1.5)
+        assert y.is_contiguous(memory_format=fmt)
+        assert range_rel_err(y.float().cpu(), ref) < (2e-3 if dtype == torch.float16 else 2e-6), (shape, offset)
+
+
 @pytest.mark.parametrize('up,down,pad', [(1, 1, [1, 1, 1, 1]), (2, 1, [2, 1, 2, 1]), (1, 2, [1, 1, 1, 1]), (1, 1, [2, 2, 2, 2]), (2, 2, [3, 0, 1, 2]),
                                         (1, 1, [-1, 0, 0, -1]), (4, 1, [3, 2, 3, 2])])
 def test_upfirdn2d(ops, up, down, pad):
@@ -76,6 +95,21 @@ def test_conv2d_resample(ops, k, up, down, flip, groups):
     assert range_rel_err(y.cpu(), ref) < 5e-5
     with pytest.raises(RuntimeError):
         ops.conv2d_resample.conv2d_resample(x.cuda(), torch.randn(8, cin_g * groups, 5, 5).cuda(), padding=2)
+
+
+@pytest.mark.parametrize('N,cin,cout,H,W,up,down,flip', [(3, 8, 8, 7, 13, 2, 1, False), (1, 512, 512, 10, 18, 1, 1, True),
+                                                       (3, 512, 8, 10, 18, 1, 2, True), (1, 8, 512, 7, 13, 2, 1, True)])
+def test_conv2d_resample_odd_sizes(ops, N, cin, cout, H, W, up, down, flip):
+    """Non-square and odd sizes, batch 1 and 3, 8 and 512 channels, against oracle.ops in fp64 on the device."""
+    from oracle import ops as oo
+    x = torch.randn(N, cin, H, W, generator=_g(17)).cuda()
+    w = (torch.randn(cout, cin, 3, 3, generator=_g(18)) / math.sqrt(cin * 9)).cuda()
+    f = oo.setup_filter().cuda()
+    kw = dict(up=up, down=down, padding=1, flip_weight=flip)
+    ref = oo.conv2d_resample(x.double(), w.double(), f=f.double(), **kw)
+    y = ops.conv2d_resample.conv2d_resample(x, w, f=f, **kw)
+    assert y.shape == ref.shape
+    assert range_rel_err(y, ref) < 5e-5
 
 
 def test_filtered_lrelu(ops):

@@ -209,6 +209,64 @@ def test_conv2d_resample_grad(ops, k, up, down, groups, flip):
     assert torch.equal(y0, conv(x.cuda().requires_grad_(), w.cuda(), f=f.cuda(), **kw).detach())
 
 
+def _fir_plans(N, cin, cout, H, W, up, down, sms):
+    """FIR launches of a 3x3 conv2d_resample call (forward, backward) -> {direction: plan} (tests/test_gpu_fir_conformance.py)."""
+    from tests.test_gpu_fir_conformance import fir_down_plan, fir_up_plan
+    cpad = -(-cout // 8) * 8                                    # the input gradient's channels, zero-padded to a multiple of 8
+    if up == 2:
+        return {'forward fir-up': fir_up_plan(N, 2 * H, 2 * W, cout, sms), 'backward fir-down': fir_down_plan(N, 2 * H, 2 * W, cpad, sms)}
+    if down == 2:
+        return {'forward fir-down': fir_down_plan(N, H, W, cin, sms), 'backward fir-up': fir_up_plan(N, H, W, cin, sms)}
+    return {}
+
+
+# Beyond 12 x 12: odd and non-square sizes, batch 1 and 3, 8 and 512 channels, and layers whose FIR passes take the streamed kernels
+# (`streamed`: the directions that must, according to the launch rules).
+_CONV_LARGE = [
+    dict(name='up_7x13_n3_c8', N=3, cin=8, cout=8, H=7, W=13, up=2, down=1, flip=False, streamed=()),
+    dict(name='same_10x18_n1_c512', N=1, cin=512, cout=512, H=10, W=18, up=1, down=1, flip=True, streamed=()),
+    dict(name='down_10x18_n3_c512', N=3, cin=512, cout=8, H=10, W=18, up=1, down=2, flip=True, streamed=()),
+    dict(name='up_192x176_streamed', N=1, cin=8, cout=64, H=192, W=176, up=2, down=1, flip=True,
+         streamed=('forward fir-up', 'backward fir-down')),
+    dict(name='down_384x352_streamed', N=1, cin=64, cout=16, H=384, W=352, up=1, down=2, flip=False,
+         streamed=('forward fir-down', 'backward fir-up')),
+]
+
+
+@pytest.mark.parametrize('c', _CONV_LARGE, ids=[c['name'] for c in _CONV_LARGE])
+def test_conv2d_resample_grad_large(ops, c, monkeypatch):
+    """Forward, dx and dw against oracle.ops under fp64 autograd on the device; where a FIR pass streams, everything is bit-identical
+    under N3D_FIR_STREAM=0 (the register-tiled FIR kernels)."""
+    from oracle import ops as oo
+    monkeypatch.delenv('N3D_FIR_STREAM', raising=False)
+    case = f'conv_large/{c["name"]}'
+    plans = _fir_plans(c['N'], c['cin'], c['cout'], c['H'], c['W'], c['up'], c['down'], torch.cuda.get_device_properties(0).multi_processor_count)
+    assert {d for d, p in plans.items() if p['streamed']} == set(c['streamed']), (case, plans)
+    x = torch.randn(c['N'], c['cin'], c['H'], c['W'], generator=_g(18)).cuda()
+    w = (torch.randn(c['cout'], c['cin'], 3, 3, generator=_g(19)) / math.sqrt(c['cin'] * 9)).cuda()
+    f = oo.setup_filter().cuda()
+    kw = dict(up=c['up'], down=c['down'], padding=1, flip_weight=c['flip'])
+    x64, w64 = x.double().requires_grad_(), w.double().requires_grad_()
+    y64 = oo.conv2d_resample(x64, w64, f=f.double(), **kw)
+    dy = torch.randn(y64.shape, generator=_g(20)).cuda()
+    dx64, dw64 = torch.autograd.grad(y64, [x64, w64], dy.double())
+    y64 = y64.detach()
+
+    def run():
+        xg, wg = x.clone().requires_grad_(), w.clone().requires_grad_()
+        y = ops.conv2d_resample.conv2d_resample(xg, wg, f=f, **kw)
+        return (y.detach(),) + torch.autograd.grad(y, [xg, wg], dy)
+
+    y, dx, dw = run()
+    _check(case, 'y', y, y64, 5e-5)
+    _check(case, 'dx', dx, dx64, _CONV_BOUND['dx'])
+    _check(case, 'dw', dw, dw64, _CONV_BOUND['dw'])
+    if c['streamed']:
+        monkeypatch.setenv('N3D_FIR_STREAM', '0')
+        for a, b in zip((y, dx, dw), run()):
+            assert torch.equal(a, b), case
+
+
 # ------------------------------------------------------------------------------------------------ n3d_conv_wgrad at the ABI
 def _shifted(t, off, cols, K):
     """t [rows, ld] -> [rows, K]: column k holds t[:, k + off] for 0 <= k + off < cols, else 0."""
