@@ -262,8 +262,12 @@ int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, const float* fa
                   float* tex_planes, float* alpha, void* stream);
 
 /* fill_mouth (renderer.py:583-602): alpha [NI,H,W] in place; cv2.floodFill from (0,0) with fixed range [seed, seed+254]
- * on alpha*255, then alpha += 1 - (filled/127.5 - 1), clipped to [0,1].  H*W <= 65536.  One CTA per image. */
+ * on alpha*255, then alpha += 1 - (filled/127.5 - 1), clipped to [0,1].  H*(W+4) <= 200 KB (512x396 at most).
+ * One CTA per image; the sweeps repeat until the fill has converged, however winding the region. */
 int n3d_fill_mouth(float* alpha, int NI, int H, int W, void* stream);
+/* n3d_fill_mouth, after which images [bin0, bin1) are binarized, alpha = (alpha != 0) (a NaN gives 1): what the reference
+ * does to the side plane's alpha (triplane_next3d.py:226).  0 <= bin0 <= bin1 <= NI; bin0 = bin1 is n3d_fill_mouth. */
+int n3d_fill_mouth_binarize(float* alpha, int NI, int H, int W, int bin0, int bin1, void* stream);
 
 /* gen_mouth_mask (triplane_next3d.py:330-344) on device: lm2d [N,68,2] -> boxes [N,4] int32 (y0,y1,x0,x1). */
 int n3d_mouth_box(const float* lm2d, int N, int32_t* boxes, void* stream);

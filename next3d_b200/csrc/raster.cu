@@ -231,8 +231,10 @@ __global__ void __launch_bounds__(256) uv_sample_kernel(const int* __restrict__ 
 // ---------------------------------------------------------------------------------------------- fill_mouth
 // One CTA per image.  state[p]: 0 = not fillable, 1 = fillable, 2 = reached from the corner.  Alternating row / column
 // sweeps (one thread per row resp. column, forward + backward) until a pass changes nothing -- a few passes for
-// face-silhouette masks.  Then res = clip(alpha + 1 - (filled/127.5 - 1)) in the reference's op order.
-__global__ void __launch_bounds__(1024) fill_mouth_kernel(float* __restrict__ alpha, int H, int W) {
+// face-silhouette masks, about one pass per turn of the longest path for a winding one.  Every pass but the last turns at
+// least one byte from 1 to 2, so at most H*W + 1 passes run.  Then res = clip(alpha + 1 - (filled/127.5 - 1)) in the
+// reference's op order; images [bin0, bin1) are then binarized, res = (res != 0), as the reference does to the side plane.
+__global__ void __launch_bounds__(1024) fill_mouth_kernel(float* __restrict__ alpha, int H, int W, int bin0, int bin1) {
     extern __shared__ unsigned char st[];
     __shared__ int s_changed;
     const int SW = W + 4;                  // row pitch in bytes: (W+4)/4 is odd -> row sweeps (one thread per row) are bank-conflict free
@@ -249,7 +251,7 @@ __global__ void __launch_bounds__(1024) fill_mouth_kernel(float* __restrict__ al
     // Four sweep directions run concurrently on disjoint thread groups (state only ever goes 1 -> 2, byte stores: benign races
     // merely delay propagation to the next pass); repeat until a pass changes nothing.
     const int group = threadIdx.x >> 8, gi = threadIdx.x & 255;
-    for (int iter = 0; iter < 4 * (H + W); ++iter) {
+    for (;;) {
         if (threadIdx.x == 0) s_changed = 0;
         __syncthreads();
         int changed = 0;
@@ -272,12 +274,15 @@ __global__ void __launch_bounds__(1024) fill_mouth_kernel(float* __restrict__ al
         __syncthreads();
         if (!any) break;
     }
+    const bool binarize = (int)blockIdx.x >= bin0 && (int)blockIdx.x < bin1;
     for (int i = threadIdx.x; i < H * W; i += blockDim.x) {
         const float al = a[i];
         const float filled = st[(i / W) * SW + (i % W)] == 2 ? 255.f : __fmul_rn(al, 255.f);
         const float m = __fsub_rn(__fdiv_rn(filled, 127.5f), 1.f);
         const float t = __fdiv_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(m, 2.f), 1.f), -1.f), 1.f), 2.f);
-        a[i] = fminf(fmaxf(__fadd_rn(al, t), 0.f), 1.f);
+        const float v = __fadd_rn(al, t);
+        // torch's clip keeps a NaN, which .bool() turns into 1: !(v <= 0) is bool(clip(v, 0, 1)) including NaN
+        a[i] = binarize ? (!(v <= 0.f) ? 1.f : 0.f) : fminf(fmaxf(v, 0.f), 1.f);
     }
 }
 
@@ -524,13 +529,18 @@ extern "C" int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, cons
     return N3D_OK;
 }
 
-extern "C" int n3d_fill_mouth(float* alpha, int NI, int H, int W, void* stream) {
+extern "C" int n3d_fill_mouth_binarize(float* alpha, int NI, int H, int W, int bin0, int bin1, void* stream) {
     N3D_CHECK_ARG(alpha && NI > 0 && H > 0 && W > 0, "n3d_fill_mouth: bad args");
+    N3D_CHECK_ARG(0 <= bin0 && bin0 <= bin1 && bin1 <= NI, "n3d_fill_mouth: binarized images [%d, %d) not within [0, %d]", bin0, bin1, NI);
     N3D_CHECK_ARG((int64_t)H * (W + 4) <= 200 * 1024, "n3d_fill_mouth: image %dx%d too large for the shared-memory state map", H, W);
     if (int rc = n3d_smem_optin((const void*)fill_mouth_kernel, 200 * 1024, "n3d_fill_mouth")) return rc;
-    fill_mouth_kernel<<<NI, 1024, (size_t)H * (W + 4), (cudaStream_t)stream>>>(alpha, H, W);
+    fill_mouth_kernel<<<NI, 1024, (size_t)H * (W + 4), (cudaStream_t)stream>>>(alpha, H, W, bin0, bin1);
     N3D_CHECK_LAUNCH("n3d_fill_mouth");
     return N3D_OK;
+}
+
+extern "C" int n3d_fill_mouth(float* alpha, int NI, int H, int W, void* stream) {
+    return n3d_fill_mouth_binarize(alpha, NI, H, W, 0, 0, stream);
 }
 
 extern "C" int n3d_mouth_box(const float* lm2d, int N, int32_t* boxes, void* stream) {

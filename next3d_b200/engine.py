@@ -599,11 +599,12 @@ class Engine:
             main.wait_stream(s_rast)
             for t in (p2f, bary, boxes, lm2d):
                 t.record_stream(main)
-        # look up texture + eye mask at the rasterized UVs, fill the mouth hole
+        # look up texture + eye mask at the rasterized UVs, fill the mouth hole; the side plane's alpha (images N .. 2N - 1 of
+        # alpha) ends binary, as the reference's (alpha.bool() | alpha.bool()).float() leaves it (triplane_next3d.py:226)
         tex_planes = self._f32(3, N, P, P, cfg.plane_ch)
         alpha = self._f32(3, N, P, P)
         K.uv_sample(p2f, bary, self.face_uv, textures, self.eye_mask, tex_planes, alpha)
-        K.fill_mouth(alpha)
+        K.fill_mouth(alpha, binarize=(N, 2 * N))
         # mouth crop -> StyleUNet -> paste back -> neural blending
         front = tex_planes[0]
         crop = self._f32(N, 64, 64, cfg.plane_ch)

@@ -221,9 +221,13 @@ def uv_sample(p2f, bary, face_uv, texture, eye_mask, tex_planes, alpha):
                           ptr(tex_planes), ptr(alpha), stream_ptr())
 
 
-def fill_mouth(alpha):
+def fill_mouth(alpha, binarize=(0, 0)):
+    """alpha [..., H, W] in place; the images [binarize[0], binarize[1]) of the flattened leading dims end as (alpha != 0)."""
     NI = alpha.numel() // (alpha.shape[-1] * alpha.shape[-2])
-    _run('n3d_fill_mouth', ptr(alpha), NI, alpha.shape[-2], alpha.shape[-1], stream_ptr())
+    if binarize[0] == binarize[1]:
+        _run('n3d_fill_mouth', ptr(alpha), NI, alpha.shape[-2], alpha.shape[-1], stream_ptr())
+    else:
+        _run('n3d_fill_mouth_binarize', ptr(alpha), NI, alpha.shape[-2], alpha.shape[-1], binarize[0], binarize[1], stream_ptr())
 
 
 def mouth_box(lm2d, boxes):
