@@ -1,7 +1,11 @@
-"""Shared helpers for the parity tests."""
+"""Shared helpers for the parity tests and the kernel conformance suites."""
+import json
+import math
 import os
+import re
 
 import numpy as np
+import pytest
 import torch
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
@@ -58,7 +62,6 @@ def pixel_rel_err(a, ref, floor=1e-3):
 def report_parity(name, a, ref):
     """Both parity metrics of one output; appended to gpurun_out/parity_report.jsonl when that directory exists (so a GPU run
     leaves the numbers behind for the design notes).  -> (range_rel, pixel_rel_max, pixel_rel_frac_above_1e-3)."""
-    import json
     r = range_rel_err(a, ref)
     pmax, pfrac = pixel_rel_err(a, ref)
     out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'gpurun_out')
@@ -66,3 +69,140 @@ def report_parity(name, a, ref):
         with open(os.path.join(out, 'parity_report.jsonl'), 'a') as f:
             f.write(json.dumps({'case': name, 'range_rel_err': r, 'pixel_rel_err_max_floor1e-3': pmax, 'pixel_frac_above_1e-3': pfrac}) + '\n')
     return r, pmax, pfrac
+
+
+# ------------------------------------------------------------------------------------------------ kernel conformance suites
+GUARD = 64                  # sentinel elements on each side of an output view: keeps the view's base alignment that of a fresh allocation
+SENTINEL = {torch.float32: (torch.int32, 0x7FC01234), torch.int32: (torch.int32, 0x7FC01234),      # NaN bit patterns no store produces
+            torch.bfloat16: (torch.int16, 0x7FC1)}
+
+
+class Guarded:
+    """An output tensor as a view into a larger allocation filled with a sentinel.  The launch owns the elements `own` selects: all of
+    the view (None), a slice of the last dimension, or a bool tensor broadcastable to the view; `own` may be assigned after
+    construction.  `init`: initial content of the view, in place of the sentinel."""
+
+    def __init__(self, shape, dtype=torch.float32, own=None, init=None):
+        n = math.prod(shape)
+        self.int_dtype, self.sentinel = SENTINEL[dtype]
+        self.buf = torch.empty(GUARD + n + GUARD, dtype=dtype, device='cuda')
+        self.view = self.buf[GUARD:GUARD + n].view(shape)
+        self.own = own
+        self.reset()
+        if init is not None:
+            self.view.copy_(init)
+
+    def reset(self):
+        self.buf.view(self.int_dtype).fill_(self.sentinel)
+
+    def bits(self):
+        return self.view.view(self.int_dtype)
+
+    def _own_mask(self):
+        if isinstance(self.own, slice):
+            m = torch.zeros(self.view.shape[-1], dtype=torch.bool, device=self.view.device)
+            m[self.own] = True
+            return m
+        return self.own
+
+    def untouched_ok(self):
+        """The guard bands and every element outside `own` still hold the sentinel's bits."""
+        b, own = self.buf.view(self.int_dtype), self._own_mask()
+        ok = bool((b[:GUARD] == self.sentinel).all()) and bool((b[-GUARD:] == self.sentinel).all())
+        return ok and (own is None or bool(((self.bits() == self.sentinel) | own).all()))
+
+    def written(self):
+        """No element of `own` holds the sentinel's bits."""
+        kept, own = self.bits() == self.sentinel, self._own_mask()
+        return not bool((kept if own is None else kept & own).any())
+
+    def snapshot(self):
+        """The bits of the whole allocation, guards included, on the host."""
+        return self.buf.view(self.int_dtype).cpu()
+
+
+class RangeErr:
+    """max |got - ref| / max |ref| accumulated over reference chunks; a NaN difference counts as infinite."""
+
+    def __init__(self):
+        self.diff = self.range = 0.0
+
+    def add(self, got, ref):
+        d = (got.double() - ref).abs().max().item()
+        self.diff = max(self.diff, d if d == d else math.inf)
+        self.range = max(self.range, ref.abs().max().item())
+
+    def value(self):
+        return self.diff / max(self.range, 1e-30)
+
+
+def record_errors(env_var, rows):
+    """Append each row (a dict) as a JSON line to the file named by the environment variable `env_var`, when it is set: scripts that
+    re-measure the worst cases beside a suite's bounds read these files."""
+    path = os.environ.get(env_var)
+    if path:
+        with open(path, 'a') as f:
+            for r in rows:
+                f.write(json.dumps(r) + '\n')
+
+
+def rerun_identical(outputs, launch):
+    """Reset the guarded outputs to the sentinel, call launch() and synchronise -> whether every output holds the same bits as
+    before the call."""
+    before = [t.snapshot() for t in outputs]
+    for t in outputs:
+        t.reset()
+    launch()
+    torch.cuda.synchronize()
+    return all(torch.equal(a, t.snapshot()) for a, t in zip(before, outputs))
+
+
+def launched_kernels(run, pattern, tmp_path):
+    """Call run() twice under torch.profiler; run() launches kernels and returns a list with one entry per launch whose kernel name
+    `pattern` matches.  -> (what the second call returned, the chrome-trace events of its matching launches in launch order, each
+    with the launch's 'grid' and 'cluster' in its 'args' where the trace records them).  A profiler session that follows another
+    one in the same process can drop its first kernel records, so only the second call is compared; skips the test when CUDA
+    activity tracing is unavailable."""
+    from torch.profiler import ProfilerActivity, profile
+    try:
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run()
+            expected = run()
+            torch.cuda.synchronize()
+    except RuntimeError as e:              # CUPTI missing or busy
+        pytest.skip(f'CUDA activity tracing unavailable: {e}')
+    trace = tmp_path / 'trace.json'
+    prof.export_chrome_trace(str(trace))
+    events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and re.search(pattern, e.get('name', ''))]
+    if not events:
+        pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')
+    events.sort(key=lambda e: e['ts'])
+    n = len(expected)
+    assert n <= len(events) <= 2 * n, [e['name'] for e in events]
+    return expected, events[-n:]
+
+
+def cdiv(a, b):
+    return -(-a // b)
+
+
+def grid_stride(work, sms, per_sm, threads=256):
+    """n3d_grid (common.cuh): one block per `threads` work items, at least 1 and at most `per_sm` blocks per SM."""
+    return max(1, min(cdiv(work, threads), sms * per_sm))
+
+
+def lib():
+    from next3d_b200 import _lib as L
+    return L
+
+
+def refused(rc, what):
+    """The entry point returned -1 and its last error contains `what`."""
+    msg = lib().lib.n3d_last_error().decode()
+    assert rc == -1 and what in msg, (rc, msg)
+
+
+def offset_view(t, nbytes):
+    """A view of `t` (a fresh, 64-byte aligned allocation) that starts `nbytes` later."""
+    assert t.data_ptr() % 64 == 0
+    return t.view(-1)[nbytes // t.element_size():]

@@ -15,16 +15,15 @@ listed in COVERAGE; the profiler test checks on the GPU that each case ran the k
 The alignment tests at the end need no GPU: descriptors over CPU tensors at 4-byte offsets must be refused before any device call.
 """
 import ctypes as C
-import json
 import math
 import re
 
 import pytest
 import torch
 
+from tests.helpers import Guarded, launched_kernels, lib, offset_view, refused
+
 DEV = 'cuda'
-GUARD = 64                  # sentinel elements on each side of an output view: keeps the view's base alignment that of a fresh allocation
-SENTINEL = {torch.float32: (torch.int32, 0x7FC01234), torch.bfloat16: (torch.int16, 0x7FC1)}      # NaN bit patterns no store produces
 
 # Range-relative error bounds per output kind, max |got - ref| / max |ref| over the owned elements, each at most 4x the worst case
 # measured over the table on an H100 SXM 80 GB (700 W power limit), which is given beside it.
@@ -287,28 +286,12 @@ def epilogue_reference(acc, oy, ox, OW, dcoef=None, bias=None, noise=None, noise
     return v
 
 
-class Guarded:
-    """An output tensor as a view into a larger allocation filled with a NaN sentinel.  `owned` marks the elements the launch
-    writes, `expect` their fp64 reference."""
+class Expected(Guarded):
+    """A guarded output whose owned elements (`own`) and their fp64 reference (`expect`) _place fills in."""
 
     def __init__(self, shape, dtype):
-        n = math.prod(shape)
-        self.int_dtype, self.sentinel = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + n + GUARD, dtype=dtype, device=DEV)
-        self.buf.view(self.int_dtype).fill_(self.sentinel)
-        self.view = self.buf[GUARD:GUARD + n].view(shape)
-        self.owned = torch.zeros(shape, dtype=torch.bool, device=DEV)
+        super().__init__(shape, dtype, own=torch.zeros(shape, dtype=torch.bool, device=DEV))
         self.expect = torch.zeros(shape, dtype=torch.float64, device=DEV)
-
-    def untouched_ok(self):
-        """Every element outside `owned` (guards included) still holds the sentinel's bits."""
-        owned = torch.zeros(self.buf.numel(), dtype=torch.bool, device=DEV)
-        owned[GUARD:GUARD + self.view.numel()] = self.owned.flatten()
-        bits = self.buf.view(self.int_dtype)
-        return bool((bits[~owned] == self.sentinel).all())
-
-    def written(self):
-        return bool((self.view.view(self.int_dtype)[self.owned] != self.sentinel).all())
 
 
 def _place(g, vals, yv, xv, oy, ox, coff, nchw, accumulate=None):
@@ -319,7 +302,7 @@ def _place(g, vals, yv, xv, oy, ox, coff, nchw, accumulate=None):
     Y, X = oy[yv][None, :, None, None], ox[xv][None, None, :, None]
     v = vals[:, yv][:, :, xv]
     idx = (n, c, Y, X) if nchw else (n, Y, X, c)
-    g.owned[idx] = True
+    g.own[idx] = True
     g.expect[idx] = v + (accumulate[idx].double() if accumulate is not None else 0.0)
 
 
@@ -351,18 +334,18 @@ def setup_case(c):
     elif c['noise'] == 'sample':
         s['noise'], s['noise_nstride'] = torch.randn(N, OH, OW, device=DEV, generator=g) * 0.3, OH * OW
     s['styles'] = [torch.randn(N, Cout, device=DEV, generator=g) for _ in c['outs']]
-    s['outs'] = [(Guarded((N, OH, OW, o['cstride']), torch.bfloat16), Guarded((N, OH, OW, o['cstride']), torch.bfloat16)) for o in c['outs']]
+    s['outs'] = [(Expected((N, OH, OW, o['cstride']), torch.bfloat16), Expected((N, OH, OW, o['cstride']), torch.bfloat16)) for o in c['outs']]
     f = c['f32']
     s['f32'] = None
     if f is not None:
         shape = (N, f['cstride'], OH, OW) if f['nchw'] else (N, OH, OW, f['cstride'])
-        s['f32'] = Guarded(((c['splits'],) if c['splits'] > 1 else ()) + shape, torch.float32)
+        s['f32'] = Expected(((c['splits'],) if c['splits'] > 1 else ()) + shape, torch.float32)
     r = c['rgb']
     if r:
         s['rgb_w'] = torch.randn(r['ch'], Cout, device=DEV, generator=g)
         s['rgb_s'] = torch.randn(N, Cout, device=DEV, generator=g) / math.sqrt(Cout)
         s['rgb_b'] = torch.randn(r['ch'], device=DEV, generator=g)
-        s['rgb'] = Guarded((N, r['ch'], OH, OW) if r['nchw'] else (N, OH, OW, r['ch']), torch.float32)
+        s['rgb'] = Expected((N, r['ch'], OH, OW) if r['nchw'] else (N, OH, OW, r['ch']), torch.float32)
     if c['splits'] > 1:             # second pass: n3d_splitk_epilogue with the full epilogue into fresh guarded outputs
         s.update(dcoef=torch.rand(N, Cout, device=DEV, generator=g) + 0.5, bias=torch.randn(Cout, device=DEV, generator=g) * 0.5,
                  gain=math.sqrt(2), slope=0.2, clamp=2.0)
@@ -370,8 +353,8 @@ def setup_case(c):
         s['noise'] = torch.randn(*((N,) if per_sample else ()), OH, OW, device=DEV, generator=g) * 0.3
         s['noise_nstride'] = OH * OW if per_sample else 0
         s['epi_styles'] = [torch.randn(N, Cout, device=DEV, generator=g) for _ in range(2)]
-        s['epi_outs'] = [(Guarded((N, OH, OW, cs), torch.bfloat16), Guarded((N, OH, OW, cs), torch.bfloat16)) for cs in (Cout, 2 * Cout)]
-        s['epi_f32'] = Guarded((N, OH, OW, Cout), torch.float32)
+        s['epi_outs'] = [(Expected((N, OH, OW, cs), torch.bfloat16), Expected((N, OH, OW, cs), torch.bfloat16)) for cs in (Cout, 2 * Cout)]
+        s['epi_f32'] = Expected((N, OH, OW, Cout), torch.float32)
     # the reference: accumulators (per split-K slice), then owned elements and expected values of every output
     yv, xv = _valid(s)
     oy = torch.arange(c['MH'], device=DEV) * oy_mul + oy_off
@@ -420,7 +403,7 @@ def _expect(s):
         prior = None
         if f['acc']:                # accumulating output: finite prior content in the owned region
             _place(s['f32'], v, yv, xv, oy, ox, f['coff'], f['nchw'])
-            s['f32'].view[s['f32'].owned] = torch.randn(int(s['f32'].owned.sum()), device=DEV, generator=_seeded(c))
+            s['f32'].view[s['f32'].own] = torch.randn(int(s['f32'].own.sum()), device=DEV, generator=_seeded(c))
             prior = s['f32'].view.clone()
         _place(s['f32'], v, yv, xv, oy, ox, f['coff'], f['nchw'], prior)
     r = c['rgb']
@@ -430,7 +413,7 @@ def _expect(s):
         prior = None
         if r['acc']:
             _place(s['rgb'], img, yv, xv, oy, ox, 0, r['nchw'])
-            s['rgb'].view[s['rgb'].owned] = torch.randn(int(s['rgb'].owned.sum()), device=DEV, generator=_seeded(c))
+            s['rgb'].view[s['rgb'].own] = torch.randn(int(s['rgb'].own.sum()), device=DEV, generator=_seeded(c))
             prior = s['rgb'].view.clone()
         _place(s['rgb'], img, yv, xv, oy, ox, 0, r['nchw'], prior)
 
@@ -441,7 +424,7 @@ def _place_slice(g, k, part, yv, xv, oy, ox):
     n = torch.arange(N, device=DEV)[:, None, None, None]
     cc = torch.arange(Cn, device=DEV)[None, None, None, :]
     idx = (torch.full_like(n, k), n, oy[yv][None, :, None, None], ox[xv][None, None, :, None], cc)
-    g.owned[idx] = True
+    g.own[idx] = True
     g.expect[idx] = part[:, yv][:, :, xv]
 
 
@@ -475,7 +458,7 @@ def launch_case(s):
 
 
 def _err(got, g):
-    ref = g.expect[g.owned]
+    ref = g.expect[g.own]
     return ((got - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item()
 
 
@@ -487,12 +470,12 @@ def check_case(s):
     def split_pair(name, hi, lo):
         assert hi.untouched_ok() and lo.untouched_ok(), f'{name}: an element outside the output was written'
         assert hi.written() and lo.written(), f'{name}: an owned element was not written'
-        errs[name] = ('split', _err(hi.view[hi.owned].double() + lo.view[lo.owned].double(), hi))
+        errs[name] = ('split', _err(hi.view[hi.own].double() + lo.view[lo.own].double(), hi))
 
     def f32(name, g, kind, accumulate=False):
         assert g.untouched_ok(), f'{name}: an element outside the output was written'
         assert accumulate or g.written(), f'{name}: an owned element was not written'
-        errs[name] = (kind, _err(g.view[g.owned].double(), g))
+        errs[name] = (kind, _err(g.view[g.own].double(), g))
 
     for k, (hi, lo) in enumerate(s['outs']):
         split_pair(f'out{k}', hi, lo)
@@ -522,23 +505,15 @@ def test_conv_gemm_matches_fp64_contract(c):
 def test_launched_instance_matches_plan(tmp_path):
     """Every case under torch.profiler: the conv_gemm_kernel<block_n, block_k> it launched (the template arguments are in the
     demangled name) and its grid are the ones `plan` predicts."""
-    from torch.profiler import ProfilerActivity, profile
     setups = [setup_case(c) for c in CASES]
     torch.cuda.synchronize()
-    try:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for s in setups:
-                launch_case(s)
-            torch.cuda.synchronize()
-    except RuntimeError as e:              # CUPTI missing or busy
-        pytest.skip(f'CUDA activity tracing unavailable: {e}')
-    trace = tmp_path / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and 'conv_gemm_kernel' in e.get('name', '')]
-    if not events:
-        pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')
-    events.sort(key=lambda e: e['ts'])
-    assert len(events) == len(CASES), [e['name'] for e in events]
+
+    def run():
+        for s in setups:
+            launch_case(s)
+        return CASES                        # one conv_gemm_kernel launch per case
+
+    _, events = launched_kernels(run, 'conv_gemm_kernel', tmp_path)
     props = torch.cuda.get_device_properties(0)
     for c, e in zip(CASES, events):
         p = plan(c['N'], c['Cin'], c['Cout'], c['MH'], c['MW'], c['splits'], bool(c['rgb']), sms=props.multi_processor_count,
@@ -554,25 +529,8 @@ def test_launched_instance_matches_plan(tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ alignment (CPU, nothing launched)
-def _lib():
-    from next3d_b200 import _lib as L
-    return L
-
-
-def _misaligned(t):
-    """A view of `t` (16-byte aligned) that starts 4 bytes later."""
-    assert t.data_ptr() % 16 == 0
-    return t.view(-1)[4 // t.element_size():]
-
-
-def _refused(rc, what):
-    L = _lib()
-    msg = L.lib.n3d_last_error().decode()
-    assert rc == -1 and what in msg, (rc, msg)
-
-
 def _desc(a, w, N=1, MH=8, MW=16):
-    L = _lib()
+    L = lib()
     p = L.ConvGemm()
     p.a_hi, p.a_lo, p.w_hi, p.w_lo = a.data_ptr(), a.data_ptr(), w.data_ptr(), w.data_ptr()
     p.NI, p.AH, p.AW, p.Cin = a.shape
@@ -588,31 +546,31 @@ def _desc(a, w, N=1, MH=8, MW=16):
 
 @pytest.mark.parametrize('field', ['out_f32', 'out0.hi', 'out1.lo'])
 def test_conv_gemm_refuses_misaligned_outputs(field):
-    L = _lib()
+    L = lib()
     a = torch.zeros(1, 8, 16, 16, dtype=torch.bfloat16)
     w = torch.zeros(1, 16, 16, dtype=torch.bfloat16)
     f32 = torch.zeros(1 * 8 * 16 * 16 + 64)
     hi = torch.zeros(1 * 8 * 16 * 16 + 64, dtype=torch.bfloat16)
     p = _desc(a, w)
     if field == 'out_f32':
-        p.out_f32, p.f32_cstride = _misaligned(f32).data_ptr(), 16
+        p.out_f32, p.f32_cstride = offset_view(f32, 4).data_ptr(), 16
         what = 'out_f32 must be 16-byte aligned'
     else:
         k, part = int(field[3]), field.split('.')[1]
-        good, bad = hi.data_ptr(), _misaligned(hi).data_ptr()
+        good, bad = hi.data_ptr(), offset_view(hi, 4).data_ptr()
         p.out[k] = L.SplitOut(bad if part == 'hi' else good, bad if part == 'lo' else good, None, 16, 0)
         what = f'split output {k} (hi / lo) must be 16-byte aligned'
-    _refused(L.lib.n3d_conv_gemm(C.byref(p), None), what)
+    refused(L.lib.n3d_conv_gemm(C.byref(p), None), what)
     if field == 'out_f32':                 # the transposed-conv entry point shares the check
         p.T = 9
         w9 = torch.zeros(9, 16, 16, dtype=torch.bfloat16)
         p.w_hi = p.w_lo = w9.data_ptr()
-        _refused(L.lib.n3d_conv_transposed_gemm(C.byref(p), None), what)
+        refused(L.lib.n3d_conv_transposed_gemm(C.byref(p), None), what)
 
 
 def test_conv_gemm_refuses_accumulate_with_split_outputs():
     """The accumulating fp32 store adds the old values into the epilogue's registers before the split outputs are formed from them."""
-    L = _lib()
+    L = lib()
     a = torch.zeros(1, 8, 16, 16, dtype=torch.bfloat16)
     w = torch.zeros(1, 16, 16, dtype=torch.bfloat16)
     f32 = torch.zeros(8 * 16 * 16)
@@ -620,23 +578,23 @@ def test_conv_gemm_refuses_accumulate_with_split_outputs():
     p = _desc(a, w)
     p.out_f32, p.f32_cstride, p.f32_accumulate = f32.data_ptr(), 16, 1
     p.out[1] = L.SplitOut(hi.data_ptr(), hi.data_ptr(), None, 16, 0)
-    _refused(L.lib.n3d_conv_gemm(C.byref(p), None), 'f32_accumulate cannot be combined with split outputs')
+    refused(L.lib.n3d_conv_gemm(C.byref(p), None), 'f32_accumulate cannot be combined with split outputs')
 
 
 def test_conv_gemm_refuses_split_stride_not_multiple_of_4():
-    L = _lib()
+    L = lib()
     a = torch.zeros(1, 8, 16, 16, dtype=torch.bfloat16)
     w = torch.zeros(9, 16, 16, dtype=torch.bfloat16)
     f32 = torch.zeros(2 * 8 * 16 * 16 + 64)
     p = _desc(a, w)
     p.mode, p.out_f32, p.f32_cstride, p.splits, p.split_stride = 1, f32.data_ptr(), 16, 2, 8 * 16 * 16 + 2
-    _refused(L.lib.n3d_conv_gemm(C.byref(p), None), 'split stride that is a multiple of 4')
+    refused(L.lib.n3d_conv_gemm(C.byref(p), None), 'split stride that is a multiple of 4')
 
 
 @pytest.mark.parametrize('entry', ['n3d_splitk_epilogue', 'n3d_fir_up_epilogue'])
 @pytest.mark.parametrize('field', ['raw', 'dcoef', 'bias', 'out_f32', 'out0.hi', 'out1.lo', 'out0.style'])
 def test_epilogues_refuse_misaligned_pointers(entry, field):
-    L = _lib()
+    L = lib()
     N, H, W, Cc = 1, 8, 8, 16
     raw = torch.zeros(N * (H + 1) * (W + 1) * Cc + 64)
     vec = torch.zeros(N * Cc + 64)
@@ -652,10 +610,10 @@ def test_epilogues_refuse_misaligned_pointers(entry, field):
         else:
             what = {'raw': 'raw must be 16-byte aligned', 'dcoef': 'dcoef and bias must be 16-byte aligned',
                     'bias': 'dcoef and bias must be 16-byte aligned', 'out_f32': 'out_f32 must be 16-byte aligned'}[field]
-        ptrs[field] = _misaligned(base[field]).data_ptr()
+        ptrs[field] = offset_view(base[field], 4).data_ptr()
     else:
         k, part = int(field[3]), field.split('.')[1]
-        setattr(outs[k], part, (_misaligned(vec) if part == 'style' else _misaligned(bf)).data_ptr())
+        setattr(outs[k], part, offset_view(vec if part == 'style' else bf, 4).data_ptr())
         what = f'split output {k} (hi / lo / style) must be 16-byte aligned'
     if entry == 'n3d_splitk_epilogue':
         rc = L.lib.n3d_splitk_epilogue(ptrs['raw'], 1, N * H * W * Cc, N, H, W, Cc, ptrs['dcoef'], ptrs['bias'], None, 0, 1.0, 0.2, -1.0,
@@ -663,4 +621,4 @@ def test_epilogues_refuse_misaligned_pointers(entry, field):
     else:
         rc = L.lib.n3d_fir_up_epilogue(ptrs['raw'], N, H, W, Cc, ptrs['dcoef'], ptrs['bias'], None, 0, 1.0, 0.2, -1.0, outs,
                                        ptrs['out_f32'], Cc, 0, None)
-    _refused(rc, what)
+    refused(rc, what)

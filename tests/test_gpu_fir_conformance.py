@@ -21,18 +21,16 @@ kernels everywhere): both reruns must be bit-identical.
 COVERAGE; the profiler test checks on the GPU that each case ran the kernel (and grid) the plan predicts.  The alignment tests at the
 end need no GPU: misaligned host pointers must be refused before any device call.
 """
-import json
 import math
-import os
 import re
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.helpers import Guarded, RangeErr, cdiv, grid_stride, launched_kernels, lib, offset_view, record_errors, refused, rerun_identical
+
 DEV = 'cuda'
-GUARD = 64                  # sentinel elements on each side of an output view: keeps the view's base alignment that of a fresh allocation
-SENTINEL = {torch.float32: (torch.int32, 0x7FC01234), torch.bfloat16: (torch.int16, 0x7FC1)}      # NaN bit patterns no store produces
 SMS = 132                   # SM count the table is planned at (H100 SXM)
 REF_CHANNELS = 16           # channels per fp64 reference chunk
 SQRT2 = math.sqrt(2.0)
@@ -53,19 +51,10 @@ BOUNDS = {
 
 
 # ------------------------------------------------------------------------------------------------ the launch rules, mirrored
-def _cdiv(a, b):
-    return -(-a // b)
-
-
-def grid_stride(work, sms=SMS, per_sm=16, threads=256):
-    """n3d_grid (common.cuh): one block per `threads` work items, at least 1 and at most `per_sm` blocks per SM."""
-    return max(1, min(_cdiv(work, threads), sms * per_sm))
-
-
 def fir_strip_rows(sms, threads_per_row, rows):
     """fir_strip_rows (engine.cu): 16 rows per strip, halved down to 4 while the launch has < 1024 threads per SM, clipped to rows."""
     S = 16
-    while S > 4 and threads_per_row * _cdiv(rows, S) < sms * 1024:
+    while S > 4 and threads_per_row * cdiv(rows, S) < sms * 1024:
         S >>= 1
     return min(S, rows)
 
@@ -82,15 +71,15 @@ def fir_up_plan(N, H2, W2, C, sms=SMS):
             ctas = N * (W2 // TC) * (H2 // tr)
             if ctas < sms:
                 continue
-            eff = ctas / (_cdiv(ctas, 2 * sms) * 2 * sms) * tr / (tr + 3)
+            eff = ctas / (cdiv(ctas, 2 * sms) * 2 * sms) * tr / (tr + 3)
             if eff > best:
                 best, TR = eff, tr
     if TR:
         return dict(kernel='fir_up_stream_kernel', streamed=True, TC=TC, TR=TR, grid=N * (W2 // TC) * (H2 // TR))
     why = ('channels' if not TC else 'width' if W2 % TC else 'height' if all(H2 % tr for tr in (32, 64, 128)) else 'ctas')
     S = fir_strip_rows(sms, N * (W2 // 2) * (C // 4), H2 // 2)
-    total = N * _cdiv(H2 // 2, S) * (W2 // 2) * (C // 4)
-    return dict(kernel='fir_up_epilogue_kernel', streamed=False, S=S, rows=H2 // 2, why=why, work=total, grid=grid_stride(total, sms))
+    total = N * cdiv(H2 // 2, S) * (W2 // 2) * (C // 4)
+    return dict(kernel='fir_up_epilogue_kernel', streamed=False, S=S, rows=H2 // 2, why=why, work=total, grid=grid_stride(total, sms, 16))
 
 
 def fir_down_plan(N, H, W, C, sms=SMS):
@@ -99,12 +88,12 @@ def fir_down_plan(N, H, W, C, sms=SMS):
     c4n, SH, SW = C // 4, (H + 2) // 2, (W + 2) // 2
     TSC = 256 // c4n if 8 <= c4n <= 128 and 256 % c4n == 0 else 0
     for ts in (32, 16):
-        if TSC and N * _cdiv(SW, TSC) * _cdiv(SH, ts) >= sms:
+        if TSC and N * cdiv(SW, TSC) * cdiv(SH, ts) >= sms:
             return dict(kernel='fir_down_stream_kernel', streamed=True, TSC=TSC, TS=ts, ragged_rows=SH % ts != 0, ragged_cols=SW % TSC != 0,
-                        grid=N * _cdiv(SW, TSC) * _cdiv(SH, ts))
+                        grid=N * cdiv(SW, TSC) * cdiv(SH, ts))
     S = fir_strip_rows(sms, N * SW * c4n, SH)
-    total = N * _cdiv(SH, S) * SW * c4n
-    return dict(kernel='fir_down_split_kernel', streamed=False, S=S, rows=SH, work=total, grid=grid_stride(total, sms))
+    total = N * cdiv(SH, S) * SW * c4n
+    return dict(kernel='fir_down_split_kernel', streamed=False, S=S, rows=SH, work=total, grid=grid_stride(total, sms, 16))
 
 
 def upsample2d_vec(C):
@@ -122,10 +111,10 @@ def plan(c, sms=SMS):
     if k == 'upsample':
         v = upsample2d_vec(Cc)
         work = N * H * W * Cc // v
-        return dict(kernel=f'upsample2d_kernel<{v}>', streamed=False, work=work, grid=grid_stride(work, sms))
+        return dict(kernel=f'upsample2d_kernel<{v}>', streamed=False, work=work, grid=grid_stride(work, sms, 16))
     work = {'downsample': N * (H // 2) * (W // 2) * Cc, 'splitk': N * H * W * Cc // 4, 'modsplit': N * H * W * Cc // 4}[k]
     name = {'downsample': 'downsample2d_kernel', 'splitk': 'splitk_epilogue_kernel', 'modsplit': 'modulate_split_kernel'}[k]
-    return dict(kernel=name, streamed=False, work=work, grid=grid_stride(work, sms))
+    return dict(kernel=name, streamed=False, work=work, grid=grid_stride(work, sms, 16))
 
 
 # ------------------------------------------------------------------------------------------------ the case table
@@ -281,45 +270,6 @@ def test_case_table_covers_every_launch_configuration():
 
 
 # ------------------------------------------------------------------------------------------------ outputs and inputs
-class Guarded:
-    """An output tensor as a view into a larger allocation filled with a NaN sentinel.  A launch owns the channels (last dim)
-    [coff, coff + cnum) of every pixel, or all of the view when cnum is None."""
-
-    def __init__(self, shape, dtype, coff=0, cnum=None):
-        n = math.prod(shape)
-        self.int_dtype, self.sentinel = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + n + GUARD, dtype=dtype, device=DEV)
-        self.view = self.buf[GUARD:GUARD + n].view(shape)
-        self.own = slice(coff, coff + (shape[-1] if cnum is None else cnum))
-        self.reset()
-
-    def reset(self):
-        self.buf.view(self.int_dtype).fill_(self.sentinel)
-
-    def untouched_ok(self):
-        """Every element outside the owned channels (guards included) still holds the sentinel's bits."""
-        bits, inner = self.buf.view(self.int_dtype), self.view.view(self.int_dtype)
-        return all(bool((t == self.sentinel).all()) for t in (bits[:GUARD], bits[-GUARD:], inner[..., :self.own.start], inner[..., self.own.stop:]))
-
-    def written(self):
-        return bool((self.view.view(self.int_dtype)[..., self.own] != self.sentinel).all())
-
-
-class RangeErr:
-    """max |got - ref| / max |ref| accumulated over reference chunks."""
-
-    def __init__(self):
-        self.diff = self.range = 0.0
-
-    def add(self, got, ref):
-        d = (got.double() - ref).abs().max().item()
-        self.diff = max(self.diff, d if d == d else math.inf)
-        self.range = max(self.range, ref.abs().max().item())
-
-    def value(self):
-        return self.diff / max(self.range, 1e-30)
-
-
 def _seeded(c):
     return torch.Generator(device=DEV).manual_seed(2000 + CASE_IDS.index(c['name']))
 
@@ -340,11 +290,11 @@ def setup_case(c):
         s['x'] = rnd(N, H, W, Cc)
     if k in _EPI or k == 'modsplit':
         for o in c['outs']:
-            hi, lo = (Guarded((N, H, W, o['cstride']), torch.bfloat16, o['coff'], Cc) for _ in range(2))
+            hi, lo = (Guarded((N, H, W, o['cstride']), torch.bfloat16, slice(o['coff'], o['coff'] + Cc)) for _ in range(2))
             s['outs'].append((hi, lo, rnd(N, Cc) if o['style'] else None))
     if k in _EPI and c['f32']:
         f = c['f32']
-        s['f32'] = Guarded((N, H, W, f['cstride']), torch.float32, f['coff'], Cc)
+        s['f32'] = Guarded((N, H, W, f['cstride']), torch.float32, slice(f['coff'], f['coff'] + Cc))
     if k == 'down':
         SH, SW = (H + 2) // 2, (W + 2) // 2
         s['outs'] = [(Guarded((4, N, SH, SW, Cc), torch.bfloat16), Guarded((4, N, SH, SW, Cc), torch.bfloat16), None)]
@@ -459,7 +409,7 @@ def check_case(s):
         SH, SW = (H + 2) // 2, (W + 2) // 2
         # the pad row and column beyond the (H+1) x (W+1) FIR output are exact zeros (parities with a = 1 / b = 1)
         for t in (hi, lo):
-            bits = t.view.view(t.int_dtype)
+            bits = t.bits()
             assert (bits[2:, :, SH - 1] == 0).all() and (bits[1::2, :, :, SW - 1] == 0).all(), f'{c["name"]}: pad row / column not zero'
         for n, c0, c1 in _chunks(s):
             x = s['x'][n, ..., c0:c1].permute(2, 0, 1).double()[None]
@@ -481,26 +431,6 @@ def check_case(s):
     return errs
 
 
-def _record(c, errs):
-    path = os.environ.get('N3D_FIR_ERRORS')
-    if path:
-        with open(path, 'a') as f:
-            for kind, e in errs.items():
-                f.write(json.dumps({'case': c['name'], 'kind': kind, 'err': e, 'bound': BOUNDS[kind]}) + '\n')
-
-
-def _snapshot(s):
-    return [t.buf.view(t.int_dtype).cpu() for t in outputs(s)]
-
-
-def _rerun_identical(s, snap):
-    for t in outputs(s):
-        t.reset()
-    launch_case(s)
-    torch.cuda.synchronize()
-    return all(torch.equal(a, b) for a, b in zip(snap, _snapshot(s)))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('c', CASES, ids=CASE_IDS)
 def test_kernel_matches_fp64_reference(c, monkeypatch):
@@ -509,44 +439,34 @@ def test_kernel_matches_fp64_reference(c, monkeypatch):
     launch_case(s)
     torch.cuda.synchronize()
     errs = check_case(s)
-    _record(c, errs)
+    record_errors('N3D_FIR_ERRORS', [{'case': c['name'], 'kind': k, 'err': e, 'bound': BOUNDS[k]} for k, e in errs.items()])
     bad = {k: e for k, e in errs.items() if not e < BOUNDS[k]}
     assert not bad, bad
-    snap = _snapshot(s)
-    assert _rerun_identical(s, snap), f'{c["name"]}: a rerun is not bit-identical'
+    rerun = lambda: rerun_identical(outputs(s), lambda: launch_case(s))        # noqa: E731
+    assert rerun(), f'{c["name"]}: a rerun is not bit-identical'
     if plan(c, torch.cuda.get_device_properties(0).multi_processor_count)['streamed']:
         monkeypatch.setenv('N3D_FIR_STREAM', '0')
-        assert _rerun_identical(s, snap), f'{c["name"]}: the register-tiled kernel is not bit-identical to the streamed one'
+        assert rerun(), f'{c["name"]}: the register-tiled kernel is not bit-identical to the streamed one'
 
 
 @pytest.mark.gpu
 def test_launched_kernel_matches_plan(tmp_path, monkeypatch):
     """Every case under torch.profiler: the kernel it launched and its grid are the ones `plan` predicts at the device's SM count."""
-    from torch.profiler import ProfilerActivity, profile
     monkeypatch.delenv('N3D_FIR_STREAM', raising=False)
     pattern = re.compile(r'fir_up_stream_kernel|fir_up_epilogue_kernel|fir_down_stream_kernel|fir_down_split_kernel|upsample2d_kernel<\d>|'
                          r'downsample2d_kernel|modulate_split_kernel|splitk_epilogue_kernel')
-    # A profiler session that follows another one in the same process can drop its first kernel records (see
-    # test_gpu_render_conformance.py), so the table runs twice and the last len(CASES) records are compared.
-    try:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(2):
-                for c in CASES:            # one case at a time: the largest ones do not fit in memory together
-                    s = setup_case(c)
-                    launch_case(s)
-                    torch.cuda.synchronize()
-                    del s
-    except RuntimeError as e:              # CUPTI missing or busy
-        pytest.skip(f'CUDA activity tracing unavailable: {e}')
-    trace = tmp_path / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and pattern.search(e.get('name', ''))]
-    if not events:
-        pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')
-    events.sort(key=lambda e: e['ts'])
-    assert len(CASES) <= len(events) <= 2 * len(CASES), [e['name'] for e in events]
+
+    def run():
+        for c in CASES:                     # one case at a time: the largest ones do not fit in memory together
+            s = setup_case(c)
+            launch_case(s)
+            torch.cuda.synchronize()
+            del s
+        return CASES                        # one launch per case
+
+    _, events = launched_kernels(run, pattern, tmp_path)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    for c, e in zip(CASES, events[-len(CASES):]):
+    for c, e in zip(CASES, events):
         p = plan(c, sms)
         assert pattern.search(e['name']).group(0) == p['kernel'], (c['name'], e['name'], p)
         grid = e.get('args', {}).get('grid')
@@ -555,57 +475,41 @@ def test_launched_kernel_matches_plan(tmp_path, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ alignment (CPU, nothing launched)
-def _lib():
-    from next3d_b200 import _lib as L
-    return L
-
-
-def _misaligned(t):
-    """A view of `t` (16-byte aligned) that starts 4 bytes later."""
-    assert t.data_ptr() % 16 == 0
-    return t.view(-1)[4 // t.element_size():]
-
-
-def _refused(rc, what):
-    msg = _lib().lib.n3d_last_error().decode()
-    assert rc == -1 and what in msg, (rc, msg)
-
-
 @pytest.mark.parametrize('field', ['x', 'hi', 'lo'])
 def test_fir_down_split_refuses_misaligned_pointers(field):
-    L = _lib()
+    L = lib()
     N, H, W, Cc = 1, 8, 8, 16
     x = torch.zeros(N * H * W * Cc + 64)
     bf = {k: torch.zeros(4 * N * 5 * 5 * Cc + 64, dtype=torch.bfloat16) for k in ('hi', 'lo')}
     p = dict(x=x.data_ptr(), hi=bf['hi'].data_ptr(), lo=bf['lo'].data_ptr())
-    p[field] = _misaligned(x if field == 'x' else bf[field]).data_ptr()
+    p[field] = offset_view(x if field == 'x' else bf[field], 4).data_ptr()
     what = 'x must be 16-byte aligned' if field == 'x' else 'hi and lo must be 8-byte aligned'
-    _refused(L.lib.n3d_fir_down_split(p['x'], N, H, W, Cc, p['hi'], p['lo'], None), what)
+    refused(L.lib.n3d_fir_down_split(p['x'], N, H, W, Cc, p['hi'], p['lo'], None), what)
 
 
 @pytest.mark.parametrize('field', ['x', 'style', 'hi', 'lo'])
 def test_modulate_split_refuses_misaligned_pointers(field):
-    L = _lib()
+    L = lib()
     N, HW, Cc = 1, 16, 16
     f32 = {k: torch.zeros(N * HW * Cc + 64) for k in ('x', 'style')}
     bf = {k: torch.zeros(N * HW * Cc + 64, dtype=torch.bfloat16) for k in ('hi', 'lo')}
     t = {**f32, **bf}
     p = {k: v.data_ptr() for k, v in t.items()}
-    p[field] = _misaligned(t[field]).data_ptr()
+    p[field] = offset_view(t[field], 4).data_ptr()
     what = 'x and style must be 16-byte aligned' if field in f32 else 'hi and lo must be 8-byte aligned'
-    _refused(L.lib.n3d_modulate_split(p['x'], HW, N, Cc, p['style'], p['hi'], p['lo'], Cc, 0, None), what)
+    refused(L.lib.n3d_modulate_split(p['x'], HW, N, Cc, p['style'], p['hi'], p['lo'], Cc, 0, None), what)
 
 
 @pytest.mark.parametrize('field', ['blended_front', 'tex_planes', 'static_planes', 'planes'])
 def test_blend_planes_refuses_misaligned_pointers(field):
-    L = _lib()
+    L = lib()
     N, H, W = 1, 4, 4
     t = dict(blended_front=torch.zeros(N * H * W * 32 + 64), tex_planes=torch.zeros(3 * N * H * W * 32 + 64),
              static_planes=torch.zeros(N * H * W * 96 + 64), planes=torch.zeros(N * 3 * H * W * 32 + 64))
     alpha = torch.zeros(3 * N * H * W)
     p = {k: v.data_ptr() for k, v in t.items()}
-    p[field] = _misaligned(t[field]).data_ptr()
-    _refused(L.lib.n3d_blend_planes(p['blended_front'], p['tex_planes'], alpha.data_ptr(), p['static_planes'], N, H, W, p['planes'], None),
+    p[field] = offset_view(t[field], 4).data_ptr()
+    refused(L.lib.n3d_blend_planes(p['blended_front'], p['tex_planes'], alpha.data_ptr(), p['static_planes'], N, H, W, p['planes'], None),
              'blended_front, tex_planes, static_planes and planes must be 16-byte aligned')
 
 
@@ -616,12 +520,13 @@ def test_upsample2d_takes_scalar_path_for_misaligned_pointers(nchw):
     from next3d_b200 import kernels as K
     from oracle import ops as oo
     N, H, W, Cc = 2, 5, 7, 8
-    x = _misaligned(torch.randn(N * H * W * Cc + 64, device=DEV, generator=torch.Generator(device=DEV).manual_seed(7)))[:N * H * W * Cc]
-    y = _misaligned(torch.full((N * 4 * H * W * Cc + 64,), float('nan'), device=DEV))[:N * 4 * H * W * Cc]
+    x = offset_view(torch.randn(N * H * W * Cc + 64, device=DEV, generator=torch.Generator(device=DEV).manual_seed(7)), 4)[:N * H * W * Cc]
+    y = offset_view(torch.full((N * 4 * H * W * Cc + 64,), float('nan'), device=DEV), 4)[:N * 4 * H * W * Cc]
     y = y.view(N, Cc, 2 * H, 2 * W) if nchw else y.view(N, 2 * H, 2 * W, Cc)
     K.upsample2d_nhwc(x.view(N, H, W, Cc), y, y_nchw=nchw)
     ref = oo.upsample2d(x.view(N, H, W, Cc).permute(0, 3, 1, 2).double(), _filter64())
     got = y if nchw else y.permute(0, 3, 1, 2)
     err = ((got.double() - ref).abs().max() / ref.abs().max()).item()
-    _record(dict(name=f'upsample_misaligned_{"nchw" if nchw else "nhwc"}'), {'upsample': err})
+    record_errors('N3D_FIR_ERRORS', [{'case': f'upsample_misaligned_{"nchw" if nchw else "nhwc"}', 'kind': 'upsample', 'err': err,
+                                      'bound': BOUNDS['upsample']}])
     assert err < BOUNDS['upsample'], err

@@ -16,9 +16,6 @@ be bit-identical.  `plan` mirrors each entry point's launch rule in plain Python
 in COVERAGE, and the profiler test checks on the GPU that each case launched the kernels and grids the plan predicts.  The refusal
 tests at the end need no GPU: arguments outside an entry point's contract must be refused before any device call.
 """
-import json
-import math
-import os
 import re
 
 import numpy as np
@@ -26,9 +23,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.helpers import Guarded, RangeErr, cdiv, grid_stride, launched_kernels, lib, record_errors, refused, rerun_identical
+
 DEV = 'cuda'
-GUARD = 64                  # sentinel elements on each side of an output view
-SENTINEL = {torch.float32: (torch.int32, 0x7FC01234), torch.int32: (torch.int32, 0x7FC01234), torch.bfloat16: (torch.int16, 0x7FC1)}
 SMS = 132                   # SM count the table is planned at (H100 SXM)
 
 # Error bounds of the inexact kernels, each at most 4x the worst case measured over the table on an H100 80GB HBM3 (700 W power
@@ -46,15 +43,6 @@ BOUNDS = {
 
 
 # ------------------------------------------------------------------------------------------------ the launch rules, mirrored
-def _cdiv(a, b):
-    return -(-a // b)
-
-
-def grid_stride(work, sms=SMS, per_sm=8, threads=256):
-    """n3d_grid (common.cuh): one block per `threads` work items, at least 1 and at most `per_sm` blocks per SM."""
-    return max(1, min(_cdiv(work, threads), sms * per_sm))
-
-
 def resize_wide(C, aligned=True):
     """n3d_resize_aa: the warp-per-pixel kernel for C = 4 * 2^k <= 128 and a 16-byte aligned src, else one thread per element."""
     return C % 4 == 0 and C <= 128 and 32 % (C // 4) == 0 and aligned
@@ -99,16 +87,16 @@ def plan(c, sms=SMS):
     """The kernels a case launches, in order, each as (name, grid)."""
     k = c['kind']
     if k == 'transform':
-        return [('transform_kernel', (grid_stride(c['N'] * c['nviews'] * c['P'], sms), 1, 1))]
+        return [('transform_kernel', (grid_stride(c['N'] * c['nviews'] * c['P'], sms, 8), 1, 1))]
     if k == 'raster':
-        bins = _cdiv(c['W'], 16) * _cdiv(c['H'], 16)
-        return [('raster_setup_kernel', (grid_stride(c['NM'] * c['F'], sms), 1, 1)), ('rasterize_kernel', (bins, c['NM'], 1))]
+        bins = cdiv(c['W'], 16) * cdiv(c['H'], 16)
+        return [('raster_setup_kernel', (grid_stride(c['NM'] * c['F'], sms, 8), 1, 1)), ('rasterize_kernel', (bins, c['NM'], 1))]
     if k == 'uv':
         return [('uv_sample_kernel', (grid_stride(c['N'] * c['H'] * c['W'] * 32, sms, 16), 1, 1))]
     if k == 'fill':
         return [('fill_mouth_kernel', (c['NI'], 1, 1))]
     if k == 'box':
-        return [('mouth_box_kernel', (_cdiv(c['N'], 64), 1, 1))]
+        return [('mouth_box_kernel', (cdiv(c['N'], 64), 1, 1))]
     if k == 'resize':
         pix = c['N'] * c['DH'] * c['DW']
         if resize_wide(c['C'], not c['misalign']):
@@ -285,35 +273,6 @@ def test_case_table_covers_every_launch_path():
     missing = [k for k, ok in COVERAGE.items() if not ok(planned)]
     assert not missing, missing
     assert len(set(CASE_IDS)) == len(CASE_IDS)
-
-
-# ------------------------------------------------------------------------------------------------ outputs
-class Guarded:
-    """An output tensor as a view into a larger allocation filled with a sentinel.  A launch owns the elements where `own` (a bool
-    tensor broadcastable to the view) is true, or all of the view when own is None."""
-
-    def __init__(self, shape, dtype, own=None):
-        n = math.prod(shape)
-        self.int_dtype, self.sentinel = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + n + GUARD, dtype=dtype, device=DEV)
-        self.view = self.buf[GUARD:GUARD + n].view(shape)
-        self.own = None if own is None else own.to(DEV).expand(shape)
-        self.reset()
-
-    def reset(self):
-        self.buf.view(self.int_dtype).fill_(self.sentinel)
-
-    def bits(self):
-        return self.view.view(self.int_dtype)
-
-    def untouched_ok(self):
-        b = self.buf.view(self.int_dtype)
-        ok = bool((b[:GUARD] == self.sentinel).all()) and bool((b[-GUARD:] == self.sentinel).all())
-        return ok and (self.own is None or bool((self.bits()[~self.own] == self.sentinel).all()))
-
-    def written(self):
-        b = self.bits()
-        return bool((b != self.sentinel).all()) if self.own is None else bool((b[self.own] != self.sentinel).all())
 
 
 def _f32(x):
@@ -649,7 +608,7 @@ def setup_case(c):
         s['dst_box'] = torch.tensor(c['dst_box'], dtype=torch.int32, device=DEV) if c['dst_box'] else None
         own = None
         if c['dst_box']:
-            own = torch.zeros(N, DH, DW, 1, dtype=torch.bool)
+            own = torch.zeros(N, DH, DW, 1, dtype=torch.bool, device=DEV)
             for i, (y0, y1, x0, x1) in enumerate(c['dst_box']):
                 own[i, y0:y1, x0:x1] = True
         s['style'] = _rnd(g, N, C) if c['outs'] in ('split', 'both') else None
@@ -723,19 +682,6 @@ def _mismatch(got, ref):
     """Count and first index of bitwise differences between two fp32 / int32 tensors."""
     d = _bits(got.cpu()) != _bits(ref.cpu())
     return int(d.sum()), (d.nonzero()[0].tolist() if d.any() else None)
-
-
-class RangeErr:
-    def __init__(self):
-        self.diff = self.range = 0.0
-
-    def add(self, got, ref):
-        d = (got.double() - ref).abs().max().item()
-        self.diff = max(self.diff, d if d == d else math.inf)
-        self.range = max(self.range, ref.abs().max().item())
-
-    def value(self):
-        return self.diff / max(self.range, 1e-30)
 
 
 def uv_reference(s):
@@ -831,18 +777,6 @@ def check_case(s):
     return errs
 
 
-def _record(name, errs):
-    path = os.environ.get('N3D_MESH_ERRORS')
-    if path:
-        with open(path, 'a') as f:
-            for kind, e in errs.items():
-                f.write(json.dumps({'case': name, 'kind': kind, 'err': e, 'bound': BOUNDS[kind]}) + '\n')
-
-
-def _snapshot(s):
-    return {n: t.buf.view(t.int_dtype).cpu() for n, t in s['outs'].items()}
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('c', CASES, ids=CASE_IDS)
 def test_kernel_matches_reference(c):
@@ -850,49 +784,33 @@ def test_kernel_matches_reference(c):
     launch_case(s)
     torch.cuda.synchronize()
     errs = check_case(s)
-    _record(c['name'], errs)
+    record_errors('N3D_MESH_ERRORS', [{'case': c['name'], 'kind': k, 'err': e, 'bound': BOUNDS[k]} for k, e in errs.items()])
     bad = {k: e for k, e in errs.items() if not e < BOUNDS[k]}
     assert not bad, bad
-    snap = _snapshot(s)
-    for t in s['outs'].values():
-        t.reset()
-    launch_case(s)
-    torch.cuda.synchronize()
-    again = _snapshot(s)
-    assert all(torch.equal(snap[n], again[n]) for n in snap), f'{c["name"]}: a rerun is not bit-identical'
+    assert rerun_identical(list(s['outs'].values()), lambda: launch_case(s)), f'{c["name"]}: a rerun is not bit-identical'
 
 
 @pytest.mark.gpu
 def test_launched_kernels_match_plan(tmp_path):
     """Every case under torch.profiler: the kernels it launched and their grids are the ones `plan` predicts at the device's SM
     count."""
-    from torch.profiler import ProfilerActivity, profile
     names = ('raster_setup_kernel', 'rasterize_kernel', 'transform_kernel', 'uv_sample_kernel', 'fill_mouth_kernel', 'mouth_box_kernel',
              'resize_aa_scalar_kernel', 'resize_aa_kernel', 'blend_kernel')
     pattern = re.compile(r'(?<![\w])(' + '|'.join(names) + r')(?![\w])')
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    expected = [e for c in CASES for e in plan(c, sms)]
     setups = [setup_case(c) for c in CASES]
     torch.cuda.synchronize()
-    # A profiler session that follows another one in the same process can drop its first kernel records (see
-    # test_gpu_render_conformance.py), so the table runs twice and the last len(expected) records are compared.
-    try:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            for _ in range(2):
-                for s in setups:
-                    launch_case(s)
-                    torch.cuda.synchronize()
-    except RuntimeError as e:              # CUPTI missing or busy
-        pytest.skip(f'CUDA activity tracing unavailable: {e}')
-    trace = tmp_path / 'trace.json'
-    prof.export_chrome_trace(str(trace))
-    events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and pattern.search(e.get('name', ''))]
-    if not events:
-        pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')
-    events.sort(key=lambda e: e['ts'])
-    assert len(expected) <= len(events) <= 2 * len(expected), [e['name'] for e in events]
-    owners = [c['name'] for c in CASES for _ in plan(c, sms)]
-    for who, (kernel, grid), e in zip(owners, expected, events[-len(expected):]):
+
+    def run():
+        expected = []
+        for s in setups:
+            launch_case(s)
+            torch.cuda.synchronize()
+            expected += [(s['c']['name'], kernel, grid) for kernel, grid in plan(s['c'], sms)]
+        return expected
+
+    expected, events = launched_kernels(run, pattern, tmp_path)
+    for (who, kernel, grid), e in zip(expected, events):
         assert pattern.search(e['name']).group(1) == kernel, (who, e['name'], kernel)
         got = e.get('args', {}).get('grid')
         if got is not None:
@@ -953,47 +871,37 @@ def test_fill_edges_are_exact():
         assert lo_out is None or prod(lo_out) < seed
 
 
-def _lib():
-    from next3d_b200 import _lib as L
-    return L
-
-
-def _refused(rc, what):
-    msg = _lib().lib.n3d_last_error().decode()
-    assert rc == -1 and what in msg, (rc, msg)
-
-
 def test_uv_sample_refuses_more_than_32_channels():
-    L = _lib()
+    L = lib()
     t = torch.zeros(1024)
     p = t.data_ptr()
-    _refused(L.lib.n3d_uv_sample(p, p, p, p, p, 1, 4, 4, 4, 4, 33, 4, 4, p, p, None), 'C 33 > 32')
+    refused(L.lib.n3d_uv_sample(p, p, p, p, p, 1, 4, 4, 4, 4, 33, 4, 4, p, p, None), 'C 33 > 32')
 
 
 @pytest.mark.parametrize('what', ['images', 'workspace'])
 def test_rasterize_refuses_bad_launches(what):
-    L = _lib()
+    L = lib()
     t = torch.zeros(4096)
     p = t.data_ptr()
     if what == 'images':
-        _refused(L.lib.n3d_rasterize(p, p, 65536, 3, 1, 16, 16, p, p, p, None), 'too many images (65536)')
+        refused(L.lib.n3d_rasterize(p, p, 65536, 3, 1, 16, 16, p, p, p, None), 'too many images (65536)')
     else:
         assert p % 16 == 0
-        _refused(L.lib.n3d_rasterize(p, p, 1, 3, 1, 16, 16, p, p, p + 4, None), 'workspace must be 16-byte aligned')
+        refused(L.lib.n3d_rasterize(p, p, 1, 3, 1, 16, 16, p, p, p + 4, None), 'workspace must be 16-byte aligned')
 
 
 @pytest.mark.parametrize('H,W,b0,b1,what', [(512, 397, 0, 0, 'too large'), (397, 512, 0, 1, 'too large'), (8, 8, 0, 3, 'binarized images'),
                                              (8, 8, 1, 0, 'binarized images'), (8, 8, -1, 1, 'binarized images')])
 def test_fill_mouth_refuses_bad_launches(H, W, b0, b1, what):
-    L = _lib()
+    L = lib()
     t = torch.zeros(16)
-    _refused(L.lib.n3d_fill_mouth_binarize(t.data_ptr(), 2, H, W, b0, b1, None), what)
+    refused(L.lib.n3d_fill_mouth_binarize(t.data_ptr(), 2, H, W, b0, b1, None), what)
     if what == 'too large':
-        _refused(L.lib.n3d_fill_mouth(t.data_ptr(), 2, H, W, None), what)
+        refused(L.lib.n3d_fill_mouth(t.data_ptr(), 2, H, W, None), what)
 
 
 def test_resize_aa_refuses_hi_without_lo():
-    L = _lib()
+    L = lib()
     t = torch.zeros(1024)
     p = t.data_ptr()
-    _refused(L.lib.n3d_resize_aa(p, 1, 4, 4, 4, None, None, 4, 4, None, None, p, None, None), 'hi without lo')
+    refused(L.lib.n3d_resize_aa(p, 1, 4, 4, 4, None, None, 4, 4, None, None, p, None, None), 'hi without lo')

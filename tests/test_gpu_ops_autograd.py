@@ -4,14 +4,12 @@ Truth is oracle.ops under torch.autograd in fp64, on the same inputs rounded as 
 (tests.helpers.range_rel_err) and at most 4x the worst error measured on an H100 80GB HBM3 at a 400 W power limit.  Set
 N3D_GRAD_ERRORS=<file> to append every measured error to that file as JSON lines.
 """
-import json
 import math
-import os
 
 import pytest
 import torch
 
-from tests.helpers import range_rel_err
+from tests.helpers import range_rel_err, record_errors
 
 pytestmark = pytest.mark.gpu
 
@@ -30,10 +28,7 @@ def _g(s):
 
 def _check(case, what, a, ref, bound):
     err = range_rel_err(a.detach().cpu(), ref.detach().cpu())
-    path = os.environ.get('N3D_GRAD_ERRORS')
-    if path:
-        with open(path, 'a') as f:
-            f.write(json.dumps({'case': case, 'what': what, 'err': err, 'bound': bound}) + '\n')
+    record_errors('N3D_GRAD_ERRORS', [{'case': case, 'what': what, 'err': err, 'bound': bound}])
     assert err < bound, (case, what, err, bound)
 
 

@@ -15,21 +15,18 @@ element must keep its bits.
 `plan` mirrors the work decomposition of make_fused / launch_render (render_fused.cu) in plain Python.  The CPU test checks that the
 table covers everything listed in COVERAGE; the profiler test checks on the GPU that each case launched the kernel instance and grid
 `plan` predicts.  The alignment tests at the end need no GPU: descriptors over misaligned CPU tensors are refused before any launch.
+N3D_RENDER_ERRORS=<file> appends every measured error to <file> as JSON lines, to re-measure the worst cases beside BOUNDS.
 """
 import ctypes as C
-import json
 import math
-import os
 import re
 
 import pytest
 import torch
 
-from tests.helpers import range_rel_err
+from tests.helpers import Guarded, launched_kernels, lib, offset_view, range_rel_err, record_errors, refused
 
 DEV = 'cuda'
-GUARD = 64                      # sentinel floats on each side of an output view
-SENTINEL = 0x7FC01234           # a NaN bit pattern no store produces
 U_MAX = 1.0 - 2.0 ** -24        # the largest value torch.rand returns
 
 # Range-relative error bounds, max |got - ref| / max |ref| per output.  'oracle': the bound of test_render_rays; 'points': that of
@@ -63,10 +60,6 @@ BOUNDS = {
 
 def bound(ref, c, out):
     return BOUNDS.get((ref, c['name'], out), BOUNDS.get((ref, c['name']), BOUNDS[ref]))
-
-
-# N3D_RENDER_ERRORS=<file>: append every measured error to <file> as JSON lines, to re-measure the worst cases beside BOUNDS.
-MEASURED = os.environ.get('N3D_RENDER_ERRORS')
 
 
 # ------------------------------------------------------------------------------------------------ the launch rule, mirrored
@@ -286,29 +279,10 @@ def oracle(s, dtype=torch.float32):
     return rgb, depth, wsum, mm
 
 
-class Guarded:
-    """An fp32 output as a view into a larger allocation filled with the sentinel; every element of the view is owned."""
-
-    def __init__(self, shape, init=None):
-        n = math.prod(shape)
-        self.buf = torch.empty(GUARD + n + GUARD, device=DEV)
-        self.buf.view(torch.int32).fill_(SENTINEL)
-        self.view = self.buf[GUARD:GUARD + n].view(shape)
-        if init is not None:
-            self.view.copy_(init)
-
-    def guards_kept(self):
-        bits = self.buf.view(torch.int32)
-        return bool((bits[:GUARD] == SENTINEL).all() and (bits[-GUARD:] == SENTINEL).all())
-
-    def written(self):
-        return bool((self.view.reshape(-1).view(torch.int32) != SENTINEL).all())
-
-
 def _outputs(c):
     N, M = c['N'], c['res'] ** 2
     init = torch.tensor([float('inf'), float('-inf')], device=DEV)
-    mm = Guarded((N, 2), init.expand(N, 2)) if c['per_image'] else Guarded((2,), init)
+    mm = Guarded((N, 2), init=init.expand(N, 2)) if c['per_image'] else Guarded((2,), init=init)
     return dict(rgb=Guarded((N, M, 32)), depth=Guarded((N, M)), wsum=Guarded((N, M)), mm=mm)
 
 
@@ -337,13 +311,6 @@ def launch_case(s, out, dv=None, views=None, normal=None, work=None):
         K.depth_clamp(out['depth'].view, out['mm'].view)
 
 
-def _record(kind, name, errs):
-    """Append the measured errors to the N3D_RENDER_ERRORS file, when that variable is set."""
-    if MEASURED:
-        with open(MEASURED, 'a') as f:
-            f.write(json.dumps({'kind': kind, 'case': name, **errs}) + '\n')
-
-
 # ------------------------------------------------------------------------------------------------ n3d_render_rays
 @pytest.mark.gpu
 @pytest.mark.parametrize('c', CASES, ids=CASE_IDS)
@@ -354,7 +321,7 @@ def test_render_rays_matches_contract(c):
     launch_case(s, out, dv)
     torch.cuda.synchronize()
     for k, g in out.items():
-        assert g.guards_kept(), f'{k}: an element outside the output was written'
+        assert g.untouched_ok(), f'{k}: an element outside the output was written'
         assert g.written(), f'{k}: an owned element was not written'
     rgb, depth, wsum, mm = (out[k].view.cpu() for k in ('rgb', 'depth', 'wsum', 'mm'))
     assert torch.isfinite(rgb).all() and torch.isfinite(depth).all() and torch.isfinite(wsum).all() and torch.isfinite(mm).all()
@@ -366,12 +333,12 @@ def test_render_rays_matches_contract(c):
         assert (rgb == (1.0 if c['white_back'] else -1.0)).all()
         far = mm[:, 1:] if c['per_image'] else mm[1]
         assert torch.equal(depth, far.expand_as(depth))
-    _record('oracle', c['name'], errs)
+    record_errors('N3D_RENDER_ERRORS', [{'kind': 'oracle', 'case': c['name'], **errs}])
     bad = {k: e for k, e in errs.items() if not e < bound('oracle', c, k)}
     if c['density'] not in ('transparent', 'opaque'):
         ref64 = oracle(s, torch.float64)
         errs64 = {k: range_rel_err(x, r) for k, x, r in zip(('rgb', 'depth', 'wsum'), (rgb, depth, wsum), ref64)}
-        _record('fp64', c['name'], errs64)
+        record_errors('N3D_RENDER_ERRORS', [{'kind': 'fp64', 'case': c['name'], **errs64}])
         bad.update({f'fp64 {k}': e for k, e in errs64.items() if not e < bound('fp64', c, k)})
     assert not bad, bad
 
@@ -402,7 +369,7 @@ def test_render_rays_normals_matches_contract(c):
     torch.cuda.synchronize()
     for k in a:
         assert torch.equal(a[k].view, b[k].view), k
-    assert normal.guards_kept() and normal.written() and work.guards_kept() and work.written()
+    assert normal.untouched_ok() and normal.written() and work.untouched_ok() and work.written()
     planes = s['planes'].repeat_interleave(c['views'], 0)
     o, d = orr.ray_sampler(s['cam2world'], s['intr'], c['res'])
     ref = onr.render_normals(s['sd'], planes, o, d, s['opts'], s['u_c'], s['u_f'], return_samples=True)
@@ -497,9 +464,9 @@ def test_sample_points_matches_oracle(pc):
     for name, g, ref in (('sigma', sigma, sig_ref[..., 0]), ('rgb', rgb, rgb_ref)):
         if g is None:
             continue
-        assert g.guards_kept() and g.written(), name
+        assert g.untouched_ok() and g.written(), name
         errs[name] = range_rel_err(g.view.cpu(), ref)
-    _record('points', pc['name'], errs)
+    record_errors('N3D_RENDER_ERRORS', [{'kind': 'points', 'case': pc['name'], **errs}])
     assert all(e < BOUNDS['points'] for e in errs.values()), errs
 
 
@@ -519,12 +486,12 @@ def test_sample_grid_non_square_planes_box_0_5():
     out = Guarded((R, R, R))
     K.sample_grid(planes.permute(0, 1, 3, 4, 2).contiguous().to(DEV)[0], R, 1.0, 0.5, _dec(sd), out.view, pad=pad)
     torch.cuda.synchronize()
-    assert out.guards_kept() and out.written()
+    assert out.untouched_ok() and out.written()
     got = out.view.cpu()
     border = ref == -1000.0
     assert border.any() and torch.equal(got[border], ref[border])
     err = range_rel_err(got[~border], ref[~border])
-    _record('grid', 'planes_48x80_box_0.5', {'sigma': err})
+    record_errors('N3D_RENDER_ERRORS', [{'kind': 'grid', 'case': 'planes_48x80_box_0.5', 'sigma': err}])
     assert err < BOUNDS['points'], err
 
 
@@ -607,7 +574,6 @@ def test_plane_sets_at_the_end_of_32_bit_texel_offsets():
 def test_launched_kernels_match_plan(tmp_path):
     """Every case under torch.profiler: the render_fused_kernel<L, export> it launched (the template arguments are in the demangled
     name) and its grid are the ones `plan` predicts; normals_fused_kernel (not a template) and points_fused_kernel<rgb> likewise."""
-    from torch.profiler import ProfilerActivity, profile
     from next3d_b200 import kernels as K
     props = torch.cuda.get_device_properties(0)
     sms = props.multi_processor_count
@@ -637,24 +603,9 @@ def test_launched_kernels_match_plan(tmp_path):
             expected.append((pc['name'], f'points_fused_kernel<{"true" if pc["rgb"] else "false"}>', points_grid(*coords.shape[:2], sms)))
         return expected
 
-    # A profiler session that follows another one in the same process can drop its first kernel records (seen after the conv_gemm
-    # profiler test in a full run), so the table runs twice and the last len(expected) records are compared.
-    try:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            launch_all()
-            expected = launch_all()
-            torch.cuda.synchronize()
-    except RuntimeError as e:              # CUPTI missing or busy
-        pytest.skip(f'CUDA activity tracing unavailable: {e}')
-    trace = tmp_path / 'trace.json'
-    prof.export_chrome_trace(str(trace))
     pat = re.compile(r'(render_fused_kernel<\d+, (?:true|false)>|normals_fused_kernel|points_fused_kernel<(?:true|false)>)')
-    events = [e for e in json.loads(trace.read_text()).get('traceEvents', []) if e.get('cat') == 'kernel' and pat.search(e.get('name', ''))]
-    if not events:
-        pytest.skip('the trace recorded no kernel activity (CUPTI unavailable)')
-    events.sort(key=lambda e: e['ts'])
-    assert len(expected) <= len(events) <= 2 * len(expected), [e['name'] for e in events]
-    for (name, kernel, grid), e in zip(expected, events[-len(expected):]):
+    expected, events = launched_kernels(launch_all, pat, tmp_path)
+    for (name, kernel, grid), e in zip(expected, events):
         assert pat.search(e['name']).group(1) == kernel, (name, e['name'], kernel)
         g = e.get('args', {}).get('grid')
         if g is not None:
@@ -662,22 +613,6 @@ def test_launched_kernels_match_plan(tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ alignment (CPU, nothing launched)
-def _lib():
-    from next3d_b200 import _lib as L
-    return L
-
-
-def _offset(t, nbytes):
-    """A view of `t` (64-byte aligned CPU allocation) that starts `nbytes` later."""
-    assert t.data_ptr() % 64 == 0
-    return t.view(-1)[nbytes // t.element_size():]
-
-
-def _refused(rc, what):
-    msg = _lib().lib.n3d_last_error().decode()
-    assert rc == -1 and what in msg, (rc, msg)
-
-
 def _render_desc(planes_ptr):
     from next3d_b200 import config, kernels as K
     planes = torch.zeros(1, 3, 4, 4, 32)
@@ -691,18 +626,18 @@ def _render_desc(planes_ptr):
 
 @pytest.mark.parametrize('entry', ['n3d_render_rays', 'n3d_render_rays_normals'])
 def test_render_refuses_misaligned_planes(entry):
-    L = _lib()
+    L = lib()
     buf = torch.zeros(3 * 4 * 4 * 32 + 64)
-    p, out = _render_desc(_offset(buf, 16).data_ptr())
+    p, out = _render_desc(offset_view(buf, 16).data_ptr())
     if entry == 'n3d_render_rays':
         rc = L.lib.n3d_render_rays(C.byref(p), None)
     else:
         rc = L.lib.n3d_render_rays_normals(C.byref(p), out.data_ptr(), out.data_ptr(), None)
-    _refused(rc, f'{entry}: planes must be 32-byte aligned')
+    refused(rc, f'{entry}: planes must be 32-byte aligned')
 
 
 def _sample_points(planes_ptr, rgb_ptr, N=1, PH=4, PW=4):
-    L = _lib()
+    L = lib()
     dec = [torch.zeros(n) for n in (64 * 32, 64, 33 * 64, 33)]
     coords, sigma = torch.zeros(N * 8 * 3), torch.zeros(N * 8)
     return L.lib.n3d_sample_points(planes_ptr, N, PH, PW, coords.data_ptr(), 8, 1.0, *(t.data_ptr() for t in dec), sigma.data_ptr(), rgb_ptr,
@@ -714,18 +649,18 @@ def test_sample_points_refuses_misaligned_buffers(field):
     planes = torch.zeros(3 * 4 * 4 * 32 + 64)
     rgb = torch.zeros(8 * 32 + 64)
     if field == 'planes':
-        rc = _sample_points(_offset(planes, 16).data_ptr(), rgb.data_ptr())
-        _refused(rc, 'n3d_sample_points: planes must be 32-byte aligned')
+        rc = _sample_points(offset_view(planes, 16).data_ptr(), rgb.data_ptr())
+        refused(rc, 'n3d_sample_points: planes must be 32-byte aligned')
     else:
-        rc = _sample_points(planes.data_ptr(), _offset(rgb, 4).data_ptr())
-        _refused(rc, 'n3d_sample_points: rgb must be 8-byte aligned')
+        rc = _sample_points(planes.data_ptr(), offset_view(rgb, 4).data_ptr())
+        refused(rc, 'n3d_sample_points: rgb must be 8-byte aligned')
 
 
 def test_sample_grid_refuses_misaligned_planes():
-    L = _lib()
+    L = lib()
     planes = torch.zeros(3 * 4 * 4 * 32 + 64)
     dec = [torch.zeros(n) for n in (64 * 32, 64, 33 * 64, 33)]
     grid = torch.zeros(8 ** 3)
-    rc = L.lib.n3d_sample_grid(_offset(planes, 16).data_ptr(), 4, 4, 8, C.c_float(1.0), C.c_float(1.0), 0, 8 ** 3, 0, C.c_float(-1000.0),
+    rc = L.lib.n3d_sample_grid(offset_view(planes, 16).data_ptr(), 4, 4, 8, C.c_float(1.0), C.c_float(1.0), 0, 8 ** 3, 0, C.c_float(-1000.0),
                                *(t.data_ptr() for t in dec), grid.data_ptr(), None)
-    _refused(rc, 'n3d_sample_grid: planes must be 32-byte aligned')
+    refused(rc, 'n3d_sample_grid: planes must be 32-byte aligned')
