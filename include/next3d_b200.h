@@ -53,7 +53,8 @@ int n3d_bias_act(const void* x, const void* b, void* y, int dtype, int64_t numel
  *   grad 2: dx = dy * act''(xref + b) * gain * dyref (act 4-9 only: the activations with a second derivative).
  * Elements whose saved output lies on or outside +-clamp (clamp >= 0) get 0; swish recomputes that output from xref + b.
  * dy, xref, yref, dyref and dx share x's dense layout; b is applied to xref only.  xref is required for act 9, yref for act 2-8
- * (a NULL yref counts as 0, as in the plugin, so `linear` with a clamp passes every element), dyref for grad 2. */
+ * (a NULL yref counts as 0, as in the plugin, so `linear` with a clamp passes every element), dyref for grad 2.  numel 0 launches
+ * nothing and accepts NULL pointers (an empty tensor's data pointer). */
 int n3d_bias_act_grad(const void* dy, const void* b, const void* xref, const void* yref, const void* dyref, void* dx, int dtype,
                       int64_t numel, int size_b, int step_b, int grad, int act, float alpha, float gain, float clamp, void* stream);
 

@@ -139,15 +139,16 @@ __global__ void __launch_bounds__(256) bias_act_grad_kernel(const T* __restrict_
 extern "C" int n3d_bias_act_grad(const void* dy, const void* b, const void* xref, const void* yref, const void* dyref, void* dx, int dtype,
                                  int64_t numel, int size_b, int step_b, int grad, int act, float alpha, float gain, float clamp,
                                  void* stream) {
-    N3D_CHECK_ARG(dy && dx && numel >= 0, "n3d_bias_act_grad: null pointer");
+    N3D_CHECK_ARG(numel >= 0, "n3d_bias_act_grad: negative numel");
     N3D_CHECK_ARG(act >= 1 && act <= 9, "n3d_bias_act_grad: act %d out of range", act);
     N3D_CHECK_ARG(grad == 1 || (grad == 2 && act >= 4), "n3d_bias_act_grad: grad mode %d is not defined for act %d", grad, act);
     N3D_CHECK_ARG(dtype == N3D_DTYPE_F32 || dtype == N3D_DTYPE_F16, "n3d_bias_act_grad: unsupported dtype %d", dtype);
+    if (numel == 0) return N3D_OK;                 // nothing to launch; an empty tensor's data pointer may be NULL
+    N3D_CHECK_ARG(dy && dx, "n3d_bias_act_grad: null pointer");
     N3D_CHECK_ARG(!b || (size_b > 0 && step_b > 0), "n3d_bias_act_grad: bad bias geometry");
     N3D_CHECK_ARG(act != 9 || xref, "n3d_bias_act_grad: null xref (swish differentiates from its input)");
     N3D_CHECK_ARG(act == 1 || act == 9 || yref, "n3d_bias_act_grad: null yref (act %d differentiates from its output)", act);
     N3D_CHECK_ARG(grad == 1 || dyref, "n3d_bias_act_grad: null dyref (grad mode 2)");
-    if (numel == 0) return N3D_OK;
     const int grid = n3d_grid(numel, 256);
     if (dtype == N3D_DTYPE_F32)
         bias_act_grad_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)dy, (const float*)b, (const float*)xref,

@@ -48,8 +48,9 @@ def _one_group(x, w, f, up, down, flip_weight):
     w_hi, w_lo = K.pack_conv_weight(w)
     xn = x.permute(0, 2, 3, 1).contiguous()
     if down == 2 and k == 3:
+        if H % 2 or W % 2:
+            raise RuntimeError(f'conv2d_resample: down=2 with a 3x3 kernel needs an even input size, got {H}x{W}')
         sh, sw = (H + 2) // 2, (W + 2) // 2
-        assert H % 2 == 0 and W % 2 == 0
         a_hi = torch.empty(4 * N, sh, sw, Cin, dtype=torch.bfloat16, device=dev)
         a_lo = torch.empty_like(a_hi)
         K.fir_down_split(xn, a_hi, a_lo)

@@ -74,7 +74,7 @@ def report_parity(name, a, ref):
 # ------------------------------------------------------------------------------------------------ kernel conformance suites
 GUARD = 64                  # sentinel elements on each side of an output view: keeps the view's base alignment that of a fresh allocation
 SENTINEL = {torch.float32: (torch.int32, 0x7FC01234), torch.int32: (torch.int32, 0x7FC01234),      # NaN bit patterns no store produces
-            torch.bfloat16: (torch.int16, 0x7FC1)}
+            torch.bfloat16: (torch.int16, 0x7FC1), torch.float16: (torch.int16, 0x7E01)}
 
 
 class Guarded:

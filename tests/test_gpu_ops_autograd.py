@@ -1,4 +1,5 @@
-"""GPU: gradients of the torch_utils.ops mirror (bias_act, upfirdn2d, conv2d_resample) and the n3d_conv_wgrad kernel.
+"""GPU: gradients of the torch_utils.ops mirror (bias_act, upfirdn2d, conv2d_resample) end to end.  The gradient kernels at their
+ABI are tested over every launch configuration by tests/test_gpu_grad_conformance.py.
 
 Truth is oracle.ops under torch.autograd in fp64, on the same inputs rounded as the kernels see them.  Bounds are range-relative
 (tests.helpers.range_rel_err) and at most 4x the worst error measured on an H100 80GB HBM3 at a 400 W power limit.  Set
@@ -260,89 +261,6 @@ def test_conv2d_resample_grad_large(ops, c, monkeypatch):
         monkeypatch.setenv('N3D_FIR_STREAM', '0')
         for a, b in zip((y, dx, dw), run()):
             assert torch.equal(a, b), case
-
-
-# ------------------------------------------------------------------------------------------------ n3d_conv_wgrad at the ABI
-def _shifted(t, off, cols, K):
-    """t [rows, ld] -> [rows, K]: column k holds t[:, k + off] for 0 <= k + off < cols, else 0."""
-    out = torch.zeros(t.shape[0], K, dtype=t.dtype, device=t.device)
-    lo, hi = max(0, -off), min(K, cols - off)
-    if hi > lo:
-        out[:, lo:hi] = t[:, lo + off:hi + off]
-    return out
-
-
-@pytest.mark.parametrize('G,M,N,T,K,a_cols,b_cols,splits', [
-    (1, 130, 136, 3, 640, 700, 640, 1),          # M and N tile tails, offsets past both ends
-    (1, 130, 136, 3, 640, 700, 640, 10),         # every slice one K step
-    (5, 3, 8, 9, 1024, 1100, 1024, 4),           # Cout = 3, narrow N, 9 taps
-    (40, 24, 32, 2, 128, 128, 200, 2),           # many groups
-    (3, 64, 64, 1, 256, 256, 256, 1),            # 1x1
-    (1, 16, 16, 1, 512 * 512, 512 * 512, 512 * 512, 32),   # K = 512^2 positions
-])
-def test_conv_wgrad_abi(G, M, N, T, K, a_cols, b_cols, splits):
-    from next3d_b200 import kernels as KK
-    gen = _g(18)
-    lda, ldb = -(-a_cols // 8) * 8 + 8, -(-b_cols // 8) * 8
-    A = torch.randn(G * M + 5, lda, generator=gen)
-    B = torch.randn(G * N + 3 * 8, ldb, generator=gen)
-    a_hi, a_lo = KK.split_bf16(A)
-    b_hi, b_lo = KK.split_bf16(B)
-    offs = [(-8, 24, 0, 8), (40, -64, 5, 0), (0, 96, 2, 16), (8, 16, 0, 24), (-128, 0, 1, 0), (64, 8, 3, 8), (16, -8, 0, 0), (-16, -16, 4, 16),
-            (72, 8, 1, 24)][:T]
-    a_off, b_off, a_row, b_row = ([o[i] for o in offs] for i in range(4))
-    sentinel = torch.full((G * T * M * N + 64,), float('nan'), device='cuda')
-    dw = sentinel[32:32 + G * T * M * N].view(G, T, M, N)
-    partial = torch.full((splits, G, T, M, N), float('nan'), device='cuda') if splits > 1 else None
-    KK.conv_wgrad(a_hi.cuda(), a_lo.cuda(), b_hi.cuda(), b_lo.cuda(), G, M, N, K, a_off, b_off, dw, splits=splits, partial=partial,
-                  a_cols=a_cols, b_cols=b_cols, a_row=a_row, b_row=b_row)
-    torch.cuda.synchronize()
-    assert sentinel[:32].isnan().all() and sentinel[-32:].isnan().all()       # nothing written outside dw
-    assert not dw.isnan().any()                                                # every element of dw written
-    ah, al, bh, bl = (t.cuda().double() for t in (a_hi, a_lo, b_hi, b_lo))
-    for g in range(G):
-        for t in range(T):
-            ra, rb = a_row[t] + g * M, b_row[t] + g * N
-            sa = [_shifted(u[ra:ra + M], a_off[t], a_cols, K) for u in (ah, al)]
-            sb = [_shifted(u[rb:rb + N], b_off[t], b_cols, K) for u in (bh, bl)]
-            ref = sa[0] @ sb[0].T + sa[0] @ sb[1].T + sa[1] @ sb[0].T
-            # exact bf16 products; the bound is the fp32 accumulation over K (2^18 positions: 8192 per slice, then 32 slices)
-            _check(f'wgrad/{G}/{M}/{N}/{T}/{K}/{splits}/g{g}t{t}', 'dw', dw[g, t].double(), ref, 1e-5 if K < 10000 else 1.2e-4)
-            if G > 4 and g > 1:
-                break
-    # the same launch again gives the same bits
-    dw2 = torch.empty_like(dw)
-    KK.conv_wgrad(a_hi.cuda(), a_lo.cuda(), b_hi.cuda(), b_lo.cuda(), G, M, N, K, a_off, b_off, dw2, splits=splits, partial=partial,
-                  a_cols=a_cols, b_cols=b_cols, a_row=a_row, b_row=b_row)
-    assert torch.equal(dw, dw2)
-
-
-def test_wgrad_operand_layout():
-    from next3d_b200 import kernels as KK
-    x = torch.randn(2, 5, 7, 6, generator=_g(19)).cuda()[:, :, :, :]
-    xc = x.contiguous(memory_format=torch.channels_last)
-    for s, pad, PH, PW, shift in [(1, 1, 9, 8, -1), (2, 0, 4, 4, 1), (1, 0, 7, 6, 0)]:
-        ld = -(-(s * s * 2 * PH * PW) // 8) * 8 + 8
-        for src in (x, xc):
-            hi = torch.full((5, ld), float('nan'), dtype=torch.bfloat16, device='cuda')
-            lo = hi.clone()
-            KK.wgrad_operand(src, s, pad, pad, PH, PW, ld, hi, lo, shift=shift)
-            ref = torch.zeros(5, ld, dtype=torch.float64)
-            xd = x.double().cpu()
-            for par in range(s * s):
-                for n in range(2):
-                    for py in range(PH):
-                        iy = s * (py - pad) + par // s
-                        if not 0 <= iy < 7:
-                            continue
-                        for px in range(PW):
-                            ix = s * (px - pad) + par % s
-                            j = ((par * 2 + n) * PH + py) * PW + px - shift
-                            if 0 <= ix < 6 and 0 <= j < ld:
-                                ref[:, j] = xd[n, :, iy, ix]
-            got = hi.double().cpu() + lo.double().cpu()
-            assert not got.isnan().any()
-            assert (got - ref).abs().max().item() <= 2 ** -16 * ref.abs().max().item()
 
 
 # ------------------------------------------------------------------------------------------------ end to end
