@@ -261,6 +261,12 @@ int n3d_rasterize(const float* verts, const int32_t* faces, int NM, int V, int F
 int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, const float* face_uv, const float* texture,
                   const float* eye_mask, int N, int H, int W, int TH, int TW, int C, int MH, int MW,
                   float* tex_planes, float* alpha, void* stream);
+/* n3d_uv_sample for several images per texture: image n (of N) reads texture[n / views], so texture is [N / views,TH,TW,C];
+ * every other argument and output is per image, as above.  views = 1 is n3d_uv_sample.  views < 1 or N not a multiple of
+ * views -> N3D_ERR_INVALID_ARG before any launch. */
+int n3d_uv_sample_views(const int32_t* pix_to_face, const float* bary, const float* face_uv, const float* texture,
+                        const float* eye_mask, int N, int views, int H, int W, int TH, int TW, int C, int MH, int MW,
+                        float* tex_planes, float* alpha, void* stream);
 
 /* fill_mouth (renderer.py:583-602): alpha [NI,H,W] in place; cv2.floodFill from (0,0) with fixed range [seed, seed+254]
  * on alpha*255, then alpha += 1 - (filled/127.5 - 1), clipped to [0,1].  H*(W+4) <= 200 KB (512x396 at most).
@@ -287,6 +293,11 @@ int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t*
  * Alignment: blended_front, tex_planes, static_planes and planes 16-byte aligned (float4 loads / stores), else N3D_ERR_INVALID_ARG. */
 int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
                      int N, int H, int W, float* planes, void* stream);
+/* n3d_blend_planes for several images per static plane set: image n (of N) reads static_planes[n / views], so static_planes is
+ * NHWC [N / views,H,W,96]; every other argument and output is per image.  views = 1 is n3d_blend_planes.  views < 1 or N not a
+ * multiple of views -> N3D_ERR_INVALID_ARG before any launch. */
+int n3d_blend_planes_views(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
+                           int N, int views, int H, int W, float* planes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Volume renderer: ray generation + stratified sampling + tri-plane fetch + MLP decode + importance resampling +

@@ -97,11 +97,13 @@ _SIGNATURES = {
     'n3d_transform_points': ([P, C.c_int, C.c_int, P, C.c_int, F32, C.c_int, P, P], C.c_int),
     'n3d_rasterize': ([P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, P, P, P], C.c_int),
     'n3d_uv_sample': ([P, P, P, P, P] + [C.c_int] * 8 + [P, P, P], C.c_int),
+    'n3d_uv_sample_views': ([P, P, P, P, P] + [C.c_int] * 9 + [P, P, P], C.c_int),
     'n3d_fill_mouth': ([P, C.c_int, C.c_int, C.c_int, P], C.c_int),
     'n3d_fill_mouth_binarize': ([P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P], C.c_int),
     'n3d_mouth_box': ([P, C.c_int, P, P], C.c_int),
     'n3d_resize_aa': ([P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P, P, P], C.c_int),
     'n3d_blend_planes': ([P, P, P, P, C.c_int, C.c_int, C.c_int, P, P], C.c_int),
+    'n3d_blend_planes_views': ([P, P, P, P, C.c_int, C.c_int, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_render_rays': ([C.POINTER(Render), P], C.c_int),
     'n3d_render_rays_normals': ([C.POINTER(Render), P, P, P], C.c_int),
     'n3d_render_normals_pass': ([C.POINTER(Render), P, P, P], C.c_int),

@@ -164,10 +164,10 @@ __device__ __forceinline__ void bilinear_setup(float gx, float gy, int W, int H,
 // One warp per output pixel, lanes = channels for the texture loads.  The per-tap arithmetic (face lookup, barycentric UV,
 // bilinear corner offset + weight) is done ONCE: lane l < 16 owns texture tap (view l/4, corner l%4), lane 16 + l owns the
 // corresponding eye-mask tap; offsets / weights are then broadcast with shuffles and the 16 texture loads (one coalesced
-// 128-byte line each) are issued together.
+// 128-byte line each) are issued together.  Image n reads texture n / views.
 __global__ void __launch_bounds__(256) uv_sample_kernel(const int* __restrict__ p2f, const float* __restrict__ bary, const float* __restrict__ face_uv,
-                                                        const float* __restrict__ tex, const float* __restrict__ mask, int N, int H, int W, int TH,
-                                                        int TW, int C, int MH, int MW, float* __restrict__ planes, float* __restrict__ alpha) {
+                                                        const float* __restrict__ tex, const float* __restrict__ mask, int N, int views, int H, int W,
+                                                        int TH, int TW, int C, int MH, int MW, float* __restrict__ planes, float* __restrict__ alpha) {
     const int lane = threadIdx.x & 31;
     const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__(256) uv_sample_kernel(const int* __restrict__ 
             alpha[((int64_t)aplane * N + n) * HW + pix] = m * (f >= 0 ? 1.f : 0.f);
         }
         // ---- texture: 16 taps broadcast from lanes 0..15
-        const float* tb = tex + (int64_t)n * TH * TW * C;
+        const float* tb = tex + (int64_t)(n / views) * TH * TW * C;
         float val[16], wgt[16];
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
@@ -476,9 +476,9 @@ __global__ void __launch_bounds__(256) resize_aa_scalar_kernel(const float* __re
 }
 
 // ---------------------------------------------------------------------------------------------- plane blend
-// planes[n,p,y,x,c] = tex[n,p,y,x,c]*a + static[n,y,x,p*32+c]*(1-a); plane 0's texture comes from the neural-blending output
+// planes[n,p,y,x,c] = tex[n,p,y,x,c]*a + static[n/views,y,x,p*32+c]*(1-a); plane 0's texture comes from the neural-blending output
 __global__ void __launch_bounds__(256) blend_kernel(const float* __restrict__ front, const float* __restrict__ tex, const float* __restrict__ alpha,
-                                                    const float* __restrict__ stat, int N, int HW, float* __restrict__ planes) {
+                                                    const float* __restrict__ stat, int N, int views, int HW, float* __restrict__ planes) {
     const int64_t total = (int64_t)N * 3 * HW * 8;     // float4 groups of the 32 channels
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c4 = (int)(i & 7);
@@ -489,7 +489,7 @@ __global__ void __launch_bounds__(256) blend_kernel(const float* __restrict__ fr
         const float a = __ldg(alpha + ((int64_t)p * N + n) * HW + pix);
         const float4 tv = p == 0 ? __ldg(reinterpret_cast<const float4*>(front + ((int64_t)n * HW + pix) * 32) + c4)
                                  : __ldg(reinterpret_cast<const float4*>(tex + (((int64_t)p * N + n) * HW + pix) * 32) + c4);
-        const float4 sv = __ldg(reinterpret_cast<const float4*>(stat + ((int64_t)n * HW + pix) * 96 + p * 32) + c4);
+        const float4 sv = __ldg(reinterpret_cast<const float4*>(stat + ((int64_t)(n / views) * HW + pix) * 96 + p * 32) + c4);
         const float b = 1.f - a;
         float4 o;
         o.x = tv.x * a + sv.x * b; o.y = tv.y * a + sv.y * b; o.z = tv.z * a + sv.z * b; o.w = tv.w * a + sv.w * b;
@@ -518,15 +518,22 @@ extern "C" int n3d_rasterize(const float* verts, const int32_t* faces, int NM, i
     return N3D_OK;
 }
 
+extern "C" int n3d_uv_sample_views(const int32_t* pix_to_face, const float* bary, const float* face_uv, const float* texture,
+                                   const float* eye_mask, int N, int views, int H, int W, int TH, int TW, int C, int MH, int MW,
+                                   float* tex_planes, float* alpha, void* stream) {
+    N3D_CHECK_ARG(pix_to_face && bary && face_uv && texture && eye_mask && tex_planes && alpha, "n3d_uv_sample: null pointer");
+    N3D_CHECK_ARG(C <= 32, "n3d_uv_sample: C %d > 32 not supported", C);
+    N3D_CHECK_ARG(views >= 1 && N % views == 0, "n3d_uv_sample: %d images are not a multiple of views %d", N, views);
+    uv_sample_kernel<<<n3d_grid((int64_t)N * H * W * 32, 256, 16), 256, 0, (cudaStream_t)stream>>>(pix_to_face, bary, face_uv, texture, eye_mask, N,
+                                                                                                views, H, W, TH, TW, C, MH, MW, tex_planes, alpha);
+    N3D_CHECK_LAUNCH("n3d_uv_sample");
+    return N3D_OK;
+}
+
 extern "C" int n3d_uv_sample(const int32_t* pix_to_face, const float* bary, const float* face_uv, const float* texture,
                              const float* eye_mask, int N, int H, int W, int TH, int TW, int C, int MH, int MW,
                              float* tex_planes, float* alpha, void* stream) {
-    N3D_CHECK_ARG(pix_to_face && bary && face_uv && texture && eye_mask && tex_planes && alpha, "n3d_uv_sample: null pointer");
-    N3D_CHECK_ARG(C <= 32, "n3d_uv_sample: C %d > 32 not supported", C);
-    uv_sample_kernel<<<n3d_grid((int64_t)N * H * W * 32, 256, 16), 256, 0, (cudaStream_t)stream>>>(pix_to_face, bary, face_uv, texture, eye_mask, N, H,
-                                                                                                W, TH, TW, C, MH, MW, tex_planes, alpha);
-    N3D_CHECK_LAUNCH("n3d_uv_sample");
-    return N3D_OK;
+    return n3d_uv_sample_views(pix_to_face, bary, face_uv, texture, eye_mask, N, 1, H, W, TH, TW, C, MH, MW, tex_planes, alpha, stream);
 }
 
 extern "C" int n3d_fill_mouth_binarize(float* alpha, int NI, int H, int W, int bin0, int bin1, void* stream) {
@@ -566,12 +573,19 @@ extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, con
     return N3D_OK;
 }
 
-extern "C" int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
-                                int N, int H, int W, float* planes, void* stream) {
+extern "C" int n3d_blend_planes_views(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
+                                      int N, int views, int H, int W, float* planes, void* stream) {
     N3D_CHECK_ARG(blended_front && tex_planes && alpha && static_planes && planes, "n3d_blend_planes: null pointer");
     N3D_CHECK_ARG((((uintptr_t)blended_front | (uintptr_t)tex_planes | (uintptr_t)static_planes | (uintptr_t)planes) & 15) == 0,
                   "n3d_blend_planes: blended_front, tex_planes, static_planes and planes must be 16-byte aligned");     // float4 loads / stores
-    blend_kernel<<<n3d_grid((int64_t)N * 3 * H * W * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(blended_front, tex_planes, alpha, static_planes, N, H * W, planes);
+    N3D_CHECK_ARG(views >= 1 && N % views == 0, "n3d_blend_planes: %d images are not a multiple of views %d", N, views);
+    blend_kernel<<<n3d_grid((int64_t)N * 3 * H * W * 8, 256, 16), 256, 0, (cudaStream_t)stream>>>(blended_front, tex_planes, alpha, static_planes, N,
+                                                                                               views, H * W, planes);
     N3D_CHECK_LAUNCH("n3d_blend_planes");
     return N3D_OK;
+}
+
+extern "C" int n3d_blend_planes(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,
+                                int N, int H, int W, float* planes, void* stream) {
+    return n3d_blend_planes_views(blended_front, tex_planes, alpha, static_planes, N, 1, H, W, planes, stream);
 }

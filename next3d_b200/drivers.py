@@ -135,9 +135,23 @@ def _frames_u8(out, image_mode):
     return to_uint8_hwc(img)
 
 
+def layout_cells(cells, gw, gh):
+    """uint8 cells [F * gh * gw, h, w, C] (the cells of each frame in row-major grid order, frame after frame) -> frames
+    [F, gh * h, gw * w, C]: layout_grid of gen_videos_next3d.py:35-49 per frame, on whatever device the cells are (the uint8
+    conversion is per pixel, so converting the cells first and laying them out after gives the script's frames)."""
+    n, h, w, C = cells.shape
+    return cells.reshape(n // (gh * gw), gh, gw, h, w, C).permute(0, 1, 3, 2, 4, 5).reshape(-1, gh * h, gw * w, C)
+
+
 def _frames(outputs, image_mode, device):
     """uint8 HWC numpy frames of successive batches, in order; `outputs` yields (generator output dict, valid count) per batch.  The
     conversion runs on the device, and the device->host copy of batch i overlaps the rendering of batch i+1."""
+    yield from _to_host(((_frames_u8(out, image_mode), n) for out, n in outputs), device)
+
+
+def _to_host(batches, device):
+    """uint8 numpy frames of successive batches of device frames (uint8 tensor [>= n, H, W, C], valid count n), in order; the
+    device->host copy of batch i overlaps the work that produces batch i+1.  Each tensor must be fresh (not reused by its producer)."""
     cuda = torch.device(device).type == 'cuda'
     copy_s = torch.cuda.Stream(device) if cuda else None
     pending = None                                               # (host tensor, event, valid count) of the previous batch
@@ -149,8 +163,7 @@ def _frames(outputs, image_mode, device):
         for k in range(n):
             yield host[k].numpy()
 
-    for out, n in outputs:
-        u8 = _frames_u8(out, image_mode)                         # fresh tensor: the generator's static output buffer is free again
+    for u8, n in batches:
         if cuda:
             host = torch.empty(u8.shape, dtype=torch.uint8).pin_memory()
             copy_s.wait_stream(torch.cuda.current_stream(device))
@@ -173,7 +186,7 @@ def reenact_schedule(drive_root, num_frames, lms_cond=True):
     """Frame schedule of reenact_avatar_next3d.py:125-160 for a driving directory (dataset.json + NNN.png / NNN.obj / NNN_kpt2d.txt):
     the script walks the sorted PNG list, skips k = 0, stops after k = num_frames and smooths the camera over the labels k-1, k, k+1
     (so the last usable frame is len(labels) - 2; the script itself runs into an IndexError there).
-    -> dict(ks, ids, obj_paths, lms_paths (or None), cams float32 [F, 25])."""
+    -> dict(ks, ids, png_paths, obj_paths, lms_paths (or None), cams float32 [F, 25])."""
     import glob
     import os
     from . import inputs
@@ -181,7 +194,7 @@ def reenact_schedule(drive_root, num_frames, lms_cond=True):
     img_list = sorted(glob.glob(drive_root + '/*.png'))
     ks = [k for k in range(len(img_list)) if 1 <= k <= num_frames and k + 1 < len(labels)]
     ids = [os.path.basename(img_list[k]).split('.')[0] for k in ks]
-    return dict(ks=ks, ids=ids, obj_paths=[drive_root + f'/{i}.obj' for i in ids],
+    return dict(ks=ks, ids=ids, png_paths=[img_list[k] for k in ks], obj_paths=[drive_root + f'/{i}.obj' for i in ids],
                 lms_paths=[drive_root + f'/{i}_kpt2d.txt' for i in ids] if lms_cond else None,
                 cams=inputs.smoothed_cameras(labels, ks))
 
@@ -201,11 +214,14 @@ def reenact_frames(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_
                               noise_mode in ('const', 'none'))
 
 
-def _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers):
+def _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=False):
     """(frame count n, cameras [n, 25], frames(a, b) -> in-order iterable of the [1, V, 3] meshes of frames a .. b-1) of a driving
-    directory (reenact_schedule; only the requested frames are parsed, on worker threads) or of a `.n3dpack` (memory-mapped)."""
+    directory (reenact_schedule; only the requested frames are parsed, on worker threads) or of a `.n3dpack` (memory-mapped).
+    photos=True: frames(a, b) yields (mesh, uint8 photo [512, 512, 3]) pairs (a directory only: a pack carries no photos)."""
     from . import inputs
     if str(drive_root).endswith('.n3dpack'):
+        if photos:
+            raise ValueError(f'{drive_root}: a .n3dpack carries no driving photos; pass the driving directory')
         pack = inputs.FramePack(drive_root)
         n = min(len(pack), num_frames)
         cams = torch.from_numpy(np.array(pack.cams[:n]))
@@ -219,7 +235,8 @@ def _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_dep
         pairs = list(zip(sch['obj_paths'], sch['lms_paths'] if lms_cond else [None] * n))
 
         def frames(a, b):
-            return inputs.FramePrefetcher(pairs[a:b], depth=prefetch_depth, workers=workers)
+            return inputs.FramePrefetcher(pairs[a:b], depth=prefetch_depth, workers=workers,
+                                          photos=sch['png_paths'][a:b] if photos else None)
     if fixed_camera is not None:
         cams = fixed_camera.reshape(1, 25).cpu().float().expand(n, -1)
     return n, cams, frames
@@ -237,6 +254,211 @@ def interpolate_ws_device(ws_keyframes, w_frames, wraps=2, kind='cubic'):
     B = scipy.interpolate.interp1d(x, eye, kind=kind, axis=0)(np.arange(Kf * w_frames) / w_frames)
     B = torch.from_numpy(B).to(ws_keyframes.device, torch.float32).contiguous()
     return K.interp_rows(B, ws_keyframes.to(torch.float32).contiguous())
+
+
+# ------------------------------------------------------------------------------------------------ grids (--grid of both scripts)
+def _grid_seeds(seeds, grid, num_keyframes, shuffle_seed):
+    """(seed of every keyframe of every cell [K * gh * gw] int64, K): gen_videos_next3d.py:78-92."""
+    gw, gh = grid
+    if num_keyframes is None:
+        if len(seeds) % (gw * gh) != 0:
+            raise ValueError('Number of input seeds must be divisible by grid W*H')
+        num_keyframes = len(seeds) // (gw * gh)
+    all_seeds = np.zeros(num_keyframes * gh * gw, dtype=np.int64)
+    for idx in range(num_keyframes * gh * gw):
+        all_seeds[idx] = seeds[idx % len(seeds)]
+    if shuffle_seed is not None:
+        np.random.RandomState(seed=shuffle_seed).shuffle(all_seeds)
+    return all_seeds, num_keyframes
+
+
+def _frontal_camera(G, n):
+    """c [n, 25]: the frontal conditioning camera of gen_videos_next3d.py:96-100 (avg_camera_pivot / avg_camera_radius, focal 4.2647)."""
+    rk = G.rendering_kwargs
+    pose = camera.look_at_pose(3.14 / 2, 3.14 / 2, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
+    intr = torch.tensor([[FOCAL_FFHQ, 0, 0.5], [0, FOCAL_FFHQ, 0.5], [0, 0, 1]], dtype=torch.float32)
+    return torch.cat([pose.reshape(-1, 16), intr.reshape(-1, 9)], 1).repeat(n, 1)
+
+
+def grid_keyframes(G, seeds, grid, num_keyframes=None, shuffle_seed=None, truncation_psi=1, truncation_cutoff=14):
+    """The keyframe latents of an interpolation grid video (gen_videos_next3d.py:78-106, `--grid=WxH`): grid = (gw, gh); seeds repeat
+    as seeds[idx % len(seeds)] over K * gh * gw keyframes (K = num_keyframes, else len(seeds) / (gw * gh), which must divide: ValueError
+    otherwise), optionally shuffled by RandomState(shuffle_seed); z = RandomState(seed).randn(z_dim), mapped with the frontal camera.
+    -> ws [gh, gw, K, L, D] on the generator's device."""
+    gw, gh = grid
+    all_seeds, K = _grid_seeds(seeds, grid, num_keyframes, shuffle_seed)
+    device = next(G.parameters()).device
+    zs = torch.from_numpy(np.stack([np.random.RandomState(seed).randn(G.z_dim) for seed in all_seeds])).to(device)
+    ws = G.mapping(z=zs, c=_frontal_camera(G, len(zs)).to(device), truncation_psi=truncation_psi, truncation_cutoff=truncation_cutoff)
+    return ws.reshape(gh, gw, K, *ws.shape[1:])
+
+
+def _whole_frames(cell_batches, gw, gh):
+    """(uint8 frames [nf, gh * h, gw * w, 3], nf) from successive batches (uint8 cells [>= n, h, w, 3], valid count n) of a cell
+    sequence ordered frame-major, cell-minor: a frame is laid out as soon as its last cell has been rendered."""
+    per, rest = gw * gh, None
+    for u8, n in cell_batches:
+        cur = u8[:n] if rest is None else torch.cat([rest, u8[:n]])
+        nf = cur.shape[0] // per
+        rest = cur[nf * per:]
+        if nf:
+            yield layout_cells(cur[:nf * per], gw, gh), nf
+
+
+def _grid_schedule(G, ws_grid, w_frames, device):
+    """(latents [F * cells, L, D] on the device, cameras [F * cells, 25]) of a grid video, image f * cells + cell: every cell
+    interpolates its own keyframes (interpolate_ws_device: cubic, 2 wraps), every cell of frame f has the frame's orbit camera
+    (gen_videos_next3d.py:128-144)."""
+    gh, gw, K = ws_grid.shape[:3]
+    F = K * w_frames
+    wsf = torch.stack([interpolate_ws_device(ws_grid[yi, xi].to(device), w_frames) for yi in range(gh) for xi in range(gw)], 1)
+    rk = G.rendering_kwargs
+    cams = orbit_camera_params(F, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
+    return wsf.reshape(F * gh * gw, *wsf.shape[2:]), cams.repeat_interleave(gh * gw, 0)
+
+
+def render_grid_frames(G, ws_grid, verts, w_frames, batch=8, image_mode='image', seed=None, sampler_noise=None):
+    """gen_videos_next3d.py:77-171 with `--grid=WxH`: yield one uint8 HWC numpy frame [gh * R, gw * R, 3] per frame of the video
+    (F = K * w_frames frames for ws_grid [gh, gw, K, L, D] from grid_keyframes), laid out like the script's layout_grid.  Cell
+    (yi, xi) interpolates its own keyframes; all cells of a frame share its orbit camera and the static mesh verts [1, V, 3]
+    (noise_mode 'const').  The F * gh * gw images run frame-major, cell-minor through `synthesis` in batches of `batch` (the last
+    one padded as in render_frames), so a batch may hold parts of two frames.  'image_depth' cells are normalised and clamped per
+    cell, as the script's one image per call; the frames stay 3-channel (the script writes 1-channel depth frames).  `seed` as in
+    render_frames; `sampler_noise=(u_coarse [F * cells, M, Dc, 1], u_fine [F * cells, M, Df])` rows are indexed by the global
+    image id f * gh * gw + yi * gw + xi."""
+    device = next(G.parameters()).device
+    gh, gw = ws_grid.shape[:2]
+    wsf, cams = _grid_schedule(G, ws_grid, w_frames, device)
+    v = verts.to(device, torch.float32).reshape(1, *verts.shape[-2:]).expand(batch, -1, -1)
+
+    def cells():
+        for idx, n, kw in _batches(wsf.shape[0], batch, seed, sampler_noise):
+            out = G.synthesis(wsf[idx], cams[idx].to(device, torch.float32, non_blocking=True), v, noise_mode='const',
+                              **_depth_kw(image_mode, device), **kw)
+            yield _frames_u8(out, image_mode), n
+    yield from _to_host(_whole_frames(cells(), gw, gh), device)
+
+
+def photo_cell(photo, device):
+    """uint8 driving photo [H, W, 3] -> its uint8 grid cell [H, W, 3] through the script's float32 arithmetic on `device`:
+    `/ 127.5 - 1` (reenact_avatar_next3d.py:134-135), then layout_grid's conversion."""
+    img = photo.to(device, non_blocking=True).permute(2, 0, 1).float().unsqueeze(0) / 127.5 - 1.
+    return to_uint8_hwc(img)[0]
+
+
+def _check_reenact_grid(G, S, grid):
+    gw, gh = grid
+    if gw * gh != S + 1:
+        raise ValueError(f'grid {gw}x{gh} has {gw * gh} cells, but the driving photo and {S} avatar(s) need {S + 1}')
+    if G.img_resolution != 512:
+        raise ValueError(f'a reenactment grid needs img_resolution 512 (the photo cell is a 512x512 crop), got {G.img_resolution}')
+
+
+def _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, cache, grid, device):
+    """uint8 frames [m, gh * 512, gw * 512, 3] of the m = len(items) frames of one batch: items are (mesh [1, V, 3], photo) pairs,
+    c [k, 25] their cameras padded to k >= m by repeating the last.  The batch holds S heads x k frames, head-major (image n is head
+    n // k).  noise_mode 'const' / 'none': the S heads' ws-only backbones come from the engine's cache (filled first when `cache`)."""
+    k, m = c.shape[0], len(items)
+    meshes = [t for t, _ in items]
+    v = torch.cat(meshes + [meshes[-1]] * (k - m), 0).to(device, torch.float32, non_blocking=True)
+    if noise_mode in ('const', 'none'):
+        if cache:
+            G.synthesis(wsd, c[:1].expand(S, -1), v[:1].expand(S, -1, -1), noise_mode=noise_mode, cache_backbone=True, seed=0)
+        kw = dict(kw, use_cached_backbone=True)
+    out = G.synthesis(wsb, c.repeat(S, 1), v.repeat(S, 1, 1), noise_mode=noise_mode, **kw)
+    av = _frames_u8(out, 'image')
+    av = av.reshape(S, k, *av.shape[1:])[:, :m].transpose(0, 1)                            # [m, S, H, W, 3]
+    photos = torch.stack([photo_cell(p, device) for _, p in items])[:, None]
+    cells = torch.cat([photos, av], 1)
+    return layout_cells(cells.reshape(-1, *cells.shape[2:]), *grid)
+
+
+def _reenact_grid_kw(seed_kw, sampler_noise, idx, S):
+    """Sampler keywords of a reenactment-grid batch of frames idx: rows f * S + s of sampler_noise, head-major like the batch."""
+    kw = dict(seed_kw)
+    if sampler_noise is not None:
+        kw['sampler_noise'] = _noise_rows(sampler_noise, [f * S + s for s in range(S) for f in idx])
+    return kw
+
+
+def reenact_grid_frames(G, ws, drive_root, num_frames, grid, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=None,
+                        sampler_noise=None, prefetch_depth=8, workers=4):
+    """reenact_avatar_next3d.py:116-167 with several seeds and `--grid=WxH`: one mesh drives S identities ws [S, L, D]; every frame is
+    the grid (gw, gh) = grid of the driving photo followed by the S avatars (gw * gh must be S + 1, else ValueError), yielded as a
+    uint8 HWC numpy frame [gh * 512, gw * 512, 3] equal to the script's layout_grid.  'image' output at img_resolution 512 only.
+    The photo is the PNG's 512x512 crop, decoded on the prefetcher's worker threads next to the mesh (a `.n3dpack` carries no photos:
+    ValueError).  Each synthesis call renders S heads x k frames (k = max(1, batch // S), the last batch padded), head-major; with
+    noise_mode 'const' / 'none' the S heads' ws-only backbones are computed once and every batch reuses them (use_cached_backbone),
+    with 'random' every batch runs the full path.  `seed`: batch b draws sampler seed seed + b; `sampler_noise=(u_coarse
+    [F * S, M, Dc, 1], u_fine [F * S, M, Df])` rows are indexed f * S + s (frame f, identity s)."""
+    S = ws.shape[0]
+    _check_reenact_grid(G, S, grid)
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=True)
+    if n == 0:
+        return
+    device = next(G.parameters()).device
+    k = max(1, batch // S)
+    wsd = ws.detach().to(device, torch.float32).reshape(S, *ws.shape[-2:])
+    wsb = wsd.repeat_interleave(k, 0)
+    it = iter(frames(0, n))
+
+    def batches():
+        for b0 in range(0, n, k):
+            m = min(k, n - b0)
+            items = [next(it) for _ in range(m)]
+            idx = list(range(b0, b0 + m)) + [b0 + m - 1] * (k - m)
+            kw = _reenact_grid_kw({} if seed is None else {'seed': int(seed) + b0 // k}, sampler_noise, idx, S)
+            c = cams[idx].to(device, torch.float32, non_blocking=True)
+            yield _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, b0 == 0, grid, device), m
+    yield from _to_host(batches(), device)
+
+
+def render_grid_frames_sharded(G, ws_grid, verts, w_frames, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None,
+                               device=None):
+    """render_grid_frames over the GPUs of a box (one process per GPU, as render_frames_sharded), sharded by frame: all cells of a
+    frame render on one rank, plan.batch frames (batch // cells as the bound, at least 1) of gh * gw cells per synthesis call.
+    -> [F, gh * R, gw * R, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the global image id
+    f * gh * gw + cell, so the frames do not depend on the number of ranks."""
+    device = device or next(G.parameters()).device
+    gh, gw = ws_grid.shape[:2]
+    cells = gh * gw
+    wsf, cams = _grid_schedule(G, ws_grid, w_frames, device)
+    plan = shard_plan(wsf.shape[0] // cells, max(1, batch // cells))
+    v = verts.to(device, torch.float32).reshape(1, *verts.shape[-2:]).expand(plan.batch * cells, -1, -1)
+
+    def step(k, idx):
+        ids = [f * cells + j for f in idx for j in range(cells)]
+        out_ = G.synthesis(wsf[ids], cams[ids].to(device, torch.float32, non_blocking=True), v, noise_mode='const',
+                           **_depth_kw(image_mode, device), **_shard_sampler(plan, k, ids, seed, sampler_noise))
+        return layout_cells(_frames_u8(out_, image_mode), gw, gh)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, step, gh * res, gw * res, device, out)
+
+
+def reenact_grid_frames_sharded(G, ws, drive_root, num_frames, grid, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const',
+                                seed=0, sampler_noise=None, out=None, device=None, prefetch_depth=8, workers=4):
+    """reenact_grid_frames over the GPUs of a box, sharded by frame as reenact_frames_sharded (each rank parses the meshes and decodes
+    the photos of its own frames only; plan.batch frames of S heads per call, batch // S as the bound).  -> [F, gh * 512, gw * 512, 3]
+    uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed f * S + s by the global frame id f."""
+    S = ws.shape[0]
+    _check_reenact_grid(G, S, grid)
+    device = device or next(G.parameters()).device
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=True)
+    plan = shard_plan(n, max(1, batch // S))
+    wsd = ws.detach().to(device, torch.float32).reshape(S, *ws.shape[-2:])
+    wsb = wsd.repeat_interleave(plan.batch, 0)
+    src = None
+    if n > 0:
+        first = plan.frames(0)[0]                                          # a rank without frames repeats the previous rank's last
+        src = _InOrder(frames(first, max(plan.spans[plan.rank][1], first + 1)), first)
+
+    def step(k, idx):
+        items = src.take(idx)
+        kw = _reenact_grid_kw(_shard_sampler(plan, k, idx, seed, None), sampler_noise, idx, S)
+        c = cams[idx].to(device, torch.float32, non_blocking=True)
+        return _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, k == 0, grid, device)
+    gw, gh = grid
+    return _gather_frames(plan, step, gh * 512, gw * 512, device, out)
 
 
 def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const', seed=0, device=None, out=None, sampler_noise=None):
@@ -259,7 +481,8 @@ def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const'
         c = cams[idx].to(device, torch.float32, non_blocking=True)
         v = verts.to(device, torch.float32).expand(plan.batch, -1, -1) if static_mesh else verts[idx].to(device, torch.float32, non_blocking=True)
         return G.synthesis(w, c, v, noise_mode=noise_mode, **_shard_sampler(plan, k, idx, seed, sampler_noise))
-    return _gather_frames(plan, step, 'image', G.img_resolution, device, out)
+    res = G.img_resolution
+    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), 'image'), res, res, device, out)
 
 
 def reenact_frames_sharded(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=0,
@@ -283,12 +506,13 @@ def reenact_frames_sharded(G, ws, drive_root, num_frames, batch=8, lms_cond=True
 
     def step(k, idx):
         c = cams[idx].to(device, torch.float32, non_blocking=True)
-        v = mesh.take(idx).to(device, torch.float32, non_blocking=True)
+        v = torch.cat(mesh.take(idx), 0).to(device, torch.float32, non_blocking=True)
         kw = _shard_sampler(plan, k, idx, seed, sampler_noise)
         if reuse:
             kw['use_cached_backbone' if k else 'cache_backbone'] = True
         return G.synthesis(wsd, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw)
-    return _gather_frames(plan, step, image_mode, _frame_resolution(G, image_mode), device, out)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), image_mode), res, res, device, out)
 
 
 def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None, device=None):
@@ -304,7 +528,8 @@ def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0
     def step(k, idx):
         return G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device),
                               **_shard_sampler(plan, k, idx, seed, sampler_noise))
-    return _gather_frames(plan, step, image_mode, _frame_resolution(G, image_mode), device, out)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), image_mode), res, res, device, out)
 
 
 class ShardPlan(NamedTuple):
@@ -348,8 +573,8 @@ def _frame_resolution(G, image_mode):
 
 
 class _InOrder:
-    """Meshes of consecutive frames first, first + 1, ... from an in-order iterable of [1, V, 3] tensors, looked up by frame id as the
-    sharded batches advance (each id is read once; ids behind the current batch are dropped)."""
+    """Items (meshes [1, V, 3], or (mesh, photo) pairs) of consecutive frames first, first + 1, ... from an in-order iterable, looked
+    up by frame id as the sharded batches advance (each id is read once; ids behind the current batch are dropped)."""
 
     def __init__(self, frames, first):
         self.it, self.next, self.have = iter(frames), first, {}
@@ -359,53 +584,67 @@ class _InOrder:
             self.have[self.next] = next(self.it)
             self.next += 1
         self.have = {i: t for i, t in self.have.items() if i >= min(idx)}
-        return torch.cat([self.have[i] for i in idx], 0)
+        return [self.have[i] for i in idx]
 
 
-def _gather_frames(plan, step, image_mode, res, device, out):
-    """The loop of the sharded drivers: for k in range(plan.steps), step(k, plan.frames(k)) renders this rank's batch k and returns the
-    generator's output dict; its uint8 frames go to a ping-pong staging buffer, are gathered to rank 0 over NCCL on a side stream
+def _gather_frames(plan, step, H, W, device, out):
+    """The loop of the sharded drivers: for k in range(plan.steps), step(k, plan.frames(k)) renders this rank's batch k and returns
+    its uint8 frames [plan.batch, H, W, 3]; they go to a ping-pong staging buffer, are gathered to rank 0 over NCCL on a side stream
     (world > 1) and copied to pinned host memory on a third stream, so the next batch renders while this one is in flight.
-    -> [F, res, res, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere.  It is filled in stream order: the caller's
-    current stream waits for the last copy, so synchronise that stream before reading the frames (back-to-back clips do not stall)."""
+    -> [F, H, W, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere.  It is filled in stream order: the caller's
+    current stream waits for the last copy, so synchronise that stream before reading the frames (back-to-back clips do not stall).
+    A CPU `device` (host-side tests under gloo) runs the same loop without streams."""
+    import contextlib
     import torch.distributed as dist
     rank, world, spans, batch = plan.rank, plan.world, plan.spans, plan.batch
+    cuda = torch.device(device).type == 'cuda'
     host = None
     if rank == 0:
-        host = out if out is not None else torch.empty(spans[-1][1], res, res, 3, dtype=torch.uint8).pin_memory()
-    main = torch.cuda.current_stream(device)
-    side, copy_s = torch.cuda.Stream(device), torch.cuda.Stream(device)
-    stage = [torch.empty(batch, res, res, 3, dtype=torch.uint8, device=device) for _ in range(2)]
-    gath = [torch.empty(world, batch, res, res, 3, dtype=torch.uint8, device=device) if rank == 0 and world > 1 else None for _ in range(2)]
+        host = out if out is not None else torch.empty(spans[-1][1], H, W, 3, dtype=torch.uint8, pin_memory=cuda)
+    main = torch.cuda.current_stream(device) if cuda else None
+    side, copy_s = (torch.cuda.Stream(device), torch.cuda.Stream(device)) if cuda else (None, None)
+
+    def on(stream):
+        return torch.cuda.stream(stream) if cuda else contextlib.nullcontext()
+
+    def record(stream):
+        if not cuda:
+            return None
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        return ev
+    stage = [torch.empty(batch, H, W, 3, dtype=torch.uint8, device=device) for _ in range(2)]
+    gath = [torch.empty(world, batch, H, W, 3, dtype=torch.uint8, device=device) if rank == 0 and world > 1 else None for _ in range(2)]
     drained = [None, None]
     for k in range(plan.steps):
-        result = step(k, plan.frames(k))
+        frames = step(k, plan.frames(k))
         s = k & 1
         if drained[s] is not None:
             main.wait_event(drained[s])                                    # batch k-2 has left this staging buffer
-        stage[s].copy_(_frames_u8(result, image_mode))
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
+        stage[s].copy_(frames)
+        if cuda:
+            side.wait_stream(main)
+        with on(side):
             if world > 1:
                 dist.gather(stage[s], list(gath[s].unbind(0)) if rank == 0 else None, dst=0)
-            ev = torch.cuda.Event()
-            ev.record(side)
+            ev = record(side)
         drained[s] = ev
         if rank == 0:
-            copy_s.wait_event(ev)
-            with torch.cuda.stream(copy_s):
+            if cuda:
+                copy_s.wait_event(ev)
+            with on(copy_s):
                 for r in range(world):
                     s0, e0 = spans[r]
                     f0 = s0 + k * batch
                     n = max(0, min(batch, e0 - f0))
                     if n > 0:
                         src = gath[s][r] if world > 1 else stage[s]
-                        host[f0:f0 + n].copy_(src[:n], non_blocking=True)
-                ev2 = torch.cuda.Event()
-                ev2.record(copy_s)
+                        host[f0:f0 + n].copy_(src[:n], non_blocking=cuda)
+                ev2 = record(copy_s)
             drained[s] = ev2                                               # the staging / gather buffers are free once the D2H left them
-    main.wait_stream(side)
-    main.wait_stream(copy_s)
+    if cuda:
+        main.wait_stream(side)
+        main.wait_stream(copy_s)
     return host
 
 

@@ -528,12 +528,13 @@ class Engine:
                                    ws=self._f32(B, *ws_shape[1:]), noise_mode=None)          # noise_mode None: nothing cached yet
         return c
 
-    def _cached(self, N, who):
-        """The filled cache for a call with batch N (None when nothing is cached); a cache of another batch size raises."""
+    def _cached(self, N, who, views=False):
+        """The filled cache for a call with batch N (None when nothing is cached).  views: N may be any multiple B * V of the cached
+        batch B (image n takes head n // V); otherwise N must equal B.  Another batch size raises."""
         c = self._cache
         if c is None or c['noise_mode'] is None:
             return None
-        if c['B'] != N:
+        if (N % c['B'] if views else N != c['B']):
             raise RuntimeError(f'next3d_b200: {who} with batch {N}, but the cached backbone holds batch {c["B"]}')
         return c
 
@@ -561,7 +562,10 @@ class Engine:
         cfg, dev = self.cfg, self.device
         N = ws.shape[0]
         P = cfg.plane_res
-        cached = self._cached(N, 'use_cached_backbone') if use_cached_backbone else None
+        # N = B * V images on a cache of B heads: image n takes its texture and static planes from head n // V.  A call that also
+        # refills the cache keeps N = B (the cache holds one set of planes per head).
+        cached = self._cached(N, 'use_cached_backbone', views=not cache_backbone) if use_cached_backbone else None
+        V = N // cached['B'] if cached is not None else 1
         v = v.to(torch.float32)
         verts, lms = v[:, :5023].contiguous(), v[:, 5023:].contiguous()
         self._set_styles(ws)
@@ -603,7 +607,7 @@ class Engine:
         # alpha) ends binary, as the reference's (alpha.bool() | alpha.bool()).float() leaves it (triplane_next3d.py:226)
         tex_planes = self._f32(3, N, P, P, cfg.plane_ch)
         alpha = self._f32(3, N, P, P)
-        K.uv_sample(p2f, bary, self.face_uv, textures, self.eye_mask, tex_planes, alpha)
+        K.uv_sample(p2f, bary, self.face_uv, textures, self.eye_mask, tex_planes, alpha, views=V)
         K.fill_mouth(alpha, binarize=(N, 2 * N))
         # mouth crop -> StyleUNet -> paste back -> neural blending
         front = tex_planes[0]
@@ -617,7 +621,7 @@ class Engine:
             main.wait_stream(s_static)
             static.record_stream(main)
         planes = self._f32(N, 3, P, P, cfg.plane_ch)
-        K.blend_planes(blended, tex_planes, alpha, static, planes)
+        K.blend_planes(blended, tex_planes, alpha, static, planes, views=V)
         if cache_backbone:
             c = self._cache_buffers(N, ws.shape)
             if cached is None:
@@ -634,7 +638,8 @@ class Engine:
     def synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
                   return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False, depth_range='batch'):
         """cache_backbone: also keep the backbone outputs, planes and ws (see _cache_buffers); use_cached_backbone: take the two
-        ws-only backbones from that cache (a cache of another batch size raises; no cache = computed as usual).  depth_range: 'batch'
+        ws-only backbones from that cache (no cache = computed as usual): N = B * V images on a cache of batch B, image n reading
+        head n // V (N = B when cache_backbone is also set; any other batch raises).  depth_range: 'batch'
         clamps every image's depth to the range of the whole call (ray_marcher.py:54 on a batch), 'image' to the image's own range
         (what a call per image gives)."""
         self._on_device(ws=ws, c=c, v=v)
@@ -763,15 +768,16 @@ class Engine:
     def _synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
                            use_cached_backbone=False, depth_range='batch'):
         """Same as synthesis() (in-kernel sampler RNG) but the ~200 launches of one forward are captured once per
-        (batch, resolution, noise_mode, cache use) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
+        (batch, cached batch, resolution, noise_mode, cache use) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
         leaves the GPU idle between kernels.  The cache-using graphs read and write the engine's cache buffers in place."""
         self._on_device(ws=ws, c=c, v=v)
         N = ws.shape[0]
         R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-        reuse = use_cached_backbone and self._cached(N, 'use_cached_backbone') is not None
+        reuse = use_cached_backbone and self._cached(N, 'use_cached_backbone', views=not cache_backbone) is not None
         if cache_backbone:
             self._cache_buffers(N, ws.shape)              # allocated before capture: the graph writes the cache at fixed addresses
-        key = (cache_backbone or reuse, cache_backbone, reuse, N, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
+        B = self._cache['B'] if reuse else N              # (N, B): the images per cached head of a reusing graph
+        key = (cache_backbone or reuse, cache_backbone, reuse, N, B, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
 
         def run(st):
             return self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,

@@ -64,12 +64,28 @@ def load_frame(obj_path, lms_path=None, pin=False):
     return t.pin_memory() if pin else t
 
 
+def load_photo(png_path, size=512, pin=False):
+    """-> uint8 [size, size, 3] tensor: `np.array(Image.open(png).crop((0, 0, size, size)))`, the driving photo of
+    reenact_avatar_next3d.py:132-133 (pixels outside the image read as 0, as PIL's crop gives them).  pin=True: page-locked."""
+    from PIL import Image
+    with Image.open(png_path) as im:
+        a = np.array(im.crop((0, 0, size, size)))
+    if a.ndim != 3 or a.shape[2] != 3:
+        raise ValueError(f'{png_path}: the driving photo must be an RGB image, got array shape {a.shape}')
+    t = torch.from_numpy(a)
+    return t.pin_memory() if pin else t
+
+
 class FramePrefetcher:
     """Iterate over (obj_path, lms_path) pairs, parsing `depth` frames ahead on worker threads (the parsers release the GIL
-    inside the native call) and yielding pinned `[1, V+68, 3]` tensors in order."""
+    inside the native call) and yielding pinned `[1, V+68, 3]` tensors in order.  With `photos` (one PNG path per frame) every
+    item is (mesh, photo), the photo decoded by load_photo on the same worker threads."""
 
-    def __init__(self, frames, depth=4, workers=2, pin=None):
+    def __init__(self, frames, depth=4, workers=2, pin=None, photos=None):
         self.frames = list(frames)
+        self.photos = None if photos is None else list(photos)
+        if self.photos is not None and len(self.photos) != len(self.frames):
+            raise ValueError(f'FramePrefetcher: {len(self.photos)} photos for {len(self.frames)} frames')
         self.depth = max(1, depth)
         self.pin = torch.cuda.is_available() if pin is None else pin
         self.pool = concurrent.futures.ThreadPoolExecutor(max_workers=workers)
@@ -77,20 +93,25 @@ class FramePrefetcher:
     def __len__(self):
         return len(self.frames)
 
+    def _load(self, i):
+        f = self.frames[i]
+        mesh = load_frame(f[0], f[1], self.pin)
+        return mesh if self.photos is None else (mesh, load_photo(self.photos[i], pin=self.pin))
+
     def __iter__(self):
         pending = []
-        it = iter(self.frames)
+        it = iter(range(len(self.frames)))
         try:
             for _ in range(self.depth):
-                f = next(it, None)
-                if f is None:
+                i = next(it, None)
+                if i is None:
                     break
-                pending.append(self.pool.submit(load_frame, f[0], f[1], self.pin))
+                pending.append(self.pool.submit(self._load, i))
             while pending:
                 out = pending.pop(0).result()
-                f = next(it, None)
-                if f is not None:
-                    pending.append(self.pool.submit(load_frame, f[0], f[1], self.pin))
+                i = next(it, None)
+                if i is not None:
+                    pending.append(self.pool.submit(self._load, i))
                 yield out
         finally:
             for p in pending:

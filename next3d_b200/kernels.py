@@ -213,12 +213,13 @@ def rasterize(verts, faces, H, W, p2f, bary, workspace=None):
     _run('n3d_rasterize', ptr(verts), ptr(faces), NM, V, faces.shape[0], H, W, ptr(p2f), ptr(bary), ptr(workspace), stream_ptr(), kernels=2)
 
 
-def uv_sample(p2f, bary, face_uv, texture, eye_mask, tex_planes, alpha):
-    N, TH, TW, Cc = texture.shape
+def uv_sample(p2f, bary, face_uv, texture, eye_mask, tex_planes, alpha, views=1):
+    """views: images per texture -- N = texture.shape[0] * views images, image n reads texture n // views."""
+    B, TH, TW, Cc = texture.shape
     _, H, W = p2f.shape
     MH, MW = eye_mask.shape[-2:]
-    _run('n3d_uv_sample', ptr(p2f), ptr(bary), ptr(face_uv), ptr(texture), ptr(eye_mask), N, H, W, TH, TW, Cc, MH, MW,
-                          ptr(tex_planes), ptr(alpha), stream_ptr())
+    _run('n3d_uv_sample_views', ptr(p2f), ptr(bary), ptr(face_uv), ptr(texture), ptr(eye_mask), B * views, views, H, W, TH, TW, Cc, MH, MW,
+                                ptr(tex_planes), ptr(alpha), stream_ptr())
 
 
 def fill_mouth(alpha, binarize=(0, 0)):
@@ -242,9 +243,10 @@ def resize_aa(src, dst=None, DH=None, DW=None, src_box=None, dst_box=None, style
                           stream_ptr())
 
 
-def blend_planes(front, tex_planes, alpha, static, planes):
+def blend_planes(front, tex_planes, alpha, static, planes, views=1):
+    """views: images per static plane set -- image n of front's N reads static n // views."""
     N, H, W, _ = front.shape
-    _run('n3d_blend_planes', ptr(front), ptr(tex_planes), ptr(alpha), ptr(static), N, H, W, ptr(planes), stream_ptr())
+    _run('n3d_blend_planes_views', ptr(front), ptr(tex_planes), ptr(alpha), ptr(static), N, views, H, W, ptr(planes), stream_ptr())
 
 
 def _render_desc(planes, cam2world, intrinsics, res, opts, seed, views=1):

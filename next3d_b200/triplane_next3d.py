@@ -193,8 +193,10 @@ class TriPlaneGenerator(torch.nn.Module):
         -grad sigma composited like the colours (renderer.py:271-355, ray_marcher.py:61-64).
         `cache_backbone=True` also keeps this call's ws-only backbone outputs, blended planes, ws and noise_mode until the next caching
         call or a weight change; `use_cached_backbone=True` takes the two ws-only backbones from that cache and re-runs everything
-        that depends on the mesh (triplane.py:120-128 of EG3D; a cache of another batch size raises, no cache computes them), and
-        `render_views` renders new cameras from the cached planes.
+        that depends on the mesh (triplane.py:120-128 of EG3D; no cache computes them), and `render_views` renders new cameras from
+        the cached planes.  With B heads cached, use_cached_backbone takes N = B * V images (ws, c, v per image): image n takes its
+        neural texture and static planes from head n // V, everything else is computed per image with the call's ws.  N not a
+        multiple of B raises RuntimeError, and so does N != B when the call also sets cache_backbone.
         Extra keyword `depth_range`: 'batch' (default, the reference's semantics for a batched call) clamps every image's depth to the
         range of all the call's samples (ray_marcher.py:54); 'image' clamps each image to its own range, so 'image_depth' of a batch
         equals that of one call per image (the reference's scripts render one frame per call)."""
