@@ -151,32 +151,36 @@ def _frames(outputs, image_mode, device):
 
 def _to_host(batches, device):
     """uint8 numpy frames of successive batches of device frames (uint8 tensor [>= n, H, W, C], valid count n), in order; the
-    device->host copy of batch i overlaps the work that produces batch i+1.  Each tensor must be fresh (not reused by its producer)."""
+    device->host copy of batch i overlaps the work that produces batch i+1.  Each tensor must be fresh (not reused by its producer).
+    A batch may also be a tuple of tensors [>= n, ...] of any dtype; then every item is the tuple of their rows."""
     cuda = torch.device(device).type == 'cuda'
     copy_s = torch.cuda.Stream(device) if cuda else None
-    pending = None                                               # (host tensor, event, valid count) of the previous batch
+    pending = None                                               # (host tensors, event, valid count, tuple batch) of the previous batch
 
     def drain(p):
-        host, ev, n = p
+        hosts, ev, n, many = p
         if ev is not None:
             ev.synchronize()
         for k in range(n):
-            yield host[k].numpy()
+            yield tuple(h[k].numpy() for h in hosts) if many else hosts[0][k].numpy()
 
-    for u8, n in batches:
+    for dev_t, n in batches:
+        many = isinstance(dev_t, tuple)
+        ts = dev_t if many else (dev_t,)
         if cuda:
-            host = torch.empty(u8.shape, dtype=torch.uint8).pin_memory()
+            hosts = tuple(torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in ts)
             copy_s.wait_stream(torch.cuda.current_stream(device))
             with torch.cuda.stream(copy_s):
-                host.copy_(u8, non_blocking=True)
-                u8.record_stream(copy_s)
+                for host, t in zip(hosts, ts):
+                    host.copy_(t, non_blocking=True)
+                    t.record_stream(copy_s)
                 ev = torch.cuda.Event()
                 ev.record(copy_s)
         else:
-            host, ev = u8, None
+            hosts, ev = ts, None
         if pending is not None:
             yield from drain(pending)
-        pending = (host, ev, n)
+        pending = (hosts, ev, n, many)
     if pending is not None:
         yield from drain(pending)
 
@@ -288,7 +292,7 @@ def grid_keyframes(G, seeds, grid, num_keyframes=None, shuffle_seed=None, trunca
     gw, gh = grid
     all_seeds, K = _grid_seeds(seeds, grid, num_keyframes, shuffle_seed)
     device = next(G.parameters()).device
-    zs = torch.from_numpy(np.stack([np.random.RandomState(seed).randn(G.z_dim) for seed in all_seeds])).to(device)
+    zs = seed_latents(all_seeds, G.z_dim).to(device)
     ws = G.mapping(z=zs, c=_frontal_camera(G, len(zs)).to(device), truncation_psi=truncation_psi, truncation_cutoff=truncation_cutoff)
     return ws.reshape(gh, gw, K, *ws.shape[1:])
 
@@ -695,3 +699,165 @@ def extract_sigma_grid(G, ws, v, shape_res=512, max_batch=1000000, noise_mode='c
     # border voxels (55 % of a 256^3 grid) never decoded.  max_batch is kept for API compatibility with the script's chunk size.
     K.sample_grid(planes[0], shape_res, box * 1, box, eng.dec, sigmas, pad=int(30 * shape_res / 256))
     return sigmas.cpu().numpy()
+
+
+# ------------------------------------------------------------------------------------------------ sample sheets (gen_samples_next3d.py)
+SHEET_YAWS = (0.4, 0.0, -0.4)          # gen_samples_next3d.py:187-188: three yaws, left to right on the sheet, all at pitch -0.2
+SHEET_PITCH = -0.2
+NUM_WS = 28                            # mapping_ws of the backbone (triplane_next3d.py:65)
+
+
+def sample_sheet_cameras(G, fov_deg=18.837):
+    """(cams [3, 25], cond [1, 25]) float32: the camera_params of yaws +0.4, 0, -0.4 at pitch -0.2 and the frontal conditioning_params
+    of gen_samples_next3d.py:186-196 (np.pi / 2 + angle, where the video script writes 3.14 / 2), looking at
+    rendering_kwargs['avg_camera_pivot'] (default [0, 0, 0]) from radius rendering_kwargs['avg_camera_radius'] (default 2.7), with
+    FOV_to_intrinsics(fov_deg).  fov_deg may be an int or a float: the script declares --fov-deg as an int with the default 18.837,
+    which click casts to 18 when the option is omitted."""
+    rk = G.rendering_kwargs
+    pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
+    radius = rk.get('avg_camera_radius', 2.7)
+    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
+
+    def params(horizontal, vertical):
+        return torch.cat([camera.look_at_pose(horizontal, vertical, pivot, radius).reshape(-1, 16), intr], 1)
+    cams = torch.cat([params(np.pi / 2 + yaw, np.pi / 2 + SHEET_PITCH) for yaw in SHEET_YAWS])
+    return cams, params(np.pi / 2, np.pi / 2)
+
+
+def seed_latents(seeds, z_dim):
+    """z [S, z_dim] float64: row s is np.random.RandomState(seeds[s]).randn(1, z_dim), the latent every inference script draws per seed."""
+    return torch.from_numpy(np.stack([np.random.RandomState(seed).randn(1, z_dim)[0] for seed in seeds]))
+
+
+def sample_sheet_ws(G, seeds, truncation_psi=1, truncation_cutoff=14, fov_deg=18.837):
+    """ws [S, 28, 512] on the generator's device: row s is the script's G.mapping(RandomState(seeds[s]).randn(1, z_dim), cond,
+    truncation_psi, truncation_cutoff) (gen_samples_next3d.py:184, 198) with cond from sample_sheet_cameras.  One mapping call maps all
+    seeds: on CUDA, n3d_mapping computes each row in its own thread block, so a row does not depend on the others."""
+    if len(seeds) == 0:
+        raise ValueError('seeds: no seed given')
+    device = next(G.parameters()).device
+    _, cond = sample_sheet_cameras(G, fov_deg)
+    z = seed_latents(seeds, G.z_dim).to(device)
+    return G.mapping(z, cond.to(device).expand(len(seeds), -1), truncation_psi=truncation_psi, truncation_cutoff=truncation_cutoff)
+
+
+def sheet_u8(front, views):
+    """uint8 sample sheets [B, H, 3 W, 3] of B heads from their images at yaw +0.4, front [B, 3, H, W], and at yaws 0 and -0.4, views
+    [2 B, 3, H, W] (view n of head n // 2): the script's torch.cat(imgs, dim=2) of its uint8 images (gen_samples_next3d.py:201-204),
+    on whatever device the images are."""
+    B, _, H, W = front.shape
+    side = to_uint8_hwc(views).reshape(B, 2, H, W, 3).transpose(1, 2).reshape(B, H, 2 * W, 3)
+    return torch.cat([to_uint8_hwc(front), side], 2)
+
+
+def _check_sheets(G, ws, v, batch, shape_res):
+    """Heads per call of the sample-sheet drivers, max(1, batch // 3), after refusing bad arguments (ValueError naming the argument)."""
+    if ws.ndim != 3 or tuple(ws.shape[1:]) != (NUM_WS, G.w_dim):
+        raise ValueError(f'ws must be [S, {NUM_WS}, {G.w_dim}], got {tuple(ws.shape)}')
+    if ws.shape[0] == 0:
+        raise ValueError('ws holds no seed (S = 0)')
+    if batch < 1:
+        raise ValueError(f'batch must be at least 1, got {batch}')
+    if shape_res < 2:
+        raise ValueError(f'shape_res must be at least 2, got {shape_res}')
+    if v.ndim != 3 or v.shape[0] != 1:
+        raise ValueError(f'v must be one mesh [1, V, 3] (the script renders every seed with the same mesh), got {tuple(v.shape)}')
+    return max(1, batch // 3)
+
+
+def _sheet_noise(sampler_noise, idx):
+    """sampler_noise keywords of the caching call (yaw +0.4 of heads idx) and of the render_views call (yaws 0, -0.4, view n of head
+    idx[n // 2]): rows 3 i + yaw of the per-image uniforms."""
+    if sampler_noise is None:
+        return {}, {}
+    return ({'sampler_noise': _noise_rows(sampler_noise, [3 * i for i in idx])},
+            {'sampler_noise': _noise_rows(sampler_noise, [3 * i + 1 + j for i in idx for j in range(2)])})
+
+
+def _sheet_batch(G, ws, idx, n, cams, v, kws, shapes, shape_res, device):
+    """(uint8 sheets [len(idx), H, 3 W, 3], float32 density grids [n, R, R, R] or None) of the heads ws[idx], of which the first n are
+    wanted: one caching synthesis call renders yaw +0.4 and keeps the heads, one render_views call renders the other two yaws from the
+    cached planes, and each wanted head's grid is decoded from its cached planes."""
+    B = len(idx)
+    w = ws[idx].to(device, torch.float32, non_blocking=True)
+    front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True, **kws[0])['image']
+    sheets = sheet_u8(front, G.render_views(cams[1:].repeat(B, 1), **kws[1])['image'])
+    if not shapes:
+        return sheets, None
+    sigmas = torch.empty(n, shape_res, shape_res, shape_res, device=device)
+    eng = G._get_engine()
+    for b in range(n):
+        eng.cached_sigma_grid(b, shape_res, sigmas[b])
+    return sheets, sigmas
+
+
+def render_sample_sheets(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=None, sampler_noise=None):
+    """gen_samples_next3d.py:182-238 for the seeds of ws [S, 28, 512] (sample_sheet_ws) and one mesh v [1, V, 3]: yields
+    (i, sheet, sigmas) in seed order.  sheet: uint8 [H, 3 W, 3] numpy, the script's three yaws side by side (sheet_u8);
+    sigmas: float32 [R, R, R] numpy with R = shape_res, equal to extract_sigma_grid(G, ws[i:i + 1], v, shape_res), or None unless
+    `shapes`.  Each step takes B = max(1, batch // 3) heads: one synthesis call with cache_backbone renders yaw +0.4 and caches the
+    heads, one render_views call renders the other two yaws as 2 B views, and each head's density grid is decoded from its cached
+    planes, so the backbones run once per head (the script runs them three times for the sheet and once per 1M-point chunk for the
+    shape).  The last step is padded by repeating its last head.  The device->host copy of step k overlaps step k+1.  With
+    G.use_cuda_graph (and no sampler_noise) the calls replay CUDA graphs.  The driver replaces whatever heads the generator had cached.
+    `seed`: step k draws sampler seeds seed + 2 k (synthesis) and seed + 2 k + 1 (render_views); None = fresh random seeds.
+    `sampler_noise=(u_coarse [3 S, M, Dc, 1], u_fine [3 S, M, Df])` rows are indexed by the global image id 3 i + yaw (yaw 0, 1, 2 =
+    +0.4, 0, -0.4).  ValueError, before any device work, for an empty or misshapen ws, batch < 1, shape_res < 2 or a v batch other
+    than 1."""
+    B = _check_sheets(G, ws, v, batch, shape_res)
+    return _sample_sheets(G, ws, v, fov_deg, B, shapes, shape_res, seed, sampler_noise)
+
+
+def _sample_sheets(G, ws, v, fov_deg, B, shapes, shape_res, seed, sampler_noise):
+    device = next(G.parameters()).device
+    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
+    v = v.to(device, torch.float32)
+
+    def steps():
+        for k, (idx, n, _) in enumerate(_batches(ws.shape[0], B, None, None)):
+            kws = _sheet_noise(sampler_noise, idx)
+            if seed is not None:
+                kws[0]['seed'], kws[1]['seed'] = int(seed) + 2 * k, int(seed) + 2 * k + 1
+            sheets, sigmas = _sheet_batch(G, ws, idx, n, cams, v, kws, shapes, shape_res, device)
+            yield ((sheets, sigmas) if shapes else sheets), n
+    for i, item in enumerate(_to_host(steps(), device)):
+        sheet, sigmas = item if shapes else (item, None)
+        yield i, sheet, sigmas
+
+
+def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=0, sampler_noise=None, out=None,
+                                 device=None):
+    """render_sample_sheets over the GPUs of a box (one process per GPU, as render_frames_sharded): the seeds are split with
+    shard_plan (plan.batch heads per step, batch // 3 as the bound) and the sheets gathered to rank 0.  -> (sheets, sigmas):
+    sheets is the [S, H, 3 W, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere, filled in stream order as in
+    render_frames_sharded; sigmas is {i: float32 [R, R, R] numpy} for this rank's own seeds i (empty unless `shapes`; the grids are not
+    gathered: one 512^3 grid is 512 MB), complete on return.  Step k of rank r draws sampler seeds seed + 2 (r * steps + k) and one
+    more; `sampler_noise` rows are indexed 3 i + yaw by the global seed index i, so the results do not depend on the number of ranks.
+    Refusals as in render_sample_sheets."""
+    B = _check_sheets(G, ws, v, batch, shape_res)
+    device = device or next(G.parameters()).device
+    cuda = torch.device(device).type == 'cuda'
+    plan = shard_plan(ws.shape[0], B)
+    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
+    v = v.to(device, torch.float32)
+    lo, hi = plan.spans[plan.rank]
+    grids = {}
+
+    def step(k, idx):
+        kws = _sheet_noise(sampler_noise, idx)
+        if sampler_noise is None:
+            s = int(seed) + 2 * (plan.rank * plan.steps + k)
+            kws[0]['seed'], kws[1]['seed'] = s, s + 1
+        # this rank's seeds without a grid yet: a prefix of idx (a short tail repeats the last seed, a rank past its span repeats a
+        # seed it has done, a rank without seeds repeats the previous rank's last)
+        new = [i for i in dict.fromkeys(idx) if lo <= i < hi and i not in grids] if shapes else []
+        sheets, sigmas = _sheet_batch(G, ws, idx, len(new), cams, v, kws, bool(new), shape_res, device)
+        for b, i in enumerate(new):
+            grids[i] = torch.empty(sigmas[b].shape, pin_memory=cuda)
+            grids[i].copy_(sigmas[b], non_blocking=cuda)
+        return sheets
+    res = G.img_resolution
+    host = _gather_frames(plan, step, res, 3 * res, device, out)
+    if cuda and grids:
+        torch.cuda.current_stream(device).synchronize()
+    return host, {i: g.numpy() for i, g in grids.items()}

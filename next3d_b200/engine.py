@@ -725,6 +725,23 @@ class Engine:
         self.launches = K.launches - n0
         return result
 
+    def cached_sigma_grid(self, b, shape_res, sigma):
+        """The shape-extraction density grid of cached head b (gen_samples_next3d.py:208-238: create_samples at box_warp, sigma
+        flipped along axis 0 and trimmed) written into sigma, float32 [shape_res]^3 on the engine's device, from the planes the
+        caching call kept: one n3d_sample_grid launch, no backbone.  Raises RuntimeError when nothing is cached or b is not a cached head."""
+        c = self._cache
+        if c is None or c['noise_mode'] is None:
+            raise RuntimeError('next3d_b200: cached_sigma_grid needs cached planes: run synthesis(..., cache_backbone=True) first')
+        if not 0 <= b < c['B']:
+            raise RuntimeError(f'next3d_b200: cached_sigma_grid of head {b}, but the cache holds {c["B"]} head(s)')
+        self._on_device(sigma=sigma)
+        if sigma.dtype != torch.float32 or tuple(sigma.shape) != (shape_res,) * 3 or not sigma.is_contiguous():
+            raise RuntimeError(f'next3d_b200: cached_sigma_grid needs a contiguous float32 [{shape_res}]^3 output, got {sigma.dtype} '
+                               f'{tuple(sigma.shape)}')
+        box = self.rk['box_warp']
+        with torch.cuda.device(self.device):
+            K.sample_grid(c['planes'][b], shape_res, box * 1, box, self.dec, sigma, pad=int(30 * shape_res / 256))
+
     # ------------------------------------------------------------------------------------------ CUDA graph replay
     def _render_key(self, R):
         rk = self.rk
