@@ -1,12 +1,19 @@
-"""Batched frame drivers (SURVEY.md section 8, row f1): the per-frame Python loops of `gen_videos_next3d.py:128-171` and
-`reenact_avatar_next3d.py:125-167` restated as (1) a frame schedule computed up front -- orbit cameras, interpolated latents --
-and (2) a loop over BATCHES of frames through `TriPlaneGenerator.synthesis` (CUDA-graph replay), with the uint8 conversion on
-the device and an asynchronous read-back, so that nothing but the generator sits on the critical path.
+"""Batched frame drivers (SURVEY.md section 8, row f1): the per-frame Python loops of `gen_videos_next3d.py:128-171`,
+`reenact_avatar_next3d.py:125-167` and `gen_samples_next3d.py:182-238` restated as (1) a schedule computed up front -- orbit cameras,
+interpolated latents, driving frames -- and (2) a loop over BATCHES of frames through `TriPlaneGenerator.synthesis` (CUDA-graph
+replay) or `render_views`, with the uint8 conversion on the device, so that nothing but the generator sits on the critical path.
+
+Each workload (interpolated frames, one-head orbits, reenactment, the two grids, sample sheets) is written once, as a private
+function that does its setup and returns `step(k, idx)`: render step k of a plan (ShardPlan), the frames idx, and return their
+uint8 frames.  Its two public drivers differ only in the plan and in how the finished batches leave the device: the single-process
+generator (local_plan: exactly `batch` frames per step) streams them to the caller through _to_host, an asynchronous read-back
+under the next step; the sharded twin (shard_plan: one process per GPU, contiguous frame ranges) gathers them to rank 0 through
+_gather_frames.  The sampler keywords of every call follow one rule (_sampler_kw).
 
 Everything here is host logic around the hot path; the per-frame values (camera matrices, interpolated ws, uint8 pixels) are the
-reference's, checked in tests/test_drivers_cpu.py against the reference's own code.
+reference's, checked in tests/test_drivers_cpu.py against the reference's own code, and the calls every driver makes in
+tests/test_driver_calls_cpu.py.
 """
-import math
 from typing import NamedTuple
 
 import numpy as np
@@ -45,85 +52,6 @@ def to_uint8_hwc(img):
     return (img * 127.5 + 128).clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
 
 
-def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_mode='const', device=None, seed=None, sampler_noise=None):
-    """Yield one uint8 HWC numpy frame per (ws, camera, mesh) triple, in order, rendering `batch` frames per synthesis call.
-
-    ws_frames [F, L, D], cams [F, 25], verts: [F, V, 3] / [1, V, 3] (static mesh) tensors, or an iterable of per-frame [1, V, 3]
-    tensors (e.g. inputs.FramePrefetcher).  The last, partial batch is padded by repeating its final frame (one graph shape) and
-    the padding is dropped.  The device->host copy of batch i overlaps the synthesis of batch i+1.  `seed`: base seed of the ray
-    sampler's RNG (batch k uses seed + k); None = a fresh random seed per call, like the reference's torch.rand.
-    `sampler_noise=(u_coarse [F, M, Dc, 1], u_fine [F, M, Df])`: per-frame sampler uniforms instead of the in-kernel RNG (parity tests:
-    frame f gets the same noise whichever batch slot it lands in).  image_mode 'image_depth' renders with depth_range='image', so
-    each depth frame is clamped to its own range as in the script (one frame per synthesis call), whatever the batching."""
-    yield from _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, False)
-
-
-def render_orbit(G, ws, cams, verts, batch=8, image_mode='image', seed=None, sampler_noise=None):
-    """Yield one uint8 HWC numpy frame per camera of cams [F, 25] for ONE head: ws [1, L, D] and mesh verts [1, V, 3] stay fixed
-    (gen_videos_next3d.py with one seed, sample sheets), so the tri-planes are computed once (noise_mode 'const') and every batch of
-    `batch` cameras is rendered from them by G.render_views -- volume rendering and super-resolution only.  Padding, `seed` and
-    `sampler_noise` as in render_frames."""
-    device = next(G.parameters()).device
-    G.synthesis(ws.to(device, torch.float32), cams[:1].to(device, torch.float32), verts.to(device, torch.float32), noise_mode='const',
-                cache_backbone=True, seed=0)
-
-    def outputs():
-        for idx, n, kw in _batches(cams.shape[0], batch, seed, sampler_noise):
-            yield G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device), **kw), n
-    yield from _frames(outputs(), image_mode, device)
-
-
-def _batches(F, batch, seed, sampler_noise):
-    """(frame indices, valid count, sampler keywords) of each batch of `batch` frames; the last batch is padded by repeating its final
-    frame (one graph shape).  Batch k gets sampler seed `seed` + k, or its frames' rows of `sampler_noise`."""
-    for b0 in range(0, F, batch):
-        n = min(batch, F - b0)
-        idx = list(range(b0, b0 + n)) + [b0 + n - 1] * (batch - n)
-        kw = {} if seed is None else {'seed': int(seed) + b0 // batch}
-        if sampler_noise is not None:
-            kw['sampler_noise'] = _noise_rows(sampler_noise, idx)
-        yield idx, n, kw
-
-
-def _noise_rows(sampler_noise, idx):
-    """The synthesis `sampler_noise` of the frames idx from per-frame rows (u_coarse [F, M, Dc, 1], u_fine [F, M, Df])."""
-    u_c, u_f = sampler_noise
-    return u_c[idx], u_f[idx].reshape(-1, u_f.shape[-1])
-
-
-def _depth_kw(image_mode, device):
-    """Depth frames are clamped to their own depth range, as the scripts' one frame per call does (gen_videos_next3d.py:155,
-    reenact_avatar_next3d.py:164), whatever the batching; the other image modes do not read the range.  The range is the CUDA
-    renderer's (depth_range='image'); a generator on another device is called without the keyword."""
-    return {'depth_range': 'image'} if image_mode == 'image_depth' and torch.device(device).type == 'cuda' else {}
-
-
-def _render_frames(G, ws_frames, cams, verts, batch, image_mode, noise_mode, device, seed, sampler_noise, reuse_backbone):
-    """render_frames.  reuse_backbone: every frame has the same ws (one identity), so the first batch caches the ws-only backbones
-    and the later ones reuse them (use_cached_backbone); with noise_mode 'const' or 'none' those are a function of ws alone, so the
-    frames are the same."""
-    device = device or next(G.parameters()).device
-    vit = None
-    if not torch.is_tensor(verts):
-        vit = iter(verts)
-
-    def outputs():
-        for k, (idx, n, kw) in enumerate(_batches(ws_frames.shape[0], batch, seed, sampler_noise)):
-            w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
-            c = cams[idx].to(device, torch.float32, non_blocking=True)
-            if vit is not None:
-                vs = [next(vit) for _ in range(n)]
-                v = torch.cat(vs + [vs[-1]] * (batch - n), 0).to(device, torch.float32, non_blocking=True)
-            elif verts.shape[0] == 1:
-                v = verts.to(device, torch.float32).expand(batch, -1, -1)
-            else:
-                v = verts[idx].to(device, torch.float32, non_blocking=True)
-            if reuse_backbone:
-                kw['use_cached_backbone' if k else 'cache_backbone'] = True
-            yield G.synthesis(w, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw), n
-    yield from _frames(outputs(), image_mode, device)
-
-
 def _frames_u8(out, image_mode):
     """[N, H, W, 3] uint8 frames of a generator output dict: out[image_mode], depth normalised per frame to [-1, 1] first."""
     img = out[image_mode]
@@ -135,6 +63,17 @@ def _frames_u8(out, image_mode):
     return to_uint8_hwc(img)
 
 
+def _depth_kw(image_mode, device):
+    """Depth frames are clamped to their own depth range, as the scripts' one frame per call does (gen_videos_next3d.py:155,
+    reenact_avatar_next3d.py:164), whatever the batching; the other image modes do not read the range.  The range is the CUDA
+    renderer's (depth_range='image'); a generator on another device is called without the keyword."""
+    return {'depth_range': 'image'} if image_mode == 'image_depth' and torch.device(device).type == 'cuda' else {}
+
+
+def _frame_resolution(G, image_mode):
+    return G.img_resolution if image_mode == 'image' else G.neural_rendering_resolution
+
+
 def layout_cells(cells, gw, gh):
     """uint8 cells [F * gh * gw, h, w, C] (the cells of each frame in row-major grid order, frame after frame) -> frames
     [F, gh * h, gw * w, C]: layout_grid of gen_videos_next3d.py:35-49 per frame, on whatever device the cells are (the uint8
@@ -143,10 +82,89 @@ def layout_cells(cells, gw, gh):
     return cells.reshape(n // (gh * gw), gh, gw, h, w, C).permute(0, 1, 3, 2, 4, 5).reshape(-1, gh * h, gw * w, C)
 
 
-def _frames(outputs, image_mode, device):
-    """uint8 HWC numpy frames of successive batches, in order; `outputs` yields (generator output dict, valid count) per batch.  The
-    conversion runs on the device, and the device->host copy of batch i overlaps the rendering of batch i+1."""
-    yield from _to_host(((_frames_u8(out, image_mode), n) for out, n in outputs), device)
+# ------------------------------------------------------------------------------------------------ plans and the two executors
+class ShardPlan(NamedTuple):
+    """How F frames are split into steps: rank r owns spans[r] and renders it in `steps` batches of `batch` frames; every rank runs
+    the same number of steps (one collective each).  local_plan is the single-process run, shard_plan the sharded drivers'."""
+    rank: int
+    world: int
+    spans: list
+    batch: int
+    steps: int
+
+    def frames(self, k):
+        """Global frame ids of this rank's batch k; a short tail repeats the last frame (one graph shape)."""
+        a, b = self.spans[self.rank]
+        lo = min(a + k * self.batch, max(b - 1, a))
+        return [min(lo + j, b - 1) for j in range(self.batch)]
+
+    def valid(self, k):
+        """How many of frames(k) are this rank's own frames (the rest repeat the last)."""
+        a, b = self.spans[self.rank]
+        return max(0, min(self.batch, b - a - k * self.batch))
+
+    def step_id(self, k):
+        """Global id rank * steps + k of this rank's step k: the sampler seed offset of the step."""
+        return self.rank * self.steps + k
+
+
+def local_plan(F, batch):
+    """The ShardPlan of a single process: F frames in ceil(F / batch) steps of exactly `batch` frames."""
+    return ShardPlan(0, 1, [(0, F)], batch, -(-F // batch))
+
+
+def shard_plan(F, batch):
+    """The ShardPlan of F frames for this process's rank in the current torch.distributed world (world 1 when uninitialised).
+    `batch` is an upper bound: the batch is the size in [batch/2, batch] that pads the largest rank's frame count least."""
+    import torch.distributed as dist
+    from . import distributed as D
+    world = dist.get_world_size() if dist.is_initialized() else 1
+    rank = dist.get_rank() if dist.is_initialized() else 0
+    spans = [D.shard_range(F, r, world) for r in range(world)]
+    nmax = max(e - s for s, e in spans)
+    batch = min(range(max(1, batch // 2), batch + 1), key=lambda bb: (-(-nmax // bb) * bb, -bb))     # least padding, then the largest
+    return ShardPlan(rank, world, spans, batch, -(-nmax // batch))
+
+
+def _sampler_kw(seed, sampler_noise, seed_id, ids):
+    """Sampler keywords of one call: the rows ids (global image ids) of the per-image uniforms sampler_noise = (u_coarse [N, M, Dc, 1],
+    u_fine [N, M, Df]) if given -- the renderer then draws no random numbers, so no seed goes with them --, else seed + seed_id (the
+    global step id; 2 step and 2 step + 1 for the two calls of a sample-sheet step) if a seed is given, else none (a fresh random
+    seed per call)."""
+    if sampler_noise is not None:
+        u_c, u_f = sampler_noise
+        return {'sampler_noise': (u_c[ids], u_f[ids].reshape(-1, u_f.shape[-1]))}
+    return {} if seed is None else {'seed': int(seed) + seed_id}
+
+
+class _InOrder:
+    """Items (meshes [1, V, 3], or (mesh, photo) pairs) of consecutive frames first, first + 1, ... from an in-order iterable, looked
+    up by frame id as the batches advance (each id is read once; ids behind the current batch are dropped)."""
+
+    def __init__(self, frames, first):
+        self.it, self.next, self.have = iter(frames), first, {}
+
+    def take(self, idx):
+        while self.next <= max(idx):
+            self.have[self.next] = next(self.it)
+            self.next += 1
+        self.have = {i: t for i, t in self.have.items() if i >= min(idx)}
+        return [self.have[i] for i in idx]
+
+
+def _in_order(plan, frames):
+    """_InOrder over this rank's frames, frames(a, b) being an in-order iterable of the items of frames a .. b-1 (a rank without
+    frames repeats the previous rank's last); None for a plan without steps."""
+    if plan.steps == 0:
+        return None
+    first = plan.frames(0)[0]
+    return _InOrder(frames(first, max(plan.spans[plan.rank][1], first + 1)), first)
+
+
+def _steps(plan, step):
+    """(step(k, plan.frames(k)), valid count) of every step of the plan, in order: the batches _to_host streams to the caller."""
+    for k in range(plan.steps):
+        yield step(k, plan.frames(k)), plan.valid(k)
 
 
 def _to_host(batches, device):
@@ -185,6 +203,159 @@ def _to_host(batches, device):
         yield from drain(pending)
 
 
+def _gather_frames(plan, step, H, W, device, out):
+    """The loop of the sharded drivers: for k in range(plan.steps), step(k, plan.frames(k)) renders this rank's batch k and returns
+    its uint8 frames [plan.batch, H, W, 3]; they go to a ping-pong staging buffer, are gathered to rank 0 over NCCL on a side stream
+    (world > 1) and copied to pinned host memory on a third stream, so the next batch renders while this one is in flight.
+    -> [F, H, W, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere.  It is filled in stream order: the caller's
+    current stream waits for the last copy, so synchronise that stream before reading the frames (back-to-back clips do not stall).
+    A CPU `device` (host-side tests under gloo) runs the same loop without streams."""
+    import contextlib
+    import torch.distributed as dist
+    rank, world, spans, batch = plan.rank, plan.world, plan.spans, plan.batch
+    cuda = torch.device(device).type == 'cuda'
+    host = None
+    if rank == 0:
+        host = out if out is not None else torch.empty(spans[-1][1], H, W, 3, dtype=torch.uint8, pin_memory=cuda)
+    main = torch.cuda.current_stream(device) if cuda else None
+    side, copy_s = (torch.cuda.Stream(device), torch.cuda.Stream(device)) if cuda else (None, None)
+
+    def on(stream):
+        return torch.cuda.stream(stream) if cuda else contextlib.nullcontext()
+
+    def record(stream):
+        if not cuda:
+            return None
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        return ev
+    stage = [torch.empty(batch, H, W, 3, dtype=torch.uint8, device=device) for _ in range(2)]
+    gath = [torch.empty(world, batch, H, W, 3, dtype=torch.uint8, device=device) if rank == 0 and world > 1 else None for _ in range(2)]
+    drained = [None, None]
+    for k in range(plan.steps):
+        frames = step(k, plan.frames(k))
+        s = k & 1
+        if drained[s] is not None:
+            main.wait_event(drained[s])                                    # batch k-2 has left this staging buffer
+        stage[s].copy_(frames)
+        if cuda:
+            side.wait_stream(main)
+        with on(side):
+            if world > 1:
+                dist.gather(stage[s], list(gath[s].unbind(0)) if rank == 0 else None, dst=0)
+            ev = record(side)
+        drained[s] = ev
+        if rank == 0:
+            if cuda:
+                copy_s.wait_event(ev)
+            with on(copy_s):
+                for r in range(world):
+                    s0, e0 = spans[r]
+                    f0 = s0 + k * batch
+                    n = max(0, min(batch, e0 - f0))
+                    if n > 0:
+                        src = gath[s][r] if world > 1 else stage[s]
+                        host[f0:f0 + n].copy_(src[:n], non_blocking=cuda)
+                ev2 = record(copy_s)
+            drained[s] = ev2                                               # the staging / gather buffers are free once the D2H left them
+    if cuda:
+        main.wait_stream(side)
+        main.wait_stream(copy_s)
+    return host
+
+
+# ------------------------------------------------------------------------------------------------ frames and orbits (gen_videos_next3d.py)
+def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_mode='const', device=None, seed=None, sampler_noise=None):
+    """Yield one uint8 HWC numpy frame per (ws, camera, mesh) triple, in order, rendering `batch` frames per synthesis call.
+
+    ws_frames [F, L, D], cams [F, 25], verts: [F, V, 3] / [1, V, 3] (static mesh) tensors, or an iterable of per-frame [1, V, 3]
+    tensors (e.g. inputs.FramePrefetcher).  The last, partial batch is padded by repeating its final frame (one graph shape) and
+    the padding is dropped.  The device->host copy of batch i overlaps the synthesis of batch i+1.  `seed`: base seed of the ray
+    sampler's RNG (batch k uses seed + k); None = a fresh random seed per call, like the reference's torch.rand.
+    `sampler_noise=(u_coarse [F, M, Dc, 1], u_fine [F, M, Df])`: per-frame sampler uniforms instead of the in-kernel RNG and `seed`
+    (parity tests: frame f gets the same noise whichever batch slot it lands in).  image_mode 'image_depth' renders with
+    depth_range='image', so each depth frame is clamped to its own range as in the script (one frame per synthesis call), whatever
+    the batching."""
+    device = device or next(G.parameters()).device
+    plan = local_plan(ws_frames.shape[0], batch)
+    verts = verts if torch.is_tensor(verts) else _InOrder(verts, 0)
+    yield from _to_host(_steps(plan, _frames_step(G, plan, ws_frames, cams, verts, image_mode, noise_mode, device, seed,
+                                                  sampler_noise)), device)
+
+
+def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const', seed=0, device=None, out=None, sampler_noise=None):
+    """Strong-scaling video driver (BASELINE.json configs[3]: one clip split over the GPUs of a box): rank r renders the contiguous
+    frame range shard_range(F, r, world) in batches through `G.synthesis`, converts to uint8 HWC on the device (4x fewer bytes than
+    the fp32 images) and the batches are gathered to rank 0 over NCCL on a side stream from a ping-pong staging buffer, so batch
+    i+1 renders while batch i is in flight; rank 0 copies every gathered batch to pinned host memory on a third stream.
+    Returns the [F, H, W, 3] uint8 host tensor (frame order) on rank 0, None elsewhere, filled in stream order (synchronise the
+    current stream before reading it).  World size 1: no collective.
+    `batch` is an upper bound: the per-call batch is the size in [batch/2, batch] that pads the rank's frame count least (30 frames per
+    rank -> 5 batches of 6, not 4 of 8).  `out`: optional pinned [F, H, W, 3] uint8 host tensor to fill on rank 0 (pinning 190 MB per
+    clip costs tens of milliseconds).  `sampler_noise`: per-frame uniforms as in render_frames, rows indexed by the global frame id,
+    so the frames do not depend on the number of ranks (batch k of rank r otherwise draws sampler seed seed + r * steps + k)."""
+    device = device or next(G.parameters()).device
+    plan = shard_plan(ws_frames.shape[0], batch)
+    step = _frames_step(G, plan, ws_frames, cams, verts, 'image', noise_mode, device, seed, sampler_noise)
+    return _gather_frames(plan, step, G.img_resolution, G.img_resolution, device, out)
+
+
+def _frames_step(G, plan, ws, cams, verts, image_mode, noise_mode, device, seed, sampler_noise, reuse_backbone=False):
+    """step(k, idx) of the frame and reenactment drivers: the uint8 frames of the frames idx, one synthesis call.  ws: per-frame
+    latents [F, L, D], or [1, L, D] for one identity; verts: per-frame [F, V, 3] or static [1, V, 3] meshes, or an _InOrder source of
+    [1, V, 3] meshes.  reuse_backbone: every frame has the same ws (one identity), so the first step caches the ws-only backbones and
+    the later ones reuse them (use_cached_backbone); with noise_mode 'const' or 'none' those are a function of ws alone, so the frames
+    are the same."""
+    def rows(t, idx):
+        if t.shape[0] == 1:
+            return t.to(device, torch.float32).expand(len(idx), -1, -1)
+        return t[idx].to(device, torch.float32, non_blocking=True)
+
+    def step(k, idx):
+        w = rows(ws, idx)
+        c = cams[idx].to(device, torch.float32, non_blocking=True)
+        v = torch.cat(verts.take(idx), 0).to(device, torch.float32, non_blocking=True) if isinstance(verts, _InOrder) else rows(verts, idx)
+        kw = _sampler_kw(seed, sampler_noise, plan.step_id(k), idx)
+        if reuse_backbone:
+            kw['use_cached_backbone' if k else 'cache_backbone'] = True
+        return _frames_u8(G.synthesis(w, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw), image_mode)
+    return step
+
+
+def render_orbit(G, ws, cams, verts, batch=8, image_mode='image', seed=None, sampler_noise=None):
+    """Yield one uint8 HWC numpy frame per camera of cams [F, 25] for ONE head: ws [1, L, D] and mesh verts [1, V, 3] stay fixed
+    (gen_videos_next3d.py with one seed, sample sheets), so the tri-planes are computed once (noise_mode 'const') and every batch of
+    `batch` cameras is rendered from them by G.render_views -- volume rendering and super-resolution only.  Padding, `seed` and
+    `sampler_noise` as in render_frames."""
+    device = next(G.parameters()).device
+    plan = local_plan(cams.shape[0], batch)
+    yield from _to_host(_steps(plan, _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, sampler_noise)), device)
+
+
+def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None, device=None):
+    """render_orbit over the GPUs of a box: every rank computes the head's planes once (ws [1, L, D], mesh verts [1, V, 3]) and
+    renders its contiguous range of the cameras cams [F, 25] with G.render_views; the frames are gathered to rank 0 as in
+    render_frames_sharded.  -> [F, H, W, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the
+    global frame id."""
+    device = device or next(G.parameters()).device
+    plan = shard_plan(cams.shape[0], batch)
+    step = _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, sampler_noise)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, step, res, res, device, out)
+
+
+def _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, sampler_noise):
+    """Computes and caches the head's tri-planes; -> step(k, idx): the uint8 frames of the cameras idx, one render_views call."""
+    G.synthesis(ws.to(device, torch.float32), cams[:1].to(device, torch.float32), verts.to(device, torch.float32), noise_mode='const',
+                cache_backbone=True, seed=0)
+
+    def step(k, idx):
+        out = G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device),
+                             **_sampler_kw(seed, sampler_noise, plan.step_id(k), idx))
+        return _frames_u8(out, image_mode)
+    return step
+
+
 # ------------------------------------------------------------------------------------------------ reenactment (reenact_avatar_next3d.py)
 def reenact_schedule(drive_root, num_frames, lms_cond=True):
     """Frame schedule of reenact_avatar_next3d.py:125-160 for a driving directory (dataset.json + NNN.png / NNN.obj / NNN_kpt2d.txt):
@@ -209,13 +380,36 @@ def reenact_frames(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_
     in order.  Meshes are parsed by the native parsers on worker threads (inputs.FramePrefetcher, pinned memory) while the GPU renders
     batches of `batch` frames; `fixed_camera` [1, 25] replaces the per-frame cameras (the script's --fixed_camera).
     A `.n3dpack` file written by inputs.write_frame_pack can be given instead of a directory (no parsing at all).  image_mode as in
-    render_frames."""
+    render_frames; for noise_mode 'const' / 'none' the first batch caches the ws-only backbones and the later ones reuse them."""
     n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers)
-    if n == 0:
-        return
-    wsf = ws.detach().cpu().float().reshape(1, *ws.shape[-2:]).expand(n, -1, -1)
-    yield from _render_frames(G, wsf, cams, frames(0, n), batch, image_mode, noise_mode, None, seed, sampler_noise,
-                              noise_mode in ('const', 'none'))
+    device = next(G.parameters()).device
+    plan = local_plan(n, batch)
+    yield from _to_host(_steps(plan, _reenact_step(G, plan, ws, cams, frames, image_mode, noise_mode, device, seed, sampler_noise)),
+                        device)
+
+
+def reenact_frames_sharded(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=0,
+                           sampler_noise=None, image_mode='image', out=None, device=None, prefetch_depth=8, workers=4):
+    """reenact_frames over the GPUs of a box (one process per GPU, as render_frames_sharded): every rank computes the frame schedule
+    (reenact_schedule, or the pack's cameras), parses -- or reads from the memory-mapped `.n3dpack` -- only the meshes of its own
+    contiguous frame range, and renders them in batches; for noise_mode 'const' / 'none' its first batch caches the ws-only backbones
+    and the later ones reuse them.  The uint8 frames are gathered to rank 0 as in render_frames_sharded.
+    -> [F, H, W, 3] uint8 host tensor on rank 0 (F = the schedule's frame count; H = W = G.img_resolution for 'image', the neural
+    rendering resolution for 'image_raw' / 'image_depth'), None elsewhere.  `sampler_noise` rows are indexed by the global frame id;
+    image_mode and `batch` as in reenact_frames / render_frames_sharded."""
+    device = device or next(G.parameters()).device
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers)
+    plan = shard_plan(n, batch)
+    step = _reenact_step(G, plan, ws, cams, frames, image_mode, noise_mode, device, seed, sampler_noise)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, step, res, res, device, out)
+
+
+def _reenact_step(G, plan, ws, cams, frames, image_mode, noise_mode, device, seed, sampler_noise):
+    """step(k, idx) of the reenactment drivers: _frames_step of the identity ws with the meshes of this rank's driving frames."""
+    ws = ws.detach().to(device, torch.float32).reshape(1, *ws.shape[-2:])
+    return _frames_step(G, plan, ws, cams, _in_order(plan, frames), image_mode, noise_mode, device, seed, sampler_noise,
+                        noise_mode in ('const', 'none'))
 
 
 def _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=False):
@@ -309,18 +503,6 @@ def _whole_frames(cell_batches, gw, gh):
             yield layout_cells(cur[:nf * per], gw, gh), nf
 
 
-def _grid_schedule(G, ws_grid, w_frames, device):
-    """(latents [F * cells, L, D] on the device, cameras [F * cells, 25]) of a grid video, image f * cells + cell: every cell
-    interpolates its own keyframes (interpolate_ws_device: cubic, 2 wraps), every cell of frame f has the frame's orbit camera
-    (gen_videos_next3d.py:128-144)."""
-    gh, gw, K = ws_grid.shape[:3]
-    F = K * w_frames
-    wsf = torch.stack([interpolate_ws_device(ws_grid[yi, xi].to(device), w_frames) for yi in range(gh) for xi in range(gw)], 1)
-    rk = G.rendering_kwargs
-    cams = orbit_camera_params(F, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
-    return wsf.reshape(F * gh * gw, *wsf.shape[2:]), cams.repeat_interleave(gh * gw, 0)
-
-
 def render_grid_frames(G, ws_grid, verts, w_frames, batch=8, image_mode='image', seed=None, sampler_noise=None):
     """gen_videos_next3d.py:77-171 with `--grid=WxH`: yield one uint8 HWC numpy frame [gh * R, gw * R, 3] per frame of the video
     (F = K * w_frames frames for ws_grid [gh, gw, K, L, D] from grid_keyframes), laid out like the script's layout_grid.  Cell
@@ -331,16 +513,47 @@ def render_grid_frames(G, ws_grid, verts, w_frames, batch=8, image_mode='image',
     render_frames; `sampler_noise=(u_coarse [F * cells, M, Dc, 1], u_fine [F * cells, M, Df])` rows are indexed by the global
     image id f * gh * gw + yi * gw + xi."""
     device = next(G.parameters()).device
-    gh, gw = ws_grid.shape[:2]
-    wsf, cams = _grid_schedule(G, ws_grid, w_frames, device)
-    v = verts.to(device, torch.float32).reshape(1, *verts.shape[-2:]).expand(batch, -1, -1)
+    gh, gw, K = ws_grid.shape[:3]
+    plan = local_plan(K * w_frames * gh * gw, batch)                                # batches of images
+    step = _grid_step(G, plan, ws_grid, verts, w_frames, image_mode, device, seed, sampler_noise)
+    yield from _to_host(_whole_frames(_steps(plan, step), gw, gh), device)
 
-    def cells():
-        for idx, n, kw in _batches(wsf.shape[0], batch, seed, sampler_noise):
-            out = G.synthesis(wsf[idx], cams[idx].to(device, torch.float32, non_blocking=True), v, noise_mode='const',
-                              **_depth_kw(image_mode, device), **kw)
-            yield _frames_u8(out, image_mode), n
-    yield from _to_host(_whole_frames(cells(), gw, gh), device)
+
+def render_grid_frames_sharded(G, ws_grid, verts, w_frames, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None,
+                               device=None):
+    """render_grid_frames over the GPUs of a box (one process per GPU, as render_frames_sharded), sharded by frame: all cells of a
+    frame render on one rank, plan.batch frames (batch // cells as the bound, at least 1) of gh * gw cells per synthesis call.
+    -> [F, gh * R, gw * R, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the global image id
+    f * gh * gw + cell, so the frames do not depend on the number of ranks."""
+    device = device or next(G.parameters()).device
+    gh, gw, K = ws_grid.shape[:3]
+    cells = gh * gw
+    plan = shard_plan(K * w_frames, max(1, batch // cells))                        # batches of frames
+    images = _grid_step(G, plan, ws_grid, verts, w_frames, image_mode, device, seed, sampler_noise)
+
+    def step(k, idx):
+        return layout_cells(images(k, [f * cells + j for f in idx for j in range(cells)]), gw, gh)
+    res = _frame_resolution(G, image_mode)
+    return _gather_frames(plan, step, gh * res, gw * res, device, out)
+
+
+def _grid_step(G, plan, ws_grid, verts, w_frames, image_mode, device, seed, sampler_noise):
+    """The schedule of a grid video, image f * cells + cell: every cell interpolates its own keyframes (interpolate_ws_device: cubic,
+    2 wraps), every cell of frame f has the frame's orbit camera (gen_videos_next3d.py:128-144).  -> step(k, ids): the uint8 cells
+    [len(ids), R, R, 3] of the global image ids, one synthesis call."""
+    gh, gw, K = ws_grid.shape[:3]
+    F = K * w_frames
+    wsf = torch.stack([interpolate_ws_device(ws_grid[yi, xi].to(device), w_frames) for yi in range(gh) for xi in range(gw)], 1)
+    wsf = wsf.reshape(F * gh * gw, *wsf.shape[2:])
+    rk = G.rendering_kwargs
+    cams = orbit_camera_params(F, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius']).repeat_interleave(gh * gw, 0)
+    v = verts.to(device, torch.float32).reshape(1, *verts.shape[-2:])
+
+    def step(k, ids):
+        out = G.synthesis(wsf[ids], cams[ids].to(device, torch.float32, non_blocking=True), v.expand(len(ids), -1, -1),
+                          noise_mode='const', **_depth_kw(image_mode, device), **_sampler_kw(seed, sampler_noise, plan.step_id(k), ids))
+        return _frames_u8(out, image_mode)
+    return step
 
 
 def photo_cell(photo, device):
@@ -358,33 +571,6 @@ def _check_reenact_grid(G, S, grid):
         raise ValueError(f'a reenactment grid needs img_resolution 512 (the photo cell is a 512x512 crop), got {G.img_resolution}')
 
 
-def _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, cache, grid, device):
-    """uint8 frames [m, gh * 512, gw * 512, 3] of the m = len(items) frames of one batch: items are (mesh [1, V, 3], photo) pairs,
-    c [k, 25] their cameras padded to k >= m by repeating the last.  The batch holds S heads x k frames, head-major (image n is head
-    n // k).  noise_mode 'const' / 'none': the S heads' ws-only backbones come from the engine's cache (filled first when `cache`)."""
-    k, m = c.shape[0], len(items)
-    meshes = [t for t, _ in items]
-    v = torch.cat(meshes + [meshes[-1]] * (k - m), 0).to(device, torch.float32, non_blocking=True)
-    if noise_mode in ('const', 'none'):
-        if cache:
-            G.synthesis(wsd, c[:1].expand(S, -1), v[:1].expand(S, -1, -1), noise_mode=noise_mode, cache_backbone=True, seed=0)
-        kw = dict(kw, use_cached_backbone=True)
-    out = G.synthesis(wsb, c.repeat(S, 1), v.repeat(S, 1, 1), noise_mode=noise_mode, **kw)
-    av = _frames_u8(out, 'image')
-    av = av.reshape(S, k, *av.shape[1:])[:, :m].transpose(0, 1)                            # [m, S, H, W, 3]
-    photos = torch.stack([photo_cell(p, device) for _, p in items])[:, None]
-    cells = torch.cat([photos, av], 1)
-    return layout_cells(cells.reshape(-1, *cells.shape[2:]), *grid)
-
-
-def _reenact_grid_kw(seed_kw, sampler_noise, idx, S):
-    """Sampler keywords of a reenactment-grid batch of frames idx: rows f * S + s of sampler_noise, head-major like the batch."""
-    kw = dict(seed_kw)
-    if sampler_noise is not None:
-        kw['sampler_noise'] = _noise_rows(sampler_noise, [f * S + s for s in range(S) for f in idx])
-    return kw
-
-
 def reenact_grid_frames(G, ws, drive_root, num_frames, grid, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=None,
                         sampler_noise=None, prefetch_depth=8, workers=4):
     """reenact_avatar_next3d.py:116-167 with several seeds and `--grid=WxH`: one mesh drives S identities ws [S, L, D]; every frame is
@@ -395,48 +581,12 @@ def reenact_grid_frames(G, ws, drive_root, num_frames, grid, batch=8, lms_cond=T
     noise_mode 'const' / 'none' the S heads' ws-only backbones are computed once and every batch reuses them (use_cached_backbone),
     with 'random' every batch runs the full path.  `seed`: batch b draws sampler seed seed + b; `sampler_noise=(u_coarse
     [F * S, M, Dc, 1], u_fine [F * S, M, Df])` rows are indexed f * S + s (frame f, identity s)."""
-    S = ws.shape[0]
-    _check_reenact_grid(G, S, grid)
+    _check_reenact_grid(G, ws.shape[0], grid)
     n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=True)
-    if n == 0:
-        return
     device = next(G.parameters()).device
-    k = max(1, batch // S)
-    wsd = ws.detach().to(device, torch.float32).reshape(S, *ws.shape[-2:])
-    wsb = wsd.repeat_interleave(k, 0)
-    it = iter(frames(0, n))
-
-    def batches():
-        for b0 in range(0, n, k):
-            m = min(k, n - b0)
-            items = [next(it) for _ in range(m)]
-            idx = list(range(b0, b0 + m)) + [b0 + m - 1] * (k - m)
-            kw = _reenact_grid_kw({} if seed is None else {'seed': int(seed) + b0 // k}, sampler_noise, idx, S)
-            c = cams[idx].to(device, torch.float32, non_blocking=True)
-            yield _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, b0 == 0, grid, device), m
-    yield from _to_host(batches(), device)
-
-
-def render_grid_frames_sharded(G, ws_grid, verts, w_frames, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None,
-                               device=None):
-    """render_grid_frames over the GPUs of a box (one process per GPU, as render_frames_sharded), sharded by frame: all cells of a
-    frame render on one rank, plan.batch frames (batch // cells as the bound, at least 1) of gh * gw cells per synthesis call.
-    -> [F, gh * R, gw * R, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the global image id
-    f * gh * gw + cell, so the frames do not depend on the number of ranks."""
-    device = device or next(G.parameters()).device
-    gh, gw = ws_grid.shape[:2]
-    cells = gh * gw
-    wsf, cams = _grid_schedule(G, ws_grid, w_frames, device)
-    plan = shard_plan(wsf.shape[0] // cells, max(1, batch // cells))
-    v = verts.to(device, torch.float32).reshape(1, *verts.shape[-2:]).expand(plan.batch * cells, -1, -1)
-
-    def step(k, idx):
-        ids = [f * cells + j for f in idx for j in range(cells)]
-        out_ = G.synthesis(wsf[ids], cams[ids].to(device, torch.float32, non_blocking=True), v, noise_mode='const',
-                           **_depth_kw(image_mode, device), **_shard_sampler(plan, k, ids, seed, sampler_noise))
-        return layout_cells(_frames_u8(out_, image_mode), gw, gh)
-    res = _frame_resolution(G, image_mode)
-    return _gather_frames(plan, step, gh * res, gw * res, device, out)
+    plan = local_plan(n, max(1, batch // ws.shape[0]))
+    step = _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, sampler_noise)
+    yield from _to_host(_steps(plan, step), device)
 
 
 def reenact_grid_frames_sharded(G, ws, drive_root, num_frames, grid, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const',
@@ -444,212 +594,39 @@ def reenact_grid_frames_sharded(G, ws, drive_root, num_frames, grid, batch=8, lm
     """reenact_grid_frames over the GPUs of a box, sharded by frame as reenact_frames_sharded (each rank parses the meshes and decodes
     the photos of its own frames only; plan.batch frames of S heads per call, batch // S as the bound).  -> [F, gh * 512, gw * 512, 3]
     uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed f * S + s by the global frame id f."""
-    S = ws.shape[0]
-    _check_reenact_grid(G, S, grid)
+    _check_reenact_grid(G, ws.shape[0], grid)
     device = device or next(G.parameters()).device
     n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=True)
-    plan = shard_plan(n, max(1, batch // S))
-    wsd = ws.detach().to(device, torch.float32).reshape(S, *ws.shape[-2:])
-    wsb = wsd.repeat_interleave(plan.batch, 0)
-    src = None
-    if n > 0:
-        first = plan.frames(0)[0]                                          # a rank without frames repeats the previous rank's last
-        src = _InOrder(frames(first, max(plan.spans[plan.rank][1], first + 1)), first)
-
-    def step(k, idx):
-        items = src.take(idx)
-        kw = _reenact_grid_kw(_shard_sampler(plan, k, idx, seed, None), sampler_noise, idx, S)
-        c = cams[idx].to(device, torch.float32, non_blocking=True)
-        return _reenact_grid_batch(G, wsd, wsb, S, items, c, noise_mode, kw, k == 0, grid, device)
+    plan = shard_plan(n, max(1, batch // ws.shape[0]))
+    step = _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, sampler_noise)
     gw, gh = grid
     return _gather_frames(plan, step, gh * 512, gw * 512, device, out)
 
 
-def render_frames_sharded(G, ws_frames, cams, verts, batch=8, noise_mode='const', seed=0, device=None, out=None, sampler_noise=None):
-    """Strong-scaling video driver (BASELINE.json configs[3]: one clip split over the GPUs of a box): rank r renders the contiguous
-    frame range shard_range(F, r, world) in batches through `G.synthesis`, converts to uint8 HWC on the device (4x fewer bytes than
-    the fp32 images) and the batches are gathered to rank 0 over NCCL on a side stream from a ping-pong staging buffer, so batch
-    i+1 renders while batch i is in flight; rank 0 copies every gathered batch to pinned host memory on a third stream.
-    Returns the [F, H, W, 3] uint8 host tensor (frame order) on rank 0, None elsewhere, filled in stream order (synchronise the
-    current stream before reading it).  World size 1: no collective.
-    `batch` is an upper bound: the per-call batch is the size in [batch/2, batch] that pads the rank's frame count least (30 frames per
-    rank -> 5 batches of 6, not 4 of 8).  `out`: optional pinned [F, H, W, 3] uint8 host tensor to fill on rank 0 (pinning 190 MB per
-    clip costs tens of milliseconds).  `sampler_noise`: per-frame uniforms as in render_frames, rows indexed by the global frame id,
-    so the frames do not depend on the number of ranks (batch k of rank r otherwise draws sampler seed seed + r * steps + k)."""
-    device = device or next(G.parameters()).device
-    plan = shard_plan(ws_frames.shape[0], batch)
-    static_mesh = verts.shape[0] == 1
+def _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, sampler_noise):
+    """step(k, idx): the uint8 grid frames [len(idx), gh * 512, gw * 512, 3] of the driving frames idx.  One synthesis call renders
+    the S heads x len(idx) frames, head-major (image n is head n // len(idx)); noise_mode 'const' / 'none': the S heads' ws-only
+    backbones come from the engine's cache, filled by the first step."""
+    S = ws.shape[0]
+    wsd = ws.detach().to(device, torch.float32).reshape(S, *ws.shape[-2:])
+    wsb = wsd.repeat_interleave(plan.batch, 0)
+    src = _in_order(plan, frames)
 
     def step(k, idx):
-        w = ws_frames[idx].to(device, torch.float32, non_blocking=True)
+        items = src.take(idx)                                                      # (mesh [1, V, 3], photo) pairs
         c = cams[idx].to(device, torch.float32, non_blocking=True)
-        v = verts.to(device, torch.float32).expand(plan.batch, -1, -1) if static_mesh else verts[idx].to(device, torch.float32, non_blocking=True)
-        return G.synthesis(w, c, v, noise_mode=noise_mode, **_shard_sampler(plan, k, idx, seed, sampler_noise))
-    res = G.img_resolution
-    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), 'image'), res, res, device, out)
-
-
-def reenact_frames_sharded(G, ws, drive_root, num_frames, batch=8, lms_cond=True, fixed_camera=None, noise_mode='const', seed=0,
-                           sampler_noise=None, image_mode='image', out=None, device=None, prefetch_depth=8, workers=4):
-    """reenact_frames over the GPUs of a box (one process per GPU, as render_frames_sharded): every rank computes the frame schedule
-    (reenact_schedule, or the pack's cameras), parses -- or reads from the memory-mapped `.n3dpack` -- only the meshes of its own
-    contiguous frame range, and renders them in batches; for noise_mode 'const' / 'none' its first batch caches the ws-only backbones
-    and the later ones reuse them.  The uint8 frames are gathered to rank 0 as in render_frames_sharded.
-    -> [F, H, W, 3] uint8 host tensor on rank 0 (F = the schedule's frame count; H = W = G.img_resolution for 'image', the neural
-    rendering resolution for 'image_raw' / 'image_depth'), None elsewhere.  `sampler_noise` rows are indexed by the global frame id;
-    image_mode and `batch` as in reenact_frames / render_frames_sharded."""
-    device = device or next(G.parameters()).device
-    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers)
-    plan = shard_plan(n, batch)
-    wsd = ws.detach().to(device, torch.float32).reshape(1, *ws.shape[-2:]).expand(plan.batch, -1, -1)
-    reuse = noise_mode in ('const', 'none')
-    mesh = None
-    if n > 0:
-        first = plan.frames(0)[0]                                          # a rank without frames repeats the previous rank's last
-        mesh = _InOrder(frames(first, max(plan.spans[plan.rank][1], first + 1)), first)
-
-    def step(k, idx):
-        c = cams[idx].to(device, torch.float32, non_blocking=True)
-        v = torch.cat(mesh.take(idx), 0).to(device, torch.float32, non_blocking=True)
-        kw = _shard_sampler(plan, k, idx, seed, sampler_noise)
-        if reuse:
-            kw['use_cached_backbone' if k else 'cache_backbone'] = True
-        return G.synthesis(wsd, c, v, noise_mode=noise_mode, **_depth_kw(image_mode, device), **kw)
-    res = _frame_resolution(G, image_mode)
-    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), image_mode), res, res, device, out)
-
-
-def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0, sampler_noise=None, out=None, device=None):
-    """render_orbit over the GPUs of a box: every rank computes the head's planes once (ws [1, L, D], mesh verts [1, V, 3]) and
-    renders its contiguous range of the cameras cams [F, 25] with G.render_views; the frames are gathered to rank 0 as in
-    render_frames_sharded.  -> [F, H, W, 3] uint8 host tensor on rank 0, None elsewhere.  `sampler_noise` rows are indexed by the
-    global frame id."""
-    device = device or next(G.parameters()).device
-    plan = shard_plan(cams.shape[0], batch)
-    G.synthesis(ws.to(device, torch.float32), cams[:1].to(device, torch.float32), verts.to(device, torch.float32), noise_mode='const',
-                cache_backbone=True, seed=0)
-
-    def step(k, idx):
-        return G.render_views(cams[idx].to(device, torch.float32, non_blocking=True), **_depth_kw(image_mode, device),
-                              **_shard_sampler(plan, k, idx, seed, sampler_noise))
-    res = _frame_resolution(G, image_mode)
-    return _gather_frames(plan, lambda k, idx: _frames_u8(step(k, idx), image_mode), res, res, device, out)
-
-
-class ShardPlan(NamedTuple):
-    """How F frames are split over the ranks of the sharded drivers: rank r owns spans[r] = shard_range(F, r, world) and renders it
-    in `steps` batches of `batch` frames; every rank runs the same number of steps (one collective each)."""
-    rank: int
-    world: int
-    spans: list
-    batch: int
-    steps: int
-
-    def frames(self, k):
-        """Global frame ids of this rank's batch k; a short tail repeats the last frame (one graph shape)."""
-        a, b = self.spans[self.rank]
-        lo = min(a + k * self.batch, max(b - 1, a))
-        return [min(lo + j, b - 1) for j in range(self.batch)]
-
-
-def shard_plan(F, batch):
-    """The ShardPlan of F frames for this process's rank in the current torch.distributed world (world 1 when uninitialised).
-    `batch` is an upper bound: the batch is the size in [batch/2, batch] that pads the largest rank's frame count least."""
-    import torch.distributed as dist
-    from . import distributed as D
-    world = dist.get_world_size() if dist.is_initialized() else 1
-    rank = dist.get_rank() if dist.is_initialized() else 0
-    spans = [D.shard_range(F, r, world) for r in range(world)]
-    nmax = max(e - s for s, e in spans)
-    batch = min(range(max(1, batch // 2), batch + 1), key=lambda bb: (-(-nmax // bb) * bb, -bb))     # least padding, then the largest
-    return ShardPlan(rank, world, spans, batch, -(-nmax // batch))
-
-
-def _shard_sampler(plan, k, idx, seed, sampler_noise):
-    """Sampler keywords of batch k of a sharded driver: the frames' global rows of sampler_noise, else seed + rank * steps + k."""
-    if sampler_noise is not None:
-        return {'sampler_noise': _noise_rows(sampler_noise, idx)}
-    return {'seed': int(seed) + plan.rank * plan.steps + k}
-
-
-def _frame_resolution(G, image_mode):
-    return G.img_resolution if image_mode == 'image' else G.neural_rendering_resolution
-
-
-class _InOrder:
-    """Items (meshes [1, V, 3], or (mesh, photo) pairs) of consecutive frames first, first + 1, ... from an in-order iterable, looked
-    up by frame id as the sharded batches advance (each id is read once; ids behind the current batch are dropped)."""
-
-    def __init__(self, frames, first):
-        self.it, self.next, self.have = iter(frames), first, {}
-
-    def take(self, idx):
-        while self.next <= max(idx):
-            self.have[self.next] = next(self.it)
-            self.next += 1
-        self.have = {i: t for i, t in self.have.items() if i >= min(idx)}
-        return [self.have[i] for i in idx]
-
-
-def _gather_frames(plan, step, H, W, device, out):
-    """The loop of the sharded drivers: for k in range(plan.steps), step(k, plan.frames(k)) renders this rank's batch k and returns
-    its uint8 frames [plan.batch, H, W, 3]; they go to a ping-pong staging buffer, are gathered to rank 0 over NCCL on a side stream
-    (world > 1) and copied to pinned host memory on a third stream, so the next batch renders while this one is in flight.
-    -> [F, H, W, 3] uint8 host tensor on rank 0 (`out` if given), None elsewhere.  It is filled in stream order: the caller's
-    current stream waits for the last copy, so synchronise that stream before reading the frames (back-to-back clips do not stall).
-    A CPU `device` (host-side tests under gloo) runs the same loop without streams."""
-    import contextlib
-    import torch.distributed as dist
-    rank, world, spans, batch = plan.rank, plan.world, plan.spans, plan.batch
-    cuda = torch.device(device).type == 'cuda'
-    host = None
-    if rank == 0:
-        host = out if out is not None else torch.empty(spans[-1][1], H, W, 3, dtype=torch.uint8, pin_memory=cuda)
-    main = torch.cuda.current_stream(device) if cuda else None
-    side, copy_s = (torch.cuda.Stream(device), torch.cuda.Stream(device)) if cuda else (None, None)
-
-    def on(stream):
-        return torch.cuda.stream(stream) if cuda else contextlib.nullcontext()
-
-    def record(stream):
-        if not cuda:
-            return None
-        ev = torch.cuda.Event()
-        ev.record(stream)
-        return ev
-    stage = [torch.empty(batch, H, W, 3, dtype=torch.uint8, device=device) for _ in range(2)]
-    gath = [torch.empty(world, batch, H, W, 3, dtype=torch.uint8, device=device) if rank == 0 and world > 1 else None for _ in range(2)]
-    drained = [None, None]
-    for k in range(plan.steps):
-        frames = step(k, plan.frames(k))
-        s = k & 1
-        if drained[s] is not None:
-            main.wait_event(drained[s])                                    # batch k-2 has left this staging buffer
-        stage[s].copy_(frames)
-        if cuda:
-            side.wait_stream(main)
-        with on(side):
-            if world > 1:
-                dist.gather(stage[s], list(gath[s].unbind(0)) if rank == 0 else None, dst=0)
-            ev = record(side)
-        drained[s] = ev
-        if rank == 0:
-            if cuda:
-                copy_s.wait_event(ev)
-            with on(copy_s):
-                for r in range(world):
-                    s0, e0 = spans[r]
-                    f0 = s0 + k * batch
-                    n = max(0, min(batch, e0 - f0))
-                    if n > 0:
-                        src = gath[s][r] if world > 1 else stage[s]
-                        host[f0:f0 + n].copy_(src[:n], non_blocking=cuda)
-                ev2 = record(copy_s)
-            drained[s] = ev2                                               # the staging / gather buffers are free once the D2H left them
-    if cuda:
-        main.wait_stream(side)
-        main.wait_stream(copy_s)
-    return host
+        v = torch.cat([mesh for mesh, _ in items], 0).to(device, torch.float32, non_blocking=True)
+        kw = _sampler_kw(seed, sampler_noise, plan.step_id(k), [f * S + s for s in range(S) for f in idx])
+        if noise_mode in ('const', 'none'):
+            if k == 0:
+                G.synthesis(wsd, c[:1].expand(S, -1), v[:1].expand(S, -1, -1), noise_mode=noise_mode, cache_backbone=True, seed=0)
+            kw['use_cached_backbone'] = True
+        av = _frames_u8(G.synthesis(wsb, c.repeat(S, 1), v.repeat(S, 1, 1), noise_mode=noise_mode, **kw), 'image')
+        av = av.reshape(S, len(idx), *av.shape[1:]).transpose(0, 1)                   # [len(idx), S, H, W, 3]
+        photos = torch.stack([photo_cell(p, device) for _, p in items])[:, None]
+        cells = torch.cat([photos, av], 1)
+        return layout_cells(cells.reshape(-1, *cells.shape[2:]), *grid)
+    return step
 
 
 # ------------------------------------------------------------------------------------------------ shape extraction (row f2)
@@ -765,32 +742,6 @@ def _check_sheets(G, ws, v, batch, shape_res):
     return max(1, batch // 3)
 
 
-def _sheet_noise(sampler_noise, idx):
-    """sampler_noise keywords of the caching call (yaw +0.4 of heads idx) and of the render_views call (yaws 0, -0.4, view n of head
-    idx[n // 2]): rows 3 i + yaw of the per-image uniforms."""
-    if sampler_noise is None:
-        return {}, {}
-    return ({'sampler_noise': _noise_rows(sampler_noise, [3 * i for i in idx])},
-            {'sampler_noise': _noise_rows(sampler_noise, [3 * i + 1 + j for i in idx for j in range(2)])})
-
-
-def _sheet_batch(G, ws, idx, n, cams, v, kws, shapes, shape_res, device):
-    """(uint8 sheets [len(idx), H, 3 W, 3], float32 density grids [n, R, R, R] or None) of the heads ws[idx], of which the first n are
-    wanted: one caching synthesis call renders yaw +0.4 and keeps the heads, one render_views call renders the other two yaws from the
-    cached planes, and each wanted head's grid is decoded from its cached planes."""
-    B = len(idx)
-    w = ws[idx].to(device, torch.float32, non_blocking=True)
-    front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True, **kws[0])['image']
-    sheets = sheet_u8(front, G.render_views(cams[1:].repeat(B, 1), **kws[1])['image'])
-    if not shapes:
-        return sheets, None
-    sigmas = torch.empty(n, shape_res, shape_res, shape_res, device=device)
-    eng = G._get_engine()
-    for b in range(n):
-        eng.cached_sigma_grid(b, shape_res, sigmas[b])
-    return sheets, sigmas
-
-
 def render_sample_sheets(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=None, sampler_noise=None):
     """gen_samples_next3d.py:182-238 for the seeds of ws [S, 28, 512] (sample_sheet_ws) and one mesh v [1, V, 3]: yields
     (i, sheet, sigmas) in seed order.  sheet: uint8 [H, 3 W, 3] numpy, the script's three yaws side by side (sheet_u8);
@@ -802,27 +753,17 @@ def render_sample_sheets(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_
     G.use_cuda_graph (and no sampler_noise) the calls replay CUDA graphs.  The driver replaces whatever heads the generator had cached.
     `seed`: step k draws sampler seeds seed + 2 k (synthesis) and seed + 2 k + 1 (render_views); None = fresh random seeds.
     `sampler_noise=(u_coarse [3 S, M, Dc, 1], u_fine [3 S, M, Df])` rows are indexed by the global image id 3 i + yaw (yaw 0, 1, 2 =
-    +0.4, 0, -0.4).  ValueError, before any device work, for an empty or misshapen ws, batch < 1, shape_res < 2 or a v batch other
-    than 1."""
+    +0.4, 0, -0.4), in place of `seed`.  ValueError, before any device work, for an empty or misshapen ws, batch < 1, shape_res < 2
+    or a v batch other than 1."""
     B = _check_sheets(G, ws, v, batch, shape_res)
-    return _sample_sheets(G, ws, v, fov_deg, B, shapes, shape_res, seed, sampler_noise)
-
-
-def _sample_sheets(G, ws, v, fov_deg, B, shapes, shape_res, seed, sampler_noise):
     device = next(G.parameters()).device
-    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
-    v = v.to(device, torch.float32)
+    plan = local_plan(ws.shape[0], B)
+    sheets = _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise)
 
-    def steps():
-        for k, (idx, n, _) in enumerate(_batches(ws.shape[0], B, None, None)):
-            kws = _sheet_noise(sampler_noise, idx)
-            if seed is not None:
-                kws[0]['seed'], kws[1]['seed'] = int(seed) + 2 * k, int(seed) + 2 * k + 1
-            sheets, sigmas = _sheet_batch(G, ws, idx, n, cams, v, kws, shapes, shape_res, device)
-            yield ((sheets, sigmas) if shapes else sheets), n
-    for i, item in enumerate(_to_host(steps(), device)):
-        sheet, sigmas = item if shapes else (item, None)
-        yield i, sheet, sigmas
+    def step(k, idx):
+        u8, _, sigmas = sheets(k, idx)
+        return (u8, sigmas) if shapes else u8
+    return ((i, *(item if shapes else (item, None))) for i, item in enumerate(_to_host(_steps(plan, step), device)))
 
 
 def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=0, sampler_noise=None, out=None,
@@ -838,26 +779,45 @@ def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False
     device = device or next(G.parameters()).device
     cuda = torch.device(device).type == 'cuda'
     plan = shard_plan(ws.shape[0], B)
-    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
-    v = v.to(device, torch.float32)
-    lo, hi = plan.spans[plan.rank]
+    sheets = _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise)
     grids = {}
 
     def step(k, idx):
-        kws = _sheet_noise(sampler_noise, idx)
-        if sampler_noise is None:
-            s = int(seed) + 2 * (plan.rank * plan.steps + k)
-            kws[0]['seed'], kws[1]['seed'] = s, s + 1
-        # this rank's seeds without a grid yet: a prefix of idx (a short tail repeats the last seed, a rank past its span repeats a
-        # seed it has done, a rank without seeds repeats the previous rank's last)
-        new = [i for i in dict.fromkeys(idx) if lo <= i < hi and i not in grids] if shapes else []
-        sheets, sigmas = _sheet_batch(G, ws, idx, len(new), cams, v, kws, bool(new), shape_res, device)
+        u8, new, sigmas = sheets(k, idx)
         for b, i in enumerate(new):
             grids[i] = torch.empty(sigmas[b].shape, pin_memory=cuda)
             grids[i].copy_(sigmas[b], non_blocking=cuda)
-        return sheets
+        return u8
     res = G.img_resolution
     host = _gather_frames(plan, step, res, 3 * res, device, out)
     if cuda and grids:
         torch.cuda.current_stream(device).synchronize()
     return host, {i: g.numpy() for i, g in grids.items()}
+
+
+def _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise):
+    """step(k, idx) -> (uint8 sheets [len(idx), H, 3 W, 3], new, float32 density grids [len(new), R, R, R] or None) of the heads
+    ws[idx]: one caching synthesis call renders yaw +0.4 and keeps the heads, one render_views call renders the other two yaws from
+    the cached planes (view n of head idx[n // 2]), and with `shapes` the grid of each head in `new` -- this rank's heads of the step
+    that have none yet -- is decoded from its cached planes.  Noise rows 3 i + yaw of the per-image uniforms."""
+    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
+    v = v.to(device, torch.float32)
+    lo, hi = plan.spans[plan.rank]
+    done = set()
+
+    def step(k, idx):
+        B, s = len(idx), 2 * plan.step_id(k)
+        w = ws[idx].to(device, torch.float32, non_blocking=True)
+        front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True,
+                            **_sampler_kw(seed, sampler_noise, s, [3 * i for i in idx]))['image']
+        views = G.render_views(cams[1:].repeat(B, 1), **_sampler_kw(seed, sampler_noise, s + 1,
+                                                                    [3 * i + 1 + j for i in idx for j in range(2)]))['image']
+        # a prefix of idx: a short tail repeats the last head, a rank past its span repeats a head it has done, a rank without heads
+        # repeats the previous rank's last
+        new = [i for i in dict.fromkeys(idx) if lo <= i < hi and i not in done] if shapes else []
+        done.update(new)
+        sigmas = torch.empty(len(new), shape_res, shape_res, shape_res, device=device) if new else None
+        for b in range(len(new)):
+            G._get_engine().cached_sigma_grid(b, shape_res, sigmas[b])
+        return sheet_u8(front, views), new, sigmas
+    return step

@@ -98,6 +98,10 @@ def test_shard_plan_world_1():
     assert p.batch == 1 and p.steps == 5
     p = drivers.shard_plan(7, 4)
     assert (p.batch, p.steps) == (4, 2) and p.frames(1) == [4, 5, 6, 6]          # the tail repeats the last frame
+    assert [p.valid(k) for k in range(2)] == [4, 3] and [p.step_id(k) for k in range(2)] == [0, 1]
+    p = drivers.local_plan(7, 3)                                                # the single-process run: exactly `batch` per step
+    assert (p.rank, p.world, p.batch, p.steps) == (0, 1, 3, 3) and p.frames(2) == [6, 6, 6] and p.valid(2) == 1
+    assert drivers.local_plan(0, 3).steps == 0
 
 
 def _worker(rank, world, port, F, batch, pack, q):
