@@ -66,8 +66,8 @@ static EncodeTiledFn lookup_encode_tiled() {
     return (EncodeTiledFn)p;
 }
 
-int n3d_encode_tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box,
-                         CUtensorMapSwizzle swizzle, const char* who) {
+int n3d_encode_tmap(CUtensorMap* tm, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                    const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who) {
     static const EncodeTiledFn enc = lookup_encode_tiled();     // looked up once; initialisation of a static is thread-safe
     if (!enc) {
         n3d_set_error("%s: cuTensorMapEncodeTiled unavailable (no CUDA driver?)", who);
@@ -79,7 +79,7 @@ int n3d_encode_tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint
         gdim[i] = dims[i]; bdim[i] = box[i]; estr[i] = 1;
         if (i < rank - 1) gstr[i] = strides[i];
     }
-    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
+    const CUresult r = enc(tm, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
                            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         n3d_set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d", who, (int)r);

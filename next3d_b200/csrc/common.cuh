@@ -45,11 +45,11 @@ N3DDeviceState* n3d_device_state(void);      // api.cu; nullptr (+ error message
 // N3D_OK, or N3D_ERR_CUDA with a message that starts with `who`.
 int n3d_smem_optin(const void* kernel, int bytes, const char* who);     // api.cu
 
-// TMA descriptor of a bf16 tensor: `rank` <= 5 dims (innermost first), byte strides of dims 1 .. rank-1, a box of `box` elements
-// per dim, `swizzle` shared-memory layout; reads outside the tensor are zero-filled.  N3D_OK, or N3D_ERR_CUDA with a message that
-// starts with `who`.
-int n3d_encode_tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box,
-                         CUtensorMapSwizzle swizzle, const char* who);     // api.cu
+// TMA descriptor of a tensor of `dtype` elements: `rank` <= 5 dims (innermost first), byte strides of dims 1 .. rank-1, a box of
+// `box` elements per dim, `swizzle` shared-memory layout; loads outside the tensor are zero-filled, stores outside it are skipped.
+// N3D_OK, or N3D_ERR_CUDA with a message that starts with `who`.
+int n3d_encode_tmap(CUtensorMap* tm, CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                    const uint32_t* box, CUtensorMapSwizzle swizzle, const char* who);     // api.cu
 
 // Clusters of `cluster` CTAs (`threads` threads, `smem_bytes` dynamic shared memory each) of `kernel` that the current device
 // runs at once (cudaOccupancyMaxActiveClusters), queried once per (device, kernel): the kernel's occupancy must not depend on

@@ -12,7 +12,8 @@
 //   Warp roles (384 threads, persistent over work items): warps 0-7 = two ping-pong consumer warpgroups; the CTA's work items
 //   alternate between them, and each owns all 128 rows of its tiles: wgmma into a register accumulator (two m64 halves), then the
 //   fused epilogue (demod/noise/bias/lrelu/clamp -> next layer's modulation -> bf16 split / fp32 stores) through a small
-//   shared-memory transpose (thread = tile row, one 64-row half at a time), overlapping the other warpgroup's MMAs.  Warpgroup 2 = TMA
+//   shared-memory transpose (thread = tile row, one 64-row half at a time), overlapping the other warpgroup's MMAs; raw fp32 output
+//   (mode 1) leaves through TMA stores instead (store_raw_tma).  Warpgroup 2 = TMA
 //   producer (one lane), which keeps filling the stage ring during the epilogue.  setmaxnreg lowers the producer to 24 registers
 //   and raises the consumers to 240 (2 x 128 x 240 + 128 x 24 = 384 x 168): ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
 //   Launches with wide tiles run as 2-CTA clusters: the two CTAs take neighbouring M tiles of the same n-tile and K steps, and
@@ -38,8 +39,13 @@ constexpr int kMinTiles = 64;                 // see the block_n choice in launc
 constexpr int kMinTilesSplit = 128;           // same for split-K launches
 constexpr int kStageArrays = 8;               // dcoef | bias | style0 | style1 | up to 4 modulated ToRGB weight rows
 constexpr int kXStride = 36;                  // floats per row of the accumulator transpose buffer (32 columns + pad)
-// per-warpgroup epilogue area: staged vectors | accumulator transpose [64][kXStride] | ToRGB partial sums [64][4]
-constexpr int kEpiBytes = kStageArrays * kMaxBlockN * 4 + 64 * kXStride * 4 + 64 * 4 * 4;
+constexpr int kStoreBoxBytes = 64 * 32 * 4;   // one TMA store box of the raw fp32 output: 64 tile rows x 32 channels
+// Per-warpgroup epilogue area (1024-byte aligned), used one of two ways:
+//   per-thread stores: staged vectors | accumulator transpose [64][kXStride] | ToRGB partial sums [64][4]
+//   TMA stores of the raw output (KParams::tma_store): two store boxes, one being filled while the other is read by the TMA
+constexpr int kThreadEpiBytes = kStageArrays * kMaxBlockN * 4 + 64 * kXStride * 4 + 64 * 4 * 4;
+constexpr int kEpiBytes = kThreadEpiBytes > 2 * kStoreBoxBytes ? kThreadEpiBytes : 2 * kStoreBoxBytes;
+static_assert(kEpiBytes % 1024 == 0, "the store boxes of both warpgroups are SWIZZLE_128B atoms");
 // shared memory left for the stage ring: opt-in maximum - both epilogue areas - barriers - 1024-byte alignment slack
 constexpr int kRingBytes = 227 * 1024 - 2 * kEpiBytes - 1024 - 256;
 constexpr int kMaxSubs = 9;                   // a stride-2 transposed conv: 4 parity-class interiors + 5 edge strips / corner
@@ -69,7 +75,13 @@ struct KParams {
     N3DFusedRgb rgb;                 // optional fused ToRGB (<= 4 image channels), see include/next3d_b200.h
     int oy_mul, ox_mul, OH, OW;
     int* err_flag;
+    // raw fp32 output of each sub-problem (tma_store): dims (Cout, x, y, N, K slice) in the sub-problem's M-space coordinates,
+    // clipped where the per-thread stores test `valid`; box (min(32, block_n), TW, the 64-row half of TH x TN, 1)
+    // (last: placed before the scalar fields, it cost the 128-wide instances spills)
+    CUtensorMap tmC[kMaxSubs];
+    int tma_store;
 };
+static_assert(sizeof(KParams) <= 4096, "KParams is passed as a kernel parameter");
 
 // mode-0 launches always have a single sub-problem
 __device__ __forceinline__ int staged_rgb_channels(const KParams& P) { return (P.rgb.out && P.sub[0].TN == 1 && P.mode == 0 && P.item_tiles == P.tiles_n) ? P.rgb.channels : 0; }
@@ -161,17 +173,61 @@ __device__ __forceinline__ void tile_mainloop(const KParams& P, float (&acc0)[BN
     if (lane == 0) release_stage(P, empty_base + 8u * (uint32_t)prev_s);
 }
 
+// Raw fp32 epilogue (KParams::tma_store): 64-row half h of a tile, min(32, BN) channels at a time, goes from the accumulator
+// fragments into one of the warpgroup's two store boxes (the layout of the tensor map's box, swizzled like it so that the
+// fragment writes do not conflict) and out with one TMA store, which the leader thread issues and commits.  Before the barrier
+// that releases a box to the TMA, the leader waits until the previous box has been read, so the other box may be refilled
+// right after the barrier while this one is read; the global writes stay in flight.  Clipping by the tensor map does what
+// `valid` does in the per-thread stores; pad tiles store nothing.
+template <int BN>
+__device__ __forceinline__ void store_raw_tma(const KParams& P, const float (&acc)[BN / 2], const TileInfo& ti, int h,
+                                              bool leader, int bar_id, uint32_t boxes) {
+    constexpr int BC = BN < 32 ? BN : 32;                  // channels per box
+    constexpr uint32_t kRow = BC * 4;                      // bytes per box row: 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
+    // Fragment element i of this thread: row r = r0 + 8 * ((i >> 1) & 1), 16-byte chunk 2 * ((i >> 2) & 3) + (lane & 3) / 2 of the
+    // box row, 8 bytes in.  The TMA swizzle of a 1024-byte aligned box XORs the chunk index with row address bits 7.. (the same for
+    // r0 and r0 + 8), so the byte offset is sw ^ (((i >> 2) & 3) << 5), plus 8 rows for the second row.
+    // (the thread's position is read here, not passed in: with values derived from it outside the item loop the 128-wide
+    // instances spill)
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t r0 = 16 * (warp & 3) + (lane >> 2);
+    const uint32_t sw = r0 * kRow + ((((uint32_t)(lane & 3) >> 1) ^ ((r0 * kRow >> 7) & (kRow / 16 - 1))) << 4) + (lane & 1) * 8;
+#pragma unroll
+    for (int cc = 0; cc < BN / BC; ++cc) {
+        // a tile fills an even number of boxes, so the two alternate across tiles as well
+        const uint32_t box = boxes + (uint32_t)((h * (BN / BC) + cc) & 1) * (uint32_t)kStoreBoxBytes;
+#pragma unroll
+        for (int e = 0; e < BC / 2; e += 2) {
+            const int i = cc * (BC / 2) + e;
+            const uint32_t off = (sw ^ (uint32_t)(((i >> 2) & 3) << 5)) + (uint32_t)((i >> 1) & 1) * 8u * kRow;
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(box + off), "f"(acc[i]), "f"(acc[i + 1]) : "memory");
+        }
+        fence_proxy_async_smem();
+        if (leader) bulk_wait_read_all();
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        if (leader) {
+            if (!ti.pad) {
+                // the half is the second half of the tile's images, or of its rows when it has one image (TH >= 8 then)
+                const KParams::Sub& S = P.sub[ti.sub];
+                const int y = ti.y0 + (S.TN > 1 ? 0 : h * (S.TH / 2)), n = ti.n0 + (S.TN > 1 ? h * (S.TN / 2) : 0);
+                tma_store_5d(&P.tmC[ti.sub], box, ti.tn * P.block_n + cc * BC, ti.x0, y, n, ti.split);
+            }
+            bulk_commit_group();
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- the kernel
 template <int BN, int BK>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ KParams P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-B aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + (uint32_t)P.stages * (uint32_t)P.stage_bytes;   // 8-byte aligned
-    // barriers: full[stages], empty[stages]; then the two warpgroups' epilogue areas
+    // the stage ring (whole KiB per stage), the two warpgroups' epilogue areas, then the barriers full[stages], empty[stages]
+    const uint32_t epi_base = smem_base + (uint32_t)P.stages * (uint32_t)P.stage_bytes;
+    const uint32_t bar_base = epi_base + 2u * (uint32_t)kEpiBytes;
     auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(P.stages + s); };
-    const uint32_t epi_off = ((bar_base + 8u * (uint32_t)(2 * P.stages) + 15u) & ~15u) - smem_u32(smem_raw);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -241,7 +297,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         const int g = warp >> 2;
         const int gtid = threadIdx.x & 127;                    // thread index inside the warpgroup
         const int xrow = gtid & 63, half = gtid >> 6;          // epilogue: tile row 64h + xrow, columns 16 * half of each 32-column chunk
-        uint8_t* const epi = smem_raw + epi_off + (uint32_t)g * (uint32_t)kEpiBytes;
+        uint8_t* const epi = smem_raw + (epi_base - smem_u32(smem_raw)) + (uint32_t)g * (uint32_t)kEpiBytes;
         float* const stg = reinterpret_cast<float*>(epi);                                   // [kStageArrays][kMaxBlockN]
         float* const xbuf = stg + kStageArrays * kMaxBlockN;                                // [64][kXStride]
         float* const rbuf = xbuf + 64 * kXStride;                                           // [64][4]
@@ -305,6 +361,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             else tile_mainloop<BN, BK, 1>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
             if (tile == (item + 1) * P.item_tiles - 1 && other_item < total_items)
                 asm volatile("bar.arrive %0, 256;" ::"r"(4 - g) : "memory");     // the other warpgroup's next item may start
+            if (P.tma_store) {
+                store_raw_tma<BN>(P, accs[0], ti, 0, gtid == 0, 1 + g, smem_u32(epi));
+                store_raw_tma<BN>(P, accs[1], ti, 1, gtid == 0, 1 + g, smem_u32(epi));
+                continue;
+            }
 
             // ---- epilogue (thread = tile row, 16 columns of each 32-column chunk), two 64-row halves
 #pragma unroll
@@ -502,6 +563,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         if (other_item < total_items) skip_item(other_item);
         item = other_item;
         }
+        if (P.tma_store && gtid == 0) bulk_wait_all();         // the store boxes are read and written before the CTA's memory goes
         // Exit barrier of the cluster: the partner may arrive on this CTA's empty barriers until its consumers are done with
         // their last item, so neither CTA exits before the consumers of both get here.  The producer warpgroup takes no part:
         // its threads exit when they are done, and a cluster barrier waits for the threads that have not exited.  (Its CTA
@@ -617,7 +679,7 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     K.nprod = p->nprod; K.a_img_stride = p->a_img_mul;
     N3DDeviceState* D = n3d_device_state();
     if (!D) return N3D_ERR_CUDA;
-    const int smem = K.stages * K.stage_bytes + 8 * (2 * K.stages) + 16 + 2 * kEpiBytes + 1024;
+    const int smem = K.stages * K.stage_bytes + 2 * kEpiBytes + 8 * (2 * K.stages) + 1024;
     typedef void (*ConvKernel)(const KParams);
     const ConvKernel kernels[2][5] = {
         {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
@@ -666,14 +728,44 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     const uint64_t wstr[2] = {wdims[0] * 2, wdims[0] * wdims[1] * 2};
     const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)K.b_rows, 1u};   // bn / 2 is a multiple of 8: whole swizzle atoms
     const CUtensorMapSwizzle swz = block_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    const CUtensorMapDataType bf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     for (int b = 0; b < K.nbox; ++b) {
         const KParams::Sub& S = K.sub[box_sub[b]];
         const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)S.TW, (uint32_t)S.TH, (uint32_t)S.TN};
-        if ((rc = n3d_encode_tmap_bf16(&K.tmA[b][0], p->a_hi, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
-        if (p->nprod == 3 && (rc = n3d_encode_tmap_bf16(&K.tmA[b][1], p->a_lo, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+        if ((rc = n3d_encode_tmap(&K.tmA[b][0], bf16, p->a_hi, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+        if (p->nprod == 3 && (rc = n3d_encode_tmap(&K.tmA[b][1], bf16, p->a_lo, 4, adims, astr, abox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
     }
-    if ((rc = n3d_encode_tmap_bf16(&K.tmB_hi, p->w_hi, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
-    if (p->nprod == 3 && (rc = n3d_encode_tmap_bf16(&K.tmB_lo, p->w_lo, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+    if ((rc = n3d_encode_tmap(&K.tmB_hi, bf16, p->w_hi, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+    if (p->nprod == 3 && (rc = n3d_encode_tmap(&K.tmB_lo, bf16, p->w_lo, 3, wdims, wstr, wbox, swz, "n3d_conv_gemm")) != N3D_OK) return rc;
+
+    // Raw fp32 output through TMA stores: mode 1 with nothing else to write, NHWC, not accumulating, 16-byte aligned pixel stride
+    // and channel offset, pixels that do not overlap, and at least one output pixel in every sub-problem (a tensor map has no
+    // empty dimension).  Every other descriptor keeps the per-thread stores.  Sub-problem i's map covers the output pixels
+    // (y * oy_mul + oy_off, x * ox_mul + ox_off) of x < x_end, y < y_end that lie inside OW x OH.
+    {
+        const int64_t cs = p->f32_cstride;
+        bool tma = p->mode == 1 && !p->out[0].hi && !p->out[1].hi && !p->f32_nchw && !p->f32_accumulate && p->oy_mul >= 1 && p->ox_mul >= 1 &&
+                   cs % 4 == 0 && p->f32_coff % 4 == 0 && p->f32_coff >= 0 && cs >= p->f32_coff + p->Cout;
+        uint64_t cdims[kMaxSubs][5];
+        for (int i = 0; i < nsub && tma; ++i) {
+            const KParams::Sub& S = K.sub[i];
+            const int xd = min(S.x_end, n3d_div_up(p->OW - S.ox_off, p->ox_mul)), yd = min(S.y_end, n3d_div_up(p->OH - S.oy_off, p->oy_mul));
+            const uint64_t d[5] = {(uint64_t)p->Cout, (uint64_t)xd, (uint64_t)yd, (uint64_t)p->N, (uint64_t)splits};
+            memcpy(cdims[i], d, sizeof(d));
+            tma = S.oy_off >= 0 && S.ox_off >= 0 && xd >= 1 && yd >= 1;
+        }
+        K.tma_store = tma;
+        const int bc = min(32, bn);
+        for (int i = 0; i < nsub && tma; ++i) {
+            const KParams::Sub& S = K.sub[i];
+            const uint64_t pix = (uint64_t)cs * 4, cstr[4] = {p->ox_mul * pix, (uint64_t)p->oy_mul * p->OW * pix, (uint64_t)p->OH * p->OW * pix,
+                                                               splits > 1 ? (uint64_t)p->split_stride * 4 : (uint64_t)p->N * p->OH * p->OW * pix};
+            const uint32_t cbox[5] = {(uint32_t)bc, (uint32_t)S.TW, (uint32_t)(S.TN > 1 ? S.TH : S.TH / 2), (uint32_t)(S.TN > 1 ? S.TN / 2 : 1), 1u};
+            const float* base = p->out_f32 + (((int64_t)S.oy_off * p->OW + S.ox_off) * cs + p->f32_coff);
+            if ((rc = n3d_encode_tmap(&K.tmC[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, 5, cdims[i], cstr, cbox,
+                                      bc == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, "n3d_conv_gemm")) != N3D_OK) return rc;
+        }
+    }
 
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];

@@ -151,7 +151,7 @@ __global__ void __launch_bounds__(256) wgrad_operand_kernel(const float* __restr
 int make_tmap_2d(CUtensorMap* tm, const void* base, int64_t cols, int64_t rows, int64_t ld, int box_rows) {
     const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows}, stride = (uint64_t)ld * 2;
     const uint32_t box[2] = {(uint32_t)kBK, (uint32_t)box_rows};
-    return n3d_encode_tmap_bf16(tm, base, 2, dims, &stride, box, CU_TENSOR_MAP_SWIZZLE_128B, "n3d_conv_wgrad");
+    return n3d_encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, 2, dims, &stride, box, CU_TENSOR_MAP_SWIZZLE_128B, "n3d_conv_wgrad");
 }
 
 bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }

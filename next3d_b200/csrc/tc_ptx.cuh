@@ -129,6 +129,18 @@ __device__ __forceinline__ void mbar_wait_short(uint32_t bar, uint32_t parity) {
     }
     __trap();
 }
+// 5-D tensor store shared -> global (TMA engine), tracked by the issuing thread's bulk async-groups: the box at `src` (laid out
+// and swizzled as the tensor map's box) is written to the tensor at the given coordinates; elements outside the tensor are
+// skipped.  The thread that issued it commits the group and later waits for it.
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                 ::"l"(tm), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed group of this thread has finished reading its shared-memory source (its global writes may still be in flight)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed group of this thread is complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
