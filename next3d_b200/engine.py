@@ -11,8 +11,9 @@ Execution model (see DESIGN.md):
   * mesh path, volume renderer, resizes, blending: one kernel each (raster.cu, render_fused.cu).
 Reference call order: triplane_next3d.py:117-188.
 """
+import contextlib
+import dataclasses
 import math
-import os
 
 import numpy as np
 import torch
@@ -48,34 +49,80 @@ class Split:
         return self.hi.shape[-1]
 
 
-class _ModLayer:
-    """A modulated layer (SynthesisLayer or ToRGBLayer) after packing."""
+@dataclasses.dataclass(eq=False)
+class _Layer:
+    """A packed convolution layer, with the part of its epilogue that its place in the network fixes.  Engine.mod holds the
+    modulated ones: SynthesisLayer (networks_stylegan2.py:311-330) and ToRGBLayer (:353-357, a 1x1 modulated conv without
+    demodulation, linear bias + clamp).  Engine.plain holds the StyleUNet Conv2dLayers (networks_stylegan2_styleunet.py:198-207),
+    their weight_gain folded into the packed weights."""
+    name: str
+    cin: int
+    cout: int
+    k: int
+    w_hi: torch.Tensor                      # split bf16 [k*k, Cout, Cin]
+    w_lo: torch.Tensor
+    bias: torch.Tensor = None
+    w_f32: torch.Tensor = None              # fp32 [Cout, Cin] of a ToRGB layer of <= 4 channels: the fused-ToRGB epilogue operand
+    noise: torch.Tensor = None              # noise_const * noise_strength
+    noise_strength: torch.Tensor = None
+    clamp: float = -1.0                     # -1: no conv_clamp
+    gain: float = 1.0                       # activation: lrelu (sqrt 2, 0.2) or linear (1, 1)
+    slope: float = 1.0
+    up: int = 1                             # 2: stride-2 transposed conv (SynthesisBlock conv0)
+    down: int = 1                           # 2: stride-2 conv over the parity-split input (EncoderResBlock conv2)
+    widx: int = -1                          # ws index of a modulated layer's style
+    is_rgb: bool = False
+    sbase: int = -1                         # element offsets (per N=1) of a modulated layer's style / dcoef blocks
+    dbase: int = -1
 
-    def __init__(self, name, cin, cout, k, up, widx, is_rgb, clamp):
-        self.name, self.cin, self.cout, self.k, self.up, self.widx, self.is_rgb, self.clamp = name, cin, cout, k, up, widx, is_rgb, clamp
-        self.w_hi = self.w_lo = self.bias = self.noise = None
-        self.sbase = self.dbase = -1          # element offsets (per N=1) of this layer's style / dcoef blocks
 
+class _BackboneCache(dict):
+    """What synthesis(cache_backbone=True) keeps for a batch of B heads: (a) the two ws-only backbone outputs 'textures' and
+    'static', (b) the blended 'planes' and (c) the call's 'ws' and 'noise_mode', in engine-owned buffers at fixed addresses, so that
+    captured graphs can read and write them and no graph replay overwrites them.  use_cached_backbone=True re-runs everything but
+    (a) (triplane.py:120-128 of EG3D); render_views renders new cameras from (b).  The cache lives until the next cache_backbone
+    call with another batch size or the engine is rebuilt."""
 
-class _PlainLayer:
-    """A non-modulated Conv2dLayer (StyleUNet encoder / fusion)."""
+    def __init__(self, B=0, textures=None, static=None, planes=None, ws=None):
+        # noise_mode: the caching call's; None while nothing is cached
+        super().__init__(B=B, textures=textures, static=static, planes=planes, ws=ws, noise_mode=None)
 
-    def __init__(self, name, cin, cout, k):
-        self.name, self.cin, self.cout, self.k = name, cin, cout, k
-        self.w_hi = self.w_lo = self.bias = None
+    @property
+    def filled(self):
+        return self['noise_mode'] is not None
+
+    def fill(self, noise_mode):
+        """Record that a caching call with `noise_mode` has written the buffers (run eagerly or replayed from a graph)."""
+        self['noise_mode'] = noise_mode
+
+    def views(self, N, views, mismatch):
+        """Images per cached head for a call with N images, None while nothing is cached.  N must equal B or, where `views` are
+        allowed, be a multiple B * V of it (image n reads head n // V); any other N raises RuntimeError(mismatch % (N, B))."""
+        if not self.filled:
+            return None
+        B = self['B']
+        if N % B if views else N != B:
+            raise RuntimeError(mismatch % (N, B))
+        return N // B
 
 
 class Engine:
+    # Split-K for the 3x3 layers up to 16^2: a batch of 8 gives 1-4 tiles of 128 pixels and a 72-step serial K loop (9 taps x 512
+    # channels): the nine taps become nine concurrent work items per tile writing raw partial sums, summed in fixed order by
+    # n3d_splitk_epilogue (deterministic; an atomics-based variant was rejected for run-to-run differences).  Chosen by resolution
+    # only: the summation order of a sample must not depend on the batch size.
+    splitk_maxres = 16
+
     def __init__(self, cfg, state_dict, device='cuda', nprod=3, uv_face_mask=None):
         if not torch.cuda.is_available():
             raise RuntimeError('next3d_b200.Engine needs a CUDA device (sm_90a); there is no CPU path')
         self.cfg, self.device, self.nprod = cfg, torch.device(device), nprod
         self.rk = cfg.rendering_kwargs
-        self.mod, self.plain = {}, {}
+        self.mod, self.plain, self.consts = {}, {}, {}
         self.launches = 0                       # kernels launched by the last synthesis() / compute_planes() call (counted in kernels.py)
         self.conv_flops = 0.0
         self.prof = None
-        self._cur_layer = ''
+        self._cur_layer = ''                    # the layer whose launch is being set up (hooks on _noise read it)
         sd = {k: v.to(self.device, non_blocking=True) if isinstance(v, torch.Tensor) else v for k, v in state_dict.items()}
         self._pack(sd)
         self._tables = {}
@@ -84,37 +131,35 @@ class Engine:
         self._mm_init = torch.tensor([float('inf'), 0.0], device=self.device)
         self._mm_init_image = torch.tensor([[float('inf'), float('-inf')]], device=self.device)     # one pair per image: repeat(N, 1)
         self._graphs = {}                       # key[0]: the graph reads or writes the backbone cache
-        self._cache = None                      # backbone cache (synthesis with cache_backbone=True), see _cache_buffers
+        self._cache = _BackboneCache()          # allocated by the first cache_backbone call, see _cache_buffers
         self._side = None                      # side streams of the concurrent branches (compute_planes)
-        self.concurrent = os.environ.get('N3D_CONCURRENT', '1') != '0'
-        self.splitk = os.environ.get('N3D_SPLITK', '1') != '0'
-        self.splitk_maxres = int(os.environ.get('N3D_SPLITK_MAXRES', '16'))
+        self.concurrent = True                  # False: the three branches of compute_planes run on one stream (per-kernel timing)
+        self.splitk = True                      # False: every conv runs as one conv_gemm pass (the reference of the split-K test)
 
     # ------------------------------------------------------------------------------------------ packing (one-time)
     def _add_mod(self, sd, name, cin, cout, k, up, widx, is_rgb=False, clamp=None, noise=True):
-        L = _ModLayer(name, cin, cout, k, up, widx, is_rgb, clamp)
         w = sd[f'{name}.weight'].float()
-        L.w_hi, L.w_lo = K.pack_conv_weight(w)
-        L.w_f32 = w.reshape(cout, cin).contiguous() if (is_rgb and cout <= 4) else None    # fused-ToRGB epilogue operand
-        L.bias = sd[f'{name}.bias'].float().contiguous()
-        L.aff_w = sd[f'{name}.affine.weight'].float().contiguous()
-        L.aff_b = sd[f'{name}.affine.bias'].float().contiguous()
-        L.wsq = None if is_rgb else w.square().sum(dim=[2, 3]).contiguous()        # [Cout, Cin]
-        if not is_rgb and noise:
-            L.noise = (sd[f'{name}.noise_const'].float() * sd[f'{name}.noise_strength'].float()).contiguous()
-            L.noise_strength = sd[f'{name}.noise_strength'].float()
-        self.mod[name] = L
-        return L
+        noise = noise and not is_rgb
+        strength = sd[f'{name}.noise_strength'].float() if noise else None
+        self.mod[name] = _Layer(
+            name, cin, cout, k, *K.pack_conv_weight(w),
+            bias=sd[f'{name}.bias'].float().contiguous(),
+            w_f32=w.reshape(cout, cin).contiguous() if is_rgb and cout <= 4 else None,
+            noise=(sd[f'{name}.noise_const'].float() * strength).contiguous() if noise else None,
+            noise_strength=strength,
+            clamp=-1.0 if clamp is None else clamp,
+            gain=1.0 if is_rgb else SQRT2, slope=1.0 if is_rgb else 0.2,          # ToRGBLayer: linear, SynthesisLayer: lrelu
+            up=up, widx=widx, is_rgb=is_rgb)
 
-    def _add_plain(self, sd, name, k):
+    def _add_plain(self, sd, name, k, lrelu=False, down=1):
         w = sd[f'{name}.weight'].float()
         cout, cin = w.shape[:2]
-        L = _PlainLayer(name, cin, cout, k)
-        L.w_hi, L.w_lo = K.pack_conv_weight(w, gain=1.0 / math.sqrt(cin * k * k))       # Conv2dLayer.weight_gain
         b = sd.get(f'{name}.bias')
-        L.bias = b.float().contiguous() if b is not None else None
-        self.plain[name] = L
-        return L
+        self.plain[name] = _Layer(
+            name, cin, cout, k, *K.pack_conv_weight(w, gain=1.0 / math.sqrt(cin * k * k)),      # Conv2dLayer.weight_gain
+            bias=b.float().contiguous() if b is not None else None,
+            gain=SQRT2 if lrelu else 1.0, slope=0.2 if lrelu else 1.0,
+            down=down)
 
     def _pack_synthesis(self, sd, prefix, cimg, ws_off, first_res=4):
         cfg = self.cfg
@@ -133,15 +178,14 @@ class Engine:
             else:
                 self._add_mod(sd, f'{p}.conv1', cout, cout, 3, 1, ws_off + 0)
                 self._add_mod(sd, f'{p}.torgb', cout, cimg, 1, 1, ws_off + 1, is_rgb=True)
-                self.consts = getattr(self, 'consts', {})
                 self.consts[prefix] = sd[f'{p}.const'].float().permute(1, 2, 0).contiguous()      # [4,4,C] NHWC
 
     def _pack_unet(self, sd, prefix, in_size, final_size):
         enc = _config.encoder_resolutions(in_size, final_size)
         for i, _ in enumerate(enc[:-1]):
             self._add_plain(sd, f'{prefix}.encoder.{i}.fromrgb', 1)
-            self._add_plain(sd, f'{prefix}.encoder.{i}.conv1', 3)
-            self._add_plain(sd, f'{prefix}.encoder.{i}.conv2', 3)
+            self._add_plain(sd, f'{prefix}.encoder.{i}.conv1', 3, lrelu=True)
+            self._add_plain(sd, f'{prefix}.encoder.{i}.conv2', 3, lrelu=True, down=2)
         n_fusion = len(enc) - 1                            # the last fusion module (highest res) is never executed
         for i in range(n_fusion):
             self._add_plain(sd, f'{prefix}.fusion.{i}', 3)
@@ -165,8 +209,6 @@ class Engine:
         # decoder (OSGDecoder, triplane_next3d.py:348-357): FullyConnectedLayer gains folded like its forward does
         self.dec = ((sd['decoder.net.0.weight'].float() * (1.0 / math.sqrt(32))).contiguous(), sd['decoder.net.0.bias'].float().contiguous(),
                     (sd['decoder.net.2.weight'].float() * (1.0 / math.sqrt(64))).contiguous(), sd['decoder.net.2.bias'].float().contiguous())
-        # mapping network stays in PyTorch (adjacent to, not inside, synthesis; SURVEY.md a17)
-        self.mapping_sd = {k[len('backbone.mapping.'):]: v.float() for k, v in sd.items() if k.startswith('backbone.mapping.')}
         # topology
         self.faces = sd['faces'][0][:, [0, 2, 1]].to(torch.int32).contiguous()                       # :207
         self.face_uv = sd['face_uvcoords'][0][:, [0, 2, 1], :2].float().contiguous()                # :208 (u, v)
@@ -181,13 +223,13 @@ class Engine:
                 L.dbase = db
                 db += L.cout
         self.style_elems, self.dcoef_elems = sb, db
-        self.aff_w = torch.cat([L.aff_w for L in order], 0).contiguous()
-        self.aff_b = torch.cat([L.aff_b for L in order], 0).contiguous()
+        self.aff_w = torch.cat([sd[f'{L.name}.affine.weight'].float() for L in order], 0).contiguous()
+        self.aff_b = torch.cat([sd[f'{L.name}.affine.bias'].float() for L in order], 0).contiguous()
         self.row_widx = torch.cat([torch.full((L.cin,), L.widx, dtype=torch.int32) for L in order]).to(self.device)
         self.row_scale = torch.cat([torch.full((L.cin,), (1.0 / math.sqrt(L.cin * L.k * L.k)) if L.is_rgb else 1.0) for L in order]).to(self.device)
         self.row_cin = torch.cat([torch.full((L.cin,), L.cin, dtype=torch.int32) for L in order]).to(self.device)
         dl = [L for L in order if not L.is_rgb]
-        self.wsq = torch.cat([L.wsq.reshape(-1) for L in dl]).contiguous()
+        self.wsq = torch.cat([sd[f'{L.name}.weight'].float().square().sum(dim=[2, 3]).reshape(-1) for L in dl]).contiguous()   # [Cout, Cin] each
         woff, acc = [], 0
         for L in dl:
             woff.append(torch.arange(L.cout, dtype=torch.int64) * L.cin + acc)
@@ -195,9 +237,6 @@ class Engine:
         self.d_woff = torch.cat(woff).to(self.device)
         self.d_cin = torch.cat([torch.full((L.cout,), L.cin, dtype=torch.int32) for L in dl]).to(self.device)
         self.d_cout = torch.cat([torch.full((L.cout,), L.cout, dtype=torch.int32) for L in dl]).to(self.device)
-        for L in order:
-            del L.aff_w, L.aff_b
-            L.wsq = None
 
     def _batch_tables(self, N):
         """Per-batch-size offset tables: every layer's style / dcoef block is dense [N, C] at base*N."""
@@ -226,13 +265,13 @@ class Engine:
         e1.record()
         self.prof.append((kind, e0, e1, flops, info))
 
-    def _gemm(self, a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, **kw):
-        """n3d_conv_gemm + bookkeeping: algorithmic FLOPs = 2 * Cin * Cout * taps * M-space positions (one product)."""
-        flops = 2.0 * a_hi.shape[-1] * w_hi.shape[1] * len(taps) * N * MH * MW
+    def _timed(self, L, flops, M, ntaps, launch, *args, **kw):
+        """launch(*args, **kw), one pass of layer L over an M x M space: adds its FLOPs to conv_flops and records it as a conv_gemm
+        profiler entry with info (layer, Cin, Cout, MH, MW, taps), the row tools/profile_convs.py prints."""
         self.conv_flops += flops
         ev = self._prof_begin()
-        K.conv_gemm(a_hi, a_lo, w_hi, w_lo, taps, N, MH, MW, **kw)
-        self._prof_end(ev, 'conv_gemm', flops, (self._cur_layer, a_hi.shape[-1], w_hi.shape[1], MH, MW, len(taps)))
+        launch(*args, **kw)
+        self._prof_end(ev, 'conv_gemm', flops, (L.name, L.cin, L.cout, M, M, ntaps))
 
     def profile_summary(self):
         """After a synthesis() with self.prof = []: {kind: (launches, total_ms, total_flops)} (synchronises)."""
@@ -266,88 +305,60 @@ class Engine:
         style = self._style(self.mod[consumer]) if consumer else None
         return K.make_split_out(buf.hi, buf.lo, style, buf.C, coff)
 
-    # ------------------------------------------------------------------------------------------ layer runners
-    def _fused_rgb(self, name, img, accumulate, nchw=False):
-        """Descriptor that folds ToRGBLayer `name` (<= 4 image channels) into the epilogue of the conv producing its input."""
-        L = self.mod[name]
-        return dict(out=img, weight=L.w_f32, style=self._style(L), bias=L.bias, clamp=L.clamp if L.clamp is not None else -1.0,
-                    nchw=nchw, accumulate=accumulate)
-
-    # ---- split-K for the 4^2 / 8^2 layers: a batch of 8 gives 1-4 tiles of 128 pixels and a 72-step serial K loop (9 taps x 512
-    # channels): the nine taps become nine concurrent work items per tile writing raw partial sums, summed in fixed order by
-    # n3d_splitk_epilogue (deterministic; an atomics-based variant was rejected for run-to-run differences).
-    def _use_splitk(self, res):
-        return self.splitk and res <= self.splitk_maxres   # by resolution only: the summation order of a sample must not depend on the batch size
-
-    def _splitk_conv(self, name, a, L, res, epi):
-        N, S = self._N, 9
-        part = self._f32(S, N, res, res, L.cout)
-        self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_conv3x3(), N, res, res, nprod=self.nprod, mode=1, out_f32=part, f32_cstride=L.cout,
-                    splits=S, split_stride=N * res * res * L.cout)
-        ev = self._prof_begin()                  # the reduction pass is part of this convolution: counted as conv time (0 extra FLOPs)
-        K.splitk_epilogue(part, **epi)
-        self._prof_end(ev, 'conv_gemm', 0.0, (name, a.hi.shape[-1], L.cout, res, res, 0))
-
-    def _modconv(self, name, a, res_in, outs, noise_mode, f32=None, rgb=None):
-        """SynthesisLayer (networks_stylegan2.py:311-330); `a` already carries this layer's modulation."""
-        L, N = self.mod[name], self._N
-        self._cur_layer = name
+    # ------------------------------------------------------------------------------------------ layers
+    def _epilogue(self, L, noise_mode='none', outs=(), f32=None, accumulate=False):
+        """Layer L's epilogue under the keyword names conv_gemm, splitk_epilogue and fir_up_epilogue share: demodulation (SynthesisLayer),
+        bias, noise, activation and clamp, then the split bf16 outputs `outs` and the fp32 NHWC output `f32`, which conv_gemm adds
+        to with `accumulate`."""
+        self._cur_layer = L.name
         noise, nstride = self._noise(L, noise_mode)
-        clamp = L.clamp if L.clamp is not None else -1.0
-        if L.up == 1 and self._use_splitk(res_in) and rgb is None:
-            self._splitk_conv(name, a, L, res_in, dict(dcoef=self._dcoef(L), bias=L.bias, noise=noise, noise_nstride=nstride, gain=SQRT2, slope=0.2,
-                                                        clamp=clamp, outs=outs, out_f32=f32, f32_cstride=L.cout if f32 is not None else 0))
-            return
-        if L.up == 1:
-            self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_conv3x3(), N, res_in, res_in, nprod=self.nprod, dcoef=self._dcoef(L), bias=L.bias,
-                        noise=noise, noise_nstride=nstride, gain=SQRT2, slope=0.2, clamp=clamp, outs=outs, out_f32=f32,
-                        f32_cstride=L.cout if f32 is not None else 0, rgb=rgb)
-            return
-        assert rgb is None
-        raw = self._f32(N, 2 * res_in + 1, 2 * res_in + 1, L.cout)
-        flops = 2.0 * L.cin * L.cout * N * (3 * res_in + 2) ** 2          # taps x positions summed over the 4 parity classes
-        self.conv_flops += flops
-        ev = self._prof_begin()
-        K.conv_transposed_gemm(a.hi, a.lo, L.w_hi, L.w_lo, N, res_in, res_in, raw, nprod=self.nprod)
-        self._prof_end(ev, 'conv_gemm', flops, (name, L.cin, L.cout, res_in + 1, res_in + 1, 9))
-        K.fir_up_epilogue(raw, L.cout, self._dcoef(L), L.bias, noise, SQRT2, 0.2, clamp, outs=outs, out_f32=f32,
-                          f32_cstride=L.cout if f32 is not None else 0, noise_nstride=nstride)
+        return dict(dcoef=self._dcoef(L) if L.dbase >= 0 else None, bias=L.bias, noise=noise, noise_nstride=nstride, gain=L.gain,
+                    slope=L.slope, clamp=L.clamp, outs=outs, out_f32=f32, f32_cstride=L.cout if f32 is not None else 0,
+                    f32_accumulate=accumulate)
 
-    def _torgb(self, name, a, res, img, accumulate, nchw=False):
-        """ToRGBLayer (networks_stylegan2.py:353-357): 1x1 modulated conv without demodulation, linear bias (+ clamp)."""
-        L = self.mod[name]
-        self._cur_layer = name
-        self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_conv1x1(), self._N, res, res, nprod=self.nprod, bias=L.bias,
-                    clamp=L.clamp if L.clamp is not None else -1.0, out_f32=img, f32_cstride=L.cout, f32_nchw=nchw, f32_accumulate=accumulate)
+    def _fused_rgb(self, L, img, nchw=False):
+        """Descriptor that folds ToRGBLayer L (<= 4 image channels) into the epilogue of the conv producing its input: img += torgb."""
+        return dict(out=img, weight=L.w_f32, style=self._style(L), bias=L.bias, clamp=L.clamp, nchw=nchw, accumulate=True)
 
-    def _plainconv(self, name, a, res, act, outs=(), f32=None, accumulate=False, stride2=False):
-        """styleunet Conv2dLayer (networks_stylegan2_styleunet.py:198-207): weight_gain folded into the packed weights."""
-        L, N = self.plain[name], self._N
-        self._cur_layer = name
-        gain, slope = (SQRT2, 0.2) if act == 'lrelu' else (1.0, 1.0)
-        if stride2:
-            self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, K.taps_stride2(), N, res // 2, res // 2, a_img_mul=N, nprod=self.nprod, bias=L.bias, gain=gain,
-                        slope=slope, outs=outs, out_f32=f32, f32_cstride=L.cout if f32 is not None else 0, f32_accumulate=accumulate)
-        elif L.k == 3 and self._use_splitk(res) and not accumulate:
-            self._splitk_conv(name, a, L, res, dict(dcoef=None, bias=L.bias, noise=None, gain=gain, slope=slope, clamp=-1.0, outs=outs, out_f32=f32,
-                                                    f32_cstride=L.cout if f32 is not None else 0))
+    def _conv(self, L, a, res, epi, rgb=None):
+        """Layer L on the split activation `a` (modulated layers: already pre-multiplied by L's style) at input resolution `res`, with
+        the epilogue `epi` of _epilogue and the fused ToRGB `rgb` of _fused_rgb: a stride-2 transposed conv (4 parity classes into a
+        raw sum, then the FIR-up epilogue), a stride-2 conv over the parity-split input, split-K (splitk_maxres), or one pass.
+        Algorithmic FLOPs = 2 * Cin * Cout * taps * M-space positions (one product)."""
+        N = self._N
+        accumulate = epi.pop('f32_accumulate')                 # conv_gemm's alone: the split-K and FIR-up epilogues overwrite
+        if L.up == 2:
+            assert rgb is None and not accumulate
+            raw = self._f32(N, 2 * res + 1, 2 * res + 1, L.cout)
+            self._timed(L, 2.0 * L.cin * L.cout * N * (3 * res + 2) ** 2, res + 1, 9,       # taps x positions over the 4 parity classes
+                        K.conv_transposed_gemm, a.hi, a.lo, L.w_hi, L.w_lo, N, res, res, raw, nprod=self.nprod)
+            K.fir_up_epilogue(raw, L.cout, **epi)
             return
-        else:
-            taps = K.taps_conv3x3() if L.k == 3 else K.taps_conv1x1()
-            self._gemm(a.hi, a.lo, L.w_hi, L.w_lo, taps, N, res, res, nprod=self.nprod, bias=L.bias, gain=gain, slope=slope, outs=outs,
-                        out_f32=f32, f32_cstride=L.cout if f32 is not None else 0, f32_accumulate=accumulate)
+        M = res // L.down
+        taps = K.taps_stride2() if L.down == 2 else K.taps_conv3x3() if L.k == 3 else K.taps_conv1x1()
+        flops = 2.0 * L.cin * L.cout * len(taps) * N * M * M
+        if L.k == 3 and L.down == 1 and self.splitk and res <= self.splitk_maxres and rgb is None and not accumulate:
+            S = 9
+            part = self._f32(S, N, res, res, L.cout)
+            self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, L.w_hi, L.w_lo, taps, N, M, M, nprod=self.nprod, mode=1,
+                        out_f32=part, f32_cstride=L.cout, splits=S, split_stride=N * res * res * L.cout)
+            self._timed(L, 0.0, M, 0, K.splitk_epilogue, part, **epi)         # the reduction is conv time (0 extra FLOPs)
+            return
+        self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, L.w_hi, L.w_lo, taps, N, M, M, a_img_mul=N if L.down == 2 else 0,
+                    nprod=self.nprod, rgb=rgb, f32_accumulate=accumulate, **epi)
 
     # ------------------------------------------------------------------------------------------ networks
-    def _synthesis_blocks(self, prefix, x, res_list, cimg, noise_mode, concat_next=None, final_nchw=None, img=None):
+    def _synthesis_blocks(self, prefix, x, res_list, cimg, noise_mode, concat_next=None, img=None):
         """Run SynthesisBlocks `res_list` (all with conv0 up) starting from split activation `x` (modulated for the first
         conv0) at resolution res_list[0]//2.  concat_next: {res: (concat Split buffer, fusion runner)} -- when the output of
         block `res` feeds a fusion conv (StyleUNet) instead of the next conv0 directly."""
         N, dev = self._N, self.device
         for i, res in enumerate(res_list):
             p = f'{prefix}.b{res}'
-            c = self.mod[f'{p}.conv1'].cout
+            conv0, conv1, torgb = self.mod[f'{p}.conv0'], self.mod[f'{p}.conv1'], self.mod[f'{p}.torgb']
+            c = conv1.cout
             x1 = Split((N, res, res, c), dev)
-            self._modconv(f'{p}.conv0', x, res // 2, [self._out(x1, f'{p}.conv1')], noise_mode)
+            self._conv(conv0, x, res // 2, self._epilogue(conv0, noise_mode, [self._out(x1, f'{p}.conv1')]))
             nxt = res_list[i + 1] if i + 1 < len(res_list) else None
             rgb_in = Split((N, res, res, c), dev)
             outs = [self._out(rgb_in, f'{p}.torgb')]
@@ -358,21 +369,15 @@ class Engine:
             elif nxt is not None:
                 x = Split((N, res, res, c), dev)
                 outs.append(self._out(x, f'{prefix}.b{nxt}.conv0'))
-            self._modconv(f'{p}.conv1', x1, res, outs, noise_mode)
-            last = nxt is None
+            self._conv(conv1, x1, res, self._epilogue(conv1, noise_mode, outs))
             if img is None:
                 img = self._f32(N, res, res, cimg)
-                self._torgb(f'{p}.torgb', rgb_in, res, img, accumulate=False)
+                self._conv(torgb, rgb_in, res, self._epilogue(torgb, f32=img))
             else:
-                if last and final_nchw is not None:
-                    K.upsample2d_nhwc(img, final_nchw, y_nchw=True)
-                    self._torgb(f'{p}.torgb', rgb_in, res, final_nchw, accumulate=True, nchw=True)
-                    img = final_nchw
-                else:
-                    up = self._f32(N, res, res, cimg)
-                    K.upsample2d_nhwc(img, up)
-                    self._torgb(f'{p}.torgb', rgb_in, res, up, accumulate=True)
-                    img = up
+                up = self._f32(N, res, res, cimg)
+                K.upsample2d_nhwc(img, up)
+                self._conv(torgb, rgb_in, res, self._epilogue(torgb, f32=up, accumulate=True))
+                img = up
             if concat_next and res in concat_next:
                 x = concat_next[res][1]()                      # run the fusion conv, returns the next conv0's input
         return img
@@ -382,13 +387,14 @@ class Engine:
         N, dev, cfg = self._N, self.device, self.cfg
         c4 = cfg.channels(4)
         const = self.consts[prefix][None].expand(N, -1, -1, -1).contiguous()
+        conv1, torgb = self.mod[f'{prefix}.b4.conv1'], self.mod[f'{prefix}.b4.torgb']
         x0 = Split((N, 4, 4, c4), dev)
-        K.modulate_split(const, self._style(self.mod[f'{prefix}.b4.conv1']), x0.hi, x0.lo)
+        K.modulate_split(const, self._style(conv1), x0.hi, x0.lo)
         rgb_in = Split((N, 4, 4, c4), dev)
         x = Split((N, 4, 4, c4), dev)
-        self._modconv(f'{prefix}.b4.conv1', x0, 4, [self._out(rgb_in, f'{prefix}.b4.torgb'), self._out(x, f'{prefix}.b8.conv0')], noise_mode)
+        self._conv(conv1, x0, 4, self._epilogue(conv1, noise_mode, [self._out(rgb_in, f'{prefix}.b4.torgb'), self._out(x, f'{prefix}.b8.conv0')]))
         img = self._f32(N, 4, 4, cimg)
-        self._torgb(f'{prefix}.b4.torgb', rgb_in, 4, img, accumulate=False)
+        self._conv(torgb, rgb_in, 4, self._epilogue(torgb, f32=img))
         return self._synthesis_blocks(prefix, x, _config.block_resolutions(cfg.plane_res)[1:], cimg, noise_mode, img=img)
 
     def _styleunet(self, prefix, x_in, in_size, final_size, num_cond_res, noise_mode):
@@ -412,6 +418,7 @@ class Engine:
         n_enc = len(enc_res) - 1
         for i, r in enumerate(enc_res[:-1]):
             p = f'{prefix}.encoder.{i}'
+            fromrgb, conv1, conv2 = self.plain[f'{p}.fromrgb'], self.plain[f'{p}.conv1'], self.plain[f'{p}.conv2']
             cin = cfg.channels(r)
             if i > 0:
                 xd = self._f32(N, r, r, cfg.plane_ch)
@@ -421,12 +428,12 @@ class Engine:
             K.modulate_split(x, None, xs.hi, xs.lo)
             h = Split((N, r, r, cin), dev)
             if skip is None:
-                self._plainconv(f'{p}.fromrgb', xs, r, 'linear', outs=[K.make_split_out(h.hi, h.lo, None, cin, 0)])
+                self._conv(fromrgb, xs, r, self._epilogue(fromrgb, outs=[K.make_split_out(h.hi, h.lo, None, cin, 0)]))
             else:
-                self._plainconv(f'{p}.fromrgb', xs, r, 'linear', f32=skip, accumulate=True)       # out = fromrgb(x) + skip
+                self._conv(fromrgb, xs, r, self._epilogue(fromrgb, f32=skip, accumulate=True))       # out = fromrgb(x) + skip
                 K.modulate_split(skip, None, h.hi, h.lo)
             c1 = self._f32(N, r, r, cin)
-            self._plainconv(f'{p}.conv1', h, r, 'lrelu', f32=c1)
+            self._conv(conv1, h, r, self._epilogue(conv1, f32=c1))
             sh = (r + 2) // 2
             par = Split((4 * N, sh, sh, cin), dev)
             K.fir_down_split(c1, par.hi, par.lo)
@@ -439,18 +446,20 @@ class Engine:
             elif j < n_cond:
                 outs.append(K.make_split_out(cat[j].hi, cat[j].lo, None, cat[j].C, cat[j].C - cout))
             skip = self._f32(N, r // 2, r // 2, cout) if i + 1 < n_enc else None
-            self._plainconv(f'{p}.conv2', par, r, 'lrelu', outs=outs, f32=skip, stride2=True)
+            self._conv(conv2, par, r, self._epilogue(conv2, outs=outs, f32=skip))
         # ---- decoder with fusion
         first = dec_res[0]
         x = Split((N, final_size, final_size, cfg.channels(final_size)), dev)
-        self._plainconv(f'{prefix}.fusion.0', cond0, final_size, 'linear', outs=[self._out(x, f'{prefix}.b{first}.conv0')])
+        fusion = self.plain[f'{prefix}.fusion.0']
+        self._conv(fusion, cond0, final_size, self._epilogue(fusion, outs=[self._out(x, f'{prefix}.b{first}.conv0')]))
         concat_next = {}
         for j in range(1, n_cond):
             r = final_size * 2 ** j
 
             def run_fusion(j=j, r=r):
                 y = Split((N, r, r, cfg.channels(r)), dev)
-                self._plainconv(f'{prefix}.fusion.{j}', cat[j], r, 'linear', outs=[self._out(y, f'{prefix}.b{2 * r}.conv0')])
+                fusion = self.plain[f'{prefix}.fusion.{j}']
+                self._conv(fusion, cat[j], r, self._epilogue(fusion, outs=[self._out(y, f'{prefix}.b{2 * r}.conv0')]))
                 return y
             concat_next[r] = (cat[j], run_fusion)
         return self._synthesis_blocks(prefix, x, dec_res, cfg.plane_ch, noise_mode, concat_next=concat_next)
@@ -466,19 +475,20 @@ class Engine:
         if need and R > 128 and not self.rk.get('sr_antialias', True):
             raise RuntimeError('next3d_b200: sr_antialias=False with a neural rendering resolution above 128 (a plain bilinear minification) is not '
                                'implemented')
+        (b0_conv0, b0_conv1, b0_torgb), (b1_conv0, b1_conv1, b1_torgb) = [[self.mod[f'{p}.{n}'] for n in ('conv0', 'conv1', 'torgb')] for p in (p0, p1)]
         x = Split((N, r0, r0, cfg.plane_ch), dev)
         rgb_lo = feat[..., :3].contiguous()                                    # image_raw channels (tiny copy)
         if need:
-            K.resize_aa(feat, None, r0, r0, style=self._style(self.mod[f'{p0}.conv0']), hi=x.hi, lo=x.lo)
+            K.resize_aa(feat, None, r0, r0, style=self._style(b0_conv0), hi=x.hi, lo=x.lo)
             rgb = self._f32(N, r0, r0, 3)
             K.resize_aa(rgb_lo, rgb)
         else:
-            K.modulate_split(feat, self._style(self.mod[f'{p0}.conv0']), x.hi, x.lo)
+            K.modulate_split(feat, self._style(b0_conv0), x.hi, x.lo)
             rgb = rgb_lo
         # block0
         res0 = r0 * (2 if cfg.sr_module == '8XDC' else 1)
         x1 = Split((N, res0, res0, c0), dev)
-        self._modconv(f'{p0}.conv0', x, r0, [self._out(x1, f'{p0}.conv1')], noise_mode_sr)
+        self._conv(b0_conv0, x, r0, self._epilogue(b0_conv0, noise_mode_sr, [self._out(x1, f'{p0}.conv1')]))
         x2 = Split((N, res0, res0, c0), dev)
         if cfg.sr_module == '8XDC':
             img = self._f32(N, res0, res0, 3)
@@ -486,13 +496,13 @@ class Engine:
         else:
             img = rgb.clone()                                                   # SynthesisBlockNoUp: no image upsample
         # the two ToRGB layers (3 channels) run inside the conv1 epilogues: img += torgb(conv1 output)
-        self._modconv(f'{p0}.conv1', x1, res0, [self._out(x2, f'{p1}.conv0')], noise_mode_sr, rgb=self._fused_rgb(f'{p0}.torgb', img, True))
+        self._conv(b0_conv1, x1, res0, self._epilogue(b0_conv1, noise_mode_sr, [self._out(x2, f'{p1}.conv0')]), rgb=self._fused_rgb(b0_torgb, img))
         # block1
         res1 = res0 * 2
         x3 = Split((N, res1, res1, c1), dev)
-        self._modconv(f'{p1}.conv0', x2, res0, [self._out(x3, f'{p1}.conv1')], noise_mode_sr)
+        self._conv(b1_conv0, x2, res0, self._epilogue(b1_conv0, noise_mode_sr, [self._out(x3, f'{p1}.conv1')]))
         K.upsample2d_nhwc(img, image_out, y_nchw=True)
-        self._modconv(f'{p1}.conv1', x3, res1, [], noise_mode_sr, rgb=self._fused_rgb(f'{p1}.torgb', image_out, True, nchw=True))
+        self._conv(b1_conv1, x3, res1, self._epilogue(b1_conv1, noise_mode_sr, []), rgb=self._fused_rgb(b1_torgb, image_out, nchw=True))
 
     # ------------------------------------------------------------------------------------------ planes + synthesis
     def _on_device(self, **tensors):
@@ -503,49 +513,45 @@ class Engine:
                 raise RuntimeError(f'next3d_b200: `{name}` is on {t.device} but the generator runs on {self.device}; move it there '
                                    f'(there is no CPU path)')
 
+    @contextlib.contextmanager
+    def _entry(self, **inputs):
+        """The bracket of an eager entry point: its tensor inputs must be on the engine's device, which is made current, and
+        `launches` / `conv_flops` count what the call issues."""
+        self._on_device(**inputs)
+        with torch.cuda.device(self.device):
+            n0, self.conv_flops = K.launches, 0.0
+            yield
+            self.launches = K.launches - n0
+
     def compute_planes(self, ws, v, noise_mode='const', return_intermediates=False):
         """Everything up to the blended tri-planes (triplane_next3d.py:137-174) -> [N,3,256,256,32] channels-last fp32."""
-        self._on_device(ws=ws, v=v)
-        with torch.cuda.device(self.device):
-            n0 = K.launches
-            out = self._compute_planes(ws, v, noise_mode, return_intermediates)
-            self.launches = K.launches - n0
-            return out
+        with self._entry(ws=ws, v=v):
+            return self._compute_planes(ws, v, noise_mode, return_intermediates)
 
-    # ------------------------------------------------------------------------------------------ backbone cache
-    # synthesis(cache_backbone=True) keeps (a) the two ws-only backbone outputs, (b) the blended planes and (c) the call's ws and
-    # noise_mode in engine-owned buffers at fixed addresses, so that captured graphs can read and write them and no graph replay
-    # overwrites them.  use_cached_backbone=True re-runs everything but (a) (triplane.py:120-128 of EG3D); render_views renders new
-    # cameras from (b).  The cache lives until the next cache_backbone call with another batch size or the engine is rebuilt.
+    # ------------------------------------------------------------------------------------------ backbone cache (_BackboneCache)
     def _cache_buffers(self, B, ws_shape):
         """The cache buffers for batch B; a new B (or ws shape) reallocates them, which empties the cache and drops every graph that
         reads or writes them."""
         c = self._cache
-        if c is None or c['B'] != B or tuple(c['ws'].shape[1:]) != tuple(ws_shape[1:]):
+        if c['ws'] is None or c['B'] != B or tuple(c['ws'].shape[1:]) != tuple(ws_shape[1:]):
             P, C = self.cfg.plane_res, self.cfg.plane_ch
             self._graphs = {k: g for k, g in self._graphs.items() if not k[0]}
-            c = self._cache = dict(B=B, textures=self._f32(B, P, P, C), static=self._f32(B, P, P, 3 * C), planes=self._f32(B, 3, P, P, C),
-                                   ws=self._f32(B, *ws_shape[1:]), noise_mode=None)          # noise_mode None: nothing cached yet
+            c = self._cache = _BackboneCache(B, textures=self._f32(B, P, P, C), static=self._f32(B, P, P, 3 * C),
+                                             planes=self._f32(B, 3, P, P, C), ws=self._f32(B, *ws_shape[1:]))
         return c
 
-    def _cached(self, N, who, views=False):
-        """The filled cache for a call with batch N (None when nothing is cached).  views: N may be any multiple B * V of the cached
-        batch B (image n takes head n // V); otherwise N must equal B.  Another batch size raises."""
-        c = self._cache
-        if c is None or c['noise_mode'] is None:
+    def _reused_views(self, N, use_cached_backbone, cache_backbone):
+        """Images per cached head when a call of N images takes its backbones from the cache, None when it computes them.  A call
+        that also refills the cache keeps N = B (the cache holds one set of planes per head)."""
+        if not use_cached_backbone:
             return None
-        if (N % c['B'] if views else N != c['B']):
-            raise RuntimeError(f'next3d_b200: {who} with batch {N}, but the cached backbone holds batch {c["B"]}')
-        return c
+        return self._cache.views(N, not cache_backbone, 'next3d_b200: use_cached_backbone with batch %d, but the cached backbone holds batch %d')
 
-    def _views_cache(self, N):
-        """(cache, views per plane set) for render_views of N cameras."""
-        c = self._cache
-        if c is None or c['noise_mode'] is None:
+    def _render_views_per_head(self, N):
+        """Views per cached head for render_views of N cameras."""
+        if not self._cache.filled:
             raise RuntimeError('next3d_b200: render_views needs cached planes: run synthesis(..., cache_backbone=True) first')
-        if N % c['B']:
-            raise RuntimeError(f'next3d_b200: render_views got {N} cameras, not a multiple of the cached batch {c["B"]}')
-        return c, N // c['B']
+        return self._cache.views(N, True, 'next3d_b200: render_views got %d cameras, not a multiple of the cached batch %d')
 
     def _set_styles(self, ws):
         """Style vectors and demodulation coefficients of every modulated layer for the batch ws [N, L, D]."""
@@ -562,10 +568,9 @@ class Engine:
         cfg, dev = self.cfg, self.device
         N = ws.shape[0]
         P = cfg.plane_res
-        # N = B * V images on a cache of B heads: image n takes its texture and static planes from head n // V.  A call that also
-        # refills the cache keeps N = B (the cache holds one set of planes per head).
-        cached = self._cached(N, 'use_cached_backbone', views=not cache_backbone) if use_cached_backbone else None
-        V = N // cached['B'] if cached is not None else 1
+        # N = B * V images on a cache of B heads: image n takes its texture and static planes from head n // V
+        reuse = self._reused_views(N, use_cached_backbone, cache_backbone)
+        V = reuse or 1
         v = v.to(torch.float32)
         verts, lms = v[:, :5023].contiguous(), v[:, 5023:].contiguous()
         self._set_styles(ws)
@@ -593,12 +598,12 @@ class Engine:
             boxes = torch.empty(N, 4, dtype=torch.int32, device=dev)
             lm2d = tl[:, 0, :, :2].contiguous()
             K.mouth_box(lm2d, boxes)
-        if cached is None:
+        if reuse is None:
             with torch.cuda.stream(s_static):
                 static = self._backbone('backbone.synthesis', cfg.plane_ch * 3, noise_mode)         # [N,256,256,96]
             textures = self._backbone('texture_backbone.synthesis', cfg.plane_ch, noise_mode)      # [N,256,256,32]
         else:
-            static, textures = cached['static'], cached['textures']
+            static, textures = self._cache['static'], self._cache['textures']
         if self.concurrent:
             main.wait_stream(s_rast)
             for t in (p2f, bary, boxes, lm2d):
@@ -617,17 +622,17 @@ class Engine:
         stitched = front.clone()
         K.resize_aa(mouth, stitched, dst_box=boxes)
         blended = self._styleunet('neural_blending.synthesis', stitched, 256, 32, 256, noise_mode)
-        if self.concurrent and cached is None:
+        if self.concurrent and reuse is None:
             main.wait_stream(s_static)
             static.record_stream(main)
         planes = self._f32(N, 3, P, P, cfg.plane_ch)
         K.blend_planes(blended, tex_planes, alpha, static, planes, views=V)
         if cache_backbone:
             c = self._cache_buffers(N, ws.shape)
-            if cached is None:
+            if reuse is None:
                 c['textures'].copy_(textures)
                 c['static'].copy_(static)
-                c['noise_mode'] = noise_mode
+                c.fill(noise_mode)
             c['planes'].copy_(planes)
             c['ws'].copy_(ws)
         if return_intermediates:
@@ -642,20 +647,12 @@ class Engine:
         head n // V (N = B when cache_backbone is also set; any other batch raises).  depth_range: 'batch'
         clamps every image's depth to the range of the whole call (ray_marcher.py:54 on a batch), 'image' to the image's own range
         (what a call per image gives)."""
-        self._on_device(ws=ws, c=c, v=v)
-        with torch.cuda.device(self.device):
-            return self._synthesis(ws, c, v, noise_mode, neural_rendering_resolution, sampler_noise, seed, return_intermediates, seed_ptr,
-                                   cache_backbone, use_cached_backbone, _depth_range(depth_range))
-
-    def _synthesis(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, sampler_noise=None, seed=0,
-                   return_intermediates=False, seed_ptr=None, cache_backbone=False, use_cached_backbone=False, depth_range='batch'):
-        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-        n0 = K.launches
-        self.conv_flops = 0.0
-        out = self._compute_planes(ws, v, noise_mode, return_intermediates, cache_backbone, use_cached_backbone)
-        planes, inter = out if return_intermediates else (out, None)
-        result, feat, wsum, ws_normals = self._render(planes, c, R, sampler_noise, seed, seed_ptr, depth_range=depth_range)
-        self.launches = K.launches - n0
+        with self._entry(ws=ws, c=c, v=v):
+            depth_range = _depth_range(depth_range)
+            R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+            out = self._compute_planes(ws, v, noise_mode, return_intermediates, cache_backbone, use_cached_backbone)
+            planes, inter = out if return_intermediates else (out, None)
+            result, feat, wsum, ws_normals = self._render(planes, c, R, sampler_noise, seed, seed_ptr, depth_range=depth_range)
         if return_intermediates:
             inter.update(planes=planes, feature_image=feat, weights_sum=wsum)
             if ws_normals is not None:                                      # per ray: D sorted sample depths, then D - 1 final weights
@@ -710,27 +707,20 @@ class Engine:
         """New camera views of the cached heads: c [N, 25] with N = B * V for a cache of batch B; view n belongs to head n // V.
         Renders from the cached planes and runs super-resolution with the cached ws; returns what synthesis returns (depth_range as
         there: 'image' gives every view its own depth range)."""
-        self._on_device(c=c)
-        with torch.cuda.device(self.device):
-            return self._render_views(c, neural_rendering_resolution, sampler_noise, seed, seed_ptr, _depth_range(depth_range))
-
-    def _render_views(self, c, neural_rendering_resolution=None, sampler_noise=None, seed=0, seed_ptr=None, depth_range='batch'):
-        cache, V = self._views_cache(c.shape[0])
-        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-        n0 = K.launches
-        self.conv_flops = 0.0
-        ws = cache['ws']
-        self._set_styles(ws[:, None].expand(ws.shape[0], V, *ws.shape[1:]).reshape(-1, *ws.shape[1:]))     # ws of head n // V
-        result = self._render(cache['planes'], c, R, sampler_noise, seed, seed_ptr, views=V, depth_range=depth_range)[0]
-        self.launches = K.launches - n0
-        return result
+        with self._entry(c=c):
+            depth_range = _depth_range(depth_range)
+            V = self._render_views_per_head(c.shape[0])
+            R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+            ws = self._cache['ws']
+            self._set_styles(ws[:, None].expand(ws.shape[0], V, *ws.shape[1:]).reshape(-1, *ws.shape[1:]))     # ws of head n // V
+            return self._render(self._cache['planes'], c, R, sampler_noise, seed, seed_ptr, views=V, depth_range=depth_range)[0]
 
     def cached_sigma_grid(self, b, shape_res, sigma):
         """The shape-extraction density grid of cached head b (gen_samples_next3d.py:208-238: create_samples at box_warp, sigma
         flipped along axis 0 and trimmed) written into sigma, float32 [shape_res]^3 on the engine's device, from the planes the
         caching call kept: one n3d_sample_grid launch, no backbone.  Raises RuntimeError when nothing is cached or b is not a cached head."""
         c = self._cache
-        if c is None or c['noise_mode'] is None:
+        if not c.filled:
             raise RuntimeError('next3d_b200: cached_sigma_grid needs cached planes: run synthesis(..., cache_backbone=True) first')
         if not 0 <= b < c['B']:
             raise RuntimeError(f'next3d_b200: cached_sigma_grid of head {b}, but the cache holds {c["B"]} head(s)')
@@ -776,43 +766,41 @@ class Engine:
         self.launches, self.conv_flops = launches, flops
         return out
 
+    # The graphed entry points capture the eager one (its Python does not run on a replay, so what it records on the engine --
+    # launches, conv_flops, a filled cache -- is restored or re-recorded after each replay).
     def synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
                           use_cached_backbone=False, depth_range='batch'):
-        with torch.cuda.device(self.device):
-            return self._synthesis_graphed(ws, c, v, noise_mode, neural_rendering_resolution, seed, cache_backbone, use_cached_backbone,
-                                           _depth_range(depth_range))
-
-    def _synthesis_graphed(self, ws, c, v, noise_mode='const', neural_rendering_resolution=None, seed=0, cache_backbone=False,
-                           use_cached_backbone=False, depth_range='batch'):
         """Same as synthesis() (in-kernel sampler RNG) but the ~200 launches of one forward are captured once per
         (batch, cached batch, resolution, noise_mode, cache use) into a CUDA graph and replayed: removes the host-side launch latency that otherwise
         leaves the GPU idle between kernels.  The cache-using graphs read and write the engine's cache buffers in place."""
+        depth_range = _depth_range(depth_range)
         self._on_device(ws=ws, c=c, v=v)
-        N = ws.shape[0]
-        R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-        reuse = use_cached_backbone and self._cached(N, 'use_cached_backbone', views=not cache_backbone) is not None
-        if cache_backbone:
-            self._cache_buffers(N, ws.shape)              # allocated before capture: the graph writes the cache at fixed addresses
-        B = self._cache['B'] if reuse else N              # (N, B): the images per cached head of a reusing graph
-        key = (cache_backbone or reuse, cache_backbone, reuse, N, B, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
+        with torch.cuda.device(self.device):
+            N = ws.shape[0]
+            R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+            reuse = self._reused_views(N, use_cached_backbone, cache_backbone) is not None
+            if cache_backbone:
+                self._cache_buffers(N, ws.shape)          # allocated before capture: the graph writes the cache at fixed addresses
+            B = self._cache['B'] if reuse else N             # (N, B): the images per cached head of a reusing graph
+            key = (cache_backbone or reuse, cache_backbone, reuse, N, B, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
 
-        def run(st):
-            return self._synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,
-                                   use_cached_backbone=reuse, depth_range=depth_range)
-        out = self._replay(key, dict(ws=ws, c=c, v=v), run, seed)
-        if cache_backbone and not reuse:
-            self._cache['noise_mode'] = noise_mode
-        return out
+            def run(st):
+                return self.synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,
+                                      use_cached_backbone=reuse, depth_range=depth_range)
+            out = self._replay(key, dict(ws=ws, c=c, v=v), run, seed)
+            if cache_backbone and not reuse:
+                self._cache.fill(noise_mode)
+            return out
 
     def render_views_graphed(self, c, neural_rendering_resolution=None, seed=0, depth_range='batch'):
         """render_views() replayed from a CUDA graph per (N, V, resolution, depth range, rendering options); in-kernel sampler RNG."""
         self._on_device(c=c)
         depth_range = _depth_range(depth_range)
         with torch.cuda.device(self.device):
-            _, V = self._views_cache(c.shape[0])
+            V = self._render_views_per_head(c.shape[0])
             R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
             key = (True, 'views', c.shape[0], V, depth_range) + self._render_key(R)
-            return self._replay(key, dict(c=c), lambda st: self._render_views(st['c'], R, seed=0, seed_ptr=st['seed'], depth_range=depth_range),
+            return self._replay(key, dict(c=c), lambda st: self.render_views(st['c'], R, seed=0, seed_ptr=st['seed'], depth_range=depth_range),
                                 seed)
 
 
