@@ -64,11 +64,12 @@ __global__ void __launch_bounds__(256) bias_act_kernel(const T* __restrict__ x, 
 
 extern "C" int n3d_bias_act(const void* x, const void* b, void* y, int dtype, int64_t numel, int size_b, int step_b,
                             int act, float alpha, float gain, float clamp, void* stream) {
-    N3D_CHECK_ARG(x && y && numel >= 0, "n3d_bias_act: null pointer");
+    N3D_CHECK_ARG(numel >= 0, "n3d_bias_act: negative numel");
     N3D_CHECK_ARG(act >= 1 && act <= 9, "n3d_bias_act: act %d out of range", act);
     N3D_CHECK_ARG(dtype == N3D_DTYPE_F32 || dtype == N3D_DTYPE_F16, "n3d_bias_act: unsupported dtype %d", dtype);
     N3D_CHECK_ARG(!b || (size_b > 0 && step_b > 0), "n3d_bias_act: bad bias geometry");
-    if (numel == 0) return N3D_OK;
+    if (numel == 0) return N3D_OK;                 // nothing to launch; an empty tensor's data pointer may be NULL
+    N3D_CHECK_ARG(x && y, "n3d_bias_act: null pointer");
     const int grid = n3d_grid((numel + 3) / 4, 256);        // 4 elements per thread
     const uintptr_t vec_align = dtype == N3D_DTYPE_F32 ? 15 : 7;     // float4 / 4 x half
     const int vec = (((uintptr_t)x | (uintptr_t)y) & vec_align) == 0;
@@ -252,7 +253,7 @@ __global__ void __launch_bounds__(256) flrelu_up_kernel(const T* __restrict__ x,
     for (int i = threadIdx.x; i < fh * fw; i += blockDim.x) {
         const int fy = i / fw, fx = i % fw;
         const int sy = flip ? fy : fh - 1 - fy, sx = flip ? fx : fw - 1 - fx;
-        sf[i] = fu ? fu[sy * fw + sx] * (float)(up * up) : 1.f;
+        sf[i] = (fu ? fu[sy * fw + sx] : 1.f) * (float)(up * up);     // the identity filter carries the up^2 gain as well
     }
     __syncthreads();
     const int64_t total = (int64_t)N * C * upH * upW;

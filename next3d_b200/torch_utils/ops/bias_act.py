@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from ... import _lib
+from ._layout import suggest_memory_format
 
 
 class _Spec(dict):
@@ -72,7 +73,7 @@ def bias_act(x, b=None, dim=1, act='linear', alpha=None, gain=None, clamp=None, 
 
 def _forward(x, b, dim, spec, alpha, gain, clamp):
     if not (x.is_contiguous() or x.is_contiguous(memory_format=torch.channels_last)):
-        x = x.contiguous()                                                     # plugin requires dense x (bias_act.cpp:51)
+        x = x.contiguous(memory_format=suggest_memory_format(x))               # plugin requires dense x (bias_act.cpp:51)
     y = torch.empty_like(x)
     size_b = step_b = 0
     if b is not None:

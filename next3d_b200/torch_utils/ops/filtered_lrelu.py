@@ -8,6 +8,7 @@ import torch
 
 from ... import _lib
 from . import bias_act, upfirdn2d
+from ._layout import suggest_memory_format
 
 _DTYPES = {torch.float32: 0, torch.float16: 1}
 
@@ -57,6 +58,7 @@ def filtered_lrelu(x, fu=None, fd=None, b=None, up=1, down=1, padding=0, gain=np
         raise RuntimeError('filtered_lrelu: the backward pass (the reference\'s sign-tensor gradient, filtered_lrelu.py:161-270) is not implemented; '
                            'call it under torch.no_grad() or with impl="ref"')
     px0, px1, py0, py1 = _parse_padding(padding)
+    fmt = suggest_memory_format(x)              # the layout the reference's plugin returns (filtered_lrelu.cpp:84)
     x = x.contiguous()
     N, C, H, W = x.shape
     fu2, fd2 = _as_2d(fu, x.device), _as_2d(fd, x.device)
@@ -72,4 +74,4 @@ def filtered_lrelu(x, fu=None, fd=None, b=None, up=1, down=1, padding=0, gain=np
                                            _lib.ptr(bb), y.data_ptr(), tmp.data_ptr(), _DTYPES[x.dtype], N, C, H, W, fuh, fuw, fdh, fdw, up, down,
                                            px0, px1, py0, py1, float(gain), float(slope), float(clamp if clamp is not None else -1),
                                            int(bool(flip_filter)), outH, outW, _lib.stream_ptr(x.device)), 'n3d_filtered_lrelu')
-    return y
+    return y.contiguous(memory_format=fmt)

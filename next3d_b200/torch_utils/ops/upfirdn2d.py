@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from ... import _lib
+from ._layout import suggest_memory_format
 
 _DTYPES = {torch.float32: 0, torch.float16: 1}
 
@@ -95,8 +96,8 @@ def _launch(x, f2d, upx, upy, downx, downy, padx0, padx1, pady0, pady1, flip_fil
     outH = (H * upy + pady0 + pady1 - fh + downy) // downy
     outW = (W * upx + padx0 + padx1 - fw + downx) // downx
     assert outH >= 1 and outW >= 1
-    cl = x.is_contiguous(memory_format=torch.channels_last) and not x.is_contiguous()
-    y = torch.empty([N, C, outH, outW], dtype=x.dtype, device=x.device, memory_format=torch.channels_last if cl else torch.contiguous_format)
+    # y in x's suggested layout, as the reference's plugin allocates it (upfirdn2d.cpp:42); the kernel takes any y strides
+    y = torch.empty([N, C, outH, outW], dtype=x.dtype, device=x.device, memory_format=suggest_memory_format(x))
     xs = (_lib.I64 * 4)(*x.stride())
     ys = (_lib.I64 * 4)(*y.stride())
     _lib.check(_lib.lib.n3d_upfirdn2d(x.data_ptr(), f2d.data_ptr(), y.data_ptr(), _DTYPES[x.dtype], N, C, H, W, xs, ys, fh, fw, upx, upy, downx, downy,

@@ -63,16 +63,23 @@ def _pad4(padding):
     return tuple(padding)
 
 
+def _scaling2(s):
+    """An up / down factor as (x, y): an int or an [x, y] pair, upfirdn2d.py:37-44."""
+    return (s, s) if isinstance(s, int) else tuple(s)
+
+
 def upfirdn2d(x, f, up=1, down=1, padding=0, flip_filter=False, gain=1.0):
-    """zero-insert upsample -> pad/crop -> correlate with the flipped filter -> decimate."""
+    """zero-insert upsample -> pad/crop -> correlate with the flipped filter -> decimate.  up / down: an int or an [x, y] pair."""
     N, C, H, W = x.shape
+    upx, upy = _scaling2(up)
+    downx, downy = _scaling2(down)
     px0, px1, py0, py1 = _pad4(padding)
     if f is None:
-        f = torch.ones(1, 1, dtype=torch.float32)
-    if up > 1:
-        z = x.new_zeros(N, C, H, up, W, up)
+        f = torch.ones(1, 1, dtype=torch.float32, device=x.device)
+    if upx > 1 or upy > 1:
+        z = x.new_zeros(N, C, H, upy, W, upx)
         z[:, :, :, 0, :, 0] = x
-        x = z.reshape(N, C, H * up, W * up)
+        x = z.reshape(N, C, H * upy, W * upx)
     x = F.pad(x, [max(px0, 0), max(px1, 0), max(py0, 0), max(py1, 0)])
     x = x[:, :, max(-py0, 0): x.shape[2] - max(-py1, 0), max(-px0, 0): x.shape[3] - max(-px1, 0)]
     f = f.to(x.dtype) * (gain ** (f.ndim / 2))
@@ -83,7 +90,7 @@ def upfirdn2d(x, f, up=1, down=1, padding=0, flip_filter=False, gain=1.0):
     else:
         x = F.conv2d(x, f[None, None, None, :].repeat(C, 1, 1, 1), groups=C)
         x = F.conv2d(x, f[None, None, :, None].repeat(C, 1, 1, 1), groups=C)
-    return x[:, :, ::down, ::down]
+    return x[:, :, ::downy, ::downx]
 
 
 def upsample2d(x, f, up=2):

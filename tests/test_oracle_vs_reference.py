@@ -84,6 +84,52 @@ def test_filtered_lrelu():
     assert torch.equal(a, o)
 
 
+def _edge_filters():
+    """Filters of the edge cases: the 4-tap filter, a non-square 3x5 one with unequal taps, 1-D taps of length 4 (raw) and 8 (the
+    reference's separable setup_filter)."""
+    g = torch.Generator().manual_seed(6)
+    f35 = torch.rand(3, 5, generator=g) + 0.1
+    return {'f4': oo.setup_filter(), 'f35': f35 / f35.sum(), 'f1d4': torch.tensor([1.0, 2.0, 5.0, 3.0]) / 11,
+            'f1d8': REF.get('setup_filter8', lambda: ref()['upfirdn2d'].setup_filter([1, 2, 3, 4, 4, 3, 2, 1]))}
+
+
+@pytest.mark.parametrize('name,f,up,down,pad,flip,gain', [
+    ('up3x2', 'f4', [3, 2], 1, [2, 1, 1, 2], False, 6.0),
+    ('down3x2_nonsquare', 'f35', 1, [3, 2], [1, 1, 2, 0], False, 1.0),
+    ('updown_1d8', 'f1d8', [2, 3], [2, 1], [3, 4, 4, 3], False, 2.0),
+    ('flip_negpad_nonsquare', 'f35', 1, 1, [-1, 2, 0, -2], True, 1.0),
+    ('flip_1d4_up2', 'f1d4', 2, 1, [-2, 3, 1, -1], True, 4.0),
+    ('negpad_up2_down2', 'f4', 2, 2, [0, -3, -2, 1], False, 4.0),
+])
+def test_upfirdn2d_edges(name, f, up, down, pad, flip, gain):
+    """Asymmetric [x, y] factors, non-square and 1-D filters, flip_filter and negative padding, against the reference's _upfirdn2d_ref."""
+    g = torch.Generator().manual_seed(7)
+    x = torch.randn(2, 3, 9, 11, generator=g)
+    fv = _edge_filters()[f]
+    a = REF.get(f'upfirdn2d_edge-{name}', lambda: ref()['upfirdn2d']._upfirdn2d_ref(x, fv, up=up, down=down, padding=pad, flip_filter=flip, gain=gain))
+    assert torch.equal(a, oo.upfirdn2d(x, fv, up=up, down=down, padding=pad, flip_filter=flip, gain=gain))
+
+
+@pytest.mark.parametrize('name,fu,fd,up,down,pad,flip,clamp', [
+    ('fu_none_up2', None, 'f4', 2, 1, [1, 2, 1, 2], False, None),
+    ('fd_none_up2_down2', 'f4', None, 2, 2, [2, 1, 2, 1], False, None),
+    ('both_none_up2', None, None, 2, 1, 0, False, 0.6),
+    ('fu_none_up2_flip', None, 'f35', 2, 2, [1, 0, 2, 1], True, None),
+    ('1d_up2_down2_flip', 'f1d8', 'f1d8', 2, 2, [6, 5, 6, 5], True, 0.5),
+    ('1d4_up2', 'f1d4', 'f1d4', 2, 1, [3, 2, 3, 2], False, None),
+])
+def test_filtered_lrelu_edges(name, fu, fd, up, down, pad, flip, clamp):
+    """The identity filters (fu / fd = None) at up 2, 1-D filters and flip_filter, against the reference's _filtered_lrelu_ref."""
+    g = torch.Generator().manual_seed(8)
+    x = torch.randn(2, 3, 10, 9, generator=g)
+    b = torch.randn(3, generator=g)
+    fs = _edge_filters()
+    fu, fd = (fs[k] if k else None for k in (fu, fd))
+    kw = dict(fu=fu, fd=fd, b=b, up=up, down=down, padding=pad, flip_filter=flip, clamp=clamp)
+    a = REF.get(f'filtered_lrelu_edge-{name}', lambda: ref()['filtered_lrelu']._filtered_lrelu_ref(x, **kw))
+    assert torch.equal(a, oo.filtered_lrelu(x, **kw))
+
+
 def test_fill_mouth_vs_cv2():
     """Our BFS restatement == the reference's cv2.floodFill-based fill_mouth, including fractional alphas."""
     g = torch.Generator().manual_seed(5)
