@@ -608,6 +608,7 @@ extern "C" int n3d_styles(const float* ws, int N, int num_ws, int wdim, const fl
                           float* styles, int rows, void* stream) {
     N3D_CHECK_ARG(ws && affine_w && affine_b && row_widx && row_scale && row_ooff && row_cin && styles, "n3d_styles: null pointer");
     N3D_CHECK_ARG(wdim % 4 == 0 && rows > 0 && N > 0, "n3d_styles: bad sizes");
+    N3D_CHECK_ARG((((uintptr_t)ws | (uintptr_t)affine_w) & 15) == 0, "n3d_styles: ws and affine_w must be 16-byte aligned");   // float4 loads
     styles_kernel<<<n3d_grid((int64_t)rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(ws, N, num_ws, wdim, affine_w, affine_b, row_widx,
                                                                                       row_scale, row_ooff, row_cin, styles, rows);
     N3D_CHECK_LAUNCH("n3d_styles");

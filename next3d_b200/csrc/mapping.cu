@@ -112,6 +112,7 @@ extern "C" int n3d_mapping(const float* z, const float* c, int N, float c_scale,
                            int truncation_cutoff, int num_ws, float* ws, void* stream) {
     N3D_CHECK_ARG(z && c && embed_w && embed_b && fc0_w && fc0_b && fc1_w && fc1_b && ws && N >= 1 && num_ws >= 1, "n3d_mapping: bad args");
     N3D_CHECK_ARG(truncation_psi == 1.f || w_avg, "n3d_mapping: truncation needs w_avg");
+    N3D_CHECK_ARG((((uintptr_t)fc0_w | (uintptr_t)fc1_w) & 15) == 0, "n3d_mapping: fc0_w and fc1_w must be 16-byte aligned");   // float4 loads
     mapping_kernel<<<N, kThreads, 0, (cudaStream_t)stream>>>(z, c, c_scale, embed_w, embed_b, fc0_w, fc0_b, fc1_w, fc1_b, w_avg, truncation_psi,
                                                              truncation_cutoff, num_ws, ws);
     N3D_CHECK_LAUNCH("n3d_mapping");

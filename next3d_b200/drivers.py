@@ -444,14 +444,17 @@ def interpolate_ws_device(ws_keyframes, w_frames, wraps=2, kind='cubic'):
     """interpolate_ws on the device: the spline is linear in its knots, so its basis B [K * w_frames, K] (interp1d evaluated once on
     the identity, wrap-around tiling folded in) is built on the host and the frames are B @ ws_keyframes in one small kernel
     (n3d_interp_rows) -- the latents never visit the host.  float32; equals interpolate_ws to ~1e-6."""
-    import scipy.interpolate
     from . import kernels as K
-    Kf = ws_keyframes.shape[0]
+    B = interpolation_basis(ws_keyframes.shape[0], w_frames, wraps, kind).to(ws_keyframes.device, torch.float32).contiguous()
+    return K.interp_rows(B, ws_keyframes.to(torch.float32).contiguous())
+
+
+def interpolation_basis(Kf, w_frames, wraps=2, kind='cubic'):
+    """The float64 basis [Kf * w_frames, Kf] of interpolate_ws over Kf keyframes: frame f is sum_k B[f, k] * keyframe k."""
+    import scipy.interpolate
     x = np.arange(-Kf * wraps, Kf * (wraps + 1))
     eye = np.tile(np.eye(Kf), [wraps * 2 + 1, 1])                                  # knot i of the tiled sequence is keyframe i % K
-    B = scipy.interpolate.interp1d(x, eye, kind=kind, axis=0)(np.arange(Kf * w_frames) / w_frames)
-    B = torch.from_numpy(B).to(ws_keyframes.device, torch.float32).contiguous()
-    return K.interp_rows(B, ws_keyframes.to(torch.float32).contiguous())
+    return torch.from_numpy(scipy.interpolate.interp1d(x, eye, kind=kind, axis=0)(np.arange(Kf * w_frames) / w_frames))
 
 
 # ------------------------------------------------------------------------------------------------ grids (--grid of both scripts)

@@ -355,21 +355,32 @@ def sample_grid(planes, grid_n, cube_length, box_warp, dec, sigma_grid, head=0, 
                             *(ptr(t) for t in dec), ptr(sigma_grid), stream_ptr())
 
 
-def mapping(z, c, c_scale, m, truncation_psi=1.0, truncation_cutoff=None, num_ws=28):
-    """MappingNetwork + truncation in one launch.  m: dict with embed_w/embed_b/fc0_w/fc0_b/fc1_w/fc1_b/w_avg fp32 device tensors."""
+def mapping_cutoff(truncation_cutoff, num_ws):
+    """The layers the reference truncates, ws[:, :truncation_cutoff] (networks_stylegan2.py:267; None: all of them), as n3d_mapping's
+    count of leading layers (< 0: all): a negative cutoff leaves its last -cutoff layers untruncated, as the slice does."""
+    if truncation_cutoff is None:
+        return -1
+    c = int(truncation_cutoff)
+    return max(num_ws + c, 0) if c < 0 else c
+
+
+def mapping(z, c, c_scale, m, truncation_psi=1.0, truncation_cutoff=None, num_ws=28, out=None):
+    """MappingNetwork + truncation in one launch.  m: dict with embed_w/embed_b/fc0_w/fc0_b/fc1_w/fc1_b/w_avg fp32 device tensors.
+    out: the [N, num_ws, 512] result, allocated when None."""
     N = z.shape[0]
-    ws = torch.empty(N, num_ws, 512, device=z.device, dtype=torch.float32)
+    ws = torch.empty(N, num_ws, 512, device=z.device, dtype=torch.float32) if out is None else out
     _run('n3d_mapping', ptr(z), ptr(c), N, float(c_scale), ptr(m['embed_w']), ptr(m['embed_b']), ptr(m['fc0_w']), ptr(m['fc0_b']),
                         ptr(m['fc1_w']), ptr(m['fc1_b']), ptr(m['w_avg']), float(truncation_psi),
-                        -1 if truncation_cutoff is None else int(truncation_cutoff), num_ws, ptr(ws), stream_ptr())
+                        mapping_cutoff(truncation_cutoff, num_ws), num_ws, ptr(ws), stream_ptr())
     return ws
 
 
-def interp_rows(B, Y):
-    """out[f] = sum_k B[f,k] * Y[k] for fp32 device tensors B [F,K], Y [K, ...] -> [F, ...]."""
+def interp_rows(B, Y, out=None):
+    """out[f] = sum_k B[f,k] * Y[k] for fp32 device tensors B [F,K], Y [K, ...] -> [F, ...] (allocated when out is None)."""
     F_, K_ = B.shape
     D = Y[0].numel()
-    out = torch.empty((F_,) + tuple(Y.shape[1:]), device=Y.device, dtype=torch.float32)
+    if out is None:
+        out = torch.empty((F_,) + tuple(Y.shape[1:]), device=Y.device, dtype=torch.float32)
     _run('n3d_interp_rows', ptr(B), ptr(Y), F_, K_, D, ptr(out), stream_ptr())
     return out
 
