@@ -14,7 +14,9 @@
  *   - return value: 0 = ok, <0 = error (N3D_ERR_*); n3d_last_error() returns a thread-local message.
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream).
  *   - "NHWC" = channels-last [N,H,W,C]; "split bf16" = two bf16 tensors (hi, lo) with hi+lo ~= the fp32 value
- *     (operands of the 3-product bf16 tensor-core scheme, see DESIGN.md).
+ *     (operands of the 3-product bf16 tensor-core scheme, see DESIGN.md).  "fp16 single" = one fp16 tensor: the operands of
+ *     the opt-in fp16 super-resolution head (one product per k-step), which the reference runs in fp16 on CUDA
+ *     (superresolution.py:268-277, networks_stylegan2.py:547-549 with sr_num_fp16_res > 0).
  */
 #ifndef NEXT3D_B200_H
 #define NEXT3D_B200_H
@@ -108,6 +110,9 @@ typedef struct {
     const float* style;   /* [N, Cout] multiplier applied before the split (next layer's modulation) or NULL */
     int32_t cstride;      /* channel stride of the destination (allows writing into a concat buffer) */
     int32_t coff;         /* channel offset in the destination */
+    int32_t f16;          /* 0 (default): split bf16 (hi, lo).  1: fp16 single -- hi is fp16 [.., cstride] holding the value rounded to
+                             fp16 (the reference's `.to(float16)` of an SR activation), lo is not read.  Any other value ->
+                             N3D_ERR_INVALID_ARG. */
 } N3DSplitOut;
 
 /* Optional ToRGB layer (networks_stylegan2.py:353-357) fused into the epilogue of the convolution that produces its input,
@@ -154,6 +159,11 @@ typedef struct {
     N3DFusedRgb rgb;
     int32_t splits;                          /* > 1: split-K (mode 1 only): K slice s of every tile writes its raw partial sums to */
     int64_t split_stride;                    /*      out_f32 + s * split_stride (elements); reduce with n3d_splitk_epilogue */
+    int32_t f16;                             /* 0 (default): bf16 operands as above.  1: fp16 operands -- a_hi fp16 NHWC, w_hi fp16
+                                                [T, Cout, Cin], nprod must be 1 (a_lo / w_lo are not read): one wgmma...f32.f16.f16 per
+                                                k16 step, fp32 accumulate, as the reference's fp16 SR convolutions on CUDA
+                                                (networks_stylegan2.py:54-79 with x.dtype == float16).  Every used out[k] must then be
+                                                fp16 single (out[k].f16 = 1), and with f16 = 0 none may be. */
 } N3DConvGemm;
 
 int n3d_conv_gemm(const N3DConvGemm* p, void* stream);
@@ -203,6 +213,10 @@ int n3d_wgrad_operand(const float* x, const int64_t x_strides[4], int N, int C, 
  * multiples of 4; else N3D_ERR_INVALID_ARG. */
 int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* hi, void* lo,
                        int out_cstride, int out_coff, void* stream);
+/* n3d_modulate_split with an fp16 single output: out = fp16(x[n,y,x,c] * style[n,c]) -- the first fp16 SR block's input at a
+ * 128^2 rendering, x.to(float16) then the modulation (networks_stylegan2.py:557, 73).  Same argument checks, out in place of hi / lo. */
+int n3d_modulate_f16(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* out, int out_cstride, int out_coff,
+                     void* stream);
 
 /* Second half of an up-sampling modulated conv (conv2d_resample.py:114-131 + networks_stylegan2.py:320-329):
  * raw [(2H+1),(2W+1)] transposed-conv output (fp32 NHWC) -> 4x4 FIR [1,3,3,1]^2/64 * 4, pad 1 -> [2H,2W], then the
@@ -286,6 +300,10 @@ int n3d_mouth_box(const float* lm2d, int N, int32_t* boxes, void* stream);
  * left untouched.  dst may be NULL when only the split output is wanted; hi/lo (optional): split_bf16(value * style[n,c]). */
 int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, float* dst, int DH, int DW,
                   const int32_t* dst_box, const float* style, void* hi, void* lo, void* stream);
+/* n3d_resize_aa with only an fp16 single output: out[n, y, x, c] = fp16(resize(src)[n, y, x, c] * style[n, c]) (style may be NULL) --
+ * the SR input features resized to 128^2 (superresolution.py:282-286), then x.to(float16) and the first fp16 block's modulation. */
+int n3d_resize_aa_f16(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, int DH, int DW, const int32_t* dst_box,
+                      const float* style, void* out, void* stream);
 
 /* planes[n,p,y,x,c] = tex[n,p,y,x,c] * alpha[n,p,y,x] + static[n,y,x,p*32+c] * (1 - alpha)  (triplane_next3d.py:171-174);
  * tex for plane 0 = blended_front NHWC [N,H,W,32] (neural-blending output), planes 1,2 = tex_planes[1:] (plane-major

@@ -27,7 +27,7 @@ class ConvTap(C.Structure):
 
 
 class SplitOut(C.Structure):
-    _fields_ = [('hi', P), ('lo', P), ('style', P), ('cstride', I32), ('coff', I32)]
+    _fields_ = [('hi', P), ('lo', P), ('style', P), ('cstride', I32), ('coff', I32), ('f16', I32)]
 
 
 class FusedRgb(C.Structure):
@@ -48,6 +48,7 @@ class ConvGemm(C.Structure):
         ('oy_mul', I32), ('oy_off', I32), ('ox_mul', I32), ('ox_off', I32), ('OH', I32), ('OW', I32),
         ('rgb', FusedRgb),
         ('splits', I32), ('split_stride', I64),
+        ('f16', I32),
     ]
 
 
@@ -87,6 +88,7 @@ _SIGNATURES = {
     'n3d_conv_wgrad': ([C.POINTER(ConvWgrad), P], C.c_int),
     'n3d_wgrad_operand': ([P, C.POINTER(I64)] + [C.c_int] * 10 + [I64, P, P, P], C.c_int),
     'n3d_modulate_split': ([P, I64, C.c_int, C.c_int, P, P, P, C.c_int, C.c_int, P], C.c_int),
+    'n3d_modulate_f16': ([P, I64, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P], C.c_int),
     'n3d_fir_up_epilogue': ([P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, P, I64, F32, F32, F32, C.POINTER(SplitOut), P, C.c_int, C.c_int, P], C.c_int),
     'n3d_parse_obj_vertices': ([C.c_char_p, I64, P, I64, C.POINTER(I64)], C.c_int),
     'n3d_parse_float_table': ([C.c_char_p, I64, P, I64, C.POINTER(I64), C.POINTER(I64)], C.c_int),
@@ -102,6 +104,7 @@ _SIGNATURES = {
     'n3d_fill_mouth_binarize': ([P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P], C.c_int),
     'n3d_mouth_box': ([P, C.c_int, P, P], C.c_int),
     'n3d_resize_aa': ([P, C.c_int, C.c_int, C.c_int, C.c_int, P, P, C.c_int, C.c_int, P, P, P, P, P], C.c_int),
+    'n3d_resize_aa_f16': ([P, C.c_int, C.c_int, C.c_int, C.c_int, P, C.c_int, C.c_int, P, P, P, P], C.c_int),
     'n3d_blend_planes': ([P, P, P, P, C.c_int, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_blend_planes_views': ([P, P, P, P, C.c_int, C.c_int, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_render_rays': ([C.POINTER(Render), P], C.c_int),

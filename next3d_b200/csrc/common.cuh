@@ -81,6 +81,12 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uin
     lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
+// Two values -> one packed fp16x2 word (element a in the low half), each rounded to nearest: the fp16 single form.
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
 // 32-byte global accesses as two 128-bit halves (sm_90 has no 256-bit LDG/STG): both halves of one sector per thread and call.
 // `p` must be 32-byte aligned.
 __device__ __forceinline__ void st_global_256(void* p, const uint32_t (&w)[8]) {

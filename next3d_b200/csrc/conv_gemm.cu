@@ -18,6 +18,9 @@
 //   and raises the consumers to 240 (2 x 128 x 240 + 128 x 24 = 384 x 168): ptxas allocates each role's code to its own budget (the launch figure it reports is 168).
 //   Launches with wide tiles run as 2-CTA clusters: the two CTAs take neighbouring M tiles of the same n-tile and K steps, and
 //   each loads half of the shared weight tile, multicast into both (decode_tile, the producer, release_stage, launch_conv).
+//   fp16 instances (template F16, N3DConvGemm::f16): fp16 operands, one wgmma...f32.f16.f16 per k16 step, a stage of one A and one
+//   B tile (so the same ring holds twice the K steps), and fp16 single outputs in place of the split pairs.  They serve the opt-in
+//   fp16 super-resolution head; the bf16 instances and their launch rule do not depend on them.
 #include <cstring>
 #include "common.cuh"
 #include <cuda.h>
@@ -148,20 +151,21 @@ __device__ __forceinline__ void k_range(const KParams& P, const TileInfo& t, int
 // Main loop of one tile: one stage = one (tap, channel chunk); a stage is released once its wgmmas retired (wait_group 1 after
 // the next stage's wgmmas are issued, so that the tensor cores always have one group queued).  Each of the warpgroup's 4 warps
 // arrives on the stage's empty barrier (of both CTAs in a cluster).
-template <int BN, int BK, int NPROD>
+template <int BN, int BK, int NPROD, bool F16>
 __device__ __forceinline__ void tile_mainloop(const KParams& P, float (&acc0)[BN / 2], float (&acc1)[BN / 2], int ksteps, uint32_t smem_base,
                                               uint32_t bar_base, int lane, int& s, uint32_t& ph) {
     const uint32_t a_bytes = (uint32_t)P.a_bytes, b_bytes = (uint32_t)P.b_bytes, stage_bytes = (uint32_t)P.stage_bytes;
     const uint32_t empty_base = bar_base + 8u * (uint32_t)P.stages;
+    const uint32_t b_off = F16 ? a_bytes : 2u * a_bytes;               // stage: A hi [| A lo] | B hi [| B lo]
     uint32_t sa = smem_base + (uint32_t)s * stage_bytes;
     mbar_wait(bar_base + 8u * (uint32_t)s, ph, P.err_flag, 3);           // first stage (ksteps >= 1): overwrite the accumulator
-    stage_mma<BN, BK, NPROD, true>(acc0, acc1, sa, sa + a_bytes, sa + 2u * a_bytes, sa + 2u * a_bytes + b_bytes);
+    stage_mma<BN, BK, NPROD, true, F16>(acc0, acc1, sa, sa + a_bytes, sa + b_off, sa + b_off + b_bytes);
     int prev_s = s;
     if (++s == P.stages) { s = 0; ph ^= 1u; }
     for (int ks = 1; ks < ksteps; ++ks) {
         sa = smem_base + (uint32_t)s * stage_bytes;
         mbar_wait(bar_base + 8u * (uint32_t)s, ph, P.err_flag, 3);
-        stage_mma<BN, BK, NPROD, false>(acc0, acc1, sa, sa + a_bytes, sa + 2u * a_bytes, sa + 2u * a_bytes + b_bytes);
+        stage_mma<BN, BK, NPROD, false, F16>(acc0, acc1, sa, sa + a_bytes, sa + b_off, sa + b_off + b_bytes);
         wgmma_wait<1>();
         __syncwarp();
         if (lane == 0) release_stage(P, empty_base + 8u * (uint32_t)prev_s);
@@ -218,8 +222,9 @@ __device__ __forceinline__ void store_raw_tma(const KParams& P, const float (&ac
 }
 
 // ---------------------------------------------------------------------------------------------- the kernel
-template <int BN, int BK>
-__global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ KParams P) {
+// Body of conv_gemm_kernel (bf16 operands) and conv_gemm_f16_kernel (F16: fp16 operands and outputs).
+template <int BN, int BK, bool F16>
+__device__ __forceinline__ void conv_gemm_body(const KParams& P) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-B aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -278,7 +283,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                     // same offset in both CTAs of a cluster.  The rank is read here, not kept: the producer's 24 registers hold no
                     // further live value without spilling.
                     const int r = (int)cluster_ctarank();
-                    const uint32_t sb = sa + 2 * P.a_bytes + (uint32_t)(r * P.b_rows * BK * 2);
+                    const uint32_t sb = sa + (F16 ? 1 : 2) * P.a_bytes + (uint32_t)(r * P.b_rows * BK * 2);
                     const int brow = tn * P.block_n + r * P.b_rows;
                     if (P.cluster == 1) {
                         tma_load_3d(sb, &P.tmB_hi, fb, kc * BK, brow, tap.wtap);
@@ -357,8 +362,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
             int kb, ke;
             k_range(P, ti, kb, ke);
             float accs[2][BN / 2];                                 // rows 0-63 | 64-127; the first stage overwrites them
-            if (P.nprod == 3) tile_mainloop<BN, BK, 3>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
-            else tile_mainloop<BN, BK, 1>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
+            if (F16) tile_mainloop<BN, BK, 1, true>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
+            else if (P.nprod == 3) tile_mainloop<BN, BK, 3, false>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
+            else tile_mainloop<BN, BK, 1, false>(P, accs[0], accs[1], ke - kb, smem_base, bar_base, lane, s, ph);
             if (tile == (item + 1) * P.item_tiles - 1 && other_item < total_items)
                 asm volatile("bar.arrive %0, 256;" ::"r"(4 - g) : "memory");     // the other warpgroup's next item may start
             if (P.tma_store) {
@@ -510,32 +516,50 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
                         }
                     }
                 }
-                // ---- split bf16 outputs (next layers' pre-modulated operands)
+                // ---- split bf16 outputs (next layers' pre-modulated operands), or fp16 single ones in the fp16 instances
 #pragma unroll
                 for (int k = 0; k < 2; ++k) {
                     const N3DSplitOut o = P.out[k];
                     if (!o.hi) continue;
-                    uint32_t h[8], l[8];
+                    if constexpr (F16) {
+                        uint32_t h[8];
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        split_bf16x2(v[2 * j] * (k == 0 ? s0[2 * j] : s1[2 * j]), v[2 * j + 1] * (k == 0 ? s0[2 * j + 1] : s1[2 * j + 1]), h[j], l[j]);
-                    __nv_bfloat16* dh = (__nv_bfloat16*)o.hi + opix * o.cstride + o.coff + co0;
-                    __nv_bfloat16* dl = (__nv_bfloat16*)o.lo + opix * o.cstride + o.coff + co0;
-                    if (nco == 16 && ((((uintptr_t)dh | (uintptr_t)dl) & 31) == 0)) {           // one full 32-byte sector per array
-                        st_global_256(dh, h); st_global_256(dl, l);
-                    } else if (nco == 16 && (((o.cstride | (o.coff + co0)) & 7) == 0)) {
+                        for (int j = 0; j < 8; ++j)
+                            h[j] = pack_half2(v[2 * j] * (k == 0 ? s0[2 * j] : s1[2 * j]), v[2 * j + 1] * (k == 0 ? s0[2 * j + 1] : s1[2 * j + 1]));
+                        __half* dh = (__half*)o.hi + opix * o.cstride + o.coff + co0;
+                        if (nco == 16 && (((uintptr_t)dh & 31) == 0)) {
+                            st_global_256(dh, h);
+                        } else if (nco == 16 && (((o.cstride | (o.coff + co0)) & 7) == 0)) {
 #pragma unroll
-                        for (int j = 0; j < 8; j += 4) {
-                            *reinterpret_cast<uint4*>(dh + 2 * j) = make_uint4(h[j], h[j + 1], h[j + 2], h[j + 3]);
-                            *reinterpret_cast<uint4*>(dl + 2 * j) = make_uint4(l[j], l[j + 1], l[j + 2], l[j + 3]);
+                            for (int j = 0; j < 8; j += 4) *reinterpret_cast<uint4*>(dh + 2 * j) = make_uint4(h[j], h[j + 1], h[j + 2], h[j + 3]);
+                        } else {
+#pragma unroll
+                            for (int j = 0; j < 16; ++j)
+                                if (j < nco) dh[j] = __ushort_as_half((unsigned short)(h[j >> 1] >> ((j & 1) * 16)));
                         }
                     } else {
+                        uint32_t h[8], l[8];
 #pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (j < nco) {
-                                dh[j] = __ushort_as_bfloat16((unsigned short)(h[j >> 1] >> ((j & 1) * 16)));
-                                dl[j] = __ushort_as_bfloat16((unsigned short)(l[j >> 1] >> ((j & 1) * 16)));
+                        for (int j = 0; j < 8; ++j)
+                            split_bf16x2(v[2 * j] * (k == 0 ? s0[2 * j] : s1[2 * j]), v[2 * j + 1] * (k == 0 ? s0[2 * j + 1] : s1[2 * j + 1]), h[j], l[j]);
+                        __nv_bfloat16* dh = (__nv_bfloat16*)o.hi + opix * o.cstride + o.coff + co0;
+                        __nv_bfloat16* dl = (__nv_bfloat16*)o.lo + opix * o.cstride + o.coff + co0;
+                        if (nco == 16 && ((((uintptr_t)dh | (uintptr_t)dl) & 31) == 0)) {           // one full 32-byte sector per array
+                            st_global_256(dh, h); st_global_256(dl, l);
+                        } else if (nco == 16 && (((o.cstride | (o.coff + co0)) & 7) == 0)) {
+#pragma unroll
+                            for (int j = 0; j < 8; j += 4) {
+                                *reinterpret_cast<uint4*>(dh + 2 * j) = make_uint4(h[j], h[j + 1], h[j + 2], h[j + 3]);
+                                *reinterpret_cast<uint4*>(dl + 2 * j) = make_uint4(l[j], l[j + 1], l[j + 2], l[j + 3]);
                             }
+                        } else {
+#pragma unroll
+                            for (int j = 0; j < 16; ++j)
+                                if (j < nco) {
+                                    dh[j] = __ushort_as_bfloat16((unsigned short)(h[j >> 1] >> ((j & 1) * 16)));
+                                    dl[j] = __ushort_as_bfloat16((unsigned short)(l[j >> 1] >> ((j & 1) * 16)));
+                                }
+                        }
                     }
                 }
             }
@@ -572,6 +596,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     }
 }
 
+template <int BN, int BK>
+__global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ KParams P) { conv_gemm_body<BN, BK, false>(P); }
+template <int BN, int BK>
+__global__ void __launch_bounds__(kThreads, 1) conv_gemm_f16_kernel(const __grid_constant__ KParams P) { conv_gemm_body<BN, BK, true>(P); }
+
 // ---------------------------------------------------------------------------------------------- host side
 int pow2_ceil(int v) { int p = 1; while (p < v) p <<= 1; return p; }
 
@@ -588,6 +617,10 @@ struct SubSpec { int tap_begin, ntaps, y0, x0, MH, MW, oy_off, ox_off; };
 int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nint, int nsub, const SubSpec* specs, void* stream) {
     N3D_CHECK_ARG(p && p->a_hi && p->w_hi, "n3d_conv_gemm: null operand");
     N3D_CHECK_ARG(p->nprod == 1 || p->nprod == 3, "n3d_conv_gemm: nprod must be 1 or 3");
+    N3D_CHECK_ARG(p->f16 == 0 || (p->f16 == 1 && p->nprod == 1), "n3d_conv_gemm: f16 must be 0 or 1, and fp16 operands take nprod 1");
+    for (int k = 0; k < 2; ++k)
+        N3D_CHECK_ARG(!p->out[k].hi || p->out[k].f16 == p->f16, "n3d_conv_gemm: output %d must be %s (out.f16 = %d)", k,
+                      p->f16 ? "fp16 single with fp16 operands" : "split bf16 with bf16 operands", p->f16);
     N3D_CHECK_ARG(p->nprod == 1 || (p->a_lo && p->w_lo), "n3d_conv_gemm: nprod 3 needs lo operands");
     N3D_CHECK_ARG(p->Cin >= 8 && p->Cin % 8 == 0, "n3d_conv_gemm: Cin %d must be a multiple of 8 (TMA 16-byte strides)", p->Cin);
     N3D_CHECK_ARG(p->Cout >= 1 && p->N >= 1, "n3d_conv_gemm: bad sizes");
@@ -596,7 +629,8 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     // the epilogue's vector stores (float4 / uint4 / 256-bit) test strides and offsets, not the base pointers
     N3D_CHECK_ARG(((uintptr_t)p->out_f32 & 15) == 0, "n3d_conv_gemm: out_f32 must be 16-byte aligned");
     for (int k = 0; k < 2; ++k)
-        N3D_CHECK_ARG((((uintptr_t)p->out[k].hi | (uintptr_t)p->out[k].lo) & 15) == 0, "n3d_conv_gemm: split output %d (hi / lo) must be 16-byte aligned", k);
+        N3D_CHECK_ARG((((uintptr_t)p->out[k].hi | (uintptr_t)p->out[k].lo) & 15) == 0 && (p->f16 || !p->out[k].hi || p->out[k].lo),
+                      "n3d_conv_gemm: split output %d (hi / lo) must be 16-byte aligned, and a split bf16 output needs both", k);
     // the accumulating fp32 store adds the old values into the epilogue's registers before the split outputs are formed from them
     N3D_CHECK_ARG(!p->f32_accumulate || (!p->out[0].hi && !p->out[1].hi), "n3d_conv_gemm: f32_accumulate cannot be combined with split outputs");
     const int splits = p->splits > 1 ? p->splits : 1;
@@ -665,11 +699,12 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     K.tiles_n = n3d_div_up(p->Cout, bn);
     K.item_tiles = item_tiles;
     // block_k: 64-channel stages where the ring still holds kMinStages of them, else 32 (same (tap, 16-channel) MMA sequence, so
-    // the same accumulation order either way)
-    const int block_k = (p->Cin % 64 == 32 || kRingBytes / (2 * (kBlockM + bn) * 64 * 2) < kMinStages) ? 32 : 64;
+    // the same accumulation order either way).  A bf16 stage holds the hi and lo tiles of A and B, an fp16 stage one of each.
+    const int tiles_per_stage = p->f16 ? 1 : 2;
+    const int block_k = (p->Cin % 64 == 32 || kRingBytes / (tiles_per_stage * (kBlockM + bn) * 64 * 2) < kMinStages) ? 32 : 64;
     K.a_bytes = kBlockM * block_k * 2;
     K.b_bytes = bn * block_k * 2;
-    K.stage_bytes = 2 * K.a_bytes + 2 * K.b_bytes;
+    K.stage_bytes = tiles_per_stage * (K.a_bytes + K.b_bytes);
     K.stages = min(kMaxStages, kRingBytes / K.stage_bytes);
     K.cin_chunks = n3d_div_up(p->Cin, block_k);
     if (splits > 1) {                                        // every K slice must own at least one step
@@ -681,11 +716,13 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     if (!D) return N3D_ERR_CUDA;
     const int smem = K.stages * K.stage_bytes + 2 * kEpiBytes + 8 * (2 * K.stages) + 1024;
     typedef void (*ConvKernel)(const KParams);
-    const ConvKernel kernels[2][5] = {
-        {conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
-        {conv_gemm_kernel<16, 64>, conv_gemm_kernel<32, 64>, conv_gemm_kernel<64, 64>, conv_gemm_kernel<96, 64>, conv_gemm_kernel<128, 64>}};
+    const ConvKernel kernels[2][2][5] = {
+        {{conv_gemm_kernel<16, 32>, conv_gemm_kernel<32, 32>, conv_gemm_kernel<64, 32>, conv_gemm_kernel<96, 32>, conv_gemm_kernel<128, 32>},
+         {conv_gemm_kernel<16, 64>, conv_gemm_kernel<32, 64>, conv_gemm_kernel<64, 64>, conv_gemm_kernel<96, 64>, conv_gemm_kernel<128, 64>}},
+        {{conv_gemm_f16_kernel<16, 32>, conv_gemm_f16_kernel<32, 32>, conv_gemm_f16_kernel<64, 32>, conv_gemm_f16_kernel<96, 32>, conv_gemm_f16_kernel<128, 32>},
+         {conv_gemm_f16_kernel<16, 64>, conv_gemm_f16_kernel<32, 64>, conv_gemm_f16_kernel<64, 64>, conv_gemm_f16_kernel<96, 64>, conv_gemm_f16_kernel<128, 64>}}};
     const int bi = bn == 16 ? 0 : bn == 32 ? 1 : bn == 64 ? 2 : bn == 96 ? 3 : 4;
-    const ConvKernel kern = kernels[block_k == 64][bi];
+    const ConvKernel kern = kernels[p->f16][block_k == 64][bi];
     int rc;
     if ((rc = n3d_smem_optin((const void*)kern, 227 * 1024, "n3d_conv_gemm")) != N3D_OK) return rc;
     // Cluster of 2 for the wide tiles (block_n 96 and 128) without split-K, where some sub-problem has two M tiles to pair.  The
@@ -728,7 +765,7 @@ int launch_conv(const N3DConvGemm* p, const N3DConvTap* taps, int ntaps, int nin
     const uint64_t wstr[2] = {wdims[0] * 2, wdims[0] * wdims[1] * 2};
     const uint32_t wbox[3] = {(uint32_t)block_k, (uint32_t)K.b_rows, 1u};   // bn / 2 is a multiple of 8: whole swizzle atoms
     const CUtensorMapSwizzle swz = block_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    const CUtensorMapDataType bf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const CUtensorMapDataType bf16 = p->f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;   // operand type
     for (int b = 0; b < K.nbox; ++b) {
         const KParams::Sub& S = K.sub[box_sub[b]];
         const uint32_t abox[4] = {(uint32_t)block_k, (uint32_t)S.TW, (uint32_t)S.TH, (uint32_t)S.TN};

@@ -64,6 +64,8 @@ __global__ void __launch_bounds__(256) demod_kernel(const float* __restrict__ st
 }
 
 // ---------------------------------------------------------------------------------------------- modulate + split
+// F16: one fp16 single output in hi (lo unused) instead of the split pair.
+template <bool F16>
 __global__ void __launch_bounds__(256) modulate_split_kernel(const float* __restrict__ x, int64_t npix, int N, int C,
                                                              const float* __restrict__ style, __nv_bfloat16* __restrict__ hi,
                                                              __nv_bfloat16* __restrict__ lo, int cstride, int coff) {
@@ -78,9 +80,13 @@ __global__ void __launch_bounds__(256) modulate_split_kernel(const float* __rest
             const float4 s = __ldg(reinterpret_cast<const float4*>(style + (int64_t)n * C) + c4);
             v.x *= s.x; v.y *= s.y; v.z *= s.z; v.w *= s.w;
         }
+        const int64_t o = pix * cstride + coff + c4 * 4;
+        if constexpr (F16) {
+            *reinterpret_cast<uint2*>(hi + o) = make_uint2(pack_half2(v.x, v.y), pack_half2(v.z, v.w));
+            continue;
+        }
         uint2 h, l;
         split_bf16x2(v.x, v.y, h.x, l.x); split_bf16x2(v.z, v.w, h.y, l.y);
-        const int64_t o = pix * cstride + coff + c4 * 4;
         *reinterpret_cast<uint2*>(hi + o) = h;
         *reinterpret_cast<uint2*>(lo + o) = l;
     }
@@ -151,7 +157,8 @@ __device__ __forceinline__ void epi_advance2(EpiCursor& P, const EpiParams& E, i
     P.sp[1] += rows2 * E.out[1].cstride;
 }
 
-// bias_act (lrelu with 0 <= slope <= 1: max(t, slope * t)) + clamp + the fp32 / modulated split-bf16 stores of one pixel.
+// bias_act (lrelu with 0 <= slope <= 1: max(t, slope * t)) + clamp + the fp32 / modulated split-bf16 (or fp16 single) stores of one
+// pixel.
 // nzg = noise * gain; dpix = pixel offset from the cursor (0, 1, W2, W2 + 1).
 __device__ __forceinline__ void epi_store(const EpiParams& E, const EpiVec& V, const EpiCursor& P, const float4& acc, float nzg, int dpix) {
     float4 t = f4_fma4(acc, V.dcg, make_float4(V.bsg.x + nzg, V.bsg.y + nzg, V.bsg.z + nzg, V.bsg.w + nzg));
@@ -167,9 +174,13 @@ __device__ __forceinline__ void epi_store(const EpiParams& E, const EpiVec& V, c
         const N3DSplitOut o = E.out[k];
         if (!o.hi) continue;
         const float4 m = f4_mul4(t, V.st[k]);
+        const int64_t off = P.sp[k] + dpix * o.cstride;
+        if (o.f16) {
+            *reinterpret_cast<uint2*>((__half*)o.hi + off) = make_uint2(pack_half2(m.x, m.y), pack_half2(m.z, m.w));
+            continue;
+        }
         uint2 h, l;
         split_bf16x2(m.x, m.y, h.x, l.x); split_bf16x2(m.z, m.w, h.y, l.y);
-        const int64_t off = P.sp[k] + dpix * o.cstride;
         *reinterpret_cast<uint2*>((__nv_bfloat16*)o.hi + off) = h;
         *reinterpret_cast<uint2*>((__nv_bfloat16*)o.lo + off) = l;
     }
@@ -649,6 +660,8 @@ static int make_epi(EpiParams* E, const char* who, const float* dcoef, const flo
         N3D_CHECK_ARG(!out[k].hi || (out[k].cstride % 4 == 0 && out[k].coff % 4 == 0), "%s: unaligned split output", who);
         N3D_CHECK_ARG(!out[k].hi || (((uintptr_t)out[k].hi | (uintptr_t)out[k].lo | (uintptr_t)out[k].style) & 15) == 0,
                       "%s: split output %d (hi / lo / style) must be 16-byte aligned", who, k);
+        N3D_CHECK_ARG(!out[k].hi || out[k].f16 == 1 || (out[k].f16 == 0 && out[k].lo), "%s: output %d: f16 must be 0 (split bf16, hi and lo) or 1 "
+                      "(fp16 single)", who, k);
     }
     N3D_CHECK_ARG(!out_f32 || (f32_cstride % 4 == 0 && f32_coff % 4 == 0), "%s: unaligned fp32 output", who);
     N3D_CHECK_ARG(((uintptr_t)out_f32 & 15) == 0, "%s: out_f32 must be 16-byte aligned", who);
@@ -664,9 +677,22 @@ extern "C" int n3d_modulate_split(const float* x, int64_t npix_per_img, int N, i
     N3D_CHECK_ARG((((uintptr_t)x | (uintptr_t)style) & 15) == 0, "n3d_modulate_split: x and style must be 16-byte aligned");   // float4 loads
     N3D_CHECK_ARG((((uintptr_t)hi | (uintptr_t)lo) & 7) == 0, "n3d_modulate_split: hi and lo must be 8-byte aligned");          // uint2 stores
     const int64_t total = (int64_t)N * npix_per_img * (C / 4);
-    modulate_split_kernel<<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)hi,
-                                                                                     (__nv_bfloat16*)lo, out_cstride, out_coff);
+    modulate_split_kernel<false><<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)hi,
+                                                                                            (__nv_bfloat16*)lo, out_cstride, out_coff);
     N3D_CHECK_LAUNCH("n3d_modulate_split");
+    return N3D_OK;
+}
+
+extern "C" int n3d_modulate_f16(const float* x, int64_t npix_per_img, int N, int C, const float* style, void* out, int out_cstride,
+                                int out_coff, void* stream) {
+    N3D_CHECK_ARG(x && out, "n3d_modulate_f16: null pointer");
+    N3D_CHECK_ARG(C % 4 == 0 && out_cstride % 4 == 0 && out_coff % 4 == 0, "n3d_modulate_f16: channels must be multiples of 4");
+    N3D_CHECK_ARG((((uintptr_t)x | (uintptr_t)style) & 15) == 0, "n3d_modulate_f16: x and style must be 16-byte aligned");     // float4 loads
+    N3D_CHECK_ARG(((uintptr_t)out & 7) == 0, "n3d_modulate_f16: out must be 8-byte aligned");                                   // uint2 stores
+    const int64_t total = (int64_t)N * npix_per_img * (C / 4);
+    modulate_split_kernel<true><<<n3d_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(x, npix_per_img, N, C, style, (__nv_bfloat16*)out,
+                                                                                           nullptr, out_cstride, out_coff);
+    N3D_CHECK_LAUNCH("n3d_modulate_f16");
     return N3D_OK;
 }
 

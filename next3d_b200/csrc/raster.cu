@@ -345,12 +345,17 @@ __device__ __forceinline__ bool resize_window(const int* __restrict__ src_box, c
     return w.ih > 0 && w.iw > 0 && w.oh > 0 && w.ow > 0;
 }
 
+// lo == NULL with hi set: one fp16 single output in hi (n3d_resize_aa_f16) instead of the split pair
 __device__ __forceinline__ void resize_store(float acc, int64_t o, int n, int C, int c, float* __restrict__ dst, const float* __restrict__ style,
                                              __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
     if (dst) dst[o] = acc;
     if (hi) {
         float s = acc;
         if (style) s *= __ldg(style + (int64_t)n * C + c);
+        if (!lo) {
+            reinterpret_cast<__half*>(hi)[o] = __float2half_rn(s);
+            return;
+        }
         __nv_bfloat16 h, l;
         split_bf16(s, h, l);
         hi[o] = h; lo[o] = l;
@@ -557,10 +562,10 @@ extern "C" int n3d_mouth_box(const float* lm2d, int N, int32_t* boxes, void* str
     return N3D_OK;
 }
 
-extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, float* dst, int DH, int DW,
-                             const int32_t* dst_box, const float* style, void* hi, void* lo, void* stream) {
-    N3D_CHECK_ARG(src && (dst || hi) && N > 0 && C > 0, "n3d_resize_aa: bad args");
-    N3D_CHECK_ARG(!hi || lo, "n3d_resize_aa: hi without lo");
+namespace {
+// n3d_resize_aa and n3d_resize_aa_f16 (lo == NULL: hi is the fp16 single output)
+int launch_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, float* dst, int DH, int DW,
+                     const int32_t* dst_box, const float* style, void* hi, void* lo, void* stream) {
     const bool wide = (C % 4 == 0) && C <= 128 && (32 % (C / 4) == 0) && ((uintptr_t)src % 16 == 0);
     const int ppw = 4;
     if (wide)
@@ -571,6 +576,20 @@ extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, con
             src, N, SH, SW, C, src_box, dst, DH, DW, dst_box, style, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo);
     N3D_CHECK_LAUNCH("n3d_resize_aa");
     return N3D_OK;
+}
+}  // namespace
+
+extern "C" int n3d_resize_aa(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, float* dst, int DH, int DW,
+                             const int32_t* dst_box, const float* style, void* hi, void* lo, void* stream) {
+    N3D_CHECK_ARG(src && (dst || hi) && N > 0 && C > 0, "n3d_resize_aa: bad args");
+    N3D_CHECK_ARG(!hi || lo, "n3d_resize_aa: hi without lo");
+    return launch_resize_aa(src, N, SH, SW, C, src_box, dst, DH, DW, dst_box, style, hi, lo, stream);
+}
+
+extern "C" int n3d_resize_aa_f16(const float* src, int N, int SH, int SW, int C, const int32_t* src_box, int DH, int DW,
+                                 const int32_t* dst_box, const float* style, void* out, void* stream) {
+    N3D_CHECK_ARG(src && out && N > 0 && C > 0, "n3d_resize_aa_f16: bad args");
+    return launch_resize_aa(src, N, SH, SW, C, src_box, nullptr, DH, DW, dst_box, style, out, nullptr, stream);
 }
 
 extern "C" int n3d_blend_planes_views(const float* blended_front, const float* tex_planes, const float* alpha, const float* static_planes,

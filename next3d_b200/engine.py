@@ -8,7 +8,10 @@ Execution model (see DESIGN.md):
     demodulation is applied in the epilogue), with noise / bias / lrelu / clamp / next-layer modulation / bf16 split fused;
   * up-convs: 4 parity-class GEMMs (stride-2 transposed conv, conv2d_resample.py:114-127) + one FIR-epilogue kernel;
   * down-convs: FIR + parity split kernel, then one GEMM over 9 unit-stride taps;
-  * mesh path, volume renderer, resizes, blending: one kernel each (raster.cu, render_fused.cu).
+  * mesh path, volume renderer, resizes, blending: one kernel each (raster.cu, render_fused.cu);
+  * super-resolution in fp16 (Engine.sr_precision = 'fp16', opt-in): the same launches on fp16 single activations and weights, one
+    product per k-step: the reference's SR precision on CUDA with sr_num_fp16_res > 0, rounded at the engine's own points
+    (INTEGRATION.md section 1).
 Reference call order: triplane_next3d.py:117-188.
 """
 import contextlib
@@ -49,6 +52,19 @@ class Split:
         return self.hi.shape[-1]
 
 
+class Half:
+    """fp16 single NHWC activation of the fp16 super-resolution head (lo is None: no second tensor)."""
+    __slots__ = ('hi', 'lo')
+
+    def __init__(self, shape, device):
+        self.hi = torch.empty(shape, dtype=torch.float16, device=device)
+        self.lo = None
+
+    @property
+    def C(self):
+        return self.hi.shape[-1]
+
+
 @dataclasses.dataclass(eq=False)
 class _Layer:
     """A packed convolution layer, with the part of its epilogue that its place in the network fixes.  Engine.mod holds the
@@ -63,6 +79,7 @@ class _Layer:
     w_lo: torch.Tensor
     bias: torch.Tensor = None
     w_f32: torch.Tensor = None              # fp32 [Cout, Cin] of a ToRGB layer of <= 4 channels: the fused-ToRGB epilogue operand
+    w16: torch.Tensor = None                # fp16 [k*k, Cout, Cin] of an SR conv, pre-normalised as for fp16 (Engine._pack)
     noise: torch.Tensor = None              # noise_const * noise_strength
     noise_strength: torch.Tensor = None
     clamp: float = -1.0                     # -1: no conv_clamp
@@ -135,6 +152,7 @@ class Engine:
         self._side = None                      # side streams of the concurrent branches (compute_planes)
         self.concurrent = True                  # False: the three branches of compute_planes run on one stream (per-kernel timing)
         self.splitk = True                      # False: every conv runs as one conv_gemm pass (the reference of the split-K test)
+        self.sr_precision = 'fp32'              # 'fp16': the super-resolution head on fp16 operands (TriPlaneGenerator.sr_precision)
 
     # ------------------------------------------------------------------------------------------ packing (one-time)
     def _add_mod(self, sd, name, cin, cout, k, up, widx, is_rgb=False, clamp=None, noise=True):
@@ -235,6 +253,18 @@ class Engine:
             woff.append(torch.arange(L.cout, dtype=torch.int64) * L.cin + acc)
             acc += L.cout * L.cin
         self.d_woff = torch.cat(woff).to(self.device)
+        # fp16 SR: the reference pre-normalises each SR conv's weights for fp16, W * (1 / sqrt(Cin k^2) / max|W[o]|)
+        # (networks_stylegan2.py:54-56).  The gain is folded into the fp16 weights and into their demodulation table wsq16;
+        # demodulation cancels it, so only the fp16 rounding sees it.
+        wsq16 = []
+        for L in dl:
+            w = sd[f'{L.name}.weight'].float()
+            if L.name.startswith('superresolution.'):
+                g = 1.0 / math.sqrt(L.cin * L.k * L.k) / w.abs().amax(dim=[1, 2, 3])
+                L.w16 = K.pack_conv_weight_f16(w, g)
+                w = w * g.reshape(-1, 1, 1, 1)
+            wsq16.append(w.square().sum(dim=[2, 3]).reshape(-1))
+        self.wsq16 = torch.cat(wsq16).contiguous()
         self.d_cin = torch.cat([torch.full((L.cout,), L.cin, dtype=torch.int32) for L in dl]).to(self.device)
         self.d_cout = torch.cat([torch.full((L.cout,), L.cout, dtype=torch.int32) for L in dl]).to(self.device)
 
@@ -301,9 +331,9 @@ class Engine:
         return (torch.randn(self._N, res, res, device=self.device) * L.noise_strength).contiguous(), res * res
 
     def _out(self, buf, consumer=None, coff=0):
-        """SplitOut descriptor writing into `buf` pre-multiplied by `consumer`'s style (None = unmodulated)."""
+        """SplitOut descriptor writing into `buf` (Split, or Half: fp16 single) pre-multiplied by `consumer`'s style (None = unmodulated)."""
         style = self._style(self.mod[consumer]) if consumer else None
-        return K.make_split_out(buf.hi, buf.lo, style, buf.C, coff)
+        return K.make_split_out(buf.hi, buf.lo, style, buf.C, coff, f16=buf.lo is None)
 
     # ------------------------------------------------------------------------------------------ layers
     def _epilogue(self, L, noise_mode='none', outs=(), f32=None, accumulate=False):
@@ -321,17 +351,18 @@ class Engine:
         return dict(out=img, weight=L.w_f32, style=self._style(L), bias=L.bias, clamp=L.clamp, nchw=nchw, accumulate=True)
 
     def _conv(self, L, a, res, epi, rgb=None):
-        """Layer L on the split activation `a` (modulated layers: already pre-multiplied by L's style) at input resolution `res`, with
+        """Layer L on the activation `a` (Split, or Half with L's fp16 weights; modulated layers: already pre-multiplied by L's style) at input resolution `res`, with
         the epilogue `epi` of _epilogue and the fused ToRGB `rgb` of _fused_rgb: a stride-2 transposed conv (4 parity classes into a
         raw sum, then the FIR-up epilogue), a stride-2 conv over the parity-split input, split-K (splitk_maxres), or one pass.
         Algorithmic FLOPs = 2 * Cin * Cout * taps * M-space positions (one product)."""
         N = self._N
         accumulate = epi.pop('f32_accumulate')                 # conv_gemm's alone: the split-K and FIR-up epilogues overwrite
+        w_hi, w_lo, nprod = (L.w16, None, 1) if a.lo is None else (L.w_hi, L.w_lo, self.nprod)
         if L.up == 2:
             assert rgb is None and not accumulate
             raw = self._f32(N, 2 * res + 1, 2 * res + 1, L.cout)
             self._timed(L, 2.0 * L.cin * L.cout * N * (3 * res + 2) ** 2, res + 1, 9,       # taps x positions over the 4 parity classes
-                        K.conv_transposed_gemm, a.hi, a.lo, L.w_hi, L.w_lo, N, res, res, raw, nprod=self.nprod)
+                        K.conv_transposed_gemm, a.hi, a.lo, w_hi, w_lo, N, res, res, raw, nprod=nprod)
             K.fir_up_epilogue(raw, L.cout, **epi)
             return
         M = res // L.down
@@ -340,12 +371,12 @@ class Engine:
         if L.k == 3 and L.down == 1 and self.splitk and res <= self.splitk_maxres and rgb is None and not accumulate:
             S = 9
             part = self._f32(S, N, res, res, L.cout)
-            self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, L.w_hi, L.w_lo, taps, N, M, M, nprod=self.nprod, mode=1,
+            self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, w_hi, w_lo, taps, N, M, M, nprod=nprod, mode=1,
                         out_f32=part, f32_cstride=L.cout, splits=S, split_stride=N * res * res * L.cout)
             self._timed(L, 0.0, M, 0, K.splitk_epilogue, part, **epi)         # the reduction is conv time (0 extra FLOPs)
             return
-        self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, L.w_hi, L.w_lo, taps, N, M, M, a_img_mul=N if L.down == 2 else 0,
-                    nprod=self.nprod, rgb=rgb, f32_accumulate=accumulate, **epi)
+        self._timed(L, flops, M, len(taps), K.conv_gemm, a.hi, a.lo, w_hi, w_lo, taps, N, M, M, a_img_mul=N if L.down == 2 else 0,
+                    nprod=nprod, rgb=rgb, f32_accumulate=accumulate, **epi)
 
     # ------------------------------------------------------------------------------------------ networks
     def _synthesis_blocks(self, prefix, x, res_list, cimg, noise_mode, concat_next=None, img=None):
@@ -465,8 +496,12 @@ class Engine:
         return self._synthesis_blocks(prefix, x, dec_res, cfg.plane_ch, noise_mode, concat_next=concat_next)
 
     def _superresolution(self, feat, noise_mode_sr, image_out):
-        """SuperresolutionHybrid8XDC / 4X (superresolution.py:77-88, 279-290).  feat: fp32 NHWC [N,R,R,32]."""
+        """SuperresolutionHybrid8XDC / 4X (superresolution.py:77-88, 279-290).  feat: fp32 NHWC [N,R,R,32].  With sr_precision 'fp16'
+        the activations between the SR convolutions are fp16 single tensors (x.to(float16) at each block's entry, networks_stylegan2.py:557)
+        and the convolutions take the fp16 weights; the ToRGB sums, the skip image and `image_out` stay fp32."""
         N, dev, cfg = self._N, self.device, self.cfg
+        f16 = self.sr_precision == 'fp16'
+        Act = Half if f16 else Split
         R = feat.shape[1]
         p0, p1 = 'superresolution.block0', 'superresolution.block1'
         c0, c1 = _config.sr_channels(cfg)
@@ -476,20 +511,26 @@ class Engine:
             raise RuntimeError('next3d_b200: sr_antialias=False with a neural rendering resolution above 128 (a plain bilinear minification) is not '
                                'implemented')
         (b0_conv0, b0_conv1, b0_torgb), (b1_conv0, b1_conv1, b1_torgb) = [[self.mod[f'{p}.{n}'] for n in ('conv0', 'conv1', 'torgb')] for p in (p0, p1)]
-        x = Split((N, r0, r0, cfg.plane_ch), dev)
+        x = Act((N, r0, r0, cfg.plane_ch), dev)
         rgb_lo = feat[..., :3].contiguous()                                    # image_raw channels (tiny copy)
         if need:
-            K.resize_aa(feat, None, r0, r0, style=self._style(b0_conv0), hi=x.hi, lo=x.lo)
+            if f16:
+                K.resize_aa_f16(feat, x.hi, style=self._style(b0_conv0))
+            else:
+                K.resize_aa(feat, None, r0, r0, style=self._style(b0_conv0), hi=x.hi, lo=x.lo)
             rgb = self._f32(N, r0, r0, 3)
             K.resize_aa(rgb_lo, rgb)
         else:
-            K.modulate_split(feat, self._style(b0_conv0), x.hi, x.lo)
+            if f16:
+                K.modulate_f16(feat, self._style(b0_conv0), x.hi)
+            else:
+                K.modulate_split(feat, self._style(b0_conv0), x.hi, x.lo)
             rgb = rgb_lo
         # block0
         res0 = r0 * (2 if cfg.sr_module == '8XDC' else 1)
-        x1 = Split((N, res0, res0, c0), dev)
+        x1 = Act((N, res0, res0, c0), dev)
         self._conv(b0_conv0, x, r0, self._epilogue(b0_conv0, noise_mode_sr, [self._out(x1, f'{p0}.conv1')]))
-        x2 = Split((N, res0, res0, c0), dev)
+        x2 = Act((N, res0, res0, c0), dev)
         if cfg.sr_module == '8XDC':
             img = self._f32(N, res0, res0, 3)
             K.upsample2d_nhwc(rgb, img)
@@ -499,7 +540,7 @@ class Engine:
         self._conv(b0_conv1, x1, res0, self._epilogue(b0_conv1, noise_mode_sr, [self._out(x2, f'{p1}.conv0')]), rgb=self._fused_rgb(b0_torgb, img))
         # block1
         res1 = res0 * 2
-        x3 = Split((N, res1, res1, c1), dev)
+        x3 = Act((N, res1, res1, c1), dev)
         self._conv(b1_conv0, x2, res0, self._epilogue(b1_conv0, noise_mode_sr, [self._out(x3, f'{p1}.conv1')]))
         K.upsample2d_nhwc(img, image_out, y_nchw=True)
         self._conv(b1_conv1, x3, res1, self._epilogue(b1_conv1, noise_mode_sr, []), rgb=self._fused_rgb(b1_torgb, image_out, nchw=True))
@@ -562,7 +603,7 @@ class Engine:
         self._styles = self._f32(self.style_elems * N)
         self._dcoefs = self._f32(self.dcoef_elems * N)
         K.styles(ws, self.aff_w, self.aff_b, self.row_widx, self.row_scale, s_ooff, self.row_cin, self._styles)
-        K.demod(self._styles, self.wsq, self.d_woff, self.d_cin, d_soff, d_ooff, self.d_cout, self._dcoefs, N)
+        K.demod(self._styles, self.wsq16 if self.sr_precision == 'fp16' else self.wsq, self.d_woff, self.d_cin, d_soff, d_ooff, self.d_cout, self._dcoefs, N)
 
     def _compute_planes(self, ws, v, noise_mode='const', return_intermediates=False, cache_backbone=False, use_cached_backbone=False):
         cfg, dev = self.cfg, self.device
@@ -737,7 +778,7 @@ class Engine:
         rk = self.rk
         return (R, rk['depth_resolution'], rk['depth_resolution_importance'], float(rk['ray_start']), float(rk['ray_end']), float(rk['box_warp']),
                 bool(rk.get('white_back', False)), rk['superresolution_noise_mode'], bool(rk.get('sr_antialias', True)),
-                bool(rk.get('return_normal', False)))
+                bool(rk.get('return_normal', False)), self.sr_precision)
 
     def _replay(self, key, inputs, run, seed):
         """Capture run(static inputs) once per key into a CUDA graph and replay it: inputs are copied into static buffers (plus a

@@ -1,7 +1,8 @@
 """Thin torch-tensor wrappers over the C ABI (one Python function per extern "C" entry point of the engine).
 
 Tensors are only used as owners of device memory; every call passes raw pointers + sizes and the current CUDA
-stream.  Layout conventions: activations NHWC fp32 or split bf16 (hi, lo); weights packed [T, Cout, Cin] split bf16.
+stream.  Layout conventions: activations NHWC fp32 or split bf16 (hi, lo); weights packed [T, Cout, Cin] split bf16.  The opt-in
+fp16 super-resolution head uses fp16 single tensors instead of the split pairs (the `f16` arguments).
 """
 import ctypes as C
 
@@ -58,13 +59,22 @@ def taps_stride2():
     return [(ky >> 1, kx >> 1, (ky & 1) * 2 + (kx & 1), ky * 3 + kx) for ky in range(3) for kx in range(3)]
 
 
-def make_split_out(hi=None, lo=None, style=None, cstride=0, coff=0):
-    return _lib.SplitOut(ptr(hi), ptr(lo), ptr(style), cstride, coff)
+def pack_conv_weight_f16(w, gain=1.0):
+    """[Cout, Cin, kh, kw] fp32 -> fp16 [kh*kw, Cout, Cin] (tap-major), pre-multiplied by `gain` ([Cout] or a scalar) before the rounding."""
+    cout, cin, kh, kw = w.shape
+    g = torch.as_tensor(gain, dtype=torch.float32, device=w.device).reshape(-1, 1, 1, 1)
+    return (w.to(torch.float32) * g).permute(2, 3, 0, 1).reshape(kh * kw, cout, cin).to(torch.float16).contiguous()
+
+
+def make_split_out(hi=None, lo=None, style=None, cstride=0, coff=0, f16=False):
+    """Output descriptor: split bf16 (hi, lo), or with f16 one fp16 tensor `hi` (lo unused)."""
+    return _lib.SplitOut(ptr(hi), ptr(lo), ptr(style), cstride, coff, int(f16))
 
 
 # ------------------------------------------------------------------------------------------------ kernels
 def _conv_desc(a_hi, a_lo, w_hi, w_lo, N, MH, MW, nprod):
-    """ConvGemm descriptor with the operands (a_*: bf16 [NI, AH, AW, Cin]; w_*: bf16 [T, Cout, Cin]) and the M-space filled in."""
+    """ConvGemm descriptor with the operands (a_*: bf16 [NI, AH, AW, Cin]; w_*: bf16 [T, Cout, Cin]; or, fp16 single operands, a_hi fp16
+    and w_hi fp16 with a_lo = w_lo = None and nprod 1) and the M-space filled in."""
     NI, AH, AW, Cin = a_hi.shape
     T, Cout, Cin_w = w_hi.shape
     assert Cin_w == Cin, (Cin_w, Cin)
@@ -75,6 +85,9 @@ def _conv_desc(a_hi, a_lo, w_hi, w_lo, N, MH, MW, nprod):
     p.T, p.Cout = T, Cout
     p.N, p.MH, p.MW = N, MH, MW
     p.nprod = nprod
+    p.f16 = int(a_hi.dtype == torch.float16)
+    if p.f16 and (w_hi.dtype != torch.float16 or a_lo is not None or w_lo is not None or nprod != 1):
+        raise ValueError('conv_gemm: fp16 operands are one fp16 activation and one fp16 weight tensor, nprod 1')
     return p
 
 
@@ -151,6 +164,12 @@ def modulate_split(x, style, hi, lo, cstride=None, coff=0):
     """x fp32 NHWC [N,H,W,C]; style [N,C] or None -> hi/lo bf16 (written at channel offset `coff`, stride `cstride`)."""
     N, H, W, Cc = x.shape
     _run('n3d_modulate_split', ptr(x), H * W, N, Cc, ptr(style), ptr(hi), ptr(lo), cstride or Cc, coff, stream_ptr())
+
+
+def modulate_f16(x, style, out, cstride=None, coff=0):
+    """x fp32 NHWC [N,H,W,C]; style [N,C] or None -> out fp16 = x * style (channel offset `coff`, stride `cstride`)."""
+    N, H, W, Cc = x.shape
+    _run('n3d_modulate_f16', ptr(x), H * W, N, Cc, ptr(style), ptr(out), cstride or Cc, coff, stream_ptr())
 
 
 def fir_up_epilogue(raw, C_, dcoef, bias, noise, gain, slope, clamp, outs=(), out_f32=None, f32_cstride=0, f32_coff=0, noise_nstride=0):
@@ -241,6 +260,13 @@ def resize_aa(src, dst=None, DH=None, DW=None, src_box=None, dst_box=None, style
         DH, DW = dst.shape[1:3]
     _run('n3d_resize_aa', ptr(src), N, SH, SW, Cc, ptr(src_box), ptr(dst), DH, DW, ptr(dst_box), ptr(style), ptr(hi), ptr(lo),
                           stream_ptr())
+
+
+def resize_aa_f16(src, out, src_box=None, dst_box=None, style=None):
+    """resize_aa into the fp16 NHWC tensor out [N, DH, DW, C] only: out = fp16(resize(src) * style)."""
+    N, SH, SW, Cc = src.shape
+    DH, DW = out.shape[1:3]
+    _run('n3d_resize_aa_f16', ptr(src), N, SH, SW, Cc, ptr(src_box), DH, DW, ptr(dst_box), ptr(style), ptr(out), stream_ptr())
 
 
 def blend_planes(front, tex_planes, alpha, static, planes, views=1):

@@ -58,6 +58,7 @@ class TriPlaneGenerator(torch.nn.Module):
         self.load_lms = True
         self.fill_mouth = True
         self.sr_num_fp16_res = sr_num_fp16_res
+        self._sr_precision = 'fp32'
         self.uv_face_mask = self._load_uv_face_mask()
         topo = None
         for name, shape, kind, _ in _config.param_spec(self.cfg):
@@ -124,6 +125,28 @@ class TriPlaneGenerator(torch.nn.Module):
             G.load_state_dict(state_dict)
         return G.eval().requires_grad_(False).to(device)
 
+    @property
+    def sr_precision(self):
+        """Precision of the super-resolution head: 'fp32' (default: fp32-grade bf16x3 convolutions, the reference's CPU result) or
+        'fp16' (opt-in, faster: fp16 activations and weights, one tensor-core product per k-step, fp32 accumulate -- the precision
+        the reference gives its SR blocks on CUDA when sr_num_fp16_res > 0, superresolution.py:268-277, networks_stylegan2.py:547-549,
+        but rounded at other points, so `image` is about 1e-3 of its range from either fp32 or the reference's fp16 answer and is
+        not the latter; INTEGRATION.md section 1).  Only `image` depends on it; the next synthesis / render_views call runs in the new mode (graphs are captured per mode).  ValueError
+        for any other value, and for 'fp16' with sr_num_fp16_res == 0 (the reference runs that SR head in fp32)."""
+        return self._sr_precision
+
+    @sr_precision.setter
+    def sr_precision(self, mode):
+        self._sr_precision = self._check_sr_precision(mode)
+
+    def _check_sr_precision(self, mode):
+        if mode not in ('fp32', 'fp16'):
+            raise ValueError(f"sr_precision must be 'fp32' or 'fp16', got {mode!r}")
+        if mode == 'fp16' and not self.sr_num_fp16_res > 0:
+            raise ValueError("sr_precision='fp16' needs sr_num_fp16_res > 0: with sr_num_fp16_res == 0 the reference runs the "
+                             "super-resolution head in fp32")
+        return mode
+
     def repack(self):
         """Re-pack weights into the engine's layouts (call after changing parameters in place)."""
         self._engine = None
@@ -147,6 +170,7 @@ class TriPlaneGenerator(torch.nn.Module):
             self._engine = Engine(cfg, self.state_dict(), device=dev, uv_face_mask=self.uv_face_mask)
             self._engine_key = key
         self._engine.rk = rk
+        self._engine.sr_precision = self._check_sr_precision(self._sr_precision)     # sr_num_fp16_res may have changed since
         return self._engine
 
     # ------------------------------------------------------------------------------------------ reference API
