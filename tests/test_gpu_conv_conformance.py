@@ -36,9 +36,12 @@ BOUNDS = {
 }
 
 # ------------------------------------------------------------------------------------------------ the launch rule, mirrored
-# Constants of conv_gemm.cu: kBlockM, kMinTiles, kMinTilesSplit, kMinStages, kMaxBlockN and the stage-ring bytes (kRingBytes).
+# Constants of conv_gemm.cu: kBlockM, kMinTiles, kMinTilesSplit, kMinStages, kMaxBlockN, kStageArrays, kXStride, kStoreBoxBytes,
+# and from them the epilogue area of a warpgroup (kEpiBytes) and the stage-ring bytes (kRingBytes).  test_mirror_constants_match_source
+# reads them from the source.
 BLOCK_M, MIN_TILES, MIN_TILES_SPLIT, MIN_STAGES, MAX_BLOCK_N = 128, 64, 128, 4, 128
-EPI_BYTES = 8 * 128 * 4 + 64 * 36 * 4 + 64 * 4 * 4
+STAGE_ARRAYS, X_STRIDE, STORE_BOX_BYTES = 8, 36, 64 * 32 * 4
+EPI_BYTES = max(STAGE_ARRAYS * MAX_BLOCK_N * 4 + 64 * X_STRIDE * 4 + 64 * 4 * 4, 2 * STORE_BOX_BYTES)
 RING_BYTES = 227 * 1024 - 2 * EPI_BYTES - 1024 - 256
 BLOCK_NS = (16, 32, 64, 96, 128)
 
@@ -50,41 +53,98 @@ def _pow2_ceil(v):
     return p
 
 
-def block_k_for(Cin, bn):
-    """block_k rule of launch_conv: 32-channel stages for Cin % 64 == 32 or where 64-channel stages leave < kMinStages in the ring."""
-    return 32 if Cin % 64 == 32 or RING_BYTES // (2 * (BLOCK_M + bn) * 64 * 2) < MIN_STAGES else 64
-
-
-def plan(N, Cin, Cout, MH, MW, splits=1, rgb=False, sms=132, cluster_slots=66):
-    """What launch_conv (conv_gemm.cu) selects for a one-sub-problem n3d_conv_gemm launch: tile geometry, block_n (widest wgmma N
-    not above Cout, halved while the launch has fewer than kMinTiles tiles; the fused ToRGB takes the narrowest width holding all
-    channels, else 128-wide n-tiles in turn), block_k, 2-CTA clusters (block_n >= 96, no split-K, >= 2 M tiles), work items and the
-    grid.  sms / cluster_slots: SMs and cudaOccupancyMaxActiveClusters of the device (132 and 66 on the H100 SXM)."""
+def tile_geometry(N, MH, MW):
+    """(TW, TH, TN, M tiles) of one sub-problem: TW up to 16 wide, then TH, then TN images (TW * TH * TN == kBlockM)."""
     TW = min(16, _pow2_ceil(MW))
     TH = min(BLOCK_M // TW, _pow2_ceil(MH))
     TN = BLOCK_M // (TW * TH)
-    tiles_m = -(-MW // TW) * -(-MH // TH) * -(-N // TN)
+    return TW, TH, TN, -(-MW // TW) * -(-MH // TH) * -(-N // TN)
+
+
+def widest_block_n(Cout, tiles_m, splits=1):
+    """The widest wgmma N not above Cout (96 only where it divides Cout rounded to 16), halved while the launch has fewer than
+    kMinTiles (kMinTilesSplit under split-K) tiles."""
     cout16 = -(-Cout // 16) * 16
     bn = next(c for c in (128, 96, 64, 32, 16) if c <= cout16 and (c != 96 or cout16 % 96 == 0))
     min_tiles = MIN_TILES_SPLIT if splits > 1 else MIN_TILES
     while bn > 32 and tiles_m * splits * -(-Cout // bn) < min_tiles:
         bn = 32 if bn == 96 else bn // 2
+    return bn
+
+
+def block_k_for(Cin, bn, f16=False):
+    """block_k rule of launch_conv: 32-channel stages for Cin % 64 == 32 or where 64-channel stages leave < kMinStages in the ring.
+    A bf16 stage holds the hi and lo tiles of A and B, an fp16 stage (f16) one of each."""
+    tiles_per_stage = 1 if f16 else 2
+    return 32 if Cin % 64 == 32 or RING_BYTES // (tiles_per_stage * (BLOCK_M + bn) * 64 * 2) < MIN_STAGES else 64
+
+
+def stages_for(bn, bk, f16=False):
+    """Stages of the ring (kMaxStages 8 at most)."""
+    return min(8, RING_BYTES // ((1 if f16 else 2) * (BLOCK_M + bn) * bk * 2))
+
+
+def plan(N, Cin, Cout, MH, MW, splits=1, rgb=False, sms=132, cluster_slots=66, f16=False):
+    """What launch_conv (conv_gemm.cu) selects for a one-sub-problem n3d_conv_gemm launch: tile geometry, block_n (widest wgmma N
+    not above Cout, halved while the launch has fewer than kMinTiles tiles; the fused ToRGB takes the narrowest width holding all
+    channels, else 128-wide n-tiles in turn), block_k, 2-CTA clusters (block_n >= 96, no split-K, >= 2 M tiles), work items and the
+    grid.  sms / cluster_slots: SMs and cudaOccupancyMaxActiveClusters of the device (132 and 66 on the H100 SXM).  f16: fp16
+    operands (N3DConvGemm.f16)."""
+    TW, TH, TN, tiles_m = tile_geometry(N, MH, MW)
+    bn = widest_block_n(Cout, tiles_m, splits)
     item_tiles = 1
     if rgb:
+        cout16 = -(-Cout // 16) * 16
         bn = next((w for w in BLOCK_NS if w >= cout16), MAX_BLOCK_N)
         item_tiles = -(-Cout // bn)
     tiles_n = -(-Cout // bn)
     cluster = 2 if splits == 1 and bn >= 96 and tiles_m >= 2 else 1
     units = -(-tiles_m // cluster) * tiles_n * splits // item_tiles
     slots = sms if cluster == 1 else cluster_slots
-    return dict(block_n=bn, block_k=block_k_for(Cin, bn), cluster=cluster, TW=TW, TH=TH, TN=TN, tiles_m=tiles_m, tiles_n=tiles_n,
-                item_tiles=item_tiles, units=units, grid=cluster * min(units, slots), items_per_cta=-(-units // slots),
-                pad=cluster == 2 and tiles_m % 2 == 1)
+    bk = block_k_for(Cin, bn, f16)
+    return dict(block_n=bn, block_k=bk, stages=stages_for(bn, bk, f16), cluster=cluster, TW=TW, TH=TH, TN=TN, tiles_m=tiles_m,
+                tiles_n=tiles_n, item_tiles=item_tiles, units=units, grid=cluster * min(units, slots), items_per_cta=-(-units // slots),
+                pad=cluster == 2 and tiles_m % 2 == 1, grouped=False)
 
 
-def reachable_instances():
-    """(block_n, block_k) pairs the rule can produce: every block_n with a Cin that is / is not 32 mod 64."""
-    return {(bn, block_k_for(cin, bn)) for bn in BLOCK_NS for cin in (32, 64)}
+def transposed_plan(N, Cin, Cout, H, W, sms=132, cluster_slots=66, f16=False):
+    """What n3d_conv_transposed_gemm selects for a stride-2 transposed 3x3 conv of an H x W input: nine sub-problems (the four
+    parity-class interiors H x W, two row strips 1 x W, two column strips H x 1, the corner 1 x 1), block_n from the sum of their M
+    tiles, a 2-CTA cluster where block_n >= 96 and the largest sub-problem has >= 2 M tiles, the four interleaved classes grouped into
+    one unit per (M tile, n-tile) when they have more items than the launch has CTA (cluster) slots, and the grid."""
+    sub_m = [tile_geometry(N, mh, mw)[3] for mh, mw in [(H, W)] * 4 + [(1, W)] * 2 + [(H, 1)] * 2 + [(1, 1)]]
+    tiles_m = sum(sub_m)
+    bn = widest_block_n(Cout, tiles_m)
+    tiles_n = -(-Cout // bn)
+    cluster = 2 if bn >= 96 and max(sub_m) >= 2 else 1
+    slots = sms if cluster == 1 else cluster_slots
+    units_grouped = -(-sub_m[0] // cluster) * tiles_n
+    groups = units_grouped if 4 * units_grouped > slots else 0
+    total_items = 4 * units_grouped + sum(-(-m // cluster) * tiles_n for m in sub_m[4:])
+    units = total_items - 3 * groups
+    bk = block_k_for(Cin, bn, f16)
+    return dict(block_n=bn, block_k=bk, stages=stages_for(bn, bk, f16), cluster=cluster, tiles_m=tiles_m, tiles_n=tiles_n, item_tiles=1,
+                units=units, grid=cluster * min(units, slots), items_per_cta=-(-units // slots), pad=cluster == 2 and any(m % 2 for m in sub_m),
+                grouped=groups > 0)
+
+
+def reachable_instances(f16=False):
+    """(block_n, block_k) pairs the rule can produce: every block_n with a Cin that is / is not 32 mod 64 (8 for bf16 operands, all
+    10 for fp16, whose stages are half the size)."""
+    return {(bn, block_k_for(cin, bn, f16)) for bn in BLOCK_NS for cin in (32, 64)}
+
+
+def source_constants():
+    """The integer constants of conv_gemm.cu (`constexpr int k... = <expr>;`), each evaluated in terms of the ones before it."""
+    import os
+    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'next3d_b200', 'csrc', 'conv_gemm.cu')).read()
+    env = {}
+    for name, expr in re.findall(r'^constexpr int (k\w+) = ([^;]+);', src, re.M):
+        cond = re.fullmatch(r'(.+?) ([<>]=?) (.+?) \? (.+?) : (.+)', expr.strip())
+        if cond:                            # c ? a : b
+            expr = f'(({cond[4]}) if ({cond[1]}) {cond[2]} ({cond[3]}) else ({cond[5]}))'
+        env[name] = int(eval(expr, {'__builtins__': {}}, dict(env)))
+    return env
 
 
 # ------------------------------------------------------------------------------------------------ the case table
@@ -142,6 +202,20 @@ CASES = [
     _case('transposed_class10_raw', 2, 40, 64, 12, 13, mode=1, taps='tr10', f32=dict(cstride=64, coff=0, nchw=False, acc=False)),
 ]
 CASE_IDS = [c['name'] for c in CASES]
+# (block_n, block_k, stages, cluster, grid) `plan` gives each case at 132 SMs: the mirror is shared with the fp16 suite, and a change
+# to it must leave these as they are
+BF16_PLANS = {
+    'bn16_bk64_nprod1': (16, 64, 5, 1, 4), 'bn16_bk32_24x3': (16, 32, 8, 1, 3), 'bn32_bk64_5x37_cout40': (32, 64, 4, 1, 12),
+    'bn32_bk32_cin160': (32, 32, 8, 1, 2), 'bn64_bk64_cout72': (64, 64, 4, 1, 68), 'bn64_bk32_cin32': (64, 32, 8, 1, 64),
+    'bn96_bk32_rgb_unclustered': (96, 32, 6, 1, 1), 'bn128_bk32_rgb_unclustered': (128, 32, 6, 1, 1),
+    'bn128_cluster_pad_accumulate': (128, 32, 6, 2, 68), 'bn128_cluster_stride2_pad': (128, 32, 6, 2, 76),
+    'bn128_cluster_tn2_pad': (128, 32, 6, 2, 66), 'bn96_cluster_torgb1x1_accumulate': (96, 32, 6, 2, 64),
+    'bn128_cluster_pingpong': (128, 32, 6, 2, 132), 'bn32_pingpong_staged': (32, 64, 4, 1, 132), 'bn32_tn8_unstaged': (32, 64, 4, 1, 2),
+    'torgb1x1_4x4': (16, 64, 5, 1, 2), 'torgb1x1_8x8': (16, 32, 8, 1, 3), 'rgb16': (16, 64, 5, 1, 4), 'rgb32': (32, 64, 4, 1, 2),
+    'rgb40': (64, 64, 4, 1, 4), 'rgb96_cluster_pad': (96, 32, 6, 2, 4), 'rgb192_cluster': (128, 32, 6, 2, 4),
+    'rgb256_cluster_pad': (128, 32, 6, 2, 4), 'splitk9': (32, 64, 4, 1, 18), 'splitk3': (32, 64, 4, 1, 12),
+    'splitk2_uneven': (32, 64, 4, 1, 6), 'transposed_class10_raw': (32, 64, 4, 1, 8),
+}
 
 
 def _taps(c):
@@ -238,6 +312,23 @@ def test_case_table_covers_every_launch_configuration():
     assert len(reachable_instances()) == 8
     assert (96, 64) not in reachable_instances() and (128, 64) not in reachable_instances()
     assert len(set(CASE_IDS)) == len(CASE_IDS)
+
+
+def test_mirror_constants_match_source():
+    """CPU: the mirror's constants are conv_gemm.cu's, and EPI_BYTES / RING_BYTES follow from them as kEpiBytes / kRingBytes do."""
+    k = source_constants()
+    assert (k['kBlockM'], k['kMinTiles'], k['kMinTilesSplit'], k['kMinStages'], k['kMaxBlockN']) == (BLOCK_M, MIN_TILES, MIN_TILES_SPLIT,
+                                                                                                   MIN_STAGES, MAX_BLOCK_N)
+    assert (k['kStageArrays'], k['kXStride'], k['kStoreBoxBytes']) == (STAGE_ARRAYS, X_STRIDE, STORE_BOX_BYTES)
+    assert k['kMaxStages'] == 8
+    assert max(k['kStageArrays'] * k['kMaxBlockN'] * 4 + 64 * k['kXStride'] * 4 + 64 * 4 * 4, 2 * k['kStoreBoxBytes']) == EPI_BYTES
+    assert k['kEpiBytes'] == EPI_BYTES and k['kRingBytes'] == RING_BYTES
+
+
+def test_plan_is_unchanged_for_bf16():
+    """CPU: the bf16 selections of the table, pinned (instance, stages, cluster, grid), so that a change of the shared mirror shows."""
+    got = {c['name']: (p['block_n'], p['block_k'], p['stages'], p['cluster'], p['grid']) for c in CASES for p in [_plan(c)]}
+    assert got == BF16_PLANS, {k: (v, BF16_PLANS.get(k)) for k, v in got.items() if BF16_PLANS.get(k) != v}
 
 
 # ------------------------------------------------------------------------------------------------ the fp64 reference
