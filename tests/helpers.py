@@ -206,3 +206,55 @@ def offset_view(t, nbytes):
     """A view of `t` (a fresh, 64-byte aligned allocation) that starts `nbytes` later."""
     assert t.data_ptr() % 64 == 0
     return t.view(-1)[nbytes // t.element_size():]
+
+
+# ------------------------------------------------------------------------------------------------ generator-level helpers
+def oracle_widx(cfg):
+    """{modulated layer: the ws index oracle.generator.synthesis feeds it}, read off the oracle's own slicing of a ws whose entries
+    are their index: the texture backbone takes ws[:, 14:], the other backbones ws[:, :14] (the StyleUNets from their first executed
+    block on), the super-resolution blocks ws[:, 13]."""
+    from next3d_b200 import config
+    from oracle import generator as og
+    idx = torch.arange(28)[None, :, None]
+    eg3d, tex = idx[:, :14], idx[:, 14:]
+    res_list = config.block_resolutions(cfg.plane_res)
+    out = {}
+
+    def blocks(prefix, ws, start):
+        for res, cur in list(zip(res_list, og._split_ws(ws, res_list)))[start:]:
+            names = ('conv1', 'torgb') if res == 4 else ('conv0', 'conv1', 'torgb')
+            for name, w in zip(names, cur.unbind(1)):
+                out[f'{prefix}.b{res}.{name}'] = int(w)
+
+    blocks('texture_backbone.synthesis', tex, 0)
+    blocks('backbone.synthesis', eg3d, 0)
+    blocks('mouth_backbone.synthesis', eg3d, int(math.log2(4)) - 1)            # styleunet(..., 64, 4, 64)
+    blocks('neural_blending.synthesis', eg3d, int(math.log2(32)) - 1)          # styleunet(..., 256, 32, 256)
+    sr = eg3d[:, -1:].repeat(1, 3, 1)
+    for b in (0, 1):
+        for name, w in zip(('conv0', 'conv1', 'torgb'), sr.unbind(1)):
+            out[f'superresolution.block{b}.{name}'] = int(w)
+    return out
+
+
+# "Hot" super-resolution biases that push outputs past the +-256 conv_clamp of the SR layers.  Every 8th output channel of each SR
+# convolution gets +400, every 8th (offset 4) -1200: lrelu(400) * sqrt 2 = 566 and lrelu(-1200) * sqrt 2 = -339.  ToRGB channel 0 gets
+# +2000 and channel 1 -2000: the ToRGB sums of the hot activations alone reach +-1000 at the seeded weights, which +-300 would not
+# outweigh.  So about 1/8 of every SR conv's outputs and 1/3 of every SR ToRGB's outputs reach each side of the clamp.
+HOT_CONV_BIAS = (400.0, -1200.0)
+HOT_RGB_BIAS = (2000.0, -2000.0)
+
+
+def hot_sr_state_dict(cfg, seed=0):
+    """weights.make_state_dict(cfg, seed) with the hot super-resolution biases above."""
+    from next3d_b200 import weights
+    sd = weights.make_state_dict(cfg, seed=seed)
+    for b in (0, 1):
+        for name in ('conv0', 'conv1'):
+            bias = sd[f'superresolution.block{b}.{name}.bias'].clone()
+            bias[0::8], bias[4::8] = HOT_CONV_BIAS
+            sd[f'superresolution.block{b}.{name}.bias'] = bias
+        bias = sd[f'superresolution.block{b}.torgb.bias'].clone()
+        bias[0], bias[1] = HOT_RGB_BIAS
+        sd[f'superresolution.block{b}.torgb.bias'] = bias
+    return sd

@@ -15,7 +15,7 @@ from next3d_b200 import config, drivers, weights
 from next3d_b200.triplane_next3d import TriPlaneGenerator
 from oracle import generator as og
 from oracle import sr_fp16
-from tests.helpers import range_rel_err, report_parity
+from tests.helpers import hot_sr_state_dict, range_rel_err, report_parity
 
 DEV = 'cuda'
 pytestmark = pytest.mark.gpu
@@ -34,13 +34,15 @@ MODE_RATIO = 2.5
 def _mean_err(a, ref):
     return ((a.double() - ref.double()).abs().mean() / ref.double().abs().max()).item()
 
-CONFIGS = {'tiny512': (config.tiny_config, 512, 2), 'full512': (config.full_config, 512, 1), 'tiny256': (config.tiny_config, 256, 1)}
+CONFIGS = {'tiny512': (config.tiny_config, 512, 2), 'full512': (config.full_config, 512, 1), 'tiny256': (config.tiny_config, 256, 1),
+           'tiny512_hot': (config.tiny_config, 512, 2)}
+HOT = {'tiny512_hot'}           # the hot SR biases of tests.helpers: every SR layer reaches the +-256 clamp on both sides
 
 
 def _setup(name, seed=0):
     factory, res, batch = CONFIGS[name]
     cfg = factory(res)
-    sd = weights.make_state_dict(cfg, seed=seed)
+    sd = hot_sr_state_dict(cfg, seed=seed) if name in HOT else weights.make_state_dict(cfg, seed=seed)
     G = TriPlaneGenerator.from_config(cfg, sd, device=DEV)
     z, c_cond, c_cam, v = weights.demo_inputs(cfg, batch, seed=seed)
     u_c, u_f = weights.sampler_noise(cfg, batch, seed=seed)

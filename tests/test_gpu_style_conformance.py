@@ -29,8 +29,8 @@ import pytest
 import torch
 
 from next3d_b200 import config, weights
-from tests.helpers import Guarded, RangeErr, cdiv, grid_stride, launched_kernels, lib, offset_view, range_rel_err, record_errors, refused, \
-    rerun_identical
+from tests.helpers import Guarded, RangeErr, cdiv, grid_stride, launched_kernels, lib, offset_view, oracle_widx, range_rel_err, \
+    record_errors, refused, rerun_identical
 
 DEV = 'cuda'
 SMS = 132                   # SM count the table is planned at (H100 SXM)
@@ -520,33 +520,6 @@ def test_launched_kernel_matches_plan(tmp_path):
 
 
 # ------------------------------------------------------------------------------------------------ the engine's tables
-def oracle_widx(cfg):
-    """{modulated layer: the ws index oracle.generator.synthesis feeds it}, read off the oracle's own slicing of a ws whose entries
-    are their index: the texture backbone takes ws[:, 14:], the other backbones ws[:, :14] (the StyleUNets from their first executed
-    block on), the super-resolution blocks ws[:, 13]."""
-    from oracle import generator as og
-    idx = torch.arange(28)[None, :, None]
-    eg3d, tex = idx[:, :14], idx[:, 14:]
-    res_list = config.block_resolutions(cfg.plane_res)
-    out = {}
-
-    def blocks(prefix, ws, start):
-        for res, cur in list(zip(res_list, og._split_ws(ws, res_list)))[start:]:
-            names = ('conv1', 'torgb') if res == 4 else ('conv0', 'conv1', 'torgb')
-            for name, w in zip(names, cur.unbind(1)):
-                out[f'{prefix}.b{res}.{name}'] = int(w)
-
-    blocks('texture_backbone.synthesis', tex, 0)
-    blocks('backbone.synthesis', eg3d, 0)
-    blocks('mouth_backbone.synthesis', eg3d, int(math.log2(4)) - 1)            # styleunet(..., 64, 4, 64)
-    blocks('neural_blending.synthesis', eg3d, int(math.log2(32)) - 1)          # styleunet(..., 256, 32, 256)
-    sr = eg3d[:, -1:].repeat(1, 3, 1)
-    for b in (0, 1):
-        for name, w in zip(('conv0', 'conv1', 'torgb'), sr.unbind(1)):
-            out[f'superresolution.block{b}.{name}'] = int(w)
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('factory', [config.tiny_config, config.full_config], ids=['tiny', 'full'])
 def test_engine_style_tables_match_fp64(factory):
