@@ -775,10 +775,18 @@ class Engine:
 
     # ------------------------------------------------------------------------------------------ CUDA graph replay
     def _render_key(self, R):
+        """The part of a graph key every graphed call shares: the rendering options a captured graph bakes in and the SR precision.
+        It first refuses the options the renderer lacks, which the eager call would refuse."""
         rk = self.rk
+        K.check_render_options(rk)
         return (R, rk['depth_resolution'], rk['depth_resolution_importance'], float(rk['ray_start']), float(rk['ray_end']), float(rk['box_warp']),
                 bool(rk.get('white_back', False)), rk['superresolution_noise_mode'], bool(rk.get('sr_antialias', True)),
                 bool(rk.get('return_normal', False)), self.sr_precision)
+
+    def _settings_key(self):
+        """The convolution settings a captured graph bakes in (each changes the result).  `concurrent` is not part of any key: the
+        branches' stream layout does not change the result."""
+        return (bool(self.splitk), self.splitk_maxres, self.nprod)
 
     def _replay(self, key, inputs, run, seed):
         """Capture run(static inputs) once per key into a CUDA graph and replay it: inputs are copied into static buffers (plus a
@@ -802,7 +810,8 @@ class Engine:
         graph, st, out, launches, flops = g
         for k, t in inputs.items():
             st[k].copy_(t, non_blocking=True)
-        st['seed'].fill_(int(seed))
+        bits = K.seed_bits(seed)                                            # the int64 counter holds the seed's 64-bit pattern
+        st['seed'].fill_(bits - (1 << 64) if bits >> 63 else bits)
         graph.replay()
         self.launches, self.conv_flops = launches, flops
         return out
@@ -819,11 +828,12 @@ class Engine:
         with torch.cuda.device(self.device):
             N = ws.shape[0]
             R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
+            render_key = self._render_key(R) + self._settings_key()      # refuses unsupported options before the cache is touched
             reuse = self._reused_views(N, use_cached_backbone, cache_backbone) is not None
             if cache_backbone:
                 self._cache_buffers(N, ws.shape)          # allocated before capture: the graph writes the cache at fixed addresses
             B = self._cache['B'] if reuse else N             # (N, B): the images per cached head of a reusing graph
-            key = (cache_backbone or reuse, cache_backbone, reuse, N, B, noise_mode, tuple(v.shape), depth_range) + self._render_key(R)
+            key = (cache_backbone or reuse, cache_backbone, reuse, N, B, noise_mode, tuple(v.shape), depth_range) + render_key
 
             def run(st):
                 return self.synthesis(st['ws'], st['c'], st['v'], noise_mode, R, seed=0, seed_ptr=st['seed'], cache_backbone=cache_backbone,
@@ -840,7 +850,7 @@ class Engine:
         with torch.cuda.device(self.device):
             V = self._render_views_per_head(c.shape[0])
             R = neural_rendering_resolution or self.cfg.neural_rendering_resolution
-            key = (True, 'views', c.shape[0], V, depth_range) + self._render_key(R)
+            key = (True, 'views', c.shape[0], V, depth_range) + self._render_key(R) + self._settings_key()
             return self._replay(key, dict(c=c), lambda st: self.render_views(st['c'], R, seed=0, seed_ptr=st['seed'], depth_range=depth_range),
                                 seed)
 

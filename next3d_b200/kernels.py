@@ -285,13 +285,22 @@ def _render_desc(planes, cam2world, intrinsics, res, opts, seed, views=1):
     p.depth_coarse, p.depth_fine = opts['depth_resolution'], opts['depth_resolution_importance']
     p.ray_start, p.ray_end, p.box_warp = float(opts['ray_start']), float(opts['ray_end']), float(opts['box_warp'])
     p.ray_span = float(opts['ray_end']) - float(opts['ray_start'])        # the jitter spacing's numerator, in double as the reference has it
-    p.seed = seed
+    p.seed = seed_bits(seed)
     return p
 
 
-def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr, views=1,
-                      depth_range_per_image=0):
-    """Render descriptor of n3d_render_rays / n3d_render_rays_normals, after rejecting the rendering options the renderer lacks."""
+SEED_MASK = (1 << 64) - 1
+
+
+def seed_bits(seed):
+    """The sampler seed as the renderer uses it: its 64-bit pattern, so any integer is accepted and seeds equal modulo 2^64 (-1 and
+    2^64 - 1, say) draw the same uniforms."""
+    return int(seed) & SEED_MASK
+
+
+def check_render_options(opts):
+    """Raise for the rendering options the fused renderer lacks.  Every render call runs this first, the graph-replayed ones too (a
+    replay runs no Python of the call it captured)."""
     unsupported = [k for k, bad in (('disparity_space_sampling', bool(opts.get('disparity_space_sampling', False))),
                                     ('density_noise', float(opts.get('density_noise', 0) or 0) > 0),
                                     ('clamp_mode', opts.get('clamp_mode', 'softplus') != 'softplus'),
@@ -299,6 +308,12 @@ def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth,
     if unsupported:     # renderer.py:98-107 (auto near/far), :153 (density noise), :186-196 (disparity sampling), ray_marcher.py:41-44
         raise RuntimeError(f'libnext3d_b200 n3d_render_rays failed (code -2, unsupported): rendering option(s) {unsupported} are not '
                            f'implemented by the fused renderer (supported: linear stratified sampling, fixed ray_start / ray_end, softplus)')
+
+
+def _render_full_desc(planes, cam2world, intrinsics, res, opts, dec, rgb, depth, wsum, depth_minmax, u_coarse, u_fine, seed, seed_ptr, views=1,
+                      depth_range_per_image=0):
+    """Render descriptor of n3d_render_rays / n3d_render_rays_normals, after rejecting the rendering options the renderer lacks."""
+    check_render_options(opts)
     p = _render_desc(planes, cam2world, intrinsics, res, opts, seed, views)
     p.u_coarse, p.u_fine, p.seed_ptr = ptr(u_coarse), ptr(u_fine), ptr(seed_ptr)
     p.w0, p.b0, p.w1, p.b1 = (ptr(t) for t in dec)

@@ -258,3 +258,34 @@ def hot_sr_state_dict(cfg, seed=0):
         bias[0], bias[1] = HOT_RGB_BIAS
         sd[f'superresolution.block{b}.torgb.bias'] = bias
     return sd
+
+
+# ------------------------------------------------------------------------------------------------ the renderer's in-kernel sampler RNG
+HASH_GAMMA = 0x9E3779B97F4A7C15         # hash_uniform (render_common.cuh): splitmix64 of seed + idx * gamma
+HASH_MIX = (0xBF58476D1CE4E5B9, 0x94D049BB133111EB)
+FINE_SEED_XOR = 0xA5A5A5A5DEADBEEF      # the fine (importance) stream's seed: seed ^ this (render_fused.cu)
+
+
+def hash_uniform(seed, idx):
+    """The renderer's counter RNG in numpy uint64 arithmetic: uniform float32 number `idx` (an integer array) of stream `seed` (any
+    integer, taken modulo 2^64).  The top 24 bits of the mixed word over 2^24: the 2^-24 grid in [0, 1 - 2^-24], torch.rand's range."""
+    u64 = np.uint64
+    with np.errstate(over='ignore'):
+        z = u64(int(seed) & ((1 << 64) - 1)) + np.asarray(idx, dtype=u64) * u64(HASH_GAMMA)
+        z = (z ^ (z >> u64(30))) * u64(HASH_MIX[0])
+        z = (z ^ (z >> u64(27))) * u64(HASH_MIX[1])
+        z ^= z >> u64(31)
+    return (z >> u64(40)).astype(np.float32) * np.float32(2.0 ** -24)
+
+
+def sampler_uniforms(seed, N, M, Dc, Df):
+    """The uniforms a render launch of N images of M rays draws in the kernel with `seed` (the descriptor's seed plus *seed_ptr), in
+    the layouts of injected ones: u_coarse [N, M, Dc, 1] with number gr * Dc + k of stream seed for sample k of global ray
+    gr = n * M + m, and u_fine [N * M, max(Df, 1)] with number gr * Df + j of stream seed ^ FINE_SEED_XOR (zeros when Df is 0)."""
+    rays = np.arange(N * M, dtype=np.uint64)[:, None]
+    u_c = hash_uniform(seed, rays * np.uint64(Dc) + np.arange(Dc, dtype=np.uint64))
+    if Df:
+        u_f = hash_uniform((int(seed) & ((1 << 64) - 1)) ^ FINE_SEED_XOR, rays * np.uint64(Df) + np.arange(Df, dtype=np.uint64))
+    else:
+        u_f = np.zeros((N * M, 1), np.float32)
+    return torch.from_numpy(u_c).reshape(N, M, Dc, 1), torch.from_numpy(u_f)

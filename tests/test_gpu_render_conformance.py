@@ -2,7 +2,8 @@
 the N3DRender contract (include/next3d_b200.h), over a table of small launches that reaches every kernel instance, lane layout and
 rendering option the contract offers: white_back, non-square / tiny / production-size planes, box_warp, rays outside the box and
 cameras inside it, skewed intrinsics, degenerate densities, the minimum sample counts, uniforms at the ends of [0, 1), ragged pixel
-blocks, views and the per-image depth range.
+blocks, views and the per-image depth range.  Every case also runs with the in-kernel sampler RNG and must be bit-identical to the
+launch fed the host statement's uniforms (tests.helpers.sampler_uniforms), which pins the RNG itself.
 
 Two references, both with the kernel's injected uniforms:
   - oracle.renderer in float32, the pinned statement of the reference's ImportanceRenderer (tests/test_oracle_vs_reference.py,
@@ -24,7 +25,7 @@ import re
 import pytest
 import torch
 
-from tests.helpers import Guarded, launched_kernels, lib, offset_view, range_rel_err, record_errors, refused
+from tests.helpers import Guarded, launched_kernels, lib, offset_view, range_rel_err, record_errors, refused, sampler_uniforms
 
 DEV = 'cuda'
 U_MAX = 1.0 - 2.0 ** -24        # the largest value torch.rand returns
@@ -96,7 +97,7 @@ def points_grid(N, Pn, sms=132):
 # ------------------------------------------------------------------------------------------------ the case table
 def _case(name, axis, **kw):
     c = dict(name=name, axis=axis, N=1, res=12, Dc=12, Df=12, PH=64, PW=64, box_warp=1.0, ray_start=2.25, ray_end=3.3,
-             white_back=False, camera='demo', density='mid', uniforms='random', views=1, per_image=0, normals=False)
+             white_back=False, camera='demo', density='mid', uniforms='random', views=1, per_image=0, normals=False, seed_ptr=False)
     c.update(kw)
     return c
 
@@ -105,14 +106,14 @@ CASES = [
     # lane layouts, fine and coarse-only; res not a multiple of the pixel block (4 x 2, 2 x 2, 1 x 2) leaves ragged groups
     _case('l16_fine', 'lanes', res=13, Dc=40, Df=24, normals=True),
     _case('l16_coarse_only', 'lanes', res=13, Dc=48, Df=0),
-    _case('l32_fine', 'lanes', res=11, Dc=64, Df=80, normals=True),
+    _case('l32_fine', 'lanes', res=11, Dc=64, Df=80, normals=True, seed_ptr=True),
     _case('l32_coarse_only', 'lanes', res=9, Dc=96, Df=0),
     _case('l64_fine', 'lanes', res=7, Dc=100, Df=150, normals=True),
     _case('l64_coarse_only', 'lanes', res=6, Dc=192, Df=0),
     # white_back in every layout, with and without fine samples (with views and the per-image depth range on some)
     _case('white_l16_fine', 'white_back', res=10, Dc=24, Df=48, white_back=True),
     _case('white_l16_coarse_only', 'white_back', res=10, Dc=48, Df=0, white_back=True, N=2, per_image=1),
-    _case('white_l32_fine', 'white_back', res=8, Dc=96, Df=49, white_back=True, N=4, views=2, per_image=1),
+    _case('white_l32_fine', 'white_back', res=8, Dc=96, Df=49, white_back=True, N=4, views=2, per_image=1, seed_ptr=True),
     _case('white_l32_coarse_only', 'white_back', res=8, Dc=49, Df=0, white_back=True),
     _case('white_l64_fine', 'white_back', res=5, Dc=97, Df=120, white_back=True, N=2, views=2),
     _case('white_l64_coarse_only', 'white_back', res=5, Dc=150, Df=0, white_back=True),
@@ -186,6 +187,8 @@ COVERAGE = {
     'normals on non-square, 5 x 3, box_warp 0.5, skewed and inside-the-box geometry':
         lambda cs: {'planes_48x80', 'planes_80x48', 'planes_5x3', 'box_warp_0.5', 'skewed_intrinsics', 'camera_inside'}
         <= {c['name'] for c, p in cs if c['normals']},
+    'the in-kernel RNG through seed_ptr, with normals and with views and the per-image depth range':
+        lambda cs: any(c['seed_ptr'] and c['normals'] for c, p in cs) and any(c['seed_ptr'] and c['views'] >= 2 and c['per_image'] for c, p in cs),
 }
 
 
@@ -293,14 +296,16 @@ def _device_inputs(s, planes=None):
                 dec=_dec(s['sd']), u_c=s['u_c'].to(DEV), u_f=s['u_f'].to(DEV))
 
 
-def launch_case(s, out, dv=None, views=None, normal=None, work=None):
-    """n3d_render_rays (or n3d_render_rays_normals with normal / work) with injected uniforms, then the depth clamp."""
+def launch_case(s, out, dv=None, views=None, normal=None, work=None, seed=0, seed_ptr=None):
+    """n3d_render_rays (or n3d_render_rays_normals with normal / work) with injected uniforms (the in-kernel RNG with `seed` and
+    `seed_ptr` where dv's are None), then the depth clamp."""
     from next3d_b200 import kernels as K
     c = s['c']
     dv = dv or _device_inputs(s)
     args = (dv['planes'], dv['cam'], dv['intr'], c['res'], s['opts'], dv['dec'], out['rgb'].view, out['depth'].view, out['wsum'].view,
             out['mm'].view)
-    kw = dict(u_coarse=dv['u_c'], u_fine=dv['u_f'], views=c['views'] if views is None else views, depth_range_per_image=c['per_image'])
+    kw = dict(u_coarse=dv['u_c'], u_fine=dv['u_f'], views=c['views'] if views is None else views, depth_range_per_image=c['per_image'],
+              seed=seed, seed_ptr=seed_ptr)
     if normal is None:
         K.render_rays(*args, **kw)
     else:
@@ -347,6 +352,46 @@ def test_render_rays_matches_contract(c):
         launch_case(s, rep, _device_inputs(s, s['planes'].repeat_interleave(c['views'], 0)), views=1)
         for k in out:
             assert torch.equal(out[k].view, rep[k].view), k
+
+
+# ------------------------------------------------------------------------------------------------ the in-kernel sampler RNG
+def rng_seeds(c):
+    """(descriptor seed, *seed_ptr or None) of a case's in-kernel RNG launch: seeds with high bits set, split between the two fields
+    (which the kernel adds modulo 2^64) in the seed_ptr cases."""
+    seed = 0xC3A5C85C97CB3127 + CASE_IDS.index(c['name'])
+    return (0x9AE16A3B2F90404F, (seed - 0x9AE16A3B2F90404F) % 2 ** 64) if c['seed_ptr'] else (seed, None)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('c', CASES, ids=CASE_IDS)
+def test_in_kernel_rng_matches_host_statement(c):
+    """u_coarse = u_fine = None with a seed == the same launch fed tests.helpers.sampler_uniforms of that seed, bit for bit, in every
+    output (n3d_render_rays_normals in the normal cases, its normals and exported samples included).  seed_ptr cases: the kernel's
+    seed is the descriptor's plus *seed_ptr, read as uint64."""
+    from next3d_b200 import kernels as K
+    s = setup_case(c)
+    N, M = c['N'], c['res'] ** 2
+    seed, extra = rng_seeds(c)
+    u_c, u_f = sampler_uniforms(seed + (extra or 0), N, M, c['Dc'], c['Df'])         # the statement takes the sum modulo 2^64
+    dv = _device_inputs(s)
+    runs = []
+    for inject in (True, False):
+        out = _outputs(c)
+        kw = {}
+        if c['normals']:
+            out['normal'] = Guarded((N, M, 3))
+            out['work'] = Guarded((K.normals_workspace_floats(N, c['res'], s['opts']),))
+            kw = dict(normal=out['normal'].view, work=out['work'].view)
+        if inject:
+            launch_case(s, out, dict(dv, u_c=u_c.to(DEV), u_f=u_f.to(DEV)), **kw)
+        else:
+            ptr = None if extra is None else torch.tensor([extra - 2 ** 64 if extra >> 63 else extra], dtype=torch.int64, device=DEV)
+            launch_case(s, out, dict(dv, u_c=None, u_f=None), seed=seed, seed_ptr=ptr, **kw)
+        runs.append(out)
+    torch.cuda.synchronize()
+    for k in runs[0]:
+        assert runs[1][k].untouched_ok() and runs[1][k].written(), k
+        assert torch.equal(runs[0][k].snapshot(), runs[1][k].snapshot()), k
 
 
 # ------------------------------------------------------------------------------------------------ n3d_render_rays_normals
