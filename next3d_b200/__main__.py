@@ -1,0 +1,219 @@
+"""Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`.
+
+The three subcommands are the reference's gen_samples_next3d.py, gen_videos_next3d.py and reenact_avatar_next3d.py with their option
+names, defaults and output file names, run on a network pickle read by next3d_b200.legacy (no reference checkout, no pickled code
+run) and rendered by the batched drivers of next3d_b200.drivers on one CUDA device.  Differences from the scripts:
+  * `--network` is a local file (no URL download);
+  * the ray sampler draws its uniforms from seed 0 (the scripts use fresh torch.rand draws), so a run is reproducible;
+  * `--lms_cond True` is required: the generator reads the 68 landmarks that follow the mesh vertices (load_lms), and without them
+    the scripts fail as well;
+  * `--shape-format .ply` (marching-cubes export) and `--cfg` other than FFHQ are refused, and so is `--interpolate False` with a
+    grid larger than 1x1 (every cell would show the same head);
+  * mp4 files are written with imageio; without it the video commands refuse before loading the network.
+"""
+import argparse
+import os
+import re
+import sys
+
+import torch
+
+SAMPLER_SEED = 0
+
+
+def _bool(s):
+    v = s.strip().lower()
+    if v in ('1', 'true', 't', 'yes', 'y', 'on'):
+        return True
+    if v in ('0', 'false', 'f', 'no', 'n', 'off'):
+        return False
+    raise argparse.ArgumentTypeError(f'{s!r} is not a valid boolean')
+
+
+def _range(s):
+    """'0,1,4-6' -> [0, 1, 4, 5, 6] (parse_range of the scripts)."""
+    out = []
+    for p in s.split(','):
+        m = re.match(r'^(\d+)-(\d+)$', p)
+        out.extend(range(int(m.group(1)), int(m.group(2)) + 1) if m else [int(p)])
+    return out
+
+
+def _tuple(s):
+    """'4x2' or '4,2' -> (4, 2) (parse_tuple of the scripts)."""
+    m = re.match(r'^(\d+)[x,](\d+)$', s)
+    if not m:
+        raise argparse.ArgumentTypeError(f'cannot parse tuple {s}')
+    return int(m.group(1)), int(m.group(2))
+
+
+def _parser():
+    p = argparse.ArgumentParser(prog='python -m next3d_b200', description=__doc__.split('\n')[0])
+    sub = p.add_subparsers(dest='command', required=True)
+    # --fov-deg is declared type=int with the default 18.837 in the scripts, which click casts to 18 when the option is omitted
+    s = sub.add_parser('gen_samples', help='sample sheets (three yaws per seed) and optional .mrc density grids')
+    s.add_argument('--network', required=True, help='network pickle (local file)')
+    s.add_argument('--seeds', type=_range, required=True)
+    s.add_argument('--obj_path', required=True)
+    s.add_argument('--lms_path', required=True)
+    s.add_argument('--trunc', dest='truncation_psi', type=float, default=1)
+    s.add_argument('--trunc-cutoff', dest='truncation_cutoff', type=int, default=14)
+    s.add_argument('--outdir', required=True)
+    s.add_argument('--shapes', type=_bool, default=False)
+    s.add_argument('--shape-res', dest='shape_res', type=int, default=512)
+    s.add_argument('--fov-deg', dest='fov_deg', type=int, default=18)
+    s.add_argument('--shape-format', dest='shape_format', choices=['.mrc', '.ply'], default='.mrc')
+    s.add_argument('--lms_cond', type=_bool, default=False)
+    s.add_argument('--reload_modules', type=_bool, default=False)
+
+    v = sub.add_parser('gen_videos', help='latent interpolation (or one-head orbit) videos')
+    v.add_argument('--network', required=True, help='network pickle (local file)')
+    v.add_argument('--seeds', type=_range, required=True)
+    v.add_argument('--obj_path', required=True)
+    v.add_argument('--lms_path', required=True)
+    v.add_argument('--shuffle-seed', dest='shuffle_seed', type=int, default=None)
+    v.add_argument('--grid', type=_tuple, default=(1, 1))
+    v.add_argument('--num-keyframes', dest='num_keyframes', type=int, default=None)
+    v.add_argument('--w-frames', dest='w_frames', type=int, default=240)
+    v.add_argument('--trunc', dest='truncation_psi', type=float, default=1)
+    v.add_argument('--trunc-cutoff', dest='truncation_cutoff', type=int, default=14)
+    v.add_argument('--outdir', required=True)
+    v.add_argument('--reload_modules', type=_bool, default=False)
+    v.add_argument('--cfg', choices=['FFHQ', 'AFHQ', 'Shapenet'], default='FFHQ')
+    v.add_argument('--image_mode', choices=['image', 'image_depth', 'image_raw'], default='image')
+    v.add_argument('--sample_mult', dest='sampling_multiplier', type=float, default=2)
+    v.add_argument('--nrr', type=int, default=None)
+    v.add_argument('--interpolate', type=_bool, default=True)
+    v.add_argument('--save_root', default=None)
+    v.add_argument('--lms_cond', type=_bool, default=False)
+
+    r = sub.add_parser('reenact', help='drive one or more identities with a tracked mesh sequence')
+    r.add_argument('--drive_root', required=True)
+    r.add_argument('--fname', default='reenact.mp4')
+    r.add_argument('--network', required=True, help='network pickle (local file)')
+    r.add_argument('--grid', dest='grid_dims', type=_tuple, default=(1, 1))
+    r.add_argument('--seeds', type=_range, required=True)
+    r.add_argument('--outdir', required=True)
+    r.add_argument('--fov-deg', dest='fov_deg', type=int, default=18)
+    r.add_argument('--trunc', dest='truncation_psi', type=float, default=1)
+    r.add_argument('--trunc-cutoff', dest='truncation_cutoff', type=int, default=14)
+    r.add_argument('--reload_modules', type=_bool, default=False)
+    r.add_argument('--lms_cond', type=_bool, default=False)
+    r.add_argument('--fixed_camera', type=_bool, default=False)
+    r.add_argument('--num_frames', type=int, default=500)
+    return p
+
+
+def _refuse(msg):
+    raise SystemExit(f'next3d_b200: {msg}')
+
+
+def _imageio():
+    try:
+        import imageio
+    except ImportError:
+        _refuse('writing mp4 videos needs the imageio package (with its ffmpeg plugin), which cannot be imported')
+    return imageio
+
+
+def _load(args):
+    from . import legacy
+    from .triplane_next3d import TriPlaneGenerator
+    print(f'Loading networks from "{args.network}"...')
+    with open(args.network, 'rb') as f:
+        G = legacy.load_network_pkl(f)['G_ema']
+    if args.reload_modules:                                  # the scripts' rebuilt generator reads the eye mask from its PNG again
+        G.uv_face_mask = TriPlaneGenerator._load_uv_face_mask()
+    return G.to('cuda')
+
+
+def _mesh(args):
+    from . import inputs
+    return inputs.load_frame(args.obj_path, args.lms_path).to('cuda')
+
+
+def _write_video(imageio, path, frames, fps, bitrate):
+    writer = imageio.get_writer(path, mode='I', fps=fps, codec='libx264', bitrate=bitrate)
+    try:
+        for frame in frames:
+            writer.append_data(frame)
+    finally:
+        writer.close()
+
+
+def gen_samples(args):
+    """gen_samples_next3d.py: seedNNNN.png sheets and, with --shapes, seedNNNN.mrc density grids."""
+    import PIL.Image
+    from . import drivers, mrc
+    if args.shape_format == '.ply':
+        _refuse('--shape-format .ply needs marching cubes, which is outside this project; use .mrc')
+    G = _load(args)
+    v = _mesh(args)
+    os.makedirs(args.outdir, exist_ok=True)
+    ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
+    for i, sheet, sigmas in drivers.render_sample_sheets(G, ws, v, fov_deg=args.fov_deg, shapes=args.shapes, shape_res=args.shape_res,
+                                                         seed=SAMPLER_SEED):
+        name = os.path.join(args.outdir, f'seed{args.seeds[i]:04d}')
+        PIL.Image.fromarray(sheet, 'RGB').save(name + '.png')
+        if sigmas is not None:
+            mrc.write_mrc(name + '.mrc', sigmas)
+
+
+def gen_videos(args):
+    """gen_videos_next3d.py: interpolation.mp4 over a --grid of seeds, or with --interpolate False one orbit video SEED.mp4 per seed."""
+    from . import drivers
+    if args.cfg != 'FFHQ':
+        _refuse(f'--cfg {args.cfg}: only the FFHQ generator is implemented')
+    if not args.interpolate and tuple(args.grid) != (1, 1):
+        _refuse('--interpolate False renders one head per video: use --grid 1x1')
+    imageio = _imageio()
+    G = _load(args)
+    rk = G.rendering_kwargs
+    rk['depth_resolution'] = int(rk['depth_resolution'] * args.sampling_multiplier)
+    rk['depth_resolution_importance'] = int(rk['depth_resolution_importance'] * args.sampling_multiplier)
+    v = _mesh(args)
+    if args.nrr is not None:
+        G.neural_rendering_resolution = args.nrr
+    psi, cutoff = args.truncation_psi, args.truncation_cutoff
+    if cutoff == 0:
+        psi = 1.0
+    if psi == 1.0:
+        cutoff = 14
+    os.makedirs(args.outdir, exist_ok=True)
+    if args.save_root is not None:
+        os.makedirs(args.save_root, exist_ok=True)
+    if args.interpolate:
+        ws = drivers.grid_keyframes(G, args.seeds, args.grid, args.num_keyframes, args.shuffle_seed, psi, cutoff)
+        frames = drivers.render_grid_frames(G, ws, v, args.w_frames, image_mode=args.image_mode, seed=SAMPLER_SEED)
+        _write_video(imageio, os.path.join(args.outdir, 'interpolation.mp4'), frames, 60, '10M')
+        return
+    for seed in args.seeds:
+        ws = drivers.grid_keyframes(G, [seed], (1, 1), args.num_keyframes, args.shuffle_seed, psi, cutoff)[0, 0]
+        cams = drivers.orbit_camera_params(ws.shape[0] * args.w_frames, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
+        frames = drivers.render_orbit(G, ws[:1], cams, v, image_mode=args.image_mode, seed=SAMPLER_SEED)
+        _write_video(imageio, os.path.join(args.outdir, f'{seed}.mp4'), frames, 60, '12M')
+
+
+def reenact(args):
+    """reenact_avatar_next3d.py: --fname (reenact.mp4), the driving photo next to one avatar per seed in a --grid."""
+    from . import drivers
+    imageio = _imageio()
+    G = _load(args)
+    G.rendering_kwargs['return_normal'] = False
+    os.makedirs(args.outdir, exist_ok=True)
+    _, cond = drivers.sample_sheet_cameras(G, args.fov_deg)
+    ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
+    frames = drivers.reenact_grid_frames(G, ws, args.drive_root, args.num_frames, args.grid_dims, lms_cond=True,
+                                         fixed_camera=cond if args.fixed_camera else None, seed=SAMPLER_SEED)
+    _write_video(imageio, os.path.join(args.outdir, args.fname), frames, 30, '12M')
+
+
+def main(argv=None):
+    args = _parser().parse_args(argv)
+    if not args.lms_cond:
+        _refuse('pass --lms_cond True: the generator reads the 68 landmarks that follow the mesh vertices (load_lms)')
+    {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact}[args.command](args)
+
+
+if __name__ == '__main__':
+    main(sys.argv[1:])

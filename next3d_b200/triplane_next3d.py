@@ -43,6 +43,9 @@ class TriPlaneGenerator(torch.nn.Module):
     def __init__(self, z_dim=512, c_dim=25, w_dim=512, img_resolution=512, img_channels=3, topology_path=None, sr_num_fp16_res=0,
                  mapping_kwargs={}, rendering_kwargs={}, sr_kwargs={}, **synthesis_kwargs):
         super().__init__()
+        # legacy.load_network_pkl passes the pickled eye mask and topology buffers, so no file is read (private keywords)
+        uv_face_mask = synthesis_kwargs.pop('_uv_face_mask', None)
+        topo = synthesis_kwargs.pop('_topology_buffers', None)
         assert z_dim == 512 and w_dim == 512 and c_dim == 25 and img_channels == 3, 'only the FFHQ Next3D topology is supported'
         assert mapping_kwargs.get('num_layers', 2) == 2, 'MappingNetwork with num_layers=2 expected (train_next3d.py:369)'
         self.z_dim, self.c_dim, self.w_dim = z_dim, c_dim, w_dim
@@ -59,8 +62,7 @@ class TriPlaneGenerator(torch.nn.Module):
         self.fill_mouth = True
         self.sr_num_fp16_res = sr_num_fp16_res
         self._sr_precision = 'fp32'
-        self.uv_face_mask = self._load_uv_face_mask()
-        topo = None
+        self.uv_face_mask = self._load_uv_face_mask() if uv_face_mask is None else uv_face_mask
         for name, shape, kind, _ in _config.param_spec(self.cfg):
             if kind == 'topology':
                 topo = topo or _weights.topology_buffers(self._load_mesh(topology_path))
