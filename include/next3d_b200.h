@@ -421,6 +421,33 @@ int n3d_parse_obj_vertices(const char* text, int64_t len, float* xyz, int64_t ma
  * (gen_samples_next3d.py:176-177): float64 parse, float32 store; every non-empty row must have *n_cols columns. */
 int n3d_parse_float_table(const char* text, int64_t len, float* values, int64_t max_values, int64_t* n_values, int64_t* n_cols);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * H.264 encoder (next3d_b200/video.py; DESIGN.md section 3): Constrained Baseline (profile_idc 66), 8-bit 4:2:0 BT.601 limited
+ * range, CAVLC, constant QP, one slice per macroblock row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip
+ * with integer-pel motion against the previous frame, deblocking disabled (so the reconstruction is the decoder's output).
+ * Stateless: the caller owns the reconstruction buffers and carries the reference from frame to frame.  The SPS / PPS are
+ * written by the caller (next3d_b200.video.sps / pps: log2_max_frame_num 4, pic_order_cnt_type 2, pic_init_qp = qp).
+ * ---------------------------------------------------------------------------------------------------------- */
+
+/* Host only.  Buffer sizes in bytes for width x height frames: plane_bytes = one padded I420 picture (width and height rounded
+ * up to multiples of 16; Y, then Cb, then Cr), scratch_bytes = per-macroblock state, slice_bytes = one bounded slot per
+ * macroblock row, sample_bytes = capacity of one encoded frame.  The slot bound is derived from the syntax written (27 residual
+ * blocks of at most 641 bits plus a 128-bit macroblock header, emulation prevention included); the Annex A limit of 3200 bits
+ * per macroblock is not enforced (it can be exceeded only at very low QP on noise).  N3D_ERR_INVALID_ARG for odd or
+ * non-positive sizes and frames above level 6.2 (139264 macroblocks, at most 1055 per side). */
+int n3d_h264_buffer_sizes(int width, int height, int64_t* plane_bytes, int64_t* scratch_bytes, int64_t* slice_bytes,
+                          int64_t* sample_bytes);
+
+/* Encode one frame.  rgb: device uint8 [height, width, 3] contiguous.  qp 0..51.  idr != 0: IDR picture (ref unused, may be
+ * NULL); else a P picture predicted from ref (the previous frame's recon, plane_bytes, != recon).  frame_num: 0..15 (frames
+ * since the last IDR, mod 16); idr_pic_id 0..65535 (must differ between consecutive IDR pictures).  cur (plane_bytes), scratch
+ * and slices are work space; recon (plane_bytes) receives the reconstruction.  sample (sample_bytes) receives the access unit as
+ * length-prefixed NAL units (4-byte big-endian lengths, one slice per macroblock row) and *sample_len (device int64) its size,
+ * or -1 if a slice exceeded its slot (the slot is never written past).  No host synchronisation. */
+int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp, int idr, int frame_num, int idr_pic_id, uint8_t* cur,
+                    const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,9 @@ run) and rendered by the batched drivers of next3d_b200.drivers on one CUDA devi
     the scripts fail as well;
   * `--shape-format .ply` (marching-cubes export) and `--cfg` other than FFHQ are refused, and so is `--interpolate False` with a
     grid larger than 1x1 (every cell would show the same head);
-  * mp4 files are written with imageio; without it the video commands refuse before loading the network.
+  * mp4 files are written with imageio (libx264 at the scripts' bitrates); without it the video commands refuse before loading
+    the network.  `--encoder n3d` writes them with this package's H.264 encoder on the GPU instead (next3d_b200.video: constant
+    `--qp`, default 18, integer-pel motion, no deblocking; INTEGRATION.md section 0) and never imports imageio.
 """
 import argparse
 import os
@@ -86,6 +88,7 @@ def _parser():
     v.add_argument('--interpolate', type=_bool, default=True)
     v.add_argument('--save_root', default=None)
     v.add_argument('--lms_cond', type=_bool, default=False)
+    _encoder_args(v)
 
     r = sub.add_parser('reenact', help='drive one or more identities with a tracked mesh sequence')
     r.add_argument('--drive_root', required=True)
@@ -101,7 +104,14 @@ def _parser():
     r.add_argument('--lms_cond', type=_bool, default=False)
     r.add_argument('--fixed_camera', type=_bool, default=False)
     r.add_argument('--num_frames', type=int, default=500)
+    _encoder_args(r)
     return p
+
+
+def _encoder_args(p):
+    p.add_argument('--encoder', choices=['imageio', 'n3d'], default='imageio',
+                   help='imageio: libx264 through imageio (the scripts); n3d: the sm_90a H.264 encoder of next3d_b200.video')
+    p.add_argument('--qp', type=int, default=18, help='constant quantiser 0..51 of --encoder n3d (lower = larger, closer)')
 
 
 def _refuse(msg):
@@ -112,8 +122,19 @@ def _imageio():
     try:
         import imageio
     except ImportError:
-        _refuse('writing mp4 videos needs the imageio package (with its ffmpeg plugin), which cannot be imported')
+        _refuse('writing mp4 videos needs the imageio package (with its ffmpeg plugin), which cannot be imported; '
+                'or pass --encoder n3d')
     return imageio
+
+
+def _video_writer(args):
+    """write(path, frames, fps, bitrate) of the chosen --encoder, checked before the network is loaded."""
+    if args.encoder == 'imageio':
+        imageio = _imageio()
+        return lambda path, frames, fps, bitrate: _write_video(imageio, path, frames, fps, bitrate)
+    if not 0 <= args.qp <= 51:
+        _refuse(f'--qp {args.qp}: the quantiser is 0..51')
+    return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, args.qp)
 
 
 def _load(args):
@@ -141,6 +162,19 @@ def _write_video(imageio, path, frames, fps, bitrate):
         writer.close()
 
 
+def _write_video_n3d(path, frames, fps, qp):
+    from .video import H264Writer
+    writer = None
+    try:
+        for frame in frames:
+            if writer is None:
+                writer = H264Writer(path, frame.shape[1], frame.shape[0], fps, qp=qp)
+            writer.write(frame)
+    finally:
+        if writer is not None:
+            writer.close()
+
+
 def gen_samples(args):
     """gen_samples_next3d.py: seedNNNN.png sheets and, with --shapes, seedNNNN.mrc density grids."""
     import PIL.Image
@@ -166,7 +200,7 @@ def gen_videos(args):
         _refuse(f'--cfg {args.cfg}: only the FFHQ generator is implemented')
     if not args.interpolate and tuple(args.grid) != (1, 1):
         _refuse('--interpolate False renders one head per video: use --grid 1x1')
-    imageio = _imageio()
+    write = _video_writer(args)
     G = _load(args)
     rk = G.rendering_kwargs
     rk['depth_resolution'] = int(rk['depth_resolution'] * args.sampling_multiplier)
@@ -185,19 +219,19 @@ def gen_videos(args):
     if args.interpolate:
         ws = drivers.grid_keyframes(G, args.seeds, args.grid, args.num_keyframes, args.shuffle_seed, psi, cutoff)
         frames = drivers.render_grid_frames(G, ws, v, args.w_frames, image_mode=args.image_mode, seed=SAMPLER_SEED)
-        _write_video(imageio, os.path.join(args.outdir, 'interpolation.mp4'), frames, 60, '10M')
+        write(os.path.join(args.outdir, 'interpolation.mp4'), frames, 60, '10M')
         return
     for seed in args.seeds:
         ws = drivers.grid_keyframes(G, [seed], (1, 1), args.num_keyframes, args.shuffle_seed, psi, cutoff)[0, 0]
         cams = drivers.orbit_camera_params(ws.shape[0] * args.w_frames, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
         frames = drivers.render_orbit(G, ws[:1], cams, v, image_mode=args.image_mode, seed=SAMPLER_SEED)
-        _write_video(imageio, os.path.join(args.outdir, f'{seed}.mp4'), frames, 60, '12M')
+        write(os.path.join(args.outdir, f'{seed}.mp4'), frames, 60, '12M')
 
 
 def reenact(args):
     """reenact_avatar_next3d.py: --fname (reenact.mp4), the driving photo next to one avatar per seed in a --grid."""
     from . import drivers
-    imageio = _imageio()
+    write = _video_writer(args)
     G = _load(args)
     G.rendering_kwargs['return_normal'] = False
     os.makedirs(args.outdir, exist_ok=True)
@@ -205,7 +239,7 @@ def reenact(args):
     ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
     frames = drivers.reenact_grid_frames(G, ws, args.drive_root, args.num_frames, args.grid_dims, lms_cond=True,
                                          fixed_camera=cond if args.fixed_camera else None, seed=SAMPLER_SEED)
-    _write_video(imageio, os.path.join(args.outdir, args.fname), frames, 30, '12M')
+    write(os.path.join(args.outdir, args.fname), frames, 30, '12M')
 
 
 def main(argv=None):

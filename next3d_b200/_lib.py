@@ -116,6 +116,8 @@ _SIGNATURES = {
     'n3d_render_floor': ([P, C.c_int, P, P], C.c_int),
     'n3d_mapping': ([P, P, C.c_int, F32, P, P, P, P, P, P, P, F32, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_interp_rows': ([P, P, C.c_int, C.c_int, I64, P, P], C.c_int),
+    'n3d_h264_buffer_sizes': ([C.c_int, C.c_int, C.POINTER(I64), C.POINTER(I64), C.POINTER(I64), C.POINTER(I64)], C.c_int),
+    'n3d_h264_encode': ([P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P], C.c_int),
     'n3d_sample_grid': ([P, C.c_int, C.c_int, C.c_int, F32, F32, I64, I64, C.c_int, F32, P, P, P, P, P, P], C.c_int),
 }
 

@@ -1,0 +1,678 @@
+// H.264 encoder (Constrained Baseline, CAVLC) for the video writer (next3d_b200/video.py; DESIGN.md section 3.5).
+//
+// One slice per macroblock (MB) row, so every neighbour above an MB is in another slice and "not available": intra 16x16 uses DC
+// or horizontal prediction, the P_Skip MV is (0,0), and the MV predictor is the left MB's MV.  Rows are independent.
+//   h264_rgb_to_yuv   uint8 RGB HWC -> padded I420 planes, BT.601 limited range in integers.
+//   h264_intra_rows   IDR frames: one warp per MB row, MBs in order (each needs its left neighbour's reconstruction); lanes 0-15
+//                     own the luma 4x4 blocks, lanes 16-23 the chroma blocks.
+//   h264_inter_mbs    P frames: one block per MB; integer-pel full search over [-kSearch, kSearch]^2 against the previous
+//                     reconstruction (coordinates clamped, as the decoder clamps them), then transform / quantise / reconstruct.
+//   h264_write_rows   CAVLC: one thread per row writes the slice NAL unit (header, MB layer, trailing bits, emulation prevention)
+//                     into its own bounded slot, length-prefixed.
+//   h264_pack         concatenates the slots into one AVCC sample (an MP4 sample of the frame).
+// The numpy restatement in tests/h264_oracle.py makes the same decisions and writes the same bytes.
+#include "common.cuh"
+
+namespace {
+
+constexpr int kSearch = 16;                     // integer-pel search range (luma samples); MVs are stored in quarter-pel units
+constexpr int kWin = 16 + 2 * kSearch;          // reference window side
+constexpr int kCands = (2 * kSearch + 1) * (2 * kSearch + 1);
+constexpr int kLevelMax = 2063;                 // largest |level| CAVLC codes with level_prefix <= 15 (Baseline) at any suffixLength
+constexpr int kMaxFs = 139264;                  // level 6.2 MaxFS (macroblocks)
+constexpr int kBlockBits = 16 + 3 + 16 * 28 + 9 + 15 * 11;   // coeff_token, T1 signs, 16 escaped levels, total_zeros, run_before
+constexpr int kMbBits = 27 * kBlockBits + 128;  // 27 residual blocks + MB header (skip run, type, mvd, cbp, qp delta)
+
+// Per-MB record between the decision kernels and the writer.  lv: levels in zig-zag order per block: 0-15 luma 4x4 blocks
+// (luma4x4BlkIdx order; index 0 unused for I_16x16), 16 luma DC (I_16x16), 17 chroma DC (Cb 0-3, Cr 4-7), 18-21 Cb AC, 22-25 Cr AC
+// (index 0 unused).  Unused entries are zero.
+struct MbRec {
+    int16_t lv[26][16];
+    int32_t mode;          // I: Intra16x16PredMode (1 horizontal, 2 DC); P: 0
+    int32_t mvx, mvy;      // quarter-pel (P)
+    int32_t pad;
+};
+
+__constant__ int8_t c_zz[16] = {0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15};
+__constant__ int8_t c_blk_x[16] = {0, 1, 0, 1, 2, 3, 2, 3, 0, 1, 0, 1, 2, 3, 2, 3};
+__constant__ int8_t c_blk_y[16] = {0, 0, 1, 1, 0, 0, 1, 1, 2, 2, 3, 3, 2, 2, 3, 3};
+__constant__ uint8_t c_lambda[52] = {0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 5, 5, 6, 7, 7, 8, 9,
+                                     10, 12, 13, 15, 17, 19, 21, 23, 26, 30, 33, 37, 42, 47, 53, 59, 66, 74, 83};
+__constant__ int c_mf[6][3] = {{13107, 5243, 8066}, {11916, 4660, 7490}, {10082, 4194, 6554}, {9362, 3647, 5825}, {8192, 3355, 5243}, {7282, 2893, 4559}};
+__constant__ int c_v[6][3] = {{10, 16, 13}, {11, 18, 14}, {13, 20, 16}, {14, 23, 18}, {16, 25, 20}, {18, 29, 23}};
+__constant__ uint8_t c_inter_cbp_code[48] = {0, 2, 3, 7, 4, 8, 17, 13, 5, 18, 9, 14, 10, 15, 16, 11, 1, 32, 33, 36, 34, 37, 44, 40,
+                                             35, 45, 38, 41, 39, 42, 43, 19, 6, 24, 25, 20, 26, 21, 46, 28, 27, 47, 22, 29, 23, 30, 31, 12};
+
+// coeff_token (Table 9-5), index 4 * TotalCoeff + TrailingOnes: 0 <= nC < 2, 2 <= nC < 4, 4 <= nC < 8, 8 <= nC
+__constant__ uint8_t c_ct_len[4][68] = {
+    {1, 0, 0, 0, 6, 2, 0, 0, 8, 6, 3, 0, 9, 8, 7, 5, 10, 9, 8, 6, 11, 10, 9, 7, 13, 11, 10, 8, 13, 13, 11, 9, 13, 13, 13, 10,
+     14, 14, 13, 11, 14, 14, 14, 13, 15, 15, 14, 14, 15, 15, 15, 14, 16, 15, 15, 15, 16, 16, 16, 15, 16, 16, 16, 16, 16, 16, 16, 16},
+    {2, 0, 0, 0, 6, 2, 0, 0, 6, 5, 3, 0, 7, 6, 6, 4, 8, 6, 6, 4, 8, 7, 7, 5, 9, 8, 8, 6, 11, 9, 9, 6, 11, 11, 11, 7,
+     12, 11, 11, 9, 12, 12, 12, 11, 12, 12, 12, 11, 13, 13, 13, 12, 13, 13, 13, 13, 13, 14, 13, 13, 14, 14, 14, 13, 14, 14, 14, 14},
+    {4, 0, 0, 0, 6, 4, 0, 0, 6, 5, 4, 0, 6, 5, 5, 4, 7, 5, 5, 4, 7, 5, 5, 4, 7, 6, 6, 4, 7, 6, 6, 4, 8, 7, 7, 5,
+     8, 8, 7, 6, 9, 8, 8, 7, 9, 9, 8, 8, 9, 9, 9, 8, 10, 9, 9, 9, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10},
+    {6, 0, 0, 0, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6,
+     6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6, 6}};
+__constant__ uint8_t c_ct_bits[4][68] = {
+    {1, 0, 0, 0, 5, 1, 0, 0, 7, 4, 1, 0, 7, 6, 5, 3, 7, 6, 5, 3, 7, 6, 5, 4, 15, 6, 5, 4, 11, 14, 5, 4, 8, 10, 13, 4,
+     15, 14, 9, 4, 11, 10, 13, 12, 15, 14, 9, 12, 11, 10, 13, 8, 15, 1, 9, 12, 11, 14, 13, 8, 7, 10, 9, 12, 4, 6, 5, 8},
+    {3, 0, 0, 0, 11, 2, 0, 0, 7, 7, 3, 0, 7, 10, 9, 5, 7, 6, 5, 4, 4, 6, 5, 6, 7, 6, 5, 8, 15, 6, 5, 4, 11, 14, 13, 4,
+     15, 10, 9, 4, 11, 14, 13, 12, 8, 10, 9, 8, 15, 14, 13, 12, 11, 10, 9, 12, 7, 11, 6, 8, 9, 8, 10, 1, 7, 6, 5, 4},
+    {15, 0, 0, 0, 15, 14, 0, 0, 11, 15, 13, 0, 8, 12, 14, 12, 15, 10, 11, 11, 11, 8, 9, 10, 9, 14, 13, 9, 8, 10, 9, 8,
+     15, 14, 13, 13, 11, 14, 10, 12, 15, 10, 13, 12, 11, 14, 9, 12, 8, 10, 13, 8, 13, 7, 9, 12, 9, 12, 11, 10, 5, 8, 7, 6,
+     1, 4, 3, 2},
+    {3, 0, 0, 0, 0, 1, 0, 0, 4, 5, 6, 0, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29,
+     30, 31, 32, 33, 34, 35, 36, 37, 38, 39, 40, 41, 42, 43, 44, 45, 46, 47, 48, 49, 50, 51, 52, 53, 54, 55, 56, 57, 58, 59,
+     60, 61, 62, 63}};
+__constant__ uint8_t c_cdc_ct_len[20] = {2, 0, 0, 0, 6, 1, 0, 0, 6, 6, 3, 0, 6, 7, 7, 6, 6, 8, 8, 7};
+__constant__ uint8_t c_cdc_ct_bits[20] = {1, 0, 0, 0, 7, 1, 0, 0, 4, 6, 1, 0, 3, 3, 2, 5, 2, 3, 2, 0};
+// total_zeros (Tables 9-7, 9-8), [TotalCoeff - 1][total_zeros]
+__constant__ uint8_t c_tz_len[15][16] = {
+    {1, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 9}, {3, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 6, 6, 6, 6}, {4, 3, 3, 3, 4, 4, 3, 3, 4, 5, 5, 6, 5, 6},
+    {5, 3, 4, 4, 3, 3, 3, 4, 3, 4, 5, 5, 5}, {4, 4, 4, 3, 3, 3, 3, 3, 4, 5, 4, 5}, {6, 5, 3, 3, 3, 3, 3, 3, 4, 3, 6},
+    {6, 5, 3, 3, 3, 2, 3, 4, 3, 6}, {6, 4, 5, 3, 2, 2, 3, 3, 6}, {6, 6, 4, 2, 2, 3, 2, 5}, {5, 5, 3, 2, 2, 2, 4}, {4, 4, 3, 3, 1, 3},
+    {4, 4, 2, 1, 3}, {3, 3, 1, 2}, {2, 2, 1}, {1, 1}};
+__constant__ uint8_t c_tz_bits[15][16] = {
+    {1, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 1}, {7, 6, 5, 4, 3, 5, 4, 3, 2, 3, 2, 3, 2, 1, 0}, {5, 7, 6, 5, 4, 3, 4, 3, 2, 3, 2, 1, 1, 0},
+    {3, 7, 5, 4, 6, 5, 4, 3, 3, 2, 2, 1, 0}, {5, 4, 3, 7, 6, 5, 4, 3, 2, 1, 1, 0}, {1, 1, 7, 6, 5, 4, 3, 2, 1, 1, 0},
+    {1, 1, 5, 4, 3, 3, 2, 1, 1, 0}, {1, 1, 1, 3, 3, 2, 2, 1, 0}, {1, 0, 1, 3, 2, 1, 1, 1}, {1, 0, 1, 3, 2, 1, 1}, {0, 1, 1, 2, 1, 3},
+    {0, 1, 1, 1, 1}, {0, 1, 1, 1}, {0, 1, 1}, {0, 1}};
+__constant__ uint8_t c_cdc_tz_len[3][4] = {{1, 2, 3, 3}, {1, 2, 2}, {1, 1}};
+__constant__ uint8_t c_cdc_tz_bits[3][4] = {{1, 1, 1, 0}, {1, 1, 0}, {1, 0}};
+// run_before (Table 9-10), [min(zerosLeft, 7) - 1][run_before]
+__constant__ uint8_t c_run_len[7][15] = {{1, 1}, {1, 2, 2}, {2, 2, 2, 2}, {2, 2, 2, 3, 3}, {2, 2, 3, 3, 3, 3}, {2, 3, 3, 3, 3, 3, 3},
+                                         {3, 3, 3, 3, 3, 3, 3, 4, 5, 6, 7, 8, 9, 10, 11}};
+__constant__ uint8_t c_run_bits[7][15] = {{1, 0}, {1, 1, 0}, {3, 2, 1, 0}, {3, 2, 1, 1, 0}, {3, 2, 3, 2, 1, 0}, {3, 0, 1, 3, 2, 5, 4},
+                                          {7, 6, 5, 4, 3, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1}};
+
+struct Frame {
+    int W, H, W16, H16, mbw, mbh, qp, qpc;
+    const uint8_t* rgb;
+    uint8_t* cur;              // padded I420 of the input
+    const uint8_t* ref;        // padded I420 reconstruction of the previous frame (P)
+    uint8_t* rec;              // padded I420 reconstruction of this frame
+    MbRec* mbs;
+    int32_t* lens;             // bytes per slot, -1 when the slot overflowed
+    uint8_t* slots;
+    int64_t slot_cap;
+    int idr, frame_num, idr_pic_id;
+    __device__ uint8_t* plane(uint8_t* base, int c) const { return base + (c == 0 ? 0 : (int64_t)W16 * H16 + (int64_t)(c - 1) * (W16 / 2) * (H16 / 2)); }
+    __device__ const uint8_t* cplane(const uint8_t* base, int c) const { return base + (c == 0 ? 0 : (int64_t)W16 * H16 + (int64_t)(c - 1) * (W16 / 2) * (H16 / 2)); }
+};
+
+// ------------------------------------------------------------------------------------------------ transforms and quantisation
+__device__ __forceinline__ int cls4(int r) { const int i = r >> 2, j = r & 3; return ((i | j) & 1) == 0 ? 0 : ((i & j) & 1) ? 1 : 2; }
+
+__device__ void fwd4(const int* x, int* w) {           // W = Cf X Cf^T, raster 4x4
+    int t[16];
+    for (int j = 0; j < 4; ++j) {                       // columns: Cf X
+        const int a = x[j], b = x[4 + j], c = x[8 + j], d = x[12 + j];
+        t[j] = a + b + c + d; t[4 + j] = 2 * a + b - c - 2 * d; t[8 + j] = a - b - c + d; t[12 + j] = a - 2 * b + 2 * c - d;
+    }
+    for (int i = 0; i < 4; ++i) {                       // rows: (Cf X) Cf^T
+        const int a = t[4 * i], b = t[4 * i + 1], c = t[4 * i + 2], d = t[4 * i + 3];
+        w[4 * i] = a + b + c + d; w[4 * i + 1] = 2 * a + b - c - 2 * d; w[4 * i + 2] = a - b - c + d; w[4 * i + 3] = a - 2 * b + 2 * c - d;
+    }
+}
+
+__device__ void inv4(const int* d, int* r) {            // 8.5.12.2, then (x + 32) >> 6
+    int f[16];
+    for (int i = 0; i < 4; ++i) {
+        const int* a = d + 4 * i;
+        const int e0 = a[0] + a[2], e1 = a[0] - a[2], e2 = (a[1] >> 1) - a[3], e3 = a[1] + (a[3] >> 1);
+        f[4 * i] = e0 + e3; f[4 * i + 1] = e1 + e2; f[4 * i + 2] = e1 - e2; f[4 * i + 3] = e0 - e3;
+    }
+    for (int j = 0; j < 4; ++j) {
+        const int a0 = f[j], a1 = f[4 + j], a2 = f[8 + j], a3 = f[12 + j];
+        const int e0 = a0 + a2, e1 = a0 - a2, e2 = (a1 >> 1) - a3, e3 = a1 + (a3 >> 1);
+        r[j] = (e0 + e3 + 32) >> 6; r[4 + j] = (e1 + e2 + 32) >> 6; r[8 + j] = (e1 - e2 + 32) >> 6; r[12 + j] = (e0 - e3 + 32) >> 6;
+    }
+}
+
+__device__ __forceinline__ int quant(int w, int mf, int qbits, int64_t f) {
+    int l = (int)(((int64_t)abs(w) * mf + f) >> qbits);
+    l = min(l, kLevelMax);
+    return w < 0 ? -l : l;
+}
+
+__device__ __forceinline__ int64_t dz(int qp, bool intra) { return (int64_t)(1 << (15 + qp / 6)) / (intra ? 3 : 6); }
+
+__device__ __forceinline__ int dequant(int c, int qp, int r) {
+    const int ls = 16 * c_v[qp % 6][cls4(r)];
+    return qp >= 24 ? (c * ls) * (1 << (qp / 6 - 4)) : (c * ls + (1 << (3 - qp / 6))) >> (4 - qp / 6);
+}
+
+// AC quantisation of one 4x4 block's coefficients w (raster) -> levels in zig-zag order (first = 0 skips the DC)
+__device__ void quant_block(const int* w, int qp, bool intra, int first, int16_t* lv) {
+    const int qbits = 15 + qp / 6;
+    const int64_t f = dz(qp, intra);
+    for (int k = 0; k < 16; ++k) {
+        const int r = c_zz[k];
+        lv[k] = k < first ? 0 : (int16_t)quant(w[r], c_mf[qp % 6][cls4(r)], qbits, f);
+    }
+}
+
+// levels (zig-zag) -> residual samples (raster); dc >= INT_MIN + 1: already scaled DC (I_16x16 luma, chroma)
+__device__ void recon_block(const int16_t* lv, int qp, bool has_dc, int dc, int* res) {
+    int d[16];
+    for (int k = 0; k < 16; ++k) d[c_zz[k]] = dequant(lv[k], qp, c_zz[k]);
+    if (has_dc) d[0] = dc;
+    inv4(d, res);
+}
+
+__device__ __forceinline__ int clip255(int v) { return min(max(v, 0), 255); }
+
+__device__ __forceinline__ int ue_bits(unsigned k) { return 2 * (32 - __clz(k + 1)) - 1; }
+__device__ __forceinline__ unsigned se_code(int v) { return v > 0 ? 2u * v - 1 : (unsigned)(-2 * v); }
+
+// Chroma DC of one component: 2x2 transform of the four blocks' DC coefficients, quantise to lv[0..3], scale back to dcc[0..3]
+__device__ void chroma_dc(const int* dc, int qpc, bool intra, int16_t* lv, int* dcc) {
+    const int t[4] = {dc[0] + dc[1] + dc[2] + dc[3], dc[0] - dc[1] + dc[2] - dc[3], dc[0] + dc[1] - dc[2] - dc[3], dc[0] - dc[1] - dc[2] + dc[3]};
+    const int mf = c_mf[qpc % 6][0], qbits = 16 + qpc / 6;
+    const int64_t f = 2 * dz(qpc, intra);
+    int c[4];
+    for (int i = 0; i < 4; ++i) lv[i] = (int16_t)(c[i] = quant(t[i], mf, qbits, f));
+    const int g[4] = {c[0] + c[1] + c[2] + c[3], c[0] - c[1] + c[2] - c[3], c[0] + c[1] - c[2] - c[3], c[0] - c[1] - c[2] + c[3]};
+    const int ls = 16 * c_v[qpc % 6][0];
+    for (int i = 0; i < 4; ++i) dcc[i] = (g[i] * ls * (1 << (qpc / 6))) >> 5;
+}
+
+// ------------------------------------------------------------------------------------------------ colour conversion
+__global__ void h264_rgb_to_yuv(Frame F) {
+    const int cw = F.W16 / 2, ch = F.H16 / 2;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < (int64_t)cw * ch; i += (int64_t)gridDim.x * blockDim.x) {
+        const int cx = (int)(i % cw), cy = (int)(i / cw);
+        uint8_t* Y = F.plane(F.cur, 0);
+        for (int j = 0; j < 4; ++j) {
+            const int x = 2 * cx + (j & 1), y = 2 * cy + (j >> 1);
+            const uint8_t* p = F.rgb + ((int64_t)min(y, F.H - 1) * F.W + min(x, F.W - 1)) * 3;
+            Y[(int64_t)y * F.W16 + x] = (uint8_t)(((66 * p[0] + 129 * p[1] + 25 * p[2] + 128) >> 8) + 16);
+        }
+        const int sx = min(cx, F.W / 2 - 1), sy = min(cy, F.H / 2 - 1);
+        int sr = 0, sg = 0, sb = 0;
+        for (int j = 0; j < 4; ++j) {
+            const uint8_t* p = F.rgb + ((int64_t)(2 * sy + (j >> 1)) * F.W + 2 * sx + (j & 1)) * 3;
+            sr += p[0]; sg += p[1]; sb += p[2];
+        }
+        F.plane(F.cur, 1)[(int64_t)cy * cw + cx] = (uint8_t)(((-38 * sr - 74 * sg + 112 * sb + 512) >> 10) + 128);
+        F.plane(F.cur, 2)[(int64_t)cy * cw + cx] = (uint8_t)(((112 * sr - 94 * sg - 18 * sb + 512) >> 10) + 128);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ IDR: I_16x16, one warp per row
+__global__ void __launch_bounds__(32) h264_intra_rows(Frame F) {
+    __shared__ int s_w[16][16];        // luma coefficients per block (raster)
+    __shared__ int s_cdc[2][4], s_dcc[2][4], s_dcy[16];
+    __shared__ int s_left[16];
+    const int row = blockIdx.x, lane = threadIdx.x;
+    const int qp = F.qp, qpc = F.qpc;
+    const int cw = F.W16 / 2;
+    const uint8_t* Ys = F.cplane(F.cur, 0);
+    uint8_t* Yr = F.plane(F.rec, 0);
+    for (int mbx = 0; mbx < F.mbw; ++mbx) {
+        MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
+        const int x0 = 16 * mbx, y0 = 16 * row;
+        // luma mode: horizontal when its SAD is not larger than DC's (lower mode number wins ties); DC only without a left MB
+        if (lane < 16) s_left[lane] = mbx ? Yr[(int64_t)(y0 + lane) * F.W16 + x0 - 1] : 128;
+        __syncwarp();
+        int sum = 0;
+        for (int i = 0; i < 16; ++i) sum += s_left[i];
+        const int dcp = mbx ? (sum + 8) >> 4 : 128;
+        int sad_h = 0, sad_dc = 0;
+        if (lane < 16) {
+            for (int x = 0; x < 16; ++x) {
+                const int s = Ys[(int64_t)(y0 + lane) * F.W16 + x0 + x];
+                sad_h += abs(s - s_left[lane]);
+                sad_dc += abs(s - dcp);
+            }
+        }
+        for (int o = 16; o; o >>= 1) {
+            sad_h += __shfl_xor_sync(0xffffffffu, sad_h, o);
+            sad_dc += __shfl_xor_sync(0xffffffffu, sad_dc, o);
+        }
+        const int mode = (mbx && sad_h <= sad_dc) ? 1 : 2;
+        // forward transforms: lanes 0-15 luma blocks, 16-23 chroma blocks
+        int w[16], res[16];
+        const int bx = lane < 16 ? c_blk_x[lane] : ((lane - 16) & 1), by = lane < 16 ? c_blk_y[lane] : (((lane - 16) >> 1) & 1);
+        const int comp = lane < 16 ? 0 : 1 + ((lane - 16) >> 2);
+        int pred[16];
+        if (lane < 16) {
+            for (int r = 0; r < 16; ++r) {
+                const int y = 4 * by + (r >> 2), x = 4 * bx + (r & 3);
+                pred[r] = mode == 1 ? s_left[y] : dcp;
+                w[r] = Ys[(int64_t)(y0 + y) * F.W16 + x0 + x] - pred[r];
+            }
+            fwd4(w, s_w[lane]);
+        } else if (lane < 24) {
+            const uint8_t* Cs = F.cplane(F.cur, comp);
+            const uint8_t* Cr = F.plane(F.rec, comp);
+            int p = 128;
+            if (mbx) {
+                int s = 0;
+                for (int i = 0; i < 4; ++i) s += Cr[(int64_t)(8 * row + 4 * by + i) * cw + 8 * mbx - 1];
+                p = (s + 2) >> 2;
+            }
+            for (int r = 0; r < 16; ++r) {
+                pred[r] = p;
+                w[r] = Cs[(int64_t)(8 * row + 4 * by + (r >> 2)) * cw + 8 * mbx + 4 * bx + (r & 3)] - p;
+            }
+            fwd4(w, w);
+            s_cdc[comp - 1][(lane - 16) & 3] = w[0];
+        }
+        __syncwarp();
+        if (lane == 0) {                                 // luma DC: Hadamard, quantise, inverse, scale
+            int m[16], t[16], c[16];
+            for (int k = 0; k < 16; ++k) m[4 * c_blk_y[k] + c_blk_x[k]] = s_w[k][0];
+            for (int j = 0; j < 4; ++j) {
+                const int a = m[j], b = m[4 + j], cc = m[8 + j], d = m[12 + j];
+                t[j] = a + b + cc + d; t[4 + j] = a + b - cc - d; t[8 + j] = a - b - cc + d; t[12 + j] = a - b + cc - d;
+            }
+            for (int i = 0; i < 4; ++i) {
+                const int a = t[4 * i], b = t[4 * i + 1], cc = t[4 * i + 2], d = t[4 * i + 3];
+                m[4 * i] = (a + b + cc + d) >> 1; m[4 * i + 1] = (a + b - cc - d) >> 1; m[4 * i + 2] = (a - b - cc + d) >> 1; m[4 * i + 3] = (a - b + cc - d) >> 1;
+            }
+            const int mf = c_mf[qp % 6][0], qbits = 16 + qp / 6;
+            const int64_t f = 2 * dz(qp, true);
+            for (int r = 0; r < 16; ++r) c[r] = quant(m[r], mf, qbits, f);
+            for (int k = 0; k < 16; ++k) R->lv[16][k] = (int16_t)c[c_zz[k]];
+            for (int j = 0; j < 4; ++j) {
+                const int a = c[j], b = c[4 + j], cc = c[8 + j], d = c[12 + j];
+                t[j] = a + b + cc + d; t[4 + j] = a + b - cc - d; t[8 + j] = a - b - cc + d; t[12 + j] = a - b + cc - d;
+            }
+            const int ls = 16 * c_v[qp % 6][0];
+            for (int i = 0; i < 4; ++i) {
+                const int a = t[4 * i], b = t[4 * i + 1], cc = t[4 * i + 2], d = t[4 * i + 3];
+                const int g[4] = {a + b + cc + d, a + b - cc - d, a - b - cc + d, a - b + cc - d};
+                for (int j = 0; j < 4; ++j)
+                    m[4 * i + j] = qp >= 36 ? (g[j] * ls) * (1 << (qp / 6 - 6)) : (g[j] * ls + (1 << (5 - qp / 6))) >> (6 - qp / 6);
+            }
+            for (int k = 0; k < 16; ++k) s_dcy[k] = m[4 * c_blk_y[k] + c_blk_x[k]];
+            R->mode = mode;
+            R->mvx = R->mvy = 0;
+        } else if (lane == 1 || lane == 2) {
+            chroma_dc(s_cdc[lane - 1], qpc, true, R->lv[17] + 4 * (lane - 1), s_dcc[lane - 1]);
+            for (int k = 0; k < 4; ++k) R->lv[17][8 + 4 * (lane - 1) + k] = 0;
+        }
+        __syncwarp();
+        if (lane < 16) {
+            quant_block(s_w[lane], qp, true, 1, R->lv[lane]);
+            recon_block(R->lv[lane], qp, true, s_dcy[lane], res);
+            for (int r = 0; r < 16; ++r)
+                Yr[(int64_t)(y0 + 4 * by + (r >> 2)) * F.W16 + x0 + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
+        } else if (lane < 24) {
+            int16_t* lv = R->lv[18 + (lane - 16)];
+            quant_block(w, qpc, true, 1, lv);
+            recon_block(lv, qpc, true, s_dcc[comp - 1][(lane - 16) & 3], res);
+            uint8_t* Cr = F.plane(F.rec, comp);
+            for (int r = 0; r < 16; ++r)
+                Cr[(int64_t)(8 * row + 4 * by + (r >> 2)) * cw + 8 * mbx + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
+        }
+        __syncwarp();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ P: one block per MB
+__global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
+    __shared__ uint8_t s_win[kWin][kWin];
+    __shared__ uint8_t s_cur[16][16];
+    __shared__ unsigned long long s_best[8];
+    __shared__ int s_cdc[2][4], s_dcc[2][4];
+    const int mbx = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
+    const int qp = F.qp, qpc = F.qpc;
+    const int x0 = 16 * mbx, y0 = 16 * row;
+    const uint8_t* Yref = F.cplane(F.ref, 0);
+    const uint8_t* Ys = F.cplane(F.cur, 0);
+    for (int i = tid; i < kWin * kWin; i += 256) {
+        const int y = min(max(y0 - kSearch + i / kWin, 0), F.H16 - 1), x = min(max(x0 - kSearch + i % kWin, 0), F.W16 - 1);
+        s_win[i / kWin][i % kWin] = Yref[(int64_t)y * F.W16 + x];
+    }
+    s_cur[tid >> 4][tid & 15] = Ys[(int64_t)(y0 + (tid >> 4)) * F.W16 + x0 + (tid & 15)];
+    __syncthreads();
+    // cost = SAD + lambda * bits of the MV against a zero predictor (so that MBs are decided independently); ties: smaller
+    // |mvx| + |mvy|, then smaller (mvy, mvx)
+    const int lam = c_lambda[qp];
+    unsigned long long best = ~0ull;
+    for (int c = tid; c < kCands; c += 256) {
+        const int my = c / (2 * kSearch + 1) - kSearch, mx = c % (2 * kSearch + 1) - kSearch;
+        int sad = 0;
+        for (int y = 0; y < 16; ++y) {
+            const uint8_t* wr = &s_win[kSearch + my + y][kSearch + mx];
+#pragma unroll
+            for (int x = 0; x < 16; ++x) sad += abs((int)s_cur[y][x] - (int)wr[x]);
+        }
+        const unsigned long long cost = (unsigned long long)(sad + lam * (ue_bits(se_code(4 * mx)) + ue_bits(se_code(4 * my))));
+        const unsigned long long key = (cost << 24) | ((unsigned long long)(abs(mx) + abs(my)) << 16) | ((unsigned long long)(my + kSearch) << 8) | (unsigned long long)(mx + kSearch);
+        best = min(best, key);
+    }
+    for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+    if ((tid & 31) == 0) s_best[tid >> 5] = best;
+    __syncthreads();
+    best = s_best[0];
+    for (int i = 1; i < 8; ++i) best = min(best, s_best[i]);
+    const int mvy = (int)((best >> 8) & 0xff) - kSearch, mvx = (int)(best & 0xff) - kSearch;
+    MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
+    const int cw = F.W16 / 2, chh = F.H16 / 2;
+    int w[16], pred[16], res[16];
+    const int lane = tid;
+    const int bx = lane < 16 ? c_blk_x[lane] : ((lane - 16) & 1), by = lane < 16 ? c_blk_y[lane] : (((lane - 16) >> 1) & 1);
+    const int comp = lane < 16 ? 0 : 1 + ((lane - 16) >> 2);
+    if (lane < 16) {
+        for (int r = 0; r < 16; ++r) {
+            const int y = 4 * by + (r >> 2), x = 4 * bx + (r & 3);
+            pred[r] = s_win[kSearch + mvy + y][kSearch + mvx + x];
+            w[r] = s_cur[y][x] - pred[r];
+        }
+        fwd4(w, w);
+        quant_block(w, qp, false, 0, R->lv[lane]);
+        recon_block(R->lv[lane], qp, false, 0, res);
+        uint8_t* Yr = F.plane(F.rec, 0);
+        for (int r = 0; r < 16; ++r)
+            Yr[(int64_t)(y0 + 4 * by + (r >> 2)) * F.W16 + x0 + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
+    } else if (lane < 24) {                              // chroma: eighth-pel bilinear at the luma MV (8.4.2.2.2)
+        const int mvcx = 4 * mvx, mvcy = 4 * mvy, fx = mvcx & 7, fy = mvcy & 7;
+        const uint8_t* Cref = F.cplane(F.ref, comp);
+        const uint8_t* Cs = F.cplane(F.cur, comp);
+        for (int r = 0; r < 16; ++r) {
+            const int yy = 8 * row + 4 * by + (r >> 2), xx = 8 * mbx + 4 * bx + (r & 3);
+            const int ry = yy + (mvcy >> 3), rx = xx + (mvcx >> 3);
+            auto at = [&](int y, int x) { return (int)Cref[(int64_t)min(max(y, 0), chh - 1) * cw + min(max(x, 0), cw - 1)]; };
+            pred[r] = ((8 - fx) * (8 - fy) * at(ry, rx) + fx * (8 - fy) * at(ry, rx + 1) + (8 - fx) * fy * at(ry + 1, rx) + fx * fy * at(ry + 1, rx + 1) + 32) >> 6;
+            w[r] = Cs[(int64_t)yy * cw + xx] - pred[r];
+        }
+        fwd4(w, w);
+        s_cdc[comp - 1][(lane - 16) & 3] = w[0];
+    } else if (lane == 32) {
+        R->mode = 0;
+        R->mvx = 4 * mvx;
+        R->mvy = 4 * mvy;
+        for (int k = 0; k < 16; ++k) R->lv[16][k] = 0;
+    }
+    __syncthreads();
+    if (lane == 0 || lane == 1) {
+        chroma_dc(s_cdc[lane], qpc, false, R->lv[17] + 4 * lane, s_dcc[lane]);
+        for (int k = 0; k < 4; ++k) R->lv[17][8 + 4 * lane + k] = 0;
+    }
+    __syncthreads();
+    if (lane >= 16 && lane < 24) {
+        int16_t* lv = R->lv[18 + (lane - 16)];
+        quant_block(w, qpc, false, 1, lv);
+        recon_block(lv, qpc, true, s_dcc[comp - 1][(lane - 16) & 3], res);
+        uint8_t* Cr = F.plane(F.rec, comp);
+        for (int r = 0; r < 16; ++r)
+            Cr[(int64_t)(8 * row + 4 * by + (r >> 2)) * cw + 8 * mbx + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ CAVLC slice writer
+struct BitWriter {
+    uint8_t* out;
+    int64_t cap, pos;
+    uint64_t acc;
+    int n, zeros;
+    bool overflow;
+    __device__ void emit(uint8_t b) {
+        if (pos < cap) out[pos] = b; else overflow = true;
+        ++pos;
+    }
+    __device__ void byte(uint8_t b) {                  // emulation prevention: 0x000003 before 0x000000 .. 0x000003
+        if (zeros >= 2 && b <= 3) { emit(3); zeros = 0; }
+        emit(b);
+        zeros = b ? 0 : zeros + 1;
+    }
+    __device__ void u(uint32_t v, int nb) {            // nb <= 32
+        if (!nb) return;
+        acc = (acc << nb) | (v & (uint32_t)((1ull << nb) - 1));
+        n += nb;
+        while (n >= 8) { n -= 8; byte((uint8_t)(acc >> n)); }
+    }
+    __device__ void ue(uint32_t k) {
+        const int len = 32 - __clz(k + 1);
+        u(0, len - 1);
+        u(k + 1, len);
+    }
+    __device__ void se(int v) { ue(se_code(v)); }
+    __device__ void trailing() { u(1, 1); if (n) u(0, 8 - n); }
+};
+
+__device__ __forceinline__ int nc_of(int na, int nb) {          // -1: not available
+    if (na >= 0 && nb >= 0) return (na + nb + 1) >> 1;
+    return na >= 0 ? na : nb >= 0 ? nb : 0;
+}
+
+// residual_block_cavlc (9.2) of n levels (zig-zag order); nc = -1: chroma DC.  Returns TotalCoeff.
+__device__ int residual_block(BitWriter& bw, const int16_t* c, int n, int nc) {
+    int pos[16], total = 0;
+    for (int i = 0; i < n; ++i) if (c[i]) pos[total++] = i;
+    int t1 = 0;
+    for (int k = total - 1; k >= 0 && t1 < 3 && abs(c[pos[k]]) == 1; --k) ++t1;
+    const int idx = 4 * total + t1;
+    if (nc == -1) {
+        bw.u(c_cdc_ct_bits[idx], c_cdc_ct_len[idx]);
+    } else {
+        const int tab = nc < 2 ? 0 : nc < 4 ? 1 : nc < 8 ? 2 : 3;
+        bw.u(c_ct_bits[tab][idx], c_ct_len[tab][idx]);
+    }
+    if (!total) return 0;
+    for (int k = 0; k < t1; ++k) bw.u(c[pos[total - 1 - k]] < 0, 1);
+    int sl = (total > 10 && t1 < 3) ? 1 : 0;
+    for (int k = t1; k < total; ++k) {
+        const int lv = c[pos[total - 1 - k]];
+        int code = lv > 0 ? 2 * lv - 2 : -2 * lv - 1;
+        if (k == t1 && t1 < 3) code -= 2;
+        int prefix, sbits, sval;
+        if (sl == 0) {
+            if (code < 14) { prefix = code; sbits = 0; sval = 0; }
+            else if (code < 30) { prefix = 14; sbits = 4; sval = code - 14; }
+            else { prefix = 15; sbits = 12; sval = code - 30; }
+        } else if (code < (15 << sl)) {
+            prefix = code >> sl; sbits = sl; sval = code & ((1 << sl) - 1);
+        } else {
+            prefix = 15; sbits = 12; sval = code - (15 << sl);
+        }
+        bw.u(1, prefix + 1);
+        bw.u(sval, sbits);
+        if (sl == 0) sl = 1;
+        if (abs(lv) > (3 << (sl - 1)) && sl < 6) ++sl;
+    }
+    if (total < n) {
+        const int tz = pos[total - 1] + 1 - total;
+        if (nc == -1) bw.u(c_cdc_tz_bits[total - 1][tz], c_cdc_tz_len[total - 1][tz]);
+        else bw.u(c_tz_bits[total - 1][tz], c_tz_len[total - 1][tz]);
+        int left = tz;
+        for (int j = total - 1; j > 0 && left > 0; --j) {
+            const int run = pos[j] - pos[j - 1] - 1, t = min(left, 7) - 1;
+            bw.u(c_run_bits[t][run], c_run_len[t][run]);
+            left -= run;
+        }
+    }
+    return total;
+}
+
+__device__ bool any_nonzero(const int16_t* p, int n) {
+    for (int i = 0; i < n; ++i) if (p[i]) return true;
+    return false;
+}
+
+__global__ void h264_write_rows(Frame F) {
+    const int row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= F.mbh) return;
+    uint8_t* slot = F.slots + row * F.slot_cap;
+    BitWriter bw{slot + 5, F.slot_cap - 5, 0, 0, 0, 0, false};
+    const bool idr = F.idr;
+    bw.ue(row * F.mbw);                      // first_mb_in_slice
+    bw.ue(idr ? 2 : 0);                      // slice_type I / P
+    bw.ue(0);                                // pic_parameter_set_id
+    bw.u(F.frame_num, 4);                    // frame_num (log2_max_frame_num = 4)
+    if (idr) {
+        bw.ue(F.idr_pic_id);
+    } else {
+        bw.u(0, 1);                          // num_ref_idx_active_override_flag
+        bw.u(0, 1);                          // ref_pic_list_modification_flag_l0
+    }
+    bw.u(0, 1);                              // no_output_of_prior_pics_flag / adaptive_ref_pic_marking_mode_flag
+    if (idr) bw.u(0, 1);                     // long_term_reference_flag
+    bw.se(0);                                // slice_qp_delta
+    bw.ue(1);                                // disable_deblocking_filter_idc
+    int left_tc[4] = {0, 0, 0, 0}, left_cc[2][2] = {{0, 0}, {0, 0}};
+    int skip_run = 0, mvpx = 0, mvpy = 0;
+    for (int mbx = 0; mbx < F.mbw; ++mbx) {
+        const MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
+        const bool left = mbx > 0;
+        if (!idr && R->mvx == 0 && R->mvy == 0 && !any_nonzero(&R->lv[0][0], 26 * 16)) {     // P_Skip
+            ++skip_run;
+            for (int i = 0; i < 4; ++i) left_tc[i] = 0;
+            left_cc[0][0] = left_cc[0][1] = left_cc[1][0] = left_cc[1][1] = 0;
+            mvpx = mvpy = 0;
+            continue;
+        }
+        int cbp_l = 0;
+        if (idr) {
+            for (int k = 0; k < 16 && !cbp_l; ++k) if (any_nonzero(R->lv[k] + 1, 15)) cbp_l = 15;
+        } else {
+            for (int k = 0; k < 16; ++k) if (any_nonzero(R->lv[k], 16)) cbp_l |= 1 << (k >> 2);
+        }
+        bool cac = false;
+        for (int k = 0; k < 8 && !cac; ++k) cac = any_nonzero(R->lv[18 + k] + 1, 15);
+        const int cbp_c = cac ? 2 : any_nonzero(R->lv[17], 8) ? 1 : 0;
+        if (idr) {
+            bw.ue(1 + R->mode + 4 * cbp_c + (cbp_l ? 12 : 0));     // mb_type I_16x16
+            bw.ue(0);                                            // intra_chroma_pred_mode DC
+            bw.se(0);                                            // mb_qp_delta
+            residual_block(bw, R->lv[16], 16, left ? left_tc[0] : 0);
+        } else {
+            bw.ue(skip_run);
+            skip_run = 0;
+            bw.ue(0);                                            // mb_type P_L0_16x16
+            bw.se(R->mvx - mvpx);
+            bw.se(R->mvy - mvpy);
+            mvpx = R->mvx;
+            mvpy = R->mvy;
+            bw.ue(c_inter_cbp_code[cbp_l + 16 * cbp_c]);
+            if (cbp_l || cbp_c) bw.se(0);                        // mb_qp_delta
+        }
+        int tc[4][4] = {};
+        for (int k = 0; k < 16; ++k) {
+            if (!(cbp_l >> (k >> 2) & 1)) continue;
+            const int bx = c_blk_x[k], by = c_blk_y[k];
+            const int na = bx ? tc[by][bx - 1] : left ? left_tc[by] : -1, nb = by ? tc[by - 1][bx] : -1;
+            tc[by][bx] = idr ? residual_block(bw, R->lv[k] + 1, 15, nc_of(na, nb)) : residual_block(bw, R->lv[k], 16, nc_of(na, nb));
+        }
+        int cc[2][2][2] = {};
+        if (cbp_c) {
+            residual_block(bw, R->lv[17], 4, -1);
+            residual_block(bw, R->lv[17] + 4, 4, -1);
+        }
+        if (cbp_c == 2) {
+            for (int comp = 0; comp < 2; ++comp)
+                for (int k = 0; k < 4; ++k) {
+                    const int bx = k & 1, by = k >> 1;
+                    const int na = bx ? cc[comp][by][0] : left ? left_cc[comp][by] : -1, nb = by ? cc[comp][0][bx] : -1;
+                    cc[comp][by][bx] = residual_block(bw, R->lv[18 + 4 * comp + k] + 1, 15, nc_of(na, nb));
+                }
+        }
+        for (int i = 0; i < 4; ++i) left_tc[i] = tc[i][3];
+        for (int comp = 0; comp < 2; ++comp) { left_cc[comp][0] = cc[comp][0][1]; left_cc[comp][1] = cc[comp][1][1]; }
+    }
+    if (skip_run) bw.ue(skip_run);
+    bw.trailing();
+    const int64_t nal = 1 + bw.pos;
+    if (bw.overflow || nal + 4 > F.slot_cap) {
+        F.lens[row] = -1;
+        return;
+    }
+    slot[0] = (uint8_t)(nal >> 24); slot[1] = (uint8_t)(nal >> 16); slot[2] = (uint8_t)(nal >> 8); slot[3] = (uint8_t)nal;
+    slot[4] = idr ? 0x65 : 0x61;             // nal_ref_idc 3, IDR slice / non-IDR slice
+    F.lens[row] = (int32_t)(nal + 4);
+}
+
+// One block per row: offset = sum of the lengths of the rows above, then copy the slot.  The last row writes the sample length
+// (-1 when any slot overflowed).
+__global__ void __launch_bounds__(256) h264_pack(Frame F, uint8_t* sample, int64_t* sample_len) {
+    __shared__ long long s_sum[8];
+    __shared__ int s_bad[8];
+    const int row = blockIdx.x, tid = threadIdx.x;
+    long long off = 0;
+    int bad = 0;
+    for (int r = tid; r <= row; r += 256) {
+        const int l = F.lens[r];
+        if (l < 0) bad = 1;
+        if (r < row) off += l;
+    }
+    for (int o = 16; o; o >>= 1) { off += __shfl_xor_sync(0xffffffffu, off, o); bad |= __shfl_xor_sync(0xffffffffu, bad, o); }
+    if ((tid & 31) == 0) { s_sum[tid >> 5] = off; s_bad[tid >> 5] = bad; }
+    __syncthreads();
+    off = 0;
+    bad = 0;
+    for (int i = 0; i < 8; ++i) { off += s_sum[i]; bad |= s_bad[i]; }
+    if (bad) {
+        if (row == F.mbh - 1 && tid == 0) *sample_len = -1;
+        return;
+    }
+    const int len = F.lens[row];
+    const uint8_t* src = F.slots + row * F.slot_cap;
+    for (int i = tid; i < len; i += 256) sample[off + i] = src[i];
+    if (row == F.mbh - 1 && tid == 0) *sample_len = off + len;
+}
+
+int sizes(int width, int height, int64_t* plane_bytes, int64_t* scratch_bytes, int64_t* slot_cap, int64_t* slice_bytes) {
+    N3D_CHECK_ARG(width > 0 && height > 0 && width % 2 == 0 && height % 2 == 0,
+                  "n3d_h264: frame size %dx%d: 4:2:0 needs even, positive dimensions", width, height);
+    const int64_t mbw = (width + 15) / 16, mbh = (height + 15) / 16;
+    N3D_CHECK_ARG(mbw * mbh <= kMaxFs && mbw * mbw <= 8 * kMaxFs && mbh * mbh <= 8 * kMaxFs,
+                  "n3d_h264: frame size %dx%d exceeds H.264 level 6.2 (%d macroblocks, at most %d per side)", width, height, kMaxFs, 1055);
+    *plane_bytes = 256 * mbw * mbh * 3 / 2;
+    *scratch_bytes = (int64_t)sizeof(MbRec) * mbw * mbh + 4 * mbh;
+    // slot: 4-byte length, NAL header, escaped RBSP: slice header (<= 128 bits), MBs, trailing skip run and bits (<= 32 bits);
+    // emulation prevention adds at most one byte per two
+    const int64_t rbsp = (mbw * kMbBits + 128 + 32 + 7) / 8;
+    *slot_cap = (5 + rbsp + rbsp / 2 + 1 + 15) / 16 * 16;
+    *slice_bytes = *slot_cap * mbh;
+    return N3D_OK;
+}
+
+}  // namespace
+
+extern "C" int n3d_h264_buffer_sizes(int width, int height, int64_t* plane_bytes, int64_t* scratch_bytes, int64_t* slice_bytes,
+                                     int64_t* sample_bytes) {
+    N3D_CHECK_ARG(plane_bytes && scratch_bytes && slice_bytes && sample_bytes, "n3d_h264_buffer_sizes: null output pointer");
+    int64_t cap;
+    const int rc = sizes(width, height, plane_bytes, scratch_bytes, &cap, slice_bytes);
+    if (rc != N3D_OK) return rc;
+    *sample_bytes = *slice_bytes;
+    return N3D_OK;
+}
+
+extern "C" int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp, int idr, int frame_num, int idr_pic_id, uint8_t* cur,
+                               const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
+                               void* stream) {
+    N3D_CHECK_ARG(rgb && cur && recon && scratch && slices && sample && sample_len, "n3d_h264_encode: null buffer");
+    N3D_CHECK_ARG(idr || ref, "n3d_h264_encode: a P frame needs the reference reconstruction (null ref)");
+    N3D_CHECK_ARG(ref != recon, "n3d_h264_encode: ref and recon must be different buffers");
+    N3D_CHECK_ARG(qp >= 0 && qp <= 51, "n3d_h264_encode: qp %d outside 0..51", qp);
+    N3D_CHECK_ARG(frame_num >= 0 && frame_num < 16 && idr_pic_id >= 0 && idr_pic_id <= 65535,
+                  "n3d_h264_encode: frame_num %d (0..15) or idr_pic_id %d (0..65535) out of range", frame_num, idr_pic_id);
+    int64_t plane_bytes, scratch_bytes, slot_cap, slice_bytes;
+    const int rc = sizes(width, height, &plane_bytes, &scratch_bytes, &slot_cap, &slice_bytes);
+    if (rc != N3D_OK) return rc;
+    Frame F;
+    F.W = width; F.H = height;
+    F.mbw = (width + 15) / 16; F.mbh = (height + 15) / 16;
+    F.W16 = 16 * F.mbw; F.H16 = 16 * F.mbh;
+    F.qp = qp;
+    static const int qpc[52] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29,
+                                29, 30, 31, 32, 32, 33, 34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39};
+    F.qpc = qpc[qp];
+    F.rgb = rgb; F.cur = cur; F.ref = ref; F.rec = recon;
+    F.mbs = (MbRec*)scratch;
+    F.lens = (int32_t*)((uint8_t*)scratch + (int64_t)sizeof(MbRec) * F.mbw * F.mbh);
+    F.slots = slices; F.slot_cap = slot_cap;
+    F.idr = idr ? 1 : 0; F.frame_num = frame_num; F.idr_pic_id = idr_pic_id;
+    cudaStream_t s = (cudaStream_t)stream;
+    h264_rgb_to_yuv<<<n3d_grid((int64_t)F.W16 * F.H16 / 4, 256), 256, 0, s>>>(F);
+    if (F.idr) h264_intra_rows<<<F.mbh, 32, 0, s>>>(F);
+    else h264_inter_mbs<<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
+    h264_write_rows<<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
+    h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
+    N3D_CHECK_LAUNCH("n3d_h264_encode");
+    return N3D_OK;
+}

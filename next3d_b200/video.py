@@ -1,0 +1,264 @@
+"""H.264 video on the device: `H264Writer` encodes uint8 RGB frames with the sm_90a encoder of csrc/h264.cu and writes an MP4
+(next3d_b200.mp4).  The stream is Constrained Baseline (profile 66): 4:2:0 BT.601 limited range, CAVLC, a constant QP, one slice
+per macroblock row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip with integer-pel motion, no deblocking
+(DESIGN.md section 3.5).  This module also writes the SPS and PPS, for the encoder and its numpy restatement alike; the slice
+headers are written by the kernels."""
+import fractions
+
+import numpy as np
+import torch
+
+from . import _lib, mp4
+
+# Table A-1: level_idc, MaxMBPS, MaxFS (macroblocks).  Level 1b needs constraint_set3 and is skipped.
+LEVELS = [(10, 1485, 99), (11, 3000, 396), (12, 6000, 396), (13, 11880, 396), (20, 11880, 396), (21, 19800, 792),
+          (22, 20250, 1620), (30, 40500, 1620), (31, 108000, 3600), (32, 216000, 5120), (40, 245760, 8192), (41, 245760, 8192),
+          (42, 522240, 8704), (50, 589824, 22080), (51, 983040, 36864), (52, 2073600, 36864), (60, 4177920, 139264),
+          (61, 8355840, 139264), (62, 16711680, 139264)]
+
+
+def level_idc(width, height, fps):
+    """Smallest level whose MaxFS, MaxMBPS and frame-dimension limits (width, height <= sqrt(8 * MaxFS) macroblocks) fit."""
+    mbw, mbh = (width + 15) // 16, (height + 15) // 16
+    for lev, mbps, fs in LEVELS:
+        if mbw * mbh <= fs and mbw * mbw <= 8 * fs and mbh * mbh <= 8 * fs and mbw * mbh * fps <= mbps:
+            return lev
+    raise ValueError(f'{width}x{height} at {fps} frames/s exceeds H.264 level 6.2')
+
+
+class _Bits:
+    def __init__(self):
+        self.s = []
+
+    def u(self, v, n):
+        self.s.append(format(int(v), f'0{n}b'))
+
+    def ue(self, k):
+        n = (k + 1).bit_length()
+        self.s.append('0' * (n - 1))
+        self.u(k + 1, n)
+
+    def se(self, v):
+        self.ue(2 * v - 1 if v > 0 else -2 * v)
+
+    def nal(self, header):
+        s = ''.join(self.s) + '1'
+        s += '0' * (-len(s) % 8)
+        rbsp = int(s, 2).to_bytes(len(s) // 8, 'big')
+        out, zeros = bytearray([header]), 0
+        for b in rbsp:                                   # emulation prevention
+            if zeros >= 2 and b <= 3:
+                out.append(3)
+                zeros = 0
+            out.append(b)
+            zeros = zeros + 1 if b == 0 else 0
+        return bytes(out)
+
+
+def _fps_fraction(fps):
+    f = fractions.Fraction(fps).limit_denominator(1001)
+    if f <= 0:
+        raise ValueError(f'fps must be positive, got {fps}')
+    return f
+
+
+def sps(width, height, fps):
+    """Sequence parameter set NAL unit (no start code)."""
+    mbw, mbh = (width + 15) // 16, (height + 15) // 16
+    f = _fps_fraction(fps)
+    b = _Bits()
+    b.u(66, 8)                                       # profile_idc: Baseline
+    b.u(0b11000000, 8)                               # constraint_set0/1: Constrained Baseline
+    b.u(level_idc(width, height, float(f)), 8)
+    b.ue(0)                                          # seq_parameter_set_id
+    b.ue(0)                                          # log2_max_frame_num_minus4: frame_num is 4 bits
+    b.ue(2)                                          # pic_order_cnt_type 2: output order = decoding order
+    b.ue(1)                                          # max_num_ref_frames
+    b.u(0, 1)                                        # gaps_in_frame_num_value_allowed_flag
+    b.ue(mbw - 1)
+    b.ue(mbh - 1)
+    b.u(1, 1)                                        # frame_mbs_only_flag
+    b.u(1, 1)                                        # direct_8x8_inference_flag
+    crop = (mbw * 16 != width) or (mbh * 16 != height)
+    b.u(crop, 1)
+    if crop:                                         # in units of 2 samples (4:2:0, frames)
+        b.ue(0)
+        b.ue((mbw * 16 - width) // 2)
+        b.ue(0)
+        b.ue((mbh * 16 - height) // 2)
+    b.u(1, 1)                                        # vui_parameters_present_flag
+    b.u(0, 1)                                        # aspect_ratio_info_present_flag
+    b.u(0, 1)                                        # overscan_info_present_flag
+    b.u(1, 1)                                        # video_signal_type_present_flag
+    b.u(5, 3)                                        # video_format: unspecified
+    b.u(0, 1)                                        # video_full_range_flag: limited range
+    b.u(1, 1)                                        # colour_description_present_flag
+    b.u(6, 8)                                        # colour_primaries: SMPTE 170M
+    b.u(6, 8)                                        # transfer_characteristics: SMPTE 170M
+    b.u(6, 8)                                        # matrix_coefficients: BT.601
+    b.u(0, 1)                                        # chroma_loc_info_present_flag
+    b.u(1, 1)                                        # timing_info_present_flag
+    b.u(f.denominator, 32)                           # num_units_in_tick
+    b.u(2 * f.numerator, 32)                         # time_scale: two ticks per frame
+    b.u(1, 1)                                        # fixed_frame_rate_flag
+    b.u(0, 1)                                        # nal_hrd_parameters_present_flag
+    b.u(0, 1)                                        # vcl_hrd_parameters_present_flag
+    b.u(0, 1)                                        # pic_struct_present_flag
+    b.u(1, 1)                                        # bitstream_restriction_flag
+    b.u(1, 1)                                        # motion_vectors_over_pic_boundaries_flag
+    b.ue(0)                                          # max_bytes_per_pic_denom: no limit
+    b.ue(0)                                          # max_bits_per_mb_denom: no limit
+    b.ue(16)                                         # log2_max_mv_length_horizontal
+    b.ue(16)                                         # log2_max_mv_length_vertical
+    b.ue(0)                                          # max_num_reorder_frames
+    b.ue(1)                                          # max_dec_frame_buffering
+    return b.nal(0x67)
+
+
+def pps(qp):
+    """Picture parameter set NAL unit: CAVLC, pic_init_qp = qp, deblocking control present (the slices disable it)."""
+    b = _Bits()
+    b.ue(0)                                          # pic_parameter_set_id
+    b.ue(0)                                          # seq_parameter_set_id
+    b.u(0, 1)                                        # entropy_coding_mode_flag: CAVLC
+    b.u(0, 1)                                        # bottom_field_pic_order_in_frame_present_flag
+    b.ue(0)                                          # num_slice_groups_minus1
+    b.ue(0)                                          # num_ref_idx_l0_default_active_minus1
+    b.ue(0)                                          # num_ref_idx_l1_default_active_minus1
+    b.u(0, 1)                                        # weighted_pred_flag
+    b.u(0, 2)                                        # weighted_bipred_idc
+    b.se(qp - 26)                                    # pic_init_qp_minus26
+    b.se(0)                                          # pic_init_qs_minus26
+    b.se(0)                                          # chroma_qp_index_offset
+    b.u(1, 1)                                        # deblocking_filter_control_present_flag
+    b.u(0, 1)                                        # constrained_intra_pred_flag
+    b.u(0, 1)                                        # redundant_pic_cnt_present_flag
+    return b.nal(0x68)
+
+
+def check_args(width, height, fps, qp, gop):
+    if width <= 0 or height <= 0 or width % 2 or height % 2:
+        raise ValueError(f'4:2:0 needs even, positive frame dimensions, got {width}x{height}')
+    if not 0 <= qp <= 51:
+        raise ValueError(f'qp must be in 0..51, got {qp}')
+    if gop < 1:
+        raise ValueError(f'gop must be at least 1, got {gop}')
+    level_idc(width, height, float(_fps_fraction(fps)))
+
+
+class H264Writer:
+    """Encode uint8 RGB frames [H, W, 3] (numpy arrays or CUDA tensors, one frame or a batch [N, H, W, 3]) into an MP4 file at
+    `path`, in order, on a stream of the writer's own.  qp: constant quantiser 0..51 (lower = larger file, closer to the input);
+    gop: an IDR frame every `gop` frames.  CUDA frames are read in place; numpy frames are copied to the device.  The encoded
+    frames reach the host every `batch` frames in one pinned copy.  Use as a context manager, or call close()."""
+
+    def __init__(self, path, width, height, fps, qp=18, gop=60, device=None, batch=8):
+        check_args(width, height, fps, qp, gop)
+        self.width, self.height, self.qp, self.gop = int(width), int(height), int(qp), int(gop)
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != 'cuda':
+            raise ValueError('H264Writer encodes on a CUDA device')
+        sizes = [_lib.I64() for _ in range(4)]
+        _lib.check(_lib.lib.n3d_h264_buffer_sizes(self.width, self.height, *[_lib.C.byref(s) for s in sizes]), 'n3d_h264_buffer_sizes')
+        self.plane_bytes, scratch_bytes, slice_bytes, self.sample_cap = (s.value for s in sizes)
+        mbw, mbh = (self.width + 15) // 16, (self.height + 15) // 16
+        self._shape = (16 * mbh, 16 * mbw)
+        self.stream = torch.cuda.Stream(self.device)
+        self.batch = max(1, min(int(batch), (1 << 29) // self.sample_cap))          # at most 512 MB of pending samples
+        with torch.cuda.device(self.device):
+            new = lambda n: torch.empty(n, dtype=torch.uint8, device=self.device)
+            self._cur, self._planes = new(self.plane_bytes), [new(self.plane_bytes), new(self.plane_bytes)]
+            self._scratch, self._slices = new(scratch_bytes), new(slice_bytes)
+            self._samples = new(self.batch * self.sample_cap)
+            self._lens = torch.zeros(self.batch, dtype=torch.int64, device=self.device)
+        self._lens_host = torch.empty(self.batch, dtype=torch.int64, pin_memory=True)
+        self._host = torch.empty(0, dtype=torch.uint8)
+        self._pending = []                                   # IDR flag of each frame encoded since the last flush
+        self.frames = 0
+        self._mp4 = mp4.Mp4Writer(path, self.width, self.height, _fps_fraction(fps), sps(self.width, self.height, fps), pps(self.qp))
+
+    def write(self, frames):
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(np.ascontiguousarray(frames))
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise TypeError('frames must be uint8 numpy arrays or tensors')
+        if frames.dim() == 3:
+            frames = frames[None]
+        if tuple(frames.shape[1:]) != (self.height, self.width, 3):
+            raise ValueError(f'expected frames of shape [N, {self.height}, {self.width}, 3], got {list(frames.shape)}')
+        producer = torch.cuda.current_stream(self.device)
+        with torch.cuda.stream(self.stream):
+            if frames.device != self.device:
+                frames = frames.to(self.device)                   # numpy / host frames: copied on the writer's stream
+            else:
+                self.stream.wait_stream(producer)                 # CUDA frames: read in place once their producer is done
+                frames.record_stream(self.stream)
+            frames = frames.contiguous()
+            for i in range(frames.shape[0]):
+                self._encode(frames[i])
+
+    def _encode(self, frame):
+        k = self.frames % self.gop
+        slot = len(self._pending)
+        ref, rec = self._planes[self.frames % 2], self._planes[(self.frames + 1) % 2]
+        _lib.check(_lib.lib.n3d_h264_encode(
+            frame.data_ptr(), self.width, self.height, self.qp, int(k == 0), k % 16, (self.frames // self.gop) % 2,
+            self._cur.data_ptr(), None if k == 0 else ref.data_ptr(), rec.data_ptr(), self._scratch.data_ptr(),
+            self._slices.data_ptr(), self._samples[slot * self.sample_cap:].data_ptr(), self._lens[slot:].data_ptr(),
+            self.stream.cuda_stream), 'n3d_h264_encode')
+        self._pending.append(k == 0)
+        self.frames += 1
+        if len(self._pending) == self.batch:
+            self._flush()
+
+    def _flush(self):
+        n = len(self._pending)
+        if n == 0:
+            return
+        with torch.cuda.stream(self.stream):
+            self._lens_host[:n].copy_(self._lens[:n], non_blocking=True)
+            self.stream.synchronize()
+            lens = self._lens_host[:n].tolist()
+            if min(lens) < 0:
+                raise RuntimeError('n3d_h264_encode: a slice exceeded its bitstream capacity')
+            if self._host.numel() < sum(lens):
+                self._host = torch.empty(max(sum(lens), 2 * self._host.numel()), dtype=torch.uint8, pin_memory=True)
+            o = 0
+            for i, ln in enumerate(lens):
+                self._host[o:o + ln].copy_(self._samples[i * self.sample_cap:i * self.sample_cap + ln], non_blocking=True)
+                o += ln
+            self.stream.synchronize()
+        data = self._host[:o].numpy().tobytes()
+        o = 0
+        for ln, idr in zip(lens, self._pending):
+            self._mp4.add(data[o:o + ln], idr)
+            o += ln
+        self._pending = []
+
+    @property
+    def recon(self):
+        """Reconstruction of the last frame, as the decoder outputs it before cropping: padded (Y [H16, W16], Cb, Cr
+        [H16/2, W16/2]) uint8 CUDA tensors (copies)."""
+        if self.frames == 0:
+            return None
+        self.stream.synchronize()
+        p = self._planes[self.frames % 2]
+        H16, W16 = self._shape
+        n = H16 * W16
+        return (p[:n].view(H16, W16).clone(), p[n:n + n // 4].view(H16 // 2, W16 // 2).clone(),
+                p[n + n // 4:n + n // 2].view(H16 // 2, W16 // 2).clone())
+
+    def close(self):
+        if self._mp4 is None:
+            return
+        try:
+            self._flush()
+        finally:
+            self._mp4.close()
+            self._mp4 = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()

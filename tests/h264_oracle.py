@@ -1,0 +1,552 @@
+"""numpy restatement of the sm_90a H.264 encoder (next3d_b200/csrc/h264.cu): the same colour conversion, mode and motion
+decisions, tie-breaks, quantisation and CAVLC, producing the same bytes and the same reconstruction.  Test infrastructure only:
+the CPU tests decode its streams with FFmpeg to prove the byte format, and the GPU tests compare the kernels with it byte for
+byte.  The parameter sets (SPS / PPS) come from next3d_b200.video, which writes them for both encoders.
+
+Stream subset (see DESIGN.md section 3.5): Constrained Baseline, one slice per macroblock row, IDR frames of I_16x16 macroblocks
+(DC or horizontal luma prediction, DC chroma), P frames of P_L0_16x16 / P_Skip with integer-pel motion, constant QP, no
+deblocking."""
+import re
+
+import numpy as np
+
+SEARCH = 16                     # integer-pel full search over [-SEARCH, SEARCH]^2 (csrc/h264.cu kSearch)
+LEVEL_MAX = 2063                # largest |level| CAVLC codes with level_prefix <= 15 at every suffixLength (Baseline)
+
+LAMBDA = [0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 5, 5, 6, 7, 7, 8, 9, 10, 12, 13, 15,
+          17, 19, 21, 23, 26, 30, 33, 37, 42, 47, 53, 59, 66, 74, 83]
+QPC = list(range(30)) + [29, 30, 31, 32, 32, 33, 34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39]
+MF = [[13107, 5243, 8066], [11916, 4660, 7490], [10082, 4194, 6554], [9362, 3647, 5825], [8192, 3355, 5243], [7282, 2893, 4559]]
+V = [[10, 16, 13], [11, 18, 14], [13, 20, 16], [14, 23, 18], [16, 25, 20], [18, 29, 23]]
+ZZ = [0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15]               # frame zig-zag scan -> raster index in a 4x4 block
+BLK = [(0, 0), (1, 0), (0, 1), (1, 1), (2, 0), (3, 0), (2, 1), (3, 1),   # luma4x4BlkIdx -> (x, y) in 4x4 units
+       (0, 2), (1, 2), (0, 3), (1, 3), (2, 2), (3, 2), (2, 3), (3, 3)]
+INTER_CBP = [0, 16, 1, 2, 4, 8, 32, 3, 5, 10, 12, 15, 47, 7, 11, 13, 14, 6, 9, 31, 35, 37, 42, 44, 33, 34, 36, 40, 39, 43, 45, 46,
+             17, 18, 20, 24, 19, 21, 26, 28, 23, 27, 29, 30, 22, 25, 38, 41]          # me(v) codeNum -> inter coded_block_pattern
+CBP_CODE = {c: k for k, c in enumerate(INTER_CBP)}
+
+# coeff_token (Table 9-5), index 4 * TotalCoeff + TrailingOnes, for 0 <= nC < 2, 2 <= nC < 4, 4 <= nC < 8, 8 <= nC
+CT_LEN = [
+    [1, 0, 0, 0, 6, 2, 0, 0, 8, 6, 3, 0, 9, 8, 7, 5, 10, 9, 8, 6, 11, 10, 9, 7, 13, 11, 10, 8, 13, 13, 11, 9, 13, 13, 13, 10,
+     14, 14, 13, 11, 14, 14, 14, 13, 15, 15, 14, 14, 15, 15, 15, 14, 16, 15, 15, 15, 16, 16, 16, 15, 16, 16, 16, 16, 16, 16, 16, 16],
+    [2, 0, 0, 0, 6, 2, 0, 0, 6, 5, 3, 0, 7, 6, 6, 4, 8, 6, 6, 4, 8, 7, 7, 5, 9, 8, 8, 6, 11, 9, 9, 6, 11, 11, 11, 7,
+     12, 11, 11, 9, 12, 12, 12, 11, 12, 12, 12, 11, 13, 13, 13, 12, 13, 13, 13, 13, 13, 14, 13, 13, 14, 14, 14, 13, 14, 14, 14, 14],
+    [4, 0, 0, 0, 6, 4, 0, 0, 6, 5, 4, 0, 6, 5, 5, 4, 7, 5, 5, 4, 7, 5, 5, 4, 7, 6, 6, 4, 7, 6, 6, 4, 8, 7, 7, 5,
+     8, 8, 7, 6, 9, 8, 8, 7, 9, 9, 8, 8, 9, 9, 9, 8, 10, 9, 9, 9, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10, 10],
+    [6, 0, 0, 0] + [6] * 64,
+]
+CT_BITS = [
+    [1, 0, 0, 0, 5, 1, 0, 0, 7, 4, 1, 0, 7, 6, 5, 3, 7, 6, 5, 3, 7, 6, 5, 4, 15, 6, 5, 4, 11, 14, 5, 4, 8, 10, 13, 4,
+     15, 14, 9, 4, 11, 10, 13, 12, 15, 14, 9, 12, 11, 10, 13, 8, 15, 1, 9, 12, 11, 14, 13, 8, 7, 10, 9, 12, 4, 6, 5, 8],
+    [3, 0, 0, 0, 11, 2, 0, 0, 7, 7, 3, 0, 7, 10, 9, 5, 7, 6, 5, 4, 4, 6, 5, 6, 7, 6, 5, 8, 15, 6, 5, 4, 11, 14, 13, 4,
+     15, 10, 9, 4, 11, 14, 13, 12, 8, 10, 9, 8, 15, 14, 13, 12, 11, 10, 9, 12, 7, 11, 6, 8, 9, 8, 10, 1, 7, 6, 5, 4],
+    [15, 0, 0, 0, 15, 14, 0, 0, 11, 15, 13, 0, 8, 12, 14, 12, 15, 10, 11, 11, 11, 8, 9, 10, 9, 14, 13, 9, 8, 10, 9, 8,
+     15, 14, 13, 13, 11, 14, 10, 12, 15, 10, 13, 12, 11, 14, 9, 12, 8, 10, 13, 8, 13, 7, 9, 12, 9, 12, 11, 10, 5, 8, 7, 6,
+     1, 4, 3, 2],
+    [3, 0, 0, 0, 0, 1, 0, 0, 4, 5, 6, 0] + list(range(8, 64)),
+]
+CDC_CT_LEN = [2, 0, 0, 0, 6, 1, 0, 0, 6, 6, 3, 0, 6, 7, 7, 6, 6, 8, 8, 7]            # chroma DC (nC = -1)
+CDC_CT_BITS = [1, 0, 0, 0, 7, 1, 0, 0, 4, 6, 1, 0, 3, 3, 2, 5, 2, 3, 2, 0]
+TZ_LEN = [[1, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 9], [3, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 6, 6, 6, 6], [4, 3, 3, 3, 4, 4, 3, 3, 4, 5, 5, 6, 5, 6],
+          [5, 3, 4, 4, 3, 3, 3, 4, 3, 4, 5, 5, 5], [4, 4, 4, 3, 3, 3, 3, 3, 4, 5, 4, 5], [6, 5, 3, 3, 3, 3, 3, 3, 4, 3, 6],
+          [6, 5, 3, 3, 3, 2, 3, 4, 3, 6], [6, 4, 5, 3, 2, 2, 3, 3, 6], [6, 6, 4, 2, 2, 3, 2, 5], [5, 5, 3, 2, 2, 2, 4], [4, 4, 3, 3, 1, 3],
+          [4, 4, 2, 1, 3], [3, 3, 1, 2], [2, 2, 1], [1, 1]]
+TZ_BITS = [[1, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 3, 2, 1], [7, 6, 5, 4, 3, 5, 4, 3, 2, 3, 2, 3, 2, 1, 0], [5, 7, 6, 5, 4, 3, 4, 3, 2, 3, 2, 1, 1, 0],
+           [3, 7, 5, 4, 6, 5, 4, 3, 3, 2, 2, 1, 0], [5, 4, 3, 7, 6, 5, 4, 3, 2, 1, 1, 0], [1, 1, 7, 6, 5, 4, 3, 2, 1, 1, 0],
+           [1, 1, 5, 4, 3, 3, 2, 1, 1, 0], [1, 1, 1, 3, 3, 2, 2, 1, 0], [1, 0, 1, 3, 2, 1, 1, 1], [1, 0, 1, 3, 2, 1, 1], [0, 1, 1, 2, 1, 3],
+           [0, 1, 1, 1, 1], [0, 1, 1, 1], [0, 1, 1], [0, 1]]
+CDC_TZ_LEN = [[1, 2, 3, 3], [1, 2, 2], [1, 1]]
+CDC_TZ_BITS = [[1, 1, 1, 0], [1, 1, 0], [1, 0]]
+RUN_LEN = [[1, 1], [1, 2, 2], [2, 2, 2, 2], [2, 2, 2, 3, 3], [2, 2, 3, 3, 3, 3], [2, 3, 3, 3, 3, 3, 3],
+           [3, 3, 3, 3, 3, 3, 3, 4, 5, 6, 7, 8, 9, 10, 11]]
+RUN_BITS = [[1, 0], [1, 1, 0], [3, 2, 1, 0], [3, 2, 1, 1, 0], [3, 2, 3, 2, 1, 0], [3, 0, 1, 3, 2, 5, 4],
+            [7, 6, 5, 4, 3, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1]]
+
+CF = np.array([[1, 1, 1, 1], [2, 1, -1, -2], [1, -1, -1, 1], [1, -2, 2, -1]], np.int64)
+HAD = np.array([[1, 1, 1, 1], [1, 1, -1, -1], [1, -1, -1, 1], [1, -1, 1, -1]], np.int64)
+A2 = np.array([[1, 1], [1, -1]], np.int64)
+
+
+def _cls4():
+    c = np.full((4, 4), 2)
+    c[0::2, 0::2] = 0
+    c[1::2, 1::2] = 1
+    return c
+
+
+CLS = _cls4()
+MF4 = np.array([np.array(m)[CLS] for m in MF], np.int64)        # [qp % 6, 4, 4]
+LS4 = np.array([16 * np.array(v)[CLS] for v in V], np.int64)    # LevelScale4x4 with flat weights
+
+
+# ------------------------------------------------------------------------------------------------ colour conversion
+def rgb_to_yuv420(rgb):
+    """uint8 RGB [H, W, 3] (H, W even) -> padded Y [H16, W16], Cb, Cr [H16/2, W16/2] uint8, BT.601 limited range in integers;
+    the padding repeats the last row / column of each plane."""
+    H, W, _ = rgb.shape
+    x = rgb.astype(np.int64)
+    R, G, B = x[..., 0], x[..., 1], x[..., 2]
+    y = ((66 * R + 129 * G + 25 * B + 128) >> 8) + 16
+    s = lambda p: p[0::2, 0::2] + p[1::2, 0::2] + p[0::2, 1::2] + p[1::2, 1::2]
+    sR, sG, sB = s(R), s(G), s(B)
+    cb = ((-38 * sR - 74 * sG + 112 * sB + 512) >> 10) + 128
+    cr = ((112 * sR - 94 * sG - 18 * sB + 512) >> 10) + 128
+    H16, W16 = (H + 15) // 16 * 16, (W + 15) // 16 * 16
+    pad = lambda p, h, w: np.pad(p, ((0, h - p.shape[0]), (0, w - p.shape[1])), mode='edge').astype(np.uint8)
+    return pad(y, H16, W16), pad(cb, H16 // 2, W16 // 2), pad(cr, H16 // 2, W16 // 2)
+
+
+# ------------------------------------------------------------------------------------------------ transforms and quantisation
+def fwd4(x):
+    return CF @ x @ CF.T
+
+
+def inv4(d):
+    """8.5.12.2 on [..., 4, 4] scaled coefficients, then (x + 32) >> 6."""
+    d = d.astype(np.int64)
+
+    def one(a):                               # 1-D inverse along the last axis
+        e0, e1 = a[..., 0] + a[..., 2], a[..., 0] - a[..., 2]
+        e2, e3 = (a[..., 1] >> 1) - a[..., 3], a[..., 1] + (a[..., 3] >> 1)
+        return np.stack([e0 + e3, e1 + e2, e1 - e2, e0 - e3], -1)
+    f = one(d)
+    h = np.swapaxes(one(np.swapaxes(f, -1, -2)), -1, -2)
+    return (h + 32) >> 6
+
+
+def quant(w, qp, intra, dc_shift=0, mf=None):
+    qbits = 15 + qp // 6 + dc_shift
+    f = ((1 << (15 + qp // 6)) // (3 if intra else 6)) << dc_shift
+    mf = MF4[qp % 6] if mf is None else mf
+    lv = (np.abs(w) * mf + f) >> qbits
+    return (np.sign(w) * np.minimum(lv, LEVEL_MAX)).astype(np.int64)
+
+
+def dequant(c, qp):
+    ls = LS4[qp % 6]
+    if qp >= 24:
+        return (c * ls) << (qp // 6 - 4)
+    return (c * ls + (1 << (3 - qp // 6))) >> (4 - qp // 6)
+
+
+def blocks(mb):
+    """[..., 16, 16] macroblock -> [..., 16, 4, 4] in luma4x4BlkIdx order."""
+    return np.stack([mb[..., 4 * by:4 * by + 4, 4 * bx:4 * bx + 4] for bx, by in BLK], -3)
+
+
+def unblocks(b):
+    out = np.zeros(b.shape[:-3] + (16, 16), b.dtype)
+    for k, (bx, by) in enumerate(BLK):
+        out[..., 4 * by:4 * by + 4, 4 * bx:4 * bx + 4] = b[..., k, :, :]
+    return out
+
+
+def cblocks(mb):
+    """[..., 8, 8] chroma macroblock -> [..., 4, 4, 4] in raster block order."""
+    return np.stack([mb[..., 4 * by:4 * by + 4, 4 * bx:4 * bx + 4] for by in range(2) for bx in range(2)], -3)
+
+
+def uncblocks(b):
+    out = np.zeros(b.shape[:-3] + (8, 8), b.dtype)
+    for k in range(4):
+        by, bx = divmod(k, 2)
+        out[..., 4 * by:4 * by + 4, 4 * bx:4 * bx + 4] = b[..., k, :, :]
+    return out
+
+
+def scan(b):
+    """[..., 4, 4] -> [..., 16] in zig-zag order."""
+    return b.reshape(b.shape[:-2] + (16,))[..., ZZ]
+
+
+def code_chroma(src, pred, qpc, intra):
+    """One chroma component of a batch of macroblocks: src, pred [..., 8, 8] -> (DC levels [..., 4], AC levels [..., 4, 16] in
+    zig-zag order (index 0 unused), reconstruction [..., 8, 8])."""
+    w = fwd4(cblocks(src.astype(np.int64) - pred))
+    dc = w[..., 0, 0]
+    t = np.einsum('ij,...jk,kl->...il', A2, dc.reshape(dc.shape[:-1] + (2, 2)), A2)
+    dcl = quant(t, qpc, intra, 1, MF4[qpc % 6][0, 0]).reshape(dc.shape)
+    acl = quant(w, qpc, intra)
+    acl[..., 0, 0] = 0
+    f = np.einsum('ij,...jk,kl->...il', A2, dcl.reshape(dcl.shape[:-1] + (2, 2)), A2)
+    dcc = ((f * LS4[qpc % 6][0, 0]) << (qpc // 6)) >> 5
+    d = dequant(acl, qpc)
+    d[..., 0, 0] = dcc.reshape(dc.shape)
+    rec = np.clip(pred + uncblocks(inv4(d)), 0, 255)
+    return dcl, scan(acl), rec
+
+
+# ------------------------------------------------------------------------------------------------ bit writing
+def ue_bits(k):
+    return 2 * (int(k) + 1).bit_length() - 1
+
+
+def se_code(v):
+    return 2 * v - 1 if v > 0 else -2 * v
+
+
+class Bits:
+    def __init__(self):
+        self.parts = []
+
+    def u(self, v, n):
+        if n:
+            self.parts.append(format(int(v), f'0{n}b'))
+
+    def ue(self, k):
+        n = (int(k) + 1).bit_length()
+        self.u(0, n - 1)
+        self.u(k + 1, n)
+
+    def se(self, v):
+        self.ue(se_code(int(v)))
+
+    def rbsp(self):
+        """Bits + rbsp_trailing_bits -> bytes."""
+        s = ''.join(self.parts) + '1'
+        s += '0' * (-len(s) % 8)
+        return int(s, 2).to_bytes(len(s) // 8, 'big')
+
+
+def escape(rbsp):
+    """Emulation prevention: 0x000003 before any 0x0000xx with xx <= 3."""
+    return re.sub(b'\x00\x00(?=[\x00-\x03])', b'\x00\x00\x03', rbsp)
+
+
+def residual_block(bw, coeffs, nc):
+    """CAVLC residual_block (9.2) of coeffs (scan order, len 16, 15 or 4); nc = -1 for chroma DC.  Returns TotalCoeff."""
+    coeffs = [int(c) for c in coeffs]
+    nz = [i for i, c in enumerate(coeffs) if c]
+    total = len(nz)
+    t1 = 0
+    for i in reversed(nz):
+        if abs(coeffs[i]) != 1 or t1 == 3:
+            break
+        t1 += 1
+    idx = 4 * total + t1
+    if nc == -1:
+        bw.u(CDC_CT_BITS[idx], CDC_CT_LEN[idx])
+    else:
+        tab = 0 if nc < 2 else 1 if nc < 4 else 2 if nc < 8 else 3
+        bw.u(CT_BITS[tab][idx], CT_LEN[tab][idx])
+    if total == 0:
+        return 0
+    levels = [coeffs[i] for i in reversed(nz)]
+    for k in range(t1):
+        bw.u(1 if levels[k] < 0 else 0, 1)
+    sl = 1 if total > 10 and t1 < 3 else 0
+    for k in range(t1, total):
+        lv = levels[k]
+        code = 2 * lv - 2 if lv > 0 else -2 * lv - 1
+        if k == t1 and t1 < 3:
+            code -= 2
+        if sl == 0:
+            if code < 14:
+                prefix, sbits, sval = code, 0, 0
+            elif code < 30:
+                prefix, sbits, sval = 14, 4, code - 14
+            else:
+                prefix, sbits, sval = 15, 12, code - 30
+        elif code < (15 << sl):
+            prefix, sbits, sval = code >> sl, sl, code & ((1 << sl) - 1)
+        else:
+            prefix, sbits, sval = 15, 12, code - (15 << sl)
+        bw.u(1, prefix + 1)
+        bw.u(sval, sbits)
+        if sl == 0:
+            sl = 1
+        if abs(lv) > (3 << (sl - 1)) and sl < 6:
+            sl += 1
+    n = len(coeffs)
+    if total < n:
+        tz = nz[-1] + 1 - total
+        if nc == -1:
+            bw.u(CDC_TZ_BITS[total - 1][tz], CDC_TZ_LEN[total - 1][tz])
+        else:
+            bw.u(TZ_BITS[total - 1][tz], TZ_LEN[total - 1][tz])
+        left = tz
+        for j in range(total - 1, 0, -1):
+            if left == 0:
+                break
+            run = nz[j] - nz[j - 1] - 1
+            t = min(left, 7) - 1
+            bw.u(RUN_BITS[t][run], RUN_LEN[t][run])
+            left -= run
+    return total
+
+
+def _nc(na, nb):
+    """nC of coeff_token (9.2.1) from the left / upper block's TotalCoeff, None when that block is not available."""
+    if na is not None and nb is not None:
+        return (na + nb + 1) >> 1
+    return na if na is not None else nb if nb is not None else 0
+
+
+# ------------------------------------------------------------------------------------------------ encoder
+def _mb_view(p, s):
+    """[R*s, C*s] plane -> [R, C, s, s] macroblock view."""
+    R, C = p.shape[0] // s, p.shape[1] // s
+    return p.reshape(R, s, C, s).swapaxes(1, 2)
+
+
+class Encoder:
+    """Encodes uint8 RGB frames into length-prefixed slice NAL units, one sample per frame.  The first frame and every gop-th one
+    after it is IDR."""
+
+    def __init__(self, width, height, qp=18, gop=60):
+        if width % 2 or height % 2 or width <= 0 or height <= 0:
+            raise ValueError('4:2:0 needs even, positive frame dimensions')
+        self.W, self.H, self.qp, self.gop = width, height, qp, gop
+        self.mbw, self.mbh = (width + 15) // 16, (height + 15) // 16
+        self.n = 0
+        self.recon = None                     # (Y, Cb, Cr) padded planes of the last frame
+        self.mvs = None                       # [mbh, mbw, 2] integer-pel MVs of the last P frame
+        self.skip = None                      # [mbh, mbw] bool
+
+    # ---------------------------------------------------------------- decisions and reconstruction
+    def _intra(self, Y, U, V):
+        """I_16x16 for every MB; column by column (each MB needs its left neighbour's reconstruction), rows at once."""
+        qp, qpc = self.qp, QPC[self.qp]
+        R, C = self.mbh, self.mbw
+        yb, ub, vb = _mb_view(Y.astype(np.int64), 16), _mb_view(U.astype(np.int64), 8), _mb_view(V.astype(np.int64), 8)
+        ry, ru, rv = np.zeros_like(yb), np.zeros_like(ub), np.zeros_like(vb)
+        mbs = [[None] * C for _ in range(R)]
+        for c in range(C):
+            src = yb[:, c]
+            if c == 0:
+                pred = np.full_like(src, 128)
+                mode = np.full(R, 2)
+            else:
+                left = ry[:, c - 1, :, 15]                                     # [R, 16]
+                dcp = ((left.sum(-1) + 8) >> 4)[:, None, None] * np.ones((1, 16, 16), np.int64)
+                hp = np.repeat(left[:, :, None], 16, -1)
+                sad_h = np.abs(src - hp).sum((-1, -2))
+                sad_dc = np.abs(src - dcp).sum((-1, -2))
+                useh = sad_h <= sad_dc
+                pred = np.where(useh[:, None, None], hp, dcp)
+                mode = np.where(useh, 1, 2)
+            w = fwd4(blocks(src - pred))                                     # [R, 16, 4, 4]
+            dcm = unblocks_dc(w[..., 0, 0])                                  # [R, 4, 4] spatial
+            hd = (HAD @ dcm @ HAD) >> 1
+            dcl = quant(hd, qp, True, 1, MF4[qp % 6][0, 0])
+            acl = quant(w, qp, True)
+            acl[..., 0, 0] = 0
+            c4 = HAD @ dcl @ HAD
+            if qp >= 36:
+                dcy = (c4 * LS4[qp % 6][0, 0]) << (qp // 6 - 6)
+            else:
+                dcy = (c4 * LS4[qp % 6][0, 0] + (1 << (5 - qp // 6))) >> (6 - qp // 6)
+            d = dequant(acl, qp)
+            d[..., 0, 0] = blocks_dc(dcy)
+            ry[:, c] = np.clip(pred + unblocks(inv4(d)), 0, 255)
+            cres = []
+            for comp, (sb, rb) in enumerate(((ub, ru), (vb, rv))):
+                if c == 0:
+                    cp = np.full((R, 8, 8), 128, np.int64)
+                else:
+                    lc = rb[:, c - 1, :, 7]                                      # [R, 8]
+                    top = (lc[:, 0:4].sum(-1) + 2) >> 2
+                    bot = (lc[:, 4:8].sum(-1) + 2) >> 2
+                    cp = np.concatenate([np.repeat(top[:, None, None], 4, 1), np.repeat(bot[:, None, None], 4, 1)], 1)
+                    cp = np.repeat(cp, 8, -1)
+                dcl_c, acl_c, rec_c = code_chroma(sb[:, c], cp, qpc, True)
+                rb[:, c] = rec_c
+                cres.append((dcl_c, acl_c))
+            for r in range(R):
+                mbs[r][c] = dict(intra=True, mode=int(mode[r]), ldc=scan(dcl[r]), lac=scan(acl[r]),
+                                 cdc=[cres[0][0][r], cres[1][0][r]], cac=[cres[0][1][r], cres[1][1][r]])
+        return mbs, (ry, ru, rv)
+
+    def _inter(self, Y, U, V):
+        """P_L0_16x16 / P_Skip for every MB at once against the previous reconstruction."""
+        qp, qpc = self.qp, QPC[self.qp]
+        R, C = self.mbh, self.mbw
+        H16, W16 = 16 * R, 16 * C
+        ry, ru, rv = (p.astype(np.int64) for p in self.recon)
+        cur = Y.astype(np.int64)
+        padded = np.pad(ry, SEARCH, mode='edge')
+        lam = LAMBDA[qp]
+        best = np.full((R, C), np.iinfo(np.int64).max, np.int64)
+        for my in range(-SEARCH, SEARCH + 1):
+            for mx in range(-SEARCH, SEARCH + 1):
+                shifted = padded[SEARCH + my:SEARCH + my + H16, SEARCH + mx:SEARCH + mx + W16]
+                sad = _mb_view(np.abs(cur - shifted), 16).sum((-1, -2))
+                cost = sad + lam * (ue_bits(se_code(4 * mx)) + ue_bits(se_code(4 * my)))
+                key = (cost << 24) | ((abs(mx) + abs(my)) << 16) | ((my + SEARCH) << 8) | (mx + SEARCH)
+                np.minimum(best, key, out=best)
+        mvy = ((best >> 8) & 0xff) - SEARCH
+        mvx = (best & 0xff) - SEARCH
+        # luma prediction: integer-pel, reference coordinates clamped to the picture
+        yy = np.arange(16)[None, None, :, None] + 16 * np.arange(R)[:, None, None, None] + mvy[:, :, None, None]
+        xx = np.arange(16)[None, None, None, :] + 16 * np.arange(C)[None, :, None, None] + mvx[:, :, None, None]
+        pred = ry[np.clip(yy, 0, H16 - 1), np.clip(xx, 0, W16 - 1)]
+        src = _mb_view(cur, 16)
+        w = fwd4(blocks(src - pred))
+        lvl = quant(w, qp, False)                                             # [R, C, 16, 4, 4]
+        rec_y = np.clip(pred + unblocks(inv4(dequant(lvl, qp))), 0, 255)
+        # chroma: eighth-pel bilinear (8.4.2.2.2) at the luma MV in quarter-pel units
+        mvcx, mvcy = 4 * mvx, 4 * mvy
+        fx, fy = (mvcx & 7)[:, :, None, None], (mvcy & 7)[:, :, None, None]
+        cy = np.arange(8)[None, None, :, None] + 8 * np.arange(R)[:, None, None, None] + (mvcy >> 3)[:, :, None, None]
+        cx = np.arange(8)[None, None, None, :] + 8 * np.arange(C)[None, :, None, None] + (mvcx >> 3)[:, :, None, None]
+        cres, crec = [], []
+        for sp, rp in ((U, ru), (V, rv)):
+            at = lambda y, x: rp[np.clip(y, 0, H16 // 2 - 1), np.clip(x, 0, W16 // 2 - 1)]
+            cp = ((8 - fx) * (8 - fy) * at(cy, cx) + fx * (8 - fy) * at(cy, cx + 1) + (8 - fx) * fy * at(cy + 1, cx)
+                  + fx * fy * at(cy + 1, cx + 1) + 32) >> 6
+            dcl_c, acl_c, rec_c = code_chroma(_mb_view(sp.astype(np.int64), 8), cp, qpc, False)
+            cres.append((dcl_c, acl_c))
+            crec.append(rec_c)
+        nonzero = (lvl != 0).any((-1, -2, -3)) | (cres[0][0] != 0).any(-1) | (cres[0][1] != 0).any((-1, -2)) \
+            | (cres[1][0] != 0).any(-1) | (cres[1][1] != 0).any((-1, -2))
+        skip = (mvx == 0) & (mvy == 0) & ~nonzero
+        mbs = [[dict(intra=False, skip=bool(skip[r, c]), mv=(int(mvx[r, c]), int(mvy[r, c])), lac=scan(lvl[r, c]),
+                     cdc=[cres[0][0][r, c], cres[1][0][r, c]], cac=[cres[0][1][r, c], cres[1][1][r, c]])
+                for c in range(C)] for r in range(R)]
+        self.mvs, self.skip = np.stack([mvx, mvy], -1), skip
+        return mbs, (rec_y, crec[0], crec[1])
+
+    # ---------------------------------------------------------------- syntax
+    def _slice(self, row, mbs, idr, frame_num, idr_pic_id):
+        bw = Bits()
+        bw.ue(row * self.mbw)                      # first_mb_in_slice
+        bw.ue(2 if idr else 0)                     # slice_type I / P
+        bw.ue(0)                                   # pic_parameter_set_id
+        bw.u(frame_num, 4)                         # log2_max_frame_num = 4
+        if idr:
+            bw.ue(idr_pic_id)
+        else:
+            bw.u(0, 1)                             # num_ref_idx_active_override_flag
+            bw.u(0, 1)                             # ref_pic_list_modification_flag_l0
+        bw.u(0, 1)                                 # no_output_of_prior_pics_flag / adaptive_ref_pic_marking_mode_flag
+        if idr:
+            bw.u(0, 1)                             # long_term_reference_flag
+        bw.se(0)                                   # slice_qp_delta
+        bw.ue(1)                                   # disable_deblocking_filter_idc
+        left_tc = [0] * 4                          # TotalCoeff of the left MB's right-column luma blocks (rows 0..3)
+        left_cc = [[0, 0], [0, 0]]                 # ... and of its right-column chroma blocks, per component
+        skip_run = 0
+        mvp = (0, 0)
+        for c, m in enumerate(mbs):
+            if not idr and m['skip']:
+                skip_run += 1
+                left_tc, left_cc, mvp = [0] * 4, [[0, 0], [0, 0]], (0, 0)
+                continue
+            tc = np.zeros((4, 4), int)             # [by, bx]
+            if idr:
+                nz_ac = any(np.any(m['lac'][k][1:]) for k in range(16))
+                cbp_l = 15 if nz_ac else 0
+            else:
+                bw.ue(skip_run)
+                skip_run = 0
+                cbp_l = sum(1 << q for q in range(4) if any(np.any(m['lac'][4 * q + k]) for k in range(4)))
+            cdc_nz = any(np.any(x) for x in m['cdc'])
+            cac_nz = any(np.any(x[:, 1:]) for x in m['cac'])
+            cbp_c = 2 if cac_nz else 1 if cdc_nz else 0
+            if idr:
+                bw.ue(1 + m['mode'] + 4 * cbp_c + (12 if cbp_l else 0))     # mb_type I_16x16_<mode>_<cbp_c>_<cbp_l>
+                bw.ue(0)                                                    # intra_chroma_pred_mode DC
+                bw.se(0)                                                    # mb_qp_delta
+                residual_block(bw, m['ldc'], left_tc[0] if c else 0)       # Intra16x16DCLevel: nC of block 0
+            else:
+                bw.ue(0)                                                    # mb_type P_L0_16x16
+                mv = (4 * m['mv'][0], 4 * m['mv'][1])
+                bw.se(mv[0] - mvp[0])
+                bw.se(mv[1] - mvp[1])
+                mvp = mv
+                bw.ue(CBP_CODE[cbp_l + 16 * cbp_c])
+                if cbp_l or cbp_c:
+                    bw.se(0)                                                # mb_qp_delta
+            for k, (bx, by) in enumerate(BLK):
+                if cbp_l >> (k // 4) & 1:
+                    na = tc[by, bx - 1] if bx else left_tc[by] if c else None
+                    tc[by, bx] = residual_block(bw, m['lac'][k][1:] if idr else m['lac'][k], _nc(na, tc[by - 1, bx] if by else None))
+            cc = [np.zeros((2, 2), int), np.zeros((2, 2), int)]
+            if cbp_c:
+                for comp in range(2):
+                    residual_block(bw, m['cdc'][comp], -1)
+            if cbp_c == 2:
+                for comp in range(2):
+                    for k in range(4):
+                        by, bx = divmod(k, 2)
+                        na = cc[comp][by, bx - 1] if bx else left_cc[comp][by] if c else None
+                        cc[comp][by, bx] = residual_block(bw, m['cac'][comp][k][1:], _nc(na, cc[comp][by - 1, bx] if by else None))
+            left_tc = [int(tc[by, 3]) for by in range(4)]
+            left_cc = [[int(cc[comp][by, 1]) for by in range(2)] for comp in range(2)]
+        if skip_run:
+            bw.ue(skip_run)
+        nal = bytes([0x65 if idr else 0x61]) + escape(bw.rbsp())
+        return len(nal).to_bytes(4, 'big') + nal
+
+    def encode(self, rgb):
+        """One uint8 RGB frame [H, W, 3] -> (AVCC sample bytes, is_idr)."""
+        rgb = np.asarray(rgb)
+        if rgb.shape != (self.H, self.W, 3) or rgb.dtype != np.uint8:
+            raise ValueError(f'expected a uint8 frame of shape {(self.H, self.W, 3)}, got {rgb.dtype} {rgb.shape}')
+        Y, U, V = rgb_to_yuv420(rgb)
+        k = self.n % self.gop
+        idr = k == 0
+        if idr:
+            mbs, rec = self._intra(Y, U, V)
+            self.mvs, self.skip = None, None
+        else:
+            mbs, rec = self._inter(Y, U, V)
+        R, C = self.mbh, self.mbw
+        self.recon = tuple(p.swapaxes(1, 2).reshape(R * p.shape[2], C * p.shape[3]).astype(np.uint8) for p in rec)
+        idr_pic_id = (self.n // self.gop) % 2
+        sample = b''.join(self._slice(r, mbs[r], idr, k % 16, idr_pic_id) for r in range(R))
+        self.n += 1
+        return sample, idr
+
+
+def unblocks_dc(dc):
+    """[..., 16] DC per luma4x4BlkIdx -> [..., 4, 4] spatial (row = block y, column = block x)."""
+    out = np.zeros(dc.shape[:-1] + (4, 4), dc.dtype)
+    for k, (bx, by) in enumerate(BLK):
+        out[..., by, bx] = dc[..., k]
+    return out
+
+
+def blocks_dc(m):
+    """Inverse of unblocks_dc."""
+    return np.stack([m[..., by, bx] for bx, by in BLK], -1)
+
+
+# ------------------------------------------------------------------------------------------------ test sequences
+TRANSLATE = (3, -1)             # per-frame shift of the 'translate' sequence: frame t samples the pattern at x + 3t, y - t
+EDGE = (2, 2)                   # ... and of 'edge', whose pattern has a hard border that moves across the picture
+
+
+def _pattern(H, W, seed):
+    rng = np.random.RandomState(seed)
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    img = np.zeros((H, W, 3))
+    for c in range(3):
+        for _ in range(6):
+            fx, fy, ph = rng.uniform(0.02, 0.25, 2).tolist() + [rng.uniform(0, 6.3)]
+            img[..., c] += np.sin(fx * x + fy * y + ph) * rng.uniform(10, 30)
+    return np.clip(img + 128, 0, 255).astype(np.uint8)
+
+
+def sequence(name, W, H, n=3):
+    """n uint8 RGB frames [H, W, 3] of one of the named test sequences."""
+    if name == 'flat':
+        return [np.full((H, W, 3), (40 + 60 * t, 120, 200 - 50 * t), np.uint8) for t in range(n)]
+    if name == 'gradient':
+        y, x = np.mgrid[0:H, 0:W]
+        return [np.stack([(x * 255 // max(W - 1, 1) + 4 * t) % 256, y * 255 // max(H - 1, 1), np.full_like(x, 90 + 10 * t)],
+                         -1).astype(np.uint8) for t in range(n)]
+    if name in ('translate', 'edge'):
+        dx, dy = TRANSLATE if name == 'translate' else EDGE
+        m = 4 * n + 8
+        big = _pattern(H + 2 * m, W + 2 * m, 1)
+        if name == 'edge':                                   # a flat region whose border moves into the picture
+            big[:, :m + W // 2] = (30, 200, 60)
+        return [big[m + dy * t:m + dy * t + H, m + dx * t:m + dx * t + W].copy() for t in range(n)]
+    if name == 'noise':
+        rng = np.random.RandomState(W * 1000 + H)
+        return [rng.randint(0, 256, (H, W, 3)).astype(np.uint8) for _ in range(n)]
+    raise ValueError(name)
+
+
+SEQUENCES = ('flat', 'gradient', 'translate', 'edge', 'noise')
