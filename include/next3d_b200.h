@@ -448,6 +448,26 @@ int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp, int idr, 
                     const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
                     void* stream);
 
+/* Rate-controlled stream: the same encoder with one QP per picture chosen on the device (no host synchronisation), quarter-sample
+ * motion vectors and in-loop deblocking across slice boundaries (the deblocked picture is recon and the next P frame's
+ * reference).  Its PPS has pic_init_qp 26 (next3d_b200.video.pps(26)); each slice carries slice_qp_delta = QP - 26.
+ * The controller state is N3D_H264_RC_STATE_BYTES of caller-owned device memory (8-byte aligned), written by n3d_h264_rc_init and
+ * updated on the stream after every n3d_h264_encode_rc from *sample_len: a one-second leaky bucket in integer arithmetic, QP
+ * changing by at most 2 between consecutive P frames and kept across IDR frames, clamped to qp_min..qp_max (equal bounds pin it). */
+#define N3D_H264_RC_STATE_BYTES 128
+
+/* Stream-ordered: writes the state for width x height frames at bits_per_second (1..2^32-1) and fps_num / fps_den frames/s
+ * (each 1..2^20), QP bounds 0 <= qp_min <= qp_max <= 51; the first QP follows from the bits per pixel.  N3D_ERR_INVALID_ARG
+ * for a null state, the sizes n3d_h264_buffer_sizes refuses, or values out of range. */
+int n3d_h264_rc_init(void* state, int width, int height, int64_t bits_per_second, int fps_num, int fps_den, int qp_min, int qp_max,
+                     void* stream);
+
+/* n3d_h264_encode with the controller state (initialised by n3d_h264_rc_init for the same size) in place of qp; the same
+ * buffers and argument checks.  No host synchronisation. */
+int n3d_h264_encode_rc(const uint8_t* rgb, int width, int height, void* state, int idr, int frame_num, int idr_pic_id, uint8_t* cur,
+                       const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,9 @@ run) and rendered by the batched drivers of next3d_b200.drivers on one CUDA devi
     grid larger than 1x1 (every cell would show the same head);
   * mp4 files are written with imageio (libx264 at the scripts' bitrates); without it the video commands refuse before loading
     the network.  `--encoder n3d` writes them with this package's H.264 encoder on the GPU instead (next3d_b200.video: constant
-    `--qp`, default 18, integer-pel motion, no deblocking; INTEGRATION.md section 0) and never imports imageio.
+    `--qp`, default 18, integer-pel motion, no deblocking; INTEGRATION.md section 0) and never imports imageio.  With
+    `--bitrate` (`script`: the scripts' 10M / 12M, or a rate such as 8M) it writes the rate-controlled stream instead: QP chosen
+    on the GPU per frame, quarter-sample motion and deblocking.
 """
 import argparse
 import os
@@ -111,7 +113,10 @@ def _parser():
 def _encoder_args(p):
     p.add_argument('--encoder', choices=['imageio', 'n3d'], default='imageio',
                    help='imageio: libx264 through imageio (the scripts); n3d: the sm_90a H.264 encoder of next3d_b200.video')
-    p.add_argument('--qp', type=int, default=18, help='constant quantiser 0..51 of --encoder n3d (lower = larger, closer)')
+    p.add_argument('--qp', type=int, default=None, help='constant quantiser 0..51 of --encoder n3d (lower = larger, closer; default 18)')
+    p.add_argument('--bitrate', default=None,
+                   help="--encoder n3d at a bitrate instead of a constant QP: 'script' (the scripts' rate per video) or bits/s "
+                        "such as 8M or 800k")
 
 
 def _refuse(msg):
@@ -129,12 +134,26 @@ def _imageio():
 
 def _video_writer(args):
     """write(path, frames, fps, bitrate) of the chosen --encoder, checked before the network is loaded."""
+    if args.bitrate is not None:
+        if args.encoder != 'n3d':
+            _refuse('--bitrate selects the rate-controlled stream of --encoder n3d; imageio already writes at the scripts\' rates')
+        if args.qp is not None:
+            _refuse('--bitrate and --qp exclude each other: the rate controller chooses the QP')
+        if args.bitrate != 'script':
+            from .video import parse_bitrate
+            try:
+                rate = parse_bitrate(args.bitrate)
+            except ValueError as e:
+                _refuse(f'--bitrate: {e}')
+            return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, None, rate)
+        return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, None, bitrate)
     if args.encoder == 'imageio':
         imageio = _imageio()
         return lambda path, frames, fps, bitrate: _write_video(imageio, path, frames, fps, bitrate)
-    if not 0 <= args.qp <= 51:
-        _refuse(f'--qp {args.qp}: the quantiser is 0..51')
-    return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, args.qp)
+    qp = 18 if args.qp is None else args.qp
+    if not 0 <= qp <= 51:
+        _refuse(f'--qp {qp}: the quantiser is 0..51')
+    return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, qp)
 
 
 def _load(args):
@@ -162,13 +181,14 @@ def _write_video(imageio, path, frames, fps, bitrate):
         writer.close()
 
 
-def _write_video_n3d(path, frames, fps, qp):
+def _write_video_n3d(path, frames, fps, qp, bitrate=None):
     from .video import H264Writer
     writer = None
     try:
         for frame in frames:
             if writer is None:
-                writer = H264Writer(path, frame.shape[1], frame.shape[0], fps, qp=qp)
+                writer = (H264Writer(path, frame.shape[1], frame.shape[0], fps, qp=qp) if bitrate is None else
+                          H264Writer(path, frame.shape[1], frame.shape[0], fps, bitrate=bitrate))
             writer.write(frame)
     finally:
         if writer is not None:

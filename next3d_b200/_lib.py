@@ -118,10 +118,13 @@ _SIGNATURES = {
     'n3d_interp_rows': ([P, P, C.c_int, C.c_int, I64, P, P], C.c_int),
     'n3d_h264_buffer_sizes': ([C.c_int, C.c_int, C.POINTER(I64), C.POINTER(I64), C.POINTER(I64), C.POINTER(I64)], C.c_int),
     'n3d_h264_encode': ([P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P], C.c_int),
+    'n3d_h264_rc_init': ([P, C.c_int, C.c_int, I64, C.c_int, C.c_int, C.c_int, C.c_int, P], C.c_int),
+    'n3d_h264_encode_rc': ([P, C.c_int, C.c_int, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P], C.c_int),
     'n3d_sample_grid': ([P, C.c_int, C.c_int, C.c_int, F32, F32, I64, I64, C.c_int, F32, P, P, P, P, P, P], C.c_int),
 }
 
 EXPORTS = sorted(_SIGNATURES)
+H264_RC_STATE_BYTES = 128             # N3D_H264_RC_STATE_BYTES
 
 for _name, (_args, _res) in _SIGNATURES.items():
     _fn = getattr(lib, _name)          # AttributeError here = the library does not export what the header declares

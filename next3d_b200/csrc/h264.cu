@@ -10,7 +10,12 @@
 //   h264_write_rows   CAVLC: one thread per row writes the slice NAL unit (header, MB layer, trailing bits, emulation prevention)
 //                     into its own bounded slot, length-prefixed.
 //   h264_pack         concatenates the slots into one AVCC sample (an MP4 sample of the frame).
-// The numpy restatement in tests/h264_oracle.py makes the same decisions and writes the same bytes.
+// The rate-controlled stream (n3d_h264_encode_rc) runs the same kernels with kRc = true: every kernel reads the picture's QP from
+// the controller state, h264_inter_mbs refines the vector to quarter samples, and two kernels are added:
+//   h264_deblock      in-loop deblocking (8.7) in place on the reconstruction: one warp per MB row, rows taken in order through an
+//                     atomic ticket, MB x of a row waiting until the row above has finished MB x + 1 (the standard's raster order).
+//   h264_rc_update    one thread: the frame's size -> the controller state and the next picture's QP.
+// The numpy restatements in tests/h264_oracle.py and tests/h264_rc_oracle.py make the same decisions and write the same bytes.
 #include "common.cuh"
 
 namespace {
@@ -22,6 +27,13 @@ constexpr int kLevelMax = 2063;                 // largest |level| CAVLC codes w
 constexpr int kMaxFs = 139264;                  // level 6.2 MaxFS (macroblocks)
 constexpr int kBlockBits = 16 + 3 + 16 * 28 + 9 + 15 * 11;   // coeff_token, T1 signs, 16 escaped levels, total_zeros, run_before
 constexpr int kMbBits = 27 * kBlockBits + 128;  // 27 residual blocks + MB header (skip run, type, mvd, cbp, qp delta)
+constexpr int kMvOff = 128;                     // key offset of quarter-sample vector components (|mv| <= 4 * kSearch + 3)
+constexpr int kPat = 22;                        // quarter-sample patch side: the 16 samples +- 1 of refinement, 2 + 3 filter taps
+constexpr uint32_t kSpinLimit = 1u << 24;       // bounded waits of h264_deblock (~1 s of __nanosleep(64)), then trap
+
+// Rate-control state (int64 fields, N3D_H264_RC_STATE_BYTES).  Fullness: the stream's excess over bitrate x time, in 1/fps_num bits.
+enum { kRcBitrate, kRcNum, kRcDen, kRcQpMin, kRcQpMax, kRcQp, kRcFullness, kRcFrames, kRcPrevIdr, kRcFields = 16 };
+static_assert(kRcFields * 8 == N3D_H264_RC_STATE_BYTES, "rate-control state size");
 
 // Per-MB record between the decision kernels and the writer.  lv: levels in zig-zag order per block: 0-15 luma 4x4 blocks
 // (luma4x4BlkIdx order; index 0 unused for I_16x16), 16 luma DC (I_16x16), 17 chroma DC (Cb 0-3, Cr 4-7), 18-21 Cb AC, 22-25 Cr AC
@@ -40,6 +52,19 @@ __constant__ uint8_t c_lambda[52] = {0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1
                                      10, 12, 13, 15, 17, 19, 21, 23, 26, 30, 33, 37, 42, 47, 53, 59, 66, 74, 83};
 __constant__ int c_mf[6][3] = {{13107, 5243, 8066}, {11916, 4660, 7490}, {10082, 4194, 6554}, {9362, 3647, 5825}, {8192, 3355, 5243}, {7282, 2893, 4559}};
 __constant__ int c_v[6][3] = {{10, 16, 13}, {11, 18, 14}, {13, 20, 16}, {14, 23, 18}, {16, 25, 20}, {18, 29, 23}};
+__constant__ uint8_t c_qpc[52] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28,
+                                  29, 29, 30, 31, 32, 32, 33, 34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39};
+// deblocking: alpha' and beta' (Table 8-16), tC0' for bS = 1, 2, 3 (Table 8-17), by indexA / indexB (= qPav: offsets 0)
+__constant__ uint8_t c_alpha[52] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 4, 4, 5, 6, 7, 8, 9, 10, 12, 13, 15, 17, 20, 22, 25,
+                                    28, 32, 36, 40, 45, 50, 56, 63, 71, 80, 90, 101, 113, 127, 144, 162, 182, 203, 226, 255, 255};
+__constant__ uint8_t c_beta[52] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 6, 6, 7, 7, 8, 8, 9, 9,
+                                   10, 10, 11, 11, 12, 12, 13, 13, 14, 14, 15, 15, 16, 16, 17, 17, 18, 18};
+__constant__ uint8_t c_tc0[52][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0},
+                                     {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 1},
+                                     {0, 0, 1}, {0, 0, 1}, {0, 0, 1}, {0, 1, 1}, {0, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1},
+                                     {1, 1, 2}, {1, 1, 2}, {1, 1, 2}, {1, 1, 2}, {1, 2, 3}, {1, 2, 3}, {2, 2, 3}, {2, 2, 4}, {2, 3, 4},
+                                     {2, 3, 4}, {3, 3, 5}, {3, 4, 6}, {3, 4, 6}, {4, 5, 7}, {4, 5, 8}, {4, 6, 9}, {5, 7, 10}, {6, 8, 11},
+                                     {6, 8, 13}, {7, 10, 14}, {8, 11, 16}, {9, 12, 18}, {10, 13, 20}, {11, 15, 23}, {13, 17, 25}};
 __constant__ uint8_t c_inter_cbp_code[48] = {0, 2, 3, 7, 4, 8, 17, 13, 5, 18, 9, 14, 10, 15, 16, 11, 1, 32, 33, 36, 34, 37, 44, 40,
                                              35, 45, 38, 41, 39, 42, 43, 19, 6, 24, 25, 20, 26, 21, 46, 28, 27, 47, 22, 29, 23, 30, 31, 12};
 
@@ -93,6 +118,8 @@ struct Frame {
     uint8_t* rec;              // padded I420 reconstruction of this frame
     MbRec* mbs;
     int32_t* lens;             // bytes per slot, -1 when the slot overflowed
+    int32_t* dbk;              // h264_deblock: [0] row ticket, [1 + r] MBs of row r filtered (reset on the stream per frame)
+    int64_t* rc;               // rate-control state (kRc kernels read the picture's QP from it)
     uint8_t* slots;
     int64_t slot_cap;
     int idr, frame_num, idr_pic_id;
@@ -200,12 +227,13 @@ __global__ void h264_rgb_to_yuv(Frame F) {
 }
 
 // ------------------------------------------------------------------------------------------------ IDR: I_16x16, one warp per row
+template <bool kRc>
 __global__ void __launch_bounds__(32) h264_intra_rows(Frame F) {
     __shared__ int s_w[16][16];        // luma coefficients per block (raster)
     __shared__ int s_cdc[2][4], s_dcc[2][4], s_dcy[16];
     __shared__ int s_left[16];
     const int row = blockIdx.x, lane = threadIdx.x;
-    const int qp = F.qp, qpc = F.qpc;
+    const int qp = kRc ? (int)F.rc[kRcQp] : F.qp, qpc = kRc ? c_qpc[qp] : F.qpc;
     const int cw = F.W16 / 2;
     const uint8_t* Ys = F.cplane(F.cur, 0);
     uint8_t* Yr = F.plane(F.rec, 0);
@@ -311,14 +339,54 @@ __global__ void __launch_bounds__(32) h264_intra_rows(Frame F) {
     }
 }
 
+// Luma sample at quarter-sample position (X4, Y4) of patch p (8.4.2.2.1, Table 8-12): the 6-tap half samples b (right), h (below)
+// and j (both), the quarter samples averages of their neighbours.  The position must keep 2 samples left / above and 3 right / below.
+__device__ int qpel(const uint8_t (*p)[kPat], int X4, int Y4) {
+    const int x = X4 >> 2, y = Y4 >> 2;
+    auto G = [&](int yy, int xx) { return (int)p[yy][xx]; };
+    auto b1 = [&](int yy, int xx) { return G(yy, xx - 2) - 5 * G(yy, xx - 1) + 20 * G(yy, xx) + 20 * G(yy, xx + 1) - 5 * G(yy, xx + 2) + G(yy, xx + 3); };
+    auto B = [&](int yy, int xx) { return clip255((b1(yy, xx) + 16) >> 5); };
+    auto Hh = [&](int yy, int xx) {
+        return clip255((G(yy - 2, xx) - 5 * G(yy - 1, xx) + 20 * G(yy, xx) + 20 * G(yy + 1, xx) - 5 * G(yy + 2, xx) + G(yy + 3, xx) + 16) >> 5);
+    };
+    auto J = [&]() {
+        return clip255((b1(y - 2, x) - 5 * b1(y - 1, x) + 20 * b1(y, x) + 20 * b1(y + 1, x) - 5 * b1(y + 2, x) + b1(y + 3, x) + 512) >> 10);
+    };
+    auto av = [](int a, int c) { return (a + c + 1) >> 1; };
+    switch (4 * (Y4 & 3) + (X4 & 3)) {
+        case 0: return G(y, x);
+        case 1: return av(G(y, x), B(y, x));
+        case 2: return B(y, x);
+        case 3: return av(G(y, x + 1), B(y, x));
+        case 4: return av(G(y, x), Hh(y, x));
+        case 5: return av(B(y, x), Hh(y, x));
+        case 6: return av(B(y, x), J());
+        case 7: return av(B(y, x), Hh(y, x + 1));
+        case 8: return Hh(y, x);
+        case 9: return av(Hh(y, x), J());
+        case 10: return J();
+        case 11: return av(J(), Hh(y, x + 1));
+        case 12: return av(G(y + 1, x), Hh(y, x));
+        case 13: return av(Hh(y, x), B(y + 1, x));
+        case 14: return av(J(), B(y + 1, x));
+        default: return av(Hh(y, x + 1), B(y + 1, x));
+    }
+}
+
+__device__ __forceinline__ unsigned long long mv_key(int cost, int qx, int qy) {
+    return ((unsigned long long)cost << 24) | ((unsigned long long)(abs(qx) + abs(qy)) << 16) | ((unsigned long long)(qy + kMvOff) << 8) |
+           (unsigned long long)(qx + kMvOff);
+}
+
 // ------------------------------------------------------------------------------------------------ P: one block per MB
+template <bool kRc>
 __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
     __shared__ uint8_t s_win[kWin][kWin];
     __shared__ uint8_t s_cur[16][16];
     __shared__ unsigned long long s_best[8];
     __shared__ int s_cdc[2][4], s_dcc[2][4];
     const int mbx = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
-    const int qp = F.qp, qpc = F.qpc;
+    const int qp = kRc ? (int)F.rc[kRcQp] : F.qp, qpc = kRc ? c_qpc[qp] : F.qpc;
     const int x0 = 16 * mbx, y0 = 16 * row;
     const uint8_t* Yref = F.cplane(F.ref, 0);
     const uint8_t* Ys = F.cplane(F.cur, 0);
@@ -350,6 +418,37 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
     best = s_best[0];
     for (int i = 1; i < 8; ++i) best = min(best, s_best[i]);
     const int mvy = (int)((best >> 8) & 0xff) - kSearch, mvx = (int)(best & 0xff) - kSearch;
+    // quarter-sample refinement (rate-controlled stream): the 8 half-sample neighbours of the integer vector, then the 8
+    // quarter-sample neighbours of the best of those, same cost and tie order; one warp per candidate over a haloed patch
+    __shared__ uint8_t s_pat[kRc ? kPat : 1][kPat];
+    __shared__ unsigned long long s_key[8];
+    int qx = 4 * mvx, qy = 4 * mvy;
+    if constexpr (kRc) {
+        for (int i = tid; i < kPat * kPat; i += 256) {
+            const int y = min(max(y0 + mvy - 3 + i / kPat, 0), F.H16 - 1), x = min(max(x0 + mvx - 3 + i % kPat, 0), F.W16 - 1);
+            s_pat[i / kPat][i % kPat] = Yref[(int64_t)y * F.W16 + x];
+        }
+        best = mv_key((int)(best >> 24), qx, qy);
+        __syncthreads();
+        const int warp = tid >> 5, lane32 = tid & 31;
+        for (int step = 2; step >= 1; --step) {
+            const int cx = qx, cy = qy;
+            const int d = warp < 4 ? warp : warp + 1, dx = d % 3 - 1, dy = d / 3 - 1;
+            const int x4 = cx + step * dx, y4 = cy + step * dy;
+            int sad = 0;
+            for (int k = 0; k < 8; ++k) {
+                const int pix = lane32 + 32 * k, y = pix >> 4, x = pix & 15;
+                sad += abs((int)s_cur[y][x] - qpel(s_pat, 4 * (x + 3) + x4 - 4 * mvx, 4 * (y + 3) + y4 - 4 * mvy));
+            }
+            for (int o = 16; o; o >>= 1) sad += __shfl_xor_sync(0xffffffffu, sad, o);
+            if (lane32 == 0) s_key[warp] = mv_key(sad + lam * (ue_bits(se_code(x4)) + ue_bits(se_code(y4))), x4, y4);
+            __syncthreads();
+            for (int i = 0; i < 8; ++i) best = min(best, s_key[i]);
+            __syncthreads();
+            qx = (int)(best & 0xff) - kMvOff;
+            qy = (int)((best >> 8) & 0xff) - kMvOff;
+        }
+    }
     MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
     const int cw = F.W16 / 2, chh = F.H16 / 2;
     int w[16], pred[16], res[16];
@@ -359,7 +458,7 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
     if (lane < 16) {
         for (int r = 0; r < 16; ++r) {
             const int y = 4 * by + (r >> 2), x = 4 * bx + (r & 3);
-            pred[r] = s_win[kSearch + mvy + y][kSearch + mvx + x];
+            pred[r] = kRc ? qpel(s_pat, 4 * (x + 3) + qx - 4 * mvx, 4 * (y + 3) + qy - 4 * mvy) : s_win[kSearch + mvy + y][kSearch + mvx + x];
             w[r] = s_cur[y][x] - pred[r];
         }
         fwd4(w, w);
@@ -369,7 +468,7 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
         for (int r = 0; r < 16; ++r)
             Yr[(int64_t)(y0 + 4 * by + (r >> 2)) * F.W16 + x0 + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
     } else if (lane < 24) {                              // chroma: eighth-pel bilinear at the luma MV (8.4.2.2.2)
-        const int mvcx = 4 * mvx, mvcy = 4 * mvy, fx = mvcx & 7, fy = mvcy & 7;
+        const int mvcx = qx, mvcy = qy, fx = mvcx & 7, fy = mvcy & 7;      // chroma eighth samples = luma quarter samples
         const uint8_t* Cref = F.cplane(F.ref, comp);
         const uint8_t* Cs = F.cplane(F.cur, comp);
         for (int r = 0; r < 16; ++r) {
@@ -383,8 +482,8 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
         s_cdc[comp - 1][(lane - 16) & 3] = w[0];
     } else if (lane == 32) {
         R->mode = 0;
-        R->mvx = 4 * mvx;
-        R->mvy = 4 * mvy;
+        R->mvx = qx;
+        R->mvy = qy;
         for (int k = 0; k < 16; ++k) R->lv[16][k] = 0;
     }
     __syncthreads();
@@ -401,6 +500,169 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
         for (int r = 0; r < 16; ++r)
             Cr[(int64_t)(8 * row + 4 * by + (r >> 2)) * cw + 8 * mbx + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
     }
+}
+
+// ------------------------------------------------------------------------------------------------ deblocking (8.7)
+// One edge line: q points at q0, step = distance from q0 to q1 (p_k = q[-(k + 1) * step], q_k = q[k * step]).  Loads bypass L1
+// (other CTAs write the rows above during the kernel).
+__device__ void filter_line(uint8_t* q, int64_t step, int bS, int idx, bool chroma) {
+    if (bS == 0) return;
+    const int a = c_alpha[idx], be = c_beta[idx];
+    auto ld = [&](int k) { return (int)__ldcg(q + k * step); };
+    const int p0 = ld(-1), q0 = ld(0), p1 = ld(-2), q1 = ld(1);
+    if (abs(p0 - q0) >= a || abs(p1 - p0) >= be || abs(q1 - q0) >= be) return;
+    if (chroma) {
+        if (bS < 4) {
+            const int tc = c_tc0[idx][bS - 1] + 1;
+            const int delta = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
+            q[-step] = (uint8_t)clip255(p0 + delta);
+            q[0] = (uint8_t)clip255(q0 - delta);
+        } else {
+            q[-step] = (uint8_t)((2 * p1 + p0 + q1 + 2) >> 2);
+            q[0] = (uint8_t)((2 * q1 + q0 + p1 + 2) >> 2);
+        }
+        return;
+    }
+    const int p2 = ld(-3), q2 = ld(2);
+    const bool ap = abs(p2 - p0) < be, aq = abs(q2 - q0) < be;
+    if (bS < 4) {
+        const int tc0 = c_tc0[idx][bS - 1], tc = tc0 + ap + aq;
+        const int delta = min(max((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc), tc);
+        q[-step] = (uint8_t)clip255(p0 + delta);
+        q[0] = (uint8_t)clip255(q0 - delta);
+        if (ap) q[-2 * step] = (uint8_t)(p1 + min(max((p2 + ((p0 + q0 + 1) >> 1) - (p1 << 1)) >> 1, -tc0), tc0));
+        if (aq) q[step] = (uint8_t)(q1 + min(max((q2 + ((p0 + q0 + 1) >> 1) - (q1 << 1)) >> 1, -tc0), tc0));
+        return;
+    }
+    const bool near = abs(p0 - q0) < ((a >> 2) + 2);
+    if (ap && near) {
+        const int p3 = ld(-4);
+        q[-step] = (uint8_t)((p2 + 2 * p1 + 2 * p0 + 2 * q0 + q1 + 4) >> 3);
+        q[-2 * step] = (uint8_t)((p2 + p1 + p0 + q0 + 2) >> 2);
+        q[-3 * step] = (uint8_t)((2 * p3 + 3 * p2 + p1 + p0 + q0 + 4) >> 3);
+    } else {
+        q[-step] = (uint8_t)((2 * p1 + p0 + q1 + 2) >> 2);
+    }
+    if (aq && near) {
+        const int q3 = ld(3);
+        q[0] = (uint8_t)((p1 + 2 * p0 + 2 * q0 + 2 * q1 + q2 + 4) >> 3);
+        q[step] = (uint8_t)((p0 + q0 + q1 + q2 + 2) >> 2);
+        q[2 * step] = (uint8_t)((2 * q3 + 3 * q2 + q1 + q0 + p0 + 4) >> 3);
+    } else {
+        q[0] = (uint8_t)((2 * q1 + q0 + p1 + 2) >> 2);
+    }
+}
+
+// Bit (4 * by + bx) set when luma 4x4 block (bx, by) of the MB has nonzero levels; lanes 0-15 of a warp.
+__device__ unsigned nz_mask(const MbRec* R, int lane) {
+    bool nz = false;
+    for (int i = 0; lane < 16 && i < 16; ++i) nz |= R->lv[lane][i] != 0;
+    const unsigned b = __ballot_sync(0xffffffffu, nz);
+    unsigned m = 0;
+    for (int k = 0; k < 16; ++k) if (b >> k & 1) m |= 1u << (4 * c_blk_y[k] + c_blk_x[k]);
+    return m;
+}
+
+// bS (8.7.2.1) of the luma edge between 4x4 blocks p and q: intra picture 4 on MB edges, 3 inside; else 2 when either block has
+// levels, 1 on MB edges whose vectors differ by >= 4 quarter samples in a component, 0 otherwise.
+__device__ __forceinline__ int bs_of(bool intra, bool mb_edge, bool nz, bool mv_differs) {
+    if (intra) return mb_edge ? 4 : 3;
+    return nz ? 2 : (mb_edge && mv_differs) ? 1 : 0;
+}
+
+// One warp per MB row, rows in ticket order; lanes 0-15 own a luma line of the edge being filtered, lanes 16-23 a Cb line, 24-31 a
+// Cr line.  Per MB: vertical edges left to right, then horizontal edges top to bottom.  MB x of row r starts once row r - 1 has
+// finished MB x + 1, the last MB whose filtering touches the samples MB x reads.
+__global__ void __launch_bounds__(32) h264_deblock(Frame F) {
+    __shared__ int s_row;
+    const int lane = threadIdx.x;
+    if (lane == 0) s_row = atomicAdd(F.dbk, 1);
+    __syncwarp();
+    const int row = s_row;
+    const int qp = (int)F.rc[kRcQp], qpc = c_qpc[qp];
+    const bool intra = F.idr;
+    volatile int32_t* done = F.dbk + 1;
+    const int cw = F.W16 / 2;
+    uint8_t* Y = F.plane(F.rec, 0);
+    uint8_t* Cp = F.plane(F.rec, lane < 24 ? 1 : 2);
+    const int line = lane < 16 ? lane : (lane - 16) & 7;
+    unsigned nz_left = 0;
+    for (int mbx = 0; mbx < F.mbw; ++mbx) {
+        if (row > 0 && lane == 0) {
+            const int need = min(mbx + 2, F.mbw);
+            uint32_t it = 0;
+            while (done[row - 1] < need) {
+                if (++it == kSpinLimit) __trap();
+                __nanosleep(64);
+            }
+            __threadfence();
+        }
+        __syncwarp();
+        const MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
+        const unsigned nz = intra ? 0u : nz_mask(R, lane);
+        const unsigned nz_top = (intra || row == 0) ? 0u : nz_mask(R - F.mbw, lane);
+        const int x0 = 16 * mbx, y0 = 16 * row;
+        for (int dir = 0; dir < 2; ++dir) {                  // 0: vertical edges, 1: horizontal edges
+            const bool has_prev = dir ? row > 0 : mbx > 0;
+            const unsigned nz_prev = dir ? nz_top : nz_left;
+            const MbRec* P = dir ? R - F.mbw : R - 1;
+            const bool mvd = has_prev && !intra && (abs(R->mvx - P->mvx) >= 4 || abs(R->mvy - P->mvy) >= 4);
+            for (int e = 0; e < 4; ++e) {
+                if (e == 0 && !has_prev) continue;
+                const int blk = (lane < 16 ? line : 2 * line) >> 2;    // 4x4 block index along the edge
+                // nz of the blocks either side: bit (4 * by + bx); vertical edges: bx = e - 1 | e, by = blk
+                const int qb = dir ? 4 * e + blk : 4 * blk + e;
+                const bool nzq = nz >> qb & 1;
+                const bool nzp = e ? (nz >> (dir ? qb - 4 : qb - 1) & 1) : (nz_prev >> (dir ? 12 + blk : 4 * blk + 3) & 1);
+                const int bS = bs_of(intra, e == 0, nzp || nzq, mvd);
+                if (lane < 16) {
+                    uint8_t* q = dir ? Y + (int64_t)(y0 + 4 * e) * F.W16 + x0 + line : Y + (int64_t)(y0 + line) * F.W16 + x0 + 4 * e;
+                    filter_line(q, dir ? F.W16 : 1, bS, qp, false);
+                } else if (!(e & 1)) {
+                    uint8_t* q = dir ? Cp + (int64_t)(8 * row + 2 * e) * cw + 8 * mbx + line : Cp + (int64_t)(8 * row + line) * cw + 8 * mbx + 2 * e;
+                    filter_line(q, dir ? cw : 1, bS, qpc, true);
+                }
+                __syncwarp();
+            }
+        }
+        nz_left = nz;
+        __threadfence();
+        __syncwarp();
+        if (lane == 0) done[row] = mbx + 1;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ rate control
+__device__ __forceinline__ int64_t floor_div(int64_t a, int64_t b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+
+// First QP from bits per pixel: 30 at 0.1, 6 less per doubling, clamped to the bounds.
+__global__ void h264_rc_init(int64_t* st, int width, int height, int64_t bitrate, int64_t num, int64_t den, int qp_min, int qp_max) {
+    for (int i = 0; i < kRcFields; ++i) st[i] = 0;
+    st[kRcBitrate] = bitrate; st[kRcNum] = num; st[kRcDen] = den; st[kRcQpMin] = qp_min; st[kRcQpMax] = qp_max;
+    int64_t x = 10 * bitrate * den, y = num * width * height;
+    int q = 30;
+    while (x >= 2 * y && q > 0) { y *= 2; q -= 6; }
+    while (2 * x < y && q < 51) { x *= 2; q += 6; }
+    st[kRcQp] = min(max(q, qp_min), qp_max);
+}
+
+// After a frame: fullness += its bits - bitrate / fps (saturating at +-8 s); after a P frame, or an IDR frame that follows an IDR
+// frame, QP moves by -2..+2 by the ratio of the frame's bits to its budget (the per-frame rate less a second's share of the
+// fullness, at least 1/8 of the rate).  IDR frames keep the QP of the P frames around them.
+__global__ void h264_rc_update(int64_t* st, const int64_t* sample_len, int idr) {
+    const int64_t len = *sample_len;
+    if (len < 0) return;                                 // overflowed slot: the writer reports it
+    const int64_t num = st[kRcNum], budget = st[kRcBitrate] * st[kRcDen], sat = 8 * st[kRcBitrate] * num;
+    const int64_t bits = 8 * len * num;
+    const int64_t full = min(max(st[kRcFullness] + bits - budget, -sat), sat);
+    st[kRcFullness] = full;
+    if (!idr || st[kRcPrevIdr]) {
+        const int64_t want = max(budget - floor_div(full, max(num / st[kRcDen], (int64_t)1)), budget / 8);
+        const int step = 100 * bits > 141 * want ? 2 : 100 * bits > 112 * want ? 1 : 141 * bits < 100 * want ? -2 : 112 * bits < 100 * want ? -1 : 0;
+        st[kRcQp] = min(max(st[kRcQp] + step, st[kRcQpMin]), st[kRcQpMax]);
+    }
+    st[kRcPrevIdr] = idr;
+    st[kRcFrames] += 1;
 }
 
 // ------------------------------------------------------------------------------------------------ CAVLC slice writer
@@ -493,6 +755,7 @@ __device__ bool any_nonzero(const int16_t* p, int n) {
     return false;
 }
 
+template <bool kRc>
 __global__ void h264_write_rows(Frame F) {
     const int row = blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= F.mbh) return;
@@ -511,8 +774,15 @@ __global__ void h264_write_rows(Frame F) {
     }
     bw.u(0, 1);                              // no_output_of_prior_pics_flag / adaptive_ref_pic_marking_mode_flag
     if (idr) bw.u(0, 1);                     // long_term_reference_flag
-    bw.se(0);                                // slice_qp_delta
-    bw.ue(1);                                // disable_deblocking_filter_idc
+    if (kRc) {
+        bw.se((int)F.rc[kRcQp] - 26);        // slice_qp_delta (pic_init_qp 26)
+        bw.ue(0);                            // disable_deblocking_filter_idc: filter, across slice boundaries too
+        bw.se(0);                            // slice_alpha_c0_offset_div2
+        bw.se(0);                            // slice_beta_offset_div2
+    } else {
+        bw.se(0);                            // slice_qp_delta
+        bw.ue(1);                            // disable_deblocking_filter_idc
+    }
     int left_tc[4] = {0, 0, 0, 0}, left_cc[2][2] = {{0, 0}, {0, 0}};
     int skip_run = 0, mvpx = 0, mvpy = 0;
     for (int mbx = 0; mbx < F.mbw; ++mbx) {
@@ -621,7 +891,7 @@ int sizes(int width, int height, int64_t* plane_bytes, int64_t* scratch_bytes, i
     N3D_CHECK_ARG(mbw * mbh <= kMaxFs && mbw * mbw <= 8 * kMaxFs && mbh * mbh <= 8 * kMaxFs,
                   "n3d_h264: frame size %dx%d exceeds H.264 level 6.2 (%d macroblocks, at most %d per side)", width, height, kMaxFs, 1055);
     *plane_bytes = 256 * mbw * mbh * 3 / 2;
-    *scratch_bytes = (int64_t)sizeof(MbRec) * mbw * mbh + 4 * mbh;
+    *scratch_bytes = (int64_t)sizeof(MbRec) * mbw * mbh + 4 * mbh + 4 * (mbh + 1);     // MBs, slot lengths, deblocking counters
     // slot: 4-byte length, NAL header, escaped RBSP: slice header (<= 128 bits), MBs, trailing skip run and bits (<= 32 bits);
     // emulation prevention adds at most one byte per two
     const int64_t rbsp = (mbw * kMbBits + 128 + 32 + 7) / 8;
@@ -642,18 +912,20 @@ extern "C" int n3d_h264_buffer_sizes(int width, int height, int64_t* plane_bytes
     return N3D_OK;
 }
 
-extern "C" int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp, int idr, int frame_num, int idr_pic_id, uint8_t* cur,
-                               const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
-                               void* stream) {
-    N3D_CHECK_ARG(rgb && cur && recon && scratch && slices && sample && sample_len, "n3d_h264_encode: null buffer");
-    N3D_CHECK_ARG(idr || ref, "n3d_h264_encode: a P frame needs the reference reconstruction (null ref)");
-    N3D_CHECK_ARG(ref != recon, "n3d_h264_encode: ref and recon must be different buffers");
-    N3D_CHECK_ARG(qp >= 0 && qp <= 51, "n3d_h264_encode: qp %d outside 0..51", qp);
+namespace {
+
+// Shared by both entry points: rc == nullptr runs the constant-QP stream at qp, else the rate-controlled stream.
+int encode(const char* name, const uint8_t* rgb, int width, int height, int qp, int64_t* rc, int idr, int frame_num, int idr_pic_id,
+           uint8_t* cur, const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
+           void* stream) {
+    N3D_CHECK_ARG(rgb && cur && recon && scratch && slices && sample && sample_len, "%s: null buffer", name);
+    N3D_CHECK_ARG(idr || ref, "%s: a P frame needs the reference reconstruction (null ref)", name);
+    N3D_CHECK_ARG(ref != recon, "%s: ref and recon must be different buffers", name);
     N3D_CHECK_ARG(frame_num >= 0 && frame_num < 16 && idr_pic_id >= 0 && idr_pic_id <= 65535,
-                  "n3d_h264_encode: frame_num %d (0..15) or idr_pic_id %d (0..65535) out of range", frame_num, idr_pic_id);
+                  "%s: frame_num %d (0..15) or idr_pic_id %d (0..65535) out of range", name, frame_num, idr_pic_id);
     int64_t plane_bytes, scratch_bytes, slot_cap, slice_bytes;
-    const int rc = sizes(width, height, &plane_bytes, &scratch_bytes, &slot_cap, &slice_bytes);
-    if (rc != N3D_OK) return rc;
+    const int rc_ = sizes(width, height, &plane_bytes, &scratch_bytes, &slot_cap, &slice_bytes);
+    if (rc_ != N3D_OK) return rc_;
     Frame F;
     F.W = width; F.H = height;
     F.mbw = (width + 15) / 16; F.mbh = (height + 15) / 16;
@@ -665,14 +937,65 @@ extern "C" int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp
     F.rgb = rgb; F.cur = cur; F.ref = ref; F.rec = recon;
     F.mbs = (MbRec*)scratch;
     F.lens = (int32_t*)((uint8_t*)scratch + (int64_t)sizeof(MbRec) * F.mbw * F.mbh);
+    F.dbk = F.lens + F.mbh;
+    F.rc = rc;
     F.slots = slices; F.slot_cap = slot_cap;
     F.idr = idr ? 1 : 0; F.frame_num = frame_num; F.idr_pic_id = idr_pic_id;
     cudaStream_t s = (cudaStream_t)stream;
     h264_rgb_to_yuv<<<n3d_grid((int64_t)F.W16 * F.H16 / 4, 256), 256, 0, s>>>(F);
-    if (F.idr) h264_intra_rows<<<F.mbh, 32, 0, s>>>(F);
-    else h264_inter_mbs<<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
-    h264_write_rows<<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
-    h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
-    N3D_CHECK_LAUNCH("n3d_h264_encode");
+    if (!rc) {
+        if (F.idr) h264_intra_rows<false><<<F.mbh, 32, 0, s>>>(F);
+        else h264_inter_mbs<false><<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
+        h264_write_rows<false><<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
+        h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
+    } else {
+        if (F.idr) h264_intra_rows<true><<<F.mbh, 32, 0, s>>>(F);
+        else h264_inter_mbs<true><<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
+        const cudaError_t e = cudaMemsetAsync(F.dbk, 0, 4 * (F.mbh + 1), s);          // deblocking counters, per frame
+        if (e != cudaSuccess) {
+            n3d_set_error("%s: resetting the deblocking counters failed: %s", name, cudaGetErrorString(e));
+            return N3D_ERR_CUDA;
+        }
+        h264_deblock<<<F.mbh, 32, 0, s>>>(F);
+        h264_write_rows<true><<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
+        h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
+        h264_rc_update<<<1, 1, 0, s>>>(rc, sample_len, F.idr);
+    }
+    N3D_CHECK_LAUNCH(name);
     return N3D_OK;
+}
+
+}  // namespace
+
+extern "C" int n3d_h264_encode(const uint8_t* rgb, int width, int height, int qp, int idr, int frame_num, int idr_pic_id, uint8_t* cur,
+                               const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
+                               void* stream) {
+    N3D_CHECK_ARG(qp >= 0 && qp <= 51, "n3d_h264_encode: qp %d outside 0..51", qp);
+    return encode("n3d_h264_encode", rgb, width, height, qp, nullptr, idr, frame_num, idr_pic_id, cur, ref, recon, scratch, slices, sample,
+                  sample_len, stream);
+}
+
+extern "C" int n3d_h264_rc_init(void* state, int width, int height, int64_t bits_per_second, int fps_num, int fps_den, int qp_min,
+                                int qp_max, void* stream) {
+    N3D_CHECK_ARG(state, "n3d_h264_rc_init: null state");
+    int64_t plane_bytes, scratch_bytes, slot_cap, slice_bytes;
+    const int rc = sizes(width, height, &plane_bytes, &scratch_bytes, &slot_cap, &slice_bytes);
+    if (rc != N3D_OK) return rc;
+    N3D_CHECK_ARG(bits_per_second > 0 && bits_per_second <= 0xffffffffLL, "n3d_h264_rc_init: bits_per_second %lld outside 1..2^32-1",
+                  (long long)bits_per_second);
+    N3D_CHECK_ARG(fps_num > 0 && fps_den > 0 && fps_num <= (1 << 20) && fps_den <= (1 << 20),
+                  "n3d_h264_rc_init: frame rate %d/%d: numerator and denominator must be in 1..2^20", fps_num, fps_den);
+    N3D_CHECK_ARG(0 <= qp_min && qp_min <= qp_max && qp_max <= 51, "n3d_h264_rc_init: qp bounds %d..%d: need 0 <= qp_min <= qp_max <= 51",
+                  qp_min, qp_max);
+    h264_rc_init<<<1, 1, 0, (cudaStream_t)stream>>>((int64_t*)state, width, height, bits_per_second, fps_num, fps_den, qp_min, qp_max);
+    N3D_CHECK_LAUNCH("n3d_h264_rc_init");
+    return N3D_OK;
+}
+
+extern "C" int n3d_h264_encode_rc(const uint8_t* rgb, int width, int height, void* state, int idr, int frame_num, int idr_pic_id,
+                                  uint8_t* cur, const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample,
+                                  int64_t* sample_len, void* stream) {
+    N3D_CHECK_ARG(state, "n3d_h264_encode_rc: null state");
+    return encode("n3d_h264_encode_rc", rgb, width, height, 0, (int64_t*)state, idr, frame_num, idr_pic_id, cur, ref, recon, scratch, slices,
+                  sample, sample_len, stream);
 }

@@ -1,9 +1,12 @@
 """H.264 video on the device: `H264Writer` encodes uint8 RGB frames with the sm_90a encoder of csrc/h264.cu and writes an MP4
-(next3d_b200.mp4).  The stream is Constrained Baseline (profile 66): 4:2:0 BT.601 limited range, CAVLC, a constant QP, one slice
-per macroblock row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip with integer-pel motion, no deblocking
-(DESIGN.md section 3.5).  This module also writes the SPS and PPS, for the encoder and its numpy restatement alike; the slice
-headers are written by the kernels."""
+(next3d_b200.mp4).  The stream is Constrained Baseline (profile 66): 4:2:0 BT.601 limited range, CAVLC, one slice per macroblock
+row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip.  Two streams (DESIGN.md section 3.5):
+  * constant QP (the default): integer-pel motion, no deblocking;
+  * with a `bitrate`: QP per picture from a rate controller on the device, quarter-sample motion and in-loop deblocking.
+This module also writes the SPS and PPS, for the encoder and its numpy restatements alike; the slice headers are written by the
+kernels."""
 import fractions
+import re
 
 import numpy as np
 import torch
@@ -15,15 +18,37 @@ LEVELS = [(10, 1485, 99), (11, 3000, 396), (12, 6000, 396), (13, 11880, 396), (2
           (22, 20250, 1620), (30, 40500, 1620), (31, 108000, 3600), (32, 216000, 5120), (40, 245760, 8192), (41, 245760, 8192),
           (42, 522240, 8704), (50, 589824, 22080), (51, 983040, 36864), (52, 2073600, 36864), (60, 4177920, 139264),
           (61, 8355840, 139264), (62, 16711680, 139264)]
+# Table A-1 MaxBR per level, in 1000 bits/s (cpbBrVclFactor of the Baseline profile)
+MAX_BR = {10: 64, 11: 192, 12: 384, 13: 768, 20: 2000, 21: 4000, 22: 4000, 30: 10000, 31: 14000, 32: 20000, 40: 20000, 41: 50000,
+          42: 50000, 50: 135000, 51: 240000, 52: 240000, 60: 240000, 61: 480000, 62: 800000}
 
 
-def level_idc(width, height, fps):
-    """Smallest level whose MaxFS, MaxMBPS and frame-dimension limits (width, height <= sqrt(8 * MaxFS) macroblocks) fit."""
+def level_idc(width, height, fps, bitrate=None):
+    """Smallest level whose MaxFS, MaxMBPS and frame-dimension limits (width, height <= sqrt(8 * MaxFS) macroblocks) fit, and
+    with a bitrate (bits/s) its MaxBR."""
     mbw, mbh = (width + 15) // 16, (height + 15) // 16
     for lev, mbps, fs in LEVELS:
-        if mbw * mbh <= fs and mbw * mbw <= 8 * fs and mbh * mbh <= 8 * fs and mbw * mbh * fps <= mbps:
+        if mbw * mbh <= fs and mbw * mbw <= 8 * fs and mbh * mbh <= 8 * fs and mbw * mbh * fps <= mbps and \
+                (bitrate is None or bitrate <= 1000 * MAX_BR[lev]):
             return lev
-    raise ValueError(f'{width}x{height} at {fps} frames/s exceeds H.264 level 6.2')
+    raise ValueError(f'{width}x{height} at {fps} frames/s' + ('' if bitrate is None else f' and {bitrate} bits/s')
+                     + ' exceeds H.264 level 6.2')
+
+
+def parse_bitrate(rate):
+    """Bits/s from an int or an FFmpeg-style string ('10M', '800k', '1.5M', '2000000'); refuses a non-positive rate."""
+    if isinstance(rate, str):
+        m = re.fullmatch(r'\s*(\d+(?:\.\d*)?|\.\d+)\s*([kKMG]?)\s*', rate)
+        if not m:
+            raise ValueError(f'bitrate {rate!r}: expected bits/s such as 12000000, 800k or 10M')
+        bits = round(float(m.group(1)) * {'': 1, 'k': 10 ** 3, 'K': 10 ** 3, 'M': 10 ** 6, 'G': 10 ** 9}[m.group(2)])
+    elif isinstance(rate, (int, np.integer)) and not isinstance(rate, bool):
+        bits = int(rate)
+    else:
+        raise ValueError(f'bitrate {rate!r}: expected an int (bits/s) or a string such as 10M')
+    if bits <= 0:
+        raise ValueError(f'bitrate must be positive, got {rate!r}')
+    return bits
 
 
 class _Bits:
@@ -62,14 +87,14 @@ def _fps_fraction(fps):
     return f
 
 
-def sps(width, height, fps):
-    """Sequence parameter set NAL unit (no start code)."""
+def sps(width, height, fps, bitrate=None):
+    """Sequence parameter set NAL unit (no start code); the level also covers `bitrate` (bits/s) when given."""
     mbw, mbh = (width + 15) // 16, (height + 15) // 16
     f = _fps_fraction(fps)
     b = _Bits()
     b.u(66, 8)                                       # profile_idc: Baseline
     b.u(0b11000000, 8)                               # constraint_set0/1: Constrained Baseline
-    b.u(level_idc(width, height, float(f)), 8)
+    b.u(level_idc(width, height, float(f), bitrate), 8)
     b.ue(0)                                          # seq_parameter_set_id
     b.ue(0)                                          # log2_max_frame_num_minus4: frame_num is 4 bits
     b.ue(2)                                          # pic_order_cnt_type 2: output order = decoding order
@@ -116,7 +141,8 @@ def sps(width, height, fps):
 
 
 def pps(qp):
-    """Picture parameter set NAL unit: CAVLC, pic_init_qp = qp, deblocking control present (the slices disable it)."""
+    """Picture parameter set NAL unit: CAVLC, pic_init_qp = qp, deblocking control present (constant-QP slices disable the
+    filter; the rate-controlled stream uses pps(26) and sets each slice's QP and filter)."""
     b = _Bits()
     b.ue(0)                                          # pic_parameter_set_id
     b.ue(0)                                          # seq_parameter_set_id
@@ -136,24 +162,32 @@ def pps(qp):
     return b.nal(0x68)
 
 
-def check_args(width, height, fps, qp, gop):
+def check_args(width, height, fps, qp, gop, bitrate=None):
     if width <= 0 or height <= 0 or width % 2 or height % 2:
         raise ValueError(f'4:2:0 needs even, positive frame dimensions, got {width}x{height}')
     if not 0 <= qp <= 51:
         raise ValueError(f'qp must be in 0..51, got {qp}')
     if gop < 1:
         raise ValueError(f'gop must be at least 1, got {gop}')
-    level_idc(width, height, float(_fps_fraction(fps)))
+    level_idc(width, height, float(_fps_fraction(fps)), bitrate)
 
 
 class H264Writer:
     """Encode uint8 RGB frames [H, W, 3] (numpy arrays or CUDA tensors, one frame or a batch [N, H, W, 3]) into an MP4 file at
     `path`, in order, on a stream of the writer's own.  qp: constant quantiser 0..51 (lower = larger file, closer to the input);
     gop: an IDR frame every `gop` frames.  CUDA frames are read in place; numpy frames are copied to the device.  The encoded
-    frames reach the host every `batch` frames in one pinned copy.  Use as a context manager, or call close()."""
+    frames reach the host every `batch` frames in one pinned copy.  Use as a context manager, or call close().
 
-    def __init__(self, path, width, height, fps, qp=18, gop=60, device=None, batch=8):
-        check_args(width, height, fps, qp, gop)
+    bitrate (bits/s: an int, or a string such as '10M' or '800k'): the rate-controlled stream instead, with qp ignored.  Its
+    controller runs on the device (no extra host synchronisation) and keeps each picture's QP within qp_range (min, max);
+    equal bounds pin the QP.  `recon` is then the deblocked picture."""
+
+    def __init__(self, path, width, height, fps, qp=18, gop=60, device=None, batch=8, bitrate=None, qp_range=(0, 51)):
+        self.bitrate = None if bitrate is None else parse_bitrate(bitrate)
+        check_args(width, height, fps, qp, gop, self.bitrate)
+        qp_min, qp_max = (int(q) for q in qp_range)
+        if not 0 <= qp_min <= qp_max <= 51:
+            raise ValueError(f'qp_range must satisfy 0 <= min <= max <= 51, got {qp_range}')
         self.width, self.height, self.qp, self.gop = int(width), int(height), int(qp), int(gop)
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.type != 'cuda':
@@ -171,11 +205,19 @@ class H264Writer:
             self._scratch, self._slices = new(scratch_bytes), new(slice_bytes)
             self._samples = new(self.batch * self.sample_cap)
             self._lens = torch.zeros(self.batch, dtype=torch.int64, device=self.device)
+            self._rc = None
+            if self.bitrate is not None:
+                f = _fps_fraction(fps)
+                self._rc = torch.empty(_lib.H264_RC_STATE_BYTES // 8, dtype=torch.int64, device=self.device)
+                self.stream.wait_stream(torch.cuda.current_stream(self.device))      # the allocation, before the writer's stream
+                _lib.check(_lib.lib.n3d_h264_rc_init(self._rc.data_ptr(), self.width, self.height, self.bitrate, f.numerator, f.denominator,
+                                                     qp_min, qp_max, self.stream.cuda_stream), 'n3d_h264_rc_init')
         self._lens_host = torch.empty(self.batch, dtype=torch.int64, pin_memory=True)
         self._host = torch.empty(0, dtype=torch.uint8)
         self._pending = []                                   # IDR flag of each frame encoded since the last flush
         self.frames = 0
-        self._mp4 = mp4.Mp4Writer(path, self.width, self.height, _fps_fraction(fps), sps(self.width, self.height, fps), pps(self.qp))
+        self._mp4 = mp4.Mp4Writer(path, self.width, self.height, _fps_fraction(fps), sps(self.width, self.height, fps, self.bitrate),
+                                  pps(self.qp if self._rc is None else 26))
 
     def write(self, frames):
         if isinstance(frames, np.ndarray):
@@ -201,11 +243,13 @@ class H264Writer:
         k = self.frames % self.gop
         slot = len(self._pending)
         ref, rec = self._planes[self.frames % 2], self._planes[(self.frames + 1) % 2]
-        _lib.check(_lib.lib.n3d_h264_encode(
-            frame.data_ptr(), self.width, self.height, self.qp, int(k == 0), k % 16, (self.frames // self.gop) % 2,
-            self._cur.data_ptr(), None if k == 0 else ref.data_ptr(), rec.data_ptr(), self._scratch.data_ptr(),
-            self._slices.data_ptr(), self._samples[slot * self.sample_cap:].data_ptr(), self._lens[slot:].data_ptr(),
-            self.stream.cuda_stream), 'n3d_h264_encode')
+        fn, name = ((_lib.lib.n3d_h264_encode, 'n3d_h264_encode') if self._rc is None else
+                    (_lib.lib.n3d_h264_encode_rc, 'n3d_h264_encode_rc'))
+        _lib.check(fn(
+            frame.data_ptr(), self.width, self.height, self.qp if self._rc is None else self._rc.data_ptr(), int(k == 0), k % 16,
+            (self.frames // self.gop) % 2, self._cur.data_ptr(), None if k == 0 else ref.data_ptr(), rec.data_ptr(),
+            self._scratch.data_ptr(), self._slices.data_ptr(), self._samples[slot * self.sample_cap:].data_ptr(),
+            self._lens[slot:].data_ptr(), self.stream.cuda_stream), name)
         self._pending.append(k == 0)
         self.frames += 1
         if len(self._pending) == self.batch:
@@ -237,8 +281,8 @@ class H264Writer:
 
     @property
     def recon(self):
-        """Reconstruction of the last frame, as the decoder outputs it before cropping: padded (Y [H16, W16], Cb, Cr
-        [H16/2, W16/2]) uint8 CUDA tensors (copies)."""
+        """Reconstruction of the last frame, as the decoder outputs it before cropping (deblocked in the rate-controlled
+        stream): padded (Y [H16, W16], Cb, Cr [H16/2, W16/2]) uint8 CUDA tensors (copies)."""
         if self.frames == 0:
             return None
         self.stream.synchronize()
