@@ -423,10 +423,14 @@ int n3d_parse_float_table(const char* text, int64_t len, float* values, int64_t 
 
 /* ------------------------------------------------------------------------------------------------------------
  * H.264 encoder (next3d_b200/video.py; DESIGN.md section 3): Constrained Baseline (profile_idc 66), 8-bit 4:2:0 BT.601 limited
- * range, CAVLC, constant QP, one slice per macroblock row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip
- * with integer-pel motion against the previous frame, deblocking disabled (so the reconstruction is the decoder's output).
- * Stateless: the caller owns the reconstruction buffers and carries the reference from frame to frame.  The SPS / PPS are
- * written by the caller (next3d_b200.video.sps / pps: log2_max_frame_num 4, pic_order_cnt_type 2, pic_init_qp = qp).
+ * range, CAVLC, one slice per macroblock row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip predicted from
+ * the previous frame.  Two streams share the buffers and the argument checks:
+ *   constant QP (n3d_h264_encode): integer-pel motion, deblocking disabled (so the reconstruction is the decoder's output);
+ *   rate-controlled (n3d_h264_encode_rc): one QP per picture chosen on the device, quarter-sample motion, in-loop deblocking.
+ * In both, recon receives the decoder's output picture, which the caller passes back as the next P frame's ref.  The caller
+ * owns the reconstruction buffers (and the controller state); the encoder keeps nothing between calls.  The SPS / PPS are
+ * written by the caller (next3d_b200.video.sps / pps: log2_max_frame_num 4, pic_order_cnt_type 2, pic_init_qp = qp for the
+ * constant-QP stream and 26 for the rate-controlled one).
  * ---------------------------------------------------------------------------------------------------------- */
 
 /* Host only.  Buffer sizes in bytes for width x height frames: plane_bytes = one padded I420 picture (width and height rounded

@@ -15,7 +15,8 @@
 //   h264_deblock      in-loop deblocking (8.7) in place on the reconstruction: one warp per MB row, rows taken in order through an
 //                     atomic ticket, MB x of a row waiting until the row above has finished MB x + 1 (the standard's raster order).
 //   h264_rc_update    one thread: the frame's size -> the controller state and the next picture's QP.
-// The numpy restatements in tests/h264_oracle.py and tests/h264_rc_oracle.py make the same decisions and write the same bytes.
+// The numpy restatement in tests/h264_oracle.py (Encoder, RcEncoder: kRc false, true) makes the same decisions and writes the
+// same bytes.
 #include "common.cuh"
 
 namespace {
@@ -111,7 +112,8 @@ __constant__ uint8_t c_run_bits[7][15] = {{1, 0}, {1, 1, 0}, {3, 2, 1, 0}, {3, 2
                                           {7, 6, 5, 4, 3, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1}};
 
 struct Frame {
-    int W, H, W16, H16, mbw, mbh, qp, qpc;
+    int W, H, W16, H16, mbw, mbh;
+    int qp;                    // the constant-QP stream's QP (kRc kernels read the picture's QP from rc)
     const uint8_t* rgb;
     uint8_t* cur;              // padded I420 of the input
     const uint8_t* ref;        // padded I420 reconstruction of the previous frame (P)
@@ -119,13 +121,17 @@ struct Frame {
     MbRec* mbs;
     int32_t* lens;             // bytes per slot, -1 when the slot overflowed
     int32_t* dbk;              // h264_deblock: [0] row ticket, [1 + r] MBs of row r filtered (reset on the stream per frame)
-    int64_t* rc;               // rate-control state (kRc kernels read the picture's QP from it)
+    int64_t* rc;               // rate-control state
     uint8_t* slots;
     int64_t slot_cap;
     int idr, frame_num, idr_pic_id;
-    __device__ uint8_t* plane(uint8_t* base, int c) const { return base + (c == 0 ? 0 : (int64_t)W16 * H16 + (int64_t)(c - 1) * (W16 / 2) * (H16 / 2)); }
-    __device__ const uint8_t* cplane(const uint8_t* base, int c) const { return base + (c == 0 ? 0 : (int64_t)W16 * H16 + (int64_t)(c - 1) * (W16 / 2) * (H16 / 2)); }
+    template <class T>         // component c (0 Y, 1 Cb, 2 Cr) of the padded I420 picture at base
+    __device__ T* plane(T* base, int c) const { return base + (c == 0 ? 0 : (int64_t)W16 * H16 + (int64_t)(c - 1) * (W16 / 2) * (H16 / 2)); }
 };
+
+// The picture's QP: the constant one, or the controller's choice for this picture.
+template <bool kRc>
+__device__ __forceinline__ int pic_qp(const Frame& F) { return kRc ? (int)F.rc[kRcQp] : F.qp; }
 
 // ------------------------------------------------------------------------------------------------ transforms and quantisation
 __device__ __forceinline__ int cls4(int r) { const int i = r >> 2, j = r & 3; return ((i | j) & 1) == 0 ? 0 : ((i & j) & 1) ? 1 : 2; }
@@ -233,9 +239,9 @@ __global__ void __launch_bounds__(32) h264_intra_rows(Frame F) {
     __shared__ int s_cdc[2][4], s_dcc[2][4], s_dcy[16];
     __shared__ int s_left[16];
     const int row = blockIdx.x, lane = threadIdx.x;
-    const int qp = kRc ? (int)F.rc[kRcQp] : F.qp, qpc = kRc ? c_qpc[qp] : F.qpc;
+    const int qp = pic_qp<kRc>(F), qpc = c_qpc[qp];
     const int cw = F.W16 / 2;
-    const uint8_t* Ys = F.cplane(F.cur, 0);
+    const uint8_t* Ys = F.plane(F.cur, 0);
     uint8_t* Yr = F.plane(F.rec, 0);
     for (int mbx = 0; mbx < F.mbw; ++mbx) {
         MbRec* R = F.mbs + (int64_t)row * F.mbw + mbx;
@@ -272,7 +278,7 @@ __global__ void __launch_bounds__(32) h264_intra_rows(Frame F) {
             }
             fwd4(w, s_w[lane]);
         } else if (lane < 24) {
-            const uint8_t* Cs = F.cplane(F.cur, comp);
+            const uint8_t* Cs = F.plane(F.cur, comp);
             const uint8_t* Cr = F.plane(F.rec, comp);
             int p = 128;
             if (mbx) {
@@ -386,10 +392,10 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
     __shared__ unsigned long long s_best[8];
     __shared__ int s_cdc[2][4], s_dcc[2][4];
     const int mbx = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
-    const int qp = kRc ? (int)F.rc[kRcQp] : F.qp, qpc = kRc ? c_qpc[qp] : F.qpc;
+    const int qp = pic_qp<kRc>(F), qpc = c_qpc[qp];
     const int x0 = 16 * mbx, y0 = 16 * row;
-    const uint8_t* Yref = F.cplane(F.ref, 0);
-    const uint8_t* Ys = F.cplane(F.cur, 0);
+    const uint8_t* Yref = F.plane(F.ref, 0);
+    const uint8_t* Ys = F.plane(F.cur, 0);
     for (int i = tid; i < kWin * kWin; i += 256) {
         const int y = min(max(y0 - kSearch + i / kWin, 0), F.H16 - 1), x = min(max(x0 - kSearch + i % kWin, 0), F.W16 - 1);
         s_win[i / kWin][i % kWin] = Yref[(int64_t)y * F.W16 + x];
@@ -408,27 +414,24 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
 #pragma unroll
             for (int x = 0; x < 16; ++x) sad += abs((int)s_cur[y][x] - (int)wr[x]);
         }
-        const unsigned long long cost = (unsigned long long)(sad + lam * (ue_bits(se_code(4 * mx)) + ue_bits(se_code(4 * my))));
-        const unsigned long long key = (cost << 24) | ((unsigned long long)(abs(mx) + abs(my)) << 16) | ((unsigned long long)(my + kSearch) << 8) | (unsigned long long)(mx + kSearch);
-        best = min(best, key);
+        best = min(best, mv_key(sad + lam * (ue_bits(se_code(4 * mx)) + ue_bits(se_code(4 * my))), 4 * mx, 4 * my));
     }
     for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
     if ((tid & 31) == 0) s_best[tid >> 5] = best;
     __syncthreads();
     best = s_best[0];
     for (int i = 1; i < 8; ++i) best = min(best, s_best[i]);
-    const int mvy = (int)((best >> 8) & 0xff) - kSearch, mvx = (int)(best & 0xff) - kSearch;
+    int qx = (int)(best & 0xff) - kMvOff, qy = (int)((best >> 8) & 0xff) - kMvOff;
+    const int mvx = qx / 4, mvy = qy / 4;                // the integer-pel vector
     // quarter-sample refinement (rate-controlled stream): the 8 half-sample neighbours of the integer vector, then the 8
     // quarter-sample neighbours of the best of those, same cost and tie order; one warp per candidate over a haloed patch
     __shared__ uint8_t s_pat[kRc ? kPat : 1][kPat];
     __shared__ unsigned long long s_key[8];
-    int qx = 4 * mvx, qy = 4 * mvy;
     if constexpr (kRc) {
         for (int i = tid; i < kPat * kPat; i += 256) {
             const int y = min(max(y0 + mvy - 3 + i / kPat, 0), F.H16 - 1), x = min(max(x0 + mvx - 3 + i % kPat, 0), F.W16 - 1);
             s_pat[i / kPat][i % kPat] = Yref[(int64_t)y * F.W16 + x];
         }
-        best = mv_key((int)(best >> 24), qx, qy);
         __syncthreads();
         const int warp = tid >> 5, lane32 = tid & 31;
         for (int step = 2; step >= 1; --step) {
@@ -469,8 +472,8 @@ __global__ void __launch_bounds__(256) h264_inter_mbs(Frame F) {
             Yr[(int64_t)(y0 + 4 * by + (r >> 2)) * F.W16 + x0 + 4 * bx + (r & 3)] = (uint8_t)clip255(pred[r] + res[r]);
     } else if (lane < 24) {                              // chroma: eighth-pel bilinear at the luma MV (8.4.2.2.2)
         const int mvcx = qx, mvcy = qy, fx = mvcx & 7, fy = mvcy & 7;      // chroma eighth samples = luma quarter samples
-        const uint8_t* Cref = F.cplane(F.ref, comp);
-        const uint8_t* Cs = F.cplane(F.cur, comp);
+        const uint8_t* Cref = F.plane(F.ref, comp);
+        const uint8_t* Cs = F.plane(F.cur, comp);
         for (int r = 0; r < 16; ++r) {
             const int yy = 8 * row + 4 * by + (r >> 2), xx = 8 * mbx + 4 * bx + (r & 3);
             const int ry = yy + (mvcy >> 3), rx = xx + (mvcx >> 3);
@@ -579,7 +582,7 @@ __global__ void __launch_bounds__(32) h264_deblock(Frame F) {
     if (lane == 0) s_row = atomicAdd(F.dbk, 1);
     __syncwarp();
     const int row = s_row;
-    const int qp = (int)F.rc[kRcQp], qpc = c_qpc[qp];
+    const int qp = pic_qp<true>(F), qpc = c_qpc[qp];
     const bool intra = F.idr;
     volatile int32_t* done = F.dbk + 1;
     const int cw = F.W16 / 2;
@@ -775,7 +778,7 @@ __global__ void h264_write_rows(Frame F) {
     bw.u(0, 1);                              // no_output_of_prior_pics_flag / adaptive_ref_pic_marking_mode_flag
     if (idr) bw.u(0, 1);                     // long_term_reference_flag
     if (kRc) {
-        bw.se((int)F.rc[kRcQp] - 26);        // slice_qp_delta (pic_init_qp 26)
+        bw.se(pic_qp<kRc>(F) - 26);          // slice_qp_delta (pic_init_qp 26)
         bw.ue(0);                            // disable_deblocking_filter_idc: filter, across slice boundaries too
         bw.se(0);                            // slice_alpha_c0_offset_div2
         bw.se(0);                            // slice_beta_offset_div2
@@ -914,6 +917,27 @@ extern "C" int n3d_h264_buffer_sizes(int width, int height, int64_t* plane_bytes
 
 namespace {
 
+// The kernels of one frame, in stream order; the rate-controlled stream adds the deblocking filter and the controller update.
+template <bool kRc>
+int launch(const char* name, const Frame& F, uint8_t* sample, int64_t* sample_len, cudaStream_t s) {
+    h264_rgb_to_yuv<<<n3d_grid((int64_t)F.W16 * F.H16 / 4, 256), 256, 0, s>>>(F);
+    if (F.idr) h264_intra_rows<kRc><<<F.mbh, 32, 0, s>>>(F);
+    else h264_inter_mbs<kRc><<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
+    if constexpr (kRc) {
+        const cudaError_t e = cudaMemsetAsync(F.dbk, 0, 4 * (F.mbh + 1), s);          // deblocking counters, per frame
+        if (e != cudaSuccess) {
+            n3d_set_error("%s: resetting the deblocking counters failed: %s", name, cudaGetErrorString(e));
+            return N3D_ERR_CUDA;
+        }
+        h264_deblock<<<F.mbh, 32, 0, s>>>(F);
+    }
+    h264_write_rows<kRc><<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
+    h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
+    if constexpr (kRc) h264_rc_update<<<1, 1, 0, s>>>(F.rc, sample_len, F.idr);
+    N3D_CHECK_LAUNCH(name);
+    return N3D_OK;
+}
+
 // Shared by both entry points: rc == nullptr runs the constant-QP stream at qp, else the rate-controlled stream.
 int encode(const char* name, const uint8_t* rgb, int width, int height, int qp, int64_t* rc, int idr, int frame_num, int idr_pic_id,
            uint8_t* cur, const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
@@ -931,9 +955,6 @@ int encode(const char* name, const uint8_t* rgb, int width, int height, int qp, 
     F.mbw = (width + 15) / 16; F.mbh = (height + 15) / 16;
     F.W16 = 16 * F.mbw; F.H16 = 16 * F.mbh;
     F.qp = qp;
-    static const int qpc[52] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29,
-                                29, 30, 31, 32, 32, 33, 34, 34, 35, 35, 36, 36, 37, 37, 37, 38, 38, 38, 39, 39, 39, 39};
-    F.qpc = qpc[qp];
     F.rgb = rgb; F.cur = cur; F.ref = ref; F.rec = recon;
     F.mbs = (MbRec*)scratch;
     F.lens = (int32_t*)((uint8_t*)scratch + (int64_t)sizeof(MbRec) * F.mbw * F.mbh);
@@ -942,27 +963,7 @@ int encode(const char* name, const uint8_t* rgb, int width, int height, int qp, 
     F.slots = slices; F.slot_cap = slot_cap;
     F.idr = idr ? 1 : 0; F.frame_num = frame_num; F.idr_pic_id = idr_pic_id;
     cudaStream_t s = (cudaStream_t)stream;
-    h264_rgb_to_yuv<<<n3d_grid((int64_t)F.W16 * F.H16 / 4, 256), 256, 0, s>>>(F);
-    if (!rc) {
-        if (F.idr) h264_intra_rows<false><<<F.mbh, 32, 0, s>>>(F);
-        else h264_inter_mbs<false><<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
-        h264_write_rows<false><<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
-        h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
-    } else {
-        if (F.idr) h264_intra_rows<true><<<F.mbh, 32, 0, s>>>(F);
-        else h264_inter_mbs<true><<<dim3(F.mbw, F.mbh), 256, 0, s>>>(F);
-        const cudaError_t e = cudaMemsetAsync(F.dbk, 0, 4 * (F.mbh + 1), s);          // deblocking counters, per frame
-        if (e != cudaSuccess) {
-            n3d_set_error("%s: resetting the deblocking counters failed: %s", name, cudaGetErrorString(e));
-            return N3D_ERR_CUDA;
-        }
-        h264_deblock<<<F.mbh, 32, 0, s>>>(F);
-        h264_write_rows<true><<<n3d_div_up(F.mbh, 32), 32, 0, s>>>(F);
-        h264_pack<<<F.mbh, 256, 0, s>>>(F, sample, sample_len);
-        h264_rc_update<<<1, 1, 0, s>>>(rc, sample_len, F.idr);
-    }
-    N3D_CHECK_LAUNCH(name);
-    return N3D_OK;
+    return rc ? launch<true>(name, F, sample, sample_len, s) : launch<false>(name, F, sample, sample_len, s);
 }
 
 }  // namespace

@@ -1,16 +1,21 @@
 """numpy restatement of the sm_90a H.264 encoder (next3d_b200/csrc/h264.cu): the same colour conversion, mode and motion
-decisions, tie-breaks, quantisation and CAVLC, producing the same bytes and the same reconstruction.  Test infrastructure only:
-the CPU tests decode its streams with FFmpeg to prove the byte format, and the GPU tests compare the kernels with it byte for
-byte.  The parameter sets (SPS / PPS) come from next3d_b200.video, which writes them for both encoders.
+decisions, tie-breaks, quantisation, CAVLC, deblocking and rate control, producing the same bytes and the same reconstruction.
+Test infrastructure only: the CPU tests decode its streams with FFmpeg to prove the byte format, and the GPU tests compare the
+kernels with it byte for byte.  The parameter sets (SPS / PPS) come from next3d_b200.video, which writes them for both encoders.
 
 Stream subset (see DESIGN.md section 3.5): Constrained Baseline, one slice per macroblock row, IDR frames of I_16x16 macroblocks
-(DC or horizontal luma prediction, DC chroma), P frames of P_L0_16x16 / P_Skip with integer-pel motion, constant QP, no
-deblocking."""
+(DC or horizontal luma prediction, DC chroma), P frames of P_L0_16x16 / P_Skip.  Two streams, as the kernels' kRc parameter:
+- `Encoder` (n3d_h264_encode): constant QP (pic_init_qp = QP), integer-pel motion, no deblocking.
+- `RcEncoder` (n3d_h264_encode_rc): pic_init_qp 26 with slice_qp_delta = QP - 26 (one QP per picture, chosen by the controller
+  before the picture is coded), vectors refined to quarter samples around the integer search's best vector, and
+  disable_deblocking_filter_idc 0 (the deblocked picture is the output and the next P frame's reference)."""
 import re
 
 import numpy as np
 
 SEARCH = 16                     # integer-pel full search over [-SEARCH, SEARCH]^2 (csrc/h264.cu kSearch)
+PAD = SEARCH + 8                # reference padding: covers the search, the quarter-sample refinement and the 6-tap filter
+MV_OFF = 128                    # key offset of quarter-sample vector components (|mv| <= 4 * SEARCH + 3)
 LEVEL_MAX = 2063                # largest |level| CAVLC codes with level_prefix <= 15 at every suffixLength (Baseline)
 
 LAMBDA = [0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 4, 4, 5, 5, 6, 7, 7, 8, 9, 10, 12, 13, 15,
@@ -177,12 +182,14 @@ def code_chroma(src, pred, qpc, intra):
 
 
 # ------------------------------------------------------------------------------------------------ bit writing
-def ue_bits(k):
-    return 2 * (int(k) + 1).bit_length() - 1
-
-
 def se_code(v):
     return 2 * v - 1 if v > 0 else -2 * v
+
+
+def se_bits(v):
+    """Length of se(v) for an array of values."""
+    k = np.where(v > 0, 2 * v - 1, -2 * v)
+    return 2 * np.frexp(k + 1.0)[1].astype(np.int64) - 1
 
 
 class Bits:
@@ -289,9 +296,20 @@ def _mb_view(p, s):
     return p.reshape(R, s, C, s).swapaxes(1, 2)
 
 
+def mv_key(cost, qx, qy):
+    """Search key of a vector (qx, qy) in quarter samples: the smallest key has the smallest cost, then the smallest |mv|_1, then
+    the smallest (mvy, mvx) (csrc/h264.cu mv_key)."""
+    return (cost << 24) | ((np.abs(qx) + np.abs(qy)) << 16) | ((qy + MV_OFF) << 8) | (qx + MV_OFF)
+
+
+def mv_of(key):
+    """(qx, qy) of mv_key keys."""
+    return (key & 0xff) - MV_OFF, ((key >> 8) & 0xff) - MV_OFF
+
+
 class Encoder:
-    """Encodes uint8 RGB frames into length-prefixed slice NAL units, one sample per frame.  The first frame and every gop-th one
-    after it is IDR."""
+    """The constant-QP stream: encodes uint8 RGB frames into length-prefixed slice NAL units, one sample per frame.  The first
+    frame and every gop-th one after it is IDR."""
 
     def __init__(self, width, height, qp=18, gop=60):
         if width % 2 or height % 2 or width <= 0 or height <= 0:
@@ -300,8 +318,9 @@ class Encoder:
         self.mbw, self.mbh = (width + 15) // 16, (height + 15) // 16
         self.n = 0
         self.recon = None                     # (Y, Cb, Cr) padded planes of the last frame
-        self.mvs = None                       # [mbh, mbw, 2] integer-pel MVs of the last P frame
+        self.mvs = None                       # [mbh, mbw, 2] MVs of the last P frame in quarter samples
         self.skip = None                      # [mbh, mbw] bool
+        self.levels = None                    # [mbh, mbw, 16, 4, 4] luma levels of the last P frame (luma4x4BlkIdx order)
 
     # ---------------------------------------------------------------- decisions and reconstruction
     def _intra(self, Y, U, V):
@@ -357,6 +376,34 @@ class Encoder:
                                  cdc=[cres[0][0][r], cres[1][0][r]], cac=[cres[0][1][r], cres[1][1][r]])
         return mbs, (ry, ru, rv)
 
+    def _integer_search(self, G, cur):
+        """Integer-pel full search over [-SEARCH, SEARCH]^2 of every MB of cur [H16, W16] against G, the reference luma padded by
+        PAD with its edge samples (the decoder's clamped coordinates).  cost = SAD + lambda * bits of the MV against a zero
+        predictor (so that MBs are decided independently).  Returns the best mv_key per MB [mbh, mbw]."""
+        S, R, C = SEARCH, self.mbh, self.mbw
+        H16, W16 = 16 * R, 16 * C
+        lam = LAMBDA[self.qp]
+        mx = 4 * np.arange(-S, S + 1)[:, None, None]
+        G, cur = G.astype(np.int16), cur.astype(np.int16)           # differences of samples fit: 4x less memory than int64
+        best = np.full((R, C), np.iinfo(np.int64).max, np.int64)
+        for my in range(-S, S + 1):                   # all mx at once
+            rows = G[PAD + my:PAD + my + H16, PAD - S:PAD + S + W16]
+            shifted = np.lib.stride_tricks.sliding_window_view(rows, W16, 1).swapaxes(0, 1)              # [mx, H16, W16]
+            sad = np.abs(cur - shifted).reshape(2 * S + 1, R, 16, C, 16).sum((2, 4), dtype=np.int64)
+            cost = sad + lam * (se_bits(mx) + se_bits(4 * my))
+            np.minimum(best, mv_key(cost, mx, 4 * my).min(0), out=best)
+        return best
+
+    def _search(self, ry, cur):
+        """Motion search of every MB against the reference luma ry: (mvx, mvy [mbh, mbw] in quarter samples, luma prediction
+        [mbh, mbw, 16, 16])."""
+        G = np.pad(ry, PAD, mode='edge')
+        qx, qy = mv_of(self._integer_search(G, cur))
+        R, C = self.mbh, self.mbw
+        yy = PAD + 16 * np.arange(R)[:, None, None, None] + np.arange(16)[None, None, :, None] + (qy >> 2)[:, :, None, None]
+        xx = PAD + 16 * np.arange(C)[None, :, None, None] + np.arange(16)[None, None, None, :] + (qx >> 2)[:, :, None, None]
+        return qx, qy, G[yy, xx]
+
     def _inter(self, Y, U, V):
         """P_L0_16x16 / P_Skip for every MB at once against the previous reconstruction."""
         qp, qpc = self.qp, QPC[self.qp]
@@ -364,31 +411,14 @@ class Encoder:
         H16, W16 = 16 * R, 16 * C
         ry, ru, rv = (p.astype(np.int64) for p in self.recon)
         cur = Y.astype(np.int64)
-        padded = np.pad(ry, SEARCH, mode='edge')
-        lam = LAMBDA[qp]
-        best = np.full((R, C), np.iinfo(np.int64).max, np.int64)
-        for my in range(-SEARCH, SEARCH + 1):
-            for mx in range(-SEARCH, SEARCH + 1):
-                shifted = padded[SEARCH + my:SEARCH + my + H16, SEARCH + mx:SEARCH + mx + W16]
-                sad = _mb_view(np.abs(cur - shifted), 16).sum((-1, -2))
-                cost = sad + lam * (ue_bits(se_code(4 * mx)) + ue_bits(se_code(4 * my)))
-                key = (cost << 24) | ((abs(mx) + abs(my)) << 16) | ((my + SEARCH) << 8) | (mx + SEARCH)
-                np.minimum(best, key, out=best)
-        mvy = ((best >> 8) & 0xff) - SEARCH
-        mvx = (best & 0xff) - SEARCH
-        # luma prediction: integer-pel, reference coordinates clamped to the picture
-        yy = np.arange(16)[None, None, :, None] + 16 * np.arange(R)[:, None, None, None] + mvy[:, :, None, None]
-        xx = np.arange(16)[None, None, None, :] + 16 * np.arange(C)[None, :, None, None] + mvx[:, :, None, None]
-        pred = ry[np.clip(yy, 0, H16 - 1), np.clip(xx, 0, W16 - 1)]
-        src = _mb_view(cur, 16)
-        w = fwd4(blocks(src - pred))
+        qx, qy, pred = self._search(ry, cur)
+        w = fwd4(blocks(_mb_view(cur, 16) - pred))
         lvl = quant(w, qp, False)                                             # [R, C, 16, 4, 4]
         rec_y = np.clip(pred + unblocks(inv4(dequant(lvl, qp))), 0, 255)
-        # chroma: eighth-pel bilinear (8.4.2.2.2) at the luma MV in quarter-pel units
-        mvcx, mvcy = 4 * mvx, 4 * mvy
-        fx, fy = (mvcx & 7)[:, :, None, None], (mvcy & 7)[:, :, None, None]
-        cy = np.arange(8)[None, None, :, None] + 8 * np.arange(R)[:, None, None, None] + (mvcy >> 3)[:, :, None, None]
-        cx = np.arange(8)[None, None, None, :] + 8 * np.arange(C)[None, :, None, None] + (mvcx >> 3)[:, :, None, None]
+        # chroma: eighth-sample bilinear (8.4.2.2.2) at the luma vector, whose quarter samples are chroma eighth samples
+        fx, fy = (qx & 7)[:, :, None, None], (qy & 7)[:, :, None, None]
+        cy = np.arange(8)[None, None, :, None] + 8 * np.arange(R)[:, None, None, None] + (qy >> 3)[:, :, None, None]
+        cx = np.arange(8)[None, None, None, :] + 8 * np.arange(C)[None, :, None, None] + (qx >> 3)[:, :, None, None]
         cres, crec = [], []
         for sp, rp in ((U, ru), (V, rv)):
             at = lambda y, x: rp[np.clip(y, 0, H16 // 2 - 1), np.clip(x, 0, W16 // 2 - 1)]
@@ -399,14 +429,19 @@ class Encoder:
             crec.append(rec_c)
         nonzero = (lvl != 0).any((-1, -2, -3)) | (cres[0][0] != 0).any(-1) | (cres[0][1] != 0).any((-1, -2)) \
             | (cres[1][0] != 0).any(-1) | (cres[1][1] != 0).any((-1, -2))
-        skip = (mvx == 0) & (mvy == 0) & ~nonzero
-        mbs = [[dict(intra=False, skip=bool(skip[r, c]), mv=(int(mvx[r, c]), int(mvy[r, c])), lac=scan(lvl[r, c]),
+        skip = (qx == 0) & (qy == 0) & ~nonzero
+        mbs = [[dict(intra=False, skip=bool(skip[r, c]), mv=(int(qx[r, c]), int(qy[r, c])), lac=scan(lvl[r, c]),
                      cdc=[cres[0][0][r, c], cres[1][0][r, c]], cac=[cres[0][1][r, c], cres[1][1][r, c]])
                 for c in range(C)] for r in range(R)]
-        self.mvs, self.skip = np.stack([mvx, mvy], -1), skip
+        self.mvs, self.skip, self.levels = np.stack([qx, qy], -1), skip, lvl
         return mbs, (rec_y, crec[0], crec[1])
 
     # ---------------------------------------------------------------- syntax
+    def _slice_qp_and_deblocking(self, bw):
+        """The last fields of the slice header."""
+        bw.se(0)                                   # slice_qp_delta (pic_init_qp = QP)
+        bw.ue(1)                                   # disable_deblocking_filter_idc
+
     def _slice(self, row, mbs, idr, frame_num, idr_pic_id):
         bw = Bits()
         bw.ue(row * self.mbw)                      # first_mb_in_slice
@@ -421,8 +456,7 @@ class Encoder:
         bw.u(0, 1)                                 # no_output_of_prior_pics_flag / adaptive_ref_pic_marking_mode_flag
         if idr:
             bw.u(0, 1)                             # long_term_reference_flag
-        bw.se(0)                                   # slice_qp_delta
-        bw.ue(1)                                   # disable_deblocking_filter_idc
+        self._slice_qp_and_deblocking(bw)
         left_tc = [0] * 4                          # TotalCoeff of the left MB's right-column luma blocks (rows 0..3)
         left_cc = [[0, 0], [0, 0]]                 # ... and of its right-column chroma blocks, per component
         skip_run = 0
@@ -450,10 +484,9 @@ class Encoder:
                 residual_block(bw, m['ldc'], left_tc[0] if c else 0)       # Intra16x16DCLevel: nC of block 0
             else:
                 bw.ue(0)                                                    # mb_type P_L0_16x16
-                mv = (4 * m['mv'][0], 4 * m['mv'][1])
-                bw.se(mv[0] - mvp[0])
-                bw.se(mv[1] - mvp[1])
-                mvp = mv
+                bw.se(m['mv'][0] - mvp[0])
+                bw.se(m['mv'][1] - mvp[1])
+                mvp = m['mv']
                 bw.ue(CBP_CODE[cbp_l + 16 * cbp_c])
                 if cbp_l or cbp_c:
                     bw.se(0)                                                # mb_qp_delta
@@ -488,7 +521,7 @@ class Encoder:
         idr = k == 0
         if idr:
             mbs, rec = self._intra(Y, U, V)
-            self.mvs, self.skip = None, None
+            self.mvs, self.skip, self.levels = None, None, None
         else:
             mbs, rec = self._inter(Y, U, V)
         R, C = self.mbh, self.mbw
@@ -510,6 +543,238 @@ def unblocks_dc(dc):
 def blocks_dc(m):
     """Inverse of unblocks_dc."""
     return np.stack([m[..., by, bx] for bx, by in BLK], -1)
+
+
+# ------------------------------------------------------------------------------------------------ quarter-sample luma
+def _tap(p, axis):
+    """6-tap filter (1, -5, 20, 20, -5, 1) between sample k and k + 1 along axis (unscaled; wraps at the borders, which PAD
+    keeps out of use)."""
+    s = lambda k: np.roll(p, -k, axis)
+    return s(-2) - 5 * s(-1) + 20 * s(0) + 20 * s(1) - 5 * s(2) + s(3)
+
+
+def half_planes(y):
+    """Reference luma [H16, W16] -> (G, b, h, j) planes padded by PAD: full samples (edge replication = the decoder's clamped
+    coordinates) and the half-sample positions right of, below, and right of and below each full sample."""
+    G = np.pad(y.astype(np.int64), PAD, mode='edge')
+    b1, h1 = _tap(G, 1), _tap(G, 0)
+    clip = lambda v: np.clip(v, 0, 255)
+    return G, clip((b1 + 16) >> 5), clip((h1 + 16) >> 5), clip((_tap(b1, 0) + 512) >> 10)
+
+
+def luma_pred(P, X4, Y4):
+    """Luma prediction samples at quarter-sample positions (X4, Y4) (arrays, picture coordinates * 4), Table 8-12."""
+    G, B, Hh, J = P
+    x, y = (X4 >> 2) + PAD, (Y4 >> 2) + PAD
+    fx, fy = X4 & 3, Y4 & 3
+    g, hh, m_, b, h, j, m, s = G[y, x], G[y, x + 1], G[y + 1, x], B[y, x], Hh[y, x], J[y, x], Hh[y, x + 1], B[y + 1, x]
+    av = lambda a, c: (a + c + 1) >> 1
+    table = [[g, av(g, b), b, av(hh, b)],
+             [av(g, h), av(b, h), av(b, j), av(b, m)],
+             [h, av(h, j), j, av(j, m)],
+             [av(m_, h), av(h, s), av(j, s), av(m, s)]]
+    out = np.zeros(np.broadcast(X4, Y4).shape, np.int64)
+    for yf in range(4):
+        for xf in range(4):
+            sel = (fx == xf) & (fy == yf)
+            out = np.where(sel, table[yf][xf], out)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ deblocking (8.7)
+# Table 8-16 (alpha', beta') and Table 8-17 (tC0' for bS = 1, 2, 3), indexed by indexA / indexB
+ALPHA = [0] * 16 + [4, 4, 5, 6, 7, 8, 9, 10, 12, 13, 15, 17, 20, 22, 25, 28, 32, 36, 40, 45, 50, 56, 63, 71, 80, 90, 101, 113, 127,
+                    144, 162, 182, 203, 226, 255, 255]
+BETA = [0] * 16 + [2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13, 14, 14, 15, 15, 16, 16, 17,
+                   17, 18, 18]
+TC0 = [(0, 0, 0)] * 17 + [(0, 0, 1)] * 4 + [(0, 1, 1)] * 2 + [(1, 1, 1)] * 4 + [(1, 1, 2)] * 4 + [(1, 2, 3)] * 2 + [
+    (2, 2, 3), (2, 2, 4), (2, 3, 4), (2, 3, 4), (3, 3, 5), (3, 4, 6), (3, 4, 6), (4, 5, 7), (4, 5, 8), (4, 6, 9), (5, 7, 10),
+    (6, 8, 11), (6, 8, 13), (7, 10, 14), (8, 11, 16), (9, 12, 18), (10, 13, 20), (11, 15, 23), (13, 17, 25)]
+
+
+def _filter(s, bS, idx, chroma):
+    """Filter lines across one edge: s [..., 8] luma samples p3..q3, or [..., 4] chroma p1..q1; bS [...]; idx = indexA = indexB."""
+    a, be = ALPHA[idx], BETA[idx]
+    if chroma:
+        p1, p0, q0, q1 = (s[..., k] for k in range(4))
+    else:
+        p3, p2, p1, p0, q0, q1, q2, q3 = (s[..., k] for k in range(8))
+    on = (bS > 0) & (np.abs(p0 - q0) < a) & (np.abs(p1 - p0) < be) & (np.abs(q1 - q0) < be)
+    weak, strong = on & (bS < 4), on & (bS == 4)
+    tc0 = np.array((0,) + TC0[idx])[np.minimum(bS, 3)]
+    out = s.copy()
+    if chroma:
+        tc = tc0 + 1
+    else:
+        ap, aq = np.abs(p2 - p0) < be, np.abs(q2 - q0) < be
+        tc = tc0 + ap + aq
+    delta = np.clip((((q0 - p0) << 2) + (p1 - q1) + 4) >> 3, -tc, tc)
+    w_p0, w_q0 = np.clip(p0 + delta, 0, 255), np.clip(q0 - delta, 0, 255)
+    if chroma:
+        out[..., 1] = np.where(weak, w_p0, np.where(strong, (2 * p1 + p0 + q1 + 2) >> 2, p0))
+        out[..., 2] = np.where(weak, w_q0, np.where(strong, (2 * q1 + q0 + p1 + 2) >> 2, q0))
+        return out
+    w_p1 = np.where(ap, p1 + np.clip((p2 + ((p0 + q0 + 1) >> 1) - (p1 << 1)) >> 1, -tc0, tc0), p1)
+    w_q1 = np.where(aq, q1 + np.clip((q2 + ((p0 + q0 + 1) >> 1) - (q1 << 1)) >> 1, -tc0, tc0), q1)
+    near = np.abs(p0 - q0) < ((a >> 2) + 2)
+    sp, sq = ap & near, aq & near
+    s_p0 = np.where(sp, (p2 + 2 * p1 + 2 * p0 + 2 * q0 + q1 + 4) >> 3, (2 * p1 + p0 + q1 + 2) >> 2)
+    s_p1 = np.where(sp, (p2 + p1 + p0 + q0 + 2) >> 2, p1)
+    s_p2 = np.where(sp, (2 * p3 + 3 * p2 + p1 + p0 + q0 + 4) >> 3, p2)
+    s_q0 = np.where(sq, (p1 + 2 * p0 + 2 * q0 + 2 * q1 + q2 + 4) >> 3, (2 * q1 + q0 + p1 + 2) >> 2)
+    s_q1 = np.where(sq, (p0 + q0 + q1 + q2 + 2) >> 2, q1)
+    s_q2 = np.where(sq, (2 * q3 + 3 * q2 + q1 + q0 + p0 + 4) >> 3, q2)
+    for k, wv, sv in ((1, p2, s_p2), (2, w_p1, s_p1), (3, w_p0, s_p0), (4, w_q0, s_q0), (5, w_q1, s_q1), (6, q2, s_q2)):
+        out[..., k] = np.where(weak, wv, np.where(strong, sv, s[..., k]))
+    return out
+
+
+def boundary_strength(intra, nz, mv):
+    """bS of the vertical (left, then internal) and horizontal (top, then internal) luma edges of every MB: [R, C, edge, 4]
+    (index along the edge in 4x4 blocks).  intra: the picture is intra; nz [R, C, 4, 4] (by, bx): the luma 4x4 block has
+    nonzero levels; mv [R, C, 2] quarter samples.  Picture borders get 0."""
+    R, C = nz.shape[:2]
+    bv, bh = np.zeros((R, C, 4, 4), np.int64), np.zeros((R, C, 4, 4), np.int64)
+    if intra:
+        bv[:, :, 1:], bh[:, :, 1:] = 3, 3
+        bv[:, 1:, 0], bh[1:, :, 0] = 4, 4
+        return bv, bh
+    for e in range(1, 4):
+        bv[:, :, e] = 2 * (nz[:, :, :, e - 1] | nz[:, :, :, e])
+        bh[:, :, e] = 2 * (nz[:, :, e - 1, :] | nz[:, :, e, :])
+    mvd = lambda a, c: (np.abs(a - c) >= 4).any(-1)[..., None]
+    bv[:, 1:, 0] = np.where(nz[:, 1:, :, 0] | nz[:, :-1, :, 3], 2, mvd(mv[:, 1:], mv[:, :-1]))
+    bh[1:, :, 0] = np.where(nz[1:, :, 0, :] | nz[:-1, :, 3, :], 2, mvd(mv[1:], mv[:-1]))
+    return bv, bh
+
+
+def deblock(planes, qp, bv, bh):
+    """In-place deblocking of padded (Y, Cb, Cr) int64 planes in the standard's order (per MB in raster order: vertical edges
+    left to right, then horizontal edges top to bottom), run on the MBs of one wavefront x + 2y at a time: an MB's filtering only
+    touches samples that the MBs to its left and above-right finished with."""
+    Y, U, V = planes
+    R, C = bv.shape[:2]
+    qpc = QPC[qp]
+    ar = np.arange
+    for t in range(C + 2 * (R - 1)):
+        r = ar(R)[(t - 2 * ar(R) >= 0) & (t - 2 * ar(R) < C)]
+        c = t - 2 * r
+        for vertical in (True, False):
+            bs = bv if vertical else bh
+            for e in range(4):
+                sel = (c > 0) if (vertical and e == 0) else (r > 0) if e == 0 else np.ones(len(r), bool)
+                rr, cc = r[sel], c[sel]
+                if not len(rr):
+                    continue
+                strength = bs[rr, cc, e]                                                 # [n, 4]
+                along = lambda base, n, k: base[:, None] + ar(n)[None, :] + k
+                if vertical:                                                             # lines = rows, samples across columns
+                    iy, ix = along(16 * rr, 16, 0)[:, :, None], along(16 * cc + 4 * e, 8, -4)[:, None, :]
+                else:
+                    iy, ix = along(16 * rr + 4 * e, 8, -4)[:, None, :], along(16 * cc, 16, 0)[:, :, None]
+                Y[iy, ix] = _filter(Y[iy, ix], np.repeat(strength, 4, 1), qp, False)
+                if e % 2:
+                    continue
+                cs = np.repeat(strength, 2, 1)                                            # chroma edge 4e/2 = luma edge e
+                if vertical:
+                    iy, ix = along(8 * rr, 8, 0)[:, :, None], along(8 * cc + 2 * e, 4, -2)[:, None, :]
+                else:
+                    iy, ix = along(8 * rr + 2 * e, 4, -2)[:, None, :], along(8 * cc, 8, 0)[:, :, None]
+                for p in (U, V):
+                    p[iy, ix] = _filter(p[iy, ix], cs, qpc, True)
+
+
+# ------------------------------------------------------------------------------------------------ rate control
+def _fdiv(a, b):
+    return a // b                                     # floor division (b > 0); the device states it explicitly
+
+
+class RateControl:
+    """The device controller (csrc/h264.cu h264_rc_update), in the same integer arithmetic.  A leaky bucket of one second: fullness
+    is the stream's excess over bitrate x time, in 1/fps_num bits, saturating at +-8 s.  The budget of the next frame is the per-frame rate minus a
+    second's share of the fullness; after each P frame (and after an IDR frame that follows an IDR frame) QP moves by -2..+2 by
+    how far that frame's bits were from its budget.  IDR frames keep the QP of the P frames around them and are paid for by the
+    P frames after them."""
+
+    def __init__(self, width, height, bitrate, fps_num, fps_den, qp_min=0, qp_max=51):
+        self.bitrate, self.num, self.den, self.qp_min, self.qp_max = bitrate, fps_num, fps_den, qp_min, qp_max
+        self.fullness, self.frames, self.prev_idr = 0, 0, 0
+        x, y, q = 10 * bitrate * fps_den, fps_num * width * height, 30              # 30 at 0.1 bits per pixel, -6 per doubling
+        while x >= 2 * y and q > 0:
+            y, q = 2 * y, q - 6
+        while 2 * x < y and q < 51:
+            x, q = 2 * x, q + 6
+        self.qp = min(max(q, qp_min), qp_max)
+
+    def update(self, nbytes, idr):
+        bits = 8 * nbytes * self.num
+        budget = self.bitrate * self.den
+        sat = 8 * self.bitrate * self.num                        # the bucket saturates at +-8 s
+        self.fullness = min(max(self.fullness + bits - budget, -sat), sat)
+        if not idr or self.prev_idr:
+            want = max(budget - _fdiv(self.fullness, max(1, self.num // self.den)), budget // 8)
+            step = (2 if 100 * bits > 141 * want else 1 if 100 * bits > 112 * want else
+                    -2 if 141 * bits < 100 * want else -1 if 112 * bits < 100 * want else 0)
+            self.qp = min(max(self.qp + step, self.qp_min), self.qp_max)
+        self.prev_idr = int(idr)
+        self.frames += 1
+
+
+# ------------------------------------------------------------------------------------------------ rate-controlled stream
+class RcEncoder(Encoder):
+    """The rate-controlled stream: Encoder's coding with a controller-chosen QP per picture, quarter-sample motion and deblocking.
+    bitrate in bits/s, fps = (num, den); qp_min == qp_max pins the QP.  After each encode(): recon is the deblocked picture, qps
+    the QP of every frame so far."""
+
+    def __init__(self, width, height, bitrate, fps=(30, 1), gop=60, qp_min=0, qp_max=51):
+        super().__init__(width, height, 26, gop)
+        self.rc = RateControl(width, height, bitrate, fps[0], fps[1], qp_min, qp_max)
+        self.qps = []
+
+    def _search(self, ry, cur):
+        """The integer search, then the 8 half-sample neighbours of its vector, then the 8 quarter-sample neighbours of the best of
+        those, with the same cost and key; luma predicted with the 6-tap filter (8.4.2.2.1)."""
+        P = half_planes(ry)
+        best = self._integer_search(P[0], cur)
+        qx, qy = mv_of(best)
+        src = _mb_view(cur, 16)
+        lam = LAMBDA[self.qp]
+        X0 = 4 * (16 * np.arange(self.mbw)[None, :, None, None] + np.arange(16)[None, None, None, :])
+        Y0 = 4 * (16 * np.arange(self.mbh)[:, None, None, None] + np.arange(16)[None, None, :, None])
+        pred_at = lambda x, y: luma_pred(P, X0 + x[:, :, None, None], Y0 + y[:, :, None, None])
+        for step in (2, 1):
+            cx, cy = qx, qy
+            for dy in (-1, 0, 1):
+                for dx in (-1, 0, 1):
+                    if dx or dy:
+                        x, y = cx + step * dx, cy + step * dy
+                        cost = np.abs(src - pred_at(x, y)).sum((-1, -2)) + lam * (se_bits(x) + se_bits(y))
+                        np.minimum(best, mv_key(cost, x, y), out=best)
+            qx, qy = mv_of(best)
+        return qx, qy, pred_at(qx, qy)
+
+    def _slice_qp_and_deblocking(self, bw):
+        bw.se(self.qp - 26)                        # slice_qp_delta (pic_init_qp 26)
+        bw.ue(0)                                   # disable_deblocking_filter_idc: filter, across slice boundaries too
+        bw.se(0)                                   # slice_alpha_c0_offset_div2
+        bw.se(0)                                   # slice_beta_offset_div2
+
+    def encode(self, rgb):
+        """Codes the frame at the controller's QP, then deblocks the reconstruction (the slices do not depend on it) and updates
+        the controller with the sample's size."""
+        self.qp = self.rc.qp
+        sample, idr = super().encode(rgb)
+        R, C = self.mbh, self.mbw
+        if idr:
+            nz, mv = np.zeros((R, C, 4, 4), bool), np.zeros((R, C, 2), np.int64)
+        else:
+            nz, mv = unblocks_dc(self.levels.any((-1, -2))), self.mvs
+        planes = tuple(p.astype(np.int64) for p in self.recon)
+        deblock(planes, self.qp, *boundary_strength(idr, nz, mv))
+        self.recon = tuple(p.astype(np.uint8) for p in planes)
+        self.rc.update(len(sample), idr)
+        self.qps.append(self.qp)
+        return sample, idr
 
 
 # ------------------------------------------------------------------------------------------------ test sequences
@@ -550,3 +815,29 @@ def sequence(name, W, H, n=3):
 
 
 SEQUENCES = ('flat', 'gradient', 'translate', 'edge', 'noise')
+
+PAN = (1.25, -0.5)              # per-frame shift of the 'pan' sequence: frame t samples the pattern at x + 1.25t, y - 0.5t
+PAN_SCALE = 3                   # ... with _pattern's frequencies times 3 (at most 0.75 rad/sample per term), so that a quarter
+                                # sample of motion moves the SAD well above the reconstruction's noise at QP 18
+
+
+def pan(W, H, n=3):
+    """n uint8 RGB frames [H, W, 3] of _pattern's analytic pattern (frequencies scaled by PAN_SCALE) panned by a fraction of a
+    sample per frame (true vector (5, -2) in quarter samples)."""
+    out = []
+    for t in range(n):
+        rng = np.random.RandomState(1)
+        y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+        x, y = PAN_SCALE * (x + PAN[0] * t), PAN_SCALE * (y + PAN[1] * t)
+        img = np.zeros((H, W, 3))
+        for c in range(3):
+            for _ in range(6):
+                fx, fy, ph = rng.uniform(0.02, 0.25, 2).tolist() + [rng.uniform(0, 6.3)]
+                img[..., c] += np.sin(fx * x + fy * y + ph) * rng.uniform(10, 30)
+        out.append(np.clip(img + 128, 0, 255).astype(np.uint8))
+    return out
+
+
+def frames(name, W, H, n=3):
+    """sequence(), and 'pan'."""
+    return pan(W, H, n) if name == 'pan' else sequence(name, W, H, n)
