@@ -14,8 +14,19 @@ run) and rendered by the batched drivers of next3d_b200.drivers on one CUDA devi
     `--qp`, default 18, integer-pel motion, no deblocking; INTEGRATION.md section 0) and never imports imageio.  With
     `--bitrate` (`script`: the scripts' 10M / 12M, or a rate such as 8M) it writes the rate-controlled stream instead: QP chosen
     on the GPU per frame, quarter-sample motion and deblocking.
+
+Under torchrun (`torchrun --nproc-per-node N -m next3d_b200 ...`) every rank loads the network and renders its share on its own
+GPU (LOCAL_RANK), with a gloo process group for the little that crosses ranks.  A video is split into whole GOPs (`--gop`,
+default 60): each rank renders exactly the calls the single-process run makes for its frames (same images, padding and sampler
+seed), encodes them with `--encoder n3d` on its GPU, and rank 0 gathers the coded samples and writes the one MP4, so the files are
+byte for byte those of one process (with `--bitrate`, each rank's share starts its own rate controller instead: a valid file, not
+the same bytes).  gen_samples splits the seeds in whole calls and every rank writes its own seeds' files.  `--encoder imageio` is
+refused under torchrun.
 """
 import argparse
+import contextlib
+import datetime
+import io
 import os
 import re
 import sys
@@ -23,6 +34,7 @@ import sys
 import torch
 
 SAMPLER_SEED = 0
+DIST_TIMEOUT = datetime.timedelta(minutes=60)        # the longest a rank waits for the others at a collective
 
 
 def _bool(s):
@@ -117,6 +129,8 @@ def _encoder_args(p):
     p.add_argument('--bitrate', default=None,
                    help="--encoder n3d at a bitrate instead of a constant QP: 'script' (the scripts' rate per video) or bits/s "
                         "such as 8M or 800k")
+    p.add_argument('--gop', type=int, default=None,
+                   help='--encoder n3d: an IDR frame every N frames (default 60); under torchrun the ranks split a video in whole GOPs')
 
 
 def _refuse(msg):
@@ -133,27 +147,44 @@ def _imageio():
 
 
 def _video_writer(args):
-    """write(path, frames, fps, bitrate) of the chosen --encoder, checked before the network is loaded."""
+    """write(path, fps, bitrate, frames, shard) of the chosen --encoder, checked before the network is loaded: imageio writes the
+    host frames of frames(), n3d the video of shard(gop, rank, world) (a drivers.*_video_shard) through write_video_sharded."""
+    if args.gop is not None and args.encoder != 'n3d':
+        _refuse('--gop sets the GOP of --encoder n3d')
+    if args.gop is not None and args.gop < 1:
+        _refuse(f'--gop {args.gop}: a GOP holds at least one frame')
+    if args.encoder == 'imageio' and _world() > 1:
+        _refuse('--encoder imageio writes on one process: under torchrun pass --encoder n3d')
+    gop = 60 if args.gop is None else args.gop
     if args.bitrate is not None:
         if args.encoder != 'n3d':
             _refuse('--bitrate selects the rate-controlled stream of --encoder n3d; imageio already writes at the scripts\' rates')
         if args.qp is not None:
             _refuse('--bitrate and --qp exclude each other: the rate controller chooses the QP')
+        rate = None
         if args.bitrate != 'script':
             from .video import parse_bitrate
             try:
                 rate = parse_bitrate(args.bitrate)
             except ValueError as e:
                 _refuse(f'--bitrate: {e}')
-            return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, None, rate)
-        return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, None, bitrate)
+        return lambda path, fps, bitrate, frames, shard: _write_video_n3d(path, shard, fps, gop, None, rate or bitrate)
     if args.encoder == 'imageio':
         imageio = _imageio()
-        return lambda path, frames, fps, bitrate: _write_video(imageio, path, frames, fps, bitrate)
+        return lambda path, fps, bitrate, frames, shard: _write_video(imageio, path, frames(), fps, bitrate)
     qp = 18 if args.qp is None else args.qp
     if not 0 <= qp <= 51:
         _refuse(f'--qp {qp}: the quantiser is 0..51')
-    return lambda path, frames, fps, bitrate: _write_video_n3d(path, frames, fps, qp)
+    return lambda path, fps, bitrate, frames, shard: _write_video_n3d(path, shard, fps, gop, qp)
+
+
+def _world():
+    return int(os.environ.get('WORLD_SIZE', '1'))
+
+
+def _rank():
+    from . import distributed as D
+    return D.rank_world()
 
 
 def _load(args):
@@ -181,36 +212,42 @@ def _write_video(imageio, path, frames, fps, bitrate):
         writer.close()
 
 
-def _write_video_n3d(path, frames, fps, qp, bitrate=None):
-    from .video import H264Writer
-    writer = None
-    try:
-        for frame in frames:
-            if writer is None:
-                writer = (H264Writer(path, frame.shape[1], frame.shape[0], fps, qp=qp) if bitrate is None else
-                          H264Writer(path, frame.shape[1], frame.shape[0], fps, bitrate=bitrate))
-            writer.write(frame)
-    finally:
-        if writer is not None:
-            writer.close()
+def _write_video_n3d(path, shard, fps, gop, qp, bitrate=None):
+    from . import drivers
+    from .video import H264Encoder
+    rank, world = _rank()
+    kw = dict(qp=qp) if bitrate is None else dict(bitrate=bitrate)
+    drivers.write_video_sharded(path, lambda: shard(gop, rank, world),
+                                lambda width, height, first: H264Encoder(width, height, fps, gop=gop, first_frame=first, **kw))
 
 
 def gen_samples(args):
-    """gen_samples_next3d.py: seedNNNN.png sheets and, with --shapes, seedNNNN.mrc density grids."""
+    """gen_samples_next3d.py: seedNNNN.png sheets and, with --shapes, seedNNNN.mrc density grids.  Under torchrun every rank renders
+    and writes the seeds of its whole calls (drivers.sheet_span)."""
     import PIL.Image
-    from . import drivers, mrc
+    from . import distributed as D, drivers, mrc
     if args.shape_format == '.ply':
         _refuse('--shape-format .ply needs marching cubes, which is outside this project; use .mrc')
     G = _load(args)
     v = _mesh(args)
-    os.makedirs(args.outdir, exist_ok=True)
-    ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
-    for i, sheet, sigmas in drivers.render_sample_sheets(G, ws, v, fov_deg=args.fov_deg, shapes=args.shapes, shape_res=args.shape_res,
-                                                         seed=SAMPLER_SEED):
-        name = os.path.join(args.outdir, f'seed{args.seeds[i]:04d}')
-        PIL.Image.fromarray(sheet, 'RGB').save(name + '.png')
-        if sigmas is not None:
-            mrc.write_mrc(name + '.mrc', sigmas)
+    rank, world = _rank()
+    err = None
+    try:
+        os.makedirs(args.outdir, exist_ok=True)
+        ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
+        a, b, call = drivers.sheet_span(len(args.seeds), 9, rank, world)
+        if a < b:
+            for i, sheet, sigmas in drivers.render_sample_sheets(G, ws[a:b], v, fov_deg=args.fov_deg, shapes=args.shapes,
+                                                                 shape_res=args.shape_res, seed=SAMPLER_SEED + 2 * call):
+                name = os.path.join(args.outdir, f'seed{args.seeds[a + i]:04d}')
+                PIL.Image.fromarray(sheet, 'RGB').save(name + '.png')
+                if sigmas is not None:
+                    mrc.write_mrc(name + '.mrc', sigmas)
+    except Exception as e:
+        if world == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    D.agree(err)
 
 
 def gen_videos(args):
@@ -238,14 +275,18 @@ def gen_videos(args):
         os.makedirs(args.save_root, exist_ok=True)
     if args.interpolate:
         ws = drivers.grid_keyframes(G, args.seeds, args.grid, args.num_keyframes, args.shuffle_seed, psi, cutoff)
-        frames = drivers.render_grid_frames(G, ws, v, args.w_frames, image_mode=args.image_mode, seed=SAMPLER_SEED)
-        write(os.path.join(args.outdir, 'interpolation.mp4'), frames, 60, '10M')
+        write(os.path.join(args.outdir, 'interpolation.mp4'), 60, '10M',
+              lambda: drivers.render_grid_frames(G, ws, v, args.w_frames, image_mode=args.image_mode, seed=SAMPLER_SEED),
+              lambda gop, rank, world: drivers.grid_video_shard(G, ws, v, args.w_frames, gop, rank, world, image_mode=args.image_mode,
+                                                                seed=SAMPLER_SEED))
         return
     for seed in args.seeds:
         ws = drivers.grid_keyframes(G, [seed], (1, 1), args.num_keyframes, args.shuffle_seed, psi, cutoff)[0, 0]
         cams = drivers.orbit_camera_params(ws.shape[0] * args.w_frames, torch.tensor(rk['avg_camera_pivot']), rk['avg_camera_radius'])
-        frames = drivers.render_orbit(G, ws[:1], cams, v, image_mode=args.image_mode, seed=SAMPLER_SEED)
-        write(os.path.join(args.outdir, f'{seed}.mp4'), frames, 60, '12M')
+        write(os.path.join(args.outdir, f'{seed}.mp4'), 60, '12M',
+              lambda: drivers.render_orbit(G, ws[:1], cams, v, image_mode=args.image_mode, seed=SAMPLER_SEED),
+              lambda gop, rank, world: drivers.orbit_video_shard(G, ws[:1], cams, v, gop, rank, world, image_mode=args.image_mode,
+                                                                 seed=SAMPLER_SEED))
 
 
 def reenact(args):
@@ -257,16 +298,38 @@ def reenact(args):
     os.makedirs(args.outdir, exist_ok=True)
     _, cond = drivers.sample_sheet_cameras(G, args.fov_deg)
     ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
-    frames = drivers.reenact_grid_frames(G, ws, args.drive_root, args.num_frames, args.grid_dims, lms_cond=True,
-                                         fixed_camera=cond if args.fixed_camera else None, seed=SAMPLER_SEED)
-    write(os.path.join(args.outdir, args.fname), frames, 30, '12M')
+    fixed = cond if args.fixed_camera else None
+    write(os.path.join(args.outdir, args.fname), 30, '12M',
+          lambda: drivers.reenact_grid_frames(G, ws, args.drive_root, args.num_frames, args.grid_dims, lms_cond=True,
+                                              fixed_camera=fixed, seed=SAMPLER_SEED),
+          lambda gop, rank, world: drivers.reenact_grid_video_shard(G, ws, args.drive_root, args.num_frames, args.grid_dims, gop, rank,
+                                                                    world, lms_cond=True, fixed_camera=fixed, seed=SAMPLER_SEED))
 
 
 def main(argv=None):
     args = _parser().parse_args(argv)
     if not args.lms_cond:
         _refuse('pass --lms_cond True: the generator reads the 68 landmarks that follow the mesh vertices (load_lms)')
-    {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact}[args.command](args)
+    command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact}[args.command]
+    if _world() == 1:
+        command(args)
+        return
+    if args.command != 'gen_samples':
+        _video_writer(args)                                  # the refusals, before the process group and the network
+    import torch.distributed as dist
+    from . import distributed as D
+    dist.init_process_group('gloo', rank=int(os.environ['RANK']), world_size=_world(), timeout=DIST_TIMEOUT)
+    try:
+        torch.cuda.set_device(int(os.environ.get('LOCAL_RANK', '0')))
+        quiet = contextlib.nullcontext() if dist.get_rank() == 0 else contextlib.redirect_stdout(io.StringIO())     # rank 0 prints
+        try:
+            with quiet:
+                command(args)
+        except D.RankError as e:
+            _refuse(str(e))
+        dist.barrier()
+    finally:
+        dist.destroy_process_group()
 
 
 if __name__ == '__main__':

@@ -61,3 +61,41 @@ def max_over_ranks(value, device):
     if dist.is_initialized() and dist.get_world_size() > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return t.item()
+
+
+class RankError(RuntimeError):
+    """A failure on one of the ranks, raised on every rank: `rank` is the first failing rank, `message` its error."""
+
+    def __init__(self, rank, message):
+        super().__init__(f'rank {rank} failed: {message}')
+        self.rank, self.message = rank, message
+
+
+def rank_world(group=None):
+    """(rank, world) in `group` (None = the default group); (0, 1) when torch.distributed is not initialised."""
+    if not dist.is_initialized():
+        return 0, 1
+    return dist.get_rank(group), dist.get_world_size(group)
+
+
+def agree(error, group=None):
+    """Every rank passes its error message or None; raises RankError on every rank if any rank passed one (the first failing
+    rank's), so that all ranks leave together instead of waiting for a rank that has gone.  No-op in one process."""
+    if rank_world(group)[1] == 1:
+        return
+    errors = [None] * dist.get_world_size(group)
+    dist.all_gather_object(errors, error, group=group)
+    for r, e in enumerate(errors):
+        if e is not None:
+            raise RankError(r, e)
+
+
+def gather_to_root(obj, group=None):
+    """The picklable `obj` of every rank, in rank order, on rank 0 of `group` (host memory: meant for a gloo group); None on the
+    other ranks.  In one process: [obj]."""
+    rank, world = rank_world(group)
+    if world == 1:
+        return [obj]
+    out = [None] * world if rank == 0 else None
+    dist.gather_object(obj, out, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+    return out

@@ -8,7 +8,9 @@ function that does its setup and returns `step(k, idx)`: render step k of a plan
 uint8 frames.  Its two public drivers differ only in the plan and in how the finished batches leave the device: the single-process
 generator (local_plan: exactly `batch` frames per step) streams them to the caller through _to_host, an asynchronous read-back
 under the next step; the sharded twin (shard_plan: one process per GPU, contiguous frame ranges) gathers them to rank 0 through
-_gather_frames.  The sampler keywords of every call follow one rule (_sampler_kw).
+_gather_frames.  The sampler keywords of every call follow one rule (_sampler_kw).  The CLI's videos under torchrun use a third
+plan, CallPlan: each rank makes exactly the single-process calls that hold its own whole GOPs (the *_video_shard drivers), and
+write_video_sharded encodes them on its GPU and gathers only the coded samples to rank 0.
 
 Everything here is host logic around the hot path; the per-frame values (camera matrices, interpolated ws, uint8 pixels) are the
 reference's, checked in tests/test_drivers_cpu.py against the reference's own code, and the calls every driver makes in
@@ -124,6 +126,66 @@ def shard_plan(F, batch):
     nmax = max(e - s for s, e in spans)
     batch = min(range(max(1, batch // 2), batch + 1), key=lambda bb: (-(-nmax // bb) * bb, -bb))     # least padding, then the largest
     return ShardPlan(rank, world, spans, batch, -(-nmax // batch))
+
+
+class CallPlan(NamedTuple):
+    """The calls of the single-process run local_plan(n, batch) that one rank makes to produce its own outputs [own[0], own[1]):
+    every call whose window of items overlaps them, calls first .. first + steps - 1, each with the items, tail padding and step id
+    (sampler seed offset) it has in the single-process run, so the outputs are those of that run whatever the number of ranks.
+    A call that straddles the boundary of two ranks' outputs runs on both.  The step builders read it as a ShardPlan of one rank
+    whose span is the window of its calls."""
+    n: int
+    batch: int
+    own: tuple
+    first: int
+    steps: int
+    rank = 0
+    world = 1
+
+    @property
+    def spans(self):
+        if self.steps == 0:
+            return [self.own]
+        return [(self.first * self.batch, min((self.first + self.steps) * self.batch, self.n))]
+
+    def frames(self, k):
+        """Item ids of call first + k: those of the single-process run, a short tail repeating item n - 1."""
+        lo = (self.first + k) * self.batch
+        return [min(lo + j, self.n - 1) for j in range(self.batch)]
+
+    def step_id(self, k):
+        return self.first + k
+
+    def keep(self, k):
+        """(lo, hi): the outputs frames(k)[lo:hi] are this rank's own."""
+        lo = (self.first + k) * self.batch
+        return max(self.own[0] - lo, 0), min(self.own[1] - lo, self.batch)
+
+
+def call_plan(n, batch, own):
+    """The CallPlan of the outputs own = (a, b) of n items in calls of `batch` (no calls when a >= b)."""
+    a, b = own
+    if a >= b:
+        return CallPlan(n, batch, (a, b), 0, 0)
+    return CallPlan(n, batch, (a, b), a // batch, (b - 1) // batch - a // batch + 1)
+
+
+def gop_span(F, gop, rank, world):
+    """Frames [a, b) of an F-frame video that `rank` of `world` renders and encodes: whole GOPs, contiguous, in rank order (rank r
+    owns GOPs shard_range(ceil(F / gop), r, world)); empty when there are fewer GOPs than ranks."""
+    from . import distributed as D
+    a, b = D.shard_range(-(-F // gop), rank, world)
+    return min(gop * a, F), min(gop * b, F)
+
+
+def sheet_span(S, batch, rank, world):
+    """(a, b, first call): the seeds [a, b) that `rank` of `world` renders with render_sample_sheets, in whole calls of
+    max(1, batch // 3) heads (calls shard_range(ceil(S / heads), r, world)), and the index of its first call in the single-process
+    run, whose sampler seeds are seed + 2 * call and one more."""
+    from . import distributed as D
+    B = max(1, batch // 3)
+    ca, cb = D.shard_range(-(-S // B), rank, world)
+    return min(B * ca, S), min(B * cb, S), ca
 
 
 def _sampler_kw(seed, sampler_noise, seed_id, ids):
@@ -264,6 +326,69 @@ def _gather_frames(plan, step, H, W, device, out):
     return host
 
 
+def _own_frames(plan, step, grid=None):
+    """uint8 device frames [n, H, W, 3] of this rank's own outputs, batch after batch: step(k, plan.frames(k)) for each call of the
+    CallPlan, trimmed to plan.keep(k).  grid = (gw, gh): the items are the cells of frames, laid out (_whole_frames) from the rank's
+    first own cell to its last."""
+    def own():
+        for k in range(plan.steps):
+            lo, hi = plan.keep(k)
+            yield step(k, plan.frames(k))[lo:], hi - lo
+    for u8, n in (own() if grid is None else _whole_frames(own(), *grid)):
+        yield u8[:n]
+
+
+def write_video_sharded(path, shard, encoder, group=None):
+    """The per-rank loop of a video split over the ranks of `group` (gloo; None = the default group, or one process when
+    torch.distributed is not initialised).  shard() -> ((a, b), frames): this rank's frames [a, b) (gop_span; possibly none) and an
+    iterable of their uint8 device frame batches in order (the *_video_shard drivers); encoder(width, height, a) -> an encoder of
+    frames a, a + 1, ... (video.H264Encoder: write(frames) / flush() -> [(sample, is_idr)], width, height, fps, sps, pps).  The
+    frames go straight from the renderer to the encoder on the device, and only the coded samples leave it: they are gathered to
+    rank 0 over `group` on host memory, and rank 0 writes them, in frame order, to one MP4 at `path` (none when there are no
+    frames).  A failure on any rank -- its rank and message -- reaches every rank at the gather, which then raises
+    distributed.RankError on every rank, and no file is left behind; in one process the exception propagates as it is."""
+    from . import distributed as D, mp4
+    rank, world = D.rank_world(group)
+    err, payload = None, None
+    try:
+        (a, b), frames = shard()
+        enc, samples = None, []
+        for f in frames:
+            if enc is None:
+                enc = encoder(f.shape[2], f.shape[1], a)
+            samples += enc.write(f)
+        if enc is not None:
+            samples += enc.flush()
+        if len(samples) != b - a:
+            raise RuntimeError(f'frames {a}..{b - 1}: {len(samples)} coded frames')
+        payload = (samples, None if enc is None else (enc.width, enc.height, enc.fps, enc.sps, enc.pps))
+    except Exception as e:
+        if world == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    D.agree(err, group)
+    parts = D.gather_to_root(payload, group)
+    err = None
+    if rank == 0:
+        try:
+            heads = {h for _, h in parts if h is not None}
+            if len(heads) > 1:
+                raise RuntimeError('the ranks coded different parameter sets')
+            if heads:
+                with mp4.Mp4Writer(path, *heads.pop()) as w:
+                    for samples, _ in parts:
+                        for sample, idr in samples:
+                            w.add(sample, idr)
+        except Exception as e:
+            import os
+            if os.path.exists(path):
+                os.remove(path)
+            if world == 1:
+                raise
+            err = f'{type(e).__name__}: {e}'
+    D.agree(err, group)
+
+
 # ------------------------------------------------------------------------------------------------ frames and orbits (gen_videos_next3d.py)
 def render_frames(G, ws_frames, cams, verts, batch=8, image_mode='image', noise_mode='const', device=None, seed=None, sampler_noise=None):
     """Yield one uint8 HWC numpy frame per (ws, camera, mesh) triple, in order, rendering `batch` frames per synthesis call.
@@ -342,6 +467,18 @@ def render_orbit_sharded(G, ws, cams, verts, batch=8, image_mode='image', seed=0
     step = _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, sampler_noise)
     res = _frame_resolution(G, image_mode)
     return _gather_frames(plan, step, res, res, device, out)
+
+
+def orbit_video_shard(G, ws, cams, verts, gop, rank=0, world=1, batch=8, image_mode='image', seed=None):
+    """render_orbit's video split over ranks for write_video_sharded: -> ((a, b), frames), this rank's frames [a, b) =
+    gop_span(F, gop, rank, world) as uint8 device frame batches, from exactly the render_views calls of render_orbit that hold
+    them (CallPlan), so the frames are render_orbit's.  A rank without frames computes nothing."""
+    device = next(G.parameters()).device
+    span = gop_span(cams.shape[0], gop, rank, world)
+    plan = call_plan(cams.shape[0], batch, span)
+    if plan.steps == 0:
+        return span, iter(())
+    return span, _own_frames(plan, _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, None))
 
 
 def _orbit_step(G, plan, ws, cams, verts, image_mode, device, seed, sampler_noise):
@@ -540,6 +677,21 @@ def render_grid_frames_sharded(G, ws_grid, verts, w_frames, batch=8, image_mode=
     return _gather_frames(plan, step, gh * res, gw * res, device, out)
 
 
+def grid_video_shard(G, ws_grid, verts, w_frames, gop, rank=0, world=1, batch=8, image_mode='image', seed=None):
+    """render_grid_frames's video split over ranks for write_video_sharded: -> ((a, b), frames), this rank's frames [a, b) =
+    gop_span(F, gop, rank, world) as uint8 device frame batches.  The items are images, as in render_grid_frames: the rank makes
+    exactly the synthesis calls of render_grid_frames that hold one of its images (same images, padding and seed), keeps its own
+    images and lays them out from its first frame, so the frames are render_grid_frames's."""
+    device = next(G.parameters()).device
+    gh, gw, K = ws_grid.shape[:3]
+    cells = gh * gw
+    a, b = gop_span(K * w_frames, gop, rank, world)
+    plan = call_plan(K * w_frames * cells, batch, (a * cells, b * cells))
+    if plan.steps == 0:
+        return (a, b), iter(())
+    return (a, b), _own_frames(plan, _grid_step(G, plan, ws_grid, verts, w_frames, image_mode, device, seed, None), (gw, gh))
+
+
 def _grid_step(G, plan, ws_grid, verts, w_frames, image_mode, device, seed, sampler_noise):
     """The schedule of a grid video, image f * cells + cell: every cell interpolates its own keyframes (interpolate_ws_device: cubic,
     2 wraps), every cell of frame f has the frame's orbit camera (gen_videos_next3d.py:128-144).  -> step(k, ids): the uint8 cells
@@ -604,6 +756,22 @@ def reenact_grid_frames_sharded(G, ws, drive_root, num_frames, grid, batch=8, lm
     step = _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, sampler_noise)
     gw, gh = grid
     return _gather_frames(plan, step, gh * 512, gw * 512, device, out)
+
+
+def reenact_grid_video_shard(G, ws, drive_root, num_frames, grid, gop, rank=0, world=1, batch=8, lms_cond=True, fixed_camera=None,
+                             noise_mode='const', seed=None, prefetch_depth=8, workers=4):
+    """reenact_grid_frames's video split over ranks for write_video_sharded: -> ((a, b), frames), this rank's frames [a, b) =
+    gop_span(F, gop, rank, world) as uint8 device frame batches.  The items are driving frames of S heads: the rank makes exactly
+    the calls of reenact_grid_frames that hold one of its frames, parsing only their meshes and photos; with noise_mode 'const' /
+    'none' its own first call caches the ws-only backbones, which are then those of the single-process run."""
+    _check_reenact_grid(G, ws.shape[0], grid)
+    n, cams, frames = _reenact_source(drive_root, num_frames, lms_cond, fixed_camera, prefetch_depth, workers, photos=True)
+    device = next(G.parameters()).device
+    span = gop_span(n, gop, rank, world)
+    plan = call_plan(n, max(1, batch // ws.shape[0]), span)
+    if plan.steps == 0:
+        return span, iter(())
+    return span, _own_frames(plan, _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, None))
 
 
 def _reenact_grid_step(G, plan, ws, cams, frames, grid, noise_mode, device, seed, sampler_noise):

@@ -1,5 +1,5 @@
-"""H.264 video on the device: `H264Writer` encodes uint8 RGB frames with the sm_90a encoder of csrc/h264.cu and writes an MP4
-(next3d_b200.mp4).  The stream is Constrained Baseline (profile 66): 4:2:0 BT.601 limited range, CAVLC, one slice per macroblock
+"""H.264 video on the device: `H264Encoder` encodes uint8 RGB frames with the sm_90a encoder of csrc/h264.cu into AVCC samples,
+and `H264Writer` writes them to an MP4 file (next3d_b200.mp4).  The stream is Constrained Baseline (profile 66): 4:2:0 BT.601 limited range, CAVLC, one slice per macroblock
 row, IDR frames of I_16x16 macroblocks, P frames of P_L0_16x16 / P_Skip.  Two streams (DESIGN.md section 3.5):
   * constant QP (the default): integer-pel motion, no deblocking;
   * with a `bitrate`: QP per picture from a rate controller on the device, quarter-sample motion and in-loop deblocking.
@@ -172,54 +172,67 @@ def check_args(width, height, fps, qp, gop, bitrate=None):
     level_idc(width, height, float(_fps_fraction(fps)), bitrate)
 
 
-class H264Writer:
-    """Encode uint8 RGB frames [H, W, 3] (numpy arrays or CUDA tensors, one frame or a batch [N, H, W, 3]) into an MP4 file at
-    `path`, in order, on a stream of the writer's own.  qp: constant quantiser 0..51 (lower = larger file, closer to the input);
-    gop: an IDR frame every `gop` frames.  CUDA frames are read in place; numpy frames are copied to the device.  The encoded
-    frames reach the host every `batch` frames in one pinned copy.  Use as a context manager, or call close().
+class H264Encoder:
+    """Encode uint8 RGB frames [H, W, 3] (numpy arrays or CUDA tensors, one frame or a batch [N, H, W, 3]) in order, on a stream
+    of the encoder's own, and hand back the coded frames as (AVCC sample bytes, is_idr).  qp: constant quantiser 0..51 (lower =
+    larger stream, closer to the input); gop: an IDR frame every `gop` frames.  CUDA frames are read in place; numpy frames are
+    copied to the device.  The coded frames reach the host `batch` frames at a time in one pinned copy, one batch behind the
+    encoder, so that the host does not wait for the frames it has just submitted: write() returns the samples finished so far
+    (possibly none), flush() the rest.  `sps` and `pps` are the stream's parameter sets.
 
     bitrate (bits/s: an int, or a string such as '10M' or '800k'): the rate-controlled stream instead, with qp ignored.  Its
     controller runs on the device (no extra host synchronisation) and keeps each picture's QP within qp_range (min, max);
-    equal bounds pin the QP.  `recon` is then the deblocked picture."""
+    equal bounds pin the QP.  `recon` is then the deblocked picture.
 
-    def __init__(self, path, width, height, fps, qp=18, gop=60, device=None, batch=8, bitrate=None, qp_range=(0, 51)):
+    first_frame (a multiple of gop): the index of the first frame in a longer video, which sets frame_num and idr_pic_id, so that
+    encoders of consecutive ranges of a clip, split at multiples of gop, concatenate to the constant-QP stream of one encoder over
+    the whole clip (nothing crosses an IDR frame).  A rate-controlled segment starts its own controller at the first QP."""
+
+    def __init__(self, width, height, fps, qp=18, gop=60, device=None, batch=8, bitrate=None, qp_range=(0, 51), first_frame=0):
         self.bitrate = None if bitrate is None else parse_bitrate(bitrate)
         check_args(width, height, fps, qp, gop, self.bitrate)
+        if first_frame < 0 or first_frame % gop:
+            raise ValueError(f'first_frame must be a non-negative multiple of gop {gop}, got {first_frame}')
         qp_min, qp_max = (int(q) for q in qp_range)
         if not 0 <= qp_min <= qp_max <= 51:
             raise ValueError(f'qp_range must satisfy 0 <= min <= max <= 51, got {qp_range}')
-        self.width, self.height, self.qp, self.gop = int(width), int(height), int(qp), int(gop)
+        self.width, self.height, self.qp, self.gop, self.first_frame = int(width), int(height), int(qp), int(gop), int(first_frame)
+        self.fps = _fps_fraction(fps)
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.type != 'cuda':
-            raise ValueError('H264Writer encodes on a CUDA device')
+            raise ValueError('H264Encoder encodes on a CUDA device')
         sizes = [_lib.I64() for _ in range(4)]
         _lib.check(_lib.lib.n3d_h264_buffer_sizes(self.width, self.height, *[_lib.C.byref(s) for s in sizes]), 'n3d_h264_buffer_sizes')
         self.plane_bytes, scratch_bytes, slice_bytes, self.sample_cap = (s.value for s in sizes)
         mbw, mbh = (self.width + 15) // 16, (self.height + 15) // 16
         self._shape = (16 * mbh, 16 * mbw)
         self.stream = torch.cuda.Stream(self.device)
-        self.batch = max(1, min(int(batch), (1 << 29) // self.sample_cap))          # at most 512 MB of pending samples
+        self._copy = torch.cuda.Stream(self.device)                # sample read-back, off the encoder's stream
+        self.batch = max(1, min(int(batch), (1 << 28) // self.sample_cap))          # two halves of at most 256 MB of samples
         with torch.cuda.device(self.device):
             new = lambda n: torch.empty(n, dtype=torch.uint8, device=self.device)
             self._cur, self._planes = new(self.plane_bytes), [new(self.plane_bytes), new(self.plane_bytes)]
             self._scratch, self._slices = new(scratch_bytes), new(slice_bytes)
-            self._samples = new(self.batch * self.sample_cap)
-            self._lens = torch.zeros(self.batch, dtype=torch.int64, device=self.device)
+            self._samples = new(2 * self.batch * self.sample_cap)
+            self._lens = torch.zeros(2 * self.batch, dtype=torch.int64, device=self.device)
             self._rc = None
             if self.bitrate is not None:
-                f = _fps_fraction(fps)
                 self._rc = torch.empty(_lib.H264_RC_STATE_BYTES // 8, dtype=torch.int64, device=self.device)
-                self.stream.wait_stream(torch.cuda.current_stream(self.device))      # the allocation, before the writer's stream
-                _lib.check(_lib.lib.n3d_h264_rc_init(self._rc.data_ptr(), self.width, self.height, self.bitrate, f.numerator, f.denominator,
-                                                     qp_min, qp_max, self.stream.cuda_stream), 'n3d_h264_rc_init')
-        self._lens_host = torch.empty(self.batch, dtype=torch.int64, pin_memory=True)
+                self.stream.wait_stream(torch.cuda.current_stream(self.device))      # the allocation, before the encoder's stream
+                _lib.check(_lib.lib.n3d_h264_rc_init(self._rc.data_ptr(), self.width, self.height, self.bitrate, self.fps.numerator,
+                                                     self.fps.denominator, qp_min, qp_max, self.stream.cuda_stream), 'n3d_h264_rc_init')
+        self._lens_host = torch.empty(2 * self.batch, dtype=torch.int64, pin_memory=True)
         self._host = torch.empty(0, dtype=torch.uint8)
-        self._pending = []                                   # IDR flag of each frame encoded since the last flush
+        self._half = 0                                       # which half of the sample slots the next frames go to
+        self._pending = []                                   # IDR flag of each frame encoded into the current half
+        self._inflight = None                                # (half, IDR flags, event) of the submitted half not yet read back
+        self._done = []                                      # (sample, is_idr) read back and not yet handed out
         self.frames = 0
-        self._mp4 = mp4.Mp4Writer(path, self.width, self.height, _fps_fraction(fps), sps(self.width, self.height, fps, self.bitrate),
-                                  pps(self.qp if self._rc is None else 26))
+        self.sps = sps(self.width, self.height, fps, self.bitrate)
+        self.pps = pps(self.qp if self._rc is None else 26)
 
     def write(self, frames):
+        """Encode the frames; -> [(sample bytes, is_idr)] of the frames finished so far, in order."""
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(np.ascontiguousarray(frames))
         if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
@@ -231,53 +244,83 @@ class H264Writer:
         producer = torch.cuda.current_stream(self.device)
         with torch.cuda.stream(self.stream):
             if frames.device != self.device:
-                frames = frames.to(self.device)                   # numpy / host frames: copied on the writer's stream
+                frames = frames.to(self.device)                   # numpy / host frames: copied on the encoder's stream
             else:
                 self.stream.wait_stream(producer)                 # CUDA frames: read in place once their producer is done
                 frames.record_stream(self.stream)
             frames = frames.contiguous()
             for i in range(frames.shape[0]):
                 self._encode(frames[i])
+        return self._take()
+
+    def flush(self):
+        """Wait for every frame written so far; -> [(sample bytes, is_idr)] of those not yet returned, in order."""
+        self._submit()
+        self._read_back()
+        return self._take()
+
+    def _take(self):
+        out, self._done = self._done, []
+        return out
 
     def _encode(self, frame):
-        k = self.frames % self.gop
-        slot = len(self._pending)
+        n = self.first_frame + self.frames                       # index of the frame in the whole video
+        k = n % self.gop
+        slot = self._half * self.batch + len(self._pending)
         ref, rec = self._planes[self.frames % 2], self._planes[(self.frames + 1) % 2]
         fn, name = ((_lib.lib.n3d_h264_encode, 'n3d_h264_encode') if self._rc is None else
                     (_lib.lib.n3d_h264_encode_rc, 'n3d_h264_encode_rc'))
         _lib.check(fn(
             frame.data_ptr(), self.width, self.height, self.qp if self._rc is None else self._rc.data_ptr(), int(k == 0), k % 16,
-            (self.frames // self.gop) % 2, self._cur.data_ptr(), None if k == 0 else ref.data_ptr(), rec.data_ptr(),
+            (n // self.gop) % 2, self._cur.data_ptr(), None if k == 0 else ref.data_ptr(), rec.data_ptr(),
             self._scratch.data_ptr(), self._slices.data_ptr(), self._samples[slot * self.sample_cap:].data_ptr(),
             self._lens[slot:].data_ptr(), self.stream.cuda_stream), name)
         self._pending.append(k == 0)
         self.frames += 1
         if len(self._pending) == self.batch:
-            self._flush()
+            self._submit()
 
-    def _flush(self):
+    def _submit(self):
+        """Close the current half: its lengths go to the host behind its frames on the encoder's stream; the half submitted
+        before it is read back (its frames were queued a batch earlier), so that its slots are free for the next frames."""
         n = len(self._pending)
         if n == 0:
             return
+        o = self._half * self.batch
         with torch.cuda.stream(self.stream):
-            self._lens_host[:n].copy_(self._lens[:n], non_blocking=True)
-            self.stream.synchronize()
-            lens = self._lens_host[:n].tolist()
-            if min(lens) < 0:
-                raise RuntimeError('n3d_h264_encode: a slice exceeded its bitstream capacity')
-            if self._host.numel() < sum(lens):
-                self._host = torch.empty(max(sum(lens), 2 * self._host.numel()), dtype=torch.uint8, pin_memory=True)
-            o = 0
-            for i, ln in enumerate(lens):
-                self._host[o:o + ln].copy_(self._samples[i * self.sample_cap:i * self.sample_cap + ln], non_blocking=True)
-                o += ln
-            self.stream.synchronize()
-        data = self._host[:o].numpy().tobytes()
-        o = 0
-        for ln, idr in zip(lens, self._pending):
-            self._mp4.add(data[o:o + ln], idr)
-            o += ln
+            self._lens_host[o:o + n].copy_(self._lens[o:o + n], non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(self.stream)
+        self._read_back()
+        self._inflight = (self._half, self._pending, ev)
         self._pending = []
+        self._half ^= 1
+
+    def _read_back(self):
+        if self._inflight is None:
+            return
+        h, idrs, ev = self._inflight
+        self._inflight = None
+        o, n = h * self.batch, len(idrs)
+        ev.synchronize()
+        lens = self._lens_host[o:o + n].tolist()
+        if min(lens) < 0:
+            raise RuntimeError('n3d_h264_encode: a slice exceeded its bitstream capacity')
+        if self._host.numel() < sum(lens):
+            self._host = torch.empty(max(sum(lens), 2 * self._host.numel()), dtype=torch.uint8, pin_memory=True)
+        self._copy.wait_event(ev)
+        with torch.cuda.stream(self._copy):
+            p = 0
+            for i, ln in enumerate(lens):
+                s = (o + i) * self.sample_cap
+                self._host[p:p + ln].copy_(self._samples[s:s + ln], non_blocking=True)
+                p += ln
+        self._copy.synchronize()
+        data = self._host[:p].numpy().tobytes()
+        p = 0
+        for ln, idr in zip(lens, idrs):
+            self._done.append((data[p:p + ln], idr))
+            p += ln
 
     @property
     def recon(self):
@@ -292,11 +335,26 @@ class H264Writer:
         return (p[:n].view(H16, W16).clone(), p[n:n + n // 4].view(H16 // 2, W16 // 2).clone(),
                 p[n + n // 4:n + n // 2].view(H16 // 2, W16 // 2).clone())
 
+
+class H264Writer(H264Encoder):
+    """H264Encoder into an MP4 file at `path` (next3d_b200.mp4.Mp4Writer): every coded frame goes to the file as soon as it is
+    back on the host.  Arguments as H264Encoder's.  Use as a context manager, or call close()."""
+
+    def __init__(self, path, width, height, fps, qp=18, gop=60, device=None, batch=8, bitrate=None, qp_range=(0, 51), first_frame=0):
+        super().__init__(width, height, fps, qp=qp, gop=gop, device=device, batch=batch, bitrate=bitrate, qp_range=qp_range,
+                         first_frame=first_frame)
+        self._mp4 = mp4.Mp4Writer(path, self.width, self.height, self.fps, self.sps, self.pps)
+
+    def write(self, frames):
+        for sample, idr in super().write(frames):
+            self._mp4.add(sample, idr)
+
     def close(self):
         if self._mp4 is None:
             return
         try:
-            self._flush()
+            for sample, idr in self.flush():
+                self._mp4.add(sample, idr)
         finally:
             self._mp4.close()
             self._mp4 = None

@@ -8,7 +8,12 @@ batch 8), CUDA-graph replay, one head driven by F synthetic frames read from a m
 each as frames/s of whole-clip runs (host clock around a run that ends in a device synchronise; the best of 3 after a warm-up run),
 then the same at world size N = every visible GPU (one spawned process per GPU, NCCL) when more than one is visible.  Finally
 n3d_render_rays alone at the C2 (batch 8, 64^2, 48 + 48) and C3 (batch 16, 128^2, 96 + 96) shapes with depth_range_per_image 0 and
-1, alternated in rounds (CUDA events, median of 30 launches per block).  Anything that did not run is reported as not measured."""
+1, alternated in rounds (CUDA events, median of 30 launches per block).  Anything that did not run is reported as not measured.
+
+python tools/bench_sharded.py --cli [--frames F] instead times whole `python -m next3d_b200 gen_videos --encoder n3d` runs (a 4x2
+grid of one keyframe per cell, F frames, default 120, `--gop 30`; loading, graph capture and the MP4 included) of a tiny and of
+a full-width random-weight pickle, at a constant QP and with `--bitrate script`, as frames/s at world 1 and at world N = every
+visible GPU (torchrun-style ranks, one per GPU), with the card's name and power limit from the same run."""
 import dataclasses
 import os
 import socket
@@ -127,7 +132,53 @@ def render_rays_flag(tiny):
     return out
 
 
+def _cli_run(argv, world):
+    """Seconds of one `python -m next3d_b200 argv` run as `world` ranks, one per GPU."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    s = socket.socket()
+    s.bind(('127.0.0.1', 0))
+    port = s.getsockname()[1]
+    s.close()
+    t0 = time.perf_counter()
+    procs = [subprocess.Popen([sys.executable, '-m', 'next3d_b200', *argv], cwd=root, stdout=subprocess.DEVNULL,
+                              env=dict(os.environ, PYTHONPATH=root, **({} if world == 1 else dict(
+                                  RANK=str(r), WORLD_SIZE=str(world), LOCAL_RANK=str(r), MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port)))))
+             for r in range(world)]
+    codes = [p.wait() for p in procs]
+    if any(codes):
+        raise SystemExit(f'gen_videos exited with {codes}')
+    return time.perf_counter() - t0
+
+
+def cli_main(frames):
+    """Frames/s of whole gen_videos --encoder n3d runs at world 1 and N."""
+    from tests.test_legacy_cpu import _demo_args, generator_fields, persistence_pickle
+    import pathlib
+    card()
+    world = torch.cuda.device_count()
+    with tempfile.TemporaryDirectory() as tmp:
+        demo = _demo_args(pathlib.Path(tmp))
+        for tiny in (True, False):
+            cfg = config.tiny_config(512) if tiny else config.full_config(512)
+            net = os.path.join(tmp, 'net.pkl')
+            with open(net, 'wb') as f:
+                f.write(persistence_pickle(cfg, weights.make_state_dict(cfg, seed=0), generator_fields(cfg, torch.ones(1, 1, 256, 256))))
+            for name, stream in (('QP 18', ['--qp', '18']), ('bitrate script', ['--bitrate', 'script'])):
+                argv = ['gen_videos', '--network', net, '--seeds', '0-7', '--grid', '4x2', '--w-frames', str(frames), '--gop', '30',
+                        '--outdir', os.path.join(tmp, 'out'), '--lms_cond', 'True', '--encoder', 'n3d', *stream, *demo]
+                fps1 = frames / _cli_run(argv, 1)
+                line = f'gen_videos {"tiny" if tiny else "full"} 4x2 grid, {frames} frames, {name}: world 1 {fps1:.2f} frames/s'
+                if world > 1:
+                    fpsN = frames / _cli_run(argv, world)
+                    line += f', world {world} {fpsN:.2f} frames/s ({fpsN / fps1:.2f}x)'
+                else:
+                    line += ', world N not measured (one GPU visible)'
+                print(line, flush=True)
+
+
 def main():
+    if '--cli' in sys.argv:
+        return cli_main(int(sys.argv[sys.argv.index('--frames') + 1]) if '--frames' in sys.argv else 120)
     tiny = '--tiny' in sys.argv
     frames = int(sys.argv[sys.argv.index('--frames') + 1]) if '--frames' in sys.argv else 96
     batch = 8
