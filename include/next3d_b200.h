@@ -472,6 +472,23 @@ int n3d_h264_encode_rc(const uint8_t* rgb, int width, int height, void* state, i
                        const uint8_t* ref, uint8_t* recon, void* scratch, uint8_t* slices, uint8_t* sample, int64_t* sample_len,
                        void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * PNG encoder (next3d_b200/png.py; DESIGN.md section 3.6): n uint8 RGB images [height, width, 3] -> n complete PNG files
+ * (signature, IHDR 8-bit RGB without interlace, one IDAT chunk, IEND).  A file's bytes are a function of its image alone: they
+ * do not depend on n, the stream or the device.  The numpy restatement is tests/png_oracle.py.
+ * ---------------------------------------------------------------------------------------------------------- */
+
+/* Host only.  scratch_bytes: work space of one n3d_png_encode call of n images; file_bytes: capacity of one file (the size of
+ * the image in stored deflate blocks, which no file exceeds).  N3D_ERR_INVALID_ARG for n, height or width < 1, width > 2^24,
+ * or an image whose IDAT chunk could exceed 2^31 - 1 bytes. */
+int n3d_png_buffer_sizes(int n, int height, int width, int64_t* scratch_bytes, int64_t* file_bytes);
+
+/* Encode n images.  rgb: device uint8 [n, height, width, 3] contiguous; scratch: scratch_bytes (256-byte aligned); files:
+ * n * file_bytes, file i at i * file_bytes; *file_lens (device int64 [n]) receives each file's length.  Stream-ordered, no host
+ * synchronisation. */
+int n3d_png_encode(const uint8_t* rgb, int n, int height, int width, void* scratch, uint8_t* files, int64_t* file_lens,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

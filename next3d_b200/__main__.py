@@ -1,4 +1,5 @@
-"""Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`.
+"""Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`, and `gen_dataset` (multi-view
+training images in dataset_tool.py's layout).
 
 The three subcommands are the reference's gen_samples_next3d.py, gen_videos_next3d.py and reenact_avatar_next3d.py with their option
 names, defaults and output file names, run on a network pickle read by next3d_b200.legacy (no reference checkout, no pickled code
@@ -119,6 +120,24 @@ def _parser():
     r.add_argument('--fixed_camera', type=_bool, default=False)
     r.add_argument('--num_frames', type=int, default=500)
     _encoder_args(r)
+
+    d = sub.add_parser('gen_dataset', help="multi-view images with camera labels, meshes and landmarks, in dataset_tool.py's layout")
+    d.add_argument('--network', required=True, help='network pickle (local file)')
+    d.add_argument('--seeds', type=_range, required=True)
+    d.add_argument('--views', type=int, default=8, help='images per head; view 0 is frontal, the others Gaussian around the pivot')
+    d.add_argument('--obj_path', default=None)
+    d.add_argument('--lms_path', default=None)
+    d.add_argument('--drive_root', default=None, help='driving directory (as reenact): expressions are drawn from its frames')
+    d.add_argument('--expressions', type=int, default=None, help='heads per seed, each with another driving frame (needs --drive_root)')
+    d.add_argument('--yaw-std', dest='yaw_std', type=float, default=0.3)
+    d.add_argument('--pitch-std', dest='pitch_std', type=float, default=0.155)
+    d.add_argument('--trunc', dest='truncation_psi', type=float, default=1)
+    d.add_argument('--trunc-cutoff', dest='truncation_cutoff', type=int, default=14)
+    d.add_argument('--fov-deg', dest='fov_deg', type=float, default=18.837)
+    d.add_argument('--outdir', required=True)
+    d.add_argument('--batch', type=int, default=4, help='heads per rendering call')
+    d.add_argument('--reload_modules', type=_bool, default=False)
+    d.add_argument('--lms_cond', type=_bool, default=False)
     return p
 
 
@@ -250,6 +269,111 @@ def gen_samples(args):
     D.agree(err)
 
 
+def _check_dataset_args(args):
+    if args.views < 1:
+        _refuse(f'--views must be at least 1, got {args.views}')
+    if args.batch < 1:
+        _refuse(f'--batch must be at least 1, got {args.batch}')
+    if args.expressions is not None and args.drive_root is None:
+        _refuse('--expressions draws driving frames: it needs --drive_root')
+    mesh = args.obj_path is not None or args.lms_path is not None
+    if mesh and args.drive_root is not None:
+        _refuse('give either --obj_path / --lms_path or --drive_root, not both')
+    if args.drive_root is None and (args.obj_path is None or args.lms_path is None):
+        _refuse('give --obj_path and --lms_path (one expression), or --drive_root')
+
+
+def _link(src, dst, data=None):
+    """dst as a hard link to src, or, without src, a new file of `data`."""
+    os.makedirs(os.path.dirname(dst), exist_ok=True)
+    if os.path.lexists(dst):
+        os.remove(dst)
+    if src is None:
+        with open(dst, 'wb') as f:
+            f.write(data)
+    else:
+        os.link(src, dst)
+
+
+def gen_dataset(args):
+    """Multi-view images of heads (seed, expression) in dataset_tool.py's layout, which the reference's ImageFolderDataset and
+    mesh loader read: images/NNNNN/imgNNNNNNNN.png (head-major, view-minor) with images/dataset.json holding each image's 25
+    camera floats, meshes/NNNNN/imgNNNNNNNN.obj and lms/NNNNN/imgNNNNNNNN.txt (each distinct mesh written once per rank and
+    hard-linked per image), and heads.npz (seed, expression, ws per head).  PNG files come from the GPU encoder
+    (next3d_b200.png).  Under torchrun the heads are split in whole calls and every rank writes its own images; every rank
+    computes every label, so rank 0 writes dataset.json and heads.npz."""
+    import json
+    import numpy as np
+    from . import distributed as D, drivers, inputs
+    from .png import PngEncoder
+    _check_dataset_args(args)
+    if args.drive_root is not None:
+        sched = drivers.reenact_schedule(args.drive_root, 1 << 30, lms_cond=True)
+        sources = list(zip(sched['obj_paths'], sched['lms_paths']))
+        if not sources:
+            _refuse(f'--drive_root {args.drive_root}: no driving frames')
+    else:
+        sources = [(args.obj_path, args.lms_path)]
+    K = args.expressions or 1
+    if K > len(sources):
+        _refuse(f'--expressions {K}: the driving directory has {len(sources)} frames')
+    G = _load(args)
+    rank, world = _rank()
+    err = None
+    try:
+        head_seeds, head_exprs = drivers.dataset_heads(args.seeds, K, len(sources))
+        used = sorted(set(head_exprs))
+        meshes = torch.cat([inputs.load_frame(*sources[e]) for e in used])
+        mesh_ids = [used.index(e) for e in head_exprs]
+        ws_seed = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
+        row = {s: i for i, s in enumerate(args.seeds)}
+        ws = ws_seed[[row[s] for s in head_seeds]]
+        cams_seed = drivers.dataset_cameras(G, args.seeds, args.views, args.yaw_std, args.pitch_std, args.fov_deg)
+        cams = cams_seed[[row[s] for s in head_seeds]]
+        V = args.views
+        img_dir, mesh_dir, lms_dir = (os.path.join(args.outdir, d) for d in ('images', 'meshes', 'lms'))
+        os.makedirs(img_dir, exist_ok=True)
+        if rank == 0:
+            labels = [[drivers.dataset_image_name(h * V + v), [float(x) for x in cams[h, v]]] for h in range(len(head_seeds))
+                      for v in range(V)]
+            with open(os.path.join(img_dir, 'dataset.json'), 'w') as f:
+                json.dump({'labels': labels}, f)
+            np.savez(os.path.join(args.outdir, 'heads.npz'), seed=np.array(head_seeds, np.int64),
+                     expression=np.array(head_exprs, np.int64), ws=ws.float().cpu().numpy())
+        plan = drivers.dataset_plan(len(head_seeds), args.batch, rank, world)
+        enc = PngEncoder(G.img_resolution, G.img_resolution, batch=2 * args.batch * V)
+        first_link = {}                                  # expression -> this rank's first mesh / landmark files of it
+        pending = []                                     # image ids submitted to the encoder, not yet written
+
+        def save(files):
+            for data in files:
+                i = pending.pop(0)
+                name = drivers.dataset_image_name(i)
+                with open(os.path.join(img_dir, name), 'wb') as f:
+                    f.write(data)
+                e = head_exprs[i // V]
+                stem = name[:-len('.png')]
+                obj, lms = os.path.join(mesh_dir, stem + '.obj'), os.path.join(lms_dir, stem + '.txt')
+                if e in first_link:
+                    _link(first_link[e][0], obj)
+                    _link(first_link[e][1], lms)
+                else:
+                    _link(None, obj, open(sources[e][0], 'rb').read())
+                    _link(None, lms, open(sources[e][1], 'rb').read())
+                    first_link[e] = (obj, lms)
+        for h0, frames in drivers.render_dataset(G, ws, meshes, mesh_ids, cams, plan, seed=SAMPLER_SEED):
+            for i in range(h0 * V, h0 * V + frames.shape[0]):
+                os.makedirs(os.path.join(img_dir, drivers.dataset_image_name(i)[:5]), exist_ok=True)
+                pending.append(i)
+            save(enc.write(frames))
+        save(enc.flush())
+    except Exception as e:
+        if world == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    D.agree(err)
+
+
 def gen_videos(args):
     """gen_videos_next3d.py: interpolation.mp4 over a --grid of seeds, or with --interpolate False one orbit video SEED.mp4 per seed."""
     from . import drivers
@@ -310,11 +434,13 @@ def main(argv=None):
     args = _parser().parse_args(argv)
     if not args.lms_cond:
         _refuse('pass --lms_cond True: the generator reads the 68 landmarks that follow the mesh vertices (load_lms)')
-    command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact}[args.command]
+    command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact, 'gen_dataset': gen_dataset}[args.command]
+    if args.command == 'gen_dataset':
+        _check_dataset_args(args)                            # the refusals, before the process group and the network
     if _world() == 1:
         command(args)
         return
-    if args.command != 'gen_samples':
+    if args.command in ('gen_videos', 'reenact'):
         _video_writer(args)                                  # the refusals, before the process group and the network
     import torch.distributed as dist
     from . import distributed as D

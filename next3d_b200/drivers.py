@@ -992,3 +992,74 @@ def _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampl
             G._get_engine().cached_sigma_grid(b, shape_res, sigmas[b])
         return sheet_u8(front, views), new, sigmas
     return step
+
+
+# ------------------------------------------------------------------------------------------------------------- multi-view datasets
+def dataset_heads(seeds, expressions=1, num_meshes=1):
+    """(head seeds, head expressions): one head per (seed, expression), seed-major.  With one mesh every seed has expression 0;
+    with num_meshes driving frames, seed s takes `expressions` distinct frame indices, sorted, drawn by
+    np.random.RandomState([s, 0]).choice(num_meshes, expressions, replace=False)."""
+    if expressions < 1 or expressions > num_meshes:
+        raise ValueError(f'expressions must be in 1..{num_meshes} (the driving frames), got {expressions}')
+    hs, he = [], []
+    for s in seeds:
+        ex = [0] if num_meshes == 1 else sorted(int(e) for e in np.random.RandomState([s, 0]).choice(num_meshes, expressions, replace=False))
+        hs += [int(s)] * len(ex)
+        he += ex
+    return hs, he
+
+
+def dataset_cameras(G, seeds, views, yaw_std=0.3, pitch_std=0.155, fov_deg=18.837):
+    """camera_params float32 [S, views, 25] of each seed's views: view 0 looks from the front (sample_sheet_cameras' conditioning
+    camera); view v >= 1 is GaussianCameraPoseSampler's draw -- yaw pi/2 + yaw_std * n1 and pitch pi/2 + pitch_std * n2, the
+    pitch clamped to (1e-5, pi - 1e-5) -- with (n1, n2) = np.random.RandomState([seed, v]).randn(2), looking at the pivot from
+    avg_camera_radius, with FOV_to_intrinsics(fov_deg)."""
+    rk = G.rendering_kwargs
+    pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
+    radius = rk.get('avg_camera_radius', 2.7)
+    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
+    out = torch.empty(len(seeds), views, 25)
+    for i, s in enumerate(seeds):
+        for v in range(views):
+            n1, n2 = np.random.RandomState([int(s), v]).randn(2) if v else (0.0, 0.0)
+            h, p = np.pi / 2 + yaw_std * n1, float(np.clip(np.pi / 2 + pitch_std * n2, 1e-5, np.pi - 1e-5))
+            out[i, v] = torch.cat([camera.look_at_pose(h, p, pivot, radius).reshape(-1, 16), intr], 1)[0]
+    return out
+
+
+def dataset_plan(n_heads, batch, rank=0, world=1):
+    """The CallPlan of `rank` of `world` over n_heads heads in calls of `batch` heads: whole calls, contiguous, in rank order
+    (calls shard_range(ceil(n_heads / batch), r, world)), each with its single-process call index; no calls when a rank has none."""
+    from . import distributed as D
+    ca, cb = D.shard_range(-(-n_heads // batch), rank, world)
+    return call_plan(n_heads, batch, (min(batch * ca, n_heads), min(batch * cb, n_heads)))
+
+
+def dataset_image_name(i):
+    """dataset_tool.py's name of image i: '00000/img00000000.png', a folder per 1000 images."""
+    return f'{i // 1000:05d}/img{i:08d}.png'
+
+
+def render_dataset(G, ws, meshes, mesh_ids, cams, plan, seed=None):
+    """Multi-view images of the heads of a dataset_plan: ws [N, 28, 512] and cams [N, V, 25] per head, meshes [M, Nv, 3] and
+    mesh_ids[h], the mesh of head h.  Per call k: one synthesis call with cache_backbone renders view 0 of its heads, one
+    render_views call the other V - 1 views of each (view n of head n // (V - 1)), with sampler seeds seed + 2 c and seed + 2 c + 1
+    for the single-process call index c.  Yields (first head, uint8 frames [n V, H, W, 3] on the generator's device) for the n
+    heads of each call that the plan owns, head-major and view-minor; a short last call repeats its last head, as render_sample_sheets
+    does."""
+    device = next(G.parameters()).device
+    N, V = cams.shape[:2]
+    cams = cams.to(device, torch.float32)
+    meshes = meshes.to(device, torch.float32)
+    mesh_ids = torch.as_tensor(mesh_ids, dtype=torch.long)
+    for k in range(plan.steps):
+        idx, (lo, hi) = plan.frames(k), plan.keep(k)
+        B, c = len(idx), plan.step_id(k)
+        w = ws[idx].to(device, torch.float32)
+        img = G.synthesis(w, cams[idx, 0], meshes[mesh_ids[idx].to(device)], noise_mode='const', cache_backbone=True,
+                          **_sampler_kw(seed, None, 2 * c, None))['image']
+        frames = to_uint8_hwc(img)[:, None]
+        if V > 1:
+            more = G.render_views(cams[idx, 1:].reshape(-1, 25), **_sampler_kw(seed, None, 2 * c + 1, None))['image']
+            frames = torch.cat([frames, to_uint8_hwc(more).reshape(B, V - 1, *frames.shape[2:])], 1)
+        yield idx[lo], frames[lo:hi].reshape(-1, *frames.shape[2:])
