@@ -21,6 +21,7 @@
 #ifndef NEXT3D_B200_H
 #define NEXT3D_B200_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -488,6 +489,30 @@ int n3d_png_buffer_sizes(int n, int height, int width, int64_t* scratch_bytes, i
  * synchronisation. */
 int n3d_png_encode(const uint8_t* rgb, int n, int height, int width, void* scratch, uint8_t* files, int64_t* file_lens,
                    void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Marching cubes (next3d_b200/isosurface.py; DESIGN.md section 3.7): the mesh of the level set of a float32 grid
+ * g[a0, a1, a2] of shape [nz, ny, nx] (the layout of n3d_sample_grid and of the .mrc data).  A voxel is inside when g > level;
+ * one vertex per grid edge whose endpoints differ, at (x, y, z) = (a2, a1, a0) plus t = (level - s0) / (s1 - s0) along the
+ * edge (fp32, IEEE division), in ascending (a0, a1, a2) of the edge's lower endpoint, then its x-, y- and z-edge; triangles cell
+ * by cell in ascending (a0, a1, a2), each cell's from its 256-entry table, wound so that the right-hand normal points from the
+ * inside toward the outside.  A grid with a dimension below 2 has no cells and an empty mesh.  The result depends on the grid
+ * and the level alone.  The numpy restatement is tests/isosurface_oracle.py.
+ * ---------------------------------------------------------------------------------------------------------- */
+
+/* Host only.  Workspace of a grid: three int64 per (a0, a1) voxel row and per tile of 4096 rows (O(nz * ny), never O(voxels)).
+ * N3D_ERR_INVALID_ARG for a dimension < 1, nz * ny > 2^31 - 4097 or nx > 2^28. */
+int n3d_isosurface_workspace_bytes(int nz, int ny, int nx, size_t* bytes);
+
+/* Pass 1: classify every voxel row, scan the rows; counts (device int64 [3]) receives {vertices, triangles, non-finite voxels},
+ * and the workspace (8-byte aligned) keeps the rows' offsets for n3d_isosurface_emit.  level must be finite.  Stream-ordered, no
+ * host synchronisation. */
+int n3d_isosurface_count(const float* grid, int nz, int ny, int nx, float level, void* workspace, int64_t* counts, void* stream);
+
+/* Pass 2, after n3d_isosurface_count of the same grid, level and workspace: verts (device float32 [V, 3]) and faces (device int32
+ * [F, 3], vertex indices) of the counted mesh.  The caller checks V and F below 2^31 first.  Stream-ordered. */
+int n3d_isosurface_emit(const float* grid, int nz, int ny, int nx, float level, const void* workspace, float* verts, int32_t* faces,
+                        void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
-"""Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`, and `gen_dataset` (multi-view
-training images in dataset_tool.py's layout).
+"""Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`, `gen_dataset` (multi-view
+training images in dataset_tool.py's layout) and `shape_utils` (the reference's .mrc -> .ply converter, marching cubes on the GPU).
 
 The three subcommands are the reference's gen_samples_next3d.py, gen_videos_next3d.py and reenact_avatar_next3d.py with their option
 names, defaults and output file names, run on a network pickle read by next3d_b200.legacy (no reference checkout, no pickled code
@@ -8,7 +8,7 @@ run) and rendered by the batched drivers of next3d_b200.drivers on one CUDA devi
   * the ray sampler draws its uniforms from seed 0 (the scripts use fresh torch.rand draws), so a run is reproducible;
   * `--lms_cond True` is required: the generator reads the 68 landmarks that follow the mesh vertices (load_lms), and without them
     the scripts fail as well;
-  * `--shape-format .ply` (marching-cubes export) and `--cfg` other than FFHQ are refused, and so is `--interpolate False` with a
+  * `--shape-format .ply` (mesh the .mrc grids with `shape_utils` instead) and `--cfg` other than FFHQ are refused, and so is `--interpolate False` with a
     grid larger than 1x1 (every cell would show the same head);
   * mp4 files are written with imageio (libx264 at the scripts' bitrates); without it the video commands refuse before loading
     the network.  `--encoder n3d` writes them with this package's H.264 encoder on the GPU instead (next3d_b200.video: constant
@@ -27,7 +27,9 @@ refused under torchrun.
 import argparse
 import contextlib
 import datetime
+import glob
 import io
+import math
 import os
 import re
 import sys
@@ -138,6 +140,10 @@ def _parser():
     d.add_argument('--batch', type=int, default=4, help='heads per rendering call')
     d.add_argument('--reload_modules', type=_bool, default=False)
     d.add_argument('--lms_cond', type=_bool, default=False)
+
+    m = sub.add_parser('shape_utils', help=".mrc density grids -> .ply meshes (the reference's shape_utils.py), marching cubes on the GPU")
+    m.add_argument('input_mrc_path', help='an .mrc file, or a directory whose *.mrc files are all converted')
+    m.add_argument('--level', type=float, default=10, help='the isosurface level for marching cubes')
     return p
 
 
@@ -246,7 +252,8 @@ def gen_samples(args):
     import PIL.Image
     from . import distributed as D, drivers, mrc
     if args.shape_format == '.ply':
-        _refuse('--shape-format .ply needs marching cubes, which is outside this project; use .mrc')
+        _refuse('--shape-format .ply: gen_samples writes the script\'s .mrc grids; mesh them with python -m next3d_b200 shape_utils '
+                'OUTDIR (marching cubes on the GPU)')
     G = _load(args)
     v = _mesh(args)
     rank, world = _rank()
@@ -374,6 +381,45 @@ def gen_dataset(args):
     D.agree(err)
 
 
+def _shape_files(args):
+    """The .mrc files shape_utils converts, sorted; the refusals come before any CUDA work."""
+    if not math.isfinite(args.level):
+        _refuse(f'--level {args.level}: the isosurface level must be finite')
+    path = args.input_mrc_path
+    if os.path.isdir(path):
+        return sorted(glob.glob(os.path.join(path, '*.mrc')))
+    if not os.path.exists(path):
+        _refuse(f'{path}: no such file or directory')
+    if not path.endswith('.mrc'):
+        _refuse(f'{path}: shape_utils converts .mrc files (or a directory of them)')
+    return [path]
+
+
+def shape_utils(args):
+    """shape_utils.py: each .mrc grid (the file, or every *.mrc directly in the directory) -> stem.ply beside it, meshed at --level
+    by next3d_b200.isosurface.  Unlike the script, a single file is meshed at --level too (the script uses level 1 and only
+    takes a path ending in .ply).  Under torchrun the ranks split the sorted files (distributed.shard_range)."""
+    from . import distributed as D, isosurface, mrc
+    files = _shape_files(args)
+    if not files:
+        print(f'no .mrc files in {args.input_mrc_path}: nothing converted')
+        return
+    rank, world = _rank()
+    a, b = D.shard_range(len(files), rank, world)
+    err = None
+    try:
+        for path in files[a:b]:
+            out = os.path.splitext(path)[0] + '.ply'
+            verts, faces = isosurface.marching_cubes(mrc.read_mrc(path), args.level)
+            isosurface.write_ply(out, verts, faces)
+            print(f'wrote to {out}')
+    except Exception as e:
+        if world == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    D.agree(err)
+
+
 def gen_videos(args):
     """gen_videos_next3d.py: interpolation.mp4 over a --grid of seeds, or with --interpolate False one orbit video SEED.mp4 per seed."""
     from . import drivers
@@ -432,11 +478,14 @@ def reenact(args):
 
 def main(argv=None):
     args = _parser().parse_args(argv)
-    if not args.lms_cond:
+    if args.command != 'shape_utils' and not args.lms_cond:
         _refuse('pass --lms_cond True: the generator reads the 68 landmarks that follow the mesh vertices (load_lms)')
-    command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact, 'gen_dataset': gen_dataset}[args.command]
+    command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact, 'gen_dataset': gen_dataset,
+               'shape_utils': shape_utils}[args.command]
     if args.command == 'gen_dataset':
         _check_dataset_args(args)                            # the refusals, before the process group and the network
+    if args.command == 'shape_utils':
+        _shape_files(args)                                   # the refusals, before the process group and any CUDA work
     if _world() == 1:
         command(args)
         return

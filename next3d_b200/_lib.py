@@ -122,6 +122,9 @@ _SIGNATURES = {
     'n3d_h264_encode_rc': ([P, C.c_int, C.c_int, P, C.c_int, C.c_int, C.c_int, P, P, P, P, P, P, P, P], C.c_int),
     'n3d_png_buffer_sizes': ([C.c_int, C.c_int, C.c_int, C.POINTER(I64), C.POINTER(I64)], C.c_int),
     'n3d_png_encode': ([P, C.c_int, C.c_int, C.c_int, P, P, P, P], C.c_int),
+    'n3d_isosurface_workspace_bytes': ([C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)], C.c_int),
+    'n3d_isosurface_count': ([P, C.c_int, C.c_int, C.c_int, F32, P, P, P], C.c_int),
+    'n3d_isosurface_emit': ([P, C.c_int, C.c_int, C.c_int, F32, P, P, P, P], C.c_int),
     'n3d_sample_grid': ([P, C.c_int, C.c_int, C.c_int, F32, F32, I64, I64, C.c_int, F32, P, P, P, P, P, P], C.c_int),
 }
 

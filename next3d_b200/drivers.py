@@ -833,10 +833,8 @@ def trim_sigma_grid(sigmas, shape_res, pad_value=-1000.0):
     return sigmas
 
 
-def extract_sigma_grid(G, ws, v, shape_res=512, max_batch=1000000, noise_mode='const'):
-    """Density grid for marching cubes (gen_samples_next3d.py:208-238) -> float32 numpy [R,R,R], flipped and trimmed like the
-    script's.  The tri-planes are computed ONCE (the script's G.sample re-runs the three backbones for every 1M-point chunk: 17
-    times at 256^3, 135 times at 512^3), the query points are generated inside the decoding kernel and only sigma is decoded."""
+def _sigma_grid(G, ws, v, shape_res, noise_mode):
+    """The density grid of extract_sigma_grid, as a float32 CUDA tensor [R, R, R]."""
     from . import kernels as K
     eng = G._get_engine()
     eng.rk = G.rendering_kwargs
@@ -844,9 +842,25 @@ def extract_sigma_grid(G, ws, v, shape_res=512, max_batch=1000000, noise_mode='c
     box = G.rendering_kwargs['box_warp']
     sigmas = torch.empty(shape_res, shape_res, shape_res, device=planes.device)
     # one launch: voxel centres generated in the kernel (bit-identical to create_samples), flip + border trim fused into the store,
-    # border voxels (55 % of a 256^3 grid) never decoded.  max_batch is kept for API compatibility with the script's chunk size.
+    # border voxels (55 % of a 256^3 grid) never decoded
     K.sample_grid(planes[0], shape_res, box * 1, box, eng.dec, sigmas, pad=int(30 * shape_res / 256))
-    return sigmas.cpu().numpy()
+    return sigmas
+
+
+def extract_sigma_grid(G, ws, v, shape_res=512, max_batch=1000000, noise_mode='const'):
+    """Density grid for marching cubes (gen_samples_next3d.py:208-238) -> float32 numpy [R,R,R], flipped and trimmed like the
+    script's.  The tri-planes are computed ONCE (the script's G.sample re-runs the three backbones for every 1M-point chunk: 17
+    times at 256^3, 135 times at 512^3), the query points are generated inside the decoding kernel and only sigma is decoded.
+    max_batch is kept for API compatibility with the script's chunk size."""
+    return _sigma_grid(G, ws, v, shape_res, noise_mode).cpu().numpy()
+
+
+def extract_mesh(G, ws, v, shape_res=512, level=10.0, noise_mode='const'):
+    """Mesh of the density grid of extract_sigma_grid at `level` (the reference's shape_utils.py default 10) -> (verts float32
+    [V, 3], faces int32 [F, 3]) CUDA tensors (next3d_b200.isosurface.marching_cubes); the grid never leaves the device.  The
+    -1000 border trim keeps the mesh closed."""
+    from .isosurface import marching_cubes
+    return marching_cubes(_sigma_grid(G, ws, v, shape_res, noise_mode), level)
 
 
 # ------------------------------------------------------------------------------------------------ sample sheets (gen_samples_next3d.py)

@@ -1,5 +1,40 @@
-"""Write a density grid as an MRC2014 map (the `.mrc` shapes of gen_samples_next3d.py:244-246, viewable in ChimeraX)."""
+"""Write a density grid as an MRC2014 map (the `.mrc` shapes of gen_samples_next3d.py:244-246, viewable in ChimeraX), and read
+such maps back (the input of the shape_utils command)."""
+import os
+
 import numpy as np
+
+HEADER_BYTES = 1024
+
+
+def read_mrc(path):
+    """The float32 data [nz, ny, nx] of an MRC map, memory-mapped (copy-on-write): what write_mrc writes and what mrcfile's
+    new_mmap(..., mrc_mode=2) writes.  The extended header (NSYMBT bytes) is skipped.  ValueError, naming the field, for
+    anything else: a mode other than 2, a machine stamp other than little-endian, an axis order other than 1, 2, 3, or a file
+    shorter than its header says."""
+    size = os.path.getsize(path)
+    if size < HEADER_BYTES:
+        raise ValueError(f'{path}: {size} bytes, shorter than the {HEADER_BYTES}-byte MRC header')
+    with open(path, 'rb') as f:
+        raw = f.read(HEADER_BYTES)
+    stamp = raw[212:214]
+    if stamp not in (b'\x44\x44', b'\x44\x41'):
+        raise ValueError(f'{path}: machine stamp {raw[212:216].hex()} is not little-endian (44 44 00 00 or 44 41 00 00)')
+    h = np.frombuffer(raw, '<i4')
+    nx, ny, nz = (int(v) for v in h[0:3])
+    if h[3] != 2:
+        raise ValueError(f'{path}: mode {h[3]}: only mode 2 (float32) is read')
+    if tuple(h[16:19]) != (1, 2, 3):
+        raise ValueError(f'{path}: map order (mapc, mapr, maps) = {tuple(int(v) for v in h[16:19])}: only 1, 2, 3 is read')
+    if min(nx, ny, nz) < 1:
+        raise ValueError(f'{path}: dimensions (nx, ny, nz) = ({nx}, {ny}, {nz}) must be positive')
+    if h[23] < 0:
+        raise ValueError(f'{path}: nsymbt {h[23]} is negative')
+    offset = HEADER_BYTES + int(h[23])
+    if size < offset + 4 * nx * ny * nz:
+        raise ValueError(f'{path}: truncated: {size} bytes, the header (nx, ny, nz, nsymbt) = ({nx}, {ny}, {nz}, {h[23]}) needs '
+                         f'{offset + 4 * nx * ny * nz}')
+    return np.memmap(path, dtype='<f4', mode='c', offset=offset, shape=(nz, ny, nx))
 
 
 def write_mrc(path, data):
