@@ -514,6 +514,39 @@ int n3d_isosurface_count(const float* grid, int nz, int ny, int nx, float level,
 int n3d_isosurface_emit(const float* grid, int nz, int ny, int nx, float level, const void* workspace, float* verts, int32_t* faces,
                         void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Vertex colours of a shape mesh (next3d_b200/bake.py; DESIGN.md section 3.8).  Cameras are the renderer's: cam2world [views, 16]
+ * row-major and normalised intrinsics [views, 9], as n3d_render_rays reads them; a world point projects to camera depth z (the
+ * camera's +z axis) and pixel (u, w) = (xc * width - 0.5, yc * height - 0.5), pixel centres at integers.  Every operation is a
+ * rounded fp32 operation without contraction; the numpy restatement is tests/bake_oracle.py.
+ * ---------------------------------------------------------------------------------------------------------- */
+
+/* World points world [nv, 3] of mesh vertices verts [nv, 3] in voxel units (x, y, z) = (a2, a1, a0) of the flipped shape grid of
+ * create_samples(grid_n, cube): s1 = y + x / R, s0 = (R - 1 - z) + s1 / R, s2 = x, p = s * cube / (R - 1) - cube / 2.  grid_n >= 2,
+ * cube finite and positive.  Stream-ordered. */
+int n3d_bake_world_points(const float* verts, int64_t nv, int grid_n, float cube, float* world, void* stream);
+
+/* Z-buffer zbuf [views, height, width] (uint64, 8-byte aligned) of the triangles faces [nf, 3] (int32) over world points verts
+ * [nv, 3]: each pixel holds the least (depth bits << 32 | triangle id) over the triangles whose edges hold its centre (edges
+ * included), depth the perspective-correct camera depth there; ~0 where no triangle covers it.  Triangles with a vertex at z <= near,
+ * a vertex index outside [0, nv), zero signed area or non-finite corners are skipped.  The result does not depend on the launch.
+ * nv, nf < 2^31; near finite and positive.  Stream-ordered. */
+int n3d_mesh_zbuffer(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* cam2world, const float* intrinsics,
+                     int views, int height, int width, float near, uint64_t* zbuf, void* stream);
+
+/* colors [nv, 3] (uint8) of the vertices verts [nv, 3] (voxel units) at world points world [nv, 3] (n3d_bake_world_points), on the
+ * density grid [grid_n]^3 they were meshed from, from the images [views, 3, height, width] (float32, -1..1) and the z-buffer of
+ * n3d_mesh_zbuffer.  In view order, a vertex is visible when z > near, its nearest pixel lies in the image and z <= the pixel's depth
+ * + eps (an empty pixel is infinitely deep); its weight is visible * max(0, n . d)^2, n the normalised outward normal -grad sigma
+ * (trilinear central differences mapped to world space) and d the unit vector to the camera centre; the colour is the weighted
+ * mean of the images' bilinear samples, else (no weight) 2 f - 1 of f = fallback[i * fallback_stride + 0..2], the decoder's colour in
+ * the range n3d_sample_points writes (about 0..1; 2 f - 1 is the ray marcher's rescaling, what image_raw shows), as uint8 clamp(c * 127.5 + 128, 0,
+ * 255).  visible [views, nv] (uint8 0/1) and weights [views, nv] (float32) receive the per-view values unless NULL.  Stream-ordered. */
+int n3d_bake_vertex_colors(const float* verts, const float* world, int64_t nv, const float* grid, int grid_n, const float* cam2world,
+                           const float* intrinsics, int views, const float* images, int height, int width, const uint64_t* zbuf,
+                           float near, float eps, const float* fallback, int fallback_stride, uint8_t* colors, uint8_t* visible,
+                           float* weights, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

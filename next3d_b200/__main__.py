@@ -1,5 +1,7 @@
 """Standalone inference scripts: `python -m next3d_b200 {gen_samples,gen_videos,reenact} ...`, `gen_dataset` (multi-view
-training images in dataset_tool.py's layout) and `shape_utils` (the reference's .mrc -> .ply converter, marching cubes on the GPU).
+training images in dataset_tool.py's layout), `shape_utils` (the reference's .mrc -> .ply converter, marching cubes on the GPU) and
+`gen_meshes` (one coloured .ply mesh per seed: gen_samples' shape, meshed on the GPU, with the rendered views baked onto its
+vertices).
 
 The three subcommands are the reference's gen_samples_next3d.py, gen_videos_next3d.py and reenact_avatar_next3d.py with their option
 names, defaults and output file names, run on a network pickle read by next3d_b200.legacy (no reference checkout, no pickled code
@@ -144,6 +146,21 @@ def _parser():
     m = sub.add_parser('shape_utils', help=".mrc density grids -> .ply meshes (the reference's shape_utils.py), marching cubes on the GPU")
     m.add_argument('input_mrc_path', help='an .mrc file, or a directory whose *.mrc files are all converted')
     m.add_argument('--level', type=float, default=10, help='the isosurface level for marching cubes')
+
+    c = sub.add_parser('gen_meshes', help='coloured .ply meshes: the shape of gen_samples meshed on the GPU, the rendered views baked '
+                                          'onto its vertices')
+    c.add_argument('--network', required=True, help='network pickle (local file)')
+    c.add_argument('--seeds', type=_range, required=True)
+    c.add_argument('--obj_path', default=None)
+    c.add_argument('--lms_path', default=None)
+    c.add_argument('--trunc', dest='truncation_psi', type=float, default=1)
+    c.add_argument('--trunc-cutoff', dest='truncation_cutoff', type=int, default=14)
+    c.add_argument('--fov-deg', dest='fov_deg', type=float, default=18, help="as gen_samples (whose omitted --fov-deg is 18)")
+    c.add_argument('--shape-res', dest='shape_res', type=int, default=512)
+    c.add_argument('--level', type=float, default=10, help='the isosurface level for marching cubes')
+    c.add_argument('--outdir', required=True)
+    c.add_argument('--reload_modules', type=_bool, default=False)
+    c.add_argument('--lms_cond', type=_bool, default=False)
     return p
 
 
@@ -420,6 +437,44 @@ def shape_utils(args):
     D.agree(err)
 
 
+def _check_mesh_args(args):
+    if not math.isfinite(args.level):
+        _refuse(f'--level {args.level}: the isosurface level must be finite')
+    if args.shape_res < 2:
+        _refuse(f'--shape-res {args.shape_res}: the grid needs at least 2 voxels per side')
+    for opt, path in (('--obj_path', args.obj_path), ('--lms_path', args.lms_path)):
+        if path is None:
+            _refuse(f'{opt} is required: the generator renders every seed with that mesh')
+        if not os.path.isfile(path):
+            _refuse(f'{opt} {path}: no such file')
+
+
+def gen_meshes(args):
+    """seedNNNN.ply per seed: the density grid of gen_samples --shapes True (same latent and conditioning, sample_sheet_ws) meshed at
+    --level by marching cubes, with vertex colours baked from drivers.BAKE_VIEWS (drivers.coloured_meshes).  Under torchrun the
+    ranks split the seeds in whole calls (drivers.dataset_plan), so every file is that of one process."""
+    from . import distributed as D, drivers, isosurface
+    _check_mesh_args(args)
+    G = _load(args)
+    v = _mesh(args)
+    rank, world = _rank()
+    err = None
+    try:
+        os.makedirs(args.outdir, exist_ok=True)
+        ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
+        plan = drivers.dataset_plan(len(args.seeds), drivers.BAKE_BATCH, rank, world)
+        for i, verts, faces, colors in drivers.coloured_meshes(G, ws, v, plan, shape_res=args.shape_res, level=args.level,
+                                                               fov_deg=args.fov_deg, seed=SAMPLER_SEED):
+            out = os.path.join(args.outdir, f'seed{args.seeds[i]:04d}.ply')
+            isosurface.write_ply(out, verts, faces, colors)
+            print(f'wrote to {out}')
+    except Exception as e:
+        if world == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    D.agree(err)
+
+
 def gen_videos(args):
     """gen_videos_next3d.py: interpolation.mp4 over a --grid of seeds, or with --interpolate False one orbit video SEED.mp4 per seed."""
     from . import drivers
@@ -481,11 +536,13 @@ def main(argv=None):
     if args.command != 'shape_utils' and not args.lms_cond:
         _refuse('pass --lms_cond True: the generator reads the 68 landmarks that follow the mesh vertices (load_lms)')
     command = {'gen_samples': gen_samples, 'gen_videos': gen_videos, 'reenact': reenact, 'gen_dataset': gen_dataset,
-               'shape_utils': shape_utils}[args.command]
+               'shape_utils': shape_utils, 'gen_meshes': gen_meshes}[args.command]
     if args.command == 'gen_dataset':
         _check_dataset_args(args)                            # the refusals, before the process group and the network
     if args.command == 'shape_utils':
         _shape_files(args)                                   # the refusals, before the process group and any CUDA work
+    if args.command == 'gen_meshes':
+        _check_mesh_args(args)                               # the refusals, before the process group and the network
     if _world() == 1:
         command(args)
         return

@@ -113,6 +113,9 @@ _SIGNATURES = {
     'n3d_depth_clamp': ([P, I64, P, P], C.c_int),
     'n3d_depth_clamp_images': ([P, C.c_int, I64, P, P], C.c_int),
     'n3d_sample_points': ([P, C.c_int, C.c_int, C.c_int, P, I64, F32, P, P, P, P, P, P, P], C.c_int),
+    'n3d_bake_world_points': ([P, I64, C.c_int, F32, P, P], C.c_int),
+    'n3d_mesh_zbuffer': ([P, I64, P, I64, P, P, C.c_int, C.c_int, C.c_int, F32, P, P], C.c_int),
+    'n3d_bake_vertex_colors': ([P, P, I64, P, C.c_int, P, P, C.c_int, P, C.c_int, C.c_int, P, F32, F32, P, C.c_int, P, P, P, P], C.c_int),
     'n3d_render_floor': ([P, C.c_int, P, P], C.c_int),
     'n3d_mapping': ([P, P, C.c_int, F32, P, P, P, P, P, P, P, F32, C.c_int, C.c_int, P, P], C.c_int),
     'n3d_interp_rows': ([P, P, C.c_int, C.c_int, I64, P, P], C.c_int),

@@ -1077,3 +1077,72 @@ def render_dataset(G, ws, meshes, mesh_ids, cams, plan, seed=None):
             more = G.render_views(cams[idx, 1:].reshape(-1, 25), **_sampler_kw(seed, None, 2 * c + 1, None))['image']
             frames = torch.cat([frames, to_uint8_hwc(more).reshape(B, V - 1, *frames.shape[2:])], 1)
         yield idx[lo], frames[lo:hi].reshape(-1, *frames.shape[2:])
+
+
+# ------------------------------------------------------------------------------------------------------------- coloured meshes
+# The views baked onto a mesh: yaws -0.8 .. 0.8 at the sample sheets' pitch -0.2, and three yaws at pitch +0.2 that see under the
+# chin and brows.  Beyond |yaw| 0.8 (2.7 sigma of gen_dataset's default yaw spread 0.3) the generator leaves its training poses
+# and the images stop being trustworthy (DESIGN.md section 3.8).
+BAKE_VIEWS = tuple((yaw, SHEET_PITCH) for yaw in (-0.8, -0.4, 0.0, 0.4, 0.8)) + tuple((yaw, 0.2) for yaw in (-0.4, 0.0, 0.4))
+BAKE_BATCH = 3                         # heads per rendering call of coloured_meshes
+
+
+def bake_cameras(G, fov_deg=18.837):
+    """camera_params float32 [len(BAKE_VIEWS), 25] of the bake views: look_at_pose(pi / 2 + yaw, pi / 2 + pitch) around
+    avg_camera_pivot from avg_camera_radius with FOV_to_intrinsics(fov_deg), as sample_sheet_cameras builds the sheets' views."""
+    rk = G.rendering_kwargs
+    pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
+    radius = rk.get('avg_camera_radius', 2.7)
+    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
+    return torch.cat([torch.cat([camera.look_at_pose(np.pi / 2 + yaw, np.pi / 2 + pitch, pivot, radius).reshape(-1, 16), intr], 1)
+                      for yaw, pitch in BAKE_VIEWS])
+
+
+def coloured_meshes(G, ws, v, plan=None, batch=BAKE_BATCH, shape_res=512, level=10.0, fov_deg=18.837, seed=0):
+    """Coloured meshes of the heads ws [S, 28, 512] (sample_sheet_ws) with one mesh v [1, V, 3]: yields (i, verts float32 [V, 3],
+    faces int32 [F, 3], colors uint8 [V, 3]) CUDA tensors in head order, for the heads the plan owns (a CallPlan of heads in calls
+    of `batch`; default: all of them, local_plan).  Per call, one caching synthesis renders bake view 0 of its heads and one
+    render_views call the other views (sampler seeds seed + 2 c and seed + 2 c + 1 for the single-process call index c); each head's
+    density grid comes from its cached planes, is meshed by marching cubes (extract_mesh's mesh), and the views are baked onto the
+    vertices (next3d_b200.bake), with the decoder's colour at the vertex where no view sees it.  A short last call repeats its
+    last head."""
+    from .bake import bake_vertex_colors, mesh_zbuffer, world_points
+    from .isosurface import marching_cubes
+    if ws.ndim != 3 or ws.shape[0] == 0:
+        raise ValueError(f'ws must be [S >= 1, 28, 512], got {tuple(ws.shape)}')
+    if shape_res < 2:
+        raise ValueError(f'shape_res must be at least 2, got {shape_res}')
+    if v.ndim != 3 or v.shape[0] != 1:
+        raise ValueError(f'v must be one mesh [1, V, 3], got {tuple(v.shape)}')
+    device = next(G.parameters()).device
+    plan = local_plan(ws.shape[0], batch) if plan is None else plan
+    eng = G._get_engine()
+    cams = bake_cameras(G, fov_deg).to(device)
+    n = cams.shape[0]
+    v = v.to(device, torch.float32)
+    grid = torch.empty(shape_res, shape_res, shape_res, device=device) if plan.steps else None
+    keep = getattr(plan, 'keep', lambda k: (0, plan.valid(k)))
+    for k in range(plan.steps):
+        idx, (lo, hi) = plan.frames(k), keep(k)
+        B, c = len(idx), plan.step_id(k)
+        w = ws[idx].to(device, torch.float32)
+        front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True,
+                            **_sampler_kw(seed, None, 2 * c, None))['image']
+        more = G.render_views(cams[1:].repeat(B, 1), **_sampler_kw(seed, None, 2 * c + 1, None))['image']
+        images = torch.cat([front[:, None], more.reshape(B, n - 1, *more.shape[1:])], 1)          # [B, views, 3, H, W]
+        box = G.rendering_kwargs['box_warp']
+        for b in range(lo, hi):
+            eng.cached_sigma_grid(b, shape_res, grid)
+            verts, faces = marching_cubes(grid, level)
+            world = world_points(verts, shape_res, box)
+            _, feat = eng.cached_sample_points(b, world)
+            zbuf = mesh_zbuffer(world, faces, cams, images.shape[-2], images.shape[-1])
+            yield idx[b], verts, faces, bake_vertex_colors(verts, world, grid, cams, images[b], zbuf, feat, box)
+
+
+def extract_coloured_mesh(G, ws, v, shape_res=512, level=10.0, fov_deg=18.837, seed=0):
+    """The coloured mesh of one head ws [1, 28, 512] with mesh v [1, V, 3] -> (verts float32 [V, 3], faces int32 [F, 3], colors
+    uint8 [V, 3]) CUDA tensors: the geometry of extract_mesh(G, ws, v, shape_res, level), the colours of coloured_meshes (its
+    first call, sampler seeds seed and seed + 1)."""
+    _, verts, faces, colors = next(coloured_meshes(G, ws[:1], v, batch=1, shape_res=shape_res, level=level, fov_deg=fov_deg, seed=seed))
+    return verts, faces, colors

@@ -773,6 +773,25 @@ class Engine:
         with torch.cuda.device(self.device):
             K.sample_grid(c['planes'][b], shape_res, box * 1, box, self.dec, sigma, pad=int(30 * shape_res / 256))
 
+    def cached_sample_points(self, b, coords):
+        """The decoder at world points coords float32 [P, 3] of cached head b (G.sample's run_model on the planes the caching call
+        kept) -> (sigma [P], features [P, K.POINT_FEATURES], the width n3d_sample_points writes whatever the plane channels).  The
+        first three features are the decoder's colour, sigmoid(x) * 1.002 - 0.001; image_raw shows them as 2 f - 1 (the ray
+        marcher's rescaling of its composite).  One n3d_sample_points launch."""
+        c = self._cache
+        if not c.filled:
+            raise RuntimeError('next3d_b200: cached_sample_points needs cached planes: run synthesis(..., cache_backbone=True) first')
+        if not 0 <= b < c['B']:
+            raise RuntimeError(f'next3d_b200: cached_sample_points of head {b}, but the cache holds {c["B"]} head(s)')
+        self._on_device(coords=coords)
+        coords = coords.to(torch.float32).contiguous()
+        P = coords.shape[0]
+        sigma, feat = self._f32(1, P), self._f32(1, P, K.POINT_FEATURES)
+        if P:
+            with torch.cuda.device(self.device):
+                K.sample_points(c['planes'][b:b + 1], coords.view(1, P, 3), self.rk['box_warp'], self.dec, sigma, feat)
+        return sigma[0], feat[0]
+
     # ------------------------------------------------------------------------------------------ CUDA graph replay
     def _render_key(self, R):
         """The part of a graph key every graphed call shares: the rendering options a captured graph bakes in and the SR precision.

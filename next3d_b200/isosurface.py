@@ -57,16 +57,19 @@ def marching_cubes(grid, level=10.0):
     return verts, faces
 
 
-def ply_header(nverts, nfaces):
-    """The header plyfile writes for the reference's two elements (shape_utils.py:89-96)."""
+def ply_header(nverts, nfaces, colors=False):
+    """The header plyfile writes for the reference's two elements (shape_utils.py:89-96); with `colors`, the vertex element also
+    has uchar red, green and blue after z."""
+    rgb = 'property uchar red\nproperty uchar green\nproperty uchar blue\n' if colors else ''
     return (f'ply\nformat binary_little_endian 1.0\nelement vertex {nverts}\nproperty float x\nproperty float y\nproperty float z\n'
-            f'element face {nfaces}\nproperty list uchar int vertex_indices\nend_header\n').encode('ascii')
+            f'{rgb}element face {nfaces}\nproperty list uchar int vertex_indices\nend_header\n').encode('ascii')
 
 
-def ply_bytes(verts, faces):
+def ply_bytes(verts, faces, colors=None):
     """Binary little-endian PLY file of verts float32 [V, 3] and faces int32 [F, 3] (tensors on any device, or numpy arrays):
     the header, V x 12 bytes of vertices, then F x 13 bytes of faces (the count byte 3 and three int32 indices).  The face
-    records are packed where the faces are, and each array is read back once."""
+    records are packed where the faces are, and each array is read back once.  colors: uint8 [V, 3] vertex colours, written as
+    uchar red, green, blue after each vertex's z (15-byte vertex records); None writes the plain file."""
     verts, faces = torch.as_tensor(verts), torch.as_tensor(faces)
     if verts.dtype != torch.float32 or verts.dim() != 2 or verts.shape[1] != 3:
         raise ValueError(f'verts must be float32 [V, 3], got {verts.dtype} {list(verts.shape)}')
@@ -76,11 +79,20 @@ def ply_bytes(verts, faces):
         raise ValueError(f'verts are on {verts.device}, faces on {faces.device}')
     count = torch.full((faces.shape[0], 1), 3, dtype=torch.uint8, device=faces.device)
     records = torch.cat([count, faces.reshape(-1).view(torch.uint8).reshape(-1, 12)], 1)          # [F, 13]
-    return (ply_header(verts.shape[0], faces.shape[0]) + verts.contiguous().cpu().numpy().astype('<f4').tobytes()
-            + records.cpu().numpy().tobytes())
+    if colors is None:
+        vbytes = verts.contiguous().cpu().numpy().astype('<f4').tobytes()
+    else:
+        colors = torch.as_tensor(colors)
+        if colors.dtype != torch.uint8 or tuple(colors.shape) != (verts.shape[0], 3):
+            raise ValueError(f'colors must be uint8 [{verts.shape[0]}, 3], got {colors.dtype} {list(colors.shape)}')
+        if colors.device != verts.device:
+            raise ValueError(f'verts are on {verts.device}, colors on {colors.device}')
+        vrec = torch.cat([verts.contiguous().reshape(-1).view(torch.uint8).reshape(-1, 12), colors], 1)   # [V, 15]
+        vbytes = vrec.cpu().numpy().tobytes()
+    return ply_header(verts.shape[0], faces.shape[0], colors is not None) + vbytes + records.cpu().numpy().tobytes()
 
 
-def write_ply(path, verts, faces):
-    data = ply_bytes(verts, faces)
+def write_ply(path, verts, faces, colors=None):
+    data = ply_bytes(verts, faces, colors)
     with open(path, 'wb') as f:
         f.write(data)

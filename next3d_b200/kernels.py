@@ -381,6 +381,9 @@ def depth_clamp_images(depth, depth_minmax):
     _run('n3d_depth_clamp_images', ptr(depth), N, depth.numel() // max(N, 1), ptr(depth_minmax), stream_ptr())
 
 
+POINT_FEATURES = 32            # channels n3d_sample_points writes per point (the decoder's output after sigma)
+
+
 def sample_points(planes, coords, box_warp, dec, sigma, rgb=None):
     N, _, PH, PW, _ = planes.shape
     Pn = coords.shape[1]
