@@ -119,11 +119,18 @@ def inv4(d):
     return (h + 32) >> 6
 
 
-def quant(w, qp, intra, dc_shift=0, mf=None):
+def quant(w, qp, intra, dc_shift=0, mf=None, census=None, kind=None):
+    """Levels of coefficients w [..., 4, 4] (or of a DC transform); census (a Counter, or None) counts the levels of this block
+    kind clamped to LEVEL_MAX (for an AC kind, outside the DC position, whose level the caller drops)."""
     qbits = 15 + qp // 6 + dc_shift
     f = ((1 << (15 + qp // 6)) // (3 if intra else 6)) << dc_shift
     mf = MF4[qp % 6] if mf is None else mf
     lv = (np.abs(w) * mf + f) >> qbits
+    if census is not None:
+        over = lv > LEVEL_MAX
+        if kind.endswith('AC'):
+            over[..., 0, 0] = False
+        census['clamp', kind] += int(over.sum())
     return (np.sign(w) * np.minimum(lv, LEVEL_MAX)).astype(np.int64)
 
 
@@ -164,14 +171,15 @@ def scan(b):
     return b.reshape(b.shape[:-2] + (16,))[..., ZZ]
 
 
-def code_chroma(src, pred, qpc, intra):
+def code_chroma(src, pred, qpc, intra, census=None):
     """One chroma component of a batch of macroblocks: src, pred [..., 8, 8] -> (DC levels [..., 4], AC levels [..., 4, 16] in
     zig-zag order (index 0 unused), reconstruction [..., 8, 8])."""
+    frame = 'I' if intra else 'P'
     w = fwd4(cblocks(src.astype(np.int64) - pred))
     dc = w[..., 0, 0]
     t = np.einsum('ij,...jk,kl->...il', A2, dc.reshape(dc.shape[:-1] + (2, 2)), A2)
-    dcl = quant(t, qpc, intra, 1, MF4[qpc % 6][0, 0]).reshape(dc.shape)
-    acl = quant(w, qpc, intra)
+    dcl = quant(t, qpc, intra, 1, MF4[qpc % 6][0, 0], census, f'{frame} chroma DC').reshape(dc.shape)
+    acl = quant(w, qpc, intra, census=census, kind=f'{frame} chroma AC')
     acl[..., 0, 0] = 0
     f = np.einsum('ij,...jk,kl->...il', A2, dcl.reshape(dcl.shape[:-1] + (2, 2)), A2)
     dcc = ((f * LS4[qpc % 6][0, 0]) << (qpc // 6)) >> 5
@@ -193,8 +201,9 @@ def se_bits(v):
 
 
 class Bits:
-    def __init__(self):
+    def __init__(self, census=None):
         self.parts = []
+        self.census = census                  # a Counter of the CAVLC syntax written (residual_block), or None
 
     def u(self, v, n):
         if n:
@@ -231,11 +240,16 @@ def residual_block(bw, coeffs, nc):
             break
         t1 += 1
     idx = 4 * total + t1
+    rec = bw.census
     if nc == -1:
         bw.u(CDC_CT_BITS[idx], CDC_CT_LEN[idx])
     else:
         tab = 0 if nc < 2 else 1 if nc < 4 else 2 if nc < 8 else 3
         bw.u(CT_BITS[tab][idx], CT_LEN[tab][idx])
+    if rec is not None:
+        rec['coeff_token', 'chroma DC' if nc == -1 else ('nC 0-1', 'nC 2-3', 'nC 4-7', 'nC >= 8')[tab]] += 1
+        if nc != -1 and total:
+            rec['TotalCoeff', total] += 1
     if total == 0:
         return 0
     levels = [coeffs[i] for i in reversed(nz)]
@@ -260,6 +274,9 @@ def residual_block(bw, coeffs, nc):
             prefix, sbits, sval = 15, 12, code - (15 << sl)
         bw.u(1, prefix + 1)
         bw.u(sval, sbits)
+        if rec is not None:
+            rec['level_prefix', prefix] += 1
+            rec['suffixLength', sl] += 1
         if sl == 0:
             sl = 1
         if abs(lv) > (3 << (sl - 1)) and sl < 6:
@@ -267,6 +284,9 @@ def residual_block(bw, coeffs, nc):
     n = len(coeffs)
     if total < n:
         tz = nz[-1] + 1 - total
+        if rec is not None:
+            rec['total_zeros', 'chroma DC' if nc == -1 else '4x4', total] += 1
+            rec['total_zeros pair', 'chroma DC' if nc == -1 else '4x4', total, tz] += 1
         if nc == -1:
             bw.u(CDC_TZ_BITS[total - 1][tz], CDC_TZ_LEN[total - 1][tz])
         else:
@@ -278,6 +298,8 @@ def residual_block(bw, coeffs, nc):
             run = nz[j] - nz[j - 1] - 1
             t = min(left, 7) - 1
             bw.u(RUN_BITS[t][run], RUN_LEN[t][run])
+            if rec is not None:
+                rec['run_before', 'zerosLeft > 6' if t == 6 else f'zerosLeft {t + 1}'] += 1
             left -= run
     return total
 
@@ -310,6 +332,8 @@ def mv_of(key):
 class Encoder:
     """The constant-QP stream: encodes uint8 RGB frames into length-prefixed slice NAL units, one sample per frame.  The first
     frame and every gop-th one after it is IDR."""
+
+    census = None                             # a Counter of the syntax and decisions of every frame encoded, or None (see record())
 
     def __init__(self, width, height, qp=18, gop=60):
         if width % 2 or height % 2 or width <= 0 or height <= 0:
@@ -347,8 +371,8 @@ class Encoder:
             w = fwd4(blocks(src - pred))                                     # [R, 16, 4, 4]
             dcm = unblocks_dc(w[..., 0, 0])                                  # [R, 4, 4] spatial
             hd = (HAD @ dcm @ HAD) >> 1
-            dcl = quant(hd, qp, True, 1, MF4[qp % 6][0, 0])
-            acl = quant(w, qp, True)
+            dcl = quant(hd, qp, True, 1, MF4[qp % 6][0, 0], self.census, 'I luma DC')
+            acl = quant(w, qp, True, census=self.census, kind='I luma AC')
             acl[..., 0, 0] = 0
             c4 = HAD @ dcl @ HAD
             if qp >= 36:
@@ -368,7 +392,7 @@ class Encoder:
                     bot = (lc[:, 4:8].sum(-1) + 2) >> 2
                     cp = np.concatenate([np.repeat(top[:, None, None], 4, 1), np.repeat(bot[:, None, None], 4, 1)], 1)
                     cp = np.repeat(cp, 8, -1)
-                dcl_c, acl_c, rec_c = code_chroma(sb[:, c], cp, qpc, True)
+                dcl_c, acl_c, rec_c = code_chroma(sb[:, c], cp, qpc, True, self.census)
                 rb[:, c] = rec_c
                 cres.append((dcl_c, acl_c))
             for r in range(R):
@@ -412,8 +436,13 @@ class Encoder:
         ry, ru, rv = (p.astype(np.int64) for p in self.recon)
         cur = Y.astype(np.int64)
         qx, qy, pred = self._search(ry, cur)
+        if self.census is not None:
+            for x, y in zip((qx & 3).ravel().tolist(), (qy & 3).ravel().tolist()):
+                self.census['quarter-sample position', x, y] += 1
+            self.census['vector at the search bound',] += int((np.maximum(np.abs(qx), np.abs(qy)) >= 4 * SEARCH).sum())
+            self.census['vector refined past the search bound',] += int((np.maximum(np.abs(qx), np.abs(qy)) > 4 * SEARCH).sum())
         w = fwd4(blocks(_mb_view(cur, 16) - pred))
-        lvl = quant(w, qp, False)                                             # [R, C, 16, 4, 4]
+        lvl = quant(w, qp, False, census=self.census, kind='P luma')          # [R, C, 16, 4, 4]
         rec_y = np.clip(pred + unblocks(inv4(dequant(lvl, qp))), 0, 255)
         # chroma: eighth-sample bilinear (8.4.2.2.2) at the luma vector, whose quarter samples are chroma eighth samples
         fx, fy = (qx & 7)[:, :, None, None], (qy & 7)[:, :, None, None]
@@ -424,7 +453,7 @@ class Encoder:
             at = lambda y, x: rp[np.clip(y, 0, H16 // 2 - 1), np.clip(x, 0, W16 // 2 - 1)]
             cp = ((8 - fx) * (8 - fy) * at(cy, cx) + fx * (8 - fy) * at(cy, cx + 1) + (8 - fx) * fy * at(cy + 1, cx)
                   + fx * fy * at(cy + 1, cx + 1) + 32) >> 6
-            dcl_c, acl_c, rec_c = code_chroma(_mb_view(sp.astype(np.int64), 8), cp, qpc, False)
+            dcl_c, acl_c, rec_c = code_chroma(_mb_view(sp.astype(np.int64), 8), cp, qpc, False, self.census)
             cres.append((dcl_c, acl_c))
             crec.append(rec_c)
         nonzero = (lvl != 0).any((-1, -2, -3)) | (cres[0][0] != 0).any(-1) | (cres[0][1] != 0).any((-1, -2)) \
@@ -443,7 +472,8 @@ class Encoder:
         bw.ue(1)                                   # disable_deblocking_filter_idc
 
     def _slice(self, row, mbs, idr, frame_num, idr_pic_id):
-        bw = Bits()
+        rec = self.census
+        bw = Bits(rec)
         bw.ue(row * self.mbw)                      # first_mb_in_slice
         bw.ue(2 if idr else 0)                     # slice_type I / P
         bw.ue(0)                                   # pic_parameter_set_id
@@ -471,12 +501,16 @@ class Encoder:
                 nz_ac = any(np.any(m['lac'][k][1:]) for k in range(16))
                 cbp_l = 15 if nz_ac else 0
             else:
+                if rec is not None and skip_run:
+                    rec['skip run', 'row start' if skip_run == c else 'mid-row'] += 1
                 bw.ue(skip_run)
                 skip_run = 0
                 cbp_l = sum(1 << q for q in range(4) if any(np.any(m['lac'][4 * q + k]) for k in range(4)))
             cdc_nz = any(np.any(x) for x in m['cdc'])
             cac_nz = any(np.any(x[:, 1:]) for x in m['cac'])
             cbp_c = 2 if cac_nz else 1 if cdc_nz else 0
+            if rec is not None:
+                rec[('I16x16', m['mode'], cbp_c, cbp_l) if idr else ('P cbp', cbp_l, cbp_c)] += 1
             if idr:
                 bw.ue(1 + m['mode'] + 4 * cbp_c + (12 if cbp_l else 0))     # mb_type I_16x16_<mode>_<cbp_c>_<cbp_l>
                 bw.ue(0)                                                    # intra_chroma_pred_mode DC
@@ -508,7 +542,13 @@ class Encoder:
             left_cc = [[int(cc[comp][by, 1]) for by in range(2)] for comp in range(2)]
         if skip_run:
             bw.ue(skip_run)
-        nal = bytes([0x65 if idr else 0x61]) + escape(bw.rbsp())
+        rbsp = bw.rbsp()
+        nal = bytes([0x65 if idr else 0x61]) + escape(rbsp)
+        if rec is not None:
+            if skip_run:
+                rec['skip run', 'whole row' if skip_run == len(mbs) else 'row end'] += 1
+            rec['emulation prevention bytes'] += len(nal) - 1 - len(rbsp)
+            rec['slice bytes max'] = max(rec['slice bytes max'], 4 + len(nal))
         return len(nal).to_bytes(4, 'big') + nal
 
     def encode(self, rgb):
@@ -527,9 +567,29 @@ class Encoder:
         R, C = self.mbh, self.mbw
         self.recon = tuple(p.swapaxes(1, 2).reshape(R * p.shape[2], C * p.shape[3]).astype(np.uint8) for p in rec)
         idr_pic_id = (self.n // self.gop) % 2
+        if self.census is not None:
+            self._record_frame(idr, k, idr_pic_id)
         sample = b''.join(self._slice(r, mbs[r], idr, k % 16, idr_pic_id) for r in range(R))
         self.n += 1
         return sample, idr
+
+
+    def record(self, census):
+        """Counts the syntax elements and decisions of the frames encoded from now on into census (a Counter; None stops).  The
+        bytes do not change."""
+        self.census = census
+        return self
+
+    def _record_frame(self, idr, k, idr_pic_id):
+        rec, W, H, R, C = self.census, self.W, self.H, self.mbh, self.mbw
+        rec['qp', 'I' if idr else 'P', self.qp] += 1
+        rec['frame_num wrap',] += int(k > 0 and k % 16 == 0)
+        if idr:
+            rec['idr_pic_id', idr_pic_id] += 1
+        for name, hit in (('2-sample crop remainder', W % 16 == 2 or H % 16 == 2), ('more than 32 MB rows', R > 32),
+                          ('more than 256 MB rows', R > 256), ('1 MB column, several rows', C == 1 and R > 1),
+                          ('2 MB columns, several rows', C == 2 and R > 1), ('more than 1024 MB columns', C > 1024)):
+            rec['size', name] += int(hit)
 
 
 def unblocks_dc(dc):
@@ -592,14 +652,21 @@ TC0 = [(0, 0, 0)] * 17 + [(0, 0, 1)] * 4 + [(0, 1, 1)] * 2 + [(1, 1, 1)] * 4 + [
     (6, 8, 11), (6, 8, 13), (7, 10, 14), (8, 11, 16), (9, 12, 18), (10, 13, 20), (11, 15, 23), (13, 17, 25)]
 
 
-def _filter(s, bS, idx, chroma):
-    """Filter lines across one edge: s [..., 8] luma samples p3..q3, or [..., 4] chroma p1..q1; bS [...]; idx = indexA = indexB."""
+def _filter(s, bS, idx, chroma, census=None):
+    """Filter lines across one edge: s [..., 8] luma samples p3..q3, or [..., 4] chroma p1..q1; bS [...]; idx = indexA = indexB.
+    census (a Counter, or None) counts the lines per (bS, whether the sample test |p0 - q0| < alpha, |p1 - p0| < beta,
+    |q1 - q0| < beta passes), so that bS 0 with a passing test (no filtering all the same) is counted too."""
     a, be = ALPHA[idx], BETA[idx]
     if chroma:
         p1, p0, q0, q1 = (s[..., k] for k in range(4))
     else:
         p3, p2, p1, p0, q0, q1, q2, q3 = (s[..., k] for k in range(8))
-    on = (bS > 0) & (np.abs(p0 - q0) < a) & (np.abs(p1 - p0) < be) & (np.abs(q1 - q0) < be)
+    test = (np.abs(p0 - q0) < a) & (np.abs(p1 - p0) < be) & (np.abs(q1 - q0) < be)
+    on = (bS > 0) & test
+    if census is not None:
+        for b in range(5):
+            for t in (True, False):
+                census['bS', 'chroma' if chroma else 'luma', b, 'filtered' if t else 'not filtered'] += int(((bS == b) & (test == t)).sum())
     weak, strong = on & (bS < 4), on & (bS == 4)
     tc0 = np.array((0,) + TC0[idx])[np.minimum(bS, 3)]
     out = s.copy()
@@ -648,7 +715,7 @@ def boundary_strength(intra, nz, mv):
     return bv, bh
 
 
-def deblock(planes, qp, bv, bh):
+def deblock(planes, qp, bv, bh, census=None):
     """In-place deblocking of padded (Y, Cb, Cr) int64 planes in the standard's order (per MB in raster order: vertical edges
     left to right, then horizontal edges top to bottom), run on the MBs of one wavefront x + 2y at a time: an MB's filtering only
     touches samples that the MBs to its left and above-right finished with."""
@@ -672,7 +739,7 @@ def deblock(planes, qp, bv, bh):
                     iy, ix = along(16 * rr, 16, 0)[:, :, None], along(16 * cc + 4 * e, 8, -4)[:, None, :]
                 else:
                     iy, ix = along(16 * rr + 4 * e, 8, -4)[:, None, :], along(16 * cc, 16, 0)[:, :, None]
-                Y[iy, ix] = _filter(Y[iy, ix], np.repeat(strength, 4, 1), qp, False)
+                Y[iy, ix] = _filter(Y[iy, ix], np.repeat(strength, 4, 1), qp, False, census)
                 if e % 2:
                     continue
                 cs = np.repeat(strength, 2, 1)                                            # chroma edge 4e/2 = luma edge e
@@ -681,7 +748,7 @@ def deblock(planes, qp, bv, bh):
                 else:
                     iy, ix = along(8 * rr + 2 * e, 4, -2)[:, None, :], along(8 * cc, 8, 0)[:, :, None]
                 for p in (U, V):
-                    p[iy, ix] = _filter(p[iy, ix], cs, qpc, True)
+                    p[iy, ix] = _filter(p[iy, ix], cs, qpc, True, census)
 
 
 # ------------------------------------------------------------------------------------------------ rate control
@@ -706,7 +773,9 @@ class RateControl:
             x, q = 2 * x, q + 6
         self.qp = min(max(q, qp_min), qp_max)
 
-    def update(self, nbytes, idr):
+    def update(self, nbytes, idr, census=None):
+        """census (a Counter, or None) counts the steps, the clamps at the QP bounds and the updates after an IDR frame that
+        follows an IDR frame."""
         bits = 8 * nbytes * self.num
         budget = self.bitrate * self.den
         sat = 8 * self.bitrate * self.num                        # the bucket saturates at +-8 s
@@ -715,6 +784,11 @@ class RateControl:
             want = max(budget - _fdiv(self.fullness, max(1, self.num // self.den)), budget // 8)
             step = (2 if 100 * bits > 141 * want else 1 if 100 * bits > 112 * want else
                     -2 if 141 * bits < 100 * want else -1 if 112 * bits < 100 * want else 0)
+            if census is not None:
+                census['rc', f'step {step:+d}'] += 1
+                census['rc', 'clamped at qp_min'] += int(self.qp + step < self.qp_min)
+                census['rc', 'clamped at qp_max'] += int(self.qp + step > self.qp_max)
+                census['rc', 'IDR frame after an IDR frame'] += int(idr)
             self.qp = min(max(self.qp + step, self.qp_min), self.qp_max)
         self.prev_idr = int(idr)
         self.frames += 1
@@ -770,9 +844,9 @@ class RcEncoder(Encoder):
         else:
             nz, mv = unblocks_dc(self.levels.any((-1, -2))), self.mvs
         planes = tuple(p.astype(np.int64) for p in self.recon)
-        deblock(planes, self.qp, *boundary_strength(idr, nz, mv))
+        deblock(planes, self.qp, *boundary_strength(idr, nz, mv), self.census)
         self.recon = tuple(p.astype(np.uint8) for p in planes)
-        self.rc.update(len(sample), idr)
+        self.rc.update(len(sample), idr, self.census)
         self.qps.append(self.qp)
         return sample, idr
 
@@ -838,6 +912,122 @@ def pan(W, H, n=3):
     return out
 
 
+# ------------------------------------------------------------------------------------------------ edge sequences
+# Built to reach the coding edges the sequences above do not (tests/test_h264_edges_cpu.py counts what they reach):
+# - 'stripes': 16-sample blue / yellow columns under noise, the colours swapping every frame.  At QP 0 the I_16x16 luma DC and the
+#   chroma DC of every MB after the first column exceed LEVEL_MAX, the noise fills every AC coefficient with large levels (escape
+#   codes, suffixLength 6), and the P frames match the swapped columns at +-16 samples, the search bound.
+# - 'cut': flat yellow, flat blue, then noise: a P frame whose chroma DC exceeds LEVEL_MAX, then a scene cut inside the GOP (a P
+#   frame with IDR-sized residuals).
+# - 'static': a still picture in which a sparse set of MBs shows the picture zoomed about its centre (a little more every
+#   frame): skip runs at the start, in the middle and at the end of a row, rows of skips, and a vector field that takes every
+#   quarter-sample position.
+# - 'motion': the smooth pattern moved by (+16.75, -16.75), (-16.75, +16.75), then (+24, +24) samples per frame: vectors at the
+#   search bound refined past it, and motion beyond it, with the reference blocks of the border MBs wholly outside the frame.
+# - 'cbp': a still, softened pattern; in the P frames MB k gets grey noise in the 8x8 quadrants of the bits of k % 16 and, by
+#   (k // 16 + t - 1) % 3 in frame t, no change of colour, a flat tint (chroma DC only) or a tint in a checker of 4x4 blocks (chroma AC): at
+#   moderate QPs, with 48 MBs, every coded_block_pattern of a P MB.
+# - 'mosaic': MB-sized tiles (flat grey, grey noise, a flat colour, grey noise, the rows of the left tile's last column tinted,
+#   the smooth pattern) that make every I_16x16 mb_type across the QPs; the noise and the pattern change in every frame.
+EDGE_SEQUENCES = ('stripes', 'cut', 'static', 'motion', 'cbp', 'mosaic')
+TINT = (39, -20, 0)                                 # an RGB offset that moves Cb and Cr but not Y (66 * 39 - 129 * 20 = -6)
+BLUE, YELLOW = (0, 0, 255), (255, 255, 0)           # Y 41 / 210, Cb 240 / 16: far apart in luma and in Cb
+MOTION = [(16.75, -16.75), (-16.75, 16.75), (24, 24)]
+
+
+def _smooth(H, W, ox=0.0, oy=0.0, zoom=1.0):
+    """_pattern's analytic pattern sampled at ((x - W/2) / zoom + W/2 + ox, (y - H/2) / zoom + H/2 + oy)."""
+    rng = np.random.RandomState(1)
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    x, y = (x - W / 2) / zoom + W / 2 + ox, (y - H / 2) / zoom + H / 2 + oy
+    img = np.zeros((H, W, 3))
+    for c in range(3):
+        for _ in range(6):
+            fx, fy, ph = rng.uniform(0.02, 0.25, 2).tolist() + [rng.uniform(0, 6.3)]
+            img[..., c] += np.sin(fx * x + fy * y + ph) * rng.uniform(10, 30)
+    return np.clip(img + 128, 0, 255).astype(np.uint8)
+
+
+def edge_sequence(name, W, H, n=3):
+    """n uint8 RGB frames [H, W, 3] of one of EDGE_SEQUENCES."""
+    if name == 'stripes':
+        col = (np.arange(W) // 16) % 2
+        out = []
+        for t in range(n):
+            base = np.where((col ^ (t % 2))[None, :, None] == 1, BLUE, YELLOW) * np.ones((H, 1, 1), np.int64)
+            noise = np.random.RandomState(7 + t).randint(-48, 49, (H, W, 3))
+            out.append(np.clip(base + noise, 0, 255).astype(np.uint8))
+        return out
+    if name == 'cut':
+        pics = [lambda: np.full((H, W, 3), YELLOW, np.uint8), lambda: np.full((H, W, 3), BLUE, np.uint8),
+                lambda: np.random.RandomState(11).randint(0, 256, (H, W, 3)).astype(np.uint8)]
+        return [pics[t % 3]() for t in range(n)]
+    if name == 'static':
+        still = _smooth(H, W)
+        R, C = (H + 15) // 16, (W + 15) // 16
+        out = [still]
+        for t in range(1, n):
+            zoomed = _smooth(H, W, zoom=1 + 0.02 * t)
+            f = still.copy()
+            for r in range(0, R, 3):                       # rows 0, 3, 6, ...: MB columns 1, 6, 11, ... (column 0 if it is the only one)
+                for c in range(min(1, C - 1), C, 5):
+                    f[16 * r:16 * r + 16, 16 * c:16 * c + 16] = zoomed[16 * r:16 * r + 16, 16 * c:16 * c + 16]
+            out.append(f)
+        return out
+    if name == 'cbp':
+        still = (_smooth(H, W).astype(np.int64) - 128) // 3 + 128
+        R, C = (H + 15) // 16, (W + 15) // 16
+        out = [still.astype(np.uint8)]
+        for t in range(1, n):
+            rng = np.random.RandomState(20 + t)
+            f = still.copy()
+            for k in range(R * C):
+                y0, x0 = 16 * (k // C), 16 * (k % C)
+                for q in range(4):
+                    if k % 16 >> q & 1:
+                        ys, xs = slice(y0 + 8 * (q // 2), y0 + 8 * (q // 2) + 8), slice(x0 + 8 * (q % 2), x0 + 8 * (q % 2) + 8)
+                        f[ys, xs] += rng.randint(-24, 25, f[ys, xs].shape[:2])[..., None]
+                tint = (k // 16 + t - 1) % 3
+                if tint:
+                    sign = np.ones((16, 16), np.int64) if tint == 1 else np.kron([[1, -1, 1, -1], [-1, 1, -1, 1]] * 2, np.ones((4, 4), np.int64))
+                    f[y0:y0 + 16, x0:x0 + 16] += (sign[..., None] * TINT)[:f[y0:y0 + 16].shape[0], :f[:, x0:x0 + 16].shape[1]]
+            out.append(np.clip(f, 0, 255).astype(np.uint8))
+        return out
+    if name == 'mosaic':
+        R, C = (H + 15) // 16, (W + 15) // 16
+        out = []
+        for t in range(n):
+            rng = np.random.RandomState(30 + t)
+            f = np.zeros((16 * R, 16 * C, 3), np.int64)
+            smooth = _smooth(16 * R, 16 * C, 1.25 * t, -0.5 * t)
+            for k in range(R * C):
+                y0, x0 = 16 * (k // C), 16 * (k % C)
+                tile = f[y0:y0 + 16, x0:x0 + 16]
+                kind = k % 6
+                if kind == 0:
+                    tile[:] = 128
+                elif kind in (1, 3):
+                    tile[:] = rng.randint(40, 200, (16, 16))[..., None]
+                elif kind == 2:
+                    tile[:] = (200, 120, 60)
+                elif kind == 4:
+                    left = f[y0:y0 + 16, x0 - 1] if x0 else np.full((16, 3), 128)
+                    tile[:] = (left + TINT)[:, None, :]
+                else:
+                    tile[:] = smooth[y0:y0 + 16, x0:x0 + 16]
+            out.append(np.clip(f[:H, :W], 0, 255).astype(np.uint8))
+        return out
+    if name == 'motion':
+        o, out = np.zeros(2), []
+        for t in range(n):
+            out.append(_smooth(H, W, *o))
+            o = o + MOTION[t % len(MOTION)]
+        return out
+    raise ValueError(name)
+
+
 def frames(name, W, H, n=3):
-    """sequence(), and 'pan'."""
-    return pan(W, H, n) if name == 'pan' else sequence(name, W, H, n)
+    """sequence(), 'pan' and edge_sequence()."""
+    if name == 'pan':
+        return pan(W, H, n)
+    return edge_sequence(name, W, H, n) if name in EDGE_SEQUENCES else sequence(name, W, H, n)
