@@ -265,7 +265,7 @@ def _write_video_n3d(path, shard, fps, gop, qp, bitrate=None):
 
 def gen_samples(args):
     """gen_samples_next3d.py: seedNNNN.png sheets and, with --shapes, seedNNNN.mrc density grids.  Under torchrun every rank renders
-    and writes the seeds of its whole calls (drivers.sheet_span)."""
+    and writes the seeds of its whole calls (drivers.head_plan)."""
     import PIL.Image
     from . import distributed as D, drivers, mrc
     if args.shape_format == '.ply':
@@ -274,23 +274,18 @@ def gen_samples(args):
     G = _load(args)
     v = _mesh(args)
     rank, world = _rank()
-    err = None
-    try:
+
+    def body():
         os.makedirs(args.outdir, exist_ok=True)
         ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
-        a, b, call = drivers.sheet_span(len(args.seeds), 9, rank, world)
-        if a < b:
-            for i, sheet, sigmas in drivers.render_sample_sheets(G, ws[a:b], v, fov_deg=args.fov_deg, shapes=args.shapes,
-                                                                 shape_res=args.shape_res, seed=SAMPLER_SEED + 2 * call):
-                name = os.path.join(args.outdir, f'seed{args.seeds[a + i]:04d}')
-                PIL.Image.fromarray(sheet, 'RGB').save(name + '.png')
-                if sigmas is not None:
-                    mrc.write_mrc(name + '.mrc', sigmas)
-    except Exception as e:
-        if world == 1:
-            raise
-        err = f'{type(e).__name__}: {e}'
-    D.agree(err)
+        plan = drivers.head_plan(len(args.seeds), 3, rank, world)
+        for i, sheet, sigmas in drivers.render_sample_sheets(G, ws, v, fov_deg=args.fov_deg, shapes=args.shapes, shape_res=args.shape_res,
+                                                             seed=SAMPLER_SEED, plan=plan):
+            name = os.path.join(args.outdir, f'seed{args.seeds[i]:04d}')
+            PIL.Image.fromarray(sheet, 'RGB').save(name + '.png')
+            if sigmas is not None:
+                mrc.write_mrc(name + '.mrc', sigmas)
+    D.run_together(body)
 
 
 def _check_dataset_args(args):
@@ -343,8 +338,8 @@ def gen_dataset(args):
         _refuse(f'--expressions {K}: the driving directory has {len(sources)} frames')
     G = _load(args)
     rank, world = _rank()
-    err = None
-    try:
+
+    def body():
         head_seeds, head_exprs = drivers.dataset_heads(args.seeds, K, len(sources))
         used = sorted(set(head_exprs))
         meshes = torch.cat([inputs.load_frame(*sources[e]) for e in used])
@@ -364,7 +359,7 @@ def gen_dataset(args):
                 json.dump({'labels': labels}, f)
             np.savez(os.path.join(args.outdir, 'heads.npz'), seed=np.array(head_seeds, np.int64),
                      expression=np.array(head_exprs, np.int64), ws=ws.float().cpu().numpy())
-        plan = drivers.dataset_plan(len(head_seeds), args.batch, rank, world)
+        plan = drivers.head_plan(len(head_seeds), args.batch, rank, world)
         enc = PngEncoder(G.img_resolution, G.img_resolution, batch=2 * args.batch * V)
         first_link = {}                                  # expression -> this rank's first mesh / landmark files of it
         pending = []                                     # image ids submitted to the encoder, not yet written
@@ -391,11 +386,7 @@ def gen_dataset(args):
                 pending.append(i)
             save(enc.write(frames))
         save(enc.flush())
-    except Exception as e:
-        if world == 1:
-            raise
-        err = f'{type(e).__name__}: {e}'
-    D.agree(err)
+    D.run_together(body)
 
 
 def _shape_files(args):
@@ -423,18 +414,14 @@ def shape_utils(args):
         return
     rank, world = _rank()
     a, b = D.shard_range(len(files), rank, world)
-    err = None
-    try:
+
+    def body():
         for path in files[a:b]:
             out = os.path.splitext(path)[0] + '.ply'
             verts, faces = isosurface.marching_cubes(mrc.read_mrc(path), args.level)
             isosurface.write_ply(out, verts, faces)
             print(f'wrote to {out}')
-    except Exception as e:
-        if world == 1:
-            raise
-        err = f'{type(e).__name__}: {e}'
-    D.agree(err)
+    D.run_together(body)
 
 
 def _check_mesh_args(args):
@@ -452,27 +439,23 @@ def _check_mesh_args(args):
 def gen_meshes(args):
     """seedNNNN.ply per seed: the density grid of gen_samples --shapes True (same latent and conditioning, sample_sheet_ws) meshed at
     --level by marching cubes, with vertex colours baked from drivers.BAKE_VIEWS (drivers.coloured_meshes).  Under torchrun the
-    ranks split the seeds in whole calls (drivers.dataset_plan), so every file is that of one process."""
+    ranks split the seeds in whole calls (drivers.head_plan), so every file is that of one process."""
     from . import distributed as D, drivers, isosurface
     _check_mesh_args(args)
     G = _load(args)
     v = _mesh(args)
     rank, world = _rank()
-    err = None
-    try:
+
+    def body():
         os.makedirs(args.outdir, exist_ok=True)
         ws = drivers.sample_sheet_ws(G, args.seeds, args.truncation_psi, args.truncation_cutoff, args.fov_deg)
-        plan = drivers.dataset_plan(len(args.seeds), drivers.BAKE_BATCH, rank, world)
+        plan = drivers.head_plan(len(args.seeds), drivers.BAKE_BATCH, rank, world)
         for i, verts, faces, colors in drivers.coloured_meshes(G, ws, v, plan, shape_res=args.shape_res, level=args.level,
                                                                fov_deg=args.fov_deg, seed=SAMPLER_SEED):
             out = os.path.join(args.outdir, f'seed{args.seeds[i]:04d}.ply')
             isosurface.write_ply(out, verts, faces, colors)
             print(f'wrote to {out}')
-    except Exception as e:
-        if world == 1:
-            raise
-        err = f'{type(e).__name__}: {e}'
-    D.agree(err)
+    D.run_together(body)
 
 
 def gen_videos(args):

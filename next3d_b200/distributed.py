@@ -90,6 +90,19 @@ def agree(error, group=None):
             raise RankError(r, e)
 
 
+def run_together(body, group=None):
+    """Run body() on this rank, then agree: in one process an exception of body() propagates unchanged; under torch.distributed a
+    failure becomes this rank's message, and every rank raises RankError once all of them have finished body()."""
+    err = None
+    try:
+        body()
+    except Exception as e:
+        if rank_world(group)[1] == 1:
+            raise
+        err = f'{type(e).__name__}: {e}'
+    agree(err, group)
+
+
 def gather_to_root(obj, group=None):
     """The picklable `obj` of every rank, in rank order, on rank 0 of `group` (host memory: meant for a gloo group); None on the
     other ranks.  In one process: [obj]."""

@@ -12,6 +12,12 @@ _gather_frames.  The sampler keywords of every call follow one rule (_sampler_kw
 plan, CallPlan: each rank makes exactly the single-process calls that hold its own whole GOPs (the *_video_shard drivers), and
 write_video_sharded encodes them on its GPU and gathers only the coded samples to rank 0.
 
+Three outputs render heads in several views -- sample sheets, multi-view datasets (render_dataset) and coloured meshes
+(coloured_meshes) -- and share one step, _head_views_step: view 0 of the call's heads through a caching synthesis call, the other
+views through one render_views call, with sampler seed ids 2 c and 2 c + 1 for call c.  Their cameras come from one builder
+(_view_cameras).  The CLI splits their heads over ranks with one plan, head_plan: a CallPlan of whole calls, so each rank makes
+single-process calls and keeps every head of them (the sheets' sharded twin keeps shard_plan).
+
 Everything here is host logic around the hot path; the per-frame values (camera matrices, interpolated ws, uint8 pixels) are the
 reference's, checked in tests/test_drivers_cpu.py against the reference's own code, and the calls every driver makes in
 tests/test_driver_calls_cpu.py.
@@ -170,6 +176,16 @@ def call_plan(n, batch, own):
     return CallPlan(n, batch, (a, b), a // batch, (b - 1) // batch - a // batch + 1)
 
 
+def head_plan(n_heads, batch, rank=0, world=1):
+    """The CallPlan of `rank` of `world` over n_heads heads in calls of `batch` heads: whole calls, contiguous, in rank order
+    (calls shard_range(ceil(n_heads / batch), r, world)), each with its single-process call index; no calls when a rank has none.
+    Every call starts at one of the rank's own heads, so keep(k) is (0, n).  head_plan(n_heads, batch) makes the calls of
+    local_plan(n_heads, batch)."""
+    from . import distributed as D
+    ca, cb = D.shard_range(-(-n_heads // batch), rank, world)
+    return call_plan(n_heads, batch, (min(batch * ca, n_heads), min(batch * cb, n_heads)))
+
+
 def gop_span(F, gop, rank, world):
     """Frames [a, b) of an F-frame video that `rank` of `world` renders and encodes: whole GOPs, contiguous, in rank order (rank r
     owns GOPs shard_range(ceil(F / gop), r, world)); empty when there are fewer GOPs than ranks."""
@@ -178,21 +194,11 @@ def gop_span(F, gop, rank, world):
     return min(gop * a, F), min(gop * b, F)
 
 
-def sheet_span(S, batch, rank, world):
-    """(a, b, first call): the seeds [a, b) that `rank` of `world` renders with render_sample_sheets, in whole calls of
-    max(1, batch // 3) heads (calls shard_range(ceil(S / heads), r, world)), and the index of its first call in the single-process
-    run, whose sampler seeds are seed + 2 * call and one more."""
-    from . import distributed as D
-    B = max(1, batch // 3)
-    ca, cb = D.shard_range(-(-S // B), rank, world)
-    return min(B * ca, S), min(B * cb, S), ca
-
-
 def _sampler_kw(seed, sampler_noise, seed_id, ids):
     """Sampler keywords of one call: the rows ids (global image ids) of the per-image uniforms sampler_noise = (u_coarse [N, M, Dc, 1],
     u_fine [N, M, Df]) if given -- the renderer then draws no random numbers, so no seed goes with them --, else seed + seed_id (the
-    global step id; 2 step and 2 step + 1 for the two calls of a sample-sheet step) if a seed is given, else none (a fresh random
-    seed per call)."""
+    global step id; 2 step and 2 step + 1 for the two calls of a multi-view head step, _head_views_step) if a seed is given, else
+    none (a fresh random seed per call)."""
     if sampler_noise is not None:
         u_c, u_f = sampler_noise
         return {'sampler_noise': (u_c[ids], u_f[ids].reshape(-1, u_f.shape[-1]))}
@@ -869,21 +875,27 @@ SHEET_PITCH = -0.2
 NUM_WS = 28                            # mapping_ws of the backbone (triplane_next3d.py:65)
 
 
-def sample_sheet_cameras(G, fov_deg=18.837):
-    """(cams [3, 25], cond [1, 25]) float32: the camera_params of yaws +0.4, 0, -0.4 at pitch -0.2 and the frontal conditioning_params
-    of gen_samples_next3d.py:186-196 (np.pi / 2 + angle, where the video script writes 3.14 / 2), looking at
-    rendering_kwargs['avg_camera_pivot'] (default [0, 0, 0]) from radius rendering_kwargs['avg_camera_radius'] (default 2.7), with
-    FOV_to_intrinsics(fov_deg).  fov_deg may be an int or a float: the script declares --fov-deg as an int with the default 18.837,
-    which click casts to 18 when the option is omitted."""
+def _view_cameras(G, angles, fov_deg):
+    """camera_params float32 [len(angles), 25] of the views angles = [(horizontal, vertical)]: look_at_pose(horizontal, vertical)
+    looking at rendering_kwargs['avg_camera_pivot'] (default [0, 0, 0]) from radius rendering_kwargs['avg_camera_radius'] (default
+    2.7), with FOV_to_intrinsics(fov_deg)."""
     rk = G.rendering_kwargs
     pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
     radius = rk.get('avg_camera_radius', 2.7)
-    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
+    out = torch.empty(len(angles), 25)
+    out[:, 16:] = camera.fov_to_intrinsics(fov_deg).reshape(9)
+    for n, (horizontal, vertical) in enumerate(angles):
+        out[n, :16] = camera.look_at_pose(horizontal, vertical, pivot, radius).reshape(16)
+    return out
 
-    def params(horizontal, vertical):
-        return torch.cat([camera.look_at_pose(horizontal, vertical, pivot, radius).reshape(-1, 16), intr], 1)
-    cams = torch.cat([params(np.pi / 2 + yaw, np.pi / 2 + SHEET_PITCH) for yaw in SHEET_YAWS])
-    return cams, params(np.pi / 2, np.pi / 2)
+
+def sample_sheet_cameras(G, fov_deg=18.837):
+    """(cams [3, 25], cond [1, 25]) float32: the camera_params of yaws +0.4, 0, -0.4 at pitch -0.2 and the frontal conditioning_params
+    of gen_samples_next3d.py:186-196 (np.pi / 2 + angle, where the video script writes 3.14 / 2), with _view_cameras' pivot, radius
+    and FOV_to_intrinsics(fov_deg).  fov_deg may be an int or a float: the script declares --fov-deg as an int with the default
+    18.837, which click casts to 18 when the option is omitted."""
+    cams = _view_cameras(G, [(np.pi / 2 + yaw, np.pi / 2 + SHEET_PITCH) for yaw in SHEET_YAWS], fov_deg)
+    return cams, _view_cameras(G, [(np.pi / 2, np.pi / 2)], fov_deg)
 
 
 def seed_latents(seeds, z_dim):
@@ -912,8 +924,8 @@ def sheet_u8(front, views):
     return torch.cat([to_uint8_hwc(front), side], 2)
 
 
-def _check_sheets(G, ws, v, batch, shape_res):
-    """Heads per call of the sample-sheet drivers, max(1, batch // 3), after refusing bad arguments (ValueError naming the argument)."""
+def _check_heads(G, ws, v, batch, shape_res):
+    """Refuse bad arguments of the sample-sheet and coloured-mesh drivers (ValueError naming the argument)."""
     if ws.ndim != 3 or tuple(ws.shape[1:]) != (NUM_WS, G.w_dim):
         raise ValueError(f'ws must be [S, {NUM_WS}, {G.w_dim}], got {tuple(ws.shape)}')
     if ws.shape[0] == 0:
@@ -924,31 +936,32 @@ def _check_sheets(G, ws, v, batch, shape_res):
         raise ValueError(f'shape_res must be at least 2, got {shape_res}')
     if v.ndim != 3 or v.shape[0] != 1:
         raise ValueError(f'v must be one mesh [1, V, 3] (the script renders every seed with the same mesh), got {tuple(v.shape)}')
-    return max(1, batch // 3)
 
 
-def render_sample_sheets(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=None, sampler_noise=None):
+def render_sample_sheets(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=None, sampler_noise=None, plan=None):
     """gen_samples_next3d.py:182-238 for the seeds of ws [S, 28, 512] (sample_sheet_ws) and one mesh v [1, V, 3]: yields
-    (i, sheet, sigmas) in seed order.  sheet: uint8 [H, 3 W, 3] numpy, the script's three yaws side by side (sheet_u8);
+    (i, sheet, sigmas) in seed order, for the seeds the plan owns (a head_plan of S heads; default: all of them in calls of
+    B = max(1, batch // 3) heads).  sheet: uint8 [H, 3 W, 3] numpy, the script's three yaws side by side (sheet_u8);
     sigmas: float32 [R, R, R] numpy with R = shape_res, equal to extract_sigma_grid(G, ws[i:i + 1], v, shape_res), or None unless
-    `shapes`.  Each step takes B = max(1, batch // 3) heads: one synthesis call with cache_backbone renders yaw +0.4 and caches the
-    heads, one render_views call renders the other two yaws as 2 B views, and each head's density grid is decoded from its cached
-    planes, so the backbones run once per head (the script runs them three times for the sheet and once per 1M-point chunk for the
-    shape).  The last step is padded by repeating its last head.  The device->host copy of step k overlaps step k+1.  With
-    G.use_cuda_graph (and no sampler_noise) the calls replay CUDA graphs.  The driver replaces whatever heads the generator had cached.
-    `seed`: step k draws sampler seeds seed + 2 k (synthesis) and seed + 2 k + 1 (render_views); None = fresh random seeds.
-    `sampler_noise=(u_coarse [3 S, M, Dc, 1], u_fine [3 S, M, Df])` rows are indexed by the global image id 3 i + yaw (yaw 0, 1, 2 =
-    +0.4, 0, -0.4), in place of `seed`.  ValueError, before any device work, for an empty or misshapen ws, batch < 1, shape_res < 2
-    or a v batch other than 1."""
-    B = _check_sheets(G, ws, v, batch, shape_res)
+    `shapes`.  Each call renders its heads' three yaws with _head_views_step -- one synthesis call with cache_backbone for yaw +0.4,
+    one render_views call for the other two -- and each head's density grid is decoded from its cached planes, so the backbones run
+    once per head (the script runs them three times for the sheet and once per 1M-point chunk for the shape).  The last call is
+    padded by repeating its last head.  The device->host copy of call k overlaps call k+1.  With G.use_cuda_graph (and no
+    sampler_noise) the calls replay CUDA graphs.  The driver replaces whatever heads the generator had cached.
+    `seed`: call c of the single-process run draws sampler seeds seed + 2 c (synthesis) and seed + 2 c + 1 (render_views); None =
+    fresh random seeds.  `sampler_noise=(u_coarse [3 S, M, Dc, 1], u_fine [3 S, M, Df])` rows are indexed by the global image id
+    3 i + yaw (yaw 0, 1, 2 = +0.4, 0, -0.4), in place of `seed`.  ValueError, before any device work, for an empty or misshapen ws,
+    batch < 1, shape_res < 2 or a v batch other than 1."""
+    _check_heads(G, ws, v, batch, shape_res)
     device = next(G.parameters()).device
-    plan = local_plan(ws.shape[0], B)
+    plan = head_plan(ws.shape[0], max(1, batch // 3)) if plan is None else plan
     sheets = _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise)
 
     def step(k, idx):
         u8, _, sigmas = sheets(k, idx)
         return (u8, sigmas) if shapes else u8
-    return ((i, *(item if shapes else (item, None))) for i, item in enumerate(_to_host(_steps(plan, step), device)))
+    batches = ((step(k, plan.frames(k)), plan.keep(k)[1]) for k in range(plan.steps))     # whole calls: keep(k) is (0, n)
+    return ((plan.own[0] + i, *(item if shapes else (item, None))) for i, item in enumerate(_to_host(batches, device)))
 
 
 def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False, shape_res=512, seed=0, sampler_noise=None, out=None,
@@ -960,10 +973,10 @@ def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False
     gathered: one 512^3 grid is 512 MB), complete on return.  Step k of rank r draws sampler seeds seed + 2 (r * steps + k) and one
     more; `sampler_noise` rows are indexed 3 i + yaw by the global seed index i, so the results do not depend on the number of ranks.
     Refusals as in render_sample_sheets."""
-    B = _check_sheets(G, ws, v, batch, shape_res)
+    _check_heads(G, ws, v, batch, shape_res)
     device = device or next(G.parameters()).device
     cuda = torch.device(device).type == 'cuda'
-    plan = shard_plan(ws.shape[0], B)
+    plan = shard_plan(ws.shape[0], max(1, batch // 3))
     sheets = _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise)
     grids = {}
 
@@ -980,23 +993,40 @@ def render_sample_sheets_sharded(G, ws, v, fov_deg=18.837, batch=9, shapes=False
     return host, {i: g.numpy() for i, g in grids.items()}
 
 
-def _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise):
-    """step(k, idx) -> (uint8 sheets [len(idx), H, 3 W, 3], new, float32 density grids [len(new), R, R, R] or None) of the heads
-    ws[idx]: one caching synthesis call renders yaw +0.4 and keeps the heads, one render_views call renders the other two yaws from
-    the cached planes (view n of head idx[n // 2]), and with `shapes` the grid of each head in `new` -- this rank's heads of the step
-    that have none yet -- is decoded from its cached planes.  Noise rows 3 i + yaw of the per-image uniforms."""
-    cams = sample_sheet_cameras(G, fov_deg)[0].to(device)
-    v = v.to(device, torch.float32)
-    lo, hi = plan.spans[plan.rank]
-    done = set()
+def _head_views_step(G, plan, ws, cams, meshes, device, seed, sampler_noise, mesh_ids=None):
+    """step(k, idx) -> the float images [len(idx), V, 3, H, W] of the heads ws[idx] in V views: one synthesis call with
+    cache_backbone renders view 0 and keeps the heads, and for V > 1 one render_views call renders views 1 .. V - 1 from the cached
+    planes (view n of head idx[n // (V - 1)]).  cams: [V, 25] shared by every head, or [N, V, 25] per head; meshes: one mesh
+    [1, Nv, 3] for every head, or [M, Nv, 3] with mesh_ids[i] the mesh of head i.  The two calls of step k draw the sampler seed
+    ids 2 c and 2 c + 1 of its call c = plan.step_id(k); the rows of the per-image uniforms are V i + view for head i."""
+    cams = cams.to(device, torch.float32)
+    meshes = meshes.to(device, torch.float32)
+    per_head, V = cams.ndim == 3, cams.shape[-2]
 
     def step(k, idx):
         B, s = len(idx), 2 * plan.step_id(k)
         w = ws[idx].to(device, torch.float32, non_blocking=True)
-        front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True,
-                            **_sampler_kw(seed, sampler_noise, s, [3 * i for i in idx]))['image']
-        views = G.render_views(cams[1:].repeat(B, 1), **_sampler_kw(seed, sampler_noise, s + 1,
-                                                                    [3 * i + 1 + j for i in idx for j in range(2)]))['image']
+        v = meshes.expand(B, -1, -1) if mesh_ids is None else meshes[mesh_ids[idx].to(device)]
+        front = G.synthesis(w, cams[idx, 0] if per_head else cams[:1].expand(B, -1), v, noise_mode='const', cache_backbone=True,
+                            **_sampler_kw(seed, sampler_noise, s, [V * i for i in idx]))['image'][:, None]
+        if V == 1:
+            return front
+        more = G.render_views(cams[idx, 1:].reshape(-1, 25) if per_head else cams[1:].repeat(B, 1),
+                              **_sampler_kw(seed, sampler_noise, s + 1, [V * i + j for i in idx for j in range(1, V)]))['image']
+        return torch.cat([front, more.reshape(B, V - 1, *more.shape[1:])], 1)
+    return step
+
+
+def _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampler_noise):
+    """step(k, idx) -> (uint8 sheets [len(idx), H, 3 W, 3], new, float32 density grids [len(new), R, R, R] or None) of the heads
+    ws[idx]: their three yaws from _head_views_step, and with `shapes` the grid of each head in `new` -- this rank's heads of the
+    step that have none yet -- decoded from its cached planes."""
+    views = _head_views_step(G, plan, ws, sample_sheet_cameras(G, fov_deg)[0], v, device, seed, sampler_noise)
+    lo, hi = plan.spans[plan.rank]
+    done = set()
+
+    def step(k, idx):
+        images = views(k, idx)
         # a prefix of idx: a short tail repeats the last head, a rank past its span repeats a head it has done, a rank without heads
         # repeats the previous rank's last
         new = [i for i in dict.fromkeys(idx) if lo <= i < hi and i not in done] if shapes else []
@@ -1004,7 +1034,7 @@ def _sheets_step(G, plan, ws, v, fov_deg, shapes, shape_res, device, seed, sampl
         sigmas = torch.empty(len(new), shape_res, shape_res, shape_res, device=device) if new else None
         for b in range(len(new)):
             G._get_engine().cached_sigma_grid(b, shape_res, sigmas[b])
-        return sheet_u8(front, views), new, sigmas
+        return sheet_u8(images[:, 0], images[:, 1:].flatten(0, 1)), new, sigmas
     return step
 
 
@@ -1027,26 +1057,13 @@ def dataset_cameras(G, seeds, views, yaw_std=0.3, pitch_std=0.155, fov_deg=18.83
     """camera_params float32 [S, views, 25] of each seed's views: view 0 looks from the front (sample_sheet_cameras' conditioning
     camera); view v >= 1 is GaussianCameraPoseSampler's draw -- yaw pi/2 + yaw_std * n1 and pitch pi/2 + pitch_std * n2, the
     pitch clamped to (1e-5, pi - 1e-5) -- with (n1, n2) = np.random.RandomState([seed, v]).randn(2), looking at the pivot from
-    avg_camera_radius, with FOV_to_intrinsics(fov_deg)."""
-    rk = G.rendering_kwargs
-    pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
-    radius = rk.get('avg_camera_radius', 2.7)
-    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
-    out = torch.empty(len(seeds), views, 25)
-    for i, s in enumerate(seeds):
+    avg_camera_radius, with FOV_to_intrinsics(fov_deg) (_view_cameras)."""
+    angles = []
+    for s in seeds:
         for v in range(views):
             n1, n2 = np.random.RandomState([int(s), v]).randn(2) if v else (0.0, 0.0)
-            h, p = np.pi / 2 + yaw_std * n1, float(np.clip(np.pi / 2 + pitch_std * n2, 1e-5, np.pi - 1e-5))
-            out[i, v] = torch.cat([camera.look_at_pose(h, p, pivot, radius).reshape(-1, 16), intr], 1)[0]
-    return out
-
-
-def dataset_plan(n_heads, batch, rank=0, world=1):
-    """The CallPlan of `rank` of `world` over n_heads heads in calls of `batch` heads: whole calls, contiguous, in rank order
-    (calls shard_range(ceil(n_heads / batch), r, world)), each with its single-process call index; no calls when a rank has none."""
-    from . import distributed as D
-    ca, cb = D.shard_range(-(-n_heads // batch), rank, world)
-    return call_plan(n_heads, batch, (min(batch * ca, n_heads), min(batch * cb, n_heads)))
+            angles.append((np.pi / 2 + yaw_std * n1, float(np.clip(np.pi / 2 + pitch_std * n2, 1e-5, np.pi - 1e-5))))
+    return _view_cameras(G, angles, fov_deg).reshape(len(seeds), views, 25)
 
 
 def dataset_image_name(i):
@@ -1055,28 +1072,17 @@ def dataset_image_name(i):
 
 
 def render_dataset(G, ws, meshes, mesh_ids, cams, plan, seed=None):
-    """Multi-view images of the heads of a dataset_plan: ws [N, 28, 512] and cams [N, V, 25] per head, meshes [M, Nv, 3] and
-    mesh_ids[h], the mesh of head h.  Per call k: one synthesis call with cache_backbone renders view 0 of its heads, one
-    render_views call the other V - 1 views of each (view n of head n // (V - 1)), with sampler seeds seed + 2 c and seed + 2 c + 1
+    """Multi-view images of the heads of a head_plan: ws [N, 28, 512] and cams [N, V, 25] per head, meshes [M, Nv, 3] and
+    mesh_ids[h], the mesh of head h.  Each call renders its heads' V views with _head_views_step: one synthesis call with
+    cache_backbone for view 0, one render_views call for the other V - 1 views, with sampler seeds seed + 2 c and seed + 2 c + 1
     for the single-process call index c.  Yields (first head, uint8 frames [n V, H, W, 3] on the generator's device) for the n
     heads of each call that the plan owns, head-major and view-minor; a short last call repeats its last head, as render_sample_sheets
     does."""
     device = next(G.parameters()).device
-    N, V = cams.shape[:2]
-    cams = cams.to(device, torch.float32)
-    meshes = meshes.to(device, torch.float32)
-    mesh_ids = torch.as_tensor(mesh_ids, dtype=torch.long)
+    step = _head_views_step(G, plan, ws, cams, meshes, device, seed, None, torch.as_tensor(mesh_ids, dtype=torch.long))
     for k in range(plan.steps):
         idx, (lo, hi) = plan.frames(k), plan.keep(k)
-        B, c = len(idx), plan.step_id(k)
-        w = ws[idx].to(device, torch.float32)
-        img = G.synthesis(w, cams[idx, 0], meshes[mesh_ids[idx].to(device)], noise_mode='const', cache_backbone=True,
-                          **_sampler_kw(seed, None, 2 * c, None))['image']
-        frames = to_uint8_hwc(img)[:, None]
-        if V > 1:
-            more = G.render_views(cams[idx, 1:].reshape(-1, 25), **_sampler_kw(seed, None, 2 * c + 1, None))['image']
-            frames = torch.cat([frames, to_uint8_hwc(more).reshape(B, V - 1, *frames.shape[2:])], 1)
-        yield idx[lo], frames[lo:hi].reshape(-1, *frames.shape[2:])
+        yield idx[lo], to_uint8_hwc(step(k, idx)[lo:hi].flatten(0, 1))
 
 
 # ------------------------------------------------------------------------------------------------------------- coloured meshes
@@ -1089,48 +1095,31 @@ BAKE_BATCH = 3                         # heads per rendering call of coloured_me
 
 def bake_cameras(G, fov_deg=18.837):
     """camera_params float32 [len(BAKE_VIEWS), 25] of the bake views: look_at_pose(pi / 2 + yaw, pi / 2 + pitch) around
-    avg_camera_pivot from avg_camera_radius with FOV_to_intrinsics(fov_deg), as sample_sheet_cameras builds the sheets' views."""
-    rk = G.rendering_kwargs
-    pivot = torch.tensor(rk.get('avg_camera_pivot', [0, 0, 0]))
-    radius = rk.get('avg_camera_radius', 2.7)
-    intr = camera.fov_to_intrinsics(fov_deg).reshape(-1, 9)
-    return torch.cat([torch.cat([camera.look_at_pose(np.pi / 2 + yaw, np.pi / 2 + pitch, pivot, radius).reshape(-1, 16), intr], 1)
-                      for yaw, pitch in BAKE_VIEWS])
+    avg_camera_pivot from avg_camera_radius with FOV_to_intrinsics(fov_deg) (_view_cameras, as the sheets' views)."""
+    return _view_cameras(G, [(np.pi / 2 + yaw, np.pi / 2 + pitch) for yaw, pitch in BAKE_VIEWS], fov_deg)
 
 
 def coloured_meshes(G, ws, v, plan=None, batch=BAKE_BATCH, shape_res=512, level=10.0, fov_deg=18.837, seed=0):
     """Coloured meshes of the heads ws [S, 28, 512] (sample_sheet_ws) with one mesh v [1, V, 3]: yields (i, verts float32 [V, 3],
-    faces int32 [F, 3], colors uint8 [V, 3]) CUDA tensors in head order, for the heads the plan owns (a CallPlan of heads in calls
-    of `batch`; default: all of them, local_plan).  Per call, one caching synthesis renders bake view 0 of its heads and one
-    render_views call the other views (sampler seeds seed + 2 c and seed + 2 c + 1 for the single-process call index c); each head's
-    density grid comes from its cached planes, is meshed by marching cubes (extract_mesh's mesh), and the views are baked onto the
-    vertices (next3d_b200.bake), with the decoder's colour at the vertex where no view sees it.  A short last call repeats its
-    last head."""
+    faces int32 [F, 3], colors uint8 [V, 3]) CUDA tensors in head order, for the heads the plan owns (a head_plan of heads in calls
+    of `batch`; default: all of them).  Each call renders the bake views of its heads with _head_views_step (one caching synthesis
+    call for bake view 0, one render_views call for the others; sampler seeds seed + 2 c and seed + 2 c + 1 for the single-process
+    call index c); each head's density grid comes from its cached planes, is meshed by marching cubes (extract_mesh's mesh), and
+    the views are baked onto the vertices (next3d_b200.bake), with the decoder's colour at the vertex where no view sees it.  A
+    short last call repeats its last head.  Refusals as in render_sample_sheets."""
     from .bake import bake_vertex_colors, mesh_zbuffer, world_points
     from .isosurface import marching_cubes
-    if ws.ndim != 3 or ws.shape[0] == 0:
-        raise ValueError(f'ws must be [S >= 1, 28, 512], got {tuple(ws.shape)}')
-    if shape_res < 2:
-        raise ValueError(f'shape_res must be at least 2, got {shape_res}')
-    if v.ndim != 3 or v.shape[0] != 1:
-        raise ValueError(f'v must be one mesh [1, V, 3], got {tuple(v.shape)}')
+    _check_heads(G, ws, v, batch, shape_res)
     device = next(G.parameters()).device
-    plan = local_plan(ws.shape[0], batch) if plan is None else plan
+    plan = head_plan(ws.shape[0], batch) if plan is None else plan
     eng = G._get_engine()
     cams = bake_cameras(G, fov_deg).to(device)
-    n = cams.shape[0]
-    v = v.to(device, torch.float32)
+    views = _head_views_step(G, plan, ws, cams, v, device, seed, None)
     grid = torch.empty(shape_res, shape_res, shape_res, device=device) if plan.steps else None
-    keep = getattr(plan, 'keep', lambda k: (0, plan.valid(k)))
+    box = G.rendering_kwargs['box_warp']
     for k in range(plan.steps):
-        idx, (lo, hi) = plan.frames(k), keep(k)
-        B, c = len(idx), plan.step_id(k)
-        w = ws[idx].to(device, torch.float32)
-        front = G.synthesis(w, cams[:1].expand(B, -1), v.expand(B, -1, -1), noise_mode='const', cache_backbone=True,
-                            **_sampler_kw(seed, None, 2 * c, None))['image']
-        more = G.render_views(cams[1:].repeat(B, 1), **_sampler_kw(seed, None, 2 * c + 1, None))['image']
-        images = torch.cat([front[:, None], more.reshape(B, n - 1, *more.shape[1:])], 1)          # [B, views, 3, H, W]
-        box = G.rendering_kwargs['box_warp']
+        idx, (lo, hi) = plan.frames(k), plan.keep(k)
+        images = views(k, idx)                                                       # [B, views, 3, H, W]
         for b in range(lo, hi):
             eng.cached_sigma_grid(b, shape_res, grid)
             verts, faces = marching_cubes(grid, level)

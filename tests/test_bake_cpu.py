@@ -1,7 +1,8 @@
 """CPU: the vertex-colour bake of next3d_b200.bake as tests/bake_oracle.py states it.  The voxel -> world map reproduces
 create_samples at integer voxels, before and after the grid's flip; the coloured PLY layout; the oracle on analytic scenes (a
 sphere sees its front hemisphere with cos^2 weights, a vertex behind a nearer quad takes the fallback, constant images give their
-colour exactly); and the gen_meshes command's refusals, which come before the network is opened."""
+colour exactly); the calls, head ids and rank split of drivers.coloured_meshes on the recording stub generator; and the gen_meshes
+command's refusals, which come before the network is opened."""
 import struct
 
 import numpy as np
@@ -197,6 +198,60 @@ def test_zbuffer_skips_near_and_degenerate_triangles():
     zb = B.zbuffer(verts, faces, [cam], 32, 32)
     ids = set((zb[zb != B.EMPTY] & np.uint64(0xFFFFFFFF)).tolist())
     assert ids == {0}
+
+
+# ------------------------------------------------------------------------------------------------ the coloured-mesh driver
+def _run_coloured_meshes(monkeypatch, ws, v, seed, plan=None, batch=3):
+    """(calls, [(head, what reached the bake)]) of drivers.coloured_meshes on the recording stub generator, with host stand-ins
+    for marching cubes, the world map, the decoder at the vertices, the z-buffer and the bake (the last returns its inputs)."""
+    from next3d_b200 import bake, drivers, isosurface
+    from tests.test_driver_calls_cpu import _StubG
+    G = _StubG()
+    G.rendering_kwargs['box_warp'] = 0.5
+    monkeypatch.setattr(isosurface, 'marching_cubes', lambda grid, level: (grid.reshape(-1, 1)[:4] * torch.tensor([1., 2., 3.]) + level,
+                                                                           torch.tensor([[0, 1, 2], [1, 2, 3]], dtype=torch.int32)))
+    monkeypatch.setattr(bake, 'world_points', lambda verts, R, cube: verts * cube + R)
+    G.cached_sample_points = lambda b, world: (None, G.cached[0][b].mean() + world)
+    monkeypatch.setattr(bake, 'mesh_zbuffer', lambda world, faces, cams, H, W: (world.sum() + faces.sum() + cams.sum()).expand(len(cams), H, W))
+    monkeypatch.setattr(bake, 'bake_vertex_colors', lambda verts, world, grid, cams, images, zbuf, feat, cube:
+                        dict(verts=verts, world=world, grid=grid.clone(), cams=cams, images=images.clone(), zbuf=zbuf, feat=feat, cube=cube))
+    out = [(i, colors) for i, _, _, colors in drivers.coloured_meshes(G, ws, v, plan, batch=batch, shape_res=2, level=0.25, seed=seed)]
+    return G.calls, out
+
+
+@pytest.mark.parametrize('S,batch', [(5, 2), (7, 3), (1, 3)])
+def test_coloured_meshes_calls_and_heads(monkeypatch, S, batch):
+    """Per call of `batch` heads (the last repeats its last head): one caching synthesis of view 0 (seed + 2 c), one render_views
+    of the other seven views of each head (seed + 2 c + 1), then one grid per head the call owns; every head is baked from its own
+    views, grid and decoder features.  At world sizes 1-3 the ranks' whole-call plans make exactly the single-process calls."""
+    from next3d_b200 import drivers
+    from tests.test_driver_calls_cpu import RES, _StubG, _image, _sigmas
+    g = torch.Generator().manual_seed(S * 10 + batch)
+    ws, v = torch.randn(S, drivers.NUM_WS, 512, generator=g), torch.randn(1, 7, 3, generator=g)
+    calls, out = _run_coloured_meshes(monkeypatch, ws, v, 3, batch=batch)
+    n = len(drivers.BAKE_VIEWS)
+    want = []
+    for c in range(-(-S // batch)):
+        want += [('synthesis', batch, True, False, 3 + 2 * c, None), ('render_views', batch * (n - 1), False, False, 4 + 2 * c, None)]
+        want += [('grid', b) for b in range(min(batch, S - c * batch))]
+    assert calls == want
+    assert [i for i, _ in out] == list(range(S))
+    cams = drivers.bake_cameras(_StubG())
+    for i, got in out:
+        assert torch.equal(got['images'], _image(ws[i:i + 1].expand(n, -1, -1), cams, v.expand(n, -1, -1), None, RES)), i
+        assert torch.equal(got['cams'], cams) and got['zbuf'].shape == (n, RES, RES)
+        assert torch.equal(got['grid'], _sigmas(ws[i], 2)), i
+        assert torch.equal(got['verts'][:, 0], _sigmas(ws[i], 2).reshape(-1)[:4] + 0.25) and got['cube'] == 0.5
+        assert torch.equal(got['feat'], ws[i].mean() + got['world']), i
+    for world in (1, 2, 3):
+        rank_calls, rank_out = [], []
+        for r in range(world):
+            c, o = _run_coloured_meshes(monkeypatch, ws, v, 3, plan=drivers.head_plan(S, batch, r, world), batch=batch)
+            rank_calls += c
+            rank_out += o
+        assert rank_calls == calls, world                                 # whole calls: none repeated, none missing
+        assert [i for i, _ in rank_out] == list(range(S))
+        assert all(torch.equal(a['images'], b['images']) and torch.equal(a['grid'], b['grid']) for (_, a), (_, b) in zip(rank_out, out))
 
 
 # ------------------------------------------------------------------------------------------------ the gen_meshes refusals

@@ -25,17 +25,17 @@ def _inputs(n_heads=7, V=3, M=2):
 
 @pytest.mark.parametrize('world', [1, 2, 3])
 @pytest.mark.parametrize('n_heads,batch', [(7, 3), (2, 3), (6, 2)])
-def test_rank_plans_are_the_single_process_run(world, n_heads, batch):
+def test_rank_head_plans_are_the_single_process_run(world, n_heads, batch):
     ws, meshes, mesh_ids, cams = _inputs(n_heads)
     G1 = _StubG()
-    single = [(h, f) for h, f in drivers.render_dataset(G1, ws, meshes, mesh_ids, cams, drivers.dataset_plan(n_heads, batch), seed=4)]
+    single = [(h, f) for h, f in drivers.render_dataset(G1, ws, meshes, mesh_ids, cams, drivers.head_plan(n_heads, batch), seed=4)]
     calls = -(-n_heads // batch)
     assert [c[:5] for c in G1.calls] == [x for k in range(calls) for x in
                                          (('synthesis', batch, True, False, 4 + 2 * k), ('render_views', 2 * batch, False, False, 5 + 2 * k))]
     got, gcalls = [], []
     for r in range(world):
         G = _StubG()
-        plan = drivers.dataset_plan(n_heads, batch, r, world)
+        plan = drivers.head_plan(n_heads, batch, r, world)
         got += list(drivers.render_dataset(G, ws, meshes, mesh_ids, cams, plan, seed=4))
         gcalls += G.calls
     assert gcalls == G1.calls                                 # whole calls: no call runs twice
@@ -43,9 +43,9 @@ def test_rank_plans_are_the_single_process_run(world, n_heads, batch):
     assert all(torch.equal(a, b) for (_, a), (_, b) in zip(got, single))
 
 
-def test_frames_equal_a_per_head_loop():
+def test_dataset_frames_equal_a_per_head_loop():
     ws, meshes, mesh_ids, cams = _inputs(5, V=3)
-    frames = torch.cat([f for _, f in drivers.render_dataset(_StubG(), ws, meshes, mesh_ids, cams, drivers.dataset_plan(5, 2),
+    frames = torch.cat([f for _, f in drivers.render_dataset(_StubG(), ws, meshes, mesh_ids, cams, drivers.head_plan(5, 2),
                                                              seed=None)])
     assert frames.shape == (15, 4, 4, 3) and frames.dtype == torch.uint8
     for h in range(5):

@@ -203,7 +203,9 @@ def test_refusals_name_the_argument(what, kw, match):
     ws, v, _ = _sheet_inputs(2)
     args = dict(ws=ws, v=v, batch=3, shape_res=8)
     args.update(kw)
-    for fn in (drivers.render_sample_sheets, drivers.render_sample_sheets_sharded):
+    def meshes(G, ws, v, batch, shapes, shape_res):
+        return list(drivers.coloured_meshes(G, ws, v, batch=batch, shape_res=shape_res))
+    for fn in (drivers.render_sample_sheets, drivers.render_sample_sheets_sharded, meshes):
         G = _StubSheetG()
         with pytest.raises(ValueError, match=match):
             fn(G, args['ws'], args['v'], batch=args['batch'], shapes=True, shape_res=args['shape_res'])

@@ -1,4 +1,4 @@
-"""CPU: the sharded video path of the CLI without a GPU.  Each rank's schedule (drivers.call_plan, gop_span, sheet_span) makes
+"""CPU: the sharded video path of the CLI without a GPU.  Each rank's schedule (drivers.call_plan, gop_span, head_plan) makes
 exactly the single-process run's calls for its own outputs -- same item ids, tail padding and sampler seed -- and the ranks' own
 frames, in rank order, are the single-process frames, at world sizes 1 to 5 (the drivers run on the recording stub generator of
 tests/test_driver_calls_cpu.py, one rank after another in this process).  Under gloo with spawned ranks, write_video_sharded
@@ -54,14 +54,16 @@ def test_gop_spans_own_every_frame_once(F, gop, world):
 
 @pytest.mark.parametrize('world', WORLDS)
 @pytest.mark.parametrize('S,batch', [(1, 9), (5, 9), (7, 6), (10, 3), (4, 1)])
-def test_sheet_spans_are_whole_calls(S, batch, world):
+def test_head_plans_are_whole_calls(S, batch, world):
     B = max(1, batch // 3)
-    spans = [drivers.sheet_span(S, batch, r, world) for r in range(world)]
-    assert spans[0][0] == 0 and spans[-1][1] == S
-    for (a, b, call), (c, _, _) in zip(spans, spans[1:]):
-        assert b == c
-    for a, b, call in spans:
+    plans = [drivers.head_plan(S, B, r, world) for r in range(world)]
+    assert plans[0].own[0] == 0 and plans[-1].own[1] == S
+    for p, q in zip(plans, plans[1:]):
+        assert p.own[1] == q.own[0]
+    for p in plans:
+        (a, b), call = p.own, p.first
         assert (a == b or a == B * call) and (b % B == 0 or b == S)
+        assert all(p.keep(k)[0] == 0 for k in range(p.steps))               # every call starts at one of the rank's own heads
 
 
 # ------------------------------------------------------------------------------------------------ the drivers, rank by rank
@@ -147,19 +149,20 @@ def test_reenact_grid_video_shards_are_the_single_process_video(tmp_path, world)
 
 
 @pytest.mark.parametrize('world', WORLDS)
-def test_sheet_shards_are_the_single_process_sheets(world):
-    """render_sample_sheets over each rank's whole calls with seed + 2 * first call: the single process's sheets and calls."""
+def test_sheet_head_plans_are_the_single_process_sheets(world):
+    """render_sample_sheets over each rank's head_plan: the single process's seeds, sheets and calls."""
     torch.manual_seed(3)
     ws, v = torch.randn(7, drivers.NUM_WS, 512), torch.randn(1, 11, 3)
     G1 = _StubG()
     single = [s for _, s, _ in drivers.render_sample_sheets(G1, ws, v, batch=6, seed=4)]
-    sheets, calls = [], []
+    ids, sheets, calls = [], [], []
     for r in range(world):
-        a, b, call = drivers.sheet_span(7, 6, r, world)
-        if a < b:
-            G = _StubG()
-            sheets += [s for _, s, _ in drivers.render_sample_sheets(G, ws[a:b], v, batch=6, seed=4 + 2 * call)]
-            calls += G.calls
+        G = _StubG()
+        got = list(drivers.render_sample_sheets(G, ws, v, batch=6, seed=4, plan=drivers.head_plan(7, 2, r, world)))
+        ids += [i for i, _, _ in got]
+        sheets += [s for _, s, _ in got]
+        calls += G.calls
+    assert ids == list(range(7))
     assert len(sheets) == len(single) and all((x == y).all() for x, y in zip(sheets, single))
     assert calls == G1.calls
 
